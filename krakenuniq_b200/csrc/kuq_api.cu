@@ -6,6 +6,7 @@
 // double-precision Ertl estimator (hyperloglogplus.cpp:722-753).  There is no CPU classification path: without
 // an sm_90 device kuq_create fails with KUQ_E_NO_DEVICE.
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -146,6 +147,14 @@ struct kuq_ctx {
   std::vector<uint32_t> merged_hist, merged_distinct;
   uint64_t direct_upper = 0;              // upper bound of the keys in the sparse-tier set (reserve_direct_inserts)
   bool seen_dirty = false;                // counted hits flagged records since the last harvest (SEEN_BIT)
+  // record tier of the sparse HLL tier (KEPT_BIT): a resident range keeps its hits' keys in the records themselves
+  uint2 *d_secondaries = nullptr;         // (secondary, primary) record pairs of the (taxon, code) groups of the range
+  uint64_t n_secondaries = 0;
+  int collisions = 0;                     // that table: 0 = not built yet, 1 = built, -1 = none (harvests fill the set)
+  double collisions_ms = 0;               // time the table took to build
+  bool kept = false;                      // some staged records carry KEPT_BIT
+  uint64_t kept_keys = 0;                 // keys held by kept records (included in d_sparse_distinct)
+  bool set_has_hits = false;              // the set holds keys of hits, which kept records could duplicate
   uint64_t sparse_grown = 0;              // times the sparse-tier set was re-allocated at a harvest
   double harvest_ms = 0;                  // device time of the last harvest
   bool lca_mode = false;                  // kuq_set_lcas_batch ran: record values are LCA results, not classifiable
@@ -157,6 +166,7 @@ struct kuq_ctx {
 namespace {
 
 void stream_close(kuq_ctx *ctx);
+int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set = false);
 
 int fail(kuq_ctx *c, int code, const char *fmt, ...) {
   if (c) {
@@ -204,6 +214,8 @@ void free_db(kuq_ctx *ctx) {
   ctx->d_pairs = nullptr; ctx->d_offsets_owned = nullptr; ctx->d_offsets = nullptr;
   cudaFree(ctx->d_tx_keys); cudaFree(ctx->d_tx_dense); cudaFree(ctx->d_tx_counts);
   ctx->d_tx_keys = ctx->d_tx_dense = nullptr; ctx->d_tx_counts = nullptr;
+  cudaFree(ctx->d_secondaries);
+  ctx->d_secondaries = nullptr; ctx->n_secondaries = 0; ctx->collisions = 0;
   ctx->db_staged = false; ctx->db_remapped = false;
 }
 
@@ -496,7 +508,7 @@ int grow_sparse_set(kuq_ctx *ctx, uint64_t cap) {
   return KUQ_OK;
 }
 
-// The resolve half inserts (taxon, code) pairs straight into the set — at most one per window of the batch.  Make room
+// Misses and the resolve half insert (taxon, code) pairs straight into the set — at most one per window of the batch.  Make room
 // BEFORE the batch instead of failing in the middle of it: `direct_upper` bounds the keys inserted that way since the
 // last exact count; when the bound says the set could pass a load factor of 0.8 the exact fill is read back, and only
 // if that still does not fit the set doubles (all slots drained first).
@@ -508,6 +520,7 @@ int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
   CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
   uint64_t used = 0;
   for (uint32_t v : distinct) used += v;
+  used -= std::min(used, ctx->kept_keys);             // keys of kept records live in the records, not in the set
   ctx->direct_upper = used;
   if ((used + windows) * 10 > ctx->sparse_cap * 8) {
     uint64_t cap = ctx->sparse_cap;
@@ -519,12 +532,86 @@ int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
   return KUQ_OK;
 }
 
-int harvest_seen(kuq_ctx *ctx, bool discard) {
-  if (!ctx->seen_dirty) return KUQ_OK;
+// Build the collision table of the staged range once, the first time a harvest can use the record tier.
+int ensure_collisions(kuq_ctx *ctx) {
+  if (ctx->collisions) return KUQ_OK;
+  ctx->collisions = -1;
+  if (ctx->stream_open || ctx->lca_mode || !ctx->db_remapped) return KUQ_OK;
+  std::vector<uint64_t> per_taxon(ctx->n_sketch, 0);
+  for (size_t i = 0; i < ctx->db_taxids.size(); i++) per_taxon[ctx->dense_of_raw[ctx->db_taxids[i]]] += ctx->db_taxid_counts[i];
+  const auto t0 = std::chrono::steady_clock::now();
+  // a table above 1/32 of the records (a taxon far above 2^25 records) is not worth it: the set path stays
+  const int rc = build_collisions(ctx->d_pairs, ctx->key_ct, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), per_taxon.data(),
+                                  ctx->n_sketch, ctx->key_ct / 32 + 1024, &ctx->d_secondaries, &ctx->n_secondaries, ctx->n_sm, ctx->aux);
+  ctx->launches += 3;
+  ctx->collisions_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (rc == 2) return fail(ctx, KUQ_E_CUDA, "building the collision table of the record tier failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (rc == 0) ctx->collisions = 1;
+  if (getenv("KUQ_TIMING"))
+    fprintf(stderr, "[timing] collision table: %llu secondaries of %llu records, %.1f ms%s\n", (unsigned long long)ctx->n_secondaries,
+            (unsigned long long)ctx->key_ct, ctx->collisions_ms, rc ? " (not built: harvests fill the set)" : "");
+  return KUQ_OK;
+}
+
+// The keys of the kept records move into the set (mode 3), which is the only store from here on: the records are about
+// to leave HBM, or the set is about to receive keys of hits that kept records could duplicate.  All slots must be idle.
+int spill_kept(kuq_ctx *ctx) {
+  if (!ctx->kept) return KUQ_OK;
+  std::vector<uint32_t> distinct(ctx->n_sketch);
+  CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
+  uint64_t used = 0;
+  for (uint32_t v : distinct) used += v;
+  if (used * 10 > ctx->sparse_cap * 8) {
+    uint64_t cap = ctx->sparse_cap;
+    while (used * 10 > cap * 6) cap <<= 1;
+    int grc = grow_sparse_set(ctx, cap);
+    if (grc) return grc;
+  }
+  SparseSet ss;
+  ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1; ss.n_used = ctx->d_sparse_used; ss.distinct = ctx->d_sparse_distinct;
+  uint32_t *d_err;
+  CU(dmalloc(&d_err, 1));
+  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
+  launch_harvest_seen(ctx->d_pairs, ctx->key_ct, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), ctx->d_dense_flag, ss, nullptr,
+                      d_err, 3, ctx->aux);
+  ctx->launches++;
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_err);
+  ctx->kept = false;
+  ctx->kept_keys = 0;
+  ctx->set_has_hits = true;
+  ctx->direct_upper = used;
+  ctx->snap_valid = false;
+  if (err) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated while taking over the kept records (%llu slots)", (unsigned long long)ctx->sparse_cap);
+  return KUQ_OK;
+}
+
+// Sparse HLL tier of the hits: the fused lookup only flags the records it counted (SEEN_BIT); here the flags of the
+// staged range become (taxon, encoded hash) keys — the union the reference builds with `taxon_counts[t] += ...` over
+// sparse sketches (hyperloglogplus.cpp:600-603) — and are cleared.  Two stores:
+//  * record tier (a resident range whose set holds no keys of hits): the key is a function of the record and the
+//    database does not change while it is resident, so the primary record of the key's (taxon, code) group is marked
+//    KEPT_BIT and the taxon's distinct count grows by one — one streaming pass, no hash-set insert;
+//  * the set (ranges that leave HBM, `to_set`, and contexts whose set receives keys of hits from elsewhere): count →
+//    grow the set if it would pass a load factor of 0.8 → insert.  The number of keys is known before they are
+//    inserted, so the set grows here instead of failing mid-batch.
+// `discard` drops every flag of both kinds instead (the keys were exported, or the counts are reset).
+int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
+  if (!ctx->seen_dirty && !(ctx->kept && (discard || to_set))) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  if (to_set && !discard) { int rc = spill_kept(ctx); if (rc) return rc; }
+  if (!ctx->seen_dirty && !(ctx->kept && discard)) return KUQ_OK;
   ctx->seen_dirty = false;
   if (!ctx->d_pairs || !ctx->key_ct) return KUQ_OK;
+  bool keep = !discard && !to_set && ctx->d_sparse_slots && !ctx->set_has_hits && !ctx->stream_open;
+  if (keep) {
+    int rc = ensure_collisions(ctx);
+    if (rc) return rc;
+    keep = ctx->collisions == 1;
+  }
   const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
   SparseSet ss;
   ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0; ss.n_used = ctx->d_sparse_used;
@@ -538,6 +625,13 @@ int harvest_seen(kuq_ctx *ctx, bool discard) {
   if (discard || !ctx->d_sparse_slots) {
     launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 2, ctx->aux);
     ctx->launches++;
+    ctx->kept = false;
+    ctx->kept_keys = 0;
+  } else if (keep) {
+    launch_harvest_keep(ctx->d_pairs, ctx->key_ct, ctx->d_secondaries, ctx->n_secondaries, ctx->d_dense_flag, ctx->d_sparse_distinct,
+                        d_stat, ctx->aux);
+    ctx->launches += ctx->n_secondaries ? 2 : 1;
+    ctx->kept = true;
   } else {
     launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 0, ctx->aux);
     ctx->launches++;
@@ -556,6 +650,7 @@ int harvest_seen(kuq_ctx *ctx, bool discard) {
       ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1;
     }
     ctx->direct_upper = used + n_new;
+    if (n_new) ctx->set_has_hits = true;
     // Insert in record order.  (Round 2 also tried staging the keys by table slice so that the inserts of a slice are
     // L2-resident: read-only probes got faster, but NEW keys did not (each one still costs a DRAM sector fetch and a
     // dirty sector write-back), and new keys are what a harvest mostly sees.)
@@ -574,8 +669,22 @@ int harvest_seen(kuq_ctx *ctx, bool discard) {
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   cudaFree(d_stat);
   ctx->snap_valid = false;
+  if (keep) {
+    ctx->kept_keys += st[0];
+    if (getenv("KUQ_TIMING")) fprintf(stderr, "[timing] harvest: %llu records became kept (%llu kept), %.2f ms\n", st[0], (unsigned long long)ctx->kept_keys, ms);
+    return KUQ_OK;
+  }
   if ((uint32_t)st[1]) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated during the harvest (%llu slots)", (unsigned long long)ctx->sparse_cap);
   return KUQ_OK;
+}
+
+KeySource set_keys(const kuq_ctx *ctx) {
+  KeySource k{ctx->d_sparse_slots, nullptr, ctx->d_sparse_slots ? ctx->sparse_cap : 0, 0};
+  return k;
+}
+KeySource kept_keys(const kuq_ctx *ctx) {
+  KeySource k{nullptr, ctx->d_pairs, ctx->kept ? ctx->key_ct : 0, (uint32_t)((ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1)) >> 32)};
+  return k;
 }
 
 int ensure_ready(kuq_ctx *ctx) {
@@ -712,7 +821,15 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p) {
     p.flags |= KUQ_F_NO_RUNS;
     s.flags |= KUQ_F_NO_RUNS;
   }
-  if (mode == MODE_RESOLVE && !(p.flags & 4u) && ctx->cfg.hll_mode <= KUQ_HLL_CHUNKED && p.n_reads) {
+  // the fused path's only direct inserts are misses (taxon 0): harvests of the record tier do not grow the set, so room
+  // for them is made before the batch as well
+  if ((mode == MODE_RESOLVE || mode == MODE_FUSED) && !(p.flags & 4u) && ctx->cfg.hll_mode <= KUQ_HLL_CHUNKED && p.n_reads) {
+    if (mode == MODE_RESOLVE && !(p.flags & 32u) && !ctx->set_has_hits) {
+      // the resolve half inserts the keys of hits into the set, which kept records could duplicate
+      int hrc = harvest_seen(ctx, false, true);
+      if (hrc) return hrc;
+      ctx->set_has_hits = true;
+    }
     int rrc = reserve_direct_inserts(ctx, s.total_bases);
     if (rrc) return rrc;
     // the set may have moved
@@ -900,8 +1017,9 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
   uint64_t rec_lo = offsets[bin_lo], rec_hi = offsets[bin_hi];
   if (rec_hi < rec_lo || rec_hi > key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
-  // taxonomy numbering survives a re-stage (chunked mode) as long as the new range only holds numbered taxids
-  { int hrc = harvest_seen(ctx, false); if (hrc) return hrc; }
+  // taxonomy numbering survives a re-stage (chunked mode) as long as the new range only holds numbered taxids; the
+  // sparse-tier keys of the records leave with them into the set
+  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
   stream_close(ctx);
   free_db(ctx);
   ctx->k = k; ctx->nt = nt; ctx->idx_type = idx_type;
@@ -967,7 +1085,7 @@ int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uin
   uint64_t n_bins = 1ull << (2 * nt);
   if (bin_hi == 0 || bin_hi > n_bins) bin_hi = n_bins;
   if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
-  { int hrc = harvest_seen(ctx, false); if (hrc) return hrc; }
+  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
   free_db(ctx);
   ctx->k = k; ctx->nt = nt; ctx->idx_type = idx_type;
   ctx->bin_lo = bin_lo; ctx->bin_hi = bin_hi;
@@ -1482,8 +1600,9 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
     uint32_t *d_sh;
     CU(dmalloc(&d_sh, (uint64_t)ctx->n_sketch * 64));
     CU(cudaMemsetAsync(d_sh, 0, (uint64_t)ctx->n_sketch * 64 * 4, ctx->aux));
-    launch_sparse_histograms(ctx->d_sparse_slots, ctx->sparse_cap, ctx->d_dense_flag, d_sh, ctx->aux);
-    ctx->launches++;
+    launch_sparse_histograms(set_keys(ctx), ctx->d_dense_flag, d_sh, ctx->aux);
+    launch_sparse_histograms(kept_keys(ctx), ctx->d_dense_flag, d_sh, ctx->aux);
+    ctx->launches += ctx->kept ? 2 : 1;
     h.sparse_hist.resize((size_t)ctx->n_sketch * 64);
     CU(cudaMemcpyAsync(h.sparse_hist.data(), d_sh, (uint64_t)ctx->n_sketch * 64 * 4, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaMemcpyAsync(h.dense_flag.data(), ctx->d_dense_flag, ctx->n_sketch, cudaMemcpyDeviceToHost, ctx->aux));
@@ -1533,8 +1652,9 @@ int clade_hist(kuq_ctx *ctx, const std::vector<uint32_t> &members, uint32_t *his
     CU(cudaMemcpyAsync(d_member, member.data(), ctx->n_sketch, cudaMemcpyHostToDevice, ctx->aux));
     CU(cudaMemsetAsync(d_set, 0, cap * 8, ctx->aux));
     CU(cudaMemsetAsync(d_hist, 0, 65 * 4, ctx->aux));
-    launch_sparse_union(ctx->d_sparse_slots, ctx->sparse_cap, d_member, d_set, cap - 1, d_hist, d_hist + 64, ctx->aux);
-    ctx->launches++;
+    launch_sparse_union(set_keys(ctx), d_member, d_set, cap - 1, d_hist, d_hist + 64, ctx->aux);
+    launch_sparse_union(kept_keys(ctx), d_member, d_set, cap - 1, d_hist, d_hist + 64, ctx->aux);
+    ctx->launches += ctx->kept ? 2 : 1;
     uint32_t hist[65];
     CU(cudaMemcpyAsync(hist, d_hist, sizeof hist, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaStreamSynchronize(ctx->aux));
@@ -1869,7 +1989,7 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
     CU(cudaMemcpyAsync(d_dep, depth_c.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
     CU(cudaMemcpyAsync(d_sid, sid.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
     CU(cudaMemsetAsync(d_dup, 0, sparse_multi.size() * 64 * 4ull, ctx->aux));
-    const int src = sparse_clade_dups(ctx->d_sparse_slots, ctx->sparse_cap, ctx->d_dense_flag, n_keys, d_pre, d_nop, d_par, d_dep,
+    const int src = sparse_clade_dups(set_keys(ctx), kept_keys(ctx), ctx->d_dense_flag, n_keys, d_pre, d_nop, d_par, d_dep,
                                       d_sid, d_dup, ctx->n_sm, ctx->aux);
     ctx->launches += 3;
     std::vector<uint32_t> dup(sparse_multi.size() * 64, 0);
@@ -1969,9 +2089,9 @@ int kuq_sparse_export(kuq_ctx *ctx, uint64_t *d_keys_out, uint64_t cap, uint64_t
   unsigned long long *d_n;
   CU(dmalloc(&d_n, 1));
   CU(cudaMemsetAsync(d_n, 0, 8, ctx->aux));
-  launch_sparse_export(ctx->d_sparse_slots, ctx->sparse_cap, ctx->d_dense_flag,
-                       reinterpret_cast<unsigned long long *>(d_keys_out), d_keys_out ? cap : 0, d_n, ctx->aux);
-  ctx->launches++;
+  for (const KeySource &src : {set_keys(ctx), kept_keys(ctx)})
+    launch_sparse_export(src, ctx->d_dense_flag, reinterpret_cast<unsigned long long *>(d_keys_out), d_keys_out ? cap : 0, d_n, ctx->aux);
+  ctx->launches += ctx->kept ? 2 : 1;
   unsigned long long cnt = 0;
   CU(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->aux));
   CU(cudaStreamSynchronize(ctx->aux));
@@ -2020,7 +2140,7 @@ int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, ui
   if (ctx->universe.empty()) return fail(ctx, KUQ_E_STATE, "declare the taxids of the whole database first (kuq_set_db_taxid_universe)");
   if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "no taxonomy set");
   CU(cudaSetDevice(ctx->device));
-  { int hrc = harvest_seen(ctx, false); if (hrc) return hrc; }
+  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
   free_db(ctx);
   stream_close(ctx);
   ctx->k = k; ctx->nt = nt; ctx->idx_type = idx_type;
@@ -2155,7 +2275,8 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
   }
   CU(cudaSetDevice(dst->device));
   for (auto &s : dst->slots) CU(cudaStreamSynchronize(s.stream));
-  { int rc = harvest_seen(dst, false); if (rc) return rc; }
+  // the imported keys may duplicate keys of dst's kept records: dst's record tier moves into its set first
+  { int rc = harvest_seen(dst, false, true); if (rc) return rc; }
   dst->snap_valid = false;
   dst->merged_summary = false;
   uint8_t *t_regs, *t_dense; unsigned long long *t_nk, *t_nr;
@@ -2263,11 +2384,12 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
   if (!ctx->d_sparse_slots) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  // Two sources: the keys already in the local set (misses, resolve-half inserts, earlier harvests) and the records
-  // flagged since the last harvest.  The flagged records are NOT inserted locally first: their keys go straight into
-  // the export buffer (and the flags are cleared) — after the exchange every key is inserted exactly once, by its owner.
+  // Two sources: the keys already in the local set (misses, resolve-half inserts, earlier harvests) and the records —
+  // flagged since the last harvest, or kept.  The flagged records are NOT inserted locally first: their keys go straight
+  // into the export buffer (and the flags are cleared) — after the exchange every key is inserted exactly once, by its
+  // owner.
   const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
-  const bool records = ctx->seen_dirty && ctx->d_pairs && ctx->key_ct;
+  const bool records = (ctx->seen_dirty || ctx->kept) && ctx->d_pairs && ctx->key_ct;
   unsigned long long *d_cnt;
   CU(dmalloc(&d_cnt, 24));                       // [0:8) counts / cursors, [8:16) part ends, [16] error word
   CU(cudaMemsetAsync(d_cnt, 0, 24 * 8, ctx->aux));
@@ -2306,7 +2428,8 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
     launch_keys_parts(1, nullptr, ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, n_parts, d_cnt,
                       reinterpret_cast<unsigned long long *>(d_keys_out), d_cnt + 8, d_err, 1, ctx->aux);
     ctx->launches++;
-    ctx->seen_dirty = false;                     // the flags are gone: their keys live in the export buffer now
+    ctx->seen_dirty = false;                     // the flags are gone: their keys live in the export buffer now (the kept
+                                                 // records drop their flag when the merged keys replace the set)
   }
   uint32_t err = 0;
   CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
@@ -2323,7 +2446,7 @@ int kuq_sparse_replace(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   if (!ctx->d_sparse_slots) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  rc = harvest_seen(ctx, true);                  // anything still flagged was exported before; drop the flags
+  rc = harvest_seen(ctx, true);                  // anything still flagged or kept was exported before; drop the flags
   if (rc) return rc;
   ctx->snap_valid = false;
   uint64_t cap = ctx->sparse_cap;
@@ -2356,8 +2479,9 @@ int kuq_sparse_summary(kuq_ctx *ctx, uint32_t *d_hist_out, uint32_t *d_distinct_
   if (rc) return rc;
   CU(cudaMemsetAsync(d_hist_out, 0, (uint64_t)ctx->n_sketch * 64 * 4, ctx->aux));
   if (ctx->d_sparse_slots) {
-    launch_sparse_histograms(ctx->d_sparse_slots, ctx->sparse_cap, ctx->d_dense_flag, d_hist_out, ctx->aux);
-    ctx->launches++;
+    launch_sparse_histograms(set_keys(ctx), ctx->d_dense_flag, d_hist_out, ctx->aux);
+    launch_sparse_histograms(kept_keys(ctx), ctx->d_dense_flag, d_hist_out, ctx->aux);
+    ctx->launches += ctx->kept ? 2 : 1;
     CU(cudaMemcpyAsync(d_distinct_out, ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToDevice, ctx->aux));
   } else {
     CU(cudaMemsetAsync(d_distinct_out, 0, ctx->n_sketch * 4ull, ctx->aux));
@@ -2468,6 +2592,9 @@ int kuq_sparse_import(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   ctx->snap_valid = false;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  rc = harvest_seen(ctx, false, true);           // imported keys may duplicate kept ones: the set becomes the store
+  if (rc) return rc;
+  ctx->set_has_hits = true;
   SparseSet ss;
   ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1; ss.n_used = ctx->d_sparse_used;
   ss.distinct = ctx->d_sparse_distinct;
@@ -2511,6 +2638,7 @@ int kuq_reset_counts(kuq_ctx *ctx) {
     CU(cudaMemset(ctx->d_sparse_used, 0, 8));
     CU(cudaMemset(ctx->d_sparse_distinct, 0, ctx->n_sketch * 4ull));
     ctx->direct_upper = 0;
+    ctx->set_has_hits = false;
   }
   if (ctx->d_exact) {
     CU(cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull));

@@ -5,7 +5,7 @@
 //  dense clades  (some member's sketch is dense → register-wise max of the members' registers, :604-621):
 //      one CTA per clade folds its members' 4 KB register arrays; register histograms of all clades in one launch.
 //  sparse clades (no dense member → union of the members' code sets, :600-603): the number of distinct codes of
-//      every subtree at once.  Keys (taxon, code) of the sparse tier are sorted by (code, preorder(taxon)); the
+//      every subtree at once.  Keys (taxon, code) of the sparse tier (set slots and kept records) are sorted by (code, preorder(taxon)); the
 //      taxa of a subtree are a preorder interval, so the occurrences of one code inside a subtree are a run of that
 //      sorted sequence and   distinct(subtree u) = keys in u − adjacent equal-code pairs inside u,
 //      and a pair lies inside u exactly when its taxa's lowest common ancestor does.  The kernel books every
@@ -42,17 +42,17 @@ __global__ void __launch_bounds__(256) k_clade_max_batch(const uint8_t *__restri
 }
 
 // keys of the taxa that are still sparse and belong to the tree → (code << 32 | preorder of the taxon)
-__global__ void __launch_bounds__(256) k_clade_sort_keys(const unsigned long long *__restrict__ slots, uint64_t cap,
+__global__ void __launch_bounds__(256) k_clade_sort_keys(const KeySource src,
                                                          const uint8_t *__restrict__ dense_flag, const uint32_t *__restrict__ pre_of_taxon,
                                                          unsigned long long *__restrict__ out, uint64_t out_cap,
                                                          unsigned long long *cursor) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  const uint64_t n_round = (cap + stride - 1) / stride * stride;          // whole warps stay in the loop (ballot below)
+  const uint64_t n_round = (src.n + stride - 1) / stride * stride;        // whole warps stay in the loop (ballot below)
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
     unsigned long long sk = 0;
     bool have = false;
-    if (i < cap) {
-      const unsigned long long key = slots[i];
+    if (i < src.n) {
+      const unsigned long long key = source_key(src, i);
       if (key) {
         const uint32_t taxon = (uint32_t)(key >> 32) - 1;
         if (!dense_flag[taxon]) {
@@ -103,10 +103,10 @@ void launch_clade_max_batch(const uint8_t *regs, const uint32_t *d_offs, const u
 }
 
 // 0 = ok, 1 = not enough device memory (the caller falls back to one union per clade), 2 = CUDA error
-int sparse_clade_dups(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag, uint64_t n_keys_upper,
+int sparse_clade_dups(const KeySource &set_keys, const KeySource &kept_keys, const uint8_t *dense_flag, uint64_t n_keys_upper,
                       const uint32_t *d_pre_of_taxon, const uint32_t *d_node_of_pre, const uint32_t *d_parent_c,
                       const uint32_t *d_depth_c, const int32_t *d_sid_of_node, uint32_t *d_dup, int n_sm, cudaStream_t stream) {
-  if (n_keys_upper < 2 || cap == 0) return 0;
+  if (n_keys_upper < 2 || set_keys.n + kept_keys.n == 0) return 0;
   unsigned long long *buf[2] = {nullptr, nullptr}, *cursor = nullptr;
   void *temp = nullptr;
   size_t temp_bytes = 0;
@@ -124,7 +124,8 @@ int sparse_clade_dups(const unsigned long long *slots, uint64_t cap, const uint8
     return 1;
   }
   cudaMemsetAsync(cursor, 0, 8, stream);
-  k_clade_sort_keys<<<n_sm * 8, 256, 0, stream>>>(slots, cap, dense_flag, d_pre_of_taxon, buf[0], n_keys_upper, cursor);
+  for (const KeySource *src : {&set_keys, &kept_keys})
+    if (src->n) k_clade_sort_keys<<<n_sm * 8, 256, 0, stream>>>(*src, dense_flag, d_pre_of_taxon, buf[0], n_keys_upper, cursor);
   unsigned long long n = 0;
   cudaMemcpyAsync(&n, cursor, 8, cudaMemcpyDeviceToHost, stream);
   if (cudaStreamSynchronize(stream) != cudaSuccess) { (void)cudaGetLastError(); cleanup(); return 2; }

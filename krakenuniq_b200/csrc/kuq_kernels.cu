@@ -55,17 +55,6 @@ __device__ __forceinline__ uint32_t revcomp32(uint32_t x, uint32_t n) {   // n <
   x = ((x >> 1) & 0x55555555u) | ((x & 0x55555555u) << 1);
   return (~x) >> (32 - 2 * n);
 }
-// murmurhash3_finalizer (hyperloglogplus.cpp:830-838)
-__device__ __forceinline__ uint64_t fmix64(uint64_t key) {
-  key += 1;
-  key ^= key >> 33;
-  key *= 0xff51afd7ed558ccdull;
-  key ^= key >> 33;
-  key *= 0xc4ceb9fe1a85ec53ull;
-  key ^= key >> 33;
-  return key;
-}
-
 // 12-byte records are only 4-byte aligned: a key is two 32-bit loads.
 __device__ __forceinline__ uint64_t load_key(const uint8_t *pairs, uint64_t pos, uint64_t key_mask) {
   const uint32_t *p = reinterpret_cast<const uint32_t *>(pairs + pos * 12);
@@ -95,17 +84,6 @@ __device__ __forceinline__ void hll_update(uint8_t *regs, uint32_t taxon, uint64
     if (prev == old) break;
     old = prev;
   }
-}
-
-// encodeHashIn32Bit(h, pPrime=25, p=12), hyperloglogplus.cpp:181-204
-__device__ __forceinline__ uint32_t encode_hash32(uint64_t hash) {
-  uint32_t idx = (uint32_t)((hash >> 39) << 7);
-  if ((idx << 12) == 0) {
-    uint64_t rest = hash << 25;
-    uint32_t add_rank = rest ? (uint32_t)__clzll((long long)rest) + 1 : 40;
-    return idx | (add_rank << 1) | 1;
-  }
-  return idx;
 }
 
 __device__ __forceinline__ uint64_t mix64(uint64_t x) {   // table hash for the device sets (not reference arithmetic)
@@ -467,10 +445,11 @@ __global__ void __launch_bounds__(256, 8) k_lookup(const __grid_constant__ Param
             // Sparse HLL tier of a hit (hyperloglogplus.cpp:499-512): the (taxon, encoded hash) pair is a function
             // of the RECORD, so instead of probing a hash set per window the record itself is flagged in the free
             // top bit of its key word — the sector is in L1/L2 already, the flag costs no DRAM read, and only the
-            // first sighting of a record issues the atomic.  k_harvest_seen turns flagged records into set keys
-            // once per run.  A stale (non-coherent) load can only miss a flag another thread just set: the
-            // atomicOr is then redundant, never wrong.
-            if (mark_seen && taxon != 0 && taxon != FOUND_ZERO && !(hiw & SEEN_BIT))
+            // first sighting of a record issues the atomic.  The harvest turns flagged records into sparse-tier
+            // keys once per run; a record whose key is kept already (KEPT_BIT) needs no flag.  A stale
+            // (non-coherent) load can only miss a flag another thread just set: the atomicOr is then redundant,
+            // never wrong.
+            if (mark_seen && taxon != 0 && taxon != FOUND_ZERO && !(hiw & (SEEN_BIT | KEPT_BIT)))
               atomicOr(const_cast<uint32_t *>(b + 3 * t + 1), SEEN_BIT);
             m = 0;
           }
@@ -1048,26 +1027,24 @@ __device__ __forceinline__ uint32_t encoded_rank_dev(uint32_t e) {
 
 // sparseRegisterHistogram (hyperloglogplus.cpp:356-366) for every taxon that stayed sparse: C[t][rank]++ over the
 // distinct codes of t (the host derives C[0] = 2^25 - |S_t|)
-__global__ void k_sparse_histograms(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag,
-                                    uint32_t *hist) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    const unsigned long long key = slots[i];
+__global__ void k_sparse_histograms(const KeySource src, const uint8_t *dense_flag, uint32_t *hist) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < src.n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const unsigned long long key = source_key(src, i);
     if (!key) continue;
     const uint32_t taxon = (uint32_t)(key >> 32) - 1;
     if (dense_flag[taxon]) continue;
     atomicAdd(hist + (size_t)taxon * 64 + min(encoded_rank_dev((uint32_t)key), 63u), 1u);
   }
 }
-void launch_sparse_histograms(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag,
-                              uint32_t *hist, cudaStream_t stream) {
-  if (cap) k_sparse_histograms<<<device_sm_count() * 16, 256, 0, stream>>>(slots, cap, dense_flag, hist);
+void launch_sparse_histograms(const KeySource &src, const uint8_t *dense_flag, uint32_t *hist, cudaStream_t stream) {
+  if (src.n) k_sparse_histograms<<<device_sm_count() * 16, 256, 0, stream>>>(src, dense_flag, hist);
 }
 
 // union of the sparse code sets of the member taxa (sparse ∪ sparse merge, hyperloglogplus.cpp:600-603)
-__global__ void k_sparse_union(const unsigned long long *slots, uint64_t cap, const uint8_t *member,
+__global__ void k_sparse_union(const KeySource src, const uint8_t *member,
                                unsigned long long *scratch, uint64_t smask, uint32_t *hist64, uint32_t *overflow) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    const unsigned long long key = slots[i];
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < src.n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const unsigned long long key = source_key(src, i);
     if (!key) continue;
     const uint32_t taxon = (uint32_t)(key >> 32) - 1;
     if (!member[taxon]) continue;
@@ -1087,17 +1064,17 @@ __global__ void k_sparse_union(const unsigned long long *slots, uint64_t cap, co
     }
   }
 }
-void launch_sparse_union(const unsigned long long *slots, uint64_t cap, const uint8_t *member,
+void launch_sparse_union(const KeySource &src, const uint8_t *member,
                          unsigned long long *scratch_set, uint64_t scratch_mask, uint32_t *hist64, uint32_t *overflow,
                          cudaStream_t stream) {
-  if (cap) k_sparse_union<<<device_sm_count() * 16, 256, 0, stream>>>(slots, cap, member, scratch_set, scratch_mask, hist64, overflow);
+  if (src.n) k_sparse_union<<<device_sm_count() * 16, 256, 0, stream>>>(src, member, scratch_set, scratch_mask, hist64, overflow);
 }
 
 // export / import of the sparse tier (cross-GPU union of the (taxon, code) sets)
-__global__ void k_sparse_export(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag,
+__global__ void k_sparse_export(const KeySource src, const uint8_t *dense_flag,
                                 unsigned long long *out, uint64_t out_cap, unsigned long long *n_out) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    const unsigned long long key = slots[i];
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < src.n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const unsigned long long key = source_key(src, i);
     const bool keep = key && !dense_flag[(uint32_t)(key >> 32) - 1];
     const uint32_t m = __ballot_sync(__activemask(), keep);
     if (!keep) continue;
@@ -1122,9 +1099,9 @@ __global__ void k_sparse_import(const unsigned long long *keys, uint64_t n, Spar
     else if (ins < 0) atomicExch(error_flag, 4u);
   }
 }
-void launch_sparse_export(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag,
+void launch_sparse_export(const KeySource &src, const uint8_t *dense_flag,
                           unsigned long long *out, uint64_t out_cap, unsigned long long *n_out, cudaStream_t stream) {
-  if (cap) k_sparse_export<<<device_sm_count() * 16, 256, 0, stream>>>(slots, cap, dense_flag, out, out_cap, n_out);
+  if (src.n) k_sparse_export<<<device_sm_count() * 16, 256, 0, stream>>>(src, dense_flag, out, out_cap, n_out);
 }
 void launch_sparse_import(const unsigned long long *keys, uint64_t n, const SparseSet &s, const uint8_t *dense_flag,
                           uint32_t *error_flag, cudaStream_t stream) {
@@ -1433,23 +1410,25 @@ __global__ void k_remap_values(uint8_t *pairs, uint64_t n_rec, const uint32_t *k
   }
 }
 
-// Flagged records → sparse-tier keys (once per run / before a range leaves HBM): for every record a counted hit
-// flagged, insert (taxon, encodeHashIn32Bit(hash(k-mer))) into the set unless the taxon went dense, and clear the
-// flag.  mode 0 = count the flagged records of taxa that are not dense (stats[0]), 1 = insert + clear, 2 = clear only.
+// Flagged records → sparse-tier keys of the set (records that leave HBM, or contexts whose set receives hit keys from
+// elsewhere): for every record a counted hit flagged, insert (taxon, encodeHashIn32Bit(hash(k-mer))) into the set
+// unless the taxon went dense, and clear the flag.  mode 0 = count the records carrying `bit` of taxa that are not
+// dense (stats[0]), 1 = insert + clear SEEN_BIT, 2 = clear SEEN_BIT and KEPT_BIT, 3 = move the kept records into the
+// set: insert + clear KEPT_BIT, without counting (their keys are counted in `distinct` already).
 __global__ void __launch_bounds__(256) k_harvest_seen(uint8_t *pairs, uint64_t n_rec, uint32_t hi_mask, const uint8_t *dense_flag,
-                                                      SparseSet set, unsigned long long *stats, uint32_t *error_flag, int mode) {
+                                                      SparseSet set, unsigned long long *stats, uint32_t *error_flag, int mode,
+                                                      uint32_t bit) {
   unsigned long long n_local = 0;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_rec; i += (uint64_t)gridDim.x * blockDim.x) {
     uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
     const uint32_t hiw = w[1];
-    if (!(hiw & SEEN_BIT)) continue;
+    if (!(hiw & bit)) continue;
     const uint32_t taxon = w[2];
     if (mode == 0) { n_local += dense_flag[taxon] ? 0 : 1; continue; }
-    w[1] = hiw & ~SEEN_BIT;
+    w[1] = hiw & ~bit;
     if (mode == 2 || dense_flag[taxon]) continue;
-    const uint64_t key = ((uint64_t)(hiw & hi_mask) << 32) | w[0];
-    const int ins = sparse_insert(set, taxon, encode_hash32(fmix64(key)));
-    if (ins > 0) atomicAdd(set.distinct + taxon, 1u);
+    const int ins = sparse_insert(set, taxon, (uint32_t)record_key(w, hiw, hi_mask));
+    if (ins > 0 && mode == 1) atomicAdd(set.distinct + taxon, 1u);
     else if (ins < 0) atomicExch(error_flag, 4u);
   }
   if (mode == 0) {
@@ -1461,7 +1440,64 @@ void launch_harvest_seen(uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, cons
                          unsigned long long *stats, uint32_t *error_flag, int mode, cudaStream_t stream) {
   if (!n_rec) return;
   const int grid = (int)min((uint64_t)device_sm_count() * 16, (n_rec + 255) / 256);
-  k_harvest_seen<<<grid, 256, 0, stream>>>(pairs, n_rec, (uint32_t)(key_mask >> 32), dense_flag, set, stats, error_flag, mode);
+  const uint32_t bit = mode == 2 ? (SEEN_BIT | KEPT_BIT) : mode == 3 ? KEPT_BIT : SEEN_BIT;
+  k_harvest_seen<<<grid, 256, 0, stream>>>(pairs, n_rec, (uint32_t)(key_mask >> 32), dense_flag, set, stats, error_flag, mode, bit);
+}
+
+// Harvest of a resident range without set inserts.  The sparse-tier key of a record is a function of the record, so
+// "the key is in the tier" is one more record flag (KEPT_BIT), held by the primary of each (taxon, code) group.
+// (a) k_fold_secondaries: a flagged secondary hands its flag to its primary.
+// (b) k_harvest_keep, one streaming pass: a flagged record that is not kept yet (and whose taxon is not dense) becomes
+//     kept and counts one distinct code of its taxon; every flag is cleared.  The per-taxon counts are gathered in a
+//     shared-memory table per CTA (a few thousand taxa would otherwise take hundreds of millions of same-address global
+//     atomics); taxa that do not find a slot there count globally.
+__global__ void k_fold_secondaries(uint8_t *pairs, const uint2 *list, uint64_t n) {
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint2 sp = list[e];                              // (secondary, primary) record indices
+    uint32_t *ws = reinterpret_cast<uint32_t *>(pairs + (uint64_t)sp.x * 12) + 1;
+    const uint32_t hiw = *ws;
+    if (!(hiw & SEEN_BIT)) continue;
+    *ws = hiw & ~SEEN_BIT;                                 // a record is the secondary of one entry only
+    atomicOr(reinterpret_cast<uint32_t *>(pairs + (uint64_t)sp.y * 12) + 1, SEEN_BIT);
+  }
+}
+
+constexpr int KEEP_SLOTS = 1024;
+__global__ void __launch_bounds__(256) k_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint8_t *dense_flag, uint32_t *distinct,
+                                                      unsigned long long *n_kept) {
+  __shared__ uint32_t s_tax[KEEP_SLOTS], s_cnt[KEEP_SLOTS];
+  for (int s = threadIdx.x; s < KEEP_SLOTS; s += blockDim.x) { s_tax[s] = 0; s_cnt[s] = 0; }
+  __syncthreads();
+  unsigned long long n_local = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_rec; i += (uint64_t)gridDim.x * blockDim.x) {
+    uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
+    const uint32_t hiw = w[1];
+    if (!(hiw & SEEN_BIT)) continue;
+    const uint32_t taxon = w[2];
+    if ((hiw & KEPT_BIT) || dense_flag[taxon]) { w[1] = hiw & ~SEEN_BIT; continue; }
+    w[1] = (hiw & ~SEEN_BIT) | KEPT_BIT;
+    n_local++;
+    uint32_t h = (taxon * 0x9E3779B1u) >> 22, probe = 0;
+    for (; probe < 8; probe++, h = (h + 1) & (KEEP_SLOTS - 1)) {
+      uint32_t cur = s_tax[h];
+      if (cur == 0) cur = atomicCAS(&s_tax[h], 0u, taxon + 1), cur = cur ? cur : taxon + 1;
+      if (cur == taxon + 1) { atomicAdd(&s_cnt[h], 1u); break; }
+    }
+    if (probe == 8) atomicAdd(distinct + taxon, 1u);
+  }
+  __syncthreads();
+  for (int s = threadIdx.x; s < KEEP_SLOTS; s += blockDim.x)
+    if (s_tax[s]) atomicAdd(distinct + s_tax[s] - 1, s_cnt[s]);
+  for (int o = 16; o; o >>= 1) n_local += __shfl_xor_sync(0xFFFFFFFFu, n_local, o);
+  if ((threadIdx.x & 31) == 0 && n_local) atomicAdd(n_kept, n_local);
+}
+void launch_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint2 *secondaries, uint64_t n_secondaries, const uint8_t *dense_flag,
+                         uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream) {
+  if (!n_rec) return;
+  if (n_secondaries)
+    k_fold_secondaries<<<(int)min((uint64_t)device_sm_count() * 8, (n_secondaries + 255) / 256), 256, 0, stream>>>(pairs, secondaries, n_secondaries);
+  const int grid = (int)min((uint64_t)device_sm_count() * 8, (n_rec + 255) / 256);
+  k_harvest_keep<<<grid, 256, 0, stream>>>(pairs, n_rec, dense_flag, distinct, n_kept);
 }
 
 // re-insert the keys of an outgrown table into its successor (no per-taxon counting: the keys were counted before)
@@ -1606,7 +1642,8 @@ __device__ __forceinline__ uint32_t key_part(unsigned long long key, uint32_t n_
   return (uint32_t)((mix64((uint32_t)key) >> 33) % n_parts);
 }
 // One kernel for both sources of keys — SRC 0: the slots of the local set, SRC 1: the records a counted hit flagged
-// (pass 1 clears the flag: the key leaves this GPU instead of entering its set).  pass 0 counts per part, pass 1
+// and the kept records (pass 1 clears SEEN_BIT: the key leaves this GPU instead of entering its set; KEPT_BIT is
+// dropped when the merged keys replace the set, kuq_sparse_replace).  pass 0 counts per part, pass 1
 // scatters through the per-part cursors.  Same-address atomics would serialise hundreds of millions of keys on
 // n_parts counters, so keys are counted / ranked on shared-memory counters (only real keys touch them — most slots are
 // empty and most records unflagged, and a per-part warp vote for every item made the kernel instruction bound), and
@@ -1650,13 +1687,9 @@ __global__ void __launch_bounds__(256) k_keys_parts(const unsigned long long *sl
         } else {
           uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
           const uint32_t hiw = hiws[j];
-          if (hiw & SEEN_BIT) {
-            if (pass == 1) w[1] = hiw & ~SEEN_BIT;
-            const uint32_t taxon = w[2];
-            if (!dense_flag[taxon]) {
-              const uint64_t kmer = ((uint64_t)(hiw & hi_mask) << 32) | w[0];
-              k = ((unsigned long long)(taxon + 1) << 32) | encode_hash32(fmix64(kmer));
-            }
+          if (hiw & (SEEN_BIT | KEPT_BIT)) {
+            if (pass == 1 && (hiw & SEEN_BIT)) w[1] = hiw & ~SEEN_BIT;
+            if (!dense_flag[w[2]]) k = record_key(w, hiw, hi_mask);
           }
         }
       }

@@ -43,6 +43,9 @@ constexpr uint32_t HLL_M = 4096;
 // Record flag in the key word's free top bit (keys hold 2k <= 62 bits; the reference masks the rest away,
 // krakendb.cpp:283-284): "a counted hit has seen this record since the last harvest" — the sparse HLL tier of hits.
 constexpr uint32_t SEEN_BIT = 0x80000000u;
+// Second record flag (bit 62, free for k <= 31): "this record's (taxon, encoded hash) is a key of the sparse tier".
+// Only one record per (taxon, code) carries it — the primary of its collision group (kuq_api.cu, build_collisions).
+constexpr uint32_t KEPT_BIT = 0x40000000u;
 constexpr int SEARCH_WINDOW = 8;           // records scanned linearly once the bisection window is this small
 
 enum Mode { MODE_FUSED = 0, MODE_LOOKUP = 1, MODE_RESOLVE = 2 };
@@ -70,8 +73,55 @@ struct SparseSet {           // device set of (dense taxon, encoded hash) pairs:
   unsigned long long *slots; // 0 = empty; key = (taxon + 1) << 32 | code
   uint64_t mask;             // capacity - 1 (power of two)
   unsigned long long *n_used;
-  uint32_t *distinct;        // [n_sketch] distinct codes inserted per taxon
+  uint32_t *distinct;        // [n_sketch] distinct codes per taxon (set keys + kept records)
 };
+
+// The sparse tier lives in two places: the slots of the set, and the staged records that carry KEPT_BIT.  Readouts
+// scan one source per launch; a source with n == 0 launches nothing.
+struct KeySource {
+  const unsigned long long *slots;   // set slots, or nullptr for the record tier
+  const uint8_t *pairs;              // records of the staged range (slots == nullptr)
+  uint64_t n;                        // slots / records
+  uint32_t hi_mask;                  // key bits of the record's high word
+};
+
+#ifdef __CUDACC__
+// murmurhash3_finalizer (hyperloglogplus.cpp:830-838)
+__device__ __forceinline__ uint64_t fmix64(uint64_t key) {
+  key += 1;
+  key ^= key >> 33;
+  key *= 0xff51afd7ed558ccdull;
+  key ^= key >> 33;
+  key *= 0xc4ceb9fe1a85ec53ull;
+  key ^= key >> 33;
+  return key;
+}
+
+// encodeHashIn32Bit(h, pPrime=25, p=12), hyperloglogplus.cpp:181-204
+__device__ __forceinline__ uint32_t encode_hash32(uint64_t hash) {
+  uint32_t idx = (uint32_t)((hash >> 39) << 7);
+  if ((idx << 12) == 0) {
+    uint64_t rest = hash << 25;
+    uint32_t add_rank = rest ? (uint32_t)__clzll((long long)rest) + 1 : 40;
+    return idx | (add_rank << 1) | 1;
+  }
+  return idx;
+}
+
+// set-key of a record: (taxon + 1) << 32 | encodeHashIn32Bit(hash(k-mer))
+__device__ __forceinline__ unsigned long long record_key(const uint32_t *w, uint32_t hiw, uint32_t hi_mask) {
+  const uint64_t kmer = ((uint64_t)(hiw & hi_mask) << 32) | w[0];
+  return ((unsigned long long)(w[2] + 1) << 32) | encode_hash32(fmix64(kmer));
+}
+
+// item i of a key source: a set slot (0 = empty) or the key of a kept record (0 = not kept)
+__device__ __forceinline__ unsigned long long source_key(const KeySource &s, uint64_t i) {
+  if (s.slots) return s.slots[i];
+  const uint32_t *w = reinterpret_cast<const uint32_t *>(s.pairs + i * 12);
+  const uint32_t hiw = w[1];
+  return (hiw & KEPT_BIT) ? record_key(w, hiw, s.hi_mask) : 0ull;
+}
+#endif
 
 // Per-batch bookkeeping of the reference's per-work-unit sketches (classify.cpp:525: one ReadCounts map per work
 // unit).  A (unit, taxon) sketch converts from sparse to dense iff an insert finds >= 1024 distinct encoded hashes
@@ -182,9 +232,17 @@ void launch_collect_taxids(const uint8_t *pairs, uint64_t n_rec, uint32_t *keys,
                            uint32_t cap_mask, uint32_t *overflow, cudaStream_t stream);
 void launch_remap_values(uint8_t *pairs, uint64_t n_rec, const uint32_t *keys, const uint32_t *dense,
                          uint32_t cap_mask, uint32_t *missing, uint64_t key_mask, cudaStream_t stream);
-// flagged records → sparse-tier keys: mode 0 count (stats[0]), 1 insert + clear, 2 clear only
+// flagged records → keys of the set: mode 0 count (stats[0]), 1 insert + clear, 2 clear SEEN_BIT and KEPT_BIT,
+// 3 kept records → set (not counted again)
 void launch_harvest_seen(uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint8_t *dense_flag, const SparseSet &set,
                          unsigned long long *stats, uint32_t *error_flag, int mode, cudaStream_t stream);
+// flagged records → kept records (no set): secondaries hand their flag to their primaries, then one pass over the
+// records sets KEPT_BIT, counts distinct[taxon] and clears SEEN_BIT (*n_kept += records that became kept)
+void launch_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint2 *secondaries, uint64_t n_secondaries, const uint8_t *dense_flag,
+                         uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream);
+// kuq_collisions.cu: (secondary, primary) record pairs of every (taxon, code) group of the staged records
+int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint64_t *records_of_taxon, uint32_t n_sketch,
+                     uint64_t max_entries, uint2 **list_out, uint64_t *n_out, int n_sm, cudaStream_t stream);
 void launch_sparse_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag,
                           cudaStream_t stream);
 void launch_register_histograms(const uint8_t *regs, uint32_t n_sketch, uint32_t *hist /*[n_sketch][64]*/,
@@ -197,18 +255,17 @@ int launch_unit_accounting(const Params &p, int n_sm, cudaStream_t stream);
 void launch_unit_clear(const UnitMap &u, uint32_t n_sketch, int n_sm, cudaStream_t stream);
 // chunked rule: one global sketch per taxon converts once it holds >= 1025 distinct codes
 void launch_flag_dense_global(const uint32_t *distinct, uint8_t *dense_flag, uint32_t n_sketch, cudaStream_t stream);
-// histogram of encoded ranks over the sparse set, per taxon: hist[t][64] (+ hist[t][63] unused)
-void launch_sparse_histograms(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag,
-                              uint32_t *hist, cudaStream_t stream);
+// histogram of encoded ranks over one source of the sparse tier, per taxon: hist[t][64] (+ hist[t][63] unused)
+void launch_sparse_histograms(const KeySource &src, const uint8_t *dense_flag, uint32_t *hist, cudaStream_t stream);
 // distinct codes of the union of the member taxa (member[t] != 0): rank histogram hist64 via a scratch set
 // exact mode: distinct k-mers over the member taxa (set union of ReadCounts::operator+=, readcounts.hpp:76-81)
 void launch_exact_union(const ExactSet &e, const uint8_t *member, unsigned long long *scratch_set, uint64_t scratch_mask,
                         unsigned long long *n_distinct, uint32_t *overflow, cudaStream_t stream);
-void launch_sparse_union(const unsigned long long *slots, uint64_t cap, const uint8_t *member,
+void launch_sparse_union(const KeySource &src, const uint8_t *member,
                          unsigned long long *scratch_set, uint64_t scratch_mask, uint32_t *hist64, uint32_t *overflow,
                          cudaStream_t stream);
 
-void launch_sparse_export(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag,
+void launch_sparse_export(const KeySource &src, const uint8_t *dense_flag,
                           unsigned long long *out, uint64_t out_cap, unsigned long long *n_out, cudaStream_t stream);
 void launch_sparse_import(const unsigned long long *keys, uint64_t n, const SparseSet &s, const uint8_t *dense_flag,
                           uint32_t *error_flag, cudaStream_t stream);
@@ -230,7 +287,7 @@ void launch_keys_parts(int src, const unsigned long long *slots, uint8_t *pairs,
 // kuq_clades.cu: all clades of the report at once
 void launch_clade_max_batch(const uint8_t *regs, const uint32_t *d_offs, const uint32_t *d_members, uint32_t n_clades,
                             uint8_t *d_out, cudaStream_t stream);
-int sparse_clade_dups(const unsigned long long *slots, uint64_t cap, const uint8_t *dense_flag, uint64_t n_keys_upper,
+int sparse_clade_dups(const KeySource &set_keys, const KeySource &kept_keys, const uint8_t *dense_flag, uint64_t n_keys_upper,
                       const uint32_t *d_pre_of_taxon, const uint32_t *d_node_of_pre, const uint32_t *d_parent_c,
                       const uint32_t *d_depth_c, const int32_t *d_sid_of_node, uint32_t *d_dup, int n_sm, cudaStream_t stream);
 // kuq_layout_exp.cu: record-layout / search-shape experiment (0 ok, 1 no memory, 2 CUDA error, 3 taxon ids > 24 bits);
