@@ -2299,19 +2299,7 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
     uint64_t *d_keys_dst = nullptr;
     if (cudaMalloc((void **)&d_keys_dst, n_keys * 8) != cudaSuccess) { (void)cudaGetLastError(); cudaSetDevice(src->device); cudaFree(d_keys_src); return fail(ctx, KUQ_E_NOMEM, "no room for %llu keys", (unsigned long long)n_keys); }
     CU(cudaMemcpyPeer(d_keys_dst, dst->device, d_keys_src, src->device, n_keys * 8));
-    // make room first: the import itself cannot grow the set
-    std::vector<uint32_t> distinct(dst->n_sketch);
-    CU(cudaMemcpy(distinct.data(), dst->d_sparse_distinct, dst->n_sketch * 4ull, cudaMemcpyDeviceToHost));
-    uint64_t used = 0;
-    for (uint32_t v : distinct) used += v;
-    if ((used + n_keys) * 10 > dst->sparse_cap * 8) {
-      uint64_t cap = dst->sparse_cap;
-      while ((used + n_keys) * 10 > cap * 6) cap <<= 1;
-      int grc = grow_sparse_set(dst, cap);
-      if (grc) { cudaFree(d_keys_dst); return grc; }
-    }
-    dst->direct_upper = used + n_keys;
-    rc = kuq_sparse_import(dst, d_keys_dst, n_keys);
+    rc = kuq_sparse_import(dst, d_keys_dst, n_keys);        // grows dst's set first when the keys need room
     cudaFree(d_keys_dst);
   }
   if (d_keys_src) { cudaSetDevice(src->device); cudaFree(d_keys_src); cudaSetDevice(dst->device); }
@@ -2594,6 +2582,19 @@ int kuq_sparse_import(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   rc = harvest_seen(ctx, false, true);           // imported keys may duplicate kept ones: the set becomes the store
   if (rc) return rc;
+  // make room first: the import kernel cannot grow the set (a context that classified few reads or none has a small
+  // set and may receive the keys of all the others)
+  std::vector<uint32_t> distinct(ctx->n_sketch);
+  CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
+  uint64_t used = 0;
+  for (uint32_t v : distinct) used += v;
+  if ((used + n) * 10 > ctx->sparse_cap * 8) {
+    uint64_t cap = ctx->sparse_cap;
+    while ((used + n) * 10 > cap * 6) cap <<= 1;
+    rc = grow_sparse_set(ctx, cap);
+    if (rc) return rc;
+  }
+  ctx->direct_upper = used + n;
   ctx->set_has_hits = true;
   SparseSet ss;
   ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1; ss.n_used = ctx->d_sparse_used;

@@ -15,6 +15,35 @@ import torch
 import torch.distributed as dist
 
 
+class Collectives:
+    """The collectives of this module, on a torch.distributed process group (`group`; None = the default group).
+    Every function below takes `group=` and accepts either a torch.distributed group or an instance of a subclass of
+    this class: a subclass can run the same merge over several contexts driven by threads of one process."""
+
+    def __init__(self, group=None):
+        self.group = group
+
+    def rank(self) -> int:
+        return dist.get_rank(self.group)
+
+    def world_size(self) -> int:
+        return dist.get_world_size(self.group)
+
+    def all_reduce(self, t: torch.Tensor, op: str):
+        """in place; op is 'max' or 'sum'"""
+        dist.all_reduce(t, op={"max": dist.ReduceOp.MAX, "sum": dist.ReduceOp.SUM}[op], group=self.group)
+
+    def all_gather(self, out: list, t: torch.Tensor):
+        dist.all_gather(out, t, group=self.group)
+
+    def all_to_all_single(self, out: torch.Tensor, t: torch.Tensor, out_splits=None, in_splits=None):
+        dist.all_to_all_single(out, t, output_split_sizes=out_splits, input_split_sizes=in_splits, group=self.group)
+
+
+def collectives(group=None) -> Collectives:
+    return group if isinstance(group, Collectives) else Collectives(group)
+
+
 def partition(n_items: int, world: int, rank: int):
     """contiguous, balanced [begin, end) of rank's share of n_items (reads of a file, bins of a database)"""
     base, rem = divmod(n_items, world)
@@ -25,43 +54,45 @@ def partition(n_items: int, world: int, rank: int):
 def merge_state_tensors(regs: torch.Tensor, n_kmers: torch.Tensor, n_reads: torch.Tensor,
                         dense_flag: torch.Tensor | None = None, group=None):
     """in-place all-reduce of the per-taxon state"""
-    dist.all_reduce(regs, op=dist.ReduceOp.MAX, group=group)
-    dist.all_reduce(n_kmers, op=dist.ReduceOp.SUM, group=group)
-    dist.all_reduce(n_reads, op=dist.ReduceOp.SUM, group=group)
+    c = collectives(group)
+    c.all_reduce(regs, "max")
+    c.all_reduce(n_kmers, "sum")
+    c.all_reduce(n_reads, "sum")
     if dense_flag is not None:
-        dist.all_reduce(dense_flag, op=dist.ReduceOp.MAX, group=group)
+        c.all_reduce(dense_flag, "max")
 
 
 def gather_sparse_keys(keys: torch.Tensor, group=None) -> torch.Tensor:
     """all-gather variable-length int64 key arrays (0 = padding); returns the keys of all OTHER ranks"""
-    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    c = collectives(group)
+    world, rank = c.world_size(), c.rank()
     n = torch.tensor([keys.numel()], dtype=torch.int64, device=keys.device)
     sizes = [torch.zeros_like(n) for _ in range(world)]
-    dist.all_gather(sizes, n, group=group)
+    c.all_gather(sizes, n)
     m = int(max(int(s.item()) for s in sizes))
     if m == 0:
         return keys.new_zeros(0)
     padded = keys.new_zeros(m)
     padded[:keys.numel()] = keys
     out = [keys.new_zeros(m) for _ in range(world)]
-    dist.all_gather(out, padded, group=group)
+    c.all_gather(out, padded)
     return torch.cat([out[r][:int(sizes[r].item())] for r in range(world) if r != rank]) if world > 1 else keys.new_zeros(0)
 
 
 def exchange_partitioned_keys(keys: torch.Tensor, counts, group=None, out: torch.Tensor | None = None) -> torch.Tensor:
     """One all-to-all of key segments: `keys` holds the segment for rank 0, 1, ... back to back (`counts[r]` keys for
     rank r); returns the keys every rank (this one included) sent to this rank.  O(keys / world) per rank."""
-    world = dist.get_world_size(group)
+    c = collectives(group)
+    world = c.world_size()
     send = torch.tensor([int(c) for c in counts], dtype=torch.int64, device=keys.device)
     recv = torch.empty_like(send)
-    dist.all_to_all_single(recv, send, group=group)
+    c.all_to_all_single(recv, send)
     recv_l = [int(x) for x in recv.tolist()]
     if out is not None and out.numel() >= sum(recv_l):
         out = out[:sum(recv_l)]
     else:
         out = keys.new_empty(sum(recv_l))
-    dist.all_to_all_single(out, keys[:int(send.sum())], output_split_sizes=recv_l,
-                           input_split_sizes=[int(c) for c in counts], group=group)
+    c.all_to_all_single(out, keys[:int(send.sum())], recv_l, [int(x) for x in counts])
     assert len(recv_l) == world
     return out
 
@@ -86,9 +117,12 @@ def merge_classifier_state(clf, device, group=None):
     nr = device_view(sp.d_n_reads, sp.n_taxa * 8, torch.int64, device)
     flag = device_view(sp.d_dense_flag, sp.n_sketch, torch.uint8, device)
     merge_state_tensors(regs, nk, nr, flag, group)
+    # the library works on its own streams: the reduced dense flags (which the export filters on) must have landed
+    torch.cuda.synchronize()
     # sparse tier: union of the (taxon, code) sets of the taxa that are still sparse everywhere
     n = clf.sparse_export()
     keys = torch.zeros(max(n, 1), dtype=torch.int64, device=device)
+    torch.cuda.synchronize()
     if n:
         n2 = clf.sparse_export(keys.data_ptr(), keys.numel())
         keys = keys[:n2]
@@ -96,6 +130,7 @@ def merge_classifier_state(clf, device, group=None):
         keys = keys[:0]
     others = gather_sparse_keys(keys, group)
     if others.numel():
+        torch.cuda.synchronize()
         clf.sparse_import(others.data_ptr(), others.numel())
     torch.cuda.synchronize()
 
@@ -110,7 +145,8 @@ def merge_classifier_state_partitioned(clf, device, group=None, timings: dict | 
          (kuq_sparse_replace) → all-reduce SUM of the per-taxon rank histograms and distinct counts
          (kuq_set_sparse_summary).  Clade unions: `clade_counts_distributed`."""
     import time
-    world = dist.get_world_size(group)
+    c = collectives(group)
+    world = c.world_size()
     t0 = time.time()
     marks = []
 
@@ -124,9 +160,9 @@ def merge_classifier_state_partitioned(clf, device, group=None, timings: dict | 
     nk = device_view(sp.d_n_kmers, sp.n_sketch * 8, torch.int64, device)
     nr = device_view(sp.d_n_reads, sp.n_taxa * 8, torch.int64, device)
     flag = device_view(sp.d_dense_flag, sp.n_sketch, torch.uint8, device)
-    dist.all_reduce(flag, op=dist.ReduceOp.MAX, group=group)
+    c.all_reduce(flag, "max")
     torch.cuda.synchronize()
-    merge_state_tensors(regs, nk, nr, None, group)
+    merge_state_tensors(regs, nk, nr, None, c)
     mark("allreduce_state")
     # no local harvest: the keys of the flagged records go straight into the export buffer (kuq.h).
     # `buffers` = (export tensor, receive tensor), int64, allocated once by the caller: multi-GB cudaMallocs inside the
@@ -142,7 +178,7 @@ def merge_classifier_state_partitioned(clf, device, group=None, timings: dict | 
         kptr, counts = clf.sparse_export_partitioned_alloc(world)
         keys = device_view(kptr, max(int(counts.sum()), 1) * 8, torch.int64, device)
     mark("export_partitioned")
-    recv = exchange_partitioned_keys(keys, counts.tolist(), group, out=None if buffers is None else buffers[1])
+    recv = exchange_partitioned_keys(keys, counts.tolist(), c, out=None if buffers is None else buffers[1])
     torch.cuda.synchronize()
     del keys
     if kptr is not None:
@@ -152,10 +188,11 @@ def merge_classifier_state_partitioned(clf, device, group=None, timings: dict | 
     mark("replace_import")
     hist = torch.zeros(sp.n_sketch * 64, dtype=torch.int32, device=device)
     distinct = torch.zeros(sp.n_sketch, dtype=torch.int32, device=device)
+    torch.cuda.synchronize()
     clf.sparse_summary(hist.data_ptr(), distinct.data_ptr())
     mark("summary")
-    dist.all_reduce(hist, op=dist.ReduceOp.SUM, group=group)
-    dist.all_reduce(distinct, op=dist.ReduceOp.SUM, group=group)
+    c.all_reduce(hist, "sum")
+    c.all_reduce(distinct, "sum")
     torch.cuda.synchronize()
     clf.set_sparse_summary(hist.data_ptr(), distinct.data_ptr())
     mark("allreduce_summary")
@@ -173,14 +210,15 @@ def clade_counts_distributed(clf, clades, device, group=None):
     """(unique, reads, kmers) per clade (list of taxid lists) after merge_classifier_state_partitioned: the union
     histograms of the code partitions add up; one all-reduce for all clades."""
     from . import binding
+    coll = collectives(group)
     parts = [clf.clade_partial(c) for c in clades]
     hist = torch.tensor(np.stack([p[3] for p in parts]).astype(np.int64) if parts else np.zeros((0, 64), np.int64), device=device)
     dense = [p[2] for p in parts]
     # dense clades: every rank holds the all-reduced registers, so its histogram is already the global one
     for i, d in enumerate(dense):
-        if d and dist.get_rank(group) != 0:
+        if d and coll.rank() != 0:
             hist[i] = 0
-    dist.all_reduce(hist, op=dist.ReduceOp.SUM, group=group)
+    coll.all_reduce(hist, "sum")
     h = hist.cpu().numpy().astype(np.uint32)
     out = []
     for i, (r, k, d, _) in enumerate(parts):

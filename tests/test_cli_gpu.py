@@ -17,7 +17,8 @@ def _run(tmp_path, tag, extra, reads, env_extra=None):
     out, rep = tmp_path / f"{tag}.kraken", tmp_path / f"{tag}.report.tsv"
     cmd = [exe, "-d", os.path.join(G, "database.kdb"), "-i", os.path.join(G, "database.idx"), "-a",
            os.path.join(G, "taxDB"), "-t", "1", "-r", str(rep), "-o", str(out)] + extra + [os.path.join(G, reads)]
-    env = dict(os.environ, KUQ_SPARSE_SLOTS=str(1 << 22), **(env_extra or {}))
+    env = dict(os.environ, KUQ_SPARSE_SLOTS=str(1 << 22))
+    env.update(env_extra or {})
     r = subprocess.run(cmd, capture_output=True, text=True, env=env)
     assert r.returncode == 0, r.stderr[-2000:]
     return out, rep, r
@@ -50,6 +51,22 @@ def test_cli_matches_reference_outputs(tmp_path, tag, extra, reads):
     n_seq = want_err[0].split(" sequences")[0]
     assert f"{n_seq} sequences (" in r.stderr
     assert want_err[1].strip() in r.stderr and want_err[2].strip() in r.stderr
+
+
+@pytest.mark.parametrize("tag,extra,env", [("preload", ["-M"], {}), ("preload_u20000", ["-M", "-u", "20000"], {}),
+                                           ("chunked", ["-M"], {"KUQ_FORCE_SHARDS": "1"})])
+def test_cli_one_device_as_several_gpus(tmp_path, tag, extra, env):
+    """one device listed twice: the multi-GPU paths of one process, with a context per listed device — replicas
+    (batches round-robin, kuq_merge_into at the end) and minimizer-range shards (run_sharded: peer stores, device
+    flags between the contexts, kuq_merge_into over shard contexts; sketches follow the -x rule).  Each context of
+    the executable reserves about 33 GB of batch slots (3 slots of 288 MiB bases), so an 80 GB card holds two."""
+    # small batches so that every context gets work; a small sparse set so that it has to grow
+    out, rep, r = _run(tmp_path, tag, extra, "reads.fa",
+                       dict(env, KUQ_DEVICES="0,0", KUQ_BATCH_READS="200", KUQ_SPARSE_SLOTS=str(1 << 12)))
+    assert "not usable" not in r.stderr, [l for l in r.stderr.splitlines() if "not usable" in l]
+    assert ("sharded over 2 GPUs" if env else "2 GPUs, database replicated") in r.stderr, r.stderr[:1500]
+    assert open(out).read() == open(os.path.join(G, f"{tag}.kraken")).read()
+    assert _report_lines(rep) == _report_lines(os.path.join(G, f"{tag}.report.tsv"))
 
 
 @pytest.mark.parametrize("threads,serial", [("8", False), ("3", False), ("1", True)])

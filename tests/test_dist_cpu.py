@@ -137,6 +137,50 @@ def _exchange_worker(rank, world, port, q):
     dist.destroy_process_group()
 
 
+@pytest.mark.parametrize("world", [1, 3, 8])
+def test_in_process_group_runs_the_same_collectives(world):
+    """tests.local_group (threads of one process) gives what the gloo ranks above give: reduced state, the other
+    ranks' keys, and the all-to-all of code-partitioned keys"""
+    from tests.local_group import run_ranks
+
+    def rank(r, coll):
+        rng = np.random.default_rng(200 + r)
+        regs = torch.from_numpy(rng.integers(0, 40, 64, dtype=np.uint8))
+        nk = torch.from_numpy(rng.integers(0, 1000, 8, dtype=np.int64))
+        inputs = (regs.clone(), nk.clone())
+        kdist.merge_state_tensors(regs, nk, nk.clone(), None, coll)
+        keys = np.unique((rng.integers(1, 6, 300 + 50 * r, dtype=np.int64) << 32) | rng.integers(0, 3000, 300 + 50 * r))
+        others = kdist.gather_sparse_keys(torch.from_numpy(keys), coll).numpy()
+        part = (keys & 0xFFFFFFFF) % world
+        order = np.argsort(part, kind="stable")
+        got = kdist.exchange_partitioned_keys(torch.from_numpy(keys[order]), np.bincount(part, minlength=world).tolist(),
+                                              coll).numpy()
+        return inputs, regs, nk, keys, others, got
+
+    res = run_ranks(world, rank)
+    want_regs = torch.stack([x[0][0] for x in res]).max(0).values
+    want_nk = torch.stack([x[0][1] for x in res]).sum(0)
+    for r, (_, regs, nk, keys, others, got) in enumerate(res):
+        assert torch.equal(regs, want_regs) and torch.equal(nk, want_nk)
+        assert np.array_equal(np.sort(others), np.sort(np.concatenate([x[3] for j, x in enumerate(res) if j != r]
+                                                                      + [np.zeros(0, np.int64)])))
+        assert np.all((got & 0xFFFFFFFF) % world == r)
+    assert np.array_equal(np.sort(np.concatenate([x[5] for x in res])), np.sort(np.concatenate([x[3] for x in res])))
+
+
+def test_in_process_group_stops_every_rank_when_one_fails():
+    from tests.local_group import run_ranks
+
+    def rank(r, coll):
+        if r == 1:
+            raise ValueError("rank 1 failed")
+        kdist.merge_state_tensors(torch.zeros(4, dtype=torch.uint8), torch.zeros(2, dtype=torch.int64),
+                                  torch.zeros(2, dtype=torch.int64), None, coll)
+
+    with pytest.raises(ValueError, match="rank 1 failed"):
+        run_ranks(3, rank, timeout=60)
+
+
 def test_partitioned_key_exchange_is_a_disjoint_cover():
     """the all-to-all of the code-partitioned sparse-tier keys: every key reaches exactly the rank that owns its code,
     so the union over ranks is the union of the inputs and no code lives on two ranks"""
