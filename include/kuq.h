@@ -44,7 +44,7 @@ extern "C" {
 #define KUQ_E_CUDA (-2)           /* a CUDA runtime call failed (kuq_last_error has the text) */
 #define KUQ_E_NO_DEVICE (-3)      /* no usable sm_90 device: there is no CPU fallback */
 #define KUQ_E_DB_FORMAT (-4)      /* krakendb.cpp:64-74: not JFLISTDN / val_len != 4; :541: bad index magic */
-#define KUQ_E_UNSUPPORTED_K (-5)  /* only 8-byte keys (k = 29..31; every published KrakenUniq DB is k=31) */
+#define KUQ_E_UNSUPPORTED_K (-5)  /* k > 31 (key_bits > 62): bits 62 / 63 of a staged key word are record flags */
 #define KUQ_E_STATE (-6)          /* call order: DB and taxonomy must be set before classifying, ... */
 #define KUQ_E_CAPACITY (-7)       /* batch larger than the configured slot capacity */
 #define KUQ_E_NOMEM (-8)          /* host or device allocation failed */
@@ -141,12 +141,17 @@ int kuq_device_count(void);
 /* ---- database -------------------------------------------------------------------------------------------- */
 /* Stage (a minimizer range of) the database into HBM.  kdb_image / idx_image are the bytes of database.kdb and
  * database.idx (mmap'ed files are fine).  Bins [bin_lo, bin_hi) are copied; bin_hi = 0 means "to the end".
- * Replaces a previously staged range (the `load_chunk` step of the chunked mode, krakendb.cpp:411-425). */
+ * Replaces a previously staged range (the `load_chunk` step of the chunked mode, krakendb.cpp:411-425).
+ * Any k up to 31.  The file's records are key_len + 4 bytes (key_len = ceil(2k / 8): 12 bytes for k = 29..31,
+ * 8 to 11 bytes below); in HBM every record takes 12 bytes {u64 key, u32 value}.  Shorter records are copied as they
+ * are and widened on the device, through a landing zone of 64 MiB (environment variable KUQ_LANDING_BYTES overrides
+ * its size) that exists only during the call. */
 int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image,
                  uint64_t idx_bytes, uint64_t bin_lo, uint64_t bin_hi);
 /* Adopt a database that already lives in HBM (records in on-disk layout, values still raw taxids; offsets =
  * the full 4^nt+1 table or, with bin_lo>0, the slice starting at bin_lo).  The buffers stay owned by the caller
- * but the record values are rewritten in place (taxid → dense id). */
+ * but the record values are rewritten in place (taxid → dense id).  The on-disk layout is the staged layout only for
+ * 12-byte records, so this call takes k = 29..31; stage other databases with kuq_stage_db. */
 int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uint64_t *d_offsets, uint32_t k,
                          uint32_t nt, uint32_t idx_type, uint64_t bin_lo, uint64_t bin_hi);
 /* Distinct taxids stored in the staged records with their record counts — what KrakenDB::count_taxons()
@@ -345,11 +350,14 @@ int kuq_scan_device(kuq_ctx *ctx, uint32_t slot, uint32_t k, uint32_t nt, uint32
  *     for r in ranges:  kuq_stream_use(r & 1);  kuq_stream_load((r + 1) & 1, range r + 1);      // order matters
  *                       kuq_lookup_device(... only_hits = 1 ...) for every batch, ids merged in the caller's buffers
  *     kuq_resolve_device(...) for every batch                                  // the final pass (classify.cpp:663-791)
- * host_records = the range's records (12 bytes each, raw taxids, as in database.kdb), host_offsets = the bin_hi -
+ * host_records = the range's records (key_len + 4 bytes each for the k given to kuq_stream_open: 12 for k = 29..31; raw
+ * taxids; as in database.kdb), host_offsets = the bin_hi -
  * bin_lo + 1 cumulative ABSOLUTE record offsets of its bins (a slice of database.idx); both should be pinned
  * (kuq_host_alloc / kuq_host_register) or the copy will not overlap.  kuq_stream_load waits, on the device, for the
  * work queued on the slots so far (the users of the buffer it overwrites), never for the host.  Record values are
- * rewritten to dense ids on arrival; kuq_stream_check reports a taxid outside the declared universe. */
+ * rewritten to dense ids on arrival; kuq_stream_check reports a taxid outside the declared universe.  The buffers hold
+ * max_records records of 12 bytes; records shorter than that (k <= 28) are widened on arrival, in pieces that pass
+ * through one landing zone of 64 MiB (KUQ_LANDING_BYTES) on the copy stream. */
 int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, uint64_t max_records, uint64_t max_bins);
 int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64_t n_records, const uint64_t *host_offsets,
                     uint64_t bin_lo, uint64_t bin_hi);
@@ -438,7 +446,8 @@ int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t 
 int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_offsets, uint32_t n_pieces,
                        const uint32_t *taxid, uint32_t flags, uint64_t *n_missing);
 /* Copy the record values of the staged database (as taxids) into the value fields of a host database.kdb image
- * with the same records — what set_lcas leaves in the memory-mapped file. */
+ * with the same records — what set_lcas leaves in the memory-mapped file.  Values are written at the file's record
+ * stride (key_len + 4 bytes), whatever the staged layout. */
 int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes);
 
 #ifdef __cplusplus

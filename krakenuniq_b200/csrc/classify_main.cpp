@@ -1187,12 +1187,11 @@ static void run_chunked(kuq_ctx *ctx, const Mapped &kdb, const Mapped &idx, uint
   if (!getenv("KUQ_CHUNKS_ON_HOST")) {
     uint64_t need = 0, max_rec = 1, max_bins = 1;
     for (auto &b : batches) need += (b.bases.size() + 64) * 5 + (b.reads.size() + 4) * 8 + 1024;
-    const uint64_t key_len_rec = 12;
     for (auto &rg : ranges) {
       max_rec = std::max<uint64_t>(max_rec, offsets[rg.second] - offsets[rg.first]);
       max_bins = std::max<uint64_t>(max_bins, rg.second - rg.first);
     }
-    const uint64_t range_bytes = 2 * (max_rec * key_len_rec + (max_bins + 1) * 8 + 4096);
+    const uint64_t range_bytes = 2 * (max_rec * 12 + (max_bins + 1) * 8 + 4096);     // 12 B per record in HBM
     const uint64_t free_b = kuq_device_free_bytes(ctx);
     if (need + range_bytes + (2ull << 30) < free_b || getenv("KUQ_FORCE_CHUNKS")) {
       uint64_t key_bits;
@@ -1200,6 +1199,7 @@ static void run_chunked(kuq_ctx *ctx, const Mapped &kdb, const Mapped &idx, uint
       const uint64_t header = 72 + 2 * (4 + 8 * key_bits);
       const uint8_t *rec0 = (const uint8_t *)kdb.p + header;
       const uint32_t k = (uint32_t)(key_bits / 2), idx_type = memcmp(q, "KRAKIDX", 7) == 0 ? 1 : 2;
+      const uint64_t pair_sz = (key_bits + 7) / 8 + 4;            // the file's record size (12 B only for k = 29..31)
       // taxonomy must be known before the stream opens (the dense numbering is fixed there): main() sets it before us
       if (kuq_stream_open(ctx, k, nt, idx_type, max_rec, max_bins)) die(EX_DATAERR, kuq_last_error(ctx));
       const bool pinned = kuq_host_register(kdb.p, kdb.size) == KUQ_OK && kuq_host_register(idx.p, idx.size) == KUQ_OK;
@@ -1223,7 +1223,7 @@ static void run_chunked(kuq_ctx *ctx, const Mapped &kdb, const Mapped &idx, uint
       }
       auto load = [&](uint32_t buf, size_t c) {
         const uint64_t lo = ranges[c].first, hi = ranges[c].second;
-        if (kuq_stream_load(ctx, buf, rec0 + offsets[lo] * key_len_rec, offsets[hi] - offsets[lo], offsets + lo, lo, hi))
+        if (kuq_stream_load(ctx, buf, rec0 + offsets[lo] * pair_sz, offsets[hi] - offsets[lo], offsets + lo, lo, hi))
           die(EX_DATAERR, kuq_last_error(ctx));
       };
       load(0, 0);
@@ -1514,6 +1514,14 @@ static void run_multi_db(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
   }
 }
 
+// What a staged database takes in HBM: 12 bytes per record whatever the file's record size (records of k <= 28 databases
+// are widened on the way in), plus the index.  Every decision about what fits a card counts these bytes, not the file's.
+static uint64_t hbm_bytes(const Mapped &kdb, const Mapped &idx) {
+  uint64_t key_ct = 0;
+  if (kdb.size >= 56) memcpy(&key_ct, (const uint8_t *)kdb.p + 48, 8);
+  return key_ct * 12 + idx.size;
+}
+
 int main(int argc, char **argv) {
   parse_command_line(argc, argv);
   if (Map_UIDs) die(EX_USAGE, "-I (UID mapping) is not supported by the GPU classify");
@@ -1550,16 +1558,17 @@ int main(int argc, char **argv) {
   // a database larger than one card: sharded over the visible GPUs when they hold it together (run_sharded), else
   // streamed through one GPU in ranges of at most 40 GB (two range buffers + the reads have to fit, run_chunked)
   bool want_shards = false;
-  if (n_db == 1 && (kdb.size + idx.size > hbm_budget || getenv("KUQ_FORCE_SHARDS"))) {
+  const uint64_t db_hbm = hbm_bytes(kdb, idx);
+  if (n_db == 1 && (db_hbm > hbm_budget || getenv("KUQ_FORCE_SHARDS"))) {
     int n_vis = 0;
     if (const char *dl = getenv("KUQ_DEVICES")) { if (strcmp(dl, "all") == 0) n_vis = kuq_device_count(); else { n_vis = 1; for (const char *c = dl; *c; c++) n_vis += *c == ','; } }
     else if (!getenv("KUQ_DEVICE")) n_vis = kuq_device_count();
-    want_shards = n_vis > 1 && (getenv("KUQ_FORCE_SHARDS") || (kdb.size + idx.size) / n_vis + (16ull << 30) < hbm_budget);
+    want_shards = n_vis > 1 && (getenv("KUQ_FORCE_SHARDS") || db_hbm / n_vis + (16ull << 30) < hbm_budget);
   }
-  if (kdb.size + idx.size > hbm_budget && !want_shards) chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
+  if (db_hbm > hbm_budget && !want_shards) chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
   if (n_db > 1) {
     for (size_t i = 0; i < n_db; i++)
-      if (kdbs[i].size + idxs[i].size > hbm_budget) die(EX_USAGE, "with several databases each one has to fit the HBM budget");
+      if (hbm_bytes(kdbs[i], idxs[i]) > hbm_budget) die(EX_USAGE, "with several databases each one has to fit the HBM budget");
     chunk_budget = 0;
   }
   if (Populate_memory_size > 0 && getenv("KUQ_FORCE_CHUNKS")) { chunk_budget = Populate_memory_size; want_shards = false; }

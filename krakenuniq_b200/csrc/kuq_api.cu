@@ -140,6 +140,9 @@ struct kuq_ctx {
   uint64_t stream_cap_records = 0, stream_cap_bins = 0;
   cudaStream_t copy_stream = nullptr;
   uint32_t *d_stream_missing = nullptr;
+  uint64_t stream_pair_sz = 12;           // record size of the streamed database's file (key_len + 4)
+  uint8_t *d_stream_land = nullptr;       // k <= 28: landing zone of stream_land_rec file records, widened from there
+  uint64_t stream_land_rec = 0;
   bool shard_counting = false;            // kuq_set_shard_counting: hits are counted by the GPU that finds them
   uint32_t extra_flags = 0;               // kuq_set_stats: KUQ_F_STATS for calls that take no flags
   uint32_t *d_sync_err = nullptr;         // set by a kuq_wait_flags that timed out
@@ -167,6 +170,15 @@ namespace {
 
 void stream_close(kuq_ctx *ctx);
 int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set = false);
+
+// Records of a database with k <= 28 are shorter than the 12 bytes they take in HBM; they pass through a device landing
+// zone of this many records on their way there.  64 MiB unless KUQ_LANDING_BYTES says otherwise (a small zone cuts a
+// small database into many pieces, which is what tests of the piece arithmetic want).
+uint64_t landing_records(uint64_t pair_sz) {
+  uint64_t bytes = 64ull << 20;
+  if (const char *e = getenv("KUQ_LANDING_BYTES")) bytes = strtoull(e, nullptr, 10);
+  return std::max<uint64_t>(1, bytes / pair_sz);
+}
 
 int fail(kuq_ctx *c, int code, const char *fmt, ...) {
   if (c) {
@@ -892,7 +904,7 @@ const char *kuq_strerror(int code) {
     case KUQ_E_CUDA: return "CUDA error";
     case KUQ_E_NO_DEVICE: return "no sm_90 CUDA device (libkuq has no CPU path)";
     case KUQ_E_DB_FORMAT: return "database in improper format";
-    case KUQ_E_UNSUPPORTED_K: return "unsupported k (only 8-byte keys: k = 29..31)";
+    case KUQ_E_UNSUPPORTED_K: return "unsupported k (k-mers of up to 31 bases)";
     case KUQ_E_STATE: return "call order / state error";
     case KUQ_E_CAPACITY: return "capacity exceeded";
     case KUQ_E_NOMEM: return "out of memory";
@@ -997,11 +1009,12 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   if (val_len != 4) return fail(ctx, KUQ_E_DB_FORMAT, "can only handle 4 byte DB values");   // :73-74
   uint32_t k = (uint32_t)(key_bits / 2);
   uint64_t key_len = key_bits / 8 + !!(key_bits % 8);
-  if (key_len != 8 || k > 31)
-    return fail(ctx, KUQ_E_UNSUPPORTED_K, "k = %u (key_len %llu): only 8-byte keys (k = 29..31) are supported", k,
+  if (key_bits > 62)
+    return fail(ctx, KUQ_E_UNSUPPORTED_K, "k = %u (key_len %llu): k-mers up to 31 bases are supported", k,
                 (unsigned long long)key_len);
+  const uint64_t pair_sz = key_len + 4;                                      // pair_size(), krakendb.cpp:76,176
   uint64_t header = 72 + 2 * (4 + 8 * key_bits);                           // :177
-  if (kdb_bytes < header + key_ct * 12) return fail(ctx, KUQ_E_DB_FORMAT, "database file truncated");
+  if (kdb_bytes < header + key_ct * pair_sz) return fail(ctx, KUQ_E_DB_FORMAT, "database file truncated");
   const uint8_t *q = (const uint8_t *)idx_image;
   uint32_t idx_type;
   if (idx_bytes < 8) return fail(ctx, KUQ_E_DB_FORMAT, "illegal Kraken DB index format");
@@ -1033,40 +1046,58 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   // bulk H2D.  The images are usually mmap'ed files: a plain cudaMemcpy from pageable memory goes through the driver's
   // single-threaded staging (~7 GB/s, page faults included).  Instead a few threads fault the pages in and copy 64 MB
   // pieces into two pinned bounce buffers while the previous piece travels (cudaMemcpyAsync on the aux stream).
+  // Records shorter than 12 bytes (k <= 28) travel as they are in the file: each piece lands in one bounded device buffer
+  // and k_widen_records writes it into d_pairs in the 12-byte layout, behind the copy on the same stream.
   {
     const uint64_t CH = 64ull << 20;
     const int NT = 8;
+    uint8_t *d_land = nullptr;
+    const uint64_t land_rec = pair_sz == 12 ? 0 : std::min(landing_records(pair_sz), CH / pair_sz);
+    if (land_rec && ctx->key_ct) CU(cudaMalloc((void **)&d_land, land_rec * pair_sz + SLACK));
     uint8_t *bounce[2] = {nullptr, nullptr};
     cudaEvent_t ev[2];
     bool ok = cudaHostAlloc((void **)&bounce[0], CH, cudaHostAllocPortable) == cudaSuccess &&
               cudaHostAlloc((void **)&bounce[1], CH, cudaHostAllocPortable) == cudaSuccess;
     if (!ok) (void)cudaGetLastError();
     for (int b = 0; b < 2; b++) CU(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
-    auto piece_copy = [&](uint8_t *d_dst, const uint8_t *h_src, uint64_t bytes) -> int {
-      if (!ok) { CU(cudaMemcpy(d_dst, h_src, bytes, cudaMemcpyHostToDevice)); return KUQ_OK; }
+    // rec_sz = 0: bytes are copied to d_dst as they are; else they are records of rec_sz bytes, widened into d_dst
+    auto piece_copy = [&](uint8_t *d_dst, const uint8_t *h_src, uint64_t bytes, uint64_t rec_sz) -> int {
+      if (!ok && !rec_sz) { CU(cudaMemcpy(d_dst, h_src, bytes, cudaMemcpyHostToDevice)); return KUQ_OK; }
+      const uint64_t step = rec_sz ? land_rec * rec_sz : CH;
       uint64_t i = 0;
-      for (uint64_t off = 0; off < bytes; off += CH, i++) {
-        const uint64_t n = std::min(CH, bytes - off);
-        const int b = (int)(i & 1);
-        CU(cudaEventSynchronize(ev[b]));                       // the bounce buffer's previous piece has left
-        std::vector<std::thread> th;
-        const uint64_t per = (n + NT - 1) / NT;
-        for (int t = 0; t < NT; t++) {
-          const uint64_t a = std::min(n, per * t), e = std::min(n, per * (t + 1));
-          if (e > a) th.emplace_back([=] { memcpy(bounce[b] + a, h_src + off + a, e - a); });
+      for (uint64_t off = 0; off < bytes; off += step, i++) {
+        const uint64_t n = std::min(step, bytes - off);
+        uint8_t *to = rec_sz ? d_land : d_dst + off;
+        if (!ok) {
+          CU(cudaMemcpyAsync(to, h_src + off, n, cudaMemcpyHostToDevice, ctx->aux));   // in order behind the last widening
+        } else {
+          const int b = (int)(i & 1);
+          CU(cudaEventSynchronize(ev[b]));                       // the bounce buffer's previous piece has left
+          std::vector<std::thread> th;
+          const uint64_t per = (n + NT - 1) / NT;
+          for (int t = 0; t < NT; t++) {
+            const uint64_t a = std::min(n, per * t), e = std::min(n, per * (t + 1));
+            if (e > a) th.emplace_back([=] { memcpy(bounce[b] + a, h_src + off + a, e - a); });
+          }
+          for (auto &x : th) x.join();
+          CU(cudaMemcpyAsync(to, bounce[b], n, cudaMemcpyHostToDevice, ctx->aux));
         }
-        for (auto &x : th) x.join();
-        CU(cudaMemcpyAsync(d_dst + off, bounce[b], n, cudaMemcpyHostToDevice, ctx->aux));
-        CU(cudaEventRecord(ev[b], ctx->aux));
+        if (rec_sz) {
+          launch_widen_records(d_land, n / rec_sz, (uint32_t)(rec_sz - 4), d_dst + off / rec_sz * 12, ctx->aux);
+          ctx->launches++;
+          CU(cudaGetLastError());
+        }
+        if (ok) CU(cudaEventRecord(ev[i & 1], ctx->aux));
       }
       CU(cudaStreamSynchronize(ctx->aux));
       return KUQ_OK;
     };
-    const uint8_t *src = p + header + rec_lo * 12;
-    int crc = piece_copy(ctx->d_pairs, src, ctx->key_ct * 12);
+    const uint8_t *src = p + header + rec_lo * pair_sz;
+    int crc = piece_copy(ctx->d_pairs, src, ctx->key_ct * pair_sz, pair_sz == 12 ? 0 : pair_sz);
     if (!crc) crc = piece_copy(reinterpret_cast<uint8_t *>(ctx->d_offsets_owned), reinterpret_cast<const uint8_t *>(offsets + bin_lo),
-                               (bin_hi - bin_lo + 1) * 8);
+                               (bin_hi - bin_lo + 1) * 8, 0);
     for (int b = 0; b < 2; b++) { cudaEventDestroy(ev[b]); if (bounce[b]) cudaFreeHost(bounce[b]); }
+    cudaFree(d_land);
     if (crc) return crc;
   }
   ctx->db_staged = true;
@@ -2127,6 +2158,8 @@ void stream_close(kuq_ctx *ctx) {
   ctx->copy_stream = nullptr;
   cudaFree(ctx->d_stream_missing);
   ctx->d_stream_missing = nullptr;
+  cudaFree(ctx->d_stream_land);
+  ctx->d_stream_land = nullptr;
   if (ctx->stream_open) { ctx->d_pairs = nullptr; ctx->d_offsets = nullptr; ctx->db_staged = false; }
   ctx->stream_open = false;
 }
@@ -2135,8 +2168,8 @@ void stream_close(kuq_ctx *ctx) {
 
 int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, uint64_t max_records, uint64_t max_bins) {
   if (!ctx || !max_records || !max_bins) return KUQ_E_INVALID_ARG;
-  if (k < 29 || k > 31) return fail(ctx, KUQ_E_UNSUPPORTED_K, "k = %u: only 8-byte keys (k = 29..31)", k);
-  if (nt < 1 || nt > 15 || (idx_type != 1 && idx_type != 2)) return fail(ctx, KUQ_E_INVALID_ARG, "bad index parameters");
+  if (k > 31) return fail(ctx, KUQ_E_UNSUPPORTED_K, "k = %u: k-mers up to 31 bases are supported", k);
+  if (nt < 1 || nt > 15 || nt > k || (idx_type != 1 && idx_type != 2)) return fail(ctx, KUQ_E_INVALID_ARG, "bad index parameters");
   if (ctx->universe.empty()) return fail(ctx, KUQ_E_STATE, "declare the taxids of the whole database first (kuq_set_db_taxid_universe)");
   if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "no taxonomy set");
   CU(cudaSetDevice(ctx->device));
@@ -2176,6 +2209,12 @@ int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, ui
     CU(dmalloc(&b.d_offsets, max_bins + 1));
     CU(cudaEventCreateWithFlags(&b.ready, cudaEventDisableTiming));
   }
+  ctx->stream_pair_sz = (2 * k + 7) / 8 + 4;     // the file's record size: key_len + 4 (krakendb.cpp:76,176)
+  ctx->stream_land_rec = 0;
+  if (ctx->stream_pair_sz != 12) {               // k <= 28: one landing zone, the pieces of both buffers pass through in turn
+    ctx->stream_land_rec = std::min(landing_records(ctx->stream_pair_sz), max_records);
+    CU(cudaMalloc((void **)&ctx->d_stream_land, ctx->stream_land_rec * ctx->stream_pair_sz + SLACK));
+  }
   ctx->stream_cap_records = max_records;
   ctx->stream_cap_bins = max_bins;
   ctx->stream_open = true;
@@ -2198,7 +2237,20 @@ int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64
     CU(cudaEventRecord(s.ev_sync, s.stream));
     CU(cudaStreamWaitEvent(ctx->copy_stream, s.ev_sync, 0));
   }
-  if (n_records) CU(cudaMemcpyAsync(b.d_pairs, host_records, n_records * 12, cudaMemcpyHostToDevice, ctx->copy_stream));
+  if (ctx->stream_pair_sz == 12) {
+    if (n_records) CU(cudaMemcpyAsync(b.d_pairs, host_records, n_records * 12, cudaMemcpyHostToDevice, ctx->copy_stream));
+  } else {
+    // records shorter than 12 bytes: piece by piece through the landing zone, each piece widened in stream order behind
+    // its copy, so the next piece's copy waits for that (on the device, like everything else here)
+    const uint64_t sz = ctx->stream_pair_sz;
+    for (uint64_t r = 0; r < n_records; r += ctx->stream_land_rec) {
+      const uint64_t n = std::min(ctx->stream_land_rec, n_records - r);
+      CU(cudaMemcpyAsync(ctx->d_stream_land, (const uint8_t *)host_records + r * sz, n * sz, cudaMemcpyHostToDevice, ctx->copy_stream));
+      launch_widen_records(ctx->d_stream_land, n, (uint32_t)(sz - 4), b.d_pairs + r * 12, ctx->copy_stream);
+      ctx->launches++;
+    }
+    CU(cudaGetLastError());
+  }
   CU(cudaMemcpyAsync(b.d_offsets, host_offsets, (bin_hi - bin_lo + 1) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
   launch_remap_values(b.d_pairs, n_records, ctx->d_tx_keys, ctx->d_tx_dense, ctx->tx_cap - 1, ctx->d_stream_missing,
                       ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), ctx->copy_stream);
@@ -2727,7 +2779,8 @@ int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes) {
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   const uint64_t key_bits = 2ull * ctx->k, header = 72 + 2 * (4 + 8 * key_bits);
-  if (kdb_bytes < header + ctx->key_ct * 12) return fail(ctx, KUQ_E_INVALID_ARG, "image too small for %llu records", (unsigned long long)ctx->key_ct);
+  const uint64_t key_len = (key_bits + 7) / 8, pair_sz = key_len + 4;            // the file's records, not HBM's 12 bytes
+  if (kdb_bytes < header + ctx->key_ct * pair_sz) return fail(ctx, KUQ_E_INVALID_ARG, "image too small for %llu records", (unsigned long long)ctx->key_ct);
   std::vector<uint8_t> rec(ctx->key_ct * 12);
   CU(cudaMemcpy(rec.data(), ctx->d_pairs, rec.size(), cudaMemcpyDeviceToHost));
   uint8_t *out = (uint8_t *)kdb_image + header;
@@ -2738,7 +2791,7 @@ int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes) {
       if (v >= ctx->n_taxa) return fail(ctx, KUQ_E_STATE, "record %llu holds an unknown dense id %u", (unsigned long long)i, v);
       v = ctx->raw_of_dense[v];
     }
-    memcpy(out + i * 12 + 8, &v, 4);
+    memcpy(out + i * pair_sz + key_len, &v, 4);
   }
   return KUQ_OK;
 }

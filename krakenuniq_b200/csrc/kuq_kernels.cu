@@ -1563,6 +1563,35 @@ void launch_remap_values(uint8_t *pairs, uint64_t n_rec, const uint32_t *keys, c
   int grid = (int)min((uint64_t)device_sm_count() * 8, (n_rec + 255) / 256);
   k_remap_values<<<grid, 256, 0, stream>>>(pairs, n_rec, keys, dense, cap_mask, missing, (uint32_t)(key_mask >> 32));
 }
+// Records of a database with k <= 28 ({key_len-byte key, u32 value}, key_len + 4 bytes each, packed) → the 12-byte
+// {u64 key, u32 value} layout every other kernel reads.  Thread per record: the record's bytes come from the four aligned
+// words that cover them (narrow must be 4-byte aligned with 16 readable bytes past the last record), funnel shifts
+// line them up, the key is zero-extended (the flag bits 62 / 63 start clear) and the value copied.
+__global__ void __launch_bounds__(256) k_widen_records(const uint8_t *__restrict__ narrow, uint64_t n, uint32_t key_len,
+                                                        uint8_t *__restrict__ wide12) {
+  const uint32_t *src = reinterpret_cast<const uint32_t *>(narrow);
+  uint32_t *dst = reinterpret_cast<uint32_t *>(wide12);
+  const uint64_t rec = key_len + 4;
+  const uint64_t key_bytes_mask = (1ull << (8 * key_len)) - 1;        // key_len <= 7
+  const uint32_t vw = key_len >> 2, vsh = 8 * (key_len & 3);
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t off = i * rec;
+    const uint32_t *w = src + (off >> 2);
+    const uint32_t sh = 8 * (uint32_t)(off & 3);
+    const uint32_t w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2), w3 = __ldg(w + 3);
+    const uint32_t a[3] = {__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh)};
+    const uint64_t key = (((uint64_t)a[1] << 32) | a[0]) & key_bytes_mask;
+    dst[3 * i] = (uint32_t)key;
+    dst[3 * i + 1] = (uint32_t)(key >> 32);
+    dst[3 * i + 2] = __funnelshift_r(a[vw], a[vw + 1], vsh);
+  }
+}
+
+void launch_widen_records(const uint8_t *narrow, uint64_t n_rec, uint32_t key_len, uint8_t *wide12, cudaStream_t stream) {
+  if (!n_rec) return;
+  int grid = (int)min((uint64_t)device_sm_count() * 8, (n_rec + 255) / 256);
+  k_widen_records<<<grid, 256, 0, stream>>>(narrow, n_rec, key_len, wide12);
+}
 void launch_register_histograms(const uint8_t *regs, uint32_t n_sketch, uint32_t *hist, cudaStream_t stream) {
   if (!n_sketch) return;
   k_register_histograms<<<min(n_sketch, (uint32_t)device_sm_count() * 16), 256, 0, stream>>>(regs, n_sketch, hist);

@@ -232,6 +232,8 @@ void launch_collect_taxids(const uint8_t *pairs, uint64_t n_rec, uint32_t *keys,
                            uint32_t cap_mask, uint32_t *overflow, cudaStream_t stream);
 void launch_remap_values(uint8_t *pairs, uint64_t n_rec, const uint32_t *keys, const uint32_t *dense,
                          uint32_t cap_mask, uint32_t *missing, uint64_t key_mask, cudaStream_t stream);
+// records of key_len (1..7) + 4 bytes (k <= 28) → 12-byte records at wide12; narrow: 4-byte aligned, 16 bytes of slack
+void launch_widen_records(const uint8_t *narrow, uint64_t n_rec, uint32_t key_len, uint8_t *wide12, cudaStream_t stream);
 // flagged records → keys of the set: mode 0 count (stats[0]), 1 insert + clear, 2 clear SEEN_BIT and KEPT_BIT,
 // 3 kept records → set (not counted again)
 void launch_harvest_seen(uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint8_t *dense_flag, const SparseSet &set,

@@ -3,8 +3,9 @@
 This is workload generation for tests and for the small bench configurations — it is not on the classification
 path.  File layouts follow the reference byte for byte (SURVEY.md App. B):
 
-* database.kdb  — ``JFLISTDN`` header (krakendb.cpp:60-78,177) + 12-byte {u64 key, u32 taxon} records sorted by
-  (bin_key, key) (db_sort.cpp:80-116);
+* database.kdb  — ``JFLISTDN`` header (krakendb.cpp:60-78,177) + packed {key, u32 taxon} records sorted by
+  (bin_key, key) (db_sort.cpp:80-116); the key takes ceil(2k / 8) little-endian bytes, so a record is 12 bytes for
+  k = 29..31 and 8 to 11 bytes for k = 13..28;
 * database.idx  — ``KRAKIX2``/``KRAKIDX`` + nt byte + 4^nt+1 u64 offsets (krakendb.cpp:118-148,534-544);
 * taxDB         — ``taxid \\t parent \\t name \\t rank`` (taxdb.hpp:563-605).
 """
@@ -86,21 +87,35 @@ def kdb_header(k: int, key_ct: int) -> np.ndarray:
     return h
 
 
-_REC = np.dtype([("key", "<u8"), ("taxon", "<u4")])  # packed: itemsize 12
+_REC = np.dtype([("key", "<u8"), ("taxon", "<u4")])  # packed: itemsize 12, the records of k = 29..31
+
+
+def key_len(k: int) -> int:
+    """bytes of a key in database.kdb (krakendb.cpp:76)"""
+    return (2 * k + 7) // 8
+
+
+def pack_records(keys: np.ndarray, vals: np.ndarray, k: int) -> np.ndarray:
+    """packed {key_len-byte key, u32 value} records, little-endian, as one uint8 array"""
+    kl = key_len(k)
+    assert 1 <= kl <= 8
+    keys = np.ascontiguousarray(keys, "<u8")
+    vals = np.ascontiguousarray(vals, "<u4")
+    rec = np.zeros((len(keys), kl + 4), np.uint8)
+    rec[:, :kl] = keys.view(np.uint8).reshape(-1, 8)[:, :kl]
+    rec[:, kl:] = vals.view(np.uint8).reshape(-1, 4)
+    return rec.reshape(-1)
 
 
 def build_db_images(kmers: np.ndarray, taxa: np.ndarray, k: int = 31, nt: int = 8, idx_type: int = 2):
-    """(canonical k-mer, taxon) pairs → (database.kdb image, database.idx image) as uint8 arrays.
-    Only 8-byte keys (k = 29..31 → 12-byte records) are produced."""
-    assert 29 <= k <= 31 and _REC.itemsize == 12
+    """(canonical k-mer, taxon) pairs → (database.kdb image, database.idx image) as uint8 arrays, for any k <= 31
+    (records of key_len(k) + 4 bytes)."""
+    assert 1 <= k <= 31 and nt <= k
     kmers = np.asarray(kmers, np.uint64)
     taxa = np.asarray(taxa, np.uint32)
     bins = bin_key(kmers, k, nt, idx_type)
     order = np.lexsort((kmers, bins))
-    rec = np.zeros(len(kmers), _REC)
-    rec["key"] = kmers[order]
-    rec["taxon"] = taxa[order]
-    kdb = np.concatenate([kdb_header(k, len(kmers)), rec.view(np.uint8)])
+    kdb = np.concatenate([kdb_header(k, len(kmers)), pack_records(kmers[order], taxa[order], k)])
     n_bins = 1 << (2 * nt)
     counts = np.bincount(bins.astype(np.int64), minlength=n_bins)
     offsets = np.zeros(n_bins + 1, np.uint64)
@@ -112,18 +127,21 @@ def build_db_images(kmers: np.ndarray, taxa: np.ndarray, k: int = 31, nt: int = 
 
 def unsorted_jdb_image(kmers: np.ndarray, k: int = 31) -> np.ndarray:
     """A `database.jdb` as Jellyfish would dump it (unsorted keys, zero values) for the reference's db_sort."""
-    rec = np.zeros(len(kmers), _REC)
-    rec["key"] = np.asarray(kmers, np.uint64)
-    return np.concatenate([kdb_header(k, len(kmers)), rec.view(np.uint8)])
+    kmers = np.asarray(kmers, np.uint64)
+    return np.concatenate([kdb_header(k, len(kmers)), pack_records(kmers, np.zeros(len(kmers), np.uint32), k)])
 
 
 def parse_kdb(kdb: np.ndarray):
-    """→ (k, keys u64[n], taxa u32[n]) from a 12-byte-record database.kdb image."""
+    """→ (k, keys u64[n], taxa u32[n]) from a database.kdb image of any record size."""
     key_bits = int(np.frombuffer(kdb[8:16].tobytes(), np.uint64)[0])
     key_ct = int(np.frombuffer(kdb[48:56].tobytes(), np.uint64)[0])
     header = 72 + 2 * (4 + 8 * key_bits)
-    rec = np.frombuffer(kdb[header:header + 12 * key_ct].tobytes(), _REC)
-    return key_bits // 2, rec["key"].copy(), rec["taxon"].copy()
+    kl = key_len(key_bits // 2)
+    rec = np.frombuffer(kdb[header:header + (kl + 4) * key_ct].tobytes(), np.uint8).reshape(key_ct, kl + 4)
+    keys = np.zeros((key_ct, 8), np.uint8)
+    keys[:, :kl] = rec[:, :kl]
+    taxa = np.ascontiguousarray(rec[:, kl:]).view("<u4").reshape(-1)
+    return key_bits // 2, keys.view("<u8").reshape(-1).astype(np.uint64), taxa.astype(np.uint32)
 
 
 class Taxonomy:
