@@ -44,6 +44,9 @@ struct Slot {
   uint8_t *u_cand = nullptr, *u_taxon_cand = nullptr;
   uint64_t *d_canon = nullptr;                 // scratch between the stages
   uint32_t *d_bins = nullptr, *d_dense = nullptr, *d_codes_in = nullptr;
+  PackedBlock *d_pack = nullptr;               // the fused path's 2-bit copy of the batch (k_pack)
+  uint32_t *d_side = nullptr;
+  bool windows_packed = false;                 // the last call's windows are in d_pack, not in d_canon / d_bins
   unsigned long long *d_ovf = nullptr;          // hit-table pool for reads with > 32 distinct taxa
   uint64_t ovf_entries = 0;
   uint32_t *d_run_start = nullptr, *d_run_count = nullptr;
@@ -208,6 +211,7 @@ void free_slot(Slot &s) {
   cudaFree(s.d_bases); cudaFree(s.d_clean); cudaFree(s.d_offsets); cudaFree(s.d_unit); cudaFree(s.d_call);
   cudaFree(s.d_nwin); cudaFree(s.d_codes); cudaFree(s.d_run_start); cudaFree(s.d_run_count); cudaFree(s.d_runs);
   cudaFree(s.d_scalars); cudaFree(s.d_canon); cudaFree(s.d_bins); cudaFree(s.d_dense); cudaFree(s.d_codes_in); cudaFree(s.d_ovf);
+  cudaFree(s.d_pack); cudaFree(s.d_side);
   cudaFree(s.u_keys); cudaFree(s.u_last); cudaFree(s.u_set_keys); cudaFree(s.u_inserts); cudaFree(s.u_distinct);
   cudaFree(s.u_set_count); cudaFree(s.u_ncand); cudaFree(s.u_cand); cudaFree(s.u_taxon_cand); cudaFree(s.u_direct);
   cudaFreeHost(s.h_call); cudaFreeHost(s.h_nwin); cudaFreeHost(s.h_run_start); cudaFreeHost(s.h_run_count);
@@ -298,6 +302,8 @@ int alloc_slot(kuq_ctx *ctx, Slot &s) {
   CU(dmalloc(&s.d_codes, mb + SLACK));
   CU(dmalloc(&s.d_canon, mb + SLACK));
   CU(dmalloc(&s.d_bins, mb + SLACK));
+  CU(dmalloc(&s.d_pack, (mb + SLACK) / 32 + 3));   // blocks up to the one after the last text position
+  CU(dmalloc(&s.d_side, (mb + SLACK) / 32 + 3));
   CU(dmalloc(&s.d_dense, mb + SLACK));
   // worst case one table of < 4 * windows entries per read: 4 entries (64 B) per base always suffices, but reads that
   // need it are rare: a pool of max(bases / 4, 1 Mi) entries + the largest single table
@@ -789,6 +795,8 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   p.total_bases = s.total_bases;
   p.canon = s.d_canon;
   p.bins = s.d_bins;
+  p.pack.blocks = s.d_pack;
+  p.pack.side = s.d_side;
   p.codes_dense = s.d_dense;
   p.run_start = s.d_run_start;
   p.run_count = s.d_run_count;
@@ -856,6 +864,8 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p) {
   } else if (ctx->cfg.hll_mode == KUQ_HLL_PRELOAD) {
     p.unit_id = nullptr;                 // no per-unit bookkeeping for this call
   }
+  p.packed = windows_packed(mode, p) ? 1u : 0u;
+  if (p.n_reads) s.windows_packed = p.packed != 0;
   CU(cudaMemsetAsync(s.d_scalars, 0, 8 * 8, s.stream));
   CU(cudaEventRecord(s.ev_k0, s.stream));
   CU(cudaEventRecord(s.ev_stage[0], s.stream));
@@ -2594,10 +2604,12 @@ int kuq_layout_experiment(kuq_ctx *ctx, uint32_t slot, uint64_t n_positions, uin
     return fail(ctx, KUQ_E_STATE, "run a batch on the slot first; n_positions must not exceed its text length");
   Params p;
   fill_params(ctx, s, p, nullptr, nullptr, nullptr, 0, 0);
+  // a fused call leaves its windows packed: the variants read scratch
+  if (s.windows_packed) launch_unpack_windows(p, n_positions, ctx->n_sm, s.stream);
   const int erc = layout_experiment(p, ctx->key_ct, s.d_canon, s.d_bins, s.d_dense, n_positions, ctx->n_sm, s.stream, reps,
-                                    ctx->cfg.hll_mode == KUQ_HLL_DENSE_ONLY, out);
+                                    ctx->cfg.hll_mode == KUQ_HLL_DENSE_ONLY && s.windows_packed, out);
   ctx->snap_valid = false;
-  ctx->launches += 2 + (uint64_t)KUQ_LAYOUT_VARIANTS * (reps + 2ull);
+  ctx->launches += 2 + (s.windows_packed ? 1 : 0) + (uint64_t)KUQ_LAYOUT_VARIANTS * (reps + 2ull);
   if (erc == 1) return fail(ctx, KUQ_E_NOMEM, "not enough free device memory for the transcoded records");
   if (erc == 3) return fail(ctx, KUQ_E_CAPACITY, "dense taxon ids need more than 24 bits");
   if (erc) return fail(ctx, KUQ_E_CUDA, "layout experiment: %s", cudaGetErrorString(cudaGetLastError()));

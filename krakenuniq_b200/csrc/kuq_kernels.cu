@@ -1,7 +1,9 @@
 // kuq_kernels.cu — see kuq_kernels.cuh for the map from kernel stages to reference functions.
 // Design history: round 1 first fused all stages into one persistent warp-per-read kernel; at 128 registers it ran
-// at 25 % occupancy and was bound by exposed latency, so the path is now three kernels that
-// each keep a small register footprint and hand windows over through HBM scratch (12 B per window, streamed).
+// at 25 % occupancy and was bound by exposed latency, so the path is now three stages that
+// each keep a small register footprint.  The lookup and resolve halves hand windows over through HBM scratch (12 B per
+// window, streamed); the fused call hands over a 2-bit packed copy of the batch (16 B per 32 positions) and the
+// thread-per-window lookup computes its window from it.
 #include "kuq_kernels.cuh"
 
 namespace kuq {
@@ -141,15 +143,22 @@ struct Block64 {         // 32 bases: 2-bit codes, first base in bits 63:62; amb
   bool skip;             // the block holds a '\n' / '\r' (not set for cleaned reads)
 };
 
+// One character → 2-bit code (A=0 C=1 G=2 T=3, case-insensitive, krakenutil.cpp:254-264); false = not ACGT.
+__device__ __forceinline__ bool base_code(uint32_t c, uint32_t &code) {
+  const uint32_t uc = c & 0xDFu;
+  const bool ok = (uc == 'A') | (uc == 'C') | (uc == 'G') | (uc == 'T');
+  code = ok ? (((c >> 1) ^ (c >> 2)) & 3u) : 0u;
+  return ok;
+}
+
 // Convert 32 characters (lane = position) — krakenutil.cpp:253-273.  Positions >= len read as ambiguous.
 __device__ __forceinline__ Block64 load_block(const char *seq, uint32_t len, uint32_t blk, uint32_t lane, bool marks) {
   uint32_t pos = blk * 32 + lane;
   uint32_t c = pos < len ? (uint32_t)(uint8_t)seq[pos] : (uint32_t)'N';
   uint32_t mk = 0;
   if (marks) { mk = c >> 7; c &= 0x7Fu; }
-  uint32_t uc = c & 0xDFu;                                  // case-insensitive, :254-264
-  bool ok = (uc == 'A') | (uc == 'C') | (uc == 'G') | (uc == 'T');
-  uint32_t code = ok ? (((c >> 1) ^ (c >> 2)) & 3u) : 0u;   // A=0 C=1 G=2 T=3
+  uint32_t code;
+  const bool ok = base_code(c, code);
   uint32_t sh = 2 * (15 - (lane & 15));
   uint32_t hi = __reduce_or_sync(0xFFFFFFFFu, lane < 16 ? code << sh : 0u);
   uint32_t lo = __reduce_or_sync(0xFFFFFFFFu, lane >= 16 ? code << sh : 0u);
@@ -165,17 +174,67 @@ __device__ __forceinline__ Block64 load_block(const char *seq, uint32_t len, uin
 constexpr uint32_t BIN_NONE = 0xFFFFFFFFu;    // scratch marker: no window at this position
 constexpr uint32_t BIN_AMBIG = 0xFFFFFFFEu;   // scratch marker: window with a non-ACGT base
 
+// k-mer of the window that starts at base `lane` of the 128-bit string a:b (first base in bits 63:62 of a), k <= 31:
+// the window's bases [lane, lane + k) in its top bits
+__device__ __forceinline__ uint64_t window_top(uint64_t a, uint64_t b, uint32_t lane) {
+  return lane ? (a << (2 * lane)) | (b >> (64 - 2 * lane)) : a;
+}
+// canonical k-mer (krakendb.cpp:238-246)
+__device__ __forceinline__ uint64_t canonical_kmer(uint64_t top, uint32_t k) {
+  const uint64_t kmer = top >> (64 - 2 * k);
+  const uint64_t rc = revcomp64(kmer, k);
+  return kmer < rc ? kmer : rc;
+}
+
+// The windows of one slot of 32 (lane = window start in the 64 bases a:b): canonical k-mer (→ canon) and minimizer bin,
+// or BIN_AMBIG for a window with a non-ACGT base.  Warp-uniform: the minimizer takes shuffles.
+// FAST = the (k, m) = (31, 15) of every published KrakenUniq database, with the window arithmetic as constants.
+template <bool FAST>
+__device__ __forceinline__ uint32_t window_bin(const DbView &db, uint64_t a, uint64_t b, uint64_t amb64, uint32_t lane,
+                                               uint64_t &canon) {
+  const uint32_t k = FAST ? 31u : db.k, nt = FAST ? 15u : db.nt;
+  const uint32_t n_mini = FAST ? 17u : db.n_mini;
+  const uint64_t hi = window_top(a, b, lane);
+  canon = canonical_kmer(hi, k);
+  const bool amb = ((amb64 >> lane) & ((1ull << k) - 1)) != 0;   // any non-ACGT base in the window, :275,280-282
+  // minimizer = min over the k-nt+1 nt-mers of (xor_mask ^ canonical(nt-mer)) (krakendb.cpp:200-215).
+  // Candidate of position q (0..63 relative to the slot): lane holds q = lane (m0) and q = 32+lane (m1).
+  uint32_t f0 = (uint32_t)(hi >> (64 - 2 * nt));
+  uint32_t r0 = revcomp32(f0, nt);
+  uint32_t m0 = db.xor_mask ^ (f0 < r0 ? f0 : r0);
+  uint32_t f1 = (uint32_t)((b << (2 * lane)) >> (64 - 2 * nt));
+  uint32_t r1 = revcomp32(f1, nt);
+  uint32_t m1 = db.xor_mask ^ (f1 < r1 ? f1 : r1);
+  // sliding-window minimum of width n_mini by doubling: after the loop m0 holds min over [q, q+n_mini)
+  uint32_t w = 1;
+#pragma unroll
+  for (int step = 0; step < 5; step++) {                  // n_mini <= 31 → at most 4 doublings
+    if (2 * w > n_mini) break;
+    uint32_t src = (lane + w) & 31;
+    uint32_t x0 = __shfl_sync(0xFFFFFFFFu, m0, src), x1 = __shfl_sync(0xFFFFFFFFu, m1, src);
+    bool wrap = lane + w >= 32;
+    m0 = min(m0, wrap ? x1 : x0);
+    m1 = min(m1, wrap ? 0xFFFFFFFFu : x1);
+    w *= 2;
+  }
+  if (w < n_mini) {                                       // [q, q+n_mini) = [q, q+w) U [q+n_mini-w, q+n_mini)
+    uint32_t d = n_mini - w;
+    uint32_t src = (lane + d) & 31;
+    uint32_t x0 = __shfl_sync(0xFFFFFFFFu, m0, src), x1 = __shfl_sync(0xFFFFFFFFu, m1, src);
+    m0 = min(m0, lane + d >= 32 ? x1 : x0);
+  }
+  return amb ? BIN_AMBIG : m0;
+}
+
 // Stage 1 for one read (one warp, one slot of 32 windows at a time): canonical k-mer and minimizer bin of every
 // window → scratch.  Pure ALU + shuffles, no dependent memory access.
-// FAST = the (k, m) = (31, 15) of every published KrakenUniq database, with the window arithmetic as constants.
 // Returns false (having possibly written a prefix of the read's windows, all of which the caller rewrites) when it
 // meets a skipped character: the read then goes through clean_read.
 template <bool FAST>
 __device__ bool scan_read(const Params &p, uint32_t r, const char *seq, uint32_t len, uint32_t raw_len,
                           uint64_t out_base, uint32_t lane, bool marks) {
   const DbView &db = p.db;
-  const uint32_t k = FAST ? 31u : db.k, nt = FAST ? 15u : db.nt;
-  const uint32_t n_mini = FAST ? 17u : db.n_mini;
+  const uint32_t k = FAST ? 31u : db.k;
   // candidate windows; every one of them is a scanner window unless the read was cleaned (marks), in which case
   // only the marked ones are (the scanner drops a window per skipped character, see clean_read)
   const uint32_t nwin = len >= k ? len - k + 1 : 0;           // classify.cpp:913-914
@@ -193,41 +252,11 @@ __device__ bool scan_read(const Params &p, uint32_t r, const char *seq, uint32_t
       const uint32_t vmask = __ballot_sync(0xFFFFFFFFu, valid);
       const uint32_t oi = n_out + __popc(vmask & ((1u << lane) - 1));   // output slot of this window
       n_out += __popc(vmask);
-      // k-mer of window i: bases [i, i+k) of the 128-bit string A:B
-      uint64_t hi = lane ? (A.codes << (2 * lane)) | (B.codes >> (64 - 2 * lane)) : A.codes;
-      uint64_t kmer = hi >> (64 - 2 * k);
-      uint64_t amb64 = ((uint64_t)B.amb << 32) | A.amb;
-      bool amb = ((amb64 >> lane) & ((1ull << k) - 1)) != 0;  // any non-ACGT base in the window, :275,280-282
-      uint64_t rc = revcomp64(kmer, k);                       // canonical k-mer (krakendb.cpp:238-246)
-      uint64_t canon = kmer < rc ? kmer : rc;
-      // minimizer = min over the k-nt+1 nt-mers of (xor_mask ^ canonical(nt-mer)) (krakendb.cpp:200-215).
-      // Candidate of position q (0..63 relative to the slot): lane holds q = lane (m0) and q = 32+lane (m1).
-      uint32_t f0 = (uint32_t)(hi >> (64 - 2 * nt));
-      uint32_t r0 = revcomp32(f0, nt);
-      uint32_t m0 = db.xor_mask ^ (f0 < r0 ? f0 : r0);
-      uint32_t f1 = (uint32_t)((B.codes << (2 * lane)) >> (64 - 2 * nt));
-      uint32_t r1 = revcomp32(f1, nt);
-      uint32_t m1 = db.xor_mask ^ (f1 < r1 ? f1 : r1);
-      // sliding-window minimum of width n_mini by doubling: after the loop m0 holds min over [q, q+n_mini)
-      uint32_t w = 1;
-#pragma unroll
-      for (int step = 0; step < 5; step++) {                  // n_mini <= 31 → at most 4 doublings
-        if (2 * w > n_mini) break;
-        uint32_t src = (lane + w) & 31;
-        uint32_t x0 = __shfl_sync(0xFFFFFFFFu, m0, src), x1 = __shfl_sync(0xFFFFFFFFu, m1, src);
-        bool wrap = lane + w >= 32;
-        m0 = min(m0, wrap ? x1 : x0);
-        m1 = min(m1, wrap ? 0xFFFFFFFFu : x1);
-        w *= 2;
-      }
-      if (w < n_mini) {                                       // [q, q+n_mini) = [q, q+w) U [q+n_mini-w, q+n_mini)
-        uint32_t d = n_mini - w;
-        uint32_t src = (lane + d) & 31;
-        uint32_t x0 = __shfl_sync(0xFFFFFFFFu, m0, src), x1 = __shfl_sync(0xFFFFFFFFu, m1, src);
-        m0 = min(m0, lane + d >= 32 ? x1 : x0);
-      }
+      // window i: bases [i, i+k) of the 128-bit string A:B
+      uint64_t canon;
+      const uint32_t bin = window_bin<FAST>(db, A.codes, B.codes, ((uint64_t)B.amb << 32) | A.amb, lane, canon);
       if (valid) {
-        p.bins[out_base + oi] = amb ? BIN_AMBIG : m0;
+        p.bins[out_base + oi] = bin;
         p.canon[out_base + oi] = canon;
       }
       A = B;
@@ -362,6 +391,156 @@ __global__ void __launch_bounds__(CTA_THREADS, 4) k_scan(const __grid_constant__
   }
 }
 
+// ------------------------------------------------------------------------------------------------------
+// the fused path's stage 1: a 2-bit packed copy of the batch instead of 12 bytes of scratch per window
+// ------------------------------------------------------------------------------------------------------
+// blocks [g_begin / 32, g_end / 32 + 2): every block a window of the text starts in, and the block after it
+__device__ __forceinline__ uint64_t pack_block_end(uint64_t g_end) { return ((g_end + 31) >> 5) + 1; }
+
+// Position-parallel: one thread converts 16 bases (one 16-byte load), two lanes make a block.  Positions outside the
+// batch's text are ambiguous; start bits are cleared (k_pack_reads sets them).  Blocks holding '\n' / '\r' keep those
+// positions in `side` and are counted in p.chunk_counter (k_scan's chunk scheduler, idle on this path).
+__global__ void __launch_bounds__(256) k_pack(const __grid_constant__ Params p) {
+  const uint64_t g_begin = p.offsets[0], g_end = p.offsets[p.n_reads];
+  const uint64_t h_begin = (g_begin >> 5) * 2, h_end = pack_block_end(g_end) * 2;   // half blocks of 16 bases
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  // warp-uniform trip count: the two lanes of a block meet in a shuffle
+  for (uint64_t h0 = h_begin + (((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull); h0 < h_end; h0 += stride) {
+    const uint64_t h = h0 + lane, pos0 = h * 16;
+    uint32_t code32 = 0, amb16 = 0xFFFFu, crlf16 = 0;
+    if (h < h_end && pos0 < g_end && pos0 + 16 > g_begin) {
+      const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p.bases + pos0));   // bases: 16-byte aligned, 64 B of slack
+      const uint32_t wd[4] = {v.x, v.y, v.z, v.w};
+      amb16 = 0;
+#pragma unroll
+      for (int i = 0; i < 16; i++) {
+        const uint32_t c = (wd[i >> 2] >> (8 * (i & 3))) & 0xFFu;
+        uint32_t code;
+        const bool ok = base_code(c, code);
+        code32 |= code << (2 * (15 - i));
+        amb16 |= ok ? 0u : 1u << i;
+        crlf16 |= (c == '\n' || c == '\r') ? 1u << i : 0u;
+      }
+      // bases outside [g_begin, g_end) belong to no read of the batch
+      const uint32_t lo = g_begin > pos0 ? (uint32_t)(g_begin - pos0) : 0u;
+      const uint32_t hi = g_end - pos0 < 16 ? (uint32_t)(g_end - pos0) : 16u;
+      const uint32_t in = (0xFFFFu >> (16 - hi)) & ~((1u << lo) - 1);
+      amb16 |= ~in & 0xFFFFu;
+      crlf16 &= in;
+    }
+    const uint32_t code_o = __shfl_xor_sync(0xFFFFFFFFu, code32, 1);
+    const uint32_t amb_o = __shfl_xor_sync(0xFFFFFFFFu, amb16, 1);
+    const uint32_t crlf_o = __shfl_xor_sync(0xFFFFFFFFu, crlf16, 1);
+    if (!(lane & 1) && h < h_end) {
+      const uint64_t j = h >> 1;
+      PackedBlock b;
+      b.codes = ((uint64_t)code32 << 32) | code_o;
+      b.amb = amb16 | (amb_o << 16);
+      b.start = 0;
+      p.pack.blocks[j] = b;
+      const uint32_t crlf = crlf16 | (crlf_o << 16);
+      p.pack.side[j] = crlf;
+      if (crlf) atomicAdd(p.chunk_counter, 1u);
+    }
+  }
+}
+
+// Read-parallel, after k_pack: read start bits (and the one at offsets[n_reads]), window counts, and the reads that
+// hold '\n' / '\r': those go through the scanner replay of k_scan (clean_read + scan_read on the cleaned copy), which
+// writes their windows to scratch at the text positions the resolve reads them from; all their positions become side.
+__global__ void __launch_bounds__(256) k_pack_reads(const __grid_constant__ Params p) {
+  const uint32_t lane = threadIdx.x & 31, k = p.db.k;
+  const bool any_crlf = *reinterpret_cast<volatile uint32_t *>(p.chunk_counter) != 0;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t r0 = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; r0 <= p.n_reads; r0 += stride) {   // warp-uniform
+    const uint32_t r = r0 + lane;
+    uint64_t b0 = 0, b1 = 0;
+    bool side = false;
+    if (r <= p.n_reads) {
+      b0 = p.offsets[r];
+      atomicOr(&p.pack.blocks[b0 >> 5].start, 1u << (b0 & 31));
+      if (r < p.n_reads) {
+        b1 = p.offsets[r + 1];
+        // '\n' / '\r' inside [b0, b1) (k_pack left only those bits in side; neighbours only add bits of their own reads)
+        for (uint64_t j = b0 >> 5; any_crlf && b1 > b0 && j <= (b1 - 1) >> 5 && !side; j++) {
+          uint64_t m = p.pack.side[j];
+          const uint64_t base = j << 5;
+          if (b0 > base) m &= ~0ull << (b0 - base);
+          if (b1 < base + 32) m &= (1ull << (b1 - base)) - 1;
+          side = m != 0;
+        }
+        const uint64_t len = b1 - b0;
+        if (!side) p.n_windows[r] = len >= k ? (uint32_t)(len - k + 1) : 0u;      // classify.cpp:913-914
+      }
+    }
+    for (uint32_t todo = __ballot_sync(0xFFFFFFFFu, side); todo; todo &= todo - 1) {
+      const int src = __ffs(todo) - 1;
+      const uint64_t s0 = __shfl_sync(0xFFFFFFFFu, b0, src), s1 = __shfl_sync(0xFFFFFFFFu, b1, src);
+      const uint32_t raw_len = (uint32_t)(s1 - s0);
+      const uint32_t len = clean_read(p.bases + s0, raw_len, p.clean + s0, k, lane);
+      scan_read<false>(p, r0 + src, p.clean + s0, len, raw_len, s0, lane, true);
+      for (uint64_t j = (s0 >> 5) + lane; j <= (s1 - 1) >> 5; j += 32) {
+        const uint64_t base = j << 5;
+        uint64_t m = 0xFFFFFFFFull;
+        if (s0 > base) m &= ~0ull << (s0 - base);
+        if (s1 < base + 32) m &= (1ull << (s1 - base)) - 1;
+        atomicOr(p.pack.side + j, (uint32_t)m);
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ PackedBlock load_packed(const PackedBlock *b) {
+  const uint4 v = __ldg(reinterpret_cast<const uint4 *>(b));
+  PackedBlock r;
+  r.codes = ((uint64_t)v.y << 32) | v.x;
+  r.amb = v.z;
+  r.start = v.w;
+  return r;
+}
+
+// Window of text position 32j + lane from the packed blocks a = j and b = j + 1 (warp-uniform, see window_bin): its
+// bin (BIN_NONE when a read starts inside (g, g + k), i.e. the read ends before the window does) and canonical k-mer.
+template <bool FAST>
+__device__ __forceinline__ uint32_t packed_window(const DbView &db, const PackedBlock &a, const PackedBlock &b, uint32_t lane,
+                                                  uint64_t &canon) {
+  const uint32_t k = FAST ? 31u : db.k;
+  const uint32_t bin = window_bin<FAST>(db, a.codes, b.codes, ((uint64_t)b.amb << 32) | a.amb, lane, canon);
+  const uint64_t starts = ((uint64_t)b.start << 32) | a.start;
+  return ((starts >> (lane + 1)) & ((1ull << (k - 1)) - 1)) ? BIN_NONE : bin;
+}
+
+// canonical k-mer of the window at text position g of a call whose windows are packed (or of scratch otherwise)
+__device__ __forceinline__ uint64_t window_canon(const Params &p, uint64_t g) {
+  const uint64_t j = g >> 5;
+  const uint32_t l = (uint32_t)g & 31u;
+  if (!p.packed || ((p.pack.side[j] >> l) & 1u)) return p.canon[g];
+  return canonical_kmer(window_top(p.pack.blocks[j].codes, p.pack.blocks[j + 1].codes, l), p.db.k);
+}
+
+// scratch (canon / bins) of the positions [0, n_pos) from the packed blocks; side positions hold their windows already
+template <bool FAST>
+__global__ void __launch_bounds__(256) k_unpack_windows(const __grid_constant__ Params p, uint64_t n_pos) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t j = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < (n_pos + 31) >> 5; j += warps) {
+    uint64_t canon;
+    const uint32_t bin = packed_window<FAST>(p.db, load_packed(p.pack.blocks + j), load_packed(p.pack.blocks + j + 1), lane, canon);
+    const uint64_t g = (j << 5) + lane;
+    if (g < n_pos && !((p.pack.side[j] >> lane) & 1u)) {
+      p.bins[g] = bin;
+      p.canon[g] = canon;
+    }
+  }
+}
+
+void launch_unpack_windows(const Params &p, uint64_t n_pos, int n_sm, cudaStream_t stream) {
+  const int grid = (int)max((uint64_t)1, min((uint64_t)n_sm * 8, (n_pos + 255) / 256));
+  if (p.db.k == 31 && p.db.nt == 15) k_unpack_windows<true><<<grid, 256, 0, stream>>>(p, n_pos);
+  else k_unpack_windows<false><<<grid, 256, 0, stream>>>(p, n_pos);
+}
+
 // Stage 2: one thread per text position.  Index fetch (KrakenDBIndex::at, krakendb.cpp:586-593), bin search
 // (kmer_query, :280-299: 4-ary narrowing while the bin is large, then a scan of <= 8 records) and — unless the
 // lookups belong to one range of a sharded database — the HLL insert of ReadCounts::add_kmer (classify.cpp:939).
@@ -371,7 +550,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 4) k_scan(const __grid_constant__
 // output, peer buffers.  Those are launch-uniform run-time switches; compiled out, the common path of the fused kernel
 // is a third shorter.
 template <int MODE, bool LEAN>
-__global__ void __launch_bounds__(256, 8) k_lookup(const __grid_constant__ Params p) {
+__device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint32_t bin, uint64_t canon) {
   const DbView &db = p.db;
   const uint32_t flags = LEAN ? (p.flags & 4u) : p.flags;
   const uint32_t only_hits = LEAN ? 0u : p.only_hits;
@@ -385,22 +564,11 @@ __global__ void __launch_bounds__(256, 8) k_lookup(const __grid_constant__ Param
   // the misses (taxon 0).  Valid because every looked-up window is counted exactly once in that layout.
   const bool shard_counting = (flags & 32u) != 0;
   const bool mark_seen = (counting || (MODE == MODE_LOOKUP && shard_counting)) && p.hll_mode <= 1u;
-  // only the text of this call's reads (the scratch beyond it may hold windows of an earlier call on the slot)
-  const uint64_t g_begin = p.offsets[0], g_end = p.offsets[p.n_reads];
-  // the scratch of the NEXT position of this thread is fetched while the current window is searched: the grid-stride
-  // loop would otherwise start every window with an exposed (streaming, but still ~1 us) load
-  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  uint64_t g = g_begin + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t bin_n = g < g_end ? __ldg(p.bins + g) : BIN_NONE;
-  uint64_t canon_n = g < g_end ? __ldg(p.canon + g) : 0ull;
-  for (; g < g_end; g += stride) {
-    const uint32_t bin = bin_n;
-    const uint64_t canon = canon_n;
-    if (g + stride < g_end) { bin_n = __ldg(p.bins + g + stride); canon_n = __ldg(p.canon + g + stride); }
-    if (bin == BIN_NONE) continue;
+  {
+    if (bin == BIN_NONE) return;
     if (bin == BIN_AMBIG) {
       if (!only_hits && !(MODE == MODE_LOOKUP && n_peers)) p.codes_dense[g] = AMBIG;
-      continue;
+      return;
     }
     uint32_t taxon = 0;
     if (MODE == MODE_RESOLVE) {
@@ -481,6 +649,53 @@ __global__ void __launch_bounds__(256, 8) k_lookup(const __grid_constant__ Param
         if (ins > 0) atomicAdd(p.sparse.distinct + taxon, 1u);
         else if (ins < 0) atomicExch(p.error_flag, 4u);       // set saturated
       }
+    }
+  }
+}
+
+// MODE_FUSED computes its windows from the packed blocks (FAST: k = 31, m = 15, see window_bin) instead of reading
+// 12 bytes of scratch per position: a warp takes 32 consecutive positions (one block) at a time, from a contiguous
+// range of blocks, so block j + 1 of one step is block j of the next.  Side positions (reads with '\n' / '\r') read
+// their windows from scratch.  The other modes read k_scan's scratch.
+// The generic-k fused path needs a few registers more than 32 (6 CTAs per SM, 40 registers, no spills).
+template <int MODE, bool LEAN, bool FAST = false>
+__global__ void __launch_bounds__(256, (MODE == MODE_FUSED && !FAST) ? 6 : 8) k_lookup(const __grid_constant__ Params p) {
+  // only the text of this call's reads (the scratch beyond it may hold windows of an earlier call on the slot)
+  const uint64_t g_begin = p.offsets[0], g_end = p.offsets[p.n_reads];
+  if constexpr (MODE == MODE_FUSED) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint64_t j_begin = g_begin >> 5, n_blk = ((g_end + 31) >> 5) - j_begin;
+    const uint64_t per = (n_blk + warps - 1) / warps;
+    uint64_t j = j_begin + warp * per;
+    const uint64_t j_end = min(j + per, j_begin + n_blk);
+    if (j >= j_end) return;
+    PackedBlock a = load_packed(p.pack.blocks + j), b = load_packed(p.pack.blocks + j + 1);
+    for (; j < j_end; j++) {
+      const PackedBlock c = load_packed(p.pack.blocks + j + 2);
+      const uint32_t side = p.pack.side[j];
+      const uint64_t g = (j << 5) + lane;
+      uint64_t canon;
+      uint32_t bin = packed_window<FAST>(p.db, a, b, lane, canon);
+      if ((side >> lane) & 1u) { bin = p.bins[g]; canon = p.canon[g]; }
+      if (g < g_begin || g >= g_end) bin = BIN_NONE;
+      lookup_window<MODE, LEAN>(p, g, bin, canon);
+      a = b;
+      b = c;
+    }
+  } else {
+    // the scratch of the NEXT position of this thread is fetched while the current window is searched: the grid-stride
+    // loop would otherwise start every window with an exposed (streaming, but still ~1 us) load
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    uint64_t g = g_begin + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t bin_n = g < g_end ? __ldg(p.bins + g) : BIN_NONE;
+    uint64_t canon_n = g < g_end ? __ldg(p.canon + g) : 0ull;
+    for (; g < g_end; g += stride) {
+      const uint32_t bin = bin_n;
+      const uint64_t canon = canon_n;
+      if (g + stride < g_end) { bin_n = __ldg(p.bins + g + stride); canon_n = __ldg(p.canon + g + stride); }
+      lookup_window<MODE, LEAN>(p, g, bin, canon);
     }
   }
 }
@@ -925,7 +1140,7 @@ __global__ void __launch_bounds__(256) k_unit_distinct(const __grid_constant__ P
       if (sl == 0xFFFFFFFFu || !u.cand[sl]) continue;
       atomicMax(u.last + sl, ((unsigned long long)r << 32) | i);
       if (*reinterpret_cast<volatile uint32_t *>(u.distinct + sl) >= 1025u) continue;   // decided already
-      const uint32_t code = encode_hash32(fmix64(p.canon[base + i]));
+      const uint32_t code = encode_hash32(fmix64(window_canon(p, base + i)));
       const unsigned long long key = ((unsigned long long)(sl + 1) << 32) | code;
       uint32_t q = (uint32_t)mix64(key) & u.set_mask;
       for (uint32_t probe = 0; probe <= u.set_mask; probe++) {
@@ -955,7 +1170,7 @@ __global__ void k_unit_apply(const __grid_constant__ Params p) {
     if (!conv && d == 1024u) {
       const unsigned long long lp = u.last[s];
       const uint32_t r = (uint32_t)(lp >> 32), i = (uint32_t)lp;
-      const uint32_t code = encode_hash32(fmix64(p.canon[p.offsets[r] + i]));
+      const uint32_t code = encode_hash32(fmix64(window_canon(p, p.offsets[r] + i)));
       const unsigned long long key = ((unsigned long long)(s + 1) << 32) | code;
       uint32_t q = (uint32_t)mix64(key) & u.set_mask;
       for (uint32_t probe = 0; probe <= u.set_mask; probe++) {
@@ -1205,10 +1420,24 @@ int classify_smem_bytes() { return N_STAGES * STAGE_BYTES + (int)sizeof(SharedSt
 //      MODE_RESOLVE: scan → HLL from merged codes → resolve    (owner of the reads after the merge)
 // picks the lean instantiation when the launch uses none of the rare switches (see k_lookup)
 template <int MODE>
-static void launch_lookup(const Params &q, int lgrid, cudaStream_t stream) {
-  const bool lean = !(q.flags & (8u | 16u | 32u)) && !q.only_hits && !q.n_peers;
+static void launch_lookup(const Params &q, int lgrid, cudaStream_t stream, bool lean) {
+  if constexpr (MODE == MODE_FUSED) {
+    if (q.db.k == 31 && q.db.nt == 15) {
+      if (lean) k_lookup<MODE, true, true><<<lgrid, 256, 0, stream>>>(q);
+      else k_lookup<MODE, false, true><<<lgrid, 256, 0, stream>>>(q);
+      return;
+    }
+  }
   if (lean) k_lookup<MODE, true><<<lgrid, 256, 0, stream>>>(q);
   else k_lookup<MODE, false><<<lgrid, 256, 0, stream>>>(q);
+}
+template <int MODE>
+static void launch_lookup(const Params &q, int lgrid, cudaStream_t stream) {
+  launch_lookup<MODE>(q, lgrid, stream, !(q.flags & (8u | 16u | 32u)) && !q.only_hits && !q.n_peers);
+}
+
+bool windows_packed(int mode, const Params &p) {
+  return mode == MODE_FUSED && p.hll_mode != 3u && !(p.quick_min != 0 && p.quick_stop);
 }
 
 int launch_classify(int mode, const Params &p, int n_sm, cudaStream_t stream, cudaEvent_t *stage_events) {
@@ -1217,10 +1446,17 @@ int launch_classify(int mode, const Params &p, int n_sm, cudaStream_t stream, cu
   cudaFuncSetAttribute(k_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   int launches = 0;
   if (p.n_reads == 0) return 0;
-  int grid = n_sm * 4;
-  if ((uint32_t)grid > p.n_chunks) grid = (int)p.n_chunks;
-  k_scan<<<grid, CTA_THREADS, smem, stream>>>(p);
-  launches++;
+  if (windows_packed(mode, p)) {
+    const uint64_t n_half = 2 * (p.total_bases / 32 + 2);
+    k_pack<<<(int)min((uint64_t)n_sm * 8, (n_half + 255) / 256), 256, 0, stream>>>(p);
+    k_pack_reads<<<(int)min((uint32_t)n_sm * 8, (p.n_reads + 256) / 256), 256, 0, stream>>>(p);
+    launches += 2;
+  } else {
+    int grid = n_sm * 4;
+    if ((uint32_t)grid > p.n_chunks) grid = (int)p.n_chunks;
+    k_scan<<<grid, CTA_THREADS, smem, stream>>>(p);
+    launches++;
+  }
   if (stage_events) cudaEventRecord(stage_events[0], stream);
   const int lgrid = (int)min((uint64_t)n_sm * 8 * 8, (p.total_bases + 255) / 256);
   const bool quick = p.quick_min != 0 && mode != MODE_LOOKUP;
@@ -1327,18 +1563,14 @@ int launch_scan_only(const Params &p, int n_sm, cudaStream_t stream) {
   return 1;
 }
 
-// stage 2 alone over scratch that is already there (kuq_layout_exp.cu times the product's kernel next to its variants):
-// p.offsets = {first, last + 1} text positions with p.n_reads = 1
-// fused = 1: k_lookup<MODE_FUSED> (counts into the sketches of p); lean: see k_lookup (the caller vouches for the flags)
+// stage 2 alone over windows that are already there (kuq_layout_exp.cu times the product's kernel next to its
+// variants): p.offsets = {first, last + 1} text positions with p.n_reads = 1
+// fused = 1: k_lookup<MODE_FUSED> over the packed blocks of p (counts into the sketches of p); fused = 0: MODE_LOOKUP over
+// scratch; lean: see k_lookup (the caller vouches for the flags)
 int launch_lookup_only(const Params &p, int n_sm, cudaStream_t stream, int fused, int lean) {
   const int lgrid = (int)max((uint64_t)1, min((uint64_t)n_sm * 8 * 8, (p.total_bases + 255) / 256));
-  if (fused) {
-    if (lean) k_lookup<MODE_FUSED, true><<<lgrid, 256, 0, stream>>>(p);
-    else k_lookup<MODE_FUSED, false><<<lgrid, 256, 0, stream>>>(p);
-  } else {
-    if (lean) k_lookup<MODE_LOOKUP, true><<<lgrid, 256, 0, stream>>>(p);
-    else k_lookup<MODE_LOOKUP, false><<<lgrid, 256, 0, stream>>>(p);
-  }
+  if (fused) launch_lookup<MODE_FUSED>(p, lgrid, stream, lean != 0);
+  else launch_lookup<MODE_LOOKUP>(p, lgrid, stream, lean != 0);
   return 1;
 }
 

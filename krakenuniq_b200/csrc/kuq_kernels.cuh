@@ -1,12 +1,14 @@
 // kuq_kernels.cuh — sm_90a kernels of the KrakenUniq classification hot path (device side of libkuq.so).
 //
-// The per-read path of the reference's classify_sequence() (src/classify.cpp:897-1012) as three kernels:
+// The per-read path of the reference's classify_sequence() (src/classify.cpp:897-1012) as three stages:
 //
 //  k_scan     read blocks --TMA bulk copy--> shared memory    (cp.async.bulk + mbarrier, double buffered)
 //   (warp     2-bit packing + ambiguity mask   KmerScanner::next_kmer   src/krakenutil.cpp:239-282
 //    per      canonical k-mer                  canonical_representation src/krakendb.cpp:238-246
 //    read)    rolling minimizer                bin_key                  src/krakendb.cpp:200-215
 //             → scratch: canonical k-mer + bin per window (12 B, coalesced)
+//   or, for the fused call, k_pack (thread per 16 bases) + k_pack_reads (thread per read): 2-bit codes, ambiguity and
+//   read-start masks per 32 text positions (16 B) — the lookup computes each window itself from two such blocks
 //  k_lookup   index fetch + bin search         kmer_query               src/krakendb.cpp:250-321, :586-593
 //   (thread   HLL register update              ReadCounts::add_kmer     src/readcounts.hpp:71-74,
 //    per                                                                 hyperloglogplus.cpp:485-523
@@ -157,6 +159,17 @@ struct ExactSet {
   unsigned long long *count;   // [n_sketch] distinct k-mers per taxon == khset size (readcounts.hpp:127-130)
 };
 
+// 2-bit packed copy of a batch (k_pack): block j holds the text positions [32j, 32j + 32), indexed like bases / 32
+struct __align__(16) PackedBlock {
+  uint64_t codes;              // 2-bit codes, position 32j in bits 63:62 (non-ACGT bases as A)
+  uint32_t amb;                // bit l = position 32j + l is not ACGT (or lies outside the batch's text)
+  uint32_t start;              // bit l = a read starts at 32j + l (also set at offsets[n_reads])
+};
+struct PackView {
+  PackedBlock *blocks;
+  uint32_t *side;              // bit l = position 32j + l belongs to a read holding '\n' / '\r': its windows are in scratch
+};
+
 struct Params {
   DbView db;
   TaxView tax;
@@ -179,6 +192,8 @@ struct Params {
   uint32_t *bins;               // minimizer bin, or BIN_AMBIG / BIN_NONE
   uint32_t *codes_dense;        // dense taxon id of the window (0 = miss) or AMBIG
   const uint32_t *codes_in;     // MODE_RESOLVE: merged dense ids
+  PackView pack;                // the fused path's windows (see windows_packed)
+  uint32_t packed;              // this call's windows come from `pack` (canon / bins hold only those of side reads)
   uint32_t *run_start;
   uint32_t *run_count;
   uint2 *runs;
@@ -215,8 +230,15 @@ struct Params {
   uint32_t lca_keep[2];         // dense ids of taxids 32630 / 81077 (0 = not in the taxonomy)
 };
 
-// returns #kernels launched; stage_events[0] / [1] (optional) are recorded after k_scan / k_lookup
+// The fused lookup computes its windows itself from the packed copy of the batch; exact counting and quick-stop runs
+// (and the lookup / resolve halves) read k_scan's scratch.  The caller sets p.packed from this before launch_classify.
+bool windows_packed(int mode, const Params &p);
+// returns #kernels launched; stage_events[0] / [1] (optional) are recorded after k_scan (or k_pack + k_pack_reads) /
+// k_lookup
 int launch_classify(int mode, const Params &p, int n_sm, cudaStream_t stream, cudaEvent_t *stage_events);
+// canon / bins of the text positions [0, n_pos) from the packed copy the last fused call left in p.pack (side reads'
+// windows are in scratch already): the scratch layout k_scan writes, for kuq_layout_experiment
+void launch_unpack_windows(const Params &p, uint64_t n_pos, int n_sm, cudaStream_t stream);
 int classify_smem_bytes();
 int device_sm_count();
 // set_lcas: k_scan + k_set_lcas over library pieces (p.unit_id = dense taxid per piece, p.stats[0] += k-mers not found)
