@@ -450,6 +450,43 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
  * stride (key_len + 4 bytes), whatever the staged layout. */
 int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes);
 
+/* k-mer set of a FASTA library: step 1 of build_db.sh (scripts/build_db.sh:116-147), `jellyfish count -m k -C` of
+ * Jellyfish 1, whose output database_0 becomes database.jdb.  The set holds one record per distinct canonical k-mer
+ * (canonical_representation, krakendb.cpp:238-246) of the windows KmerScanner (krakenutil.cpp:239-282) yields over each
+ * sequence: key_len(k) = ceil(2k / 8) little-endian key bytes + the u32 number of occurrences (saturated at 2^32 - 1),
+ * the records of database.kdb.  Records come in ascending key order; Jellyfish writes them in hash order, which only
+ * db_shrink depends on.  Needs no context.
+ *
+ * kuq_kmer_set_create: device ordinal, k = 1..31, budget = bytes of HBM for the packed library and one pass over a
+ *   range of k-mers (0 → environment variable KUQ_KMER_SET_BUDGET, else 3/4 of the free device memory).  Batches of
+ *   KUQ_KMER_SET_BATCH bases (default 256 Mi) are staged through two pinned buffers; their device buffers come on top
+ *   of the budget until the first kuq_kmer_set_next / _info.  err (optional) receives a message on failure.
+ * kuq_kmer_set_add: sequences r = bases[offsets[r] .. offsets[r + 1]) — what FastaReader::next_sequence
+ *   (seqreader.cpp:34-79) returns; any letter but ACGTacgt makes its windows ambiguous, windows never cross sequences,
+ *   and a '\n' / '\r' (CRLF files) is left out of the k-mers but costs the window KmerScanner then skips
+ *   (krakenutil.cpp:265-269; sequences holding them take a slower host path).  Copies the bases; asynchronous on the device, so the caller can
+ *   parse the next batch while this one is packed.  A sequence longer than a batch is cut into pieces overlapping by
+ *   k - 1 bases (set_lcas.cpp:363-364), which keeps the multiset of windows.
+ * kuq_kmer_set_next: up to cap_records records into records_out (cap_records * (key_len + 4) bytes), continuing in
+ *   ascending key order; *n_out = 0 at the end.  The first call plans the passes from a histogram of the top 16 key
+ *   bits (KUQ_E_CAPACITY when one histogram bucket alone exceeds a pass under the budget); every pass extracts, sorts and
+ *   collapses one range of keys, so the whole set never sits in host memory.
+ * kuq_kmer_set_info: *key_ct = records produced so far (the set's size once kuq_kmer_set_next returned 0 records),
+ *   *n_passes = planned passes.
+ * kuq_kmer_set_stats (measurement aid): device time in ms of the stages so far — [0] pack + histogram, [1] extract,
+ *   [2] sort, [3] collapse, [4] record copy to the host —, the number of windows, the planner's estimate of the device
+ *   bytes a pass needs (library included), the measured drop of free device memory at the passes' peak, and whether the
+ *   packed library is in HBM (1) or pinned host memory (0). */
+typedef struct kuq_kmer_set kuq_kmer_set;
+int kuq_kmer_set_create(int device, uint32_t k, uint64_t budget, kuq_kmer_set **out, char *err, uint64_t err_cap);
+int kuq_kmer_set_add(kuq_kmer_set *h, const char *bases, const uint64_t *offsets, uint32_t n_seqs);
+int kuq_kmer_set_next(kuq_kmer_set *h, void *records_out, uint64_t cap_records, uint64_t *n_out);
+int kuq_kmer_set_info(kuq_kmer_set *h, uint64_t *key_ct, uint32_t *n_passes);
+int kuq_kmer_set_stats(kuq_kmer_set *h, double *stage_ms5, uint64_t *windows, uint64_t *ws_estimate_bytes,
+                       uint64_t *peak_bytes, int *lib_on_device);
+const char *kuq_kmer_set_last_error(const kuq_kmer_set *h);
+void kuq_kmer_set_destroy(kuq_kmer_set *h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -177,6 +177,13 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_layout_experiment": (C.c_int, [vp, C.c_uint32, C.c_uint64, C.c_uint32, C.POINTER(LayoutResult)]),
         "kuq_random_gather_peak": (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_uint32, C.POINTER(C.c_double),
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+        "kuq_kmer_set_create": (C.c_int, [C.c_int, C.c_uint32, C.c_uint64, C.POINTER(vp), C.c_char_p, C.c_uint64]),
+        "kuq_kmer_set_add": (C.c_int, [vp, vp, u64p, C.c_uint32]),
+        "kuq_kmer_set_next": (C.c_int, [vp, vp, C.c_uint64, u64p]),
+        "kuq_kmer_set_info": (C.c_int, [vp, u64p, u32p]),
+        "kuq_kmer_set_stats": (C.c_int, [vp, C.POINTER(C.c_double), u64p, u64p, u64p, C.POINTER(C.c_int)]),
+        "kuq_kmer_set_last_error": (C.c_char_p, [vp]),
+        "kuq_kmer_set_destroy": (None, [vp]),
     }
     for name, (res, args) in sigs.items():
         f = getattr(L, name)            # AttributeError here = the library does not export what kuq.h declares
@@ -610,3 +617,93 @@ def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0):
     if rc != 0:
         raise KuqError(rc, err.value.decode() or L.kuq_strerror(rc).decode())
     return kdb, idx
+
+
+def kdb_header(k: int, key_ct: int) -> np.ndarray:
+    """header of a Jellyfish-1 style k-mer file (SURVEY App. A16): JFLISTDN, key_bits = 2k, val_len = 4, key_ct"""
+    h = np.zeros(72 + 2 * (4 + 8 * 2 * k), np.uint8)
+    h[:8] = np.frombuffer(b"JFLISTDN", np.uint8)
+    h[8:24] = np.array([2 * k, 4], "<u8").view(np.uint8)
+    h[48:56] = np.array([key_ct], "<u8").view(np.uint8)
+    return h
+
+
+class KmerSet:
+    """kuq_kmer_set_*: the canonical k-mer set of a library with its counts (step 1 of build_db.sh) on the GPU."""
+
+    def __init__(self, k, budget=None, device=0):
+        self.L = load_library()
+        self.k, self.rec = k, (2 * k + 7) // 8 + 4
+        h, err = C.c_void_p(), C.create_string_buffer(1024)
+        rc = self.L.kuq_kmer_set_create(device, k, budget or 0, C.byref(h), err, 1024)
+        if rc != 0:
+            raise KuqError(rc, err.value.decode() or self.L.kuq_strerror(rc).decode())
+        self.h = h
+
+    def _ck(self, rc):
+        if rc != 0:
+            raise KuqError(rc, f"{self.L.kuq_strerror(rc).decode()}: {self.L.kuq_kmer_set_last_error(self.h).decode()}")
+
+    def add(self, bases: np.ndarray, offsets: np.ndarray):
+        bases = np.ascontiguousarray(bases, np.uint8)
+        offsets = np.ascontiguousarray(offsets, np.uint64)
+        buf = bases if bases.size else np.zeros(1, np.uint8)
+        self._ck(self.L.kuq_kmer_set_add(self.h, buf.ctypes.data, _p(offsets, u64p), len(offsets) - 1))
+
+    def next(self, out: np.ndarray) -> int:
+        """fill `out` (uint8, a multiple of the record size) with the next records; returns how many (0 = done)"""
+        n = C.c_uint64(0)
+        self._ck(self.L.kuq_kmer_set_next(self.h, out.ctypes.data, out.size // self.rec, C.byref(n)))
+        return n.value
+
+    def info(self):
+        """(records produced so far, planned passes)"""
+        n, p = C.c_uint64(0), C.c_uint32(0)
+        self._ck(self.L.kuq_kmer_set_info(self.h, C.byref(n), C.byref(p)))
+        return n.value, p.value
+
+    def stats(self):
+        ms, w, est, peak, dev = (C.c_double * 5)(), C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_int()
+        self._ck(self.L.kuq_kmer_set_stats(self.h, ms, C.byref(w), C.byref(est), C.byref(peak), C.byref(dev)))
+        return {"stage_ms": dict(zip(["pack_hist", "extract", "sort", "collapse", "d2h"], list(ms))), "windows": w.value,
+                "ws_estimate_bytes": est.value, "peak_bytes": peak.value, "library_in_hbm": bool(dev.value)}
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.kuq_kmer_set_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def kmer_set(bases: np.ndarray, offsets: np.ndarray, k: int, budget=None, batch=None, device=0):
+    """The k-mer file `kmer_set count -m k -C` writes (database_0) for the sequences bases[offsets[r]:offsets[r+1]]:
+    header + one record per distinct canonical k-mer with its count, ascending.  batch = bases per device batch
+    (KUQ_KMER_SET_BATCH).  Returns (image uint8, number of passes)."""
+    old = os.environ.get("KUQ_KMER_SET_BATCH")
+    if batch:
+        os.environ["KUQ_KMER_SET_BATCH"] = str(int(batch))
+    try:
+        ks = KmerSet(k, budget, device)
+    finally:
+        if batch:
+            if old is None:
+                del os.environ["KUQ_KMER_SET_BATCH"]
+            else:
+                os.environ["KUQ_KMER_SET_BATCH"] = old
+    try:
+        ks.add(bases, offsets)
+        parts, buf = [], np.zeros((1 << 20) * ks.rec, np.uint8)
+        while True:
+            n = ks.next(buf)
+            if not n:
+                break
+            parts.append(buf[:n * ks.rec].copy())
+        key_ct, passes = ks.info()
+    finally:
+        ks.close()
+    return np.concatenate([kdb_header(k, key_ct)] + parts), passes

@@ -46,12 +46,6 @@ __device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gmem_src
 // ------------------------------------------------------------------------------------------------------
 // bit arithmetic
 // ------------------------------------------------------------------------------------------------------
-// KrakenDB::reverse_complement (krakendb.cpp:218-225): reverse the 2-bit groups, complement, shift down.
-__device__ __forceinline__ uint64_t revcomp64(uint64_t x, uint32_t n) {
-  x = __brevll(x);                                                              // reverses bits inside groups too
-  x = ((x >> 1) & 0x5555555555555555ull) | ((x & 0x5555555555555555ull) << 1);  // ... so swap them back
-  return (~x) >> (64 - 2 * n);
-}
 __device__ __forceinline__ uint32_t revcomp32(uint32_t x, uint32_t n) {   // n <= 15
   x = __brev(x);
   x = ((x >> 1) & 0x55555555u) | ((x & 0x55555555u) << 1);
@@ -143,13 +137,6 @@ struct Block64 {         // 32 bases: 2-bit codes, first base in bits 63:62; amb
   bool skip;             // the block holds a '\n' / '\r' (not set for cleaned reads)
 };
 
-// One character → 2-bit code (A=0 C=1 G=2 T=3, case-insensitive, krakenutil.cpp:254-264); false = not ACGT.
-__device__ __forceinline__ bool base_code(uint32_t c, uint32_t &code) {
-  const uint32_t uc = c & 0xDFu;
-  const bool ok = (uc == 'A') | (uc == 'C') | (uc == 'G') | (uc == 'T');
-  code = ok ? (((c >> 1) ^ (c >> 2)) & 3u) : 0u;
-  return ok;
-}
 
 // Convert 32 characters (lane = position) — krakenutil.cpp:253-273.  Positions >= len read as ambiguous.
 __device__ __forceinline__ Block64 load_block(const char *seq, uint32_t len, uint32_t blk, uint32_t lane, bool marks) {
@@ -174,17 +161,6 @@ __device__ __forceinline__ Block64 load_block(const char *seq, uint32_t len, uin
 constexpr uint32_t BIN_NONE = 0xFFFFFFFFu;    // scratch marker: no window at this position
 constexpr uint32_t BIN_AMBIG = 0xFFFFFFFEu;   // scratch marker: window with a non-ACGT base
 
-// k-mer of the window that starts at base `lane` of the 128-bit string a:b (first base in bits 63:62 of a), k <= 31:
-// the window's bases [lane, lane + k) in its top bits
-__device__ __forceinline__ uint64_t window_top(uint64_t a, uint64_t b, uint32_t lane) {
-  return lane ? (a << (2 * lane)) | (b >> (64 - 2 * lane)) : a;
-}
-// canonical k-mer (krakendb.cpp:238-246)
-__device__ __forceinline__ uint64_t canonical_kmer(uint64_t top, uint32_t k) {
-  const uint64_t kmer = top >> (64 - 2 * k);
-  const uint64_t rc = revcomp64(kmer, k);
-  return kmer < rc ? kmer : rc;
-}
 
 // The windows of one slot of 32 (lane = window start in the 64 bases a:b): canonical k-mer (→ canon) and minimizer bin,
 // or BIN_AMBIG for a window with a non-ACGT base.  Warp-uniform: the minimizer takes shuffles.

@@ -110,6 +110,31 @@ __device__ __forceinline__ uint32_t encode_hash32(uint64_t hash) {
   return idx;
 }
 
+// KrakenDB::reverse_complement (krakendb.cpp:218-225): reverse the 2-bit groups, complement, shift down.
+__device__ __forceinline__ uint64_t revcomp64(uint64_t x, uint32_t n) {
+  x = __brevll(x);                                                              // reverses bits inside groups too
+  x = ((x >> 1) & 0x5555555555555555ull) | ((x & 0x5555555555555555ull) << 1);  // ... so swap them back
+  return (~x) >> (64 - 2 * n);
+}
+// One character → 2-bit code (A=0 C=1 G=2 T=3, case-insensitive, krakenutil.cpp:254-264); false = not ACGT.
+__device__ __forceinline__ bool base_code(uint32_t c, uint32_t &code) {
+  const uint32_t uc = c & 0xDFu;
+  const bool ok = (uc == 'A') | (uc == 'C') | (uc == 'G') | (uc == 'T');
+  code = ok ? (((c >> 1) ^ (c >> 2)) & 3u) : 0u;
+  return ok;
+}
+// k-mer of the window that starts at base `lane` of the 128-bit string a:b (first base in bits 63:62 of a), k <= 31:
+// the window's bases [lane, lane + k) in its top bits
+__device__ __forceinline__ uint64_t window_top(uint64_t a, uint64_t b, uint32_t lane) {
+  return lane ? (a << (2 * lane)) | (b >> (64 - 2 * lane)) : a;
+}
+// canonical k-mer (krakendb.cpp:238-246)
+__device__ __forceinline__ uint64_t canonical_kmer(uint64_t top, uint32_t k) {
+  const uint64_t kmer = top >> (64 - 2 * k);
+  const uint64_t rc = revcomp64(kmer, k);
+  return kmer < rc ? kmer : rc;
+}
+
 // set-key of a record: (taxon + 1) << 32 | encodeHashIn32Bit(hash(k-mer))
 __device__ __forceinline__ unsigned long long record_key(const uint32_t *w, uint32_t hiw, uint32_t hi_mask) {
   const uint64_t kmer = ((uint64_t)(hiw & hi_mask) << 32) | w[0];
