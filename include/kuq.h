@@ -286,6 +286,13 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
 /* The 4096 p=12 registers of one taxon (all zero if it received no k-mer). */
 int kuq_get_registers(kuq_ctx *ctx, uint32_t taxid, uint8_t *regs4096);
 int kuq_state_ptrs_get(kuq_ctx *ctx, kuq_state_ptrs *out);
+/* KUQ_HLL_PRELOAD: the work units a batch can hold before the (unit, taxon) pairs of further units spill from the
+ * dense per-batch table into the per-batch hash map (min(max_bases / work_unit_size + 8, 64 Mi / taxa with a sketch)).
+ * A batch of at most this many units only puts candidate pairs into the map, which cannot overflow it.
+ * Needs the database and the taxonomy. */
+int kuq_unit_table_rows(kuq_ctx *ctx, uint32_t *rows);
+/* KUQ_HLL_PRELOAD expects the unit ids of a batch in ascending order (as kuq_*_batch cut them when unit_id is NULL);
+ * ids out of order are accepted and give the same results, but each candidate pair then scans the whole batch. */
 /* Sparse tier across GPUs (replicas / shards with the exact HLL rule): export the (taxon, encoded hash) keys of the
  * taxa that are still sparse into d_keys_out (HBM; pass NULL / cap 0 to query *n), all-gather them, and import the
  * peers' keys; together with allreduce(MAX) on d_dense_flag / d_regs and SUM on the counters this is the merge

@@ -147,6 +147,7 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_clade_counts_tree": (C.c_int, [vp, u32p, C.c_uint32, u64p, u64p, u64p]),
         "kuq_get_registers": (C.c_int, [vp, C.c_uint32, u8p]),
         "kuq_state_ptrs_get": (C.c_int, [vp, C.POINTER(StatePtrs)]),
+        "kuq_unit_table_rows": (C.c_int, [vp, u32p]),
         "kuq_dense_taxids": (C.c_int, [vp, u32p, C.c_uint32, u32p]),
         "kuq_sparse_export": (C.c_int, [vp, vp, C.c_uint64, u64p]),
         "kuq_sparse_import": (C.c_int, [vp, vp, C.c_uint64]),
@@ -456,6 +457,12 @@ class Classifier:
         r = np.zeros(4096, np.uint8)
         self._ck(self.L.kuq_get_registers(self.h, int(taxid), _p(r, u8p)))
         return r
+
+    def unit_table_rows(self):
+        """units a preloaded batch holds before (unit, taxon) pairs spill into the per-batch hash map"""
+        n = np.zeros(1, np.uint32)
+        self._ck(self.L.kuq_unit_table_rows(self.h, _p(n, u32p)))
+        return int(n[0])
 
     def state_ptrs(self):
         s = StatePtrs()

@@ -53,6 +53,11 @@ static bool Populate_memory = false, Only_classified_kraken_output = false, Prin
 static uint64_t Populate_memory_size = 0;
 static string Classified_output_file, Unclassified_output_file, Kraken_output_file, Report_output_file, TaxDB_file;
 static size_t Work_unit_size = 500000;      // DEF_WORK_UNIT_SIZE, classify.cpp:38
+// Preloaded runs: a batch closes at a unit boundary once it holds this many work units, the rows of the library's dense
+// (unit, taxon) table (kuq_unit_table_rows).  The per-batch hash map then only holds candidate pairs (at most one per
+// 1025 bases), far below its 2 Mi pairs whatever the units hit.  Small -u with tens of thousands of taxa gives smaller
+// batches; everything else is cut by size first.
+static size_t Max_units_per_batch = SIZE_MAX;
 static int Num_threads = 1;
 static int HLL_PRECISION = 14;              // readcounts.hpp:29 (only selects report columns, classify.cpp:289)
 static unsigned long long total_classified = 0, total_sequences = 0, total_bases = 0;
@@ -827,22 +832,23 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename) {
     // KUQ_BATCH_READS: close a batch at the first unit boundary after this many reads (tests: small batches)
     const size_t batch_reads = getenv("KUQ_BATCH_READS") ? std::max<size_t>(1, strtoull(getenv("KUQ_BATCH_READS"), NULL, 10)) : (1u << 20) - 4096;
     uint64_t unit_nt = 0, batch_nt = 0;
-    size_t begin = 0, unit_first = 0;
+    size_t begin = 0, unit_first = 0, batch_units = 0;
     const uint64_t SLOT_NT = 280ull << 20;            // below the slot capacity (288 MiB)
     for (size_t i = 0; i < n_total; i++) {
       const uint64_t len = cum[i + 1] - cum[i];
       if (len > SLOT_NT) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
       if (batch_nt + len > SLOT_NT && i > begin) {    // a very long sequence is coming: close the batch before it
         batches.push_back({begin, i, batch_nt});
-        begin = i; batch_nt = 0;
+        begin = i; batch_nt = 0; batch_units = 0;
       }
       unit_nt += len; batch_nt += len;
       bool close_unit = unit_nt >= Work_unit_size;
-      if (close_unit) { unit_nt = 0; unit_first = i + 1; }
-      if ((close_unit && (batch_nt >= BATCH_NT || i + 1 - begin >= std::min<size_t>(batch_reads, (1u << 20) - 4096))) ||
+      if (close_unit) { unit_nt = 0; unit_first = i + 1; batch_units++; }
+      if ((close_unit && (batch_nt >= BATCH_NT || i + 1 - begin >= std::min<size_t>(batch_reads, (1u << 20) - 4096) ||
+                          batch_units >= Max_units_per_batch)) ||
           (!close_unit && (i + 1 - begin >= (1u << 20) - 1 || batch_nt >= (150ull << 20)))) {
         batches.push_back({begin, i + 1, batch_nt});
-        begin = i + 1; batch_nt = 0;
+        begin = i + 1; batch_nt = 0; batch_units = 0;
         if (!close_unit) unit_first = i + 1;
       }
     }
@@ -1020,6 +1026,7 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
   int cur = 0, inflight = -1;
   uint64_t unit_nt = 0;
   size_t unit_first_read = 0;       // first read of the open work unit inside the current batch
+  size_t batch_units = 0;           // units closed in the current batch
   auto wait_emit = [&](int which) {
     kuq_batch_result res;
     if (kuq_wait_batch(ctx, (uint32_t)which, &res)) die(EX_SOFTWARE, kuq_last_error(ctx));
@@ -1038,6 +1045,7 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
       die(EX_SOFTWARE, kuq_last_error(ctx));
     if (inflight >= 0) wait_emit(inflight);
     inflight = which;
+    batch_units = 0;
   };
   Read r;
   while (reader.valid) {
@@ -1059,7 +1067,7 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
       b2.reads.push_back(r);
       b2.offs.push_back(b2.bases.size());
       unit_nt += r.seq_len;
-      if (unit_nt >= Work_unit_size) { unit_nt = 0; unit_first_read = b2.reads.size(); }
+      if (unit_nt >= Work_unit_size) { unit_nt = 0; unit_first_read = b2.reads.size(); batch_units++; }
       continue;
     }
     b.reads.push_back(r);
@@ -1068,7 +1076,7 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
     if (unit_nt >= Work_unit_size) {                                 // the unit closes (classify.cpp:514-520)
       unit_nt = 0;
       unit_first_read = b.reads.size();
-      if (b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 4096) {
+      if (b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 4096 || ++batch_units >= Max_units_per_batch) {
         submit(cur);
         cur ^= 1;
         unit_first_read = 0;
@@ -1128,6 +1136,7 @@ static void load_file_batches(const char *filename, vector<Batch> &out, bool uni
   Read r;
   uint64_t unit_nt = 0;
   size_t unit_first_read = 0;        // first read of the open work unit inside the current batch
+  size_t batch_units = 0;
   while (reader.valid) {
     Batch &b = out.back();
     if (!reader.next(r, b.bases)) break;
@@ -1139,11 +1148,11 @@ static void load_file_batches(const char *filename, vector<Batch> &out, bool uni
     } else {
       unit_nt += r.seq_len;
       const bool close_unit = unit_nt >= Work_unit_size;
-      if (close_unit) { unit_nt = 0; unit_first_read = b.reads.size(); }
-      cut = close_unit ? (b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 4096)
+      if (close_unit) { unit_nt = 0; unit_first_read = b.reads.size(); batch_units++; }
+      cut = close_unit ? (b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 4096 || batch_units >= Max_units_per_batch)
                        : (b.reads.size() >= (1u << 20) - 1 || b.bases.size() >= (150ull << 20));   // one huge unit: counted as two
     }
-    if (cut) { out.emplace_back(); out.back().fastq = fq; unit_first_read = 0; }
+    if (cut) { out.emplace_back(); out.back().fastq = fq; unit_first_read = 0; batch_units = 0; }
   }
   if (unit_aligned && unit_nt == 0 && unit_first_read < out.back().reads.size()) {
     Batch &b = out.back();
@@ -1652,6 +1661,11 @@ int main(int argc, char **argv) {
     tax.parent_map(ids, parents);
     for (kuq_ctx *c : All_ctx)
       if (kuq_set_taxonomy(c, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(c));
+  }
+  if (cfg.hll_mode == KUQ_HLL_PRELOAD && n_db == 1) {
+    uint32_t rows = 0;
+    if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    if (rows) Max_units_per_batch = rows;
   }
   if (Print_classified) Classified_out.open(Classified_output_file);
   if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);

@@ -27,7 +27,6 @@ namespace {
 constexpr uint64_t INDEX2_XOR_MASK = 0xe37e28c4271b5a2dULL;   // krakendb.cpp:45
 constexpr uint32_t SLACK = 64;                                // bytes readable past the end of a bases buffer
 constexpr uint32_t UMAP_CAP = 1u << 21;                       // (unit, taxon) pairs per batch
-constexpr uint32_t USET_CAP = 1u << 22;                       // distinct (pair, code) entries per batch
 
 struct Slot {
   cudaStream_t stream = nullptr;
@@ -38,10 +37,9 @@ struct Slot {
   uint64_t *d_offsets = nullptr;
   uint32_t *d_unit = nullptr, *d_call = nullptr, *d_nwin = nullptr, *d_codes = nullptr;
   // HLL mode rule bookkeeping (KUQ_HLL_PRELOAD), allocated on first use
-  unsigned long long *u_keys = nullptr, *u_last = nullptr, *u_set_keys = nullptr;
-  uint32_t *u_inserts = nullptr, *u_distinct = nullptr, *u_set_count = nullptr, *u_ncand = nullptr, *u_direct = nullptr;
+  unsigned long long *u_keys = nullptr;
+  uint32_t *u_inserts = nullptr, *u_cand = nullptr, *u_ncand = nullptr, *u_direct = nullptr, *u_codes = nullptr;
   uint32_t u_direct_rows = 0;
-  uint8_t *u_cand = nullptr, *u_taxon_cand = nullptr;
   uint64_t *d_canon = nullptr;                 // scratch between the stages
   uint32_t *d_bins = nullptr, *d_dense = nullptr, *d_codes_in = nullptr;
   PackedBlock *d_pack = nullptr;               // the fused path's 2-bit copy of the batch (k_pack)
@@ -212,8 +210,8 @@ void free_slot(Slot &s) {
   cudaFree(s.d_nwin); cudaFree(s.d_codes); cudaFree(s.d_run_start); cudaFree(s.d_run_count); cudaFree(s.d_runs);
   cudaFree(s.d_scalars); cudaFree(s.d_canon); cudaFree(s.d_bins); cudaFree(s.d_dense); cudaFree(s.d_codes_in); cudaFree(s.d_ovf);
   cudaFree(s.d_pack); cudaFree(s.d_side);
-  cudaFree(s.u_keys); cudaFree(s.u_last); cudaFree(s.u_set_keys); cudaFree(s.u_inserts); cudaFree(s.u_distinct);
-  cudaFree(s.u_set_count); cudaFree(s.u_ncand); cudaFree(s.u_cand); cudaFree(s.u_taxon_cand); cudaFree(s.u_direct);
+  cudaFree(s.u_keys); cudaFree(s.u_inserts); cudaFree(s.u_ncand); cudaFree(s.u_cand); cudaFree(s.u_direct);
+  cudaFree(s.u_codes);
   cudaFreeHost(s.h_call); cudaFreeHost(s.h_nwin); cudaFreeHost(s.h_run_start); cudaFreeHost(s.h_run_count);
   cudaFreeHost(s.h_codes); cudaFreeHost(s.h_runs); cudaFreeHost(s.h_scalars); cudaFreeHost(s.h_unit);
   if (s.ev_k0) cudaEventDestroy(s.ev_k0);
@@ -711,22 +709,22 @@ int ensure_ready(kuq_ctx *ctx) {
   return remap_db(ctx);
 }
 
+// dense (unit, taxon) table: the units a batch can hold when the library cuts them, at most 64 Mi counters
+uint64_t unit_table_rows(const kuq_ctx *ctx) {
+  const uint64_t rows = ctx->cfg.max_bases_per_batch / std::max<uint64_t>(ctx->cfg.work_unit_size, 1) + 8;
+  return std::min<uint64_t>(rows, (64ull << 20) / std::max<uint32_t>(ctx->n_sketch, 1));
+}
+
 void set_unit_ptrs(Params &p, Slot &s);
 int prepare_unit_map(kuq_ctx *ctx, Slot &s) {
   if (ctx->cfg.hll_mode != KUQ_HLL_PRELOAD) return KUQ_OK;
   if (!s.u_keys) {
     CU(dmalloc(&s.u_keys, UMAP_CAP));
-    CU(dmalloc(&s.u_last, UMAP_CAP));
     CU(dmalloc(&s.u_inserts, UMAP_CAP));
-    CU(dmalloc(&s.u_distinct, UMAP_CAP));
-    CU(dmalloc(&s.u_cand, UMAP_CAP));
-    CU(dmalloc(&s.u_taxon_cand, ctx->n_sketch));
-    CU(dmalloc(&s.u_ncand, 1));
-    CU(dmalloc(&s.u_set_keys, USET_CAP));
-    CU(dmalloc(&s.u_set_count, USET_CAP));
-    // dense (unit, taxon) table: the units a batch can hold when the library cuts them, at most 64 Mi counters
-    uint64_t rows = ctx->cfg.max_bases_per_batch / std::max<uint64_t>(ctx->cfg.work_unit_size, 1) + 8;
-    rows = std::min<uint64_t>(rows, (64ull << 20) / std::max<uint32_t>(ctx->n_sketch, 1));
+    CU(dmalloc(&s.u_cand, UMAP_CAP));         // every candidate is a distinct map slot
+    CU(dmalloc(&s.u_ncand, 2));
+    CU(dmalloc(&s.u_codes, (size_t)ctx->n_sm * UNIT_DECIDE_CTAS_PER_SM * 2 * UNIT_CODES));
+    const uint64_t rows = unit_table_rows(ctx);
     s.u_direct_rows = (uint32_t)rows;
     if (rows) CU(dmalloc(&s.u_direct, rows * ctx->n_sketch));
   }
@@ -750,15 +748,10 @@ void cut_units(kuq_ctx *ctx, const uint64_t *offsets, uint32_t n, uint32_t *unit
 void set_unit_ptrs(Params &p, Slot &s) {
   p.units.keys = s.u_keys;
   p.units.inserts = s.u_inserts;
-  p.units.distinct = s.u_distinct;
-  p.units.last = s.u_last;
   p.units.cand = s.u_cand;
   p.units.mask = UMAP_CAP - 1;
-  p.units.taxon_cand = s.u_taxon_cand;
   p.units.n_cand = s.u_ncand;
-  p.units.set_keys = s.u_set_keys;
-  p.units.set_count = s.u_set_count;
-  p.units.set_mask = USET_CAP - 1;
+  p.units.codes = s.u_codes;
   p.units.direct = s.u_direct;
   p.units.direct_rows = s.u_direct_rows;
 }
@@ -1753,7 +1746,10 @@ int kuq_read_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *n_reads, uint64_t *
     // the sketch the reference would hold: dense registers if some per-unit (or the global) sketch converted,
     // else the union of the encoded hashes (sparse tier)
     const bool exact = ctx->cfg.hll_mode == KUQ_HLL_EXACT;
-    const bool sparse = d < ctx->n_sketch && !exact && ctx->cfg.hll_mode != KUQ_HLL_DENSE_ONLY && !h.dense_flag[d];
+    // A taxon outside the database (no sketch here) that is the call of some read, e.g. the LCA of tied hits, has a
+    // READCOUNTS entry in the reference all the same: an empty sketch, which is sparse.
+    const bool sparse = !exact && ctx->cfg.hll_mode != KUQ_HLL_DENSE_ONLY &&
+                        (d < ctx->n_sketch ? !h.dense_flag[d] : h.n_reads[d] > 0);
     uint64_t u = 0;
     if (exact) u = d < ctx->n_sketch ? h.exact[d] : 0;     // khset size, readcounts.hpp:127-130
     else if (d < ctx->n_sketch && nk)
@@ -2114,6 +2110,14 @@ int kuq_state_ptrs_get(kuq_ctx *ctx, kuq_state_ptrs *out) {
   out->d_dense_flag = ctx->d_dense_flag;
   out->n_sketch = ctx->n_sketch;
   out->n_taxa = ctx->n_taxa;
+  return KUQ_OK;
+}
+
+int kuq_unit_table_rows(kuq_ctx *ctx, uint32_t *rows) {
+  if (!ctx || !rows) return KUQ_E_INVALID_ARG;
+  int rc = finalize(ctx);
+  if (rc) return rc;
+  *rows = (uint32_t)unit_table_rows(ctx);
   return KUQ_OK;
 }
 

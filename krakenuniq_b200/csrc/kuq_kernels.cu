@@ -677,10 +677,14 @@ __global__ void __launch_bounds__(256, (MODE == MODE_FUSED && !FAST) ? 6 : 8) k_
 }
 
 // ---- per-batch (unit, taxon) map ----------------------------------------------------------------------------
+// Linear probing gives up after UMAP_PROBES slots (error 2, KUQ_E_CAPACITY).  classify's batches hold at most the
+// dense table's rows of units, so the map holds only candidates (< 300 k pairs, under 15 % load) and a run that long
+// does not occur; a map that a C ABI caller overfills fails in microseconds, not in a scan of all 2 Mi slots per insert.
+constexpr uint32_t UMAP_PROBES = 4096;
 __device__ __forceinline__ uint32_t umap_slot(const UnitMap &u, uint32_t unit, uint32_t taxon, bool insert) {
   const unsigned long long key = ((unsigned long long)(unit + 1) << 32) | taxon;
   uint32_t slot = (uint32_t)mix64(key) & u.mask;
-  for (uint32_t probe = 0; probe <= u.mask; probe++) {
+  for (uint32_t probe = 0; probe < UMAP_PROBES; probe++) {
     unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(u.keys + slot);
     if (cur == key) return slot;
     if (cur == 0) {
@@ -1082,104 +1086,121 @@ __global__ void k_unit_mark(const __grid_constant__ Params p) {
       const uint32_t sl = umap_slot(u, row0 + row, taxon, true);
       if (sl == 0xFFFFFFFFu) { atomicExch(p.error_flag, 2u); continue; }
       u.inserts[sl] = cnt;
-      u.cand[sl] = 1;
-      u.taxon_cand[taxon] = 1;
-      atomicAdd(u.n_cand, 1u);
+      u.cand[atomicAdd(u.n_cand, 1u)] = sl;
     }
   }
+  // the map's own pairs: units past the table (the pairs moved above are in rows < direct_rows and listed already)
   for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s <= u.mask; s += gridDim.x * blockDim.x) {
     const unsigned long long key = u.keys[s];
     if (!key) continue;
     const uint32_t taxon = (uint32_t)key;
-    if (u.inserts[s] >= 1025u && !p.dense_flag[taxon] && !u.cand[s]) {
-      u.cand[s] = 1;
-      u.taxon_cand[taxon] = 1;
-      atomicAdd(u.n_cand, 1u);
-    }
+    if ((uint32_t)(key >> 32) - 1u - p.unit_id[0] < u.direct_rows) continue;
+    if (u.inserts[s] >= 1025u && !p.dense_flag[taxon]) u.cand[atomicAdd(u.n_cand, 1u)] = s;
   }
+  // k_unit_decide finds a unit's reads by binary search, which needs ascending unit ids (classify's always are)
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r + 1 < p.n_reads; r += gridDim.x * blockDim.x)
+    if (p.unit_id[r] > p.unit_id[r + 1]) { u.n_cand[1] = 1; break; }
 }
 
-// warp per read; only windows of candidate (unit, taxon) pairs do any work
-__global__ void __launch_bounds__(256) k_unit_distinct(const __grid_constant__ Params p) {
-  const UnitMap &u = p.units;
-  if (*reinterpret_cast<volatile uint32_t *>(u.n_cand) == 0) return;
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t warps_total = gridDim.x * (blockDim.x >> 5);
-  for (uint32_t r = blockIdx.x * (blockDim.x >> 5) + warp; r < p.n_reads; r += warps_total) {
-    const uint64_t base = p.offsets[r];
-    const uint32_t nwin = p.n_windows[r];
-    const uint32_t unit = p.unit_id[r];
-    for (uint32_t i = lane; i < nwin; i += 32) {
-      const uint32_t t = p.codes_dense[base + i];
-      if (t == AMBIG || !u.taxon_cand[t]) continue;
-      const uint32_t sl = umap_slot(u, unit, t, false);
-      if (sl == 0xFFFFFFFFu || !u.cand[sl]) continue;
-      atomicMax(u.last + sl, ((unsigned long long)r << 32) | i);
-      if (*reinterpret_cast<volatile uint32_t *>(u.distinct + sl) >= 1025u) continue;   // decided already
-      const uint32_t code = encode_hash32(fmix64(window_canon(p, base + i)));
-      const unsigned long long key = ((unsigned long long)(sl + 1) << 32) | code;
-      uint32_t q = (uint32_t)mix64(key) & u.set_mask;
-      for (uint32_t probe = 0; probe <= u.set_mask; probe++) {
-        unsigned long long cur = *reinterpret_cast<volatile unsigned long long *>(u.set_keys + q);
-        if (cur == 0) {
-          cur = atomicCAS(u.set_keys + q, 0ull, key);
-          if (cur == 0) { atomicAdd(u.distinct + sl, 1u); cur = key; }
-        }
-        if (cur == key) { atomicAdd(u.set_count + q, 1u); break; }
-        q = (q + 1) & u.set_mask;
-        if (probe == u.set_mask) atomicExch(p.error_flag, 3u);
-      }
-    }
+// first index in [0, n) whose value is >= v, n if none; a[] ascending.  All lanes of the warp return it.
+__device__ uint32_t warp_lower_bound(const uint32_t *a, uint32_t n, uint32_t v, uint32_t lane) {
+  uint32_t lo = 0, hi = n;                              // the answer lies in [lo, hi]
+  while (hi - lo > 32) {
+    const uint32_t step = (hi - lo) / 32;
+    const uint32_t below = __popc(__ballot_sync(0xFFFFFFFFu, a[lo + lane * step] < v));
+    if (below == 0) return lo;
+    if (below < 32) hi = lo + below * step;
+    lo += (below - 1) * step + 1;
   }
+  const uint32_t i = lo + lane;
+  return lo + __popc(__ballot_sync(0xFFFFFFFFu, i < hi && a[i] < v));
 }
 
+// One block per candidate (unit, taxon) pair at a time: the distinct codes of the pair's inserts go to the block's own
+// table of UNIT_CODES slots (u.codes, in L2).  Counting stops at 1025 codes; with 256 threads inserting at once the
+// table then holds at most 1024 + 256 codes, so it never fills and no batch, however many candidates it has, runs out
+// of room.  (The table is not in shared memory: this launch runs next to other slots' lookups in every preloaded batch,
+// candidates or not, and should not take shared memory from them.)
 // A (unit, taxon) sketch receiving inserts x_1..x_N converts iff D >= 1025, or D == 1024 and the 1024th distinct
 // code arrives before the last insert (SURVEY.md §7.3): i.e. the last insert repeats a code seen earlier.
-__global__ void k_unit_apply(const __grid_constant__ Params p) {
+__global__ void __launch_bounds__(256) k_unit_decide(const __grid_constant__ Params p) {
   const UnitMap &u = p.units;
-  if (*reinterpret_cast<volatile uint32_t *>(u.n_cand) == 0) return;
-  for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s <= u.mask; s += gridDim.x * blockDim.x) {
-    if (!u.cand[s]) continue;
-    const uint32_t taxon = (uint32_t)u.keys[s];
-    const uint32_t d = u.distinct[s];
-    bool conv = d >= 1025u;
-    if (!conv && d == 1024u) {
-      const unsigned long long lp = u.last[s];
-      const uint32_t r = (uint32_t)(lp >> 32), i = (uint32_t)lp;
-      const uint32_t code = encode_hash32(fmix64(window_canon(p, p.offsets[r] + i)));
-      const unsigned long long key = ((unsigned long long)(s + 1) << 32) | code;
-      uint32_t q = (uint32_t)mix64(key) & u.set_mask;
-      for (uint32_t probe = 0; probe <= u.set_mask; probe++) {
-        unsigned long long cur = u.set_keys[q];
-        if (cur == key) { conv = u.set_count[q] >= 2u; break; }
-        if (cur == 0) break;
-        q = (q + 1) & u.set_mask;
+  const uint32_t n_cand = *reinterpret_cast<volatile uint32_t *>(u.n_cand);
+  if (blockIdx.x >= n_cand) return;
+  uint32_t *s_code = u.codes + (size_t)blockIdx.x * 2 * UNIT_CODES, *s_count = s_code + UNIT_CODES;
+  __shared__ uint32_t s_distinct, s_lo, s_hi;
+  __shared__ unsigned long long s_last;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  const bool ascending = u.n_cand[1] == 0;
+  volatile uint32_t *v_distinct = &s_distinct;
+  const volatile uint8_t *v_dense = p.dense_flag;
+  for (uint32_t c = blockIdx.x; c < n_cand; c += gridDim.x) {
+    const uint32_t sl = u.cand[c];
+    const unsigned long long key = u.keys[sl];
+    const uint32_t unit = (uint32_t)(key >> 32) - 1u, taxon = (uint32_t)key;
+    for (uint32_t j = threadIdx.x; j < UNIT_CODES; j += blockDim.x) { s_code[j] = 0; s_count[j] = 0; }
+    if (warp == 0) {
+      uint32_t lo = 0, hi = p.n_reads;
+      if (ascending) {
+        lo = warp_lower_bound(p.unit_id, p.n_reads, unit, lane);
+        hi = unit == 0xFFFFFFFFu ? p.n_reads : warp_lower_bound(p.unit_id, p.n_reads, unit + 1, lane);
+      }
+      if (lane == 0) { s_lo = lo; s_hi = hi; s_distinct = 0; s_last = 0; }
+    }
+    __syncthreads();
+    const uint32_t lo = s_lo, hi = s_hi;
+    for (uint32_t r = lo + warp; r < hi; r += n_warps) {
+      if (*v_distinct >= 1025u || v_dense[taxon]) break;            // decided (here, or by another pair of the taxon)
+      if (!ascending && p.unit_id[r] != unit) continue;
+      const uint64_t base = p.offsets[r];
+      const uint32_t nwin = p.n_windows[r];
+      for (uint32_t i = lane; i < nwin; i += 32) {
+        if (p.codes_dense[base + i] != taxon) continue;
+        atomicMax(&s_last, ((unsigned long long)r << 32) | i);
+        if (*v_distinct >= 1025u) continue;
+        const uint32_t code = encode_hash32(fmix64(window_canon(p, base + i)));     // never 0
+        uint32_t q = (code * 0x9E3779B1u) >> 21;
+        for (uint32_t probe = 0; probe < UNIT_CODES; probe++) {
+          uint32_t cur = reinterpret_cast<volatile uint32_t *>(s_code)[q];   // (L1 bypassed: other threads CAS here)
+          if (cur == 0) {
+            cur = atomicCAS(s_code + q, 0u, code);
+            if (cur == 0) { atomicAdd(&s_distinct, 1u); cur = code; }
+          }
+          if (cur == code) { atomicAdd(s_count + q, 1u); break; }
+          q = (q + 1) & (UNIT_CODES - 1);
+        }
       }
     }
-    if (conv) p.dense_flag[taxon] = 1;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const uint32_t d = s_distinct;
+      bool conv = d >= 1025u;
+      if (!conv && d == 1024u) {
+        const uint32_t r = (uint32_t)(s_last >> 32), i = (uint32_t)s_last;
+        const uint32_t code = encode_hash32(fmix64(window_canon(p, p.offsets[r] + i)));
+        uint32_t q = (code * 0x9E3779B1u) >> 21;
+        const volatile uint32_t *v_code = s_code, *v_count = s_count;
+        for (uint32_t probe = 0; probe < UNIT_CODES && v_code[q]; probe++) {
+          if (v_code[q] == code) { conv = v_count[q] >= 2u; break; }
+          q = (q + 1) & (UNIT_CODES - 1);
+        }
+      }
+      if (conv) p.dense_flag[taxon] = 1;
+    }
+    __syncthreads();
   }
 }
 
-// one launch instead of nine memsets: empty the per-batch (unit, taxon) map and its distinct-code set
+// one launch instead of several memsets: empty the per-batch (unit, taxon) map and its dense table
 __global__ void __launch_bounds__(256) k_unit_clear(UnitMap u, uint32_t n_sketch) {
   const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (uint64_t)gridDim.x * blockDim.x;
   const uint4 z = make_uint4(0, 0, 0, 0);
-  const uint64_t cap = (uint64_t)u.mask + 1, scap = (uint64_t)u.set_mask + 1;     // powers of two >= 1024
-  for (uint64_t i = tid; i < cap / 2; i += nth) {
-    reinterpret_cast<uint4 *>(u.keys)[i] = z;
-    reinterpret_cast<uint4 *>(u.last)[i] = z;
-  }
-  for (uint64_t i = tid; i < cap / 4; i += nth) {
-    reinterpret_cast<uint4 *>(u.inserts)[i] = z;
-    reinterpret_cast<uint4 *>(u.distinct)[i] = z;
-  }
-  for (uint64_t i = tid; i < cap / 16; i += nth) reinterpret_cast<uint4 *>(u.cand)[i] = z;
-  for (uint64_t i = tid; i < scap / 2; i += nth) reinterpret_cast<uint4 *>(u.set_keys)[i] = z;
-  for (uint64_t i = tid; i < scap / 4; i += nth) reinterpret_cast<uint4 *>(u.set_count)[i] = z;
-  for (uint64_t i = tid; i < n_sketch; i += nth) u.taxon_cand[i] = 0;
+  const uint64_t cap = (uint64_t)u.mask + 1;     // a power of two >= 1024
+  for (uint64_t i = tid; i < cap / 2; i += nth) reinterpret_cast<uint4 *>(u.keys)[i] = z;
+  for (uint64_t i = tid; i < cap / 4; i += nth) reinterpret_cast<uint4 *>(u.inserts)[i] = z;
   const uint64_t nd = (uint64_t)u.direct_rows * n_sketch;
   for (uint64_t i = tid; i < nd; i += nth) u.direct[i] = 0;
-  if (tid == 0) *u.n_cand = 0;
+  if (tid == 0) { u.n_cand[0] = 0; u.n_cand[1] = 0; }
 }
 // SM count of the current device, for the grid-stride helpers below that have no context at hand
 int device_sm_count() {
@@ -1195,10 +1216,8 @@ void launch_unit_clear(const UnitMap &u, uint32_t n_sketch, int n_sm, cudaStream
 int launch_unit_accounting(const Params &p, int n_sm, cudaStream_t stream) {
   if (p.n_reads == 0) return 0;
   k_unit_mark<<<n_sm * 4, 256, 0, stream>>>(p);
-  const int rgrid = (int)min((uint32_t)n_sm * 8, (p.n_reads + 7) / 8);
-  k_unit_distinct<<<rgrid, 256, 0, stream>>>(p);
-  k_unit_apply<<<n_sm * 4, 256, 0, stream>>>(p);
-  return 3;
+  k_unit_decide<<<n_sm * UNIT_DECIDE_CTAS_PER_SM, 256, 0, stream>>>(p);     // blocks past the candidate count return at once
+  return 2;
 }
 
 __global__ void k_flag_dense_global(const uint32_t *distinct, uint8_t *dense_flag, uint32_t n_sketch) {

@@ -153,18 +153,15 @@ __device__ __forceinline__ unsigned long long source_key(const KeySource &s, uin
 // Per-batch bookkeeping of the reference's per-work-unit sketches (classify.cpp:525: one ReadCounts map per work
 // unit).  A (unit, taxon) sketch converts from sparse to dense iff an insert finds >= 1024 distinct encoded hashes
 // already stored (hyperloglogplus.cpp:496-498), so only pairs with > 1024 inserts need their distinct count.
+constexpr uint32_t UNIT_CODES = 2048;               // distinct-code table of one candidate pair (k_unit_decide)
+constexpr uint32_t UNIT_DECIDE_CTAS_PER_SM = 4;
 struct UnitMap {
   unsigned long long *keys;   // 0 = empty; (unit + 1) << 32 | taxon   (open addressing, per batch)
   uint32_t *inserts;          // N(unit, taxon): add_kmer calls
-  uint32_t *distinct;         // D(unit, taxon): distinct encoded hashes (only counted for candidates, saturating)
-  unsigned long long *last;   // (read << 32 | window) of the last insert of the pair
-  uint8_t *cand;              // 1 = candidate (N >= 1025 and the taxon is not already known dense)
   uint32_t mask;              // capacity - 1
-  uint8_t *taxon_cand;        // [n_sketch] some unit of this batch makes the taxon a candidate
-  uint32_t *n_cand;           // number of candidate pairs of the batch
-  unsigned long long *set_keys;  // distinct (pair slot, code): 0 = empty; (slot + 1) << 32 | code
-  uint32_t *set_count;           // occurrences of the key
-  uint32_t set_mask;
+  uint32_t *cand;             // map slots of the candidate pairs (N >= 1025, taxon not already known dense)
+  uint32_t *n_cand;           // [0] number of candidate pairs of the batch, [1] != 0: unit ids not ascending
+  uint32_t *codes;            // k_unit_decide: per CTA, UNIT_CODES distinct codes + UNIT_CODES occurrence counts
   // fast path for the insert counts: units of a batch are (nearly always) consecutive ids, so N(unit, taxon) lives in a
   // dense table direct[(unit - unit_id[0]) * n_sketch + taxon] — one fire-and-forget atomic per (read, taxon), no probe.
   // Pairs outside the table (rows >= direct_rows) use the hash map above; k_unit_mark moves the candidates there.
