@@ -5,7 +5,7 @@
 // hardware.  The oracle's CPU statements of both tools are pinned against the reference executables
 // (tests/test_oracle_db_build.py).
 //
-// set_lcas options NOT supported (exit with a message): -I (UIDs), -a / -A (new taxonomy ids).
+// set_lcas options NOT supported (exit with a message): -I (UIDs).
 #include <fcntl.h>
 #include <getopt.h>
 #include <sys/mman.h>
@@ -13,6 +13,7 @@
 #include <sysexits.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <cctype>
 #include <cstdio>
 #include <cstdlib>
@@ -120,7 +121,9 @@ int main(int argc, char **argv) {
 // ====================================================================================================================
 static const char *TOOL = "set_lcas";
 static const size_t SKIP_LEN = 50000;                    // set_lcas.cpp:31
+static const uint32_t TID_HUMAN = 9606, TID_MOUSE = 10090;  // host taxa get no sequence taxa, :83-84
 static bool Allow_extra_kmers = false, verbose = false, Operate_in_RAM = false, Pretend = false;
+static bool Add_taxids_for_sequences = false, Add_taxids_for_assembly = false;   // -a / -A (set_lcas.cpp:528-533)
 static uint32_t Minimum_sequence_size = 0;
 static uint32_t Lca_flags = 0;                           // -T → KUQ_LCA_FORCE_CONTAMINANT, -R → KUQ_LCA_RESET
 static string DB_filename, Index_filename, TaxDB_filename, File_to_taxon_map_filename, ID_to_taxon_map_filename,
@@ -139,7 +142,9 @@ static void usage(int exit_code = EX_USAGE) {
        << "  -f filename      File to taxon map" << endl
        << "  -F filename      Multi-FASTA file with sequence data" << endl
        << "  -m filename      Sequence ID to taxon map" << endl
-       << "  -T               When a k-mer appears in a 'synthetic construct' sequence, force the taxID to be the 'synthetic construct' taxID, instead of the LCA." << endl
+       << "  -a               Add taxonomy IDs (starting with 1000000001) for sequences to Taxonomy DB" << endl
+       << "  -A               Add taxonomy IDs (starting with 1000000001) for assemblies (third column in seqid2taxid.map) to Taxonomy DB" << endl
+       << "  -T             When a k-mer appears in a 'synthetic construct' sequence, force the taxID to be the 'synthetic construct' taxID, instead of the LCA." << endl
        << "  -R               Reset the taxIDs of the k-mers of the sequences to 0" << endl
        << "  -E #             Exclude sequences that are shorter than the threshold." << endl
        << "  -c filename      Write k-mer counts per taxon to filename" << endl
@@ -147,7 +152,7 @@ static void usage(int exit_code = EX_USAGE) {
        << "  -v               Verbose output" << endl
        << "  -h               Print this message" << endl << endl
        << "-F and -m must be specified together.  If -f is given, -F/-m are ignored." << endl
-       << "(GPU build: -I, -a and -A are not supported)" << endl;
+       << "(GPU build: -I is not supported)" << endl;
   exit(exit_code);
 }
 
@@ -221,6 +226,108 @@ static void add_sequence(Batch &b, const string &seq, uint32_t taxid) {
   }
 }
 
+// ---- the taxonomy as TaxonomyDB holds it (readTaxonomyIndex_, taxdb.hpp:563-605), and the taxa -a / -A add to it ----
+struct Taxon {
+  uint32_t parent;                 // the row's parent pointer; `linked` false = NULL (the root, an unknown parent, row 0)
+  bool linked;
+  string name, rank;
+};
+// One insert per taxDB line in file order (the first line of a taxid wins), then taxid 0 'unclassified'.  The
+// insert sequence is the reference's, so iterating this map visits taxids in the reference's order, which decides
+// where new taxids start (set_lcas.cpp:219-224).
+static unordered_map<uint32_t, Taxon> Taxa;
+static uint32_t New_taxid_start = 1000000000;            // set_lcas.cpp:51
+static unordered_map<string, uint32_t> Name_to_taxid;   // assembly names and sequence ids share one cache
+
+static void read_taxdb(const string &path) {
+  ifstream in(path.c_str());
+  if (!in.is_open()) die(EX_NOINPUT, "unable to open taxonomy index file " + path, TOOL);
+  string line;
+  while (getline(in, line)) {                            // id \t parent \t name \t rank
+    size_t a = line.find('\t'), b = a == string::npos ? a : line.find('\t', a + 1);
+    if (a == string::npos || b == string::npos) continue;
+    const size_t c = line.find('\t', b + 1);
+    Taxon t{(uint32_t)strtoul(line.substr(a + 1, b - a - 1).c_str(), NULL, 10), false,
+            line.substr(b + 1, c == string::npos ? string::npos : c - b - 1), c == string::npos ? "" : line.substr(c + 1)};
+    Taxa.emplace((uint32_t)strtoul(line.substr(0, a).c_str(), NULL, 10), t);
+  }
+  Taxa.emplace(0u, Taxon{0, false, "unclassified", "no rank"});
+  for (auto &kv : Taxa)                                  // createPointers, taxdb.hpp:412-433
+    kv.second.linked = kv.second.parent != kv.first && Taxa.count(kv.second.parent);
+}
+
+// Parent_map (getParentMap, taxdb.hpp:383-398): the parent pointer's taxid, 0 for none
+static uint32_t parent_map(uint32_t taxid) {
+  const Taxon &t = Taxa.at(taxid);
+  return t.linked ? t.parent : 0;
+}
+
+// get_new_taxid (set_lcas.cpp:183-203): the id is used up even when the parent is unknown and nothing is added
+static uint32_t new_taxid(const string &name, uint32_t parent, const char *rank) {
+  auto it = Name_to_taxid.find(name);
+  if (it != Name_to_taxid.end()) return it->second;
+  const uint32_t id = ++New_taxid_start;
+  if (parent == id) return 0;
+  if (!Taxa.count(parent)) {
+    cerr << "ERROR with taxon [" << id << ";" << rank << ";" << name << "] - parent taxon " << parent << " not in database!" << endl;
+    return 0;
+  }
+  if (!Taxa.emplace(id, Taxon{parent, true, name, rank}).second) return 0;
+  Name_to_taxid[name] = id;
+  return id;
+}
+
+// writeTaxonomyIndex (taxdb.hpp:533-547): ascending taxids, a row without a parent pointer names itself
+static void write_taxdb(const string &path) {
+  vector<uint32_t> keys;
+  for (auto &kv : Taxa) keys.push_back(kv.first);
+  sort(keys.begin(), keys.end());
+  string out;
+  for (uint32_t id : keys) {
+    const Taxon &t = Taxa.at(id);
+    out += to_string(id) + '\t' + to_string(t.linked ? t.parent : id) + '\t' + t.name + '\t' + t.rank + '\n';
+  }
+  write_file(path, out.data(), out.size(), TOOL);
+}
+
+// read_seqid_to_taxid_map (set_lcas.cpp:205-266): the first mapping of a sequence id wins.  With -A / -a the
+// assembly (third column) and sequence taxa are created here, before any sequence is read, and each mapping is
+// printed on stdout.
+static unordered_map<string, uint32_t> read_seqid_map(const string &path) {
+  cerr << "Reading sequence ID to taxonomy ID mapping ... ";
+  unordered_map<string, uint32_t> id_to_taxon;
+  ifstream map_file(path.c_str());
+  if (map_file.rdstate() & ifstream::failbit) die(EX_NOINPUT, "can't open " + path, TOOL);
+  const bool add = Add_taxids_for_assembly || Add_taxids_for_sequences;
+  if (add) {
+    for (auto &kv : Taxa)
+      if (kv.first >= New_taxid_start) New_taxid_start = kv.first + 100;
+    cerr << "[starting new taxonomy IDs with " << (New_taxid_start + 1) << ']';
+  }
+  string line, seq_id, name;
+  uint32_t taxid = 0;
+  while (map_file.good()) {
+    getline(map_file, line);
+    if (line.empty()) break;
+    istringstream iss(line);
+    iss >> seq_id >> taxid;
+    if (id_to_taxon.count(seq_id)) continue;
+    const uint32_t orig_taxid = taxid;
+    if (Add_taxids_for_assembly && iss.good()) {         // one separator, then the rest of the line
+      iss.get();
+      getline(iss, name);
+      if (!name.empty()) taxid = new_taxid(name, taxid, "assembly");
+    }
+    if (Add_taxids_for_sequences && orig_taxid != TID_HUMAN && orig_taxid != TID_MOUSE)
+      taxid = new_taxid(seq_id, taxid, "sequence");
+    if (add) cout << seq_id << '\t' << taxid << '\n';
+    id_to_taxon[seq_id] = taxid;
+  }
+  if (id_to_taxon.empty()) cerr << "Error: No ID mappings present!!" << endl;
+  cerr << " got " << id_to_taxon.size() << " mappings." << endl;
+  return id_to_taxon;
+}
+
 int main(int argc, char **argv) {
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
   int opt;
@@ -245,7 +352,9 @@ int main(int argc, char **argv) {
       case 'n': case 'S': break;
       case 'T': Lca_flags |= KUQ_LCA_FORCE_CONTAMINANT; break;
       case 'R': Lca_flags |= KUQ_LCA_RESET; break;
-      case 'I': case 'a': case 'A':
+      case 'a': Add_taxids_for_sequences = true; break;
+      case 'A': Add_taxids_for_assembly = true; break;
+      case 'I':
         die(EX_USAGE, string("option -") + (char)opt + " is not supported by the GPU set_lcas", TOOL);
       default: usage();
     }
@@ -254,30 +363,7 @@ int main(int argc, char **argv) {
   if (File_to_taxon_map_filename.empty() && (Multi_fasta_filename.empty() || ID_to_taxon_map_filename.empty())) usage();
   const bool one_fasta_file = File_to_taxon_map_filename.empty();
 
-  // taxonomy → Parent_map (getParentMap, taxdb.hpp:383-398): taxid, parent taxid from the first two columns; a row
-  // whose parent has no row of its own, or is the row itself, has parent 0
-  vector<uint32_t> ids, parents;
-  unordered_map<uint32_t, uint32_t> parent_of;
-  {
-    ifstream in(TaxDB_filename.c_str());
-    if (!in.is_open()) die(EX_NOINPUT, "unable to open taxonomy index file " + TaxDB_filename, TOOL);
-    string line;
-    vector<pair<uint32_t, uint32_t>> rows;
-    while (getline(in, line)) {
-      size_t a = line.find('\t'), b = a == string::npos ? a : line.find('\t', a + 1);
-      if (a == string::npos || b == string::npos) continue;
-      uint32_t id = (uint32_t)strtoul(line.substr(0, a).c_str(), NULL, 10);
-      uint32_t par = (uint32_t)strtoul(line.substr(a + 1, b - a - 1).c_str(), NULL, 10);
-      if (parent_of.count(id)) continue;
-      parent_of[id] = par;
-      rows.emplace_back(id, par);
-    }
-    for (auto &r : rows) {
-      if (r.first == 0) continue;
-      ids.push_back(r.first);
-      parents.push_back((r.second == r.first || !parent_of.count(r.second)) ? 0 : r.second);
-    }
-  }
+  read_taxdb(TaxDB_filename);
 
   Mapped kdb, idx;
   kdb.open(DB_filename, TOOL);
@@ -295,27 +381,20 @@ int main(int argc, char **argv) {
   int rc = kuq_create(&cfg, &Ctx);
   if (rc) die(EX_UNAVAILABLE, string("libkuq: ") + kuq_strerror(rc), TOOL);
   if (kuq_stage_db(Ctx, kdb.p, kdb.size, idx.p, idx.size, 0, 0)) die(EX_DATAERR, kuq_last_error(Ctx), TOOL);
-  if (kuq_set_taxonomy(Ctx, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+  unordered_map<string, uint32_t> id_to_taxon;
+  if (one_fasta_file) id_to_taxon = read_seqid_map(ID_to_taxon_map_filename);   // may add taxa
+  {
+    vector<uint32_t> ids, parents;                        // Parent_map, new taxa included
+    for (auto &kv : Taxa) {
+      if (kv.first == 0) continue;
+      ids.push_back(kv.first);
+      parents.push_back(parent_map(kv.first));
+    }
+    if (kuq_set_taxonomy(Ctx, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+  }
 
   Batch batch;
   if (one_fasta_file) {                                   // process_single_file, set_lcas.cpp:272-386
-    cerr << "Reading sequence ID to taxonomy ID mapping ... ";
-    unordered_map<string, uint32_t> id_to_taxon;          // read_seqid_to_taxid_map, :200-270 (first mapping wins)
-    {
-      ifstream map_file(ID_to_taxon_map_filename.c_str());
-      if (map_file.rdstate() & ifstream::failbit) die(EX_NOINPUT, "can't open " + ID_to_taxon_map_filename, TOOL);
-      string line, seq_id;
-      uint32_t taxid = 0;
-      while (map_file.good()) {
-        getline(map_file, line);
-        if (line.empty()) break;
-        istringstream iss(line);
-        iss >> seq_id >> taxid;
-        if (!id_to_taxon.count(seq_id)) id_to_taxon[seq_id] = taxid;
-      }
-      if (id_to_taxon.empty()) cerr << "Error: No ID mappings present!!" << endl;
-      cerr << " got " << id_to_taxon.size() << " mappings." << endl;
-    }
     Fasta reader(Multi_fasta_filename);
     const string prefix = "kraken:taxid|";
     uint32_t seqs_processed = 0, seqs_skipped = 0, seqs_no_taxid = 0;
@@ -339,6 +418,8 @@ int main(int argc, char **argv) {
       if (taxid == 0 && id.size() >= prefix.size() && id.compare(0, prefix.size(), prefix) == 0) {   // :315-323
         taxid = (uint32_t)strtol(id.c_str() + prefix.size(), NULL, 10);
         if (taxid == 0) cerr << "Error: taxonomy ID is zero for sequence '" << id << "'?!" << endl;
+        const size_t begin = header.find_first_not_of("\t ");
+        if (begin != string::npos) header = header.substr(begin);
       }
       if (taxid == 0) {
         cerr << "Error! Didn't find taxonomy ID mapping for sequence " << id << "!!" << endl;
@@ -350,12 +431,16 @@ int main(int argc, char **argv) {
         ++seqs_skipped;
         continue;
       }
-      if (!parent_of.count(taxid) || taxid == 0) {        // :336-341
+      if (taxid == 0 || !Taxa.count(taxid)) {             // :336-341
         cerr << "Skipping sequence " << id << " since taxonomy ID " << taxid << " is not in taxonomy database!" << endl;
         ++seqs_skipped;
         continue;
       }
-      add_sequence(batch, seq, taxid);
+      if (Add_taxids_for_sequences) {                     // the taxon is named after the header line, :344-353
+        const uint32_t par = parent_map(taxid);
+        if (taxid != TID_HUMAN && par != TID_HUMAN && taxid != TID_MOUSE && par != TID_MOUSE) Taxa.at(taxid).name = header;
+      }
+      add_sequence(batch, seq, taxid);                    // -T tests the mapped taxid, :344
       ++seqs_processed;
       cerr << "\rProcessed " << seqs_processed << " sequences";
     }
@@ -380,7 +465,7 @@ int main(int argc, char **argv) {
       Fasta reader(filename);
       string id, header, seq;
       reader.next(id, header, seq);                       // the first sequence only, :414-421
-      if (!parent_of.count(taxid) || taxid == 0)
+      if (taxid == 0 || !Taxa.count(taxid))
         cerr << "Skipping " << filename << " since taxonomy ID " << taxid << " is not in taxonomy database!" << endl;
       else
         add_sequence(batch, seq, taxid);
@@ -415,6 +500,10 @@ int main(int argc, char **argv) {
     if (Operate_in_RAM) cerr << "Writing database from RAM back to " << target << " ..." << endl;
     write_file(target, out.data(), out.size(), TOOL);
     if (!Output_DB_filename.empty() && !Operate_in_RAM) write_file(Output_DB_filename, out.data(), out.size(), TOOL);
+  }
+  if ((Add_taxids_for_sequences || Add_taxids_for_assembly) && !Pretend) {   // the taxDB is rewritten in place, :171-177
+    cerr << "Writing new TaxDB ..." << endl;
+    write_taxdb(TaxDB_filename);
   }
   kuq_destroy(Ctx);
   return 0;
