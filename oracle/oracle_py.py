@@ -387,6 +387,10 @@ class RefShim:
         L.kuref_hll_cardinality.argtypes = [C.c_void_p]
         L.kuref_hll_n_observed.restype = C.c_uint64
         L.kuref_hll_n_observed.argtypes = [C.c_void_p]
+        L.kuref_get_rank64.restype = C.c_uint32
+        L.kuref_get_rank64.argtypes = [C.c_uint64, C.c_uint32]
+        L.kuref_get_encoded_rank.restype = C.c_uint32
+        L.kuref_get_encoded_rank.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32]
 
     def open_db(self, kdb: np.ndarray, idx: np.ndarray):
         return RefDB(self, kdb, idx)

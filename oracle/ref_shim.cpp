@@ -18,6 +18,10 @@
 
 using namespace kraken;
 
+// Non-inline free functions of hyperloglogplus.cpp (:131-161) that its header does not declare.
+uint8_t getRank(const uint64_t hash_value, const uint8_t p);
+uint8_t getEncodedRank(const uint32_t encoded_hash_value, const uint8_t pPrime, const uint8_t p);
+
 namespace {
 struct RefDB {
   KrakenDB *db;          // never deleted: ~KrakenDB munmaps an uninitialised pointer (src/krakendb.cpp:81-83)
@@ -119,5 +123,11 @@ void kuref_hll_merge(void *dst, void *src) { *(HLL *)dst += *(const HLL *)src; }
 void kuref_hll_merge_move(void *dst, void *src) { *(HLL *)dst += std::move(*(HLL *)src); }  // merge(&&), :586-625
 uint64_t kuref_hll_cardinality(void *h) { return ((HLL *)h)->ertlCardinality(); }    // :722-753
 uint64_t kuref_hll_n_observed(void *h) { return ((HLL *)h)->nObserved(); }
+// getRank(uint64_t hash, p) — src/hyperloglogplus.cpp:140-147
+uint32_t kuref_get_rank64(uint64_t hash, uint32_t p) { return getRank(hash, (uint8_t)p); }
+// getEncodedRank(encoded, pPrime, p) — src/hyperloglogplus.cpp:152-161
+uint32_t kuref_get_encoded_rank(uint32_t encoded, uint32_t p_prime, uint32_t p) {
+  return getEncodedRank(encoded, (uint8_t)p_prime, (uint8_t)p);
+}
 
 }  // extern "C"
