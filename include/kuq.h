@@ -435,15 +435,28 @@ int kuq_layout_experiment(kuq_ctx *ctx, uint32_t slot, uint64_t n_positions, uin
 /* ---- database build (SURVEY.md §8 f4) ---------------------------------------------------------------------- */
 /* db_sort [-z] -n nt (db_sort.cpp:41-116 + KrakenDB::make_index, krakendb.cpp:118-148): unsorted Jellyfish-style
  * image → database.kdb image (kdb_out: header + key_ct * (key_len + 4) bytes) and KRAKIX2 index image (idx_out:
- * 8 + 8 * (4^nt + 1) bytes).  Needs no context.  err (optional) receives a message on failure. */
+ * 8 + 8 * (4^nt + 1) bytes).  Needs no context.  err (optional) receives a message on failure.
+ * kuq_db_sort = kuq_db_sort_budget with budget 0. */
 int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, void *kdb_out,
                 void *idx_out, char *err, uint64_t err_cap);
+/* db_sort within `budget` bytes of device memory (0 → environment variable KUQ_DB_SORT_BUDGET, else 3/4 of the free
+ * device memory).  When the one-piece working set (about 2 * (key_len + 4) + 60 bytes per record plus 8 * (4^nt + 1)
+ * for the index) does not fit, the sort runs in passes over the two host images: the input streams through the device
+ * twice (bin histogram → index; grouping by minimizer range into the output image), then every range is sorted in
+ * place.  The result is the same bytes; PCIe carries about five times the database.  *n_passes (optional) = 1 for the
+ * one-piece sort, else the number of ranges.  KUQ_E_CAPACITY when the index or one minimizer bin does not fit. */
+int kuq_db_sort_budget(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
+                       void *kdb_out, void *idx_out, uint32_t *n_passes, char *err, uint64_t err_cap);
 /* set_lcas (set_lcas.cpp:429-476): for every k-mer of the library pieces that the staged database holds,
  * value = lca(taxid of the piece, value).  A piece is a stretch of one library sequence; consecutive pieces of a
  * sequence overlap by k-1 bases (the reference's SKIP_LEN pieces, :363-364).  The context needs the database
- * (kuq_stage_db, whole) and the taxonomy (kuq_set_taxonomy); every taxid must be in the taxonomy — the reference
+ * (kuq_stage_db) and the taxonomy (kuq_set_taxonomy); every taxid must be in the taxonomy — the reference
  * skips other sequences (:336-341) and so must the caller.  *n_missing = k-mers of this batch the database lacks (set_lcas
  * without -x stops there, :441-443).  After the first call the context cannot classify any more.
+ * With a minimizer range [bin_lo, bin_hi) staged, only the k-mers whose bin lies in the range are looked up; the others
+ * are neither updated nor counted as missing.  A database larger than HBM is built range by range: declare the taxids
+ * of all its records (kuq_set_db_taxid_universe) before the taxonomy, then per range kuq_stage_db, the same batches in
+ * the same order, kuq_export_db_values; the missing counts of the ranges add up to the one-piece count.
  * flags: KUQ_LCA_FORCE_CONTAMINANT = set_lcas -T (what build_db.sh always passes: a value of 32630 'synthetic
  * construct' / 81077 'artificial sequences' sticks and a piece with such a taxid overwrites instead of taking the LCA,
  * :462-474; between those two taxids the first to arrive wins, so one batch may hold pieces of only one of them),
@@ -454,7 +467,8 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
                        const uint32_t *taxid, uint32_t flags, uint64_t *n_missing);
 /* Copy the record values of the staged database (as taxids) into the value fields of a host database.kdb image
  * with the same records — what set_lcas leaves in the memory-mapped file.  Values are written at the file's record
- * stride (key_len + 4 bytes), whatever the staged layout. */
+ * stride (key_len + 4 bytes), whatever the staged layout.  A staged range writes only its own records, at their
+ * positions in the file. */
 int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes);
 
 /* k-mer set of a FASTA library: step 1 of build_db.sh (scripts/build_db.sh:116-147), `jellyfish count -m k -C` of

@@ -108,6 +108,8 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_set_db_taxid_universe": (C.c_int, [vp, u32p, C.c_uint32]),
         "kuq_mark_zero_hits": (C.c_int, [vp, C.c_int]),
         "kuq_db_sort": (C.c_int, [C.c_int, vp, C.c_uint64, C.c_uint32, C.c_int, vp, vp, C.c_char_p, C.c_uint64]),
+        "kuq_db_sort_budget": (C.c_int, [C.c_int, vp, C.c_uint64, C.c_uint32, C.c_int, C.c_uint64, vp, vp, u32p, C.c_char_p,
+                                         C.c_uint64]),
         "kuq_set_lcas_batch": (C.c_int, [vp, vp, u64p, C.c_uint32, u32p, C.c_uint32, u64p]),
         "kuq_export_db_values": (C.c_int, [vp, vp, C.c_uint64]),
         "kuq_set_quick_mode": (C.c_int, [vp, C.c_uint32, C.c_int]),
@@ -610,8 +612,10 @@ def decode_runs(res, i):
     return [(int(a), int(b)) for a, b in res["runs"][s:s + c]]
 
 
-def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0):
-    """kuq_db_sort: unsorted Jellyfish-style image → (database.kdb image, KRAKIX2 index image), on the GPU"""
+def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0, budget=0, with_passes=False):
+    """kuq_db_sort_budget: unsorted Jellyfish-style image → (database.kdb image, KRAKIX2 index image), on the GPU within
+    `budget` bytes of device memory (0 → KUQ_DB_SORT_BUDGET, else 3/4 of the free memory).  with_passes: also return
+    the number of passes (1 = in one piece, else the number of minimizer ranges)."""
     L = load_library()
     jdb = np.ascontiguousarray(jdb, np.uint8)
     key_bits = int(np.frombuffer(jdb[8:16].tobytes(), np.uint64)[0])
@@ -620,10 +624,12 @@ def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0):
     kdb = np.zeros(size, np.uint8)
     idx = np.zeros(8 + 8 * (4 ** nt + 1), np.uint8)
     err = C.create_string_buffer(512)
-    rc = L.kuq_db_sort(device, jdb.ctypes.data, jdb.size, nt, 1 if zero_vals else 0, kdb.ctypes.data, idx.ctypes.data, err, 512)
+    passes = C.c_uint32(0)
+    rc = L.kuq_db_sort_budget(device, jdb.ctypes.data, jdb.size, nt, 1 if zero_vals else 0, budget, kdb.ctypes.data,
+                              idx.ctypes.data, C.byref(passes), err, 512)
     if rc != 0:
         raise KuqError(rc, err.value.decode() or L.kuq_strerror(rc).decode())
-    return kdb, idx
+    return (kdb, idx, passes.value) if with_passes else (kdb, idx)
 
 
 def kdb_header(k: int, key_ct: int) -> np.ndarray:

@@ -43,6 +43,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_ranges.h"
 
 using namespace std;
 
@@ -1103,23 +1104,10 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
 }
 
 // ---- chunked mode: `-x size` with a database that does not fit (process_file_with_db_chunk, classify.cpp:566-791) --
-// Ranges of minimizer bins whose records + index slice fit the budget (prepare_chunking / upper_bound,
-// krakendb.cpp:430-522).  Any byte-balanced partition gives the same results (a key lives in one bin).
+// Ranges of minimizer bins whose records (12 bytes each in HBM) + index slice fit the budget: kuq_ranges.h.
 static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uint64_t n_bins, uint64_t budget) {
   vector<pair<uint64_t, uint64_t>> ranges;
-  uint64_t first = 0;
-  while (first < n_bins) {
-    uint64_t lo = first, hi = n_bins;                 // largest `end` in (first, n_bins] that still fits
-    auto fits = [&](uint64_t end) { return (end - first + 1) * 8 + (offsets[end] - offsets[first]) * 12 + 8 <= budget; };
-    if (!fits(first + 1)) die(EX_SOFTWARE, "a single minimizer bin exceeds the chunk budget; raise -x");
-    lo = first + 1;
-    while (lo < hi) {
-      uint64_t mid = lo + (hi - lo + 1) / 2;
-      if (fits(mid)) lo = mid; else hi = mid - 1;
-    }
-    if (offsets[lo] > offsets[first]) ranges.emplace_back(first, lo);   // skip ranges without records (:496-499)
-    first = lo;
-  }
+  if (!plan_ranges(offsets, n_bins, budget, 12, ranges)) die(EX_SOFTWARE, "a single minimizer bin exceeds the chunk budget; raise -x");
   return ranges;
 }
 

@@ -27,6 +27,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_ranges.h"
 
 using namespace std;
 
@@ -64,7 +65,9 @@ static void write_file(const string &path, const void *data, size_t size, const 
 // ====================================================================================================================
 static const char *TOOL = "db_sort";
 static void usage(int exit_code = EX_USAGE) {
-  cerr << "Usage: db_sort [-z] [-M] [-t threads] [-n nt] <-d input db> <-o output db> <-i output idx>\n";
+  cerr << "Usage: db_sort [-z] [-M] [-t threads] [-n nt] <-d input db> <-o output db> <-i output idx>\n"
+       << "KUQ_DB_SORT_BUDGET (bytes of device memory; default 3/4 of the free memory): a database whose sort does not fit\n"
+       << "is sorted in passes over minimizer ranges.\n";
   exit(exit_code);
 }
 
@@ -107,8 +110,10 @@ int main(int argc, char **argv) {
   cerr << "db_sort: Sorting ...";
   char err[512] = "";
   int dev = getenv("KUQ_DEVICE") ? atoi(getenv("KUQ_DEVICE")) : 0;
-  int rc = kuq_db_sort(dev, in.p, in.size, nt, zero_vals, kdb.data(), idx.data(), err, sizeof err);
+  uint32_t passes = 0;                                  // budget: KUQ_DB_SORT_BUDGET, else 3/4 of free device memory
+  int rc = kuq_db_sort_budget(dev, in.p, in.size, nt, zero_vals, 0, kdb.data(), idx.data(), &passes, err, sizeof err);
   if (rc) die(rc == KUQ_E_NO_DEVICE ? EX_UNAVAILABLE : EX_DATAERR, err[0] ? err : kuq_strerror(rc), TOOL);
+  cerr << "db_sort: " << passes << (passes == 1 ? " pass" : " passes") << endl;
   cerr << "db_sort: Sorting complete - writing database to disk ..." << endl;
   write_file(index, idx.data(), idx.size(), TOOL);       // make_index, krakendb.cpp:141-147
   write_file(output, kdb.data(), kdb.size(), TOOL);      // db_sort.cpp:69-73
@@ -199,14 +204,23 @@ static kuq_ctx *Ctx = NULL;
 static uint32_t K = 0;
 static uint64_t Missing_total = 0;
 static const uint64_t BATCH_NT = 64ull << 20;
+// With the database staged in several minimizer ranges, every batch is kept to be replayed against the later ranges:
+// the library may be a pipe that can be read once (build_db.sh passes -F <(cat_library)).
+static bool Keep_batches = false;
+static vector<Batch> Kept;
 
-static void flush(Batch &b) {
-  if (b.taxids.empty()) return;
+static void run_batch(const Batch &b) {
   uint64_t missing = 0;
   if (kuq_set_lcas_batch(Ctx, b.bases.data(), b.offs.data(), (uint32_t)b.taxids.size(), b.taxids.data(), Lca_flags, &missing))
     die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
   if (missing && !Allow_extra_kmers) die(EX_DATAERR, "kmer found in sequence that is not in database", TOOL);   // :441-443
   Missing_total += missing;
+}
+
+static void flush(Batch &b) {
+  if (b.taxids.empty()) return;
+  run_batch(b);
+  if (Keep_batches) { Kept.push_back(std::move(b)); b = Batch(); return; }
   b.bases.clear(); b.offs.assign(1, 0); b.taxids.clear(); b.contaminant = 0;
 }
 
@@ -328,6 +342,38 @@ static unordered_map<string, uint32_t> read_seqid_map(const string &path) {
   return id_to_taxon;
 }
 
+// The minimizer ranges staged one at a time: as few as KUQ_SET_LCAS_BUDGET bytes of device memory allow (default: the
+// free memory less 1 GiB for the batch and the staging buffers), 12 bytes per record in HBM.  Together they cover every
+// bin, so that a k-mer whose bin holds no records is still counted as missing.  {(0, 0)} = the whole database at once;
+// so is an index that does not parse (kuq_stage_db reports it).
+static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const Mapped &kdb, const Mapped &idx) {
+  const vector<pair<uint64_t, uint64_t>> whole{{0, 0}};
+  const uint8_t *q = (const uint8_t *)idx.p;
+  if (idx.size < 8 || kdb.size < 56) return whole;
+  const uint32_t nt = q[7];
+  const uint64_t n_bins = 1ull << (2 * (nt & 15));
+  uint64_t key_ct;
+  memcpy(&key_ct, (const char *)kdb.p + 48, 8);
+  const uint64_t *offsets = (const uint64_t *)(q + 8);
+  if (nt < 1 || nt > 15 || idx.size < 8 + 8 * (n_bins + 1) || offsets[n_bins] > key_ct) return whole;
+  uint64_t budget = getenv("KUQ_SET_LCAS_BUDGET") ? strtoull(getenv("KUQ_SET_LCAS_BUDGET"), NULL, 10) : 0;
+  if (!budget) {
+    const uint64_t free_b = kuq_device_free_bytes(Ctx);
+    budget = free_b > (2ull << 30) ? free_b - (1ull << 30) : free_b / 2;
+  }
+  vector<pair<uint64_t, uint64_t>> ranges;
+  if (!plan_ranges(offsets, n_bins, budget, 12, ranges)) die(EX_SOFTWARE, "a single minimizer bin exceeds KUQ_SET_LCAS_BUDGET", TOOL);
+  if (ranges.size() <= 1) return whole;
+  ranges.front().first = 0;                              // bins of ranges without records join the range before them
+  for (size_t r = 1; r < ranges.size(); r++) ranges[r - 1].second = ranges[r].first;
+  ranges.back().second = n_bins;
+  return ranges;
+}
+
+static void stage(const Mapped &kdb, const Mapped &idx, const pair<uint64_t, uint64_t> &range) {
+  if (kuq_stage_db(Ctx, kdb.p, kdb.size, idx.p, idx.size, range.first, range.second)) die(EX_DATAERR, kuq_last_error(Ctx), TOOL);
+}
+
 int main(int argc, char **argv) {
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
   int opt;
@@ -380,7 +426,27 @@ int main(int argc, char **argv) {
   if (getenv("KUQ_DEVICE")) cfg.device = atoi(getenv("KUQ_DEVICE"));
   int rc = kuq_create(&cfg, &Ctx);
   if (rc) die(EX_UNAVAILABLE, string("libkuq: ") + kuq_strerror(rc), TOOL);
-  if (kuq_stage_db(Ctx, kdb.p, kdb.size, idx.p, idx.size, 0, 0)) die(EX_DATAERR, kuq_last_error(Ctx), TOOL);
+  const vector<pair<uint64_t, uint64_t>> ranges = plan_lca_ranges(kdb, idx);
+  if (ranges.size() > 1) {
+    // one taxid numbering for every range: the values of all records (as classify -x numbers them); range 0 last, so
+    // that it stays staged for the pass that reads the library
+    cerr << "Database staged in " << ranges.size() << " minimizer ranges" << endl;
+    vector<uint32_t> all;
+    for (size_t r = ranges.size(); r-- > 0;) {
+      stage(kdb, idx, ranges[r]);
+      uint32_t m = 0;
+      kuq_db_taxids(Ctx, NULL, NULL, 0, &m);
+      vector<uint32_t> t(m);
+      if (m && kuq_db_taxids(Ctx, t.data(), NULL, m, &m)) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+      all.insert(all.end(), t.begin(), t.end());
+    }
+    sort(all.begin(), all.end());
+    all.erase(unique(all.begin(), all.end()), all.end());
+    if (kuq_set_db_taxid_universe(Ctx, all.data(), (uint32_t)all.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+    Keep_batches = true;
+  } else {
+    stage(kdb, idx, ranges[0]);
+  }
   unordered_map<string, uint32_t> id_to_taxon;
   if (one_fasta_file) id_to_taxon = read_seqid_map(ID_to_taxon_map_filename);   // may add taxa
   {
@@ -475,10 +541,15 @@ int main(int argc, char **argv) {
     cerr << "\r                                                       ";
     cerr << "\rFinished processing " << seqs_processed << " sequences" << endl;
   }
-  if (verbose && Missing_total) cerr << Missing_total << " k-mers of the library are not in the database" << endl;
-
   vector<char> out((const char *)kdb.p, (const char *)kdb.p + kdb.size);
   if (kuq_export_db_values(Ctx, out.data(), out.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+  for (size_t r = 1; r < ranges.size(); r++) {            // the same batches in the same order against each further range
+    stage(kdb, idx, ranges[r]);
+    for (const Batch &b : Kept) run_batch(b);
+    if (kuq_export_db_values(Ctx, out.data(), out.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+    cerr << "Finished minimizer range " << (r + 1) << " of " << ranges.size() << endl;
+  }
+  if (verbose && Missing_total) cerr << Missing_total << " k-mers of the library are not in the database" << endl;
   if (!Kmer_count_filename.empty()) {                     // count_taxons, krakendb.cpp:90-113 → :141-150
     cerr << "Writing kmer counts to " << Kmer_count_filename << "..." << endl;
     const uint64_t key_len = key_bits / 8 + !!(key_bits % 8), header = 72 + 2 * (4 + 8 * key_bits);

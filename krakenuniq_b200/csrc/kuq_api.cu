@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_bounce.cuh"
 #include "kuq_kernels.cuh"
 
 using namespace kuq;
@@ -1046,51 +1047,27 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   CU(cudaMalloc((void **)&ctx->d_pairs, ctx->key_ct * 12 + SLACK));
   CU(dmalloc(&ctx->d_offsets_owned, bin_hi - bin_lo + 1));
   ctx->d_offsets = ctx->d_offsets_owned;
-  // bulk H2D.  The images are usually mmap'ed files: a plain cudaMemcpy from pageable memory goes through the driver's
-  // single-threaded staging (~7 GB/s, page faults included).  Instead a few threads fault the pages in and copy 64 MB
-  // pieces into two pinned bounce buffers while the previous piece travels (cudaMemcpyAsync on the aux stream).
-  // Records shorter than 12 bytes (k <= 28) travel as they are in the file: each piece lands in one bounded device buffer
-  // and k_widen_records writes it into d_pairs in the 12-byte layout, behind the copy on the same stream.
+  // bulk H2D through pinned bounce buffers (kuq_bounce.cuh) on the aux stream.  Records shorter than 12 bytes (k <= 28)
+  // travel as they are in the file: each piece lands in one bounded device buffer and k_widen_records writes it into
+  // d_pairs in the 12-byte layout, behind the copy on the same stream.
   {
-    const uint64_t CH = 64ull << 20;
-    const int NT = 8;
+    PinnedBounce bounce;
+    CU(bounce.init());
     uint8_t *d_land = nullptr;
-    const uint64_t land_rec = pair_sz == 12 ? 0 : std::min(landing_records(pair_sz), CH / pair_sz);
+    const uint64_t land_rec = pair_sz == 12 ? 0 : std::min(landing_records(pair_sz), PinnedBounce::CH / pair_sz);
     if (land_rec && ctx->key_ct) CU(cudaMalloc((void **)&d_land, land_rec * pair_sz + SLACK));
-    uint8_t *bounce[2] = {nullptr, nullptr};
-    cudaEvent_t ev[2];
-    bool ok = cudaHostAlloc((void **)&bounce[0], CH, cudaHostAllocPortable) == cudaSuccess &&
-              cudaHostAlloc((void **)&bounce[1], CH, cudaHostAllocPortable) == cudaSuccess;
-    if (!ok) (void)cudaGetLastError();
-    for (int b = 0; b < 2; b++) CU(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
     // rec_sz = 0: bytes are copied to d_dst as they are; else they are records of rec_sz bytes, widened into d_dst
     auto piece_copy = [&](uint8_t *d_dst, const uint8_t *h_src, uint64_t bytes, uint64_t rec_sz) -> int {
-      if (!ok && !rec_sz) { CU(cudaMemcpy(d_dst, h_src, bytes, cudaMemcpyHostToDevice)); return KUQ_OK; }
-      const uint64_t step = rec_sz ? land_rec * rec_sz : CH;
-      uint64_t i = 0;
-      for (uint64_t off = 0; off < bytes; off += step, i++) {
-        const uint64_t n = std::min(step, bytes - off);
-        uint8_t *to = rec_sz ? d_land : d_dst + off;
-        if (!ok) {
-          CU(cudaMemcpyAsync(to, h_src + off, n, cudaMemcpyHostToDevice, ctx->aux));   // in order behind the last widening
-        } else {
-          const int b = (int)(i & 1);
-          CU(cudaEventSynchronize(ev[b]));                       // the bounce buffer's previous piece has left
-          std::vector<std::thread> th;
-          const uint64_t per = (n + NT - 1) / NT;
-          for (int t = 0; t < NT; t++) {
-            const uint64_t a = std::min(n, per * t), e = std::min(n, per * (t + 1));
-            if (e > a) th.emplace_back([=] { memcpy(bounce[b] + a, h_src + off + a, e - a); });
-          }
-          for (auto &x : th) x.join();
-          CU(cudaMemcpyAsync(to, bounce[b], n, cudaMemcpyHostToDevice, ctx->aux));
-        }
-        if (rec_sz) {
+      if (!rec_sz) {
+        CU(bounce.to_device(d_dst, h_src, bytes, ctx->aux));
+      } else {
+        for (uint64_t off = 0, step = land_rec * rec_sz; off < bytes; off += step) {
+          const uint64_t n = std::min(step, bytes - off);
+          CU(bounce.h2d(d_land, h_src + off, n, ctx->aux));       // in order behind the last widening
           launch_widen_records(d_land, n / rec_sz, (uint32_t)(rec_sz - 4), d_dst + off / rec_sz * 12, ctx->aux);
           ctx->launches++;
           CU(cudaGetLastError());
         }
-        if (ok) CU(cudaEventRecord(ev[i & 1], ctx->aux));
       }
       CU(cudaStreamSynchronize(ctx->aux));
       return KUQ_OK;
@@ -1099,7 +1076,6 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
     int crc = piece_copy(ctx->d_pairs, src, ctx->key_ct * pair_sz, pair_sz == 12 ? 0 : pair_sz);
     if (!crc) crc = piece_copy(reinterpret_cast<uint8_t *>(ctx->d_offsets_owned), reinterpret_cast<const uint8_t *>(offsets + bin_lo),
                                (bin_hi - bin_lo + 1) * 8, 0);
-    for (int b = 0; b < 2; b++) { cudaEventDestroy(ev[b]); if (bounce[b]) cudaFreeHost(bounce[b]); }
     cudaFree(d_land);
     if (crc) return crc;
   }
@@ -2726,8 +2702,8 @@ uint64_t kuq_ertl_dense(const uint8_t *regs, uint64_t n_observed) {
 }
 
 // ---- database build (SURVEY.md §8 f4; ROUND 1: compiled, not yet run on hardware) ---------------------------------
-int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, void *kdb_out,
-                void *idx_out, char *err, uint64_t err_cap) {
+int kuq_db_sort_budget(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
+                       void *kdb_out, void *idx_out, uint32_t *n_passes, char *err, uint64_t err_cap) {
   int n_dev = 0;
   if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
     if (err && err_cap) snprintf(err, err_cap, "db_sort: no CUDA device (there is no CPU path)");
@@ -2735,8 +2711,16 @@ int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t 
     return KUQ_E_NO_DEVICE;
   }
   if (device < 0 || device >= n_dev || cudaSetDevice(device) != cudaSuccess) return KUQ_E_INVALID_ARG;
-  int rc = dbsort_device((const uint8_t *)jdb_image, jdb_bytes, nt, zero_vals, (uint8_t *)kdb_out, (uint8_t *)idx_out, err, err_cap);
-  return rc ? KUQ_E_DB_FORMAT : KUQ_OK;
+  uint32_t passes = 0;
+  int rc = dbsort_device((const uint8_t *)jdb_image, jdb_bytes, nt, zero_vals, budget, (uint8_t *)kdb_out, (uint8_t *)idx_out,
+                         &passes, err, err_cap);
+  if (n_passes) *n_passes = passes;
+  return rc;
+}
+
+int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, void *kdb_out,
+                void *idx_out, char *err, uint64_t err_cap) {
+  return kuq_db_sort_budget(device, jdb_image, jdb_bytes, nt, zero_vals, 0, kdb_out, idx_out, NULL, err, err_cap);
 }
 
 int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_offsets, uint32_t n_pieces,
@@ -2750,7 +2734,6 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
   rc = ensure_ready(ctx);
   if (rc) return rc;
   if (n_pieces > ctx->cfg.max_reads_per_batch) return fail(ctx, KUQ_E_CAPACITY, "%u pieces > slot capacity %u", n_pieces, ctx->cfg.max_reads_per_batch);
-  if (ctx->bin_lo != 0 || ctx->rec_base != 0) return fail(ctx, KUQ_E_STATE, "set_lcas needs the whole database staged");
   for (uint32_t i = 0; i < n_pieces; i++) {
     // the reference skips sequences whose taxid the taxonomy does not hold (set_lcas.cpp:336-341): the caller's job
     auto it = ctx->dense_of_raw.find(taxid[i]);
@@ -2791,15 +2774,15 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
 int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes) {
   if (!ctx || !kdb_image) return KUQ_E_INVALID_ARG;
   if (!ctx->db_staged || !ctx->db_owned) return fail(ctx, KUQ_E_STATE, "no database staged from a host image");
-  if (ctx->bin_lo != 0 || ctx->rec_base != 0) return fail(ctx, KUQ_E_STATE, "only a fully staged database can be exported");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   const uint64_t key_bits = 2ull * ctx->k, header = 72 + 2 * (4 + 8 * key_bits);
   const uint64_t key_len = (key_bits + 7) / 8, pair_sz = key_len + 4;            // the file's records, not HBM's 12 bytes
-  if (kdb_bytes < header + ctx->key_ct * pair_sz) return fail(ctx, KUQ_E_INVALID_ARG, "image too small for %llu records", (unsigned long long)ctx->key_ct);
+  if (kdb_bytes < header + (ctx->rec_base + ctx->key_ct) * pair_sz)
+    return fail(ctx, KUQ_E_INVALID_ARG, "image too small for %llu records", (unsigned long long)(ctx->rec_base + ctx->key_ct));
   std::vector<uint8_t> rec(ctx->key_ct * 12);
   CU(cudaMemcpy(rec.data(), ctx->d_pairs, rec.size(), cudaMemcpyDeviceToHost));
-  uint8_t *out = (uint8_t *)kdb_image + header;
+  uint8_t *out = (uint8_t *)kdb_image + header + ctx->rec_base * pair_sz;       // a staged range: its records only
   for (uint64_t i = 0; i < ctx->key_ct; i++) {
     uint32_t v;
     memcpy(&v, rec.data() + i * 12 + 8, 4);

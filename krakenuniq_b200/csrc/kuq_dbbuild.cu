@@ -7,8 +7,18 @@
 // DeviceRadixSort (library code; database build is not the hot path north_star names), the kernels around them —
 // minimizer of every stored key, bin histogram, record gather — are ours.  Records never move during the sorts:
 // only (key, index) and (bin, index) pairs do, and one gather at the end writes the 12-byte records.
+//
+// A database whose one-piece working set does not fit the byte budget is sorted in passes over the host images:
+//   A. the record body streams through the device once for the bin histogram, whose running sum is database.idx;
+//   B. it streams once more and every chunk is grouped, stably, by minimizer range (kuq_ranges.h cuts the ranges
+//      from the index); each range's slice goes to that range's cursor in the output image;
+//   C. each range's records come back to the device, get the two sorts of the one-piece path, and return in place.
+// Within a range the records keep input order until C, so repeated keys come out as in the one-piece sort.
+#include "../../include/kuq.h"
+#include "kuq_bounce.cuh"
 #include "kuq_kernels.cuh"
 #include "kuq_minimizer.cuh"
+#include "kuq_ranges.h"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -20,31 +30,61 @@
 namespace kuq {
 namespace {
 
-// one thread per record: key, its bin, its position; the bin histogram on the way (make_index :126-134)
-__global__ void k_dbs_keys(const uint8_t *pairs, uint64_t n, uint32_t key_len, uint32_t k, uint32_t nt,
-                           unsigned long long *keys, uint32_t *bins, unsigned long long *index,
-                           unsigned long long *bin_counts) {
+typedef unsigned long long ull;
+
+__device__ __forceinline__ uint64_t record_key(const uint8_t *r, uint32_t key_len) {
+  uint64_t key = 0;
+  for (uint32_t b = 0; b < key_len; b++) key |= (uint64_t)r[b] << (8 * b);  // memcpy(&kmer, pair, key_len), :99-100
+  return key;
+}
+
+// one thread per record: key, its bin (relative to bin_lo), its position; the bin histogram on the way if asked
+// (make_index :126-134)
+__global__ void k_dbs_keys(const uint8_t *pairs, uint64_t n, uint32_t key_len, uint32_t k, uint32_t nt, uint32_t bin_lo,
+                           ull *keys, uint32_t *bins, ull *index, ull *bin_counts) {
   const uint32_t pair_sz = key_len + 4;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint8_t *r = pairs + i * pair_sz;
-    uint64_t key = 0;
-    for (uint32_t b = 0; b < key_len; b++) key |= (uint64_t)r[b] << (8 * b);  // memcpy(&kmer, pair, key_len), :99-100
+    const uint64_t key = record_key(pairs + i * pair_sz, key_len);
     const uint32_t bin = bin_key_of(key, k, nt);
     keys[i] = key;
-    bins[i] = bin;
+    bins[i] = bin - bin_lo;
     index[i] = i;
-    atomicAdd(bin_counts + bin + 1, 1ull);                                     // offsets[b + 1] after the scan
+    if (bin_counts) atomicAdd(bin_counts + bin + 1, 1ull);                     // offsets[b + 1] after the scan
   }
 }
 
-__global__ void k_dbs_gather_bins(const uint32_t *bins, const unsigned long long *index, uint64_t n, uint32_t *out) {
+// pass A: the bin histogram alone
+__global__ void k_dbs_hist(const uint8_t *pairs, uint64_t n, uint32_t key_len, uint32_t k, uint32_t nt, ull *bin_counts) {
+  const uint32_t pair_sz = key_len + 4;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    atomicAdd(bin_counts + bin_key_of(record_key(pairs + i * pair_sz, key_len), k, nt) + 1, 1ull);
+}
+
+// pass B: the range of each record (range r starts at bin starts[r]; every record's bin lies in some range), its
+// position, and the chunk's record count per range
+__global__ void k_dbs_range_of(const uint8_t *pairs, uint64_t n, uint32_t key_len, uint32_t k, uint32_t nt,
+                               const uint32_t *starts, uint32_t n_ranges, uint32_t *rid, ull *index, ull *range_counts) {
+  const uint32_t pair_sz = key_len + 4;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t bin = bin_key_of(record_key(pairs + i * pair_sz, key_len), k, nt);
+    uint32_t lo = 0, hi = n_ranges;                                            // last start <= bin
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(starts + mid) <= bin) lo = mid; else hi = mid;
+    }
+    rid[i] = lo;
+    index[i] = i;
+    atomicAdd(range_counts + lo, 1ull);
+  }
+}
+
+__global__ void k_dbs_gather_bins(const uint32_t *bins, const ull *index, uint64_t n, uint32_t *out) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
     out[i] = bins[index[i]];
 }
 
 // output record i = input record index[i]; -z zeroes the value (db_sort.cpp:105-106)
-__global__ void k_dbs_emit(const uint8_t *in, const unsigned long long *index, uint64_t n, uint32_t key_len,
-                           int zero_vals, uint8_t *out) {
+__global__ void k_dbs_emit(const uint8_t *in, const ull *index, uint64_t n, uint32_t key_len, int zero_vals, uint8_t *out) {
   const uint32_t pair_sz = key_len + 4;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint8_t *src = in + index[i] * pair_sz;
@@ -54,14 +94,14 @@ __global__ void k_dbs_emit(const uint8_t *in, const unsigned long long *index, u
   }
 }
 
-int seterr(char *err, size_t cap, const char *fmt, ...) {
+int seterr(int code, char *err, size_t cap, const char *fmt, ...) {
   if (err && cap) {
     va_list ap;
     va_start(ap, fmt);
     vsnprintf(err, cap, fmt, ap);
     va_end(ap);
   }
-  return -1;
+  return code;
 }
 
 struct Buffers {                    // frees on scope exit whatever was allocated
@@ -79,82 +119,283 @@ struct Buffers {                    // frees on scope exit whatever was allocate
 #define DB_CU(call)                                                                                      \
   do {                                                                                                   \
     cudaError_t e__ = (call);                                                                            \
-    if (e__ != cudaSuccess) return seterr(err, err_cap, "db_sort: %s: %s", #call, cudaGetErrorString(e__)); \
+    if (e__ != cudaSuccess) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: %s: %s", #call, cudaGetErrorString(e__)); \
   } while (0)
+
+struct Geometry {
+  uint32_t k, nt, key_len;
+  uint64_t key_bits, pair_sz, header, n, entries;
+};
+
+int bits_for(uint64_t span) {       // radix bits of values in [0, span)
+  int b = 1;
+  while ((1ull << b) < span) b++;
+  return b;
+}
+
+// ---- the two-sort core: records [0, n) of a slice whose bins start at bin_lo → sorted by (bin, key) ----------------
+const uint64_t CORE_REC = 44;        // device bytes per record besides its two copies: keys x2, index x2, bins x3
+// Planned bytes per record of a pass-C range besides its two copies: CORE_REC plus CUB's alternate key and value
+// arrays of the key sort (16 B) and its look-back state; the plan is checked against CUB's queried size.
+const uint64_t PASS_C_REC = CORE_REC + 20;
+const uint64_t RESERVE = 1ull << 18; // budget kept back from the pass-C plan for CUB's fixed-size state
+
+struct Core {
+  uint8_t *in = nullptr, *out = nullptr, *tmp = nullptr;
+  ull *keys = nullptr, *keys2 = nullptr, *idx = nullptr, *idx2 = nullptr;
+  uint32_t *bins = nullptr, *bins2 = nullptr, *bins3 = nullptr;
+  size_t tmp_bytes = 0;
+};
+
+// CUB's temporary bytes for the two sorts of n records with bins of bin_bits bits
+cudaError_t core_tmp(uint64_t n, int key_bits, int bin_bits, size_t *bytes) {
+  size_t a = 0, b = 0;
+  *bytes = 0;
+  if (!n) return cudaSuccess;
+  cudaError_t rc = cub::DeviceRadixSort::SortPairs((void *)nullptr, a, (ull *)nullptr, (ull *)nullptr, (ull *)nullptr,
+                                                   (ull *)nullptr, (int64_t)n, 0, key_bits);
+  if (rc == cudaSuccess)
+    rc = cub::DeviceRadixSort::SortPairs((void *)nullptr, b, (uint32_t *)nullptr, (uint32_t *)nullptr, (ull *)nullptr,
+                                         (ull *)nullptr, (int64_t)n, 0, bin_bits);
+  *bytes = a > b ? a : b;
+  return rc;
+}
+
+uint64_t core_bytes(uint64_t n, uint64_t pair_sz, size_t tmp) { return n * (2 * pair_sz + CORE_REC) + tmp + 10 * 16; }
+
+cudaError_t core_alloc(Buffers &buf, Core &c, uint64_t n, uint64_t pair_sz, size_t tmp) {
+  cudaError_t rc;
+  if ((rc = buf.get(&c.in, n * pair_sz)) || (rc = buf.get(&c.out, n * pair_sz)) || (rc = buf.get(&c.keys, n)) ||
+      (rc = buf.get(&c.keys2, n)) || (rc = buf.get(&c.idx, n)) || (rc = buf.get(&c.idx2, n)) || (rc = buf.get(&c.bins, n)) ||
+      (rc = buf.get(&c.bins2, n)) || (rc = buf.get(&c.bins3, n)) || (rc = buf.get(&c.tmp, tmp)))
+    return rc;
+  c.tmp_bytes = tmp;
+  return cudaSuccess;
+}
+
+// c.in[0, n) → c.out sorted by (bin, key), -z applied; the bins lie in [bin_lo, bin_lo + 2^bin_bits).  hist (optional)
+// receives the bin histogram at hist[bin + 1].
+cudaError_t core_sort(Core &c, uint64_t n, const Geometry &g, uint32_t bin_lo, int bin_bits, int zero_vals, ull *hist,
+                      cudaStream_t st) {
+  if (!n) return cudaSuccess;
+  const int grid = device_sm_count() * 8;
+  k_dbs_keys<<<grid, 256, 0, st>>>(c.in, n, g.key_len, g.k, g.nt, bin_lo, c.keys, c.bins, c.idx, hist);
+  // by key (pair_cmp, db_sort.cpp:118-128) ...
+  size_t need = c.tmp_bytes;
+  cudaError_t rc = cub::DeviceRadixSort::SortPairs(c.tmp, need, c.keys, c.keys2, c.idx, c.idx2, (int64_t)n, 0, (int)g.key_bits, st);
+  if (rc != cudaSuccess) return rc;
+  // ... then, stably, by bin (:96-107): the order inside a bin stays the key order
+  k_dbs_gather_bins<<<grid, 256, 0, st>>>(c.bins, c.idx2, n, c.bins2);
+  need = c.tmp_bytes;
+  rc = cub::DeviceRadixSort::SortPairs(c.tmp, need, c.bins2, c.bins3, c.idx2, c.idx, (int64_t)n, 0, bin_bits, st);
+  if (rc != cudaSuccess) return rc;
+  k_dbs_emit<<<grid, 256, 0, st>>>(c.in, c.idx, n, g.key_len, zero_vals, c.out);
+  return cudaGetLastError();
+}
+
+uint64_t largest_bin(const uint64_t *offsets, uint64_t entries) {
+  uint64_t m = 0;
+  for (uint64_t b = 0; b < entries; b++) m = std::max(m, offsets[b + 1] - offsets[b]);
+  return m;
+}
 
 }  // namespace
 
 // Host images in, host images out (kdb_out: header + key_ct * pair size bytes — what db_sort.cpp:70-72 writes;
-// idx_out: 8 + 8 * (4^nt + 1) bytes).  Returns 0 or -1 (+ err).
-int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint8_t *kdb_out, uint8_t *idx_out,
-                  char *err, size_t err_cap) {
-  if (!jdb || !kdb_out || !idx_out) return seterr(err, err_cap, "db_sort: NULL image");
-  if (jdb_bytes < 56 || memcmp(jdb, "JFLISTDN", 8) != 0) return seterr(err, err_cap, "db_sort: not a Jellyfish-style database (krakendb.cpp:67)");
-  if (nt < 1 || nt > 15) return seterr(err, err_cap, "db_sort: -n must be 1..15");
+// idx_out: 8 + 8 * (4^nt + 1) bytes).  budget = bytes of device memory (0 → KUQ_DB_SORT_BUDGET, else 3/4 of the free
+// memory).  Returns KUQ_OK, KUQ_E_CAPACITY (a bin or the histogram does not fit the budget) or KUQ_E_DB_FORMAT (+ err).
+int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget, uint8_t *kdb_out,
+                  uint8_t *idx_out, uint32_t *n_passes, char *err, size_t err_cap) {
+  if (!jdb || !kdb_out || !idx_out) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: NULL image");
+  if (jdb_bytes < 56 || memcmp(jdb, "JFLISTDN", 8) != 0)
+    return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: not a Jellyfish-style database (krakendb.cpp:67)");
+  if (nt < 1 || nt > 15) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: -n must be 1..15");
   uint64_t key_bits, val_len, key_ct;
   memcpy(&key_bits, jdb + 8, 8);
   memcpy(&val_len, jdb + 16, 8);
   memcpy(&key_ct, jdb + 48, 8);
-  if (val_len != 4) return seterr(err, err_cap, "db_sort: can only handle 4 byte DB values (krakendb.cpp:73-74)");
-  if (key_bits < 2 * nt || key_bits > 64) return seterr(err, err_cap, "db_sort: key_bits %llu out of range", (unsigned long long)key_bits);
-  const uint32_t k = (uint32_t)(key_bits / 2), key_len = (uint32_t)(key_bits / 8 + !!(key_bits % 8));
-  const uint64_t pair_sz = key_len + 4, header = 72 + 2 * (4 + 8 * key_bits);
-  if (jdb_bytes < header + key_ct * pair_sz) return seterr(err, err_cap, "db_sort: image shorter than its header says");
-  const uint64_t entries = 1ull << (2 * nt);
-  const uint64_t n = key_ct;
-
-  Buffers buf;
-  uint8_t *d_in = nullptr, *d_out = nullptr;
-  unsigned long long *d_keys = nullptr, *d_keys2 = nullptr, *d_idx = nullptr, *d_idx2 = nullptr, *d_off = nullptr;
-  uint32_t *d_bins = nullptr, *d_bins2 = nullptr, *d_bins3 = nullptr;
-  DB_CU(buf.get(&d_in, n * pair_sz));
-  DB_CU(buf.get(&d_out, n * pair_sz));
-  DB_CU(buf.get(&d_keys, n));
-  DB_CU(buf.get(&d_keys2, n));
-  DB_CU(buf.get(&d_idx, n));
-  DB_CU(buf.get(&d_idx2, n));
-  DB_CU(buf.get(&d_bins, n));
-  DB_CU(buf.get(&d_bins2, n));
-  DB_CU(buf.get(&d_bins3, n));
-  DB_CU(buf.get(&d_off, entries + 1));
-  cudaStream_t st = 0;
-  DB_CU(cudaMemcpyAsync(d_in, jdb + header, n * pair_sz, cudaMemcpyHostToDevice, st));
-  DB_CU(cudaMemsetAsync(d_off, 0, (entries + 1) * 8, st));
-  const int grid = device_sm_count() * 8;
-  if (n) k_dbs_keys<<<grid, 256, 0, st>>>(d_in, n, key_len, k, nt, d_keys, d_bins, d_idx, d_off);
-
-  // offsets = running sum of the bin sizes (make_index :136-139)
-  size_t tmp_bytes = 0, need = 0;
-  DB_CU(cub::DeviceScan::InclusiveSum((void *)nullptr, need, d_off, d_off, (int64_t)(entries + 1), st));
-  tmp_bytes = need;
-  if (n) {
-    DB_CU(cub::DeviceRadixSort::SortPairs((void *)nullptr, need, d_keys, d_keys2, d_idx, d_idx2, (int64_t)n, 0, (int)key_bits, st));
-    if (need > tmp_bytes) tmp_bytes = need;
-    DB_CU(cub::DeviceRadixSort::SortPairs((void *)nullptr, need, d_bins2, d_bins3, d_idx2, d_idx, (int64_t)n, 0, (int)(2 * nt), st));
-    if (need > tmp_bytes) tmp_bytes = need;
+  if (val_len != 4) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: can only handle 4 byte DB values (krakendb.cpp:73-74)");
+  if (key_bits < 2 * nt || key_bits > 64)
+    return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: key_bits %llu out of range", (unsigned long long)key_bits);
+  Geometry g;
+  g.k = (uint32_t)(key_bits / 2);
+  g.nt = nt;
+  g.key_len = (uint32_t)(key_bits / 8 + !!(key_bits % 8));
+  g.key_bits = key_bits;
+  g.pair_sz = g.key_len + 4;
+  g.header = 72 + 2 * (4 + 8 * key_bits);
+  g.n = key_ct;
+  g.entries = 1ull << (2 * nt);
+  if (jdb_bytes < g.header + key_ct * g.pair_sz) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: image shorter than its header says");
+  const uint64_t n = g.n, pair_sz = g.pair_sz, entries = g.entries;
+  if (!budget) {
+    size_t free_b = 0, total_b = 0;
+    DB_CU(cudaMemGetInfo(&free_b, &total_b));
+    const char *s = getenv("KUQ_DB_SORT_BUDGET");
+    budget = s && *s ? strtoull(s, nullptr, 10) : 0;
+    if (!budget) budget = free_b / 4 * 3;
   }
-  uint8_t *d_tmp = nullptr;
-  DB_CU(buf.get(&d_tmp, tmp_bytes));
-  need = tmp_bytes;
-  DB_CU(cub::DeviceScan::InclusiveSum(d_tmp, need, d_off, d_off, (int64_t)(entries + 1), st));
-  if (n) {
-    // by key (pair_cmp, db_sort.cpp:118-128) ...
-    need = tmp_bytes;
-    DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp, need, d_keys, d_keys2, d_idx, d_idx2, (int64_t)n, 0, (int)key_bits, st));
-    // ... then, stably, by bin (:96-107): the order inside a bin stays the key order
-    k_dbs_gather_bins<<<grid, 256, 0, st>>>(d_bins, d_idx2, n, d_bins2);
-    need = tmp_bytes;
-    DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp, need, d_bins2, d_bins3, d_idx2, d_idx, (int64_t)n, 0, (int)(2 * nt), st));
-    k_dbs_emit<<<grid, 256, 0, st>>>(d_in, d_idx, n, key_len, zero_vals, d_out);
-  }
-  DB_CU(cudaGetLastError());
-  memcpy(kdb_out, jdb, header);                                                // db_sort.cpp:56-58,71
-  DB_CU(cudaMemcpyAsync(kdb_out + header, d_out, n * pair_sz, cudaMemcpyDeviceToHost, st));
+  memcpy(kdb_out, jdb, g.header);                                              // db_sort.cpp:56-58,71
   memcpy(idx_out, "KRAKIX2", 7);                                               // krakendb.cpp:144-147
   idx_out[7] = (uint8_t)nt;
-  DB_CU(cudaMemcpyAsync(idx_out + 8, d_off, (entries + 1) * 8, cudaMemcpyDeviceToHost, st));
-  DB_CU(cudaStreamSynchronize(st));
-  return 0;
+  const uint8_t *body = jdb + g.header;
+  uint8_t *obody = kdb_out + g.header;
+  const uint64_t idx_dev = (entries + 1) * 8 + 16;
+  size_t tmp = 0, scan_tmp = 0;
+  DB_CU(core_tmp(n, (int)key_bits, 2 * nt, &tmp));
+  DB_CU(cub::DeviceScan::InclusiveSum((void *)nullptr, scan_tmp, (ull *)nullptr, (ull *)nullptr, (int64_t)(entries + 1)));
+  PinnedBounce bounce;
+  DB_CU(bounce.init());
+  cudaStream_t st = 0;
+  const int grid = device_sm_count() * 8;
+  *n_passes = 1;
+
+  // ---- in one piece: the whole input and the index on the device ----
+  if (core_bytes(n, pair_sz, std::max(tmp, scan_tmp)) + idx_dev <= budget) {
+    Buffers buf;
+    Core c;
+    ull *d_off = nullptr;
+    DB_CU(core_alloc(buf, c, n, pair_sz, std::max(tmp, scan_tmp)));
+    DB_CU(buf.get(&d_off, entries + 1));
+    DB_CU(bounce.to_device(c.in, body, n * pair_sz, st));
+    DB_CU(cudaMemsetAsync(d_off, 0, (entries + 1) * 8, st));
+    DB_CU(core_sort(c, n, g, 0, 2 * nt, zero_vals, d_off, st));
+    // offsets = running sum of the bin sizes (make_index :136-139)
+    size_t need = c.tmp_bytes;
+    DB_CU(cub::DeviceScan::InclusiveSum(c.tmp, need, d_off, d_off, (int64_t)(entries + 1), st));
+    DB_CU(bounce.to_host(obody, c.out, n * pair_sz, st));
+    DB_CU(bounce.to_host(idx_out + 8, d_off, (entries + 1) * 8, st));
+    return KUQ_OK;
+  }
+
+  // ---- pass A: the bin histogram, streamed; its running sum is the index ----
+  {
+    uint64_t chunk = std::max<uint64_t>(1, std::min(n, PinnedBounce::CH / pair_sz));
+    while (chunk > 1 && idx_dev + scan_tmp + chunk * pair_sz + 32 > budget) chunk /= 2;
+    if (idx_dev + scan_tmp + chunk * pair_sz + 32 > budget)
+      return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: the bin histogram of -n %u (%llu bytes) does not fit KUQ_DB_SORT_BUDGET = %llu bytes",
+                    nt, (unsigned long long)idx_dev, (unsigned long long)budget);
+    Buffers buf;
+    uint8_t *d_chunk = nullptr, *d_tmp = nullptr;
+    ull *d_off = nullptr;
+    DB_CU(buf.get(&d_chunk, chunk * pair_sz));
+    DB_CU(buf.get(&d_off, entries + 1));
+    DB_CU(buf.get(&d_tmp, scan_tmp));
+    DB_CU(cudaMemsetAsync(d_off, 0, (entries + 1) * 8, st));
+    for (uint64_t s = 0; s < n; s += chunk) {
+      const uint64_t m = std::min(chunk, n - s);
+      DB_CU(bounce.h2d(d_chunk, body + s * pair_sz, m * pair_sz, st));   // the host copy of the next overlaps this kernel
+      k_dbs_hist<<<grid, 256, 0, st>>>(d_chunk, m, g.key_len, g.k, nt, d_off);
+      DB_CU(cudaGetLastError());
+    }
+    size_t need = scan_tmp;
+    DB_CU(cub::DeviceScan::InclusiveSum(d_tmp, need, d_off, d_off, (int64_t)(entries + 1), st));
+    DB_CU(bounce.to_host(idx_out + 8, d_off, (entries + 1) * 8, st));
+  }
+  const uint64_t *offsets = reinterpret_cast<const uint64_t *>(idx_out + 8);
+
+  // ---- the ranges of pass C: planned from the index, checked against CUB's queried temporary size ----
+  std::vector<std::pair<uint64_t, uint64_t>> ranges;
+  uint64_t max_rec = 0;
+  size_t ctmp = 0;
+  {
+    uint64_t plan_budget = budget > RESERVE ? budget - RESERVE : 0;
+    for (int attempt = 0;; attempt++) {
+      if (!plan_ranges(offsets, entries, plan_budget, 2 * pair_sz + PASS_C_REC, ranges))
+        return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: a minimizer bin of %llu records does not fit KUQ_DB_SORT_BUDGET = %llu bytes",
+                      (unsigned long long)largest_bin(offsets, entries), (unsigned long long)budget);
+      int max_bits = 1;
+      max_rec = 0;
+      for (auto &r : ranges) {
+        max_rec = std::max(max_rec, offsets[r.second] - offsets[r.first]);
+        max_bits = std::max(max_bits, bits_for(r.second - r.first));
+      }
+      DB_CU(core_tmp(max_rec, (int)key_bits, max_bits, &ctmp));
+      const uint64_t need = core_bytes(max_rec, pair_sz, ctmp);
+      if (need <= budget) break;
+      if (attempt == 8 || need - budget >= plan_budget)
+        return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: a range of %llu records needs %llu bytes, more than KUQ_DB_SORT_BUDGET = %llu",
+                      (unsigned long long)max_rec, (unsigned long long)need, (unsigned long long)budget);
+      plan_budget -= need - budget;
+    }
+  }
+  const uint32_t R = (uint32_t)ranges.size();
+
+  // ---- pass B: group every chunk by range, stably; each range's slice goes to that range's cursor ----
+  if (n) {
+    const int rbits = bits_for(R);
+    auto stream_need = [&](uint64_t c, size_t *sort_tmp) -> cudaError_t {
+      *sort_tmp = 0;
+      return cub::DeviceRadixSort::SortPairs((void *)nullptr, *sort_tmp, (uint32_t *)nullptr, (uint32_t *)nullptr, (ull *)nullptr,
+                                             (ull *)nullptr, (int64_t)c, 0, rbits);
+    };
+    auto fits = [&](uint64_t c, size_t t) { return c * (2 * pair_sz + 24) + t + (uint64_t)R * 12 + 8 * 16 <= budget; };
+    uint64_t chunk = std::min(n, PinnedBounce::CH / pair_sz);
+    size_t stmp = 0;
+    DB_CU(stream_need(chunk, &stmp));
+    while (chunk > 1 && !fits(chunk, stmp)) { chunk /= 2; DB_CU(stream_need(chunk, &stmp)); }
+    if (!fits(chunk, stmp))
+      return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: %u ranges do not fit KUQ_DB_SORT_BUDGET = %llu bytes", R,
+                    (unsigned long long)budget);
+    Buffers buf;
+    uint8_t *d_chunk = nullptr, *d_grp = nullptr, *d_tmp = nullptr;
+    uint32_t *d_rid = nullptr, *d_rid2 = nullptr, *d_starts = nullptr;
+    ull *d_idx = nullptr, *d_idx2 = nullptr, *d_cnt = nullptr;
+    DB_CU(buf.get(&d_chunk, chunk * pair_sz));
+    DB_CU(buf.get(&d_grp, chunk * pair_sz));
+    DB_CU(buf.get(&d_rid, chunk));
+    DB_CU(buf.get(&d_rid2, chunk));
+    DB_CU(buf.get(&d_idx, chunk));
+    DB_CU(buf.get(&d_idx2, chunk));
+    DB_CU(buf.get(&d_starts, R));
+    DB_CU(buf.get(&d_cnt, R));
+    DB_CU(buf.get(&d_tmp, stmp));
+    std::vector<uint32_t> starts(R);
+    std::vector<uint64_t> cursor(R), cnt(R), pos(R);
+    for (uint32_t r = 0; r < R; r++) { starts[r] = (uint32_t)ranges[r].first; cursor[r] = offsets[ranges[r].first]; }
+    DB_CU(cudaMemcpy(d_starts, starts.data(), R * 4ull, cudaMemcpyHostToDevice));
+    DB_CU(bounce.h2d(d_chunk, body, std::min(chunk, n) * pair_sz, st));
+    for (uint64_t s = 0; s < n; s += chunk) {
+      const uint64_t m = std::min(chunk, n - s);
+      DB_CU(cudaMemsetAsync(d_cnt, 0, R * 8ull, st));
+      k_dbs_range_of<<<grid, 256, 0, st>>>(d_chunk, m, g.key_len, g.k, nt, d_starts, R, d_rid, d_idx, d_cnt);
+      size_t need = stmp;
+      DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp, need, d_rid, d_rid2, d_idx, d_idx2, (int64_t)m, 0, rbits, st));
+      k_dbs_emit<<<grid, 256, 0, st>>>(d_chunk, d_idx2, m, g.key_len, 0, d_grp);
+      DB_CU(cudaGetLastError());
+      if (s + m < n)                                                 // the host copy of the next chunk overlaps these kernels
+        DB_CU(bounce.h2d(d_chunk, body + (s + m) * pair_sz, std::min(chunk, n - s - m) * pair_sz, st));
+      DB_CU(cudaMemcpyAsync(cnt.data(), d_cnt, R * 8ull, cudaMemcpyDeviceToHost, st));
+      const uint8_t *grp = nullptr;
+      DB_CU(bounce.d2h(&grp, d_grp, m * pair_sz, st));
+      uint64_t at = 0;
+      for (uint32_t r = 0; r < R; r++) { pos[r] = at; at += cnt[r]; }
+      std::vector<std::thread> th;
+      const uint32_t per = (R + PinnedBounce::NT - 1) / PinnedBounce::NT;
+      for (uint32_t a = 0; a < R; a += per)
+        th.emplace_back([&, a] {
+          for (uint32_t r = a; r < std::min(R, a + per); r++)
+            if (cnt[r]) memcpy(obody + cursor[r] * pair_sz, grp + pos[r] * pair_sz, cnt[r] * pair_sz);
+        });
+      for (auto &x : th) x.join();
+      for (uint32_t r = 0; r < R; r++) cursor[r] += cnt[r];
+    }
+  }
+
+  // ---- pass C: sort each range in place ----
+  {
+    Buffers buf;
+    Core c;
+    DB_CU(core_alloc(buf, c, max_rec, pair_sz, ctmp));
+    for (auto &r : ranges) {
+      const uint64_t a = offsets[r.first], m = offsets[r.second] - a;
+      DB_CU(bounce.to_device(c.in, obody + a * pair_sz, m * pair_sz, st));
+      DB_CU(core_sort(c, m, g, (uint32_t)r.first, bits_for(r.second - r.first), zero_vals, nullptr, st));
+      DB_CU(bounce.to_host(obody + a * pair_sz, c.out, m * pair_sz, st));
+    }
+  }
+  *n_passes = R ? R : 1;
+  return KUQ_OK;
 }
 
 }  // namespace kuq

@@ -267,9 +267,9 @@ int device_sm_count();
 int launch_set_lcas(const Params &p, int n_sm, cudaStream_t stream);
 int launch_scan_only(const Params &p, int n_sm, cudaStream_t stream);
 int launch_lookup_only(const Params &p, int n_sm, cudaStream_t stream, int fused, int lean);
-// db_sort on the device (kuq_dbbuild.cu)
-int dbsort_device(const uint8_t *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint8_t *kdb_out,
-                  uint8_t *idx_out, char *err, size_t err_cap);
+// db_sort on the device (kuq_dbbuild.cu): returns a KUQ_* code, *n_passes = per-range sorts (1 = in one piece)
+int dbsort_device(const uint8_t *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
+                  uint8_t *kdb_out, uint8_t *idx_out, uint32_t *n_passes, char *err, size_t err_cap);
 
 // database staging helpers
 void launch_collect_taxids(const uint8_t *pairs, uint64_t n_rec, uint32_t *keys, unsigned long long *counts,
