@@ -400,6 +400,14 @@ uint64_t kuq_ertl_dense(const uint8_t *regs4096, uint64_t n_observed);
 int kuq_random_gather_peak(int device, uint64_t buffer_bytes, uint64_t n_sectors_to_read, uint32_t bytes_per_access,
                            double *gsectors_per_s, double *gbytes_per_s, double *kernel_ms);
 
+/* ---- test aid: the record-tier harvest on caller-owned device buffers ------------------------------------------ */
+/* The harvest kuq_finish runs on a resident range, on device memory the caller owns: n_rec 12-byte records at d_pairs
+ * (4-byte aligned), n_secondaries (secondary, primary) record index pairs (2 x u32 each), d_dense_flag[n_sketch]; record taxa < n_sketch.
+ * Flagged secondaries hand their flag to their primaries; then every flagged record that is neither kept nor of a dense
+ * taxon becomes kept and adds 1 to d_distinct[taxon] and to *d_n_kept; every flag is cleared.  Synchronous. */
+int kuq_harvest_keep_device(int device, void *d_pairs, uint64_t n_rec, const void *d_secondaries, uint64_t n_secondaries,
+                            const uint8_t *d_dense_flag, uint32_t n_sketch, uint32_t *d_distinct, uint64_t *d_n_kept);
+
 /* Record-layout / search-shape experiment for the bin search (kmer_query, krakendb.cpp:250-321) — measurement aid.
  * Transcodes the staged 12-byte records once into 8-byte minimizer-relative records (the 16 bases outside the bin's
  * minimizer + minimizer position / orientation + 24-bit dense taxon; k = 31, m = 15 only) and times a lookup-only

@@ -180,6 +180,7 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_layout_experiment": (C.c_int, [vp, C.c_uint32, C.c_uint64, C.c_uint32, C.POINTER(LayoutResult)]),
         "kuq_random_gather_peak": (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_uint32, C.POINTER(C.c_double),
                                             C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+        "kuq_harvest_keep_device": (C.c_int, [C.c_int, vp, C.c_uint64, vp, C.c_uint64, vp, C.c_uint32, vp, vp]),
         "kuq_kmer_set_create": (C.c_int, [C.c_int, C.c_uint32, C.c_uint64, C.POINTER(vp), C.c_char_p, C.c_uint64]),
         "kuq_kmer_set_add": (C.c_int, [vp, vp, u64p, C.c_uint32]),
         "kuq_kmer_set_next": (C.c_int, [vp, vp, C.c_uint64, u64p]),
@@ -604,6 +605,14 @@ def random_gather_peak(device=0, buffer_bytes=16 << 30, n_sectors=1 << 30, bytes
     if rc != 0:
         raise KuqError(rc, L.kuq_strerror(rc).decode())
     return gs.value, gb.value, ms.value
+
+
+def harvest_keep_device(d_pairs, n_rec, d_secondaries, n_secondaries, d_dense_flag, n_sketch, d_distinct, d_n_kept, device=0):
+    """kuq_harvest_keep_device: the record-tier harvest of kuq_finish on caller-owned device buffers (pointers)"""
+    L = load_library()
+    rc = L.kuq_harvest_keep_device(device, d_pairs, n_rec, d_secondaries, n_secondaries, d_dense_flag, n_sketch, d_distinct, d_n_kept)
+    if rc != 0:
+        raise KuqError(rc, L.kuq_strerror(rc).decode())
 
 
 def decode_runs(res, i):

@@ -162,6 +162,10 @@ struct kuq_ctx {
   bool set_has_hits = false;              // the set holds keys of hits, which kept records could duplicate
   uint64_t sparse_grown = 0;              // times the sparse-tier set was re-allocated at a harvest
   double harvest_ms = 0;                  // device time of the last harvest
+  // the harvest's counters and timing events, made at the first harvest and kept: a cudaMalloc / cudaFree pair per
+  // harvest held the device idle at the end of every run
+  unsigned long long *d_harvest_stat = nullptr;
+  cudaEvent_t harvest_ev[2] = {nullptr, nullptr};
   bool lca_mode = false;                  // kuq_set_lcas_batch ran: record values are LCA results, not classifiable
   // work-unit cutting across batches (classify.cpp:506-521)
   uint64_t unit_nt = 0;
@@ -633,11 +637,13 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   SparseSet ss;
   ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0; ss.n_used = ctx->d_sparse_used;
   ss.distinct = ctx->d_sparse_distinct;
-  unsigned long long *d_stat;
-  CU(dmalloc(&d_stat, 2));
+  if (!ctx->d_harvest_stat) {
+    CU(dmalloc(&ctx->d_harvest_stat, 2));
+    CU(cudaEventCreate(&ctx->harvest_ev[0])); CU(cudaEventCreate(&ctx->harvest_ev[1]));
+  }
+  unsigned long long *d_stat = ctx->d_harvest_stat;
+  cudaEvent_t e0 = ctx->harvest_ev[0], e1 = ctx->harvest_ev[1];
   CU(cudaMemsetAsync(d_stat, 0, 16, ctx->aux));
-  cudaEvent_t e0, e1;
-  CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
   CU(cudaEventRecord(e0, ctx->aux));
   if (discard || !ctx->d_sparse_slots) {
     launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 2, ctx->aux);
@@ -645,8 +651,8 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
     ctx->kept = false;
     ctx->kept_keys = 0;
   } else if (keep) {
-    launch_harvest_keep(ctx->d_pairs, ctx->key_ct, ctx->d_secondaries, ctx->n_secondaries, ctx->d_dense_flag, ctx->d_sparse_distinct,
-                        d_stat, ctx->aux);
+    launch_harvest_keep(ctx->d_pairs, ctx->key_ct, ctx->d_secondaries, ctx->n_secondaries, ctx->d_dense_flag, ctx->n_sketch,
+                        ctx->d_sparse_distinct, d_stat, ctx->aux);
     ctx->launches += ctx->n_secondaries ? 2 : 1;
     ctx->kept = true;
   } else {
@@ -663,7 +669,7 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
       uint64_t cap = ctx->sparse_cap;
       while ((used + n_new) * 10 > cap * 6) cap <<= 1;
       int grc = grow_sparse_set(ctx, cap);
-      if (grc) { cudaFree(d_stat); return grc; }
+      if (grc) return grc;
       ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1;
     }
     ctx->direct_upper = used + n_new;
@@ -683,8 +689,6 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1);
   ctx->harvest_ms = ms;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  cudaFree(d_stat);
   ctx->snap_valid = false;
   if (keep) {
     ctx->kept_keys += st[0];
@@ -985,6 +989,8 @@ void kuq_destroy(kuq_ctx *ctx) {
   free_db(ctx);
   free_tax_state(ctx);
   cudaFree(ctx->d_sync_err);
+  cudaFree(ctx->d_harvest_stat);
+  for (cudaEvent_t e : ctx->harvest_ev) if (e) cudaEventDestroy(e);
   if (ctx->aux) cudaStreamDestroy(ctx->aux);
   delete ctx;
 }
@@ -2699,6 +2705,18 @@ uint64_t kuq_ertl_dense(const uint8_t *regs, uint64_t n_observed) {
   memset(C, 0, sizeof C);
   for (uint32_t i = 0; i < HLL_M; i++) C[regs[i] > 65 ? 65 : regs[i]]++;
   return ertl_from_hist(C, 64 - HLL_P, HLL_M, n_observed);
+}
+
+int kuq_harvest_keep_device(int device, void *d_pairs, uint64_t n_rec, const void *d_secondaries, uint64_t n_secondaries,
+                            const uint8_t *d_dense_flag, uint32_t n_sketch, uint32_t *d_distinct, uint64_t *d_n_kept) {
+  if ((reinterpret_cast<uintptr_t>(d_pairs) & 3) || (n_rec && (!d_pairs || !d_dense_flag || !d_distinct || !d_n_kept)) ||
+      (n_secondaries && !d_secondaries))
+    return KUQ_E_INVALID_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) { (void)cudaGetLastError(); return KUQ_E_NO_DEVICE; }
+  launch_harvest_keep(static_cast<uint8_t *>(d_pairs), n_rec, static_cast<const uint2 *>(d_secondaries), n_secondaries, d_dense_flag,
+                      n_sketch, d_distinct, reinterpret_cast<unsigned long long *>(d_n_kept), 0);
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaGetLastError() != cudaSuccess) return KUQ_E_CUDA;
+  return KUQ_OK;
 }
 
 // ---- database build (SURVEY.md §8 f4; ROUND 1: compiled, not yet run on hardware) ---------------------------------

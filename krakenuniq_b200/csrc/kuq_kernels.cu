@@ -1689,21 +1689,31 @@ __global__ void k_fold_secondaries(uint8_t *pairs, const uint2 *list, uint64_t n
   }
 }
 
+// k_harvest_keep streams the records in groups of 4 (48 bytes = three 16-byte loads, KEEP_UNROLL groups in flight per
+// thread).  The records are 4-byte aligned only: the groups start at the first 16-byte aligned record, and the up to 3
+// records before it and after the last whole group are handled one by one.  A group without a flagged record is not
+// written; otherwise only the high words whose flags change are stored, so sectors without a flagged record stay clean.
+// Per-taxon counts: with at most KEEP_DIRECT_TAXA taxa, each CTA holds one shared counter per taxon, indexed by the
+// taxon (a dense taxon's counter holds KEEP_DENSE, so one shared load answers "dense?" too).  A hashed table of
+// KEEP_SLOTS taxa would overflow into same-address global atomics once the records span more taxa than it holds (the
+// bench's 2000 genomes do); that table remains for larger taxonomies.
 constexpr int KEEP_SLOTS = 1024;
-__global__ void __launch_bounds__(256) k_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint8_t *dense_flag, uint32_t *distinct,
-                                                      unsigned long long *n_kept) {
-  __shared__ uint32_t s_tax[KEEP_SLOTS], s_cnt[KEEP_SLOTS];
-  for (int s = threadIdx.x; s < KEEP_SLOTS; s += blockDim.x) { s_tax[s] = 0; s_cnt[s] = 0; }
-  __syncthreads();
-  unsigned long long n_local = 0;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_rec; i += (uint64_t)gridDim.x * blockDim.x) {
-    uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
-    const uint32_t hiw = w[1];
-    if (!(hiw & SEEN_BIT)) continue;
-    const uint32_t taxon = w[2];
-    if ((hiw & KEPT_BIT) || dense_flag[taxon]) { w[1] = hiw & ~SEEN_BIT; continue; }
-    w[1] = (hiw & ~SEEN_BIT) | KEPT_BIT;
-    n_local++;
+constexpr int KEEP_UNROLL = 2;
+constexpr int KEEP_THREADS = 256;
+constexpr uint32_t KEEP_DIRECT_TAXA = 16384;     // 64 KiB of counters per CTA
+constexpr uint32_t KEEP_DENSE = 0xFFFFFFFFu;
+
+// one flagged record's high word: SEEN cleared; neither KEPT nor of a dense taxon → KEPT, counted
+template <bool DIRECT>
+__device__ __forceinline__ uint32_t keep_record(uint32_t *s_tab, const uint8_t *dense_flag, uint32_t *distinct, uint32_t hiw,
+                                                uint32_t taxon, unsigned long long &n_local) {
+  if (hiw & KEPT_BIT) return hiw & ~SEEN_BIT;
+  if (DIRECT) {
+    if (s_tab[taxon] == KEEP_DENSE) return hiw & ~SEEN_BIT;
+    atomicAdd(&s_tab[taxon], 1u);
+  } else {
+    if (dense_flag[taxon]) return hiw & ~SEEN_BIT;
+    uint32_t *s_tax = s_tab, *s_cnt = s_tab + KEEP_SLOTS;
     uint32_t h = (taxon * 0x9E3779B1u) >> 22, probe = 0;
     for (; probe < 8; probe++, h = (h + 1) & (KEEP_SLOTS - 1)) {
       uint32_t cur = s_tax[h];
@@ -1712,19 +1722,84 @@ __global__ void __launch_bounds__(256) k_harvest_keep(uint8_t *pairs, uint64_t n
     }
     if (probe == 8) atomicAdd(distinct + taxon, 1u);
   }
+  n_local++;
+  return (hiw & ~SEEN_BIT) | KEPT_BIT;
+}
+
+template <bool DIRECT>
+__global__ void __launch_bounds__(KEEP_THREADS) k_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint8_t *dense_flag,
+                                                                uint32_t n_sketch, uint32_t *distinct, unsigned long long *n_kept) {
+  extern __shared__ uint32_t s_tab[];             // DIRECT: [n_sketch] counters; else [KEEP_SLOTS] taxa + [KEEP_SLOTS] counts
+  if (DIRECT) {
+    for (uint32_t s = threadIdx.x; s < n_sketch; s += blockDim.x) s_tab[s] = dense_flag[s] ? KEEP_DENSE : 0u;
+  } else {
+    for (int s = threadIdx.x; s < 2 * KEEP_SLOTS; s += blockDim.x) s_tab[s] = 0;
+  }
   __syncthreads();
-  for (int s = threadIdx.x; s < KEEP_SLOTS; s += blockDim.x)
-    if (s_tax[s]) atomicAdd(distinct + s_tax[s] - 1, s_cnt[s]);
+  unsigned long long n_local = 0;
+  // records before the first 16-byte boundary: 12 * head + (pairs mod 16) == 0 (mod 16), pairs 4-byte aligned
+  const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(pairs) & 15u);
+  const uint64_t head = min((uint64_t)(mis / 4u), n_rec);
+  const uint64_t n_groups = (n_rec - head) / 4, tail = head + 4 * n_groups;
+  const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (tid < head + (n_rec - tail)) {                     // the edges, one record per thread
+    const uint64_t i = tid < head ? tid : tail + (tid - head);
+    uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
+    const uint32_t hiw = w[1];
+    if (hiw & SEEN_BIT) w[1] = keep_record<DIRECT>(s_tab, dense_flag, distinct, hiw, w[2], n_local);
+  }
+  uint4 *groups = reinterpret_cast<uint4 *>(pairs + head * 12);
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x * KEEP_UNROLL;
+  for (uint64_t g0 = (uint64_t)blockIdx.x * blockDim.x * KEEP_UNROLL + threadIdx.x; g0 < n_groups; g0 += stride) {
+    uint4 v[KEEP_UNROLL][3];
+#pragma unroll
+    for (int u = 0; u < KEEP_UNROLL; u++) {
+      const uint64_t g = g0 + (uint64_t)u * blockDim.x;
+      if (g < n_groups) {
+        v[u][0] = groups[g * 3]; v[u][1] = groups[g * 3 + 1]; v[u][2] = groups[g * 3 + 2];
+      } else {
+        v[u][0] = v[u][1] = v[u][2] = make_uint4(0, 0, 0, 0);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < KEEP_UNROLL; u++) {
+      // record r of the group: words 3r, 3r + 1 (high key word, flags), 3r + 2 (taxon)
+      const uint32_t hi[4] = {v[u][0].y, v[u][1].x, v[u][1].w, v[u][2].z};
+      const uint32_t tx[4] = {v[u][0].z, v[u][1].y, v[u][2].x, v[u][2].w};
+      if (!((hi[0] | hi[1] | hi[2] | hi[3]) & SEEN_BIT)) continue;
+      uint32_t *w = reinterpret_cast<uint32_t *>(groups + (g0 + (uint64_t)u * blockDim.x) * 3);
+#pragma unroll
+      for (int r = 0; r < 4; r++)
+        if (hi[r] & SEEN_BIT) w[3 * r + 1] = keep_record<DIRECT>(s_tab, dense_flag, distinct, hi[r], tx[r], n_local);
+    }
+  }
+  __syncthreads();
+  if (DIRECT) {
+    for (uint32_t s = threadIdx.x; s < n_sketch; s += blockDim.x)
+      if (s_tab[s] && s_tab[s] != KEEP_DENSE) atomicAdd(distinct + s, s_tab[s]);
+  } else {
+    for (int s = threadIdx.x; s < KEEP_SLOTS; s += blockDim.x)
+      if (s_tab[s]) atomicAdd(distinct + s_tab[s] - 1, s_tab[KEEP_SLOTS + s]);
+  }
   for (int o = 16; o; o >>= 1) n_local += __shfl_xor_sync(0xFFFFFFFFu, n_local, o);
   if ((threadIdx.x & 31) == 0 && n_local) atomicAdd(n_kept, n_local);
 }
 void launch_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint2 *secondaries, uint64_t n_secondaries, const uint8_t *dense_flag,
-                         uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream) {
+                         uint32_t n_sketch, uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream) {
   if (!n_rec) return;
+  const int n_sm = device_sm_count();
   if (n_secondaries)
-    k_fold_secondaries<<<(int)min((uint64_t)device_sm_count() * 8, (n_secondaries + 255) / 256), 256, 0, stream>>>(pairs, secondaries, n_secondaries);
-  const int grid = (int)min((uint64_t)device_sm_count() * 8, (n_rec + 255) / 256);
-  k_harvest_keep<<<grid, 256, 0, stream>>>(pairs, n_rec, dense_flag, distinct, n_kept);
+    k_fold_secondaries<<<(int)min((uint64_t)n_sm * 8, (n_secondaries + 255) / 256), 256, 0, stream>>>(pairs, secondaries, n_secondaries);
+  const bool direct = n_sketch <= KEEP_DIRECT_TAXA;
+  const auto kernel = direct ? k_harvest_keep<true> : k_harvest_keep<false>;
+  const size_t smem = direct ? 4ull * n_sketch : 8ull * KEEP_SLOTS;
+  // per device (function attributes belong to the current context); the harvest runs once per run
+  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * KEEP_DIRECT_TAXA);
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, KEEP_THREADS, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  const uint64_t per_cta = (uint64_t)KEEP_THREADS * KEEP_UNROLL * 4;     // records per CTA per iteration
+  const int grid = (int)min((uint64_t)n_sm * per_sm, (n_rec + per_cta - 1) / per_cta);     // >= 1: n_rec > 0
+  kernel<<<grid, KEEP_THREADS, smem, stream>>>(pairs, n_rec, dense_flag, n_sketch, distinct, n_kept);
 }
 
 // re-insert the keys of an outgrown table into its successor (no per-taxon counting: the keys were counted before)

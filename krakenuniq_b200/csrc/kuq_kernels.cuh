@@ -283,9 +283,10 @@ void launch_widen_records(const uint8_t *narrow, uint64_t n_rec, uint32_t key_le
 void launch_harvest_seen(uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint8_t *dense_flag, const SparseSet &set,
                          unsigned long long *stats, uint32_t *error_flag, int mode, cudaStream_t stream);
 // flagged records → kept records (no set): secondaries hand their flag to their primaries, then one pass over the
-// records sets KEPT_BIT, counts distinct[taxon] and clears SEEN_BIT (*n_kept += records that became kept)
+// records sets KEPT_BIT, counts distinct[taxon] and clears SEEN_BIT (*n_kept += records that became kept).  pairs:
+// 4-byte aligned; dense_flag has n_sketch entries, and every record's taxon is below n_sketch.
 void launch_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint2 *secondaries, uint64_t n_secondaries, const uint8_t *dense_flag,
-                         uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream);
+                         uint32_t n_sketch, uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream);
 // kuq_collisions.cu: (secondary, primary) record pairs of every (taxon, code) group of the staged records
 int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint64_t *records_of_taxon, uint32_t n_sketch,
                      uint64_t max_entries, uint2 **list_out, uint64_t *n_out, int n_sm, cudaStream_t stream);
