@@ -154,6 +154,19 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
  * 12-byte records, so this call takes k = 29..31; stage other databases with kuq_stage_db. */
 int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uint64_t *d_offsets, uint32_t k,
                          uint32_t nt, uint32_t idx_type, uint64_t bin_lo, uint64_t bin_hi);
+/* Several databases resident at once (`classify -d a -d b`, classify.cpp:928-936): stage one more WHOLE database behind
+ * those already staged (with none staged, the call is kuq_stage_db of the whole database).  Staging order is the order
+ * in which the databases are asked: every k-mer takes the value of the first one that holds the key, a stored taxon 0
+ * included.  Records are widened and remapped like kuq_stage_db's; the databases share k (else KUQ_E_INVALID_ARG) and may
+ * differ in minimizer length and index type.  kuq_stage_db drops every appended database again.
+ * On a context with several databases kuq_submit_batch / kuq_classify_batch / kuq_classify_device run, on the slot's
+ * stream and into its own buffers: k_scan, the in-order lookup (one launch per run of consecutive databases with the same
+ * (nt, index type), up to 8 databases per launch; later runs fill only windows no earlier run answered), then the
+ * resolve half.  Results take the same form as on one database; the sparse HLL tier is filled by the resolve half (no
+ * record flags).  kuq_lookup_batch / kuq_lookup_device return the merged first-hit codes, a stored zero always as
+ * KUQ_CODE_FOUND_ZERO.  kuq_db_taxids reports the union over the staged databases (record counts summed).  Shard
+ * counting and kuq_lookup_device_peers are refused (KUQ_E_STATE). */
+int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes);
 /* Distinct taxids stored in the staged records with their record counts — what KrakenDB::count_taxons()
  * (krakendb.cpp:90-113) computes for database.kdb.counts.  Pass cap = 0 to query *n only. */
 int kuq_db_taxids(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n);
@@ -214,7 +227,11 @@ int kuq_classify_device(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const 
 /* Stage 1 only (classify_sequence_with_db_chunk): per-window DENSE taxon ids of the staged DB range into
  * d_codes_out (indexed like the bases; 0 where the range has no hit; KUQ_CODE_AMBIG for ambiguous windows).
  * d_codes_out may be peer memory of another GPU (NVLink P2P stores) when only_hits != 0: then only hits are
- * written, so several ranges can be merged into one zero-initialised buffer without a reduction. */
+ * written, so several ranges can be merged into one zero-initialised buffer without a reduction.
+ * only_hits = KUQ_LOOKUP_FILL_EMPTY: write hits only, and skip windows whose code in d_codes_out is non-zero already
+ * (answered by an earlier database) before any index fetch — the databases after the first of a streamed run of
+ * several databases; a stored zero is written as KUQ_CODE_FOUND_ZERO. */
+#define KUQ_LOOKUP_FILL_EMPTY 2u
 int kuq_lookup_device(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets,
                       uint32_t n_reads, uint64_t total_bases, uint32_t *d_codes_out, uint32_t only_hits);
 /* Stage 2 only: calls, hit lists and counters from merged per-window dense ids (the final pass of the chunked
@@ -364,7 +381,8 @@ int kuq_scan_device(kuq_ctx *ctx, uint32_t slot, uint32_t k, uint32_t nt, uint32
  * work queued on the slots so far (the users of the buffer it overwrites), never for the host.  Record values are
  * rewritten to dense ids on arrival; kuq_stream_check reports a taxid outside the declared universe.  The buffers hold
  * max_records records of 12 bytes; records shorter than that (k <= 28) are widened on arrival, in pieces that pass
- * through one landing zone of 64 MiB (KUQ_LANDING_BYTES) on the copy stream. */
+ * through one landing zone of 64 MiB (KUQ_LANDING_BYTES) on the copy stream.  kuq_stream_open may be called again once
+ * the slots are idle (it waits for them): the next database of a streamed run may have another nt or index type. */
 int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, uint64_t max_records, uint64_t max_bins);
 int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64_t n_records, const uint64_t *host_offsets,
                     uint64_t bin_lo, uint64_t bin_hi);

@@ -16,6 +16,8 @@ import numpy as np
 from . import build as _build
 
 AMBIG = 0xFFFFFFFF
+CODE_FOUND_ZERO = 0xFFFFFFFD      # KUQ_CODE_FOUND_ZERO: the first database holding the k-mer stores taxon 0
+LOOKUP_FILL_EMPTY = 2             # KUQ_LOOKUP_FILL_EMPTY (lookup_device only_hits)
 HLL_PRELOAD, HLL_CHUNKED, HLL_DENSE_ONLY, HLL_EXACT = 0, 1, 2, 3
 F_WANT_CODES, F_NO_RUNS, F_NO_COUNTS, F_STATS = 1, 2, 4, 8
 
@@ -102,6 +104,7 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_version": (C.c_char_p, []),
         "kuq_device_count": (C.c_int, []),
         "kuq_stage_db": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint64, C.c_uint64]),
+        "kuq_stage_db_append": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint64]),
         "kuq_attach_db_device": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64,
                                            C.c_uint64]),
         "kuq_db_taxids": (C.c_int, [vp, u32p, u64p, C.c_uint32, u32p]),
@@ -248,6 +251,13 @@ class Classifier:
         idx = np.ascontiguousarray(idx).view(np.uint8) if not isinstance(idx, np.memmap) else idx
         self._ck(self.L.kuq_stage_db(self.h, kdb.ctypes.data, kdb.size, idx.ctypes.data, idx.size, bin_lo, bin_hi))
 
+    def stage_db_append(self, kdb: np.ndarray, idx: np.ndarray):
+        """one more whole database, asked after those staged already (classify -d a -d b; kuq_stage_db_append).
+        Same k; nt and index type may differ.  stage_db drops the appended databases again."""
+        kdb = np.ascontiguousarray(kdb).view(np.uint8) if not isinstance(kdb, np.memmap) else kdb
+        idx = np.ascontiguousarray(idx).view(np.uint8) if not isinstance(idx, np.memmap) else idx
+        self._ck(self.L.kuq_stage_db_append(self.h, kdb.ctypes.data, kdb.size, idx.ctypes.data, idx.size))
+
     def stage_db_files(self, kdb_path, idx_path, bin_lo=0, bin_hi=0):
         self.stage_db(np.memmap(kdb_path, np.uint8, "r"), np.memmap(idx_path, np.uint8, "r"), bin_lo, bin_hi)
 
@@ -367,6 +377,8 @@ class Classifier:
         self._ck(self.L.kuq_classify_device(self.h, slot, d_bases, d_offsets, n_reads, total_bases, d_unit, flags))
 
     def lookup_device(self, slot, d_bases, d_offsets, n_reads, total_bases, d_codes_out, only_hits=0):
+        """per-window dense ids into d_codes_out.  only_hits: 0 = every window, 1 = hits only, 2 = LOOKUP_FILL_EMPTY
+        (hits only, and windows already coded non-zero are skipped: the later databases of a streamed run)."""
         self._ck(self.L.kuq_lookup_device(self.h, slot, d_bases, d_offsets, n_reads, total_bases, d_codes_out,
                                           only_hits))
 

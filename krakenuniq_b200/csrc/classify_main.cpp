@@ -36,6 +36,7 @@
 #include <iomanip>
 #include <iostream>
 #include <map>
+#include <memory>
 #include <set>
 #include <sstream>
 #include <string>
@@ -515,10 +516,9 @@ struct Batch {
   string bases;
   vector<uint64_t> offs{0};
   vector<Read> reads;
-  vector<uint32_t> codes;             // chunked mode: per-window dense ids merged over the database ranges
   bool fastq = false;
   int file = 0;                       // index of the input file (work units do not span files)
-  void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); codes.clear(); }
+  void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); }
 };
 
 static OutStream Kraken_out, Classified_out, Unclassified_out;
@@ -1111,198 +1111,276 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
   return ranges;
 }
 
-// unit_aligned: batches end where a work unit of process_file ends (classify.cpp:506-521) and a last unit of total
-// length 0 is dropped like there (:523-524) — what the per-work-unit sketch rule of the preloaded path needs.  The -x
-// path of the reference reads sequence by sequence without work units (:566-791): unit_aligned = false.
-static void load_file_batches(const char *filename, vector<Batch> &out, bool unit_aligned = false) {
+// The batches of one input file, read one at a time.  unit_aligned: batches end where a work unit of process_file ends
+// (classify.cpp:506-521) and a last unit of total length 0 is dropped like there (:523-524) — what the per-work-unit
+// sketch rule of the preloaded path needs.  The -x path of the reference reads sequence by sequence without work units
+// (:566-791): unit_aligned = false.  A batch closes (at a unit boundary when aligned) once it holds max_nt bases.
+struct BatchReader {
   SeqReader reader;
-  if (!reader.in.open(filename)) die(EX_NOINPUT, string("can't open ") + filename);
-  bool fq = reader.fastq = reader.in.peek() == '@';
-  const uint64_t BATCH_NT = 96ull << 20;
-  out.emplace_back();
-  out.back().fastq = fq;
-  Read r;
+  bool fq = false, unit_aligned = false, done = false;
+  uint64_t max_nt = 96ull << 20;
   uint64_t unit_nt = 0;
-  size_t unit_first_read = 0;        // first read of the open work unit inside the current batch
-  size_t batch_units = 0;
-  while (reader.valid) {
-    Batch &b = out.back();
-    if (!reader.next(r, b.bases)) break;
-    b.reads.push_back(r);
-    b.offs.push_back(b.bases.size());
-    bool cut;
-    if (!unit_aligned) {
-      cut = b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 1;
-    } else {
-      unit_nt += r.seq_len;
-      const bool close_unit = unit_nt >= Work_unit_size;
-      if (close_unit) { unit_nt = 0; unit_first_read = b.reads.size(); batch_units++; }
-      cut = close_unit ? (b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 4096 || batch_units >= Max_units_per_batch)
-                       : (b.reads.size() >= (1u << 20) - 1 || b.bases.size() >= (150ull << 20));   // one huge unit: counted as two
+  BatchReader(const char *filename, bool aligned) : unit_aligned(aligned) {
+    if (!reader.in.open(filename)) die(EX_NOINPUT, string("can't open ") + filename);
+    fq = reader.fastq = reader.in.peek() == '@';
+  }
+  bool next(Batch &b) {
+    b.clear();
+    b.fastq = fq;
+    if (done) return false;
+    Read r;
+    size_t unit_first_read = 0;        // first read of the open work unit inside this batch
+    size_t batch_units = 0;
+    while (reader.valid) {
+      if (!reader.next(r, b.bases)) break;
+      b.reads.push_back(r);
+      b.offs.push_back(b.bases.size());
+      bool cut;
+      if (!unit_aligned) {
+        cut = b.bases.size() >= max_nt || b.reads.size() >= (1u << 20) - 1;
+      } else {
+        unit_nt += r.seq_len;
+        const bool close_unit = unit_nt >= Work_unit_size;
+        if (close_unit) { unit_nt = 0; unit_first_read = b.reads.size(); batch_units++; }
+        cut = close_unit ? (b.bases.size() >= max_nt || b.reads.size() >= (1u << 20) - 4096 || batch_units >= Max_units_per_batch)
+                         : (b.reads.size() >= (1u << 20) - 1 || b.bases.size() >= (150ull << 20));   // one huge unit: counted as two
+      }
+      if (cut) return true;
     }
-    if (cut) { out.emplace_back(); out.back().fastq = fq; unit_first_read = 0; batch_units = 0; }
+    if (unit_aligned && unit_nt == 0 && unit_first_read < b.reads.size()) {
+      b.bases.resize(b.offs[unit_first_read]);
+      b.reads.resize(unit_first_read);
+      b.offs.resize(unit_first_read + 1);
+    }
+    done = true;
+    reader.in.close();
+    return !b.reads.empty();
   }
-  if (unit_aligned && unit_nt == 0 && unit_first_read < out.back().reads.size()) {
-    Batch &b = out.back();
-    b.bases.resize(b.offs[unit_first_read]);
-    b.reads.resize(unit_first_read);
-    b.offs.resize(unit_first_read + 1);
-  }
-  if (out.back().reads.empty()) out.pop_back();
-  reader.in.close();
+};
+
+static void load_file_batches(const char *filename, vector<Batch> &out, bool unit_aligned) {
+  BatchReader br(filename, unit_aligned);
+  Batch b;
+  while (br.next(b)) out.push_back(std::move(b));
 }
 
-static void run_chunked(kuq_ctx *ctx, const Mapped &kdb, const Mapped &idx, uint64_t budget, int argc, char **argv,
-                        map<uint32_t, uint64_t> &db_counts) {
-  const uint8_t *q = (const uint8_t *)idx.p;
-  const uint32_t nt = q[7];
-  const uint64_t n_bins = 1ull << (2 * nt);
-  const uint64_t *offsets = (const uint64_t *)(q + 8);
-  vector<pair<uint64_t, uint64_t>> ranges = plan_ranges(offsets, n_bins, budget);
-  cerr << "Database split into " << ranges.size() << " chunks" << endl;
-  // pass 0: the taxids of all records, so that every range numbers taxa identically (also database.kdb.counts)
-  for (auto &rg : ranges) {
-    if (kuq_stage_db(ctx, kdb.p, kdb.size, idx.p, idx.size, rg.first, rg.second)) die(EX_DATAERR, kuq_last_error(ctx));
-    uint32_t m = 0;
-    kuq_db_taxids(ctx, NULL, NULL, 0, &m);
-    vector<uint32_t> tt(m);
-    vector<uint64_t> cc(m);
-    if (m) kuq_db_taxids(ctx, tt.data(), cc.data(), m, &m);
-    for (uint32_t i = 0; i < m; i++) db_counts[tt[i]] += cc[i];
-  }
-  {
-    vector<uint32_t> all;
-    for (auto &kv : db_counts) all.push_back(kv.first);
-    if (kuq_set_db_taxid_universe(ctx, all.data(), (uint32_t)all.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
-  }
-  vector<Batch> batches;
-  for (int i = optind; i < argc; i++) load_file_batches(argv[i], batches);
-  // Preferred path: reads and per-window ids stay in HBM for the whole run and the ranges stream through two device
-  // buffers from the (pinned, if the mapping can be registered) database file while the previous range is looked up
-  // (kuq_stream_*).  Needs 5 bytes per base + 8 per read of device memory next to the two range buffers; a run that does
-  // not fit falls back to the host-side merge below.
-  if (!getenv("KUQ_CHUNKS_ON_HOST")) {
-    uint64_t need = 0, max_rec = 1, max_bins = 1;
-    for (auto &b : batches) need += (b.bases.size() + 64) * 5 + (b.reads.size() + 4) * 8 + 1024;
-    for (auto &rg : ranges) {
-      max_rec = std::max<uint64_t>(max_rec, offsets[rg.second] - offsets[rg.first]);
+// ---- databases that do not fit the HBM budget: streamed through two range buffers ----------------------------------
+// One database larger than the budget (the -x path, process_file_with_db_chunk, classify.cpp:566-791), or several
+// databases that do not fit it together (`-d a -d b`, classify.cpp:928-936).  The input is read in rounds: a round's
+// reads and per-window ids stay in HBM (5 bytes per base + 8 per read, + 4 per read of unit ids) next to the two range
+// buffers, as many batches as fit the budget and at least one.  Each round goes through the databases in command-line
+// order and each database through its minimizer ranges (kuq_stream_*: the next range travels while the current one is
+// looked up).  The first database writes its hits, a stored zero as KUQ_CODE_FOUND_ZERO; the later ones only fill the
+// windows that no earlier database answered (KUQ_LOOKUP_FILL_EMPTY).  Then the round's batches are resolved and written
+// in input order.  One database keeps the -x rule (one sketch per taxon; batches need not hold whole work units);
+// several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b` without -x.
+static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, uint64_t range_budget,
+                         uint64_t hbm_budget, int argc, char **argv, vector<map<uint32_t, uint64_t>> &db_counts) {
+  const size_t n_db = kdbs.size();
+  const bool unit_rule = n_db > 1;
+  struct Plan {
+    const uint8_t *rec0;
+    const uint64_t *offsets;
+    uint64_t pair_sz;
+    uint32_t k, nt, idx_type;
+    vector<pair<uint64_t, uint64_t>> ranges;
+  };
+  vector<Plan> plans(n_db);
+  set<uint32_t> all;
+  uint64_t max_rec = 1, max_bins = 1;
+  for (size_t d = 0; d < n_db; d++) {
+    Plan &pl = plans[d];
+    const uint8_t *q = (const uint8_t *)idxs[d].p;
+    uint64_t key_bits;
+    memcpy(&key_bits, (const uint8_t *)kdbs[d].p + 8, 8);
+    pl.k = (uint32_t)(key_bits / 2);
+    pl.nt = q[7];
+    pl.idx_type = memcmp(q, "KRAKIDX", 7) == 0 ? 1 : 2;
+    pl.pair_sz = (key_bits + 7) / 8 + 4;                          // the file's record size (12 B only for k = 29..31)
+    pl.rec0 = (const uint8_t *)kdbs[d].p + 72 + 2 * (4 + 8 * key_bits);
+    pl.offsets = (const uint64_t *)(q + 8);
+    pl.ranges = plan_ranges(pl.offsets, 1ull << (2 * pl.nt), range_budget);
+    // pass 0: the taxids of all records, so that every range numbers taxa identically (also database.kdb.counts)
+    for (auto &rg : pl.ranges) {
+      max_rec = std::max<uint64_t>(max_rec, pl.offsets[rg.second] - pl.offsets[rg.first]);
       max_bins = std::max<uint64_t>(max_bins, rg.second - rg.first);
+      if (kuq_stage_db(ctx, kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, rg.first, rg.second)) die(EX_DATAERR, kuq_last_error(ctx));
+      uint32_t m = 0;
+      kuq_db_taxids(ctx, NULL, NULL, 0, &m);
+      vector<uint32_t> tt(m);
+      vector<uint64_t> cc(m);
+      if (m) kuq_db_taxids(ctx, tt.data(), cc.data(), m, &m);
+      for (uint32_t i = 0; i < m; i++) { db_counts[d][tt[i]] += cc[i]; all.insert(tt[i]); }
     }
-    const uint64_t range_bytes = 2 * (max_rec * 12 + (max_bins + 1) * 8 + 4096);     // 12 B per record in HBM
-    const uint64_t free_b = kuq_device_free_bytes(ctx);
-    if (need + range_bytes + (2ull << 30) < free_b || getenv("KUQ_FORCE_CHUNKS")) {
-      uint64_t key_bits;
-      memcpy(&key_bits, (const uint8_t *)kdb.p + 8, 8);
-      const uint64_t header = 72 + 2 * (4 + 8 * key_bits);
-      const uint8_t *rec0 = (const uint8_t *)kdb.p + header;
-      const uint32_t k = (uint32_t)(key_bits / 2), idx_type = memcmp(q, "KRAKIDX", 7) == 0 ? 1 : 2;
-      const uint64_t pair_sz = (key_bits + 7) / 8 + 4;            // the file's record size (12 B only for k = 29..31)
-      // taxonomy must be known before the stream opens (the dense numbering is fixed there): main() sets it before us
-      if (kuq_stream_open(ctx, k, nt, idx_type, max_rec, max_bins)) die(EX_DATAERR, kuq_last_error(ctx));
-      const bool pinned = kuq_host_register(kdb.p, kdb.size) == KUQ_OK && kuq_host_register(idx.p, idx.size) == KUQ_OK;
-      if (Timing) fprintf(stderr, "[timing] chunked: %zu ranges, database mapping %s\n", ranges.size(), pinned ? "pinned" : "pageable");
-      struct DevBatch { void *bases, *offs, *codes; };
-      vector<DevBatch> dev(batches.size());
-      for (size_t bi = 0; bi < batches.size(); bi++) {
-        Batch &b = batches[bi];
-        DevBatch &d = dev[bi];
-        d.bases = kuq_device_alloc(ctx, b.bases.size() + 64);
-        d.offs = kuq_device_alloc(ctx, (b.reads.size() + 4) * 8);
-        d.codes = kuq_device_alloc(ctx, (b.bases.size() + 64) * 4);
-        if (!d.bases || !d.offs || !d.codes) die(EX_OSERR, "device allocation for the read batches failed");
-        vector<uint64_t> offs(b.offs);
-        offs.push_back(offs.back()); offs.push_back(offs.back());
-        if (kuq_device_memset(ctx, 0, (char *)d.bases + b.bases.size(), 'N', 64) ||
-            kuq_copy_to_device(ctx, 0, d.bases, b.bases.data(), b.bases.size()) ||
-            kuq_copy_to_device(ctx, 0, d.offs, offs.data(), offs.size() * 8) ||
-            kuq_device_memset(ctx, 0, d.codes, 0, (b.bases.size() + 64) * 4) || kuq_sync_slot(ctx, 0))
-          die(EX_SOFTWARE, kuq_last_error(ctx));
+  }
+  if (n_db == 1) cerr << "Database split into " << plans[0].ranges.size() << " chunks" << endl;
+  {
+    vector<uint32_t> u(all.begin(), all.end());
+    if (kuq_set_db_taxid_universe(ctx, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
+  }
+  if (unit_rule) {
+    if (kuq_mark_zero_hits(ctx, 1)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    uint32_t rows = 0;
+    if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    if (rows) Max_units_per_batch = rows;
+  }
+  // device memory of a round: the budget (and what the card has free) minus the two range buffers
+  const uint64_t range_bytes = 2 * (max_rec * 12 + (max_bins + 1) * 8 + 4096);     // 12 B per record in HBM
+  const uint64_t free_b = kuq_device_free_bytes(ctx);
+  const uint64_t cap = std::min<uint64_t>(hbm_budget, free_b > (2ull << 30) ? free_b - (2ull << 30) : 0);
+  const uint64_t round_bytes = cap > range_bytes ? cap - range_bytes : 0;
+  const uint64_t batch_nt = std::max<uint64_t>(1, std::min<uint64_t>(96ull << 20, round_bytes / 6));
+  uint64_t db_bytes = 0;                                           // what every round copies to the device
+  for (size_t d = 0; d < n_db; d++) db_bytes += kdbs[d].size + idxs[d].size;
+  if (round_bytes < db_bytes)
+    fprintf(stderr, "classify: %llu MiB of device memory per round of reads next to the range buffers, while every round "
+                    "copies the %llu MiB of the database(s) again: more device memory (KUQ_HBM_BUDGET) means fewer rounds\n",
+            (unsigned long long)(round_bytes >> 20), (unsigned long long)(db_bytes >> 20));
+  // Mappings registered as pinned memory (the range copies overlap the lookups only from pinned memory), in command-line
+  // order while they take at most half of the host's physical memory together: the rest streams from pageable memory
+  // rather than page-locking what the reads and the rest of the host need.
+  vector<int> pinned;
+  {
+    const uint64_t phys = (uint64_t)sysconf(_SC_PHYS_PAGES) * (uint64_t)sysconf(_SC_PAGESIZE);
+    uint64_t locked = 0;
+    for (size_t d = 0; d < n_db; d++)
+      for (const Mapped *m : {&kdbs[d], &idxs[d]}) {
+        const bool ok = locked + m->size <= phys / 2 && kuq_host_register(m->p, m->size) == KUQ_OK;
+        if (ok) locked += m->size;
+        pinned.push_back(ok);
+      }
+  }
+  if (Timing) fprintf(stderr, "[timing] streamed: %zu database(s), %llu MiB per round\n", n_db, (unsigned long long)(round_bytes >> 20));
+
+  // the input, batch by batch across the files
+  int fi = optind;
+  std::unique_ptr<BatchReader> br;
+  auto pull = [&](Batch &b) -> bool {
+    for (;;) {
+      if (!br) {
+        if (fi >= argc) return false;
+        br.reset(new BatchReader(argv[fi], unit_rule));
+        br->max_nt = batch_nt;
+      }
+      if (br->next(b)) { b.file = fi; return true; }
+      br.reset();
+      fi++;
+    }
+  };
+  // work-unit ids of the per-work-unit rule: process_file's cutting (classify.cpp:506-521), units end with their file
+  uint32_t unit_next = 0;
+  uint64_t unit_nt = 0;
+  int unit_file = -1;
+  struct DevBatch { void *bases, *offs, *codes, *units; };
+  vector<Batch> round;
+  Batch pending;
+  bool have_pending = false;
+  uint32_t open_nt = 0, open_type = 0;                             // parameters the range buffers are open for
+  size_t n_rounds = 0;
+  for (;;) {
+    round.clear();
+    uint64_t bytes = 0;
+    for (;;) {
+      if (!have_pending) have_pending = pull(pending);
+      if (!have_pending) break;
+      const uint64_t need = (pending.bases.size() + 64) * 5 + (pending.reads.size() + 4) * (unit_rule ? 12 : 8) + 1024;
+      if (!round.empty() && bytes + need > round_bytes) break;
+      bytes += need;
+      round.push_back(std::move(pending));
+      have_pending = false;
+    }
+    if (round.empty()) break;
+    n_rounds++;
+    vector<DevBatch> dev(round.size());
+    for (size_t bi = 0; bi < round.size(); bi++) {
+      Batch &b = round[bi];
+      DevBatch &d = dev[bi];
+      d.bases = kuq_device_alloc(ctx, b.bases.size() + 64);
+      d.offs = kuq_device_alloc(ctx, (b.reads.size() + 4) * 8);
+      d.codes = kuq_device_alloc(ctx, (b.bases.size() + 64) * 4);
+      d.units = unit_rule ? kuq_device_alloc(ctx, (b.reads.size() + 4) * 4) : NULL;
+      if (!d.bases || !d.offs || !d.codes || (unit_rule && !d.units)) die(EX_OSERR, "device allocation for the read batches failed");
+      vector<uint64_t> offs(b.offs);
+      offs.push_back(offs.back()); offs.push_back(offs.back());
+      if (kuq_device_memset(ctx, 0, (char *)d.bases + b.bases.size(), 'N', 64) ||
+          kuq_copy_to_device(ctx, 0, d.bases, b.bases.data(), b.bases.size()) ||
+          kuq_copy_to_device(ctx, 0, d.offs, offs.data(), offs.size() * 8) ||
+          kuq_device_memset(ctx, 0, d.codes, 0, (b.bases.size() + 64) * 4))
+        die(EX_SOFTWARE, kuq_last_error(ctx));
+      if (unit_rule) {
+        if (unit_file >= 0 && b.file != unit_file) { unit_next++; unit_nt = 0; }
+        unit_file = b.file;
+        vector<uint32_t> units(b.reads.size());
+        for (size_t i = 0; i < b.reads.size(); i++) {
+          units[i] = unit_next;
+          unit_nt += b.reads[i].seq_len;
+          if (unit_nt >= Work_unit_size) { unit_next++; unit_nt = 0; }
+        }
+        if (kuq_copy_to_device(ctx, 0, d.units, units.data(), units.size() * 4)) die(EX_SOFTWARE, kuq_last_error(ctx));
+      }
+      if (kuq_sync_slot(ctx, 0)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    }
+    for (size_t db = 0; db < n_db; db++) {
+      const Plan &pl = plans[db];
+      if (pl.nt != open_nt || pl.idx_type != open_type) {
+        // taxonomy and universe are known before the stream opens (the dense numbering is fixed there)
+        if ((open_nt && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, max_rec, max_bins))
+          die(EX_DATAERR, kuq_last_error(ctx));
+        open_nt = pl.nt;
+        open_type = pl.idx_type;
       }
       auto load = [&](uint32_t buf, size_t c) {
-        const uint64_t lo = ranges[c].first, hi = ranges[c].second;
-        if (kuq_stream_load(ctx, buf, rec0 + offsets[lo] * pair_sz, offsets[hi] - offsets[lo], offsets + lo, lo, hi))
+        const uint64_t lo = pl.ranges[c].first, hi = pl.ranges[c].second;
+        if (kuq_stream_load(ctx, buf, pl.rec0 + pl.offsets[lo] * pl.pair_sz, pl.offsets[hi] - pl.offsets[lo], pl.offsets + lo, lo, hi))
           die(EX_DATAERR, kuq_last_error(ctx));
       };
       load(0, 0);
-      for (size_t c = 0; c < ranges.size(); c++) {
+      for (size_t c = 0; c < pl.ranges.size(); c++) {
         if (kuq_stream_use(ctx, (uint32_t)(c & 1))) die(EX_SOFTWARE, kuq_last_error(ctx));
-        if (c + 1 < ranges.size()) load((uint32_t)((c + 1) & 1), c + 1);
+        if (c + 1 < pl.ranges.size()) load((uint32_t)((c + 1) & 1), c + 1);
         uint64_t seqs = 0;
-        for (size_t bi = 0; bi < batches.size(); bi++) {
-          Batch &b = batches[bi];
+        for (size_t bi = 0; bi < round.size(); bi++) {
+          Batch &b = round[bi];
           if (kuq_lookup_device(ctx, (uint32_t)(bi & 1), (const char *)dev[bi].bases, (const uint64_t *)dev[bi].offs,
-                                (uint32_t)b.reads.size(), b.bases.size(), (uint32_t *)dev[bi].codes, 1))
+                                (uint32_t)b.reads.size(), b.bases.size(), (uint32_t *)dev[bi].codes, db == 0 ? 1 : KUQ_LOOKUP_FILL_EMPTY))
             die(EX_SOFTWARE, kuq_last_error(ctx));
           seqs += b.reads.size();
         }
-        fprintf(stderr, "\r Processed %llu sequences (database chunk %zu of %zu)\n", (unsigned long long)seqs, c + 1, ranges.size());
+        if (n_db == 1) fprintf(stderr, "\r Processed %llu sequences (database chunk %zu of %zu)\n", (unsigned long long)seqs, c + 1, pl.ranges.size());
+        else fprintf(stderr, "\r Processed %llu sequences (database %zu of %zu, chunk %zu of %zu)", (unsigned long long)seqs, db + 1, n_db,
+                     c + 1, pl.ranges.size());
       }
-      if (kuq_sync_slot(ctx, 0) || kuq_sync_slot(ctx, 1) || kuq_stream_check(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
-      for (size_t bi = 0; bi < batches.size(); bi++) {              // final pass (classify.cpp:663-791)
-        Batch &b = batches[bi];
-        kuq_batch_result res;
-        if (kuq_resolve_device(ctx, 0, (const char *)dev[bi].bases, (const uint64_t *)dev[bi].offs, (uint32_t)b.reads.size(),
-                               b.bases.size(), (const uint32_t *)dev[bi].codes, NULL, 0) ||
-            kuq_collect_device_batch(ctx, 0, &res))
-          die(EX_SOFTWARE, kuq_last_error(ctx));
-        Fastq_input = b.fastq;
-        emit_results(b, res);
-        total_classified += res.n_classified;
-        total_sequences += b.reads.size();
-        total_bases += b.bases.size();
-        fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
-      }
-      if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
-      for (auto &d : dev) { kuq_device_free(ctx, d.bases); kuq_device_free(ctx, d.offs); kuq_device_free(ctx, d.codes); }
-      if (pinned) { kuq_host_unregister(kdb.p); kuq_host_unregister(idx.p); }
-      return;
     }
-    cerr << "classify: the reads (" << need / (1 << 20) << " MiB on the device) do not fit next to the database ranges: merging on the host" << endl;
-  }
-  {
-    // host-side merge needs 5 x the input in RAM: say so instead of running into the OOM killer
-    uint64_t bytes = 0;
-    for (auto &b : batches) bytes += b.bases.size() * 5;
-    const uint64_t avail = (uint64_t)sysconf(_SC_AVPHYS_PAGES) * (uint64_t)sysconf(_SC_PAGESIZE);
-    if (bytes > avail) die(EX_OSERR, "the host-side merge of the database chunks needs about " + std::to_string(bytes >> 30) +
-                                     " GiB of RAM, " + std::to_string(avail >> 30) + " GiB are available: split the input");
-  }
-  for (auto &b : batches) b.codes.assign(b.bases.size() + 1, 0);
-  vector<uint32_t> tmp;
-  for (size_t c = 0; c < ranges.size(); c++) {
-    // with one range staged in pass 0 last, re-staging it is skipped
-    if (!(ranges.size() == 1))
-      if (kuq_stage_db(ctx, kdb.p, kdb.size, idx.p, idx.size, ranges[c].first, ranges[c].second)) die(EX_DATAERR, kuq_last_error(ctx));
-    uint64_t seqs = 0;
-    for (auto &b : batches) {
-      tmp.assign(b.bases.size() + 1, 0);
-      if (kuq_lookup_batch(ctx, b.bases.data(), b.offs.data(), (uint32_t)b.reads.size(), tmp.data(), NULL))
+    if (kuq_sync_slot(ctx, 0) || kuq_sync_slot(ctx, 1) || kuq_stream_check(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    for (size_t bi = 0; bi < round.size(); bi++) {                 // final pass (classify.cpp:663-791)
+      Batch &b = round[bi];
+      kuq_batch_result res;
+      if (kuq_resolve_device(ctx, 0, (const char *)dev[bi].bases, (const uint64_t *)dev[bi].offs, (uint32_t)b.reads.size(),
+                             b.bases.size(), (const uint32_t *)dev[bi].codes, (const uint32_t *)dev[bi].units, 0) ||
+          kuq_collect_device_batch(ctx, 0, &res))
         die(EX_SOFTWARE, kuq_last_error(ctx));
-      {
-        uint32_t *dst = b.codes.data();
-        const uint32_t *src = tmp.data();
-        const long long n = (long long)b.bases.size();
-#pragma omp parallel for schedule(static) num_threads(Num_threads)
-        for (long long j = 0; j < n; j++) if (src[j] > dst[j]) dst[j] = src[j];                     // merge, :390-485
-      }
-      seqs += b.reads.size();
-      fprintf(stderr, "\r Processed %llu sequences (database chunk %zu of %zu)", (unsigned long long)seqs, c + 1, ranges.size());
+      Fastq_input = b.fastq;
+      emit_results(b, res);
+      total_classified += res.n_classified;
+      total_sequences += b.reads.size();
+      total_bases += b.bases.size();
+      fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
     }
-    fprintf(stderr, "\r Processed %llu sequences\n", (unsigned long long)seqs);
-  }
-  // final pass: classify from the merged taxa (classify.cpp:663-791)
-  for (auto &b : batches) {
-    kuq_batch_result res;
-    if (kuq_resolve_batch(ctx, b.bases.data(), b.offs.data(), (uint32_t)b.reads.size(), b.codes.data(), NULL, 0, &res))
-      die(EX_SOFTWARE, kuq_last_error(ctx));
-    Fastq_input = b.fastq;
-    emit_results(b, res);
-    total_classified += res.n_classified;
-    total_sequences += b.reads.size();
-    total_bases += b.bases.size();
-    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
+    for (auto &d : dev) {
+      kuq_device_free(ctx, d.bases); kuq_device_free(ctx, d.offs); kuq_device_free(ctx, d.codes);
+      if (d.units) kuq_device_free(ctx, d.units);
+    }
   }
   if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
+  for (size_t d = 0; d < n_db; d++) {
+    if (pinned[2 * d]) kuq_host_unregister(kdbs[d].p);
+    if (pinned[2 * d + 1]) kuq_host_unregister(idxs[d].p);
+  }
+  if (n_db > 1) {
+    string per;
+    for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(plans[d].ranges.size());
+    fprintf(stderr, "\nclassify: %zu databases streamed: %zu rounds, ranges per database %s\n", n_db, n_rounds, per.c_str());
+  }
 }
 
 // ---- a database that fits the GPUs of the node together but not one of them: minimizer-range shards (SURVEY §8(e).2) ---
@@ -1434,83 +1512,6 @@ static void run_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const 
   }
 }
 
-// ---- several databases: `-d a -d b` (classify.cpp:928-936) ----------------------------------------------------
-// For every k-mer the reference asks the databases in command-line order and keeps the value of the first one
-// that holds the key — a stored taxon 0 included.  One database is resident in HBM at a time: the reads are
-// looked up against each in turn (kuq_lookup_batch reports a stored zero as KUQ_CODE_FOUND_ZERO), the first
-// non-zero code per window survives, and a final pass classifies from the merged codes with the per-work-unit
-// sketch rule of the preloaded path.  The databases may differ in minimizer length and index type, not in k.
-static void run_multi_db(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, int argc, char **argv,
-                         vector<map<uint32_t, uint64_t>> &db_counts) {
-  const size_t n_db = kdbs.size();
-  db_counts.assign(n_db, {});
-  set<uint32_t> all;
-  for (size_t d = 0; d < n_db; d++) {                      // pass 0: one numbering of the taxa for all databases
-    if (kuq_stage_db(ctx, kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, 0, 0)) die(EX_DATAERR, kuq_last_error(ctx));
-    uint32_t m = 0;
-    kuq_db_taxids(ctx, NULL, NULL, 0, &m);
-    vector<uint32_t> tt(m);
-    vector<uint64_t> cc(m);
-    if (m) kuq_db_taxids(ctx, tt.data(), cc.data(), m, &m);
-    for (uint32_t i = 0; i < m; i++) { db_counts[d][tt[i]] += cc[i]; all.insert(tt[i]); }
-  }
-  {
-    vector<uint32_t> u(all.begin(), all.end());
-    if (kuq_set_db_taxid_universe(ctx, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
-  }
-  if (kuq_mark_zero_hits(ctx, 1)) die(EX_SOFTWARE, "kuq_mark_zero_hits");
-  vector<Batch> batches;
-  for (int i = optind; i < argc; i++) {
-    size_t first = batches.size();
-    load_file_batches(argv[i], batches, true);
-    for (size_t j = first; j < batches.size(); j++) batches[j].file = i;
-  }
-  {
-    // the merged per-window ids of all reads stay on the host between the databases (4 bytes per base + one batch of
-    // scratch): say so instead of running into the OOM killer
-    uint64_t bytes = 0, largest = 0;
-    for (auto &b : batches) { bytes += b.bases.size() * 4; largest = std::max<uint64_t>(largest, b.bases.size() * 4); }
-    const uint64_t avail = (uint64_t)sysconf(_SC_AVPHYS_PAGES) * (uint64_t)sysconf(_SC_PAGESIZE);
-    if (bytes + largest > avail) die(EX_OSERR, "classifying against several databases needs about " + std::to_string((bytes + largest) >> 30) +
-                                               " GiB of RAM for the merged k-mer ids, " + std::to_string(avail >> 30) + " GiB are available: split the input");
-  }
-  for (auto &b : batches) b.codes.assign(b.bases.size() + 1, 0);
-  vector<uint32_t> tmp;
-  for (size_t d = 0; d < n_db; d++) {
-    if (kuq_stage_db(ctx, kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, 0, 0)) die(EX_DATAERR, kuq_last_error(ctx));
-    uint64_t seqs = 0;
-    for (auto &b : batches) {
-      tmp.assign(b.bases.size() + 1, 0);
-      if (kuq_lookup_batch(ctx, b.bases.data(), b.offs.data(), (uint32_t)b.reads.size(), tmp.data(), NULL))
-        die(EX_SOFTWARE, kuq_last_error(ctx));
-      {
-        uint32_t *dst = b.codes.data();
-        const uint32_t *src = tmp.data();
-        const long long n = (long long)b.bases.size();
-#pragma omp parallel for schedule(static) num_threads(Num_threads)
-        for (long long j = 0; j < n; j++) if (dst[j] == 0) dst[j] = src[j];                         // first hit wins
-      }
-      seqs += b.reads.size();
-      fprintf(stderr, "\r Processed %llu sequences (database %zu of %zu)", (unsigned long long)seqs, d + 1, n_db);
-    }
-    fprintf(stderr, "\r Processed %llu sequences\n", (unsigned long long)seqs);
-  }
-  for (size_t bi = 0; bi < batches.size(); bi++) {
-    Batch &b = batches[bi];
-    kuq_batch_result res;
-    if (kuq_resolve_batch(ctx, b.bases.data(), b.offs.data(), (uint32_t)b.reads.size(), b.codes.data(), NULL, 0, &res))
-      die(EX_SOFTWARE, kuq_last_error(ctx));
-    Fastq_input = b.fastq;
-    emit_results(b, res);
-    total_classified += res.n_classified;
-    total_sequences += b.reads.size();
-    total_bases += b.bases.size();
-    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
-    if (bi + 1 == batches.size() || batches[bi + 1].file != b.file)
-      if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));      // work units do not span input files
-  }
-}
-
 // What a staged database takes in HBM: 12 bytes per record whatever the file's record size (records of k <= 28 databases
 // are widened on the way in), plus the index.  Every decision about what fits a card counts these bytes, not the file's.
 static uint64_t hbm_bytes(const Mapped &kdb, const Mapped &idx) {
@@ -1553,7 +1554,7 @@ int main(int argc, char **argv) {
   if (getenv("KUQ_HBM_BUDGET")) hbm_budget = strtoull(getenv("KUQ_HBM_BUDGET"), NULL, 10);
   uint64_t chunk_budget = 0;
   // a database larger than one card: sharded over the visible GPUs when they hold it together (run_sharded), else
-  // streamed through one GPU in ranges of at most 40 GB (two range buffers + the reads have to fit, run_chunked)
+  // streamed through one GPU in ranges of at most 40 GB (two range buffers + a round of reads have to fit, run_streamed)
   bool want_shards = false;
   const uint64_t db_hbm = hbm_bytes(kdb, idx);
   if (n_db == 1 && (db_hbm > hbm_budget || getenv("KUQ_FORCE_SHARDS"))) {
@@ -1563,10 +1564,11 @@ int main(int argc, char **argv) {
     want_shards = n_vis > 1 && (getenv("KUQ_FORCE_SHARDS") || db_hbm / n_vis + (16ull << 30) < hbm_budget);
   }
   if (db_hbm > hbm_budget && !want_shards) chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
+  // several databases: resident together when their records fit the budget together, else streamed (run_streamed)
   if (n_db > 1) {
-    for (size_t i = 0; i < n_db; i++)
-      if (hbm_bytes(kdbs[i], idxs[i]) > hbm_budget) die(EX_USAGE, "with several databases each one has to fit the HBM budget");
-    chunk_budget = 0;
+    uint64_t all_hbm = 0;
+    for (size_t i = 0; i < n_db; i++) all_hbm += hbm_bytes(kdbs[i], idxs[i]);
+    chunk_budget = all_hbm > hbm_budget ? std::min<uint64_t>(hbm_budget / 4, 40ull << 30) : 0;
   }
   if (Populate_memory_size > 0 && getenv("KUQ_FORCE_CHUNKS")) { chunk_budget = Populate_memory_size; want_shards = false; }
   kuq_config cfg;
@@ -1574,25 +1576,26 @@ int main(int argc, char **argv) {
   cfg.n_slots = 3;                             // classify b + 1 on the GPU, format b, gather b + 2 (process_file_parallel)
   cfg.max_bases_per_batch = 288ull << 20;      // one read may be a whole chromosome (the largest human one is 248 Mbp)
   cfg.work_unit_size = Work_unit_size;
-  // -x (or a database that has to be split) → one global sketch per taxon (classify.cpp:719); else per work unit
-  cfg.hll_mode = (Populate_memory_size > 0 || chunk_budget || want_shards) ? KUQ_HLL_CHUNKED : KUQ_HLL_PRELOAD;
+  // -x (or a database that has to be split) → one global sketch per taxon (classify.cpp:719); else per work unit, which
+  // is also the reference's rule for several databases
+  cfg.hll_mode = (Populate_memory_size > 0 || (chunk_budget && n_db == 1) || want_shards) ? KUQ_HLL_CHUNKED : KUQ_HLL_PRELOAD;
 #ifdef EXACT_COUNTING
   // classifyExact (classify.cpp:46-49): sets of k-mers instead of sketches; work units and chunks make no difference
   cfg.hll_mode = KUQ_HLL_EXACT;
   if (want_shards) { want_shards = false; chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30); }   // exact sets are not merged across devices
   if (Quick_mode) die(EX_USAGE, "-q is not supported by the GPU classifyExact");
 #endif
-  if ((chunk_budget || want_shards) && !Populate_memory_size)
+  if ((chunk_budget || want_shards) && !Populate_memory_size && n_db == 1)
     cerr << "classify: database larger than one GPU's HBM budget: " << (want_shards ? "sharding it over the GPUs" : "processing it in ranges")
          << " (unique k-mer counts follow the -x rule)" << endl;
   if (getenv("KUQ_SPARSE_SLOTS")) cfg.sparse_set_slots = strtoull(getenv("KUQ_SPARSE_SLOTS"), NULL, 10);
   if (getenv("KUQ_DEVICE")) cfg.device = atoi(getenv("KUQ_DEVICE"));
-  // devices: KUQ_DEVICES=0,2,3 (or "all"); default = every visible sm_90 GPU when the database is replicated (one
-  // database that fits a card), else one device (KUQ_DEVICE).  Ranges / several databases run on the first device.
+  // devices: KUQ_DEVICES=0,2,3 (or "all"); default = every visible sm_90 GPU when the databases are replicated (they fit
+  // a card together), else one device (KUQ_DEVICE).  Streamed ranges run on the first device.
   vector<int> devices;
   {
     const char *dl = getenv("KUQ_DEVICES");
-    const bool replicable = !chunk_budget && n_db == 1 && cfg.hll_mode != KUQ_HLL_EXACT;   // exact k-mer sets are not merged across devices
+    const bool replicable = !chunk_budget && cfg.hll_mode != KUQ_HLL_EXACT;   // exact k-mer sets are not merged across devices
     // (replicas when the database fits a card, shards when it only fits the cards together)
     if (dl && strcmp(dl, "all") != 0) {
       for (const char *q = dl; *q;) { devices.push_back(atoi(q)); while (*q && *q != ',') q++; if (*q) q++; }
@@ -1615,13 +1618,14 @@ int main(int argc, char **argv) {
     All_ctx.push_back(cx);
   }
   if (want_shards && All_ctx.size() < 2) { want_shards = false; chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30); }
-  if (All_ctx.size() > 1 && !want_shards) fprintf(stderr, "classify: %zu GPUs, database replicated, batches round-robin\n", All_ctx.size());
+  if (All_ctx.size() > 1 && !want_shards && n_db == 1) fprintf(stderr, "classify: %zu GPUs, database replicated, batches round-robin\n", All_ctx.size());
+  if (n_db > 1 && !chunk_budget) fprintf(stderr, "classify: %zu databases resident on %zu GPU(s)\n", n_db, All_ctx.size());
   // -q: the preloaded path leaves a read at its -m'th hit; with -x every k-mer is counted (classify.cpp:943-944 / :701-738)
   for (kuq_ctx *c : All_ctx)
     if (Quick_mode && kuq_set_quick_mode(c, Minimum_hit_count, Populate_memory_size == 0)) die(EX_SOFTWARE, kuq_last_error(c));
-  map<uint32_t, uint64_t> chunk_db_counts;
-  vector<map<uint32_t, uint64_t>> multi_db_counts;
-  if (!chunk_budget && !want_shards && n_db == 1) {
+  // records per taxid of each database (the .counts files), when the run stages databases in pieces or several of them
+  vector<map<uint32_t, uint64_t>> db_counts(n_db);
+  if (!chunk_budget && !want_shards) {
     double T0__ = now_s();
     // the pinned staging sets of the ingest pipeline are allocated while the database travels to the GPUs
     std::thread prealloc([] {
@@ -1630,11 +1634,31 @@ int main(int argc, char **argv) {
       for (auto &s : tmp) prepare_stage(s, 150ull << 20, 1u << 20);
       Prealloc_stages.swap(tmp);
     });
-    // every device stages the database from the same mapped files, in parallel
+    // every device stages the databases, in command-line order, from the same mapped files, in parallel; the first one
+    // reads each database's taxids as the difference of the staged union before and after it
     vector<int> rcs(All_ctx.size(), 0);
+    vector<map<uint32_t, uint64_t>> union_after(n_db);
 #pragma omp parallel for num_threads((int)All_ctx.size()) schedule(static, 1)
-    for (int g = 0; g < (int)All_ctx.size(); g++) rcs[g] = kuq_stage_db(All_ctx[g], kdb.p, kdb.size, idx.p, idx.size, 0, 0);
+    for (int g = 0; g < (int)All_ctx.size(); g++) {
+      for (size_t d = 0; d < n_db && !rcs[g]; d++) {
+        rcs[g] = d ? kuq_stage_db_append(All_ctx[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size)
+                   : kuq_stage_db(All_ctx[g], kdb.p, kdb.size, idx.p, idx.size, 0, 0);
+        if (g == 0 && !rcs[g] && n_db > 1) {
+          uint32_t m = 0;
+          kuq_db_taxids(All_ctx[g], NULL, NULL, 0, &m);
+          vector<uint32_t> tt(m);
+          vector<uint64_t> cc(m);
+          if (m) kuq_db_taxids(All_ctx[g], tt.data(), cc.data(), m, &m);
+          for (uint32_t i = 0; i < m; i++) union_after[d][tt[i]] = cc[i];
+        }
+      }
+    }
     for (size_t g = 0; g < All_ctx.size(); g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(All_ctx[g]));
+    for (size_t d = 0; d < n_db && n_db > 1; d++)
+      for (auto &kv : union_after[d]) {
+        const uint64_t before = d && union_after[d - 1].count(kv.first) ? union_after[d - 1][kv.first] : 0;
+        if (kv.second > before) db_counts[d][kv.first] = kv.second - before;
+      }
     prealloc.join();
     TICK("stage_db");
   }
@@ -1650,7 +1674,7 @@ int main(int argc, char **argv) {
     for (kuq_ctx *c : All_ctx)
       if (kuq_set_taxonomy(c, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(c));
   }
-  if (cfg.hll_mode == KUQ_HLL_PRELOAD && n_db == 1) {
+  if (cfg.hll_mode == KUQ_HLL_PRELOAD && !chunk_budget) {           // (streamed runs ask once their taxa are known)
     uint32_t rows = 0;
     if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
     if (rows) Max_units_per_batch = rows;
@@ -1666,9 +1690,8 @@ int main(int argc, char **argv) {
 
   struct timeval tv1, tv2;
   gettimeofday(&tv1, NULL);
-  if (n_db > 1) run_multi_db(ctx, kdbs, idxs, argc, argv, multi_db_counts);
-  else if (want_shards) run_sharded(All_ctx, kdb, idx, argc, argv, chunk_db_counts);
-  else if (chunk_budget) run_chunked(ctx, kdb, idx, chunk_budget, argc, argv, chunk_db_counts);
+  if (want_shards) run_sharded(All_ctx, kdb, idx, argc, argv, db_counts[0]);
+  else if (chunk_budget) run_streamed(ctx, kdbs, idxs, chunk_budget, hbm_budget, argc, argv, db_counts);
   else for (int i = optind; i < argc; i++) process_file(ctx, argv[i]);
   // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
   for (size_t g = 1; g < All_ctx.size(); g++)
@@ -1700,10 +1723,8 @@ int main(int argc, char **argv) {
     if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
       cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
       ofstream ofs(fname);
-      if (n_db > 1) {
-        for (auto &kv : multi_db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
-      } else if (chunk_budget || want_shards) {
-        for (auto &kv : chunk_db_counts) ofs << kv.first << '\t' << kv.second << '\n';
+      if (n_db > 1 || chunk_budget || want_shards) {
+        for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
       } else {
         uint32_t m = 0;
         kuq_db_taxids(ctx, NULL, NULL, 0, &m);

@@ -106,6 +106,20 @@ struct kuq_ctx {
   uint32_t *d_tx_keys = nullptr, *d_tx_dense = nullptr;
   unsigned long long *d_tx_counts = nullptr;
   uint32_t tx_cap = 0;
+  // whole databases asked after the one above, in this order (kuq_stage_db_append); same k
+  struct ExtraDb {
+    uint8_t *d_pairs = nullptr;
+    uint64_t *d_offsets = nullptr;
+    uint64_t key_ct = 0;
+    uint32_t nt = 0, idx_type = 0;
+    uint32_t *d_tx_keys = nullptr, *d_tx_dense = nullptr;
+    unsigned long long *d_tx_counts = nullptr;
+    uint32_t tx_cap = 0;
+    std::vector<uint32_t> taxids;
+    std::vector<uint64_t> counts;
+    bool remapped = false;
+  };
+  std::vector<ExtraDb> more;
 
   // taxonomy
   bool tax_set = false, finalized = false;
@@ -236,6 +250,10 @@ void free_db(kuq_ctx *ctx) {
   cudaFree(ctx->d_secondaries);
   ctx->d_secondaries = nullptr; ctx->n_secondaries = 0; ctx->collisions = 0;
   ctx->db_staged = false; ctx->db_remapped = false;
+  for (auto &e : ctx->more) {
+    cudaFree(e.d_pairs); cudaFree(e.d_offsets); cudaFree(e.d_tx_keys); cudaFree(e.d_tx_dense); cudaFree(e.d_tx_counts);
+  }
+  ctx->more.clear();
 }
 
 void free_tax_state(kuq_ctx *ctx) {
@@ -337,21 +355,23 @@ int check_slot(kuq_ctx *ctx, uint32_t slot) {
   return KUQ_OK;
 }
 
-// Scan the staged records for their distinct taxids (+counts): count_taxons (krakendb.cpp:90-113) on the GPU.
-int collect_taxids(kuq_ctx *ctx) {
+// Scan the staged records for their distinct taxids (+counts): count_taxons (krakendb.cpp:90-113) on the GPU.  The
+// device hash (keys, dense ids to be filled, counts) and the sorted taxids / counts go to the caller's fields.
+int collect_taxids(kuq_ctx *ctx, const uint8_t *pairs, uint64_t key_ct, uint32_t *&d_keys, uint32_t *&d_dense,
+                   unsigned long long *&d_counts, uint32_t &tx_cap, std::vector<uint32_t> &taxids, std::vector<uint64_t> &tcounts) {
   uint32_t cap = 1u << 16;
   for (;;) {
-    cudaFree(ctx->d_tx_keys); cudaFree(ctx->d_tx_counts); cudaFree(ctx->d_tx_dense);
-    ctx->d_tx_keys = ctx->d_tx_dense = nullptr; ctx->d_tx_counts = nullptr;
-    CU(dmalloc(&ctx->d_tx_keys, cap));
-    CU(dmalloc(&ctx->d_tx_counts, cap));
-    CU(dmalloc(&ctx->d_tx_dense, cap));
-    CU(cudaMemsetAsync(ctx->d_tx_keys, 0, cap * 4ull, ctx->aux));
-    CU(cudaMemsetAsync(ctx->d_tx_counts, 0, cap * 8ull, ctx->aux));
+    cudaFree(d_keys); cudaFree(d_counts); cudaFree(d_dense);
+    d_keys = d_dense = nullptr; d_counts = nullptr;
+    CU(dmalloc(&d_keys, cap));
+    CU(dmalloc(&d_counts, cap));
+    CU(dmalloc(&d_dense, cap));
+    CU(cudaMemsetAsync(d_keys, 0, cap * 4ull, ctx->aux));
+    CU(cudaMemsetAsync(d_counts, 0, cap * 8ull, ctx->aux));
     uint32_t *d_over;
     CU(dmalloc(&d_over, 1));
     CU(cudaMemsetAsync(d_over, 0, 4, ctx->aux));
-    launch_collect_taxids(ctx->d_pairs, ctx->key_ct, ctx->d_tx_keys, ctx->d_tx_counts, cap - 1, d_over, ctx->aux);
+    launch_collect_taxids(pairs, key_ct, d_keys, d_counts, cap - 1, d_over, ctx->aux);
     ctx->launches++;
     uint32_t over = 0;
     CU(cudaMemcpyAsync(&over, d_over, 4, cudaMemcpyDeviceToHost, ctx->aux));
@@ -360,8 +380,8 @@ int collect_taxids(kuq_ctx *ctx) {
     if (over == 2) return fail(ctx, KUQ_E_DB_FORMAT, "taxid 0xFFFFFFFF is reserved");
     std::vector<uint32_t> keys(cap);
     std::vector<unsigned long long> counts(cap);
-    CU(cudaMemcpy(keys.data(), ctx->d_tx_keys, cap * 4ull, cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(counts.data(), ctx->d_tx_counts, cap * 8ull, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(keys.data(), d_keys, cap * 4ull, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(counts.data(), d_counts, cap * 8ull, cudaMemcpyDeviceToHost));
     uint64_t used = 0;
     for (uint32_t i = 0; i < cap; i++) used += keys[i] != 0;
     if (over == 1 || used * 2 > cap) {            // too full: the probe chains got long or overflowed
@@ -373,11 +393,15 @@ int collect_taxids(kuq_ctx *ctx) {
     v.reserve(used);
     for (uint32_t i = 0; i < cap; i++) if (keys[i]) v.emplace_back(keys[i] - 1, counts[i]);
     std::sort(v.begin(), v.end());
-    ctx->db_taxids.clear(); ctx->db_taxid_counts.clear();
-    for (auto &pr : v) { ctx->db_taxids.push_back(pr.first); ctx->db_taxid_counts.push_back(pr.second); }
-    ctx->tx_cap = cap;
+    taxids.clear(); tcounts.clear();
+    for (auto &pr : v) { taxids.push_back(pr.first); tcounts.push_back(pr.second); }
+    tx_cap = cap;
     return KUQ_OK;
   }
+}
+int collect_taxids(kuq_ctx *ctx) {
+  return collect_taxids(ctx, ctx->d_pairs, ctx->key_ct, ctx->d_tx_keys, ctx->d_tx_dense, ctx->d_tx_counts, ctx->tx_cap,
+                        ctx->db_taxids, ctx->db_taxid_counts);
 }
 
 // Dense numbering: 0 = "no taxon", 1 = taxid 1 (the reference's hard-wired root, krakenutil.cpp:96,106), then every
@@ -388,6 +412,8 @@ int finalize(kuq_ctx *ctx) {
   if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
   if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "no taxonomy set");
   std::vector<uint32_t> dbt = ctx->universe.empty() ? ctx->db_taxids : ctx->universe;
+  if (ctx->universe.empty())
+    for (auto &e : ctx->more) dbt.insert(dbt.end(), e.taxids.begin(), e.taxids.end());
   std::sort(dbt.begin(), dbt.end());
   dbt.erase(std::unique(dbt.begin(), dbt.end()), dbt.end());
   std::vector<uint32_t> &raw = ctx->raw_of_dense;
@@ -406,7 +432,9 @@ int finalize(kuq_ctx *ctx) {
   for (uint32_t t : rest) { ctx->dense_of_raw[t] = (uint32_t)raw.size(); raw.push_back(t); }
   ctx->n_taxa = (uint32_t)raw.size();
   // staged taxids must all be numbered
-  for (uint32_t t : ctx->db_taxids)
+  std::vector<uint32_t> staged = ctx->db_taxids;
+  for (auto &e : ctx->more) staged.insert(staged.end(), e.taxids.begin(), e.taxids.end());
+  for (uint32_t t : staged)
     if (!ctx->dense_of_raw.count(t) || ctx->dense_of_raw[t] >= ctx->n_sketch)
       return fail(ctx, KUQ_E_STATE, "staged records hold taxid %u that is not in the declared taxid universe", t);
 
@@ -473,31 +501,43 @@ int finalize(kuq_ctx *ctx) {
   return KUQ_OK;
 }
 
-// rewrite the staged record values taxid → dense id (once per staged range)
-int remap_db(kuq_ctx *ctx) {
-  if (ctx->db_remapped) return KUQ_OK;
-  std::vector<uint32_t> keys(ctx->tx_cap), dense(ctx->tx_cap, 0);
-  CU(cudaMemcpy(keys.data(), ctx->d_tx_keys, ctx->tx_cap * 4ull, cudaMemcpyDeviceToHost));
-  for (uint32_t i = 0; i < ctx->tx_cap; i++)
+// rewrite the staged record values taxid → dense id (once per staged range or appended database)
+int remap_values(kuq_ctx *ctx, uint8_t *pairs, uint64_t key_ct, const uint32_t *d_keys, uint32_t *d_dense, uint32_t tx_cap) {
+  std::vector<uint32_t> keys(tx_cap), dense(tx_cap, 0);
+  CU(cudaMemcpy(keys.data(), d_keys, tx_cap * 4ull, cudaMemcpyDeviceToHost));
+  for (uint32_t i = 0; i < tx_cap; i++)
     if (keys[i]) {
       auto it = ctx->dense_of_raw.find(keys[i] - 1);
       if (it == ctx->dense_of_raw.end() || it->second >= ctx->n_sketch)
         return fail(ctx, KUQ_E_STATE, "staged records hold taxid %u outside the numbered universe", keys[i] - 1);
       dense[i] = it->second;
     }
-  CU(cudaMemcpy(ctx->d_tx_dense, dense.data(), ctx->tx_cap * 4ull, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(d_dense, dense.data(), tx_cap * 4ull, cudaMemcpyHostToDevice));
   uint32_t *d_missing;
   CU(dmalloc(&d_missing, 1));
   CU(cudaMemset(d_missing, 0, 4));
-  launch_remap_values(ctx->d_pairs, ctx->key_ct, ctx->d_tx_keys, ctx->d_tx_dense, ctx->tx_cap - 1, d_missing,
-                      ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), ctx->aux);
+  launch_remap_values(pairs, key_ct, d_keys, d_dense, tx_cap - 1, d_missing, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1),
+                      ctx->aux);
   ctx->launches++;
   uint32_t missing = 0;
   CU(cudaMemcpyAsync(&missing, d_missing, 4, cudaMemcpyDeviceToHost, ctx->aux));
   CU(cudaStreamSynchronize(ctx->aux));
   cudaFree(d_missing);
   if (missing) return fail(ctx, KUQ_E_STATE, "internal: a record value was missing from the taxid table");
-  ctx->db_remapped = true;
+  return KUQ_OK;
+}
+int remap_db(kuq_ctx *ctx) {
+  if (!ctx->db_remapped) {
+    int rc = remap_values(ctx, ctx->d_pairs, ctx->key_ct, ctx->d_tx_keys, ctx->d_tx_dense, ctx->tx_cap);
+    if (rc) return rc;
+    ctx->db_remapped = true;
+  }
+  for (auto &e : ctx->more) {
+    if (e.remapped) continue;
+    int rc = remap_values(ctx, e.d_pairs, e.key_ct, e.d_tx_keys, e.d_tx_dense, e.tx_cap);
+    if (rc) return rc;
+    e.remapped = true;
+  }
   return KUQ_OK;
 }
 
@@ -761,19 +801,26 @@ void set_unit_ptrs(Params &p, Slot &s) {
   p.units.direct_rows = s.u_direct_rows;
 }
 
+DbView db_view(const kuq_ctx *ctx, const uint8_t *pairs, const uint64_t *offsets, uint64_t rec_base, uint64_t bin_lo,
+                uint64_t bin_hi, uint32_t nt, uint32_t idx_type) {
+  DbView v;
+  v.pairs = pairs;
+  v.offsets = offsets;
+  v.rec_base = rec_base;
+  v.key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
+  v.bin_lo = (uint32_t)bin_lo;
+  v.bin_hi = (uint32_t)bin_hi;
+  v.k = ctx->k;
+  v.nt = nt;
+  v.xor_mask = (uint32_t)((idx_type == 1 ? 0ull : INDEX2_XOR_MASK) & ((1ull << (2 * nt)) - 1));
+  v.n_mini = ctx->k - nt + 1;
+  return v;
+}
+
 void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const uint64_t *d_offsets,
                  const uint32_t *d_unit, uint32_t n_reads, uint32_t flags) {
   memset(&p, 0, sizeof p);
-  p.db.pairs = ctx->d_pairs;
-  p.db.offsets = ctx->d_offsets;
-  p.db.rec_base = ctx->rec_base;
-  p.db.key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
-  p.db.bin_lo = (uint32_t)ctx->bin_lo;
-  p.db.bin_hi = (uint32_t)ctx->bin_hi;
-  p.db.k = ctx->k;
-  p.db.nt = ctx->nt;
-  p.db.xor_mask = (uint32_t)((ctx->idx_type == 1 ? 0ull : INDEX2_XOR_MASK) & ((1ull << (2 * ctx->nt)) - 1));
-  p.db.n_mini = ctx->k - ctx->nt + 1;
+  p.db = db_view(ctx, ctx->d_pairs, ctx->d_offsets, ctx->rec_base, ctx->bin_lo, ctx->bin_hi, ctx->nt, ctx->idx_type);
   p.tax.parent = ctx->d_parent;
   p.tax.depth = ctx->d_depth;
   p.tax.raw = ctx->d_raw;
@@ -822,8 +869,43 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   set_unit_ptrs(p, s);
 }
 
+// The in-order lookup over every staged database (kuq_stage_db_append) into p0.codes_dense: one launch per run of
+// consecutive databases with the same (nt, index type), at most MAX_DBS per launch; runs after the first fill only the
+// windows no earlier run answered, and k_scan runs again where the window parameters change.
+int launch_multi_lookup(kuq_ctx *ctx, Slot &s, const Params &p0, uint32_t only_hits) {
+  std::vector<DbView> v{p0.db};
+  for (auto &e : ctx->more) v.push_back(db_view(ctx, e.d_pairs, e.d_offsets, 0, 0, 1ull << (2 * e.nt), e.nt, e.idx_type));
+  const DbView *scanned = nullptr;
+  for (size_t i = 0; i < v.size();) {
+    Params q = p0;
+    q.db = v[i];
+    q.n_dbs = 0;
+    while (i < v.size() && q.n_dbs < MAX_DBS && v[i].nt == q.db.nt && v[i].xor_mask == q.db.xor_mask) q.dbs[q.n_dbs++] = v[i++];
+    q.only_hits = scanned ? KUQ_LOOKUP_FILL_EMPTY : only_hits;
+    const bool scan = !scanned || scanned->nt != q.db.nt || scanned->xor_mask != q.db.xor_mask;
+    if (scan) CU(cudaMemsetAsync(q.chunk_counter, 0, 4, s.stream));
+    ctx->launches += launch_lookup_multi(q, ctx->n_sm, s.stream, scan);
+    scanned = &v[i - 1];
+  }
+  return KUQ_OK;
+}
+
 int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p) {
   if (ctx->lca_mode) return fail(ctx, KUQ_E_STATE, "this context built a database (kuq_set_lcas_batch): stage it anew to classify");
+  // several databases (or a fill-empty lookup): the in-order lookup, then — for a classification — the resolve half
+  // over the slot's merged codes
+  const bool multi = (!ctx->more.empty() && mode != MODE_RESOLVE) || (mode == MODE_LOOKUP && p.only_hits == KUQ_LOOKUP_FILL_EMPTY);
+  if (multi && (p.n_peers || ctx->shard_counting))
+    return fail(ctx, KUQ_E_STATE, "shard counting and peer lookups take one database");
+  uint32_t *multi_out = p.codes_dense;
+  const uint32_t multi_only_hits = mode == MODE_LOOKUP ? p.only_hits : 0;
+  if (multi && mode == MODE_FUSED) {
+    // the merged codes live in the slot's output-code buffer: the resolve half reads them (codes_in) before k_resolve
+    // writes its per-window taxids there
+    multi_out = s.d_codes;
+    p.codes_in = s.d_codes;
+    mode = MODE_RESOLVE;
+  }
   ctx->snap_valid = false;
   p.flags |= ctx->extra_flags;
   if (mode == MODE_LOOKUP && ctx->mark_zero_hits) p.flags |= 16u;
@@ -868,7 +950,14 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p) {
   CU(cudaEventRecord(s.ev_k0, s.stream));
   CU(cudaEventRecord(s.ev_stage[0], s.stream));
   CU(cudaEventRecord(s.ev_stage[1], s.stream));
-  if (p.n_reads) ctx->launches += launch_classify(mode, p, ctx->n_sm, s.stream, s.ev_stage);
+  if (p.n_reads && multi) {
+    Params q = p;
+    q.codes_dense = multi_out;
+    int mrc = launch_multi_lookup(ctx, s, q, multi_only_hits);
+    if (mrc) return mrc;
+    if (mode != MODE_LOOKUP) CU(cudaMemsetAsync(p.chunk_counter, 0, 4, s.stream));   // k_scan of the resolve half
+  }
+  if (p.n_reads && !(multi && mode == MODE_LOOKUP)) ctx->launches += launch_classify(mode, p, ctx->n_sm, s.stream, s.ev_stage);
   // the fused path flags the records of its counted hits (k_lookup); quick / exact runs go through the other halves
   if (p.n_reads && mode == MODE_FUSED && !(p.flags & 4u) && ctx->cfg.hll_mode <= KUQ_HLL_CHUNKED &&
       !(ctx->quick_min && ctx->quick_stop))
@@ -1005,10 +1094,15 @@ void *kuq_host_alloc(uint64_t bytes) {
 void kuq_host_free(void *p) { if (p) cudaFreeHost(p); }
 
 // ---- database -------------------------------------------------------------------------------------------------
-int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes,
-                 uint64_t bin_lo, uint64_t bin_hi) {
-  if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
-  CU(cudaSetDevice(ctx->device));
+namespace {
+struct DbFile {                  // a validated database.kdb + index image
+  const uint8_t *records;        // first record
+  uint64_t key_ct, pair_sz;
+  uint32_t k, nt, idx_type;
+  const uint64_t *offsets;       // 4^nt + 1 cumulative record offsets
+};
+
+int parse_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes, DbFile &f) {
   const uint8_t *p = (const uint8_t *)kdb_image;
   if (kdb_bytes < 56 || memcmp(p, "JFLISTDN", 8) != 0)                     // krakendb.cpp:32,67-68
     return fail(ctx, KUQ_E_DB_FORMAT, "database in improper format");
@@ -1035,33 +1129,25 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   if (nt < 1 || nt > 15 || nt > k) return fail(ctx, KUQ_E_DB_FORMAT, "index minimizer length %u out of range", nt);
   uint64_t n_bins = 1ull << (2 * nt);
   if (idx_bytes < 8 + 8 * (n_bins + 1)) return fail(ctx, KUQ_E_DB_FORMAT, "index file truncated");
-  const uint64_t *offsets = (const uint64_t *)(q + 8);
-  if (bin_hi == 0 || bin_hi > n_bins) bin_hi = n_bins;
-  if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
-  uint64_t rec_lo = offsets[bin_lo], rec_hi = offsets[bin_hi];
-  if (rec_hi < rec_lo || rec_hi > key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
-  // taxonomy numbering survives a re-stage (chunked mode) as long as the new range only holds numbered taxids; the
-  // sparse-tier keys of the records leave with them into the set
-  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
-  stream_close(ctx);
-  free_db(ctx);
-  ctx->k = k; ctx->nt = nt; ctx->idx_type = idx_type;
-  ctx->bin_lo = bin_lo; ctx->bin_hi = bin_hi;
-  ctx->rec_base = rec_lo;
-  ctx->key_ct = rec_hi - rec_lo;
-  ctx->db_owned = true;
-  CU(cudaMalloc((void **)&ctx->d_pairs, ctx->key_ct * 12 + SLACK));
-  CU(dmalloc(&ctx->d_offsets_owned, bin_hi - bin_lo + 1));
-  ctx->d_offsets = ctx->d_offsets_owned;
-  // bulk H2D through pinned bounce buffers (kuq_bounce.cuh) on the aux stream.  Records shorter than 12 bytes (k <= 28)
-  // travel as they are in the file: each piece lands in one bounded device buffer and k_widen_records writes it into
-  // d_pairs in the 12-byte layout, behind the copy on the same stream.
+  f.records = p + header;
+  f.key_ct = key_ct; f.pair_sz = pair_sz;
+  f.k = k; f.nt = nt; f.idx_type = idx_type;
+  f.offsets = (const uint64_t *)(q + 8);
+  return KUQ_OK;
+}
+
+// records [offsets[bin_lo], offsets[bin_hi]) of f → d_pairs (12-byte layout), offsets [bin_lo, bin_hi] → d_offsets.
+// Bulk H2D through pinned bounce buffers (kuq_bounce.cuh) on the aux stream.  Records shorter than 12 bytes (k <= 28)
+// travel as they are in the file: each piece lands in one bounded device buffer and k_widen_records writes it into
+// d_pairs in the 12-byte layout, behind the copy on the same stream.
+int upload_db(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi, uint8_t *d_pairs, uint64_t *d_offsets) {
+  const uint64_t pair_sz = f.pair_sz, rec_lo = f.offsets[bin_lo], n_rec = f.offsets[bin_hi] - rec_lo;
   {
     PinnedBounce bounce;
     CU(bounce.init());
     uint8_t *d_land = nullptr;
     const uint64_t land_rec = pair_sz == 12 ? 0 : std::min(landing_records(pair_sz), PinnedBounce::CH / pair_sz);
-    if (land_rec && ctx->key_ct) CU(cudaMalloc((void **)&d_land, land_rec * pair_sz + SLACK));
+    if (land_rec && n_rec) CU(cudaMalloc((void **)&d_land, land_rec * pair_sz + SLACK));
     // rec_sz = 0: bytes are copied to d_dst as they are; else they are records of rec_sz bytes, widened into d_dst
     auto piece_copy = [&](uint8_t *d_dst, const uint8_t *h_src, uint64_t bytes, uint64_t rec_sz) -> int {
       if (!rec_sz) {
@@ -1078,16 +1164,75 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
       CU(cudaStreamSynchronize(ctx->aux));
       return KUQ_OK;
     };
-    const uint8_t *src = p + header + rec_lo * pair_sz;
-    int crc = piece_copy(ctx->d_pairs, src, ctx->key_ct * pair_sz, pair_sz == 12 ? 0 : pair_sz);
-    if (!crc) crc = piece_copy(reinterpret_cast<uint8_t *>(ctx->d_offsets_owned), reinterpret_cast<const uint8_t *>(offsets + bin_lo),
+    int crc = piece_copy(d_pairs, f.records + rec_lo * pair_sz, n_rec * pair_sz, pair_sz == 12 ? 0 : pair_sz);
+    if (!crc) crc = piece_copy(reinterpret_cast<uint8_t *>(d_offsets), reinterpret_cast<const uint8_t *>(f.offsets + bin_lo),
                                (bin_hi - bin_lo + 1) * 8, 0);
     cudaFree(d_land);
     if (crc) return crc;
   }
-  ctx->db_staged = true;
-  int rc = collect_taxids(ctx);
+  return KUQ_OK;
+}
+}  // namespace
+
+int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes,
+                 uint64_t bin_lo, uint64_t bin_hi) {
+  if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
+  CU(cudaSetDevice(ctx->device));
+  DbFile f;
+  int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
   if (rc) return rc;
+  const uint64_t n_bins = 1ull << (2 * f.nt);
+  if (bin_hi == 0 || bin_hi > n_bins) bin_hi = n_bins;
+  if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
+  uint64_t rec_lo = f.offsets[bin_lo], rec_hi = f.offsets[bin_hi];
+  if (rec_hi < rec_lo || rec_hi > f.key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
+  // taxonomy numbering survives a re-stage (chunked mode) as long as the new range only holds numbered taxids; the
+  // sparse-tier keys of the records leave with them into the set
+  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
+  stream_close(ctx);
+  free_db(ctx);
+  ctx->k = f.k; ctx->nt = f.nt; ctx->idx_type = f.idx_type;
+  ctx->bin_lo = bin_lo; ctx->bin_hi = bin_hi;
+  ctx->rec_base = rec_lo;
+  ctx->key_ct = rec_hi - rec_lo;
+  ctx->db_owned = true;
+  CU(cudaMalloc((void **)&ctx->d_pairs, ctx->key_ct * 12 + SLACK));
+  CU(dmalloc(&ctx->d_offsets_owned, bin_hi - bin_lo + 1));
+  ctx->d_offsets = ctx->d_offsets_owned;
+  rc = upload_db(ctx, f, bin_lo, bin_hi, ctx->d_pairs, ctx->d_offsets_owned);
+  if (rc) return rc;
+  ctx->db_staged = true;
+  rc = collect_taxids(ctx);
+  if (rc) return rc;
+  if (ctx->finalized) return remap_db(ctx);
+  return KUQ_OK;
+}
+
+int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes) {
+  if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
+  if (!ctx->db_staged || ctx->stream_open) return kuq_stage_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, 0, 0);
+  CU(cudaSetDevice(ctx->device));
+  DbFile f;
+  int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
+  if (rc) return rc;
+  if (f.k != ctx->k) return fail(ctx, KUQ_E_INVALID_ARG, "the databases differ in k: %u vs %u", ctx->k, f.k);
+  const uint64_t n_bins = 1ull << (2 * f.nt);
+  if (f.offsets[n_bins] != f.key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
+  ctx->more.emplace_back();
+  kuq_ctx::ExtraDb &e = ctx->more.back();
+  e.key_ct = f.key_ct; e.nt = f.nt; e.idx_type = f.idx_type;
+  auto drop = [&](int code) { ctx->more.pop_back(); return code; };
+  if (dmalloc(&e.d_pairs, e.key_ct * 12 + SLACK) != cudaSuccess || dmalloc(&e.d_offsets, n_bins + 1) != cudaSuccess) {
+    (void)cudaGetLastError();
+    cudaFree(e.d_pairs); cudaFree(e.d_offsets);
+    return drop(fail(ctx, KUQ_E_NOMEM, "no room for database %zu (%llu records)", ctx->more.size() + 1, (unsigned long long)e.key_ct));
+  }
+  rc = upload_db(ctx, f, 0, n_bins, e.d_pairs, e.d_offsets);
+  if (!rc) rc = collect_taxids(ctx, e.d_pairs, e.key_ct, e.d_tx_keys, e.d_tx_dense, e.d_tx_counts, e.tx_cap, e.taxids, e.counts);
+  if (rc) {
+    cudaFree(e.d_pairs); cudaFree(e.d_offsets); cudaFree(e.d_tx_keys); cudaFree(e.d_tx_dense); cudaFree(e.d_tx_counts);
+    return drop(rc);
+  }
   if (ctx->finalized) return remap_db(ctx);
   return KUQ_OK;
 }
@@ -1122,12 +1267,22 @@ int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uin
 int kuq_db_taxids(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n) {
   if (!ctx || !n) return KUQ_E_INVALID_ARG;
   if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
-  *n = (uint32_t)ctx->db_taxids.size();
+  std::vector<std::pair<uint32_t, uint64_t>> all;          // over the appended databases too (counts summed)
+  for (size_t i = 0; i < ctx->db_taxids.size(); i++) all.emplace_back(ctx->db_taxids[i], ctx->db_taxid_counts[i]);
+  for (auto &e : ctx->more)
+    for (size_t i = 0; i < e.taxids.size(); i++) all.emplace_back(e.taxids[i], e.counts[i]);
+  std::sort(all.begin(), all.end());
+  std::vector<std::pair<uint32_t, uint64_t>> u;
+  for (auto &pr : all) {
+    if (!u.empty() && u.back().first == pr.first) u.back().second += pr.second;
+    else u.push_back(pr);
+  }
+  *n = (uint32_t)u.size();
   if (cap == 0) return KUQ_OK;
   if (cap < *n) return fail(ctx, KUQ_E_CAPACITY, "need room for %u taxids", *n);
   for (uint32_t i = 0; i < *n; i++) {
-    if (taxid) taxid[i] = ctx->db_taxids[i];
-    if (count) count[i] = ctx->db_taxid_counts[i];
+    if (taxid) taxid[i] = u[i].first;
+    if (count) count[i] = u[i].second;
   }
   return KUQ_OK;
 }
@@ -2169,6 +2324,7 @@ int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, ui
   if (ctx->universe.empty()) return fail(ctx, KUQ_E_STATE, "declare the taxids of the whole database first (kuq_set_db_taxid_universe)");
   if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "no taxonomy set");
   CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));   // a re-open frees the buffers they may still read
   { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
   free_db(ctx);
   stream_close(ctx);

@@ -629,12 +629,69 @@ __device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint3
   }
 }
 
+// Several databases (classify -d A -d B, classify.cpp:928-936): the window asks p.dbs[0], p.dbs[1], ... in order and
+// the first database that holds the key answers — a stored taxon 0 too, written as FOUND_ZERO so that it also ends the
+// search of later launches.  Same bin search as lookup_window (kept apart so that the fused kernels stay as they are).
+// only_hits 1 writes hits only; 2 (fill empty) skips a window an earlier launch coded already, before any index fetch.
+__device__ __forceinline__ bool search_bin(const DbView &db, uint32_t bin, uint64_t canon, uint32_t &value) {
+  const uint64_t *o = db.offsets + (bin - db.bin_lo);
+  const uint64_t o0 = __ldg(o), o1 = __ldg(o + 1);
+  uint64_t lo = o0 - db.rec_base;
+  uint32_t n = (uint32_t)(o1 - o0);
+  while (n > (uint32_t)SEARCH_WINDOW) {
+    const uint32_t q = n >> 2;
+    const uint64_t k1 = load_key(db.pairs, lo + q, db.key_mask);
+    const uint64_t k2 = load_key(db.pairs, lo + 2 * q, db.key_mask);
+    const uint64_t k3 = load_key(db.pairs, lo + 3 * q, db.key_mask);
+    const uint32_t c = (canon >= k1 ? 1u : 0u) + (canon >= k2 ? 1u : 0u) + (canon >= k3 ? 1u : 0u);
+    lo += (uint64_t)c * q;
+    n = (c == 3u) ? n - 3 * q : q;
+  }
+  const uint32_t *b = reinterpret_cast<const uint32_t *>(db.pairs + lo * 12);
+  const uint32_t clo = (uint32_t)canon, chi = (uint32_t)(canon >> 32), hi_mask = (uint32_t)(db.key_mask >> 32);
+  for (uint32_t t = 0; t < n; t++) {
+    if (__ldg(b + 3 * t) != clo || (__ldg(b + 3 * t + 1) & hi_mask) != chi) continue;
+    value = __ldg(b + 3 * t + 2);
+    return true;
+  }
+  return false;
+}
+
+__device__ __forceinline__ void lookup_window_multi(const Params &p, uint64_t g, uint32_t bin, uint64_t canon) {
+  if (bin == BIN_NONE) return;
+  if (p.only_hits == 2u && p.codes_dense[g] != 0) return;
+  if (bin == BIN_AMBIG) {
+    if (!p.only_hits) p.codes_dense[g] = AMBIG;
+    return;
+  }
+  uint32_t taxon = 0;
+#pragma unroll
+  for (uint32_t d = 0; d < MAX_DBS; d++) {            // constant indices: the views stay in the parameter bank
+    if (d >= p.n_dbs) break;
+    const DbView &db = p.dbs[d];
+    if (bin < db.bin_lo || bin >= db.bin_hi) continue;
+    if (p.flags & 8u) {                                // one fetch per database asked
+      const uint64_t *o = db.offsets + (bin - db.bin_lo);
+      const uint32_t n = (uint32_t)(__ldg(o + 1) - __ldg(o));
+      atomicAdd(p.stats, 1ull);
+      atomicAdd(p.stats + 1, (unsigned long long)(n ? 32 - __clz(n) : 0));
+    }
+    uint32_t v;
+    if (search_bin(db, bin, canon, v)) {
+      taxon = v ? v : FOUND_ZERO;
+      break;
+    }
+  }
+  if (!p.only_hits || taxon != 0) p.codes_dense[g] = taxon;
+}
+
 // MODE_FUSED computes its windows from the packed blocks (FAST: k = 31, m = 15, see window_bin) instead of reading
 // 12 bytes of scratch per position: a warp takes 32 consecutive positions (one block) at a time, from a contiguous
 // range of blocks, so block j + 1 of one step is block j of the next.  Side positions (reads with '\n' / '\r') read
 // their windows from scratch.  The other modes read k_scan's scratch.
 // The generic-k fused path needs a few registers more than 32 (6 CTAs per SM, 40 registers, no spills).
-template <int MODE, bool LEAN, bool FAST = false>
+// MULTI: MODE_LOOKUP over p.dbs (lookup_window_multi).
+template <int MODE, bool LEAN, bool FAST = false, bool MULTI = false>
 __global__ void __launch_bounds__(256, (MODE == MODE_FUSED && !FAST) ? 6 : 8) k_lookup(const __grid_constant__ Params p) {
   // only the text of this call's reads (the scratch beyond it may hold windows of an earlier call on the slot)
   const uint64_t g_begin = p.offsets[0], g_end = p.offsets[p.n_reads];
@@ -671,7 +728,8 @@ __global__ void __launch_bounds__(256, (MODE == MODE_FUSED && !FAST) ? 6 : 8) k_
       const uint32_t bin = bin_n;
       const uint64_t canon = canon_n;
       if (g + stride < g_end) { bin_n = __ldg(p.bins + g + stride); canon_n = __ldg(p.canon + g + stride); }
-      lookup_window<MODE, LEAN>(p, g, bin, canon);
+      if constexpr (MULTI) lookup_window_multi(p, g, bin, canon);
+      else lookup_window<MODE, LEAN>(p, g, bin, canon);
     }
   }
 }
@@ -1567,6 +1625,14 @@ int launch_lookup_only(const Params &p, int n_sm, cudaStream_t stream, int fused
   if (fused) launch_lookup<MODE_FUSED>(p, lgrid, stream, lean != 0);
   else launch_lookup<MODE_LOOKUP>(p, lgrid, stream, lean != 0);
   return 1;
+}
+
+int launch_lookup_multi(const Params &p, int n_sm, cudaStream_t stream, bool scan) {
+  if (p.n_reads == 0) return 0;
+  const int launches = scan ? launch_scan_only(p, n_sm, stream) : 0;
+  const int lgrid = (int)min((uint64_t)n_sm * 8 * 8, (p.total_bases + 255) / 256);
+  k_lookup<MODE_LOOKUP, false, false, true><<<lgrid, 256, 0, stream>>>(p);
+  return launches + 1;
 }
 
 // scan the pieces, then fold their taxids into the record values; returns #kernels launched

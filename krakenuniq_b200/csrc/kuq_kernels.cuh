@@ -49,6 +49,7 @@ constexpr uint32_t SEEN_BIT = 0x80000000u;
 // Only one record per (taxon, code) carries it — the primary of its collision group (kuq_api.cu, build_collisions).
 constexpr uint32_t KEPT_BIT = 0x40000000u;
 constexpr int SEARCH_WINDOW = 8;           // records scanned linearly once the bisection window is this small
+constexpr uint32_t MAX_DBS = 8;            // databases one launch of the in-order lookup asks (Params::dbs)
 
 enum Mode { MODE_FUSED = 0, MODE_LOOKUP = 1, MODE_RESOLVE = 2 };
 
@@ -230,6 +231,11 @@ struct Params {
   uint32_t n_peers;
   uint32_t *peer_codes[8];
   uint64_t peer_bounds[9];
+  // MODE_LOOKUP over several databases (launch_lookup_multi): dbs[0, n_dbs) of one (k, nt, index type) are asked in
+  // order; db = dbs[0] gives k_scan its window parameters.  only_hits 2 (fill empty): windows coded non-zero already are
+  // skipped before any index fetch.
+  DbView dbs[MAX_DBS];
+  uint32_t n_dbs;
   unsigned long long *stats;    // flag 8: [0] += looked-up windows, [1] += sum of ceil(log2(bin size + 1))
   // per-taxon state
   uint8_t *regs;                // [n_sketch][4096]
@@ -267,6 +273,9 @@ int device_sm_count();
 int launch_set_lcas(const Params &p, int n_sm, cudaStream_t stream);
 int launch_scan_only(const Params &p, int n_sm, cudaStream_t stream);
 int launch_lookup_only(const Params &p, int n_sm, cudaStream_t stream, int fused, int lean);
+// several databases: [k_scan with p.db's parameters when `scan`] + the in-order lookup over p.dbs into p.codes_dense;
+// p.chunk_counter must be 0 when `scan`.  Returns #kernels launched.
+int launch_lookup_multi(const Params &p, int n_sm, cudaStream_t stream, bool scan);
 // db_sort on the device (kuq_dbbuild.cu): returns a KUQ_* code, *n_passes = per-range sorts (1 = in one piece)
 int dbsort_device(const uint8_t *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
                   uint8_t *kdb_out, uint8_t *idx_out, uint32_t *n_passes, char *err, size_t err_cap);
