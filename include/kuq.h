@@ -165,8 +165,18 @@ int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uin
  * resolve half.  Results take the same form as on one database; the sparse HLL tier is filled by the resolve half (no
  * record flags).  kuq_lookup_batch / kuq_lookup_device return the merged first-hit codes, a stored zero always as
  * KUQ_CODE_FOUND_ZERO.  kuq_db_taxids reports the union over the staged databases (record counts summed).  Shard
- * counting and kuq_lookup_device_peers are refused (KUQ_E_STATE). */
+ * counting and kuq_lookup_device_peers are refused (KUQ_E_STATE); kuq_lookup_device_peers_run shards them.
+ * kuq_stage_db_append = kuq_stage_db_append_range(..., 0, 0). */
 int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes);
+/* The same for the minimizer bins [bin_lo, bin_hi) of the database: (0, 0) = the whole database, bin_hi = 0 = to the
+ * end, bin_lo == bin_hi != 0 = an empty slice (a GPU that holds none of this database's bins; pass 4^nt, 4^nt for an
+ * empty slice at the start).  A range outside the 4^nt bins gives KUQ_E_INVALID_ARG and leaves the context as it was.
+ * With nothing staged yet the range becomes the first database, an empty slice included. */
+int kuq_stage_db_append_range(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image,
+                              uint64_t idx_bytes, uint64_t bin_lo, uint64_t bin_hi);
+/* Runs of the staged databases: maximal groups of consecutive databases with equal (nt, index type).  Each run is one
+ * phase of the sharded lookup (kuq_lookup_device_peers_run). */
+int kuq_db_runs(kuq_ctx *ctx, uint32_t *n_runs);
 /* Distinct taxids stored in the staged records with their record counts — what KrakenDB::count_taxons()
  * (krakendb.cpp:90-113) computes for database.kdb.counts.  Pass cap = 0 to query *n only. */
 int kuq_db_taxids(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n);
@@ -247,6 +257,28 @@ int kuq_resolve_device(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const u
 int kuq_lookup_device_peers(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets,
                             uint32_t n_reads, uint64_t total_bases, uint32_t *const *d_codes_peers,
                             const uint64_t *base_bounds, uint32_t n_peers);
+/* Several databases sharded by minimizer range over the GPUs of a node (`classify -d a -d b` when they fit the GPUs only
+ * together).  Every database of a run (kuq_db_runs) holds the same bins [cut_r[g], cut_r[g + 1]) on GPU g: one cut per
+ * run over the GPUs.  One call does one run: a window whose bin lies in this GPU's range asks the run's databases in
+ * order and the first hit — a stored zero as KUQ_CODE_FOUND_ZERO — is stored into d_codes_peers[j] of the GPU j that
+ * resolves the read (text positions [base_bounds[j], base_bounds[j + 1])).  Run 0 writes hits only; a later run first
+ * reads the owner's word (a coherent system-scope load) and skips the window when an earlier run answered it on any GPU.
+ * Sketches are the owners' business, in the resolve half, so shard counting stays refused (KUQ_E_STATE).
+ * Before the first batch every GPU gets kuq_set_db_taxid_universe(taxids of all databases over all ranges), so that all
+ * number taxa identically, and kuq_enable_peer_access to every other GPU.  Per batch, with flag arrays as for kuq_lookup_device_peers (done counters and ready counters, one per GPU):
+ *     every GPU: the batch into its HBM (all reads: every GPU looks up every window of its ranges)
+ *     for r in runs:  every GPU g:  kuq_wait_flags(ready >= step + 1)          when r == 0 (owners cleared the buffers)
+ *                                   kuq_wait_flags(done >= step * R + r)       when r > 0  (every GPU finished run r - 1)
+ *                                   kuq_lookup_device_peers_run(..., r)
+ *                                   kuq_signal_peers(done, step * R + r + 1)
+ *     every owner g:  kuq_wait_flags(done >= (step + 1) * R);  kuq_resolve_device(its share, with work-unit ids);
+ *                     clear its slice of its buffer;  kuq_signal_peers(ready, step + 3)
+ * (R = number of runs, ready starting at 2 with two id buffers alternating by step.)  Shares must hold whole work units:
+ * the per-work-unit sketch rule (KUQ_HLL_PRELOAD) decides each unit on the GPU that resolves it.  At the end, kuq_finish
+ * on every context and kuq_merge_into the first, as for replicas. */
+int kuq_lookup_device_peers_run(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets,
+                                uint32_t n_reads, uint64_t total_bases, uint32_t *const *d_codes_peers,
+                                const uint64_t *base_bounds, uint32_t n_peers, uint32_t run);
 /* Device memory that other ranks can map (cudaMalloc + CUDA IPC); handles are 64 opaque bytes. */
 void *kuq_device_alloc(kuq_ctx *ctx, uint64_t bytes);
 void kuq_device_free(kuq_ctx *ctx, void *p);

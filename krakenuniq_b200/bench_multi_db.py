@@ -8,7 +8,10 @@ substitutions, 20 % random reads).  Three runs of the executable, each timed fro
 reads' pass, without loading the databases), best of `--repeats`:
   - A alone;
   - A + B resident (their records fit the HBM budget together);
-  - A + B streamed: KUQ_HBM_BUDGET set between A alone and A + B, so the databases stream through two range buffers.
+  - A + B streamed: KUQ_HBM_BUDGET set between A alone and A + B, so the databases stream through two range buffers;
+  - A + B sharded: KUQ_FORCE_SHARDS=1 over the visible GPUs (KUQ_DEVICES), each GPU holding a minimizer range of both
+    databases.  On a one-GPU machine the GPUs are two contexts on device 0 (KUQ_DEVICES=0,0): that measures what the
+    lookup phases, the device flags and the owners' shares cost, not a multi-GPU speed-up.
 The script drives only the command line, so `--classify` can time another build of the executable (for example the
 parent commit's) on the same inputs; md5 sums of the Kraken outputs let the outputs of two builds be compared.
 Run from the repository root after `python -m krakenuniq_b200.build`:
@@ -96,8 +99,12 @@ def main():
     try:
         key_a, key_b, n_reads = make_inputs(tmp, a.records_a, a.records_b, a.reads, a.seed)
         ha, hb = hbm_bytes(tmp, "a"), hbm_bytes(tmp, "b")
+        n_gpu = torch.cuda.device_count()
+        shard_devices = ",".join(str(g) for g in range(n_gpu)) if n_gpu > 1 else "0,0"
+        shard_name = f"A+B sharded over {n_gpu} GPUs" if n_gpu > 1 else "A+B sharded (2 contexts on one GPU: phase and flag cost)"
         runs = [("A", ["a"], {}), ("A+B resident", ["a", "b"], {}),
-                ("A+B streamed", ["a", "b"], {"KUQ_HBM_BUDGET": str(ha + hb // 2)})]
+                ("A+B streamed", ["a", "b"], {"KUQ_HBM_BUDGET": str(ha + hb // 2)}),
+                (shard_name, ["a", "b"], {"KUQ_FORCE_SHARDS": "1", "KUQ_DEVICES": shard_devices})]
         for name, dbs, env in runs:
             for exe in exes:                         # builds alternate within a configuration
                 secs, md5 = [], None
@@ -114,7 +121,8 @@ def main():
                     secs.append(float(line.split("processed in ")[1].split("s")[0]))
                     with open(os.path.join(tmp, "out.kraken"), "rb") as f:
                         md5 = hashlib.md5(f.read()).hexdigest()
-                    mode = [x.strip() for x in r.stderr.splitlines() if "databases" in x and ("resident" in x or "streamed" in x)]
+                    mode = [x.strip() for x in r.stderr.splitlines()
+                            if "databases" in x and ("resident" in x or "streamed" in x or "sharded" in x)]
                 if secs:
                     print(json.dumps({"config": name, "classify": exe, "gpu": gpu, "reads": n_reads, "records_a": key_a,
                                       "records_b": key_b, "hbm_bytes": [ha, hb], "env": env, "processed_s": secs,

@@ -105,6 +105,8 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_device_count": (C.c_int, []),
         "kuq_stage_db": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint64, C.c_uint64]),
         "kuq_stage_db_append": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint64]),
+        "kuq_stage_db_append_range": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint64, C.c_uint64]),
+        "kuq_db_runs": (C.c_int, [vp, u32p]),
         "kuq_attach_db_device": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64,
                                            C.c_uint64]),
         "kuq_db_taxids": (C.c_int, [vp, u32p, u64p, C.c_uint32, u32p]),
@@ -129,6 +131,8 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_resolve_device": (C.c_int, [vp, C.c_uint32, vp, vp, C.c_uint32, C.c_uint64, vp, vp, C.c_uint32]),
         "kuq_lookup_device_peers": (C.c_int, [vp, C.c_uint32, vp, vp, C.c_uint32, C.c_uint64, C.POINTER(vp), u64p,
                                              C.c_uint32]),
+        "kuq_lookup_device_peers_run": (C.c_int, [vp, C.c_uint32, vp, vp, C.c_uint32, C.c_uint64, C.POINTER(vp), u64p,
+                                                 C.c_uint32, C.c_uint32]),
         "kuq_device_alloc": (vp, [vp, C.c_uint64]),
         "kuq_device_free": (None, [vp, vp]),
         "kuq_device_memset": (C.c_int, [vp, C.c_uint32, vp, C.c_int, C.c_uint64]),
@@ -257,6 +261,19 @@ class Classifier:
         kdb = np.ascontiguousarray(kdb).view(np.uint8) if not isinstance(kdb, np.memmap) else kdb
         idx = np.ascontiguousarray(idx).view(np.uint8) if not isinstance(idx, np.memmap) else idx
         self._ck(self.L.kuq_stage_db_append(self.h, kdb.ctypes.data, kdb.size, idx.ctypes.data, idx.size))
+
+    def stage_db_append_range(self, kdb: np.ndarray, idx: np.ndarray, bin_lo=0, bin_hi=0):
+        """minimizer bins [bin_lo, bin_hi) of one more database (kuq_stage_db_append_range): (0, 0) = all of it,
+        bin_lo == bin_hi != 0 = an empty slice"""
+        kdb = np.ascontiguousarray(kdb).view(np.uint8) if not isinstance(kdb, np.memmap) else kdb
+        idx = np.ascontiguousarray(idx).view(np.uint8) if not isinstance(idx, np.memmap) else idx
+        self._ck(self.L.kuq_stage_db_append_range(self.h, kdb.ctypes.data, kdb.size, idx.ctypes.data, idx.size,
+                                                  int(bin_lo), int(bin_hi)))
+
+    def db_runs(self):
+        n = C.c_uint32(0)
+        self._ck(self.L.kuq_db_runs(self.h, C.byref(n)))
+        return n.value
 
     def stage_db_files(self, kdb_path, idx_path, bin_lo=0, bin_hi=0):
         self.stage_db(np.memmap(kdb_path, np.uint8, "r"), np.memmap(idx_path, np.uint8, "r"), bin_lo, bin_hi)
@@ -393,6 +410,22 @@ class Classifier:
         assert len(bounds) == n + 1
         self._ck(self.L.kuq_lookup_device_peers(self.h, slot, d_bases, d_offsets, n_reads, total_bases, arr,
                                                 _p(bounds, u64p), n))
+
+    def collect_device(self, slot, offsets=None):
+        """kuq_collect_device_batch: the results of the slot's last device call, like wait()"""
+        res = BatchResult()
+        self._ck(self.L.kuq_collect_device_batch(self.h, slot, C.byref(res)))
+        return self._result(res, offsets if offsets is not None else np.zeros(2, np.uint64))
+
+    def lookup_device_peers_run(self, slot, d_bases, d_offsets, n_reads, total_bases, peer_ptrs, base_bounds, run):
+        """one run (kuq_db_runs) of the in-order lookup of databases sharded by minimizer range, hits stored into the
+        resolving GPU's buffer (kuq_lookup_device_peers_run)"""
+        n = len(peer_ptrs)
+        arr = (C.c_void_p * n)(*[C.c_void_p(int(x)) for x in peer_ptrs])
+        bounds = np.ascontiguousarray(base_bounds, np.uint64)
+        assert len(bounds) == n + 1
+        self._ck(self.L.kuq_lookup_device_peers_run(self.h, slot, d_bases, d_offsets, n_reads, total_bases, arr,
+                                                    _p(bounds, u64p), n, int(run)))
 
     def device_alloc(self, nbytes):
         p = self.L.kuq_device_alloc(self.h, nbytes)

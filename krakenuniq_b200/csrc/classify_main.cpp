@@ -1322,6 +1322,7 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     }
     for (size_t db = 0; db < n_db; db++) {
       const Plan &pl = plans[db];
+      if (pl.ranges.empty()) continue;                             // a database without records answers nothing
       if (pl.nt != open_nt || pl.idx_type != open_type) {
         // taxonomy and universe are known before the stream opens (the dense numbering is fixed there)
         if ((open_nt && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, max_rec, max_bins))
@@ -1383,24 +1384,158 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
   }
 }
 
-// ---- a database that fits the GPUs of the node together but not one of them: minimizer-range shards (SURVEY §8(e).2) ---
-// GPU g stages range g.  Every GPU scans every batch and looks up the k-mers whose minimizer it owns; each hit is stored
-// straight into the id buffer of the GPU that resolves the read (peer stores over NVLink, kuq_lookup_device_peers), which
-// also does the hit's sketch work; device flags order the phases (no host barrier between GPUs); every GPU resolves a
-// contiguous share of the batch cut at work-unit boundaries.  One process, so peer access instead of CUDA IPC.  The
-// sketches follow the chunked rule, as for any database the reference could only run with -x.
+// ---- databases that fit the GPUs of the node together but not one of them: minimizer-range shards (SURVEY §8(e).2) --
+// GPU g stages bin range g of every database (kuq_ranges.h, plan_shards).  Every GPU scans every batch and looks up the
+// k-mers whose minimizer it holds; each hit is stored straight into the id buffer of the GPU that resolves the read (peer
+// stores over NVLink); device flags order the phases (no host barrier between GPUs); every GPU resolves a contiguous
+// share of the batch.  One process, so peer access instead of CUDA IPC.
+//   One database (run_sharded): one lookup phase, and the GPU that finds a hit also does its sketch work; the sketches
+//   follow the chunked rule, as for any database the reference could only run with -x.
+//   Several databases (run_sharded_multi): one lookup phase per run of databases with equal (nt, index type); a later
+//   phase fills only the windows no earlier phase answered on any GPU.  The owners do all the sketch work in the resolve
+//   half, with the work-unit ids of the per-work-unit rule (the reference's rule for -d a -d b), so shares hold whole
+//   work units.
+// shard_loop is what both share: batches, id buffers, flags, shares, phases, resolve and output.
+static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool multi, int argc, char **argv) {
+  const int G = (int)ctxs.size();
+  const uint64_t R = n_phases;
+  vector<Batch> batches;
+  for (int i = optind; i < argc; i++) {
+    const size_t from = batches.size();
+    load_file_batches(argv[i], batches, /*unit_aligned=*/true);
+    for (size_t j = from; j < batches.size(); j++) batches[j].file = i;
+  }
+  uint64_t max_bases = 64, max_reads = 4;
+  for (auto &b : batches) { max_bases = std::max<uint64_t>(max_bases, b.bases.size()); max_reads = std::max<uint64_t>(max_reads, b.reads.size()); }
+  // per GPU and id-buffer parity: the batch, its offsets, the offsets (and unit ids) of the GPU's share, the id buffer
+  struct Dev { void *bases[2], *offs[2], *share_offs[2], *units[2], *ids[2], *flags; };
+  vector<Dev> dev(G);
+  const uint64_t id_bytes = (max_bases + 64) * 4;
+  for (int g = 0; g < G; g++) {
+    Dev &d = dev[g];
+    for (int k = 0; k < 2; k++) {
+      d.bases[k] = kuq_device_alloc(ctxs[g], max_bases + 64);
+      d.offs[k] = kuq_device_alloc(ctxs[g], (max_reads + 4) * 8);
+      d.share_offs[k] = kuq_device_alloc(ctxs[g], (max_reads + 4) * 8);
+      d.units[k] = multi ? kuq_device_alloc(ctxs[g], (max_reads + 4) * 4) : NULL;
+      d.ids[k] = kuq_device_alloc(ctxs[g], id_bytes);
+      if (!d.bases[k] || !d.offs[k] || !d.share_offs[k] || (multi && !d.units[k]) || !d.ids[k])
+        die(EX_OSERR, "device allocation for the sharded batches failed");
+      if (kuq_device_memset(ctxs[g], 0, d.ids[k], 0, id_bytes)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    }
+    d.flags = kuq_device_alloc(ctxs[g], 256);            // [0:8) done counters, [16:24) ready counters
+    if (!d.flags || kuq_device_memset(ctxs[g], 0, d.flags, 0, 256)) die(EX_OSERR, "device allocation failed");
+    const uint64_t two[8] = {2, 2, 2, 2, 2, 2, 2, 2};     // both id buffers are clean for steps 0 and 1
+    if (kuq_copy_to_device(ctxs[g], 0, (char *)d.flags + 128, two, 64) || kuq_sync_slot(ctxs[g], 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+  }
+  vector<uint32_t *> peer_ids(G);
+  vector<uint64_t *> peer_done(G), peer_ready(G);
+  // work-unit ids of the per-work-unit rule: process_file's cutting (classify.cpp:506-521), units end with their file
+  uint32_t unit_next = 0;
+  uint64_t unit_nt = 0;
+  int unit_file = -1;
+  vector<uint32_t> units;
+  uint64_t step = 0;
+  for (auto &b : batches) {
+    const size_t n = b.reads.size();
+    const int par = (int)(step & 1);
+    if (multi) {
+      if (unit_file >= 0 && b.file != unit_file) { unit_next++; unit_nt = 0; }
+      unit_file = b.file;
+      units.resize(n);
+      for (size_t i = 0; i < n; i++) {
+        units[i] = unit_next;
+        unit_nt += b.reads[i].seq_len;
+        if (unit_nt >= Work_unit_size) { unit_next++; unit_nt = 0; }
+      }
+    }
+    // shares: contiguous; with work-unit ids a share starts where a unit starts (k_unit_decide sees every read of a unit
+    // on one GPU), else anywhere (the chunked rule does not depend on units)
+    vector<size_t> first(G + 1, 0);
+    first[G] = n;
+    for (int g = 1; g < G; g++) {
+      size_t x = std::max(first[g - 1], std::min(n, (n * g / G) & ~(size_t)1));
+      while (multi && x > 0 && x < n && units[x] == units[x - 1]) x++;
+      first[g] = x;
+    }
+    vector<uint64_t> bounds(G + 1);
+    for (int g = 0; g <= G; g++) bounds[g] = b.offs[first[g]];
+    bounds[0] = 0;
+    vector<uint64_t> offs(b.offs);
+    offs.push_back(offs.back()); offs.push_back(offs.back());
+    // the batch goes to every GPU (a pageable copy may wait for the stream: everything it can wait for is queued)
+    for (int g = 0; g < G; g++) {
+      const size_t share = first[g + 1] - first[g];
+      if (kuq_copy_to_device(ctxs[g], 0, dev[g].bases[par], b.bases.data(), b.bases.size()) ||
+          kuq_device_memset(ctxs[g], 0, (char *)dev[g].bases[par] + b.bases.size(), 'N', 64) ||
+          kuq_copy_to_device(ctxs[g], 0, dev[g].offs[par], offs.data(), offs.size() * 8) ||
+          kuq_copy_to_device(ctxs[g], 0, dev[g].share_offs[par], offs.data() + first[g], (share + 3) * 8) ||
+          (multi && share && kuq_copy_to_device(ctxs[g], 0, dev[g].units[par], units.data() + first[g], share * 4)))
+        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    }
+    for (int h = 0; h < G; h++) {
+      peer_ids[h] = (uint32_t *)dev[h].ids[par];
+      peer_done[h] = (uint64_t *)dev[h].flags;
+      peer_ready[h] = (uint64_t *)((char *)dev[h].flags + 128);
+    }
+    // lookup phases with peer scatter, then the owners resolve — all stream ordered, flags between the GPUs.  Phase r
+    // starts when the owners cleared their buffers (r = 0) or every GPU finished phase r - 1, and signals done
+    // step * R + r + 1.
+    for (uint32_t r = 0; r < n_phases; r++)
+      for (int g = 0; g < G; g++) {
+        const uint64_t *wait_on = r == 0 ? (const uint64_t *)((char *)dev[g].flags + 128) : (const uint64_t *)dev[g].flags;
+        if (kuq_wait_flags(ctxs[g], 0, wait_on, (uint32_t)G, r == 0 ? step + 1 : step * R + r, 0) ||
+            (multi ? kuq_lookup_device_peers_run(ctxs[g], 0, (const char *)dev[g].bases[par], (const uint64_t *)dev[g].offs[par],
+                                                 (uint32_t)n, b.bases.size(), peer_ids.data(), bounds.data(), (uint32_t)G, r)
+                   : kuq_lookup_device_peers(ctxs[g], 0, (const char *)dev[g].bases[par], (const uint64_t *)dev[g].offs[par],
+                                             (uint32_t)n, b.bases.size(), peer_ids.data(), bounds.data(), (uint32_t)G)) ||
+            kuq_signal_peers(ctxs[g], 0, peer_done.data(), (uint32_t)G, (uint32_t)g, step * R + r + 1))
+          die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      }
+    for (int g = 0; g < G; g++) {
+      const size_t share = first[g + 1] - first[g];
+      if (kuq_wait_flags(ctxs[g], 0, (const uint64_t *)dev[g].flags, (uint32_t)G, (step + 1) * R, 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      if (share && kuq_resolve_device(ctxs[g], 0, (const char *)dev[g].bases[par], (const uint64_t *)dev[g].share_offs[par],
+                                      (uint32_t)share, b.bases.size(), (const uint32_t *)dev[g].ids[par],
+                                      multi ? (const uint32_t *)dev[g].units[par] : NULL, 0))
+        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      if (kuq_device_memset(ctxs[g], 0, (char *)dev[g].ids[par] + bounds[g] * 4, 0, (bounds[g + 1] - bounds[g]) * 4) ||
+          kuq_signal_peers(ctxs[g], 0, peer_ready.data(), (uint32_t)G, (uint32_t)g, step + 3))
+        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    }
+    // results of the shares, in read order
+    Fastq_input = b.fastq;
+    for (int g = 0; g < G; g++) {
+      const size_t share = first[g + 1] - first[g];
+      if (!share) { if (kuq_sync_slot(ctxs[g], 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g])); continue; }
+      kuq_batch_result res;
+      if (kuq_collect_device_batch(ctxs[g], 0, &res)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      emit_results(b, res, first[g], share);
+      total_classified += res.n_classified;
+    }
+    total_sequences += n;
+    total_bases += b.bases.size();
+    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
+    step++;
+  }
+  for (int g = 0; g < G; g++) {
+    if (kuq_finish(ctxs[g])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    for (int k = 0; k < 2; k++)
+      for (void *p : {dev[g].bases[k], dev[g].offs[k], dev[g].share_offs[k], dev[g].units[k], dev[g].ids[k]})
+        if (p) kuq_device_free(ctxs[g], p);
+    kuq_device_free(ctxs[g], dev[g].flags);
+  }
+}
+
+static ShardDb shard_db(const Mapped &idx) {
+  const uint8_t *q = (const uint8_t *)idx.p;
+  return ShardDb{(const uint64_t *)(q + 8), q[7], memcmp(q, "KRAKIDX", 7) == 0 ? 1u : 2u};
+}
+
 static void run_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const Mapped &idx, int argc, char **argv,
                         map<uint32_t, uint64_t> &db_counts) {
   const int G = (int)ctxs.size();
-  const uint8_t *q = (const uint8_t *)idx.p;
-  const uint32_t nt = q[7];
-  const uint64_t n_bins = 1ull << (2 * nt);
-  const uint64_t *offsets = (const uint64_t *)(q + 8);
-  const uint64_t key_ct = offsets[n_bins];
-  vector<uint64_t> cut(G + 1, 0);
-  cut[G] = n_bins;
-  for (int g = 1; g < G; g++) cut[g] = std::lower_bound(offsets, offsets + n_bins, key_ct / G * g) - offsets;
-  for (int g = 1; g <= G; g++) if (cut[g] < cut[g - 1]) cut[g] = cut[g - 1];
+  const vector<uint64_t> cut = plan_shards({shard_db(idx)}, G)[0].cut;
   cerr << "Database sharded over " << G << " GPUs by minimizer range" << endl;
   {
     vector<int> rcs(G, 0);
@@ -1425,91 +1560,55 @@ static void run_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const 
       die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
     for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
   }
-  vector<Batch> batches;
-  for (int i = optind; i < argc; i++) load_file_batches(argv[i], batches, /*unit_aligned=*/true);
-  uint64_t max_bases = 64, max_reads = 4;
-  for (auto &b : batches) { max_bases = std::max<uint64_t>(max_bases, b.bases.size()); max_reads = std::max<uint64_t>(max_reads, b.reads.size()); }
-  struct Dev { void *bases[2], *offs[2], *ids[2], *flags; };
-  vector<Dev> dev(G);
-  const uint64_t id_bytes = (max_bases + 64) * 4;
+  shard_loop(ctxs, 1, false, argc, argv);
+}
+
+// Several databases: every GPU stages, in command-line order, the bins of its range of each database's run (a range may
+// be empty); each database's records per taxid (.counts) are the growth of the staged union it causes, summed over GPUs.
+static void run_sharded_multi(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, int argc,
+                              char **argv, vector<map<uint32_t, uint64_t>> &db_counts) {
+  const int G = (int)ctxs.size();
+  const size_t n_db = kdbs.size();
+  vector<ShardDb> sd;
+  for (auto &m : idxs) sd.push_back(shard_db(m));
+  const vector<ShardRun> runs = plan_shards(sd, G);
+  fprintf(stderr, "classify: %zu databases sharded over %d GPUs by minimizer range (%zu lookup phases)\n", n_db, G, runs.size());
+  vector<vector<map<uint32_t, uint64_t>>> after(G, vector<map<uint32_t, uint64_t>>(n_db));
+  vector<int> rcs(G, 0);
+#pragma omp parallel for num_threads(G) schedule(static, 1)
+  for (int g = 0; g < G; g++)
+    for (const ShardRun &run : runs)
+      for (size_t d = run.first; d < run.end && !rcs[g]; d++) {
+        uint64_t lo = run.cut[g], hi = run.cut[g + 1];
+        if (lo == hi) lo = hi = 1ull << (2 * sd[d].nt);             // an empty slice
+        rcs[g] = kuq_stage_db_append_range(ctxs[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, lo, hi);
+        uint32_t m = 0;
+        if (!rcs[g]) rcs[g] = kuq_db_taxids(ctxs[g], NULL, NULL, 0, &m);
+        vector<uint32_t> tt(m);
+        vector<uint64_t> cc(m);
+        if (!rcs[g] && m) rcs[g] = kuq_db_taxids(ctxs[g], tt.data(), cc.data(), m, &m);
+        for (uint32_t i = 0; i < m; i++) after[g][d][tt[i]] = cc[i];
+      }
+  for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
+  set<uint32_t> all;
+  for (int g = 0; g < G; g++)
+    for (size_t d = 0; d < n_db; d++)
+      for (auto &kv : after[g][d]) {
+        const uint64_t before = d && after[g][d - 1].count(kv.first) ? after[g][d - 1][kv.first] : 0;
+        if (kv.second > before) { db_counts[d][kv.first] += kv.second - before; all.insert(kv.first); }
+      }
+  vector<uint32_t> u(all.begin(), all.end());
   for (int g = 0; g < G; g++) {
-    Dev &d = dev[g];
-    for (int k = 0; k < 2; k++) {
-      d.bases[k] = kuq_device_alloc(ctxs[g], max_bases + 64);
-      d.offs[k] = kuq_device_alloc(ctxs[g], (max_reads + 4) * 8);
-      d.ids[k] = kuq_device_alloc(ctxs[g], id_bytes);
-      if (!d.bases[k] || !d.offs[k] || !d.ids[k]) die(EX_OSERR, "device allocation for the sharded batches failed");
-      if (kuq_device_memset(ctxs[g], 0, d.ids[k], 0, id_bytes)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    }
-    d.flags = kuq_device_alloc(ctxs[g], 256);            // [0:8) done counters, [16:24) ready counters
-    if (!d.flags || kuq_device_memset(ctxs[g], 0, d.flags, 0, 256)) die(EX_OSERR, "device allocation failed");
-    const uint64_t two[8] = {2, 2, 2, 2, 2, 2, 2, 2};     // both id buffers are clean for steps 0 and 1
-    if (kuq_copy_to_device(ctxs[g], 0, (char *)d.flags + 128, two, 64) || kuq_sync_slot(ctxs[g], 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    uint32_t n_runs = 0;
+    if (kuq_db_runs(ctxs[g], &n_runs) || kuq_set_db_taxid_universe(ctxs[g], u.data(), (uint32_t)u.size()))
+      die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    if (n_runs != runs.size()) die(EX_SOFTWARE, "the library groups the databases into other lookup runs than the planner");
+    for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
   }
-  uint64_t step = 0;
-  for (auto &b : batches) {
-    const size_t n = b.reads.size();
-    const int par = (int)(step & 1);
-    // shares: contiguous, cut where a work unit ends (the chunked rule does not depend on units; even cuts keep the
-    // offset slices 16-byte aligned)
-    vector<size_t> first(G + 1, 0);
-    first[G] = n;
-    for (int g = 1; g < G; g++) first[g] = std::min(n, (n * g / G) & ~(size_t)1);
-    vector<uint64_t> bounds(G + 1);
-    for (int g = 0; g <= G; g++) bounds[g] = b.offs[first[g]];
-    bounds[0] = 0;
-    vector<uint64_t> offs(b.offs);
-    offs.push_back(offs.back()); offs.push_back(offs.back());
-    // phase 1: the batch goes to every GPU (a pageable copy may wait for the stream: everything it can wait for is queued)
-    for (int g = 0; g < G; g++) {
-      if (kuq_copy_to_device(ctxs[g], 0, dev[g].bases[par], b.bases.data(), b.bases.size()) ||
-          kuq_device_memset(ctxs[g], 0, (char *)dev[g].bases[par] + b.bases.size(), 'N', 64) ||
-          kuq_copy_to_device(ctxs[g], 0, dev[g].offs[par], offs.data(), offs.size() * 8))
-        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    }
-    // phase 2: lookups with peer scatter; phase 3: owners resolve — all stream ordered, flags between the GPUs
-    for (int g = 0; g < G; g++) {
-      vector<uint32_t *> peer_ids(G);
-      vector<uint64_t *> peer_done(G);
-      for (int h = 0; h < G; h++) { peer_ids[h] = (uint32_t *)dev[h].ids[par]; peer_done[h] = (uint64_t *)dev[h].flags; }
-      if (kuq_wait_flags(ctxs[g], 0, (const uint64_t *)((char *)dev[g].flags + 128), (uint32_t)G, step + 1, 0) ||
-          kuq_lookup_device_peers(ctxs[g], 0, (const char *)dev[g].bases[par], (const uint64_t *)dev[g].offs[par], (uint32_t)n,
-                                  b.bases.size(), peer_ids.data(), bounds.data(), (uint32_t)G) ||
-          kuq_signal_peers(ctxs[g], 0, peer_done.data(), (uint32_t)G, (uint32_t)g, step + 1))
-        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    }
-    for (int g = 0; g < G; g++) {
-      vector<uint64_t *> peer_ready(G);
-      for (int h = 0; h < G; h++) peer_ready[h] = (uint64_t *)((char *)dev[h].flags + 128);
-      const size_t share = first[g + 1] - first[g];
-      if (kuq_wait_flags(ctxs[g], 0, (const uint64_t *)dev[g].flags, (uint32_t)G, step + 1, 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-      if (share && kuq_resolve_device(ctxs[g], 0, (const char *)dev[g].bases[par], (const uint64_t *)dev[g].offs[par] + first[g],
-                                      (uint32_t)share, b.bases.size(), (const uint32_t *)dev[g].ids[par], NULL, 0))
-        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-      if (kuq_device_memset(ctxs[g], 0, (char *)dev[g].ids[par] + bounds[g] * 4, 0, (bounds[g + 1] - bounds[g]) * 4) ||
-          kuq_signal_peers(ctxs[g], 0, peer_ready.data(), (uint32_t)G, (uint32_t)g, step + 3))
-        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    }
-    // phase 4: results of the shares, in read order
-    Fastq_input = b.fastq;
-    for (int g = 0; g < G; g++) {
-      const size_t share = first[g + 1] - first[g];
-      if (!share) { if (kuq_sync_slot(ctxs[g], 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g])); continue; }
-      kuq_batch_result res;
-      if (kuq_collect_device_batch(ctxs[g], 0, &res)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-      emit_results(b, res, first[g], share);
-      total_classified += res.n_classified;
-    }
-    total_sequences += n;
-    total_bases += b.bases.size();
-    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
-    step++;
-  }
-  for (int g = 0; g < G; g++) {
-    if (kuq_finish(ctxs[g])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    for (int k = 0; k < 2; k++) { kuq_device_free(ctxs[g], dev[g].bases[k]); kuq_device_free(ctxs[g], dev[g].offs[k]); kuq_device_free(ctxs[g], dev[g].ids[k]); }
-    kuq_device_free(ctxs[g], dev[g].flags);
-  }
+  uint32_t rows = 0;
+  if (kuq_unit_table_rows(ctxs[0], &rows)) die(EX_SOFTWARE, kuq_last_error(ctxs[0]));
+  if (rows) Max_units_per_batch = rows;
+  shard_loop(ctxs, (uint32_t)runs.size(), true, argc, argv);
 }
 
 // What a staged database takes in HBM: 12 bytes per record whatever the file's record size (records of k <= 28 databases
@@ -1553,36 +1652,38 @@ int main(int argc, char **argv) {
   uint64_t hbm_budget = 60ull << 30;          // of an 80 GB H100: room left for the sparse tier and the batch slots
   if (getenv("KUQ_HBM_BUDGET")) hbm_budget = strtoull(getenv("KUQ_HBM_BUDGET"), NULL, 10);
   uint64_t chunk_budget = 0;
-  // a database larger than one card: sharded over the visible GPUs when they hold it together (run_sharded), else
-  // streamed through one GPU in ranges of at most 40 GB (two range buffers + a round of reads have to fit, run_streamed)
+  // The databases (one, or several together) larger than one card: sharded over the visible GPUs when they hold them
+  // together (run_sharded / run_sharded_multi), else streamed through one GPU in ranges of at most 40 GB (two range
+  // buffers + a round of reads have to fit, run_streamed).  Several databases that fit the budget together are resident.
   bool want_shards = false;
-  const uint64_t db_hbm = hbm_bytes(kdb, idx);
-  if (n_db == 1 && (db_hbm > hbm_budget || getenv("KUQ_FORCE_SHARDS"))) {
+  uint64_t all_hbm = 0;
+  for (size_t i = 0; i < n_db; i++) all_hbm += hbm_bytes(kdbs[i], idxs[i]);
+  if (all_hbm > hbm_budget || getenv("KUQ_FORCE_SHARDS")) {
     int n_vis = 0;
     if (const char *dl = getenv("KUQ_DEVICES")) { if (strcmp(dl, "all") == 0) n_vis = kuq_device_count(); else { n_vis = 1; for (const char *c = dl; *c; c++) n_vis += *c == ','; } }
     else if (!getenv("KUQ_DEVICE")) n_vis = kuq_device_count();
-    want_shards = n_vis > 1 && (getenv("KUQ_FORCE_SHARDS") || db_hbm / n_vis + (16ull << 30) < hbm_budget);
+    want_shards = n_vis > 1 && (getenv("KUQ_FORCE_SHARDS") || all_hbm / n_vis + (16ull << 30) < hbm_budget);
   }
-  if (db_hbm > hbm_budget && !want_shards) chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
-  // several databases: resident together when their records fit the budget together, else streamed (run_streamed)
-  if (n_db > 1) {
-    uint64_t all_hbm = 0;
-    for (size_t i = 0; i < n_db; i++) all_hbm += hbm_bytes(kdbs[i], idxs[i]);
-    chunk_budget = all_hbm > hbm_budget ? std::min<uint64_t>(hbm_budget / 4, 40ull << 30) : 0;
-  }
+  if (all_hbm > hbm_budget && !want_shards) chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
   if (Populate_memory_size > 0 && getenv("KUQ_FORCE_CHUNKS")) { chunk_budget = Populate_memory_size; want_shards = false; }
   kuq_config cfg;
   kuq_config_default(&cfg);
   cfg.n_slots = 3;                             // classify b + 1 on the GPU, format b, gather b + 2 (process_file_parallel)
+  if (want_shards) cfg.n_slots = 2;            // shards use slot 0, and slots 0 and 1 if they fall back to streaming
   cfg.max_bases_per_batch = 288ull << 20;      // one read may be a whole chromosome (the largest human one is 248 Mbp)
   cfg.work_unit_size = Work_unit_size;
   // -x (or a database that has to be split) → one global sketch per taxon (classify.cpp:719); else per work unit, which
-  // is also the reference's rule for several databases
-  cfg.hll_mode = (Populate_memory_size > 0 || (chunk_budget && n_db == 1) || want_shards) ? KUQ_HLL_CHUNKED : KUQ_HLL_PRELOAD;
+  // is also the reference's rule for several databases (resident, streamed or sharded)
+  cfg.hll_mode = (Populate_memory_size > 0 || ((chunk_budget || want_shards) && n_db == 1)) ? KUQ_HLL_CHUNKED : KUQ_HLL_PRELOAD;
 #ifdef EXACT_COUNTING
   // classifyExact (classify.cpp:46-49): sets of k-mers instead of sketches; work units and chunks make no difference
   cfg.hll_mode = KUQ_HLL_EXACT;
-  if (want_shards) { want_shards = false; chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30); }   // exact sets are not merged across devices
+  if (want_shards) {                           // exact sets are not merged across devices
+    want_shards = false;
+    chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
+    if (n_db > 1) cerr << "classify: classifyExact streams several databases through one GPU instead of sharding them "
+                          "(exact k-mer sets are not merged across devices)" << endl;
+  }
   if (Quick_mode) die(EX_USAGE, "-q is not supported by the GPU classifyExact");
 #endif
   if ((chunk_budget || want_shards) && !Populate_memory_size && n_db == 1)
@@ -1619,7 +1720,7 @@ int main(int argc, char **argv) {
   }
   if (want_shards && All_ctx.size() < 2) { want_shards = false; chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30); }
   if (All_ctx.size() > 1 && !want_shards && n_db == 1) fprintf(stderr, "classify: %zu GPUs, database replicated, batches round-robin\n", All_ctx.size());
-  if (n_db > 1 && !chunk_budget) fprintf(stderr, "classify: %zu databases resident on %zu GPU(s)\n", n_db, All_ctx.size());
+  if (n_db > 1 && !chunk_budget && !want_shards) fprintf(stderr, "classify: %zu databases resident on %zu GPU(s)\n", n_db, All_ctx.size());
   // -q: the preloaded path leaves a read at its -m'th hit; with -x every k-mer is counted (classify.cpp:943-944 / :701-738)
   for (kuq_ctx *c : All_ctx)
     if (Quick_mode && kuq_set_quick_mode(c, Minimum_hit_count, Populate_memory_size == 0)) die(EX_SOFTWARE, kuq_last_error(c));
@@ -1674,7 +1775,7 @@ int main(int argc, char **argv) {
     for (kuq_ctx *c : All_ctx)
       if (kuq_set_taxonomy(c, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(c));
   }
-  if (cfg.hll_mode == KUQ_HLL_PRELOAD && !chunk_budget) {           // (streamed runs ask once their taxa are known)
+  if (cfg.hll_mode == KUQ_HLL_PRELOAD && !chunk_budget && !want_shards) {   // (streamed / sharded runs ask once their taxa are known)
     uint32_t rows = 0;
     if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
     if (rows) Max_units_per_batch = rows;
@@ -1690,7 +1791,8 @@ int main(int argc, char **argv) {
 
   struct timeval tv1, tv2;
   gettimeofday(&tv1, NULL);
-  if (want_shards) run_sharded(All_ctx, kdb, idx, argc, argv, db_counts[0]);
+  if (want_shards && n_db == 1) run_sharded(All_ctx, kdb, idx, argc, argv, db_counts[0]);
+  else if (want_shards) run_sharded_multi(All_ctx, kdbs, idxs, argc, argv, db_counts);
   else if (chunk_budget) run_streamed(ctx, kdbs, idxs, chunk_budget, hbm_budget, argc, argv, db_counts);
   else for (int i = optind; i < argc; i++) process_file(ctx, argv[i]);
   // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)

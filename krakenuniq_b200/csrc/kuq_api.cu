@@ -106,11 +106,11 @@ struct kuq_ctx {
   uint32_t *d_tx_keys = nullptr, *d_tx_dense = nullptr;
   unsigned long long *d_tx_counts = nullptr;
   uint32_t tx_cap = 0;
-  // whole databases asked after the one above, in this order (kuq_stage_db_append); same k
+  // databases (or minimizer ranges of them) asked after the one above, in this order (kuq_stage_db_append_range); same k
   struct ExtraDb {
     uint8_t *d_pairs = nullptr;
     uint64_t *d_offsets = nullptr;
-    uint64_t key_ct = 0;
+    uint64_t key_ct = 0, rec_base = 0, bin_lo = 0, bin_hi = 0;
     uint32_t nt = 0, idx_type = 0;
     uint32_t *d_tx_keys = nullptr, *d_tx_dense = nullptr;
     unsigned long long *d_tx_counts = nullptr;
@@ -869,18 +869,43 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   set_unit_ptrs(p, s);
 }
 
-// The in-order lookup over every staged database (kuq_stage_db_append) into p0.codes_dense: one launch per run of
+// The staged databases in the order they are asked, each with its own minimizer range.  A run = consecutive databases
+// with the same window parameters (nt, index type).
+std::vector<DbView> db_views(const kuq_ctx *ctx) {
+  std::vector<DbView> v{db_view(ctx, ctx->d_pairs, ctx->d_offsets, ctx->rec_base, ctx->bin_lo, ctx->bin_hi, ctx->nt, ctx->idx_type)};
+  for (auto &e : ctx->more) v.push_back(db_view(ctx, e.d_pairs, e.d_offsets, e.rec_base, e.bin_lo, e.bin_hi, e.nt, e.idx_type));
+  return v;
+}
+bool same_run(const DbView &a, const DbView &b) { return a.nt == b.nt && a.xor_mask == b.xor_mask; }
+uint32_t count_runs(const kuq_ctx *ctx) {
+  const std::vector<DbView> v = db_views(ctx);
+  uint32_t n = 1;
+  for (size_t i = 1; i < v.size(); i++) n += !same_run(v[i], v[i - 1]);
+  return n;
+}
+
+// The in-order lookup over every staged database (kuq_stage_db_append_range) into p0.codes_dense: one launch per run of
 // consecutive databases with the same (nt, index type), at most MAX_DBS per launch; runs after the first fill only the
-// windows no earlier run answered, and k_scan runs again where the window parameters change.
-int launch_multi_lookup(kuq_ctx *ctx, Slot &s, const Params &p0, uint32_t only_hits) {
-  std::vector<DbView> v{p0.db};
-  for (auto &e : ctx->more) v.push_back(db_view(ctx, e.d_pairs, e.d_offsets, 0, 0, 1ull << (2 * e.nt), e.nt, e.idx_type));
+// windows no earlier run answered, and k_scan runs again where the window parameters change.  run >= 0: only that run,
+// its first launch with `only_hits` and a k_scan of its own (kuq_lookup_device_peers_run, one run per call).
+int launch_multi_lookup(kuq_ctx *ctx, Slot &s, const Params &p0, uint32_t only_hits, int run = -1) {
+  const std::vector<DbView> v = db_views(ctx);
   const DbView *scanned = nullptr;
+  int r = -1;
   for (size_t i = 0; i < v.size();) {
+    if (i == 0 || !same_run(v[i], v[i - 1])) r++;
     Params q = p0;
     q.db = v[i];
     q.n_dbs = 0;
-    while (i < v.size() && q.n_dbs < MAX_DBS && v[i].nt == q.db.nt && v[i].xor_mask == q.db.xor_mask) q.dbs[q.n_dbs++] = v[i++];
+    while (i < v.size() && q.n_dbs < MAX_DBS && same_run(v[i], q.db)) q.dbs[q.n_dbs++] = v[i++];
+    if (run >= 0 && r != run) continue;
+    q.run_lo = q.run_hi = 0;                           // the bins this launch's databases hold (empty slices aside)
+    for (uint32_t d = 0; d < q.n_dbs; d++) {
+      if (q.dbs[d].bin_lo >= q.dbs[d].bin_hi) continue;
+      if (q.run_lo >= q.run_hi) { q.run_lo = q.dbs[d].bin_lo; q.run_hi = q.dbs[d].bin_hi; continue; }
+      q.run_lo = std::min(q.run_lo, q.dbs[d].bin_lo);
+      q.run_hi = std::max(q.run_hi, q.dbs[d].bin_hi);
+    }
     q.only_hits = scanned ? KUQ_LOOKUP_FILL_EMPTY : only_hits;
     const bool scan = !scanned || scanned->nt != q.db.nt || scanned->xor_mask != q.db.xor_mask;
     if (scan) CU(cudaMemsetAsync(q.chunk_counter, 0, 4, s.stream));
@@ -890,13 +915,15 @@ int launch_multi_lookup(kuq_ctx *ctx, Slot &s, const Params &p0, uint32_t only_h
   return KUQ_OK;
 }
 
-int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p) {
+// run >= 0: one run of the in-order lookup with peer scatter (kuq_lookup_device_peers_run)
+int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
   if (ctx->lca_mode) return fail(ctx, KUQ_E_STATE, "this context built a database (kuq_set_lcas_batch): stage it anew to classify");
   // several databases (or a fill-empty lookup): the in-order lookup, then — for a classification — the resolve half
   // over the slot's merged codes
-  const bool multi = (!ctx->more.empty() && mode != MODE_RESOLVE) || (mode == MODE_LOOKUP && p.only_hits == KUQ_LOOKUP_FILL_EMPTY);
-  if (multi && (p.n_peers || ctx->shard_counting))
-    return fail(ctx, KUQ_E_STATE, "shard counting and peer lookups take one database");
+  const bool multi = (!ctx->more.empty() && mode != MODE_RESOLVE) || (mode == MODE_LOOKUP && p.only_hits == KUQ_LOOKUP_FILL_EMPTY) ||
+                     run >= 0;
+  if (multi && ((p.n_peers && run < 0) || ctx->shard_counting))
+    return fail(ctx, KUQ_E_STATE, "shard counting and kuq_lookup_device_peers take one database (several: kuq_lookup_device_peers_run)");
   uint32_t *multi_out = p.codes_dense;
   const uint32_t multi_only_hits = mode == MODE_LOOKUP ? p.only_hits : 0;
   if (multi && mode == MODE_FUSED) {
@@ -953,7 +980,7 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p) {
   if (p.n_reads && multi) {
     Params q = p;
     q.codes_dense = multi_out;
-    int mrc = launch_multi_lookup(ctx, s, q, multi_only_hits);
+    int mrc = launch_multi_lookup(ctx, s, q, multi_only_hits, run);
     if (mrc) return mrc;
     if (mode != MODE_LOOKUP) CU(cudaMemsetAsync(p.chunk_counter, 0, 4, s.stream));   // k_scan of the resolve half
   }
@@ -1174,16 +1201,9 @@ int upload_db(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi, u
 }
 }  // namespace
 
-int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes,
-                 uint64_t bin_lo, uint64_t bin_hi) {
-  if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
-  CU(cudaSetDevice(ctx->device));
-  DbFile f;
-  int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
-  if (rc) return rc;
-  const uint64_t n_bins = 1ull << (2 * f.nt);
-  if (bin_hi == 0 || bin_hi > n_bins) bin_hi = n_bins;
-  if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
+namespace {
+// bins [bin_lo, bin_hi) of f (validated by the caller; may be empty) become the first database of the context
+int stage_first(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi) {
   uint64_t rec_lo = f.offsets[bin_lo], rec_hi = f.offsets[bin_hi];
   if (rec_hi < rec_lo || rec_hi > f.key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
   // taxonomy numbering survives a re-stage (chunked mode) as long as the new range only holds numbered taxids; the
@@ -1199,7 +1219,7 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   CU(cudaMalloc((void **)&ctx->d_pairs, ctx->key_ct * 12 + SLACK));
   CU(dmalloc(&ctx->d_offsets_owned, bin_hi - bin_lo + 1));
   ctx->d_offsets = ctx->d_offsets_owned;
-  rc = upload_db(ctx, f, bin_lo, bin_hi, ctx->d_pairs, ctx->d_offsets_owned);
+  int rc = upload_db(ctx, f, bin_lo, bin_hi, ctx->d_pairs, ctx->d_offsets_owned);
   if (rc) return rc;
   ctx->db_staged = true;
   rc = collect_taxids(ctx);
@@ -1207,33 +1227,67 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   if (ctx->finalized) return remap_db(ctx);
   return KUQ_OK;
 }
+}  // namespace
 
-int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes) {
+int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes,
+                 uint64_t bin_lo, uint64_t bin_hi) {
   if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
-  if (!ctx->db_staged || ctx->stream_open) return kuq_stage_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, 0, 0);
   CU(cudaSetDevice(ctx->device));
   DbFile f;
   int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
   if (rc) return rc;
-  if (f.k != ctx->k) return fail(ctx, KUQ_E_INVALID_ARG, "the databases differ in k: %u vs %u", ctx->k, f.k);
   const uint64_t n_bins = 1ull << (2 * f.nt);
-  if (f.offsets[n_bins] != f.key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
+  if (bin_hi == 0 || bin_hi > n_bins) bin_hi = n_bins;
+  if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
+  return stage_first(ctx, f, bin_lo, bin_hi);
+}
+
+int kuq_stage_db_append_range(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image,
+                              uint64_t idx_bytes, uint64_t bin_lo, uint64_t bin_hi) {
+  if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
+  CU(cudaSetDevice(ctx->device));
+  DbFile f;
+  int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
+  if (rc) return rc;
+  const uint64_t n_bins = 1ull << (2 * f.nt);
+  if (bin_hi == 0) bin_hi = n_bins;                  // (0, 0) = the whole database; lo == hi != 0 = an empty slice
+  if (bin_lo > bin_hi || bin_hi > n_bins)
+    return fail(ctx, KUQ_E_INVALID_ARG, "minimizer range [%llu, %llu) outside the %llu bins of nt = %u", (unsigned long long)bin_lo,
+                (unsigned long long)bin_hi, (unsigned long long)n_bins, f.nt);
+  if (!ctx->db_staged || ctx->stream_open) return stage_first(ctx, f, bin_lo, bin_hi);
+  if (f.k != ctx->k) return fail(ctx, KUQ_E_INVALID_ARG, "the databases differ in k: %u vs %u", ctx->k, f.k);
+  if (f.offsets[n_bins] != f.key_ct || f.offsets[bin_lo] > f.offsets[bin_hi])
+    return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
   ctx->more.emplace_back();
   kuq_ctx::ExtraDb &e = ctx->more.back();
-  e.key_ct = f.key_ct; e.nt = f.nt; e.idx_type = f.idx_type;
+  e.rec_base = f.offsets[bin_lo];
+  e.key_ct = f.offsets[bin_hi] - e.rec_base;
+  e.bin_lo = bin_lo; e.bin_hi = bin_hi;
+  e.nt = f.nt; e.idx_type = f.idx_type;
   auto drop = [&](int code) { ctx->more.pop_back(); return code; };
-  if (dmalloc(&e.d_pairs, e.key_ct * 12 + SLACK) != cudaSuccess || dmalloc(&e.d_offsets, n_bins + 1) != cudaSuccess) {
+  if (dmalloc(&e.d_pairs, e.key_ct * 12 + SLACK) != cudaSuccess || dmalloc(&e.d_offsets, bin_hi - bin_lo + 1) != cudaSuccess) {
     (void)cudaGetLastError();
     cudaFree(e.d_pairs); cudaFree(e.d_offsets);
     return drop(fail(ctx, KUQ_E_NOMEM, "no room for database %zu (%llu records)", ctx->more.size() + 1, (unsigned long long)e.key_ct));
   }
-  rc = upload_db(ctx, f, 0, n_bins, e.d_pairs, e.d_offsets);
+  rc = upload_db(ctx, f, bin_lo, bin_hi, e.d_pairs, e.d_offsets);
   if (!rc) rc = collect_taxids(ctx, e.d_pairs, e.key_ct, e.d_tx_keys, e.d_tx_dense, e.d_tx_counts, e.tx_cap, e.taxids, e.counts);
   if (rc) {
     cudaFree(e.d_pairs); cudaFree(e.d_offsets); cudaFree(e.d_tx_keys); cudaFree(e.d_tx_dense); cudaFree(e.d_tx_counts);
     return drop(rc);
   }
   if (ctx->finalized) return remap_db(ctx);
+  return KUQ_OK;
+}
+
+int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes) {
+  return kuq_stage_db_append_range(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, 0, 0);
+}
+
+int kuq_db_runs(kuq_ctx *ctx, uint32_t *n_runs) {
+  if (!ctx || !n_runs) return KUQ_E_INVALID_ARG;
+  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
+  *n_runs = count_runs(ctx);
   return KUQ_OK;
 }
 
@@ -1548,9 +1602,10 @@ int kuq_resolve_device(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const u
   return device_call(ctx, slot, MODE_RESOLVE, d_bases, d_read_offsets, n_reads, total_bases, d_unit_id, flags, nullptr, d_codes_in, 0);
 }
 
-int kuq_lookup_device_peers(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets,
-                            uint32_t n_reads, uint64_t total_bases, uint32_t *const *d_codes_peers,
-                            const uint64_t *base_bounds, uint32_t n_peers) {
+// run < 0: kuq_lookup_device_peers (one database, hits only); run >= 0: that run of the in-order lookup
+static int peers_call(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets, uint32_t n_reads,
+                      uint64_t total_bases, uint32_t *const *d_codes_peers, const uint64_t *base_bounds, uint32_t n_peers,
+                      int run) {
   if (!d_codes_peers || !base_bounds || n_peers == 0 || n_peers > 8) return KUQ_E_INVALID_ARG;
   int rc = check_slot(ctx, slot);
   if (rc) return rc;
@@ -1565,11 +1620,27 @@ int kuq_lookup_device_peers(kuq_ctx *ctx, uint32_t slot, const char *d_bases, co
   s.n_reads = n_reads; s.flags = 0; s.total_bases = total_bases; s.external = true;
   Params p;
   fill_params(ctx, s, p, d_bases, d_read_offsets, nullptr, n_reads, 0);
-  p.only_hits = 1;
+  p.only_hits = run > 0 ? KUQ_LOOKUP_FILL_EMPTY : 1;
   p.n_peers = n_peers;
   for (uint32_t j = 0; j < n_peers; j++) { p.peer_codes[j] = d_codes_peers[j]; p.peer_bounds[j] = base_bounds[j]; }
   p.peer_bounds[n_peers] = base_bounds[n_peers];
-  return launch_on_slot(ctx, s, MODE_LOOKUP, p);
+  return launch_on_slot(ctx, s, MODE_LOOKUP, p, run);
+}
+
+int kuq_lookup_device_peers(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets,
+                            uint32_t n_reads, uint64_t total_bases, uint32_t *const *d_codes_peers,
+                            const uint64_t *base_bounds, uint32_t n_peers) {
+  return peers_call(ctx, slot, d_bases, d_read_offsets, n_reads, total_bases, d_codes_peers, base_bounds, n_peers, -1);
+}
+
+int kuq_lookup_device_peers_run(kuq_ctx *ctx, uint32_t slot, const char *d_bases, const uint64_t *d_read_offsets,
+                                uint32_t n_reads, uint64_t total_bases, uint32_t *const *d_codes_peers,
+                                const uint64_t *base_bounds, uint32_t n_peers, uint32_t run) {
+  if (!ctx) return KUQ_E_INVALID_ARG;
+  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
+  const uint32_t n_runs = count_runs(ctx);
+  if (run >= n_runs) return fail(ctx, KUQ_E_INVALID_ARG, "run %u of %u", run, n_runs);
+  return peers_call(ctx, slot, d_bases, d_read_offsets, n_reads, total_bases, d_codes_peers, base_bounds, n_peers, (int)run);
 }
 
 // ---- device memory that can be shared with the other ranks of a node (CUDA IPC) --------------------------------

@@ -657,12 +657,31 @@ __device__ __forceinline__ bool search_bin(const DbView &db, uint32_t bin, uint6
   return false;
 }
 
+// A word another GPU may have stored over NVLink in an earlier phase: a coherent system-scope load, never the
+// non-coherent read-only path.
+__device__ __forceinline__ uint32_t load_relaxed_sys(const uint32_t *a) {
+  uint32_t v;
+  asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a) : "memory");
+  return v;
+}
+
 __device__ __forceinline__ void lookup_window_multi(const Params &p, uint64_t g, uint32_t bin, uint64_t canon) {
   if (bin == BIN_NONE) return;
-  if (p.only_hits == 2u && p.codes_dense[g] != 0) return;
-  if (bin == BIN_AMBIG) {
-    if (!p.only_hits) p.codes_dense[g] = AMBIG;
-    return;
+  uint32_t *out = p.codes_dense + g;
+  if (p.n_peers) {
+    // databases sharded by minimizer range: ambiguous windows are the resolving GPU's own business, windows of other
+    // GPUs' ranges are skipped before anything is loaded, and the hit goes to the GPU that resolves the read
+    if (bin == BIN_AMBIG || bin < p.run_lo || bin >= p.run_hi) return;
+    uint32_t j = 0;
+    while (j + 1 < p.n_peers && g >= p.peer_bounds[j + 1]) j++;
+    out = p.peer_codes[j] + g;
+    if (p.only_hits == 2u && load_relaxed_sys(out) != 0) return;     // answered by an earlier run, on any GPU
+  } else {
+    if (p.only_hits == 2u && *out != 0) return;
+    if (bin == BIN_AMBIG) {
+      if (!p.only_hits) *out = AMBIG;
+      return;
+    }
   }
   uint32_t taxon = 0;
 #pragma unroll
@@ -682,7 +701,7 @@ __device__ __forceinline__ void lookup_window_multi(const Params &p, uint64_t g,
       break;
     }
   }
-  if (!p.only_hits || taxon != 0) p.codes_dense[g] = taxon;
+  if (!p.only_hits || taxon != 0) *out = taxon;
 }
 
 // MODE_FUSED computes its windows from the packed blocks (FAST: k = 31, m = 15, see window_bin) instead of reading

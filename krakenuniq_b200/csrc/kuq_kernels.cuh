@@ -233,9 +233,12 @@ struct Params {
   uint64_t peer_bounds[9];
   // MODE_LOOKUP over several databases (launch_lookup_multi): dbs[0, n_dbs) of one (k, nt, index type) are asked in
   // order; db = dbs[0] gives k_scan its window parameters.  only_hits 2 (fill empty): windows coded non-zero already are
-  // skipped before any index fetch.
+  // skipped before any index fetch.  With n_peers (databases sharded by minimizer range over the GPUs), a window whose
+  // bin lies in [run_lo, run_hi) — the bins this GPU holds of the launch's databases — is asked here and its hit stored
+  // into the buffer of the GPU that resolves the read; fill empty then reads that GPU's word first.
   DbView dbs[MAX_DBS];
   uint32_t n_dbs;
+  uint32_t run_lo, run_hi;
   unsigned long long *stats;    // flag 8: [0] += looked-up windows, [1] += sum of ceil(log2(bin size + 1))
   // per-taxon state
   uint8_t *regs;                // [n_sketch][4096]

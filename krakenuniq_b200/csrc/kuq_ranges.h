@@ -29,4 +29,49 @@ inline bool plan_ranges(const uint64_t *offsets, uint64_t n_bins, uint64_t budge
   return true;
 }
 
+// Databases sharded over G GPUs by minimizer range (classify with one or several -d on a node whose GPUs hold them
+// only together).  Consecutive databases with equal (nt, index type) form a run: their windows have the same bins, so
+// one lookup launch asks them in order.  Each run gets ONE cut of its 4^nt bins into G ranges, balanced by the run's
+// summed record counts, and every database of the run is staged with the same range on GPU g: a window's whole
+// in-order search inside a run happens on one GPU.  A range may be empty (cut[g] == cut[g + 1]).  With one database the
+// cut points are those of the lower bound of key_ct / G * g in its index.
+struct ShardDb {
+  const uint64_t *offsets;   // the index's 4^nt + 1 running record counts
+  uint32_t nt, idx_type;
+};
+struct ShardRun {
+  size_t first, end;                 // databases [first, end)
+  std::vector<uint64_t> cut;         // G + 1 bin boundaries: GPU g holds [cut[g], cut[g + 1])
+};
+inline std::vector<ShardRun> plan_shards(const std::vector<ShardDb> &dbs, int G) {
+  std::vector<ShardRun> runs;
+  for (size_t i = 0; i < dbs.size();) {
+    ShardRun r;
+    r.first = i;
+    while (i < dbs.size() && dbs[i].nt == dbs[r.first].nt && dbs[i].idx_type == dbs[r.first].idx_type) i++;
+    r.end = i;
+    const uint64_t n_bins = 1ull << (2 * dbs[r.first].nt);
+    auto sum = [&](uint64_t b) {                      // records of the run in bins [0, b)
+      uint64_t s = 0;
+      for (size_t d = r.first; d < r.end; d++) s += dbs[d].offsets[b];
+      return s;
+    };
+    const uint64_t total = sum(n_bins);
+    r.cut.assign(G + 1, 0);
+    r.cut[G] = n_bins;
+    for (int g = 1; g < G; g++) {                     // first bin b < n_bins with sum(b) >= total / G * g, else n_bins
+      const uint64_t want = total / G * g;
+      uint64_t lo = 0, hi = n_bins;
+      while (lo < hi) {
+        const uint64_t mid = lo + (hi - lo) / 2;
+        if (sum(mid) < want) lo = mid + 1; else hi = mid;
+      }
+      r.cut[g] = lo;
+    }
+    for (int g = 1; g <= G; g++) if (r.cut[g] < r.cut[g - 1]) r.cut[g] = r.cut[g - 1];
+    runs.push_back(std::move(r));
+  }
+  return runs;
+}
+
 #endif
