@@ -174,10 +174,12 @@ struct kuq_ctx {
   bool kept = false;                      // some staged records carry KEPT_BIT
   uint64_t kept_keys = 0;                 // keys held by kept records (included in d_sparse_distinct)
   bool set_has_hits = false;              // the set holds keys of hits, which kept records could duplicate
+  bool keep_dirty = false;                // fused calls kept records at their first sighting (F_KEEP) since settle_kept
   uint64_t sparse_grown = 0;              // times the sparse-tier set was re-allocated at a harvest
   double harvest_ms = 0;                  // device time of the last harvest
-  // the harvest's counters and timing events, made at the first harvest and kept: a cudaMalloc / cudaFree pair per
-  // harvest held the device idle at the end of every run
+  // the harvest's counters and timing events, made at the first harvest (or keep-mode call) and kept: a cudaMalloc /
+  // cudaFree pair per harvest held the device idle at the end of every run.  [0], [1]: the harvest's; [2]: records that
+  // keep-mode calls made kept since settle_kept (k_resolve counts them)
   unsigned long long *d_harvest_stat = nullptr;
   cudaEvent_t harvest_ev[2] = {nullptr, nullptr};
   bool lca_mode = false;                  // kuq_set_lcas_batch ran: record values are LCA results, not classifiable
@@ -581,7 +583,11 @@ int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
   CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
   uint64_t used = 0;
   for (uint32_t v : distinct) used += v;
-  used -= std::min(used, ctx->kept_keys);             // keys of kept records live in the records, not in the set
+  // keys of kept records live in the records, not in the set; those of keep-mode calls since the last settle_kept are
+  // counted in distinct[] and in d_harvest_stat[2] alike (duplicates of collision groups included)
+  unsigned long long pending = 0;
+  if (ctx->keep_dirty) CU(cudaMemcpy(&pending, ctx->d_harvest_stat + 2, 8, cudaMemcpyDeviceToHost));
+  used -= std::min<uint64_t>(used, ctx->kept_keys + pending);
   ctx->direct_upper = used;
   if ((used + windows) * 10 > ctx->sparse_cap * 8) {
     uint64_t cap = ctx->sparse_cap;
@@ -593,7 +599,7 @@ int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
   return KUQ_OK;
 }
 
-// Build the collision table of the staged range once, the first time a harvest can use the record tier.
+// Build the collision table of the staged range once, the first time keep mode or a harvest can use the record tier.
 int ensure_collisions(kuq_ctx *ctx) {
   if (ctx->collisions) return KUQ_OK;
   ctx->collisions = -1;
@@ -611,6 +617,60 @@ int ensure_collisions(kuq_ctx *ctx) {
   if (getenv("KUQ_TIMING"))
     fprintf(stderr, "[timing] collision table: %llu secondaries of %llu records, %.1f ms%s\n", (unsigned long long)ctx->n_secondaries,
             (unsigned long long)ctx->key_ct, ctx->collisions_ms, rc ? " (not built: harvests fill the set)" : "");
+  return KUQ_OK;
+}
+
+int harvest_state(kuq_ctx *ctx) {
+  if (ctx->d_harvest_stat) return KUQ_OK;
+  CU(dmalloc(&ctx->d_harvest_stat, 3));
+  CU(cudaMemset(ctx->d_harvest_stat, 0, 3 * 8));
+  CU(cudaEventCreate(&ctx->harvest_ev[0])); CU(cudaEventCreate(&ctx->harvest_ev[1]));
+  return KUQ_OK;
+}
+
+// Keep mode (F_KEEP): a fused call whose counted hits would become kept records at the next harvest anyway (preload
+// rule, a resident range with its collision table, a set without keys of hits, no flags pending) keeps them in the
+// lookup, and the harvest shrinks to settle_kept.  KUQ_KEEP_AT_HARVEST=1 keeps the flag-and-harvest path instead (A/B
+// runs and tests compare both in one build).
+int use_keep_mode(kuq_ctx *ctx, int mode, const Params &p, bool *keep) {
+  *keep = false;
+  if (mode != MODE_FUSED || !p.n_reads || (p.flags & 4u) || ctx->cfg.hll_mode != KUQ_HLL_PRELOAD || !ctx->d_sparse_slots ||
+      ctx->set_has_hits || ctx->stream_open || ctx->seen_dirty || (ctx->quick_min && ctx->quick_stop))
+    return KUQ_OK;
+  const char *env = getenv("KUQ_KEEP_AT_HARVEST");
+  if (env && *env && strcmp(env, "0") != 0) return KUQ_OK;
+  int rc = ensure_collisions(ctx);
+  if (rc) return rc;
+  if (ctx->collisions != 1) return KUQ_OK;
+  rc = harvest_state(ctx);
+  if (rc) return rc;
+  *keep = true;
+  return KUQ_OK;
+}
+
+// After keep-mode calls: kept secondaries hand KEPT_BIT to their primaries (k_settle_kept takes the duplicates back out of
+// distinct[]) and the records those calls kept join kept_keys — the state the flag-and-harvest path leaves.  All slots
+// must be idle.
+int settle_kept(kuq_ctx *ctx) {
+  ctx->keep_dirty = false;
+  unsigned long long *d_stat = ctx->d_harvest_stat;
+  CU(cudaMemsetAsync(d_stat, 0, 8, ctx->aux));
+  CU(cudaEventRecord(ctx->harvest_ev[0], ctx->aux));
+  launch_settle_kept(ctx->d_pairs, ctx->d_secondaries, ctx->n_secondaries, ctx->d_sparse_distinct, d_stat, ctx->aux);
+  if (ctx->n_secondaries) ctx->launches++;
+  CU(cudaEventRecord(ctx->harvest_ev[1], ctx->aux));
+  unsigned long long st[3] = {0, 0, 0};
+  CU(cudaMemcpyAsync(st, d_stat, 24, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaMemsetAsync(d_stat + 2, 0, 8, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, ctx->harvest_ev[0], ctx->harvest_ev[1]);
+  ctx->harvest_ms = ms;
+  ctx->kept_keys += st[2] - st[0];
+  ctx->snap_valid = false;
+  if (getenv("KUQ_TIMING"))
+    fprintf(stderr, "[timing] settle: %llu records kept at sighting, %llu of them duplicates (%llu kept), %.3f ms\n", st[2], st[0],
+            (unsigned long long)ctx->kept_keys, ms);
   return KUQ_OK;
 }
 
@@ -660,9 +720,15 @@ int spill_kept(kuq_ctx *ctx) {
 //    inserted, so the set grows here instead of failing mid-batch.
 // `discard` drops every flag of both kinds instead (the keys were exported, or the counts are reset).
 int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
-  if (!ctx->seen_dirty && !(ctx->kept && (discard || to_set))) return KUQ_OK;
+  if (!ctx->seen_dirty && !ctx->keep_dirty && !(ctx->kept && (discard || to_set))) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  double settle_ms = 0;
+  if (ctx->keep_dirty) {
+    int rc = settle_kept(ctx);
+    if (rc) return rc;
+    settle_ms = ctx->harvest_ms;
+  }
   if (to_set && !discard) { int rc = spill_kept(ctx); if (rc) return rc; }
   if (!ctx->seen_dirty && !(ctx->kept && discard)) return KUQ_OK;
   ctx->seen_dirty = false;
@@ -677,10 +743,7 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   SparseSet ss;
   ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0; ss.n_used = ctx->d_sparse_used;
   ss.distinct = ctx->d_sparse_distinct;
-  if (!ctx->d_harvest_stat) {
-    CU(dmalloc(&ctx->d_harvest_stat, 2));
-    CU(cudaEventCreate(&ctx->harvest_ev[0])); CU(cudaEventCreate(&ctx->harvest_ev[1]));
-  }
+  { int rc = harvest_state(ctx); if (rc) return rc; }
   unsigned long long *d_stat = ctx->d_harvest_stat;
   cudaEvent_t e0 = ctx->harvest_ev[0], e1 = ctx->harvest_ev[1];
   CU(cudaMemsetAsync(d_stat, 0, 16, ctx->aux));
@@ -728,7 +791,7 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   CU(cudaStreamSynchronize(ctx->aux));
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1);
-  ctx->harvest_ms = ms;
+  ctx->harvest_ms = settle_ms + ms;
   ctx->snap_valid = false;
   if (keep) {
     ctx->kept_keys += st[0];
@@ -832,7 +895,7 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   p.clean = s.d_clean;
   p.n_reads = n_reads;
   p.n_chunks = (n_reads + CHUNK_READS - 1) / CHUNK_READS;
-  p.flags = flags;
+  p.flags = flags & ~F_KEEP;                 // launch_on_slot decides keep mode
   p.hll_mode = ctx->cfg.hll_mode;
   p.call = s.d_call;
   p.n_windows = s.d_nwin;
@@ -971,6 +1034,14 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
   } else if (ctx->cfg.hll_mode == KUQ_HLL_PRELOAD) {
     p.unit_id = nullptr;                 // no per-unit bookkeeping for this call
   }
+  bool keep = false;
+  { int krc = use_keep_mode(ctx, mode, p, &keep); if (krc) return krc; }
+  if (keep) {
+    p.flags |= F_KEEP;
+    p.n_new_kept = ctx->d_harvest_stat + 2;
+    ctx->kept = true;
+    ctx->keep_dirty = true;
+  }
   p.packed = windows_packed(mode, p) ? 1u : 0u;
   if (p.n_reads) s.windows_packed = p.packed != 0;
   CU(cudaMemsetAsync(s.d_scalars, 0, 8 * 8, s.stream));
@@ -987,7 +1058,7 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
   if (p.n_reads && !(multi && mode == MODE_LOOKUP)) ctx->launches += launch_classify(mode, p, ctx->n_sm, s.stream, s.ev_stage);
   // the fused path flags the records of its counted hits (k_lookup); quick / exact runs go through the other halves
   if (p.n_reads && mode == MODE_FUSED && !(p.flags & 4u) && ctx->cfg.hll_mode <= KUQ_HLL_CHUNKED &&
-      !(ctx->quick_min && ctx->quick_stop))
+      !(ctx->quick_min && ctx->quick_stop) && !keep)
     ctx->seen_dirty = true;
   CU(cudaEventRecord(s.ev_k1, s.stream));
   s.timed = true;
@@ -2647,6 +2718,7 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
   if (!ctx->d_sparse_slots) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  if (ctx->keep_dirty) { rc = settle_kept(ctx); if (rc) return rc; }   // one kept record per key
   // Two sources: the keys already in the local set (misses, resolve-half inserts, earlier harvests) and the records —
   // flagged since the last harvest, or kept.  The flagged records are NOT inserted locally first: their keys go straight
   // into the export buffer (and the flags are cleared) — after the exchange every key is inserted exactly once, by its
@@ -2841,6 +2913,7 @@ int kuq_sparse_tier_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *keys, uint64_t
     if (ctx->d_sparse_distinct) {
       CU(cudaSetDevice(ctx->device));
       for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+      if (ctx->keep_dirty) { rc = settle_kept(ctx); if (rc) return rc; }     // duplicates of collision groups out
       std::vector<uint32_t> d(ctx->n_sketch);
       CU(cudaMemcpy(d.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
       for (uint32_t v : d) *keys += v;

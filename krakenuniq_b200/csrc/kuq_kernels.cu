@@ -528,11 +528,12 @@ void launch_unpack_windows(const Params &p, uint64_t n_pos, int n_sm, cudaStream
 template <int MODE, bool LEAN>
 __device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint32_t bin, uint64_t canon) {
   const DbView &db = p.db;
-  const uint32_t flags = LEAN ? (p.flags & 4u) : p.flags;
+  const uint32_t flags = LEAN ? (p.flags & (4u | F_KEEP)) : p.flags;
   const uint32_t only_hits = LEAN ? 0u : p.only_hits;
   const uint32_t n_peers = LEAN ? 0u : p.n_peers;
   const uint32_t hi_mask = (uint32_t)(db.key_mask >> 32);
   const bool counting = (MODE == MODE_FUSED) && !(flags & 4u);
+  const bool keep = counting && (flags & F_KEEP);
   // hits of the fused path reach the sparse tier through the record flag (see below); dense-only / exact runs have
   // no sparse tier
   // flag 32 (database sharded over GPUs, one database): the GPU that FINDS a hit owns its sketch work — register
@@ -546,7 +547,7 @@ __device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint3
       if (!only_hits && !(MODE == MODE_LOOKUP && n_peers)) p.codes_dense[g] = AMBIG;
       return;
     }
-    uint32_t taxon = 0;
+    uint32_t taxon = 0, kept_new = 0;
     if (MODE == MODE_RESOLVE) {
       taxon = p.codes_in[g];                                 // merged dense ids of all database ranges
       if (taxon == FOUND_ZERO) taxon = 0;                    // a stored taxon 0 counts like a miss from here on
@@ -593,8 +594,14 @@ __device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint3
             // keys once per run; a record whose key is kept already (KEPT_BIT) needs no flag.  A stale
             // (non-coherent) load can only miss a flag another thread just set: the atomicOr is then redundant,
             // never wrong.
-            if (mark_seen && taxon != 0 && taxon != FOUND_ZERO && !(hiw & (SEEN_BIT | KEPT_BIT)))
-              atomicOr(const_cast<uint32_t *>(b + 3 * t + 1), SEEN_BIT);
+            // Keep mode (F_KEEP) skips the flag and the harvest: the record becomes kept here, unless its taxon is dense
+            // already (as keep_record decides).  Other windows may sight the record in this step too: only the one whose
+            // atomic found KEPT_BIT clear counts it, through its code (k_resolve).
+            if (mark_seen && taxon != 0 && taxon != FOUND_ZERO && !(hiw & (SEEN_BIT | KEPT_BIT))) {
+              uint32_t *w = const_cast<uint32_t *>(b + 3 * t + 1);
+              if (!keep) atomicOr(w, SEEN_BIT);
+              else if (!p.dense_flag[taxon] && !(atomicOr(w, KEPT_BIT) & KEPT_BIT)) kept_new = KEEP_NEW;
+            }
             m = 0;
           }
         }
@@ -612,7 +619,7 @@ __device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint3
         p.peer_codes[j][g] = taxon;
       }
     } else if (MODE == MODE_RESOLVE || !only_hits || taxon != 0) {
-      p.codes_dense[g] = taxon;
+      p.codes_dense[g] = taxon | kept_new;
     }
     if (MODE == MODE_LOOKUP && shard_counting) {
       if (taxon != 0 && taxon != FOUND_ZERO) hll_update(p.regs, taxon, fmix64(canon));
@@ -811,8 +818,12 @@ __device__ uint32_t resolve_overflow(const Params &p, const OverflowPool &pool, 
   };
   // hit_counts[taxon]++ over all windows
   for (uint32_t i = lane; i < nwin; i += 32) {
-    const uint32_t t = codes_src[out_base + i];
+    uint32_t t = codes_src[out_base + i];
     if (t == AMBIG || t == 0) continue;
+    if (t & KEEP_NEW) {                               // rare path: the record's new distinct code is booked right here
+      t &= ~KEEP_NEW;
+      if (counting) atomicAdd(p.sparse.distinct + t, 1u);
+    }
     uint32_t s = (uint32_t)mix64(t) & (cap - 1);
     for (;;) {
       unsigned long long e = *reinterpret_cast<volatile unsigned long long *>(tab + 2 * s);
@@ -896,7 +907,7 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
   // the run cursor, n_kmers[0] and n_reads[0].  Each warp therefore allocates run slots in blocks of RUN_BLOCK
   // and keeps the hot counters in registers until it is done.
   uint32_t blk_next = 0, blk_end = 0;                           // this warp's block of run slots
-  uint32_t acc_miss = 0, acc_unclassified = 0, acc_classified = 0;
+  uint32_t acc_miss = 0, acc_unclassified = 0, acc_classified = 0, acc_kept = 0;
   uint32_t unit_cur = 0xFFFFFFFFu, unit_miss = 0;               // misses of the current work unit, not yet booked
   const bool units = counting && p.hll_mode == 0u && p.unit_id;
   const uint32_t unit_row0 = units ? p.unit_id[0] : 0u;
@@ -956,6 +967,7 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
       if (units) unit_b = p.unit_id[r + 2];
     }
     uint32_t my_t = 0, my_c = 0;                                // hit list: lane j holds entry j (dense id, count)
+    uint32_t my_k = 0;                                          // F_KEEP: windows of entry j that made their record kept
     uint32_t n_hits = 0, n_miss = 0, n_runs = 0;
     uint32_t carry_code = 0;
     bool overflow = false;
@@ -968,7 +980,9 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
       const bool valid = i < nwin;
       const bool amb = valid && c == AMBIG;
       const bool look = valid && !amb;
-      const uint32_t taxon = look ? c : 0;
+      const uint32_t taxon = look ? c & ~KEEP_NEW : 0;
+      const uint32_t kept_m = __ballot_sync(0xFFFFFFFFu, look && (c & KEEP_NEW));
+      acc_kept += __popc(kept_m);
       const uint32_t out_code = amb ? AMBIG : taxon;
       if (want_codes && valid) p.codes[out_base + i] = amb ? AMBIG : (taxon ? __ldg(p.tax.raw + taxon) : 0u);
       // runs of the hit list
@@ -994,13 +1008,13 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
         const int ldr = __ffs(rem) - 1;
         const uint32_t t = __shfl_sync(0xFFFFFFFFu, taxon, ldr);
         const uint32_t same = __ballot_sync(0xFFFFFFFFu, look && taxon == t) & rem;
-        const uint32_t cnt = __popc(same);
+        const uint32_t cnt = __popc(same), kcnt = __popc(same & kept_m);
         rem &= ~same;
         const uint32_t pos = __ballot_sync(0xFFFFFFFFu, lane < n_hits && my_t == t);
         if (pos) {
-          if (lane == (uint32_t)(__ffs(pos) - 1)) my_c += cnt;
+          if (lane == (uint32_t)(__ffs(pos) - 1)) { my_c += cnt; my_k += kcnt; }
         } else if (n_hits < 32) {
-          if (lane == n_hits) { my_t = t; my_c = cnt; }
+          if (lane == n_hits) { my_t = t; my_c = cnt; my_k = kcnt; }
           n_hits++;
         } else {
           overflow = true;
@@ -1071,7 +1085,10 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
       if (lane < n_hits) book_unit(unit, my_t, my_c);
     }
     if (counting) {
-      if (lane < n_hits) atomicAdd(p.n_kmers + my_t, (unsigned long long)my_c);
+      if (lane < n_hits) {
+        atomicAdd(p.n_kmers + my_t, (unsigned long long)my_c);
+        if (my_k) atomicAdd(p.sparse.distinct + my_t, my_k);
+      }
       acc_miss += n_miss;
       if (call) {
         acc_classified++;
@@ -1120,6 +1137,7 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
           bool valid = i < nwin;
           auto code_at = [&](uint32_t w) {
             uint32_t c = codes_src[out_base + w];
+            if (c != AMBIG) c &= ~KEEP_NEW;
             return c == AMBIG ? AMBIG : (c ? __ldg(p.tax.raw + c) : 0u);
           };
           uint32_t c = valid ? code_at(i) : 0;
@@ -1145,6 +1163,7 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
     if (acc_miss) atomicAdd(p.n_kmers, (unsigned long long)acc_miss);
     if (acc_unclassified) atomicAdd(p.n_reads_ctr, (unsigned long long)acc_unclassified);
     if (acc_classified) atomicAdd(p.n_classified, (unsigned long long)acc_classified);
+    if (acc_kept) atomicAdd(p.n_new_kept, (unsigned long long)acc_kept);
   }
 }
 
@@ -1232,7 +1251,7 @@ __global__ void __launch_bounds__(256) k_unit_decide(const __grid_constant__ Par
       const uint64_t base = p.offsets[r];
       const uint32_t nwin = p.n_windows[r];
       for (uint32_t i = lane; i < nwin; i += 32) {
-        if (p.codes_dense[base + i] != taxon) continue;
+        if ((p.codes_dense[base + i] & ~KEEP_NEW) != taxon) continue;     // AMBIG & ~KEEP_NEW is no dense id
         atomicMax(&s_last, ((unsigned long long)r << 32) | i);
         if (*v_distinct >= 1025u) continue;
         const uint32_t code = encode_hash32(fmix64(window_canon(p, base + i)));     // never 0
@@ -1772,6 +1791,31 @@ __global__ void k_fold_secondaries(uint8_t *pairs, const uint2 *list, uint64_t n
     *ws = hiw & ~SEEN_BIT;                                 // a record is the secondary of one entry only
     atomicOr(reinterpret_cast<uint32_t *>(pairs + (uint64_t)sp.y * 12) + 1, SEEN_BIT);
   }
+}
+
+// Keep mode counts every record whose KEPT_BIT it set, secondaries included: the flag moves to the primary, and a
+// primary that had it already (two members of the group were kept) held the code already.  Order-independent.
+__global__ void k_settle_kept(uint8_t *pairs, const uint2 *list, uint64_t n, uint32_t *distinct, unsigned long long *n_dup) {
+  unsigned long long dup = 0;
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint2 sp = list[e];                              // (secondary, primary) record indices
+    uint32_t *ws = reinterpret_cast<uint32_t *>(pairs + (uint64_t)sp.x * 12) + 1;
+    const uint32_t hiw = *ws;
+    if (!(hiw & KEPT_BIT)) continue;
+    *ws = hiw & ~KEPT_BIT;
+    if (atomicOr(reinterpret_cast<uint32_t *>(pairs + (uint64_t)sp.y * 12) + 1, KEPT_BIT) & KEPT_BIT) {
+      atomicSub(distinct + ws[1], 1u);                     // ws[1]: the taxon, the same for the whole group
+      dup++;
+    }
+  }
+  for (int o = 16; o; o >>= 1) dup += __shfl_xor_sync(0xFFFFFFFFu, dup, o);
+  if ((threadIdx.x & 31) == 0 && dup) atomicAdd(n_dup, dup);
+}
+void launch_settle_kept(uint8_t *pairs, const uint2 *secondaries, uint64_t n_secondaries, uint32_t *distinct,
+                        unsigned long long *n_dup, cudaStream_t stream) {
+  if (!n_secondaries) return;
+  k_settle_kept<<<(int)min((uint64_t)device_sm_count() * 8, (n_secondaries + 255) / 256), 256, 0, stream>>>(
+      pairs, secondaries, n_secondaries, distinct, n_dup);
 }
 
 // k_harvest_keep streams the records in groups of 4 (48 bytes = three 16-byte loads, KEEP_UNROLL groups in flight per

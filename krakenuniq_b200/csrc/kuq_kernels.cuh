@@ -48,6 +48,12 @@ constexpr uint32_t SEEN_BIT = 0x80000000u;
 // Second record flag (bit 62, free for k <= 31): "this record's (taxon, encoded hash) is a key of the sparse tier".
 // Only one record per (taxon, code) carries it — the primary of its collision group (kuq_api.cu, build_collisions).
 constexpr uint32_t KEPT_BIT = 0x40000000u;
+// Params::flags bit of a fused call that keeps records at their first sighting (keep mode): the lookup sets KEPT_BIT
+// itself instead of SEEN_BIT, and marks the window whose atomic made the record kept with KEEP_NEW in codes_dense;
+// k_resolve counts those windows into distinct[taxon] and *n_new_kept.  Secondaries of collision groups can become kept
+// too; settle_kept (kuq_api.cu) hands their flag to the primary and takes the duplicate count back.
+constexpr uint32_t F_KEEP = 64u;
+constexpr uint32_t KEEP_NEW = 0x80000000u;   // never part of a dense id; AMBIG carries it too, so test AMBIG first
 constexpr int SEARCH_WINDOW = 8;           // records scanned linearly once the bisection window is this small
 constexpr uint32_t MAX_DBS = 8;            // databases one launch of the in-order lookup asks (Params::dbs)
 
@@ -246,6 +252,7 @@ struct Params {
   unsigned long long *n_reads_ctr; // [n_taxa]
   uint8_t *dense_flag;          // [n_sketch]
   SparseSet sparse;
+  unsigned long long *n_new_kept;  // F_KEEP: records the batch made kept (k_resolve adds them)
   UnitMap units;
   // pool for the hit tables of reads with more than 32 distinct taxa (2 u64 per entry)
   unsigned long long *ovf_mem;
@@ -299,6 +306,10 @@ void launch_harvest_seen(uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, cons
 // 4-byte aligned; dense_flag has n_sketch entries, and every record's taxon is below n_sketch.
 void launch_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint2 *secondaries, uint64_t n_secondaries, const uint8_t *dense_flag,
                          uint32_t n_sketch, uint32_t *distinct, unsigned long long *n_kept, cudaStream_t stream);
+// after keep-mode calls: a kept secondary hands KEPT_BIT to its primary; where the primary had it already the code was
+// counted twice, so distinct[taxon] drops by one and *n_dup grows by one
+void launch_settle_kept(uint8_t *pairs, const uint2 *secondaries, uint64_t n_secondaries, uint32_t *distinct,
+                        unsigned long long *n_dup, cudaStream_t stream);
 // kuq_collisions.cu: (secondary, primary) record pairs of every (taxon, code) group of the staged records
 int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint64_t *records_of_taxon, uint32_t n_sketch,
                      uint64_t max_entries, uint2 **list_out, uint64_t *n_out, int n_sm, cudaStream_t stream);
