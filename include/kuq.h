@@ -60,7 +60,9 @@ extern "C" {
 #define KUQ_HLL_DENSE_ONLY 2 /* p=12 registers only, no sparse-tier emulation (fastest; estimates = dense Ertl) */
 #define KUQ_HLL_EXACT 3     /* classifyExact (EXACT_COUNTING, classify.cpp:46-49): sets of k-mers instead of sketches;
                                `unique` of kuq_read_counts / kuq_clade_counts is the exact set / union size.  The
-                               (taxon, k-mer) table takes kuq_config.sparse_set_slots entries of 16 bytes. */
+                               (taxon, k-mer) table starts with kuq_config.sparse_set_slots entries of 16 bytes and
+                               grows before a batch whose windows could take it past a load factor of 0.8
+                               (kuq_exact_info); kuq_merge_into unites the sets of two contexts. */
 
 /* flags of the classify calls */
 #define KUQ_F_WANT_CODES 1u     /* also return the per-window codes (4 B per base position) */
@@ -79,7 +81,8 @@ typedef struct kuq_config {
   uint32_t hll_mode;             /* KUQ_HLL_* */
   uint32_t reserved0;
   uint64_t sparse_set_slots;     /* capacity (slots of 8 B) of the device set that backs the sparse HLL tier;
-                                    0 → 1<<26 */
+                                    KUQ_HLL_EXACT: initial entries (16 B) of the exact k-mer set.  Both grow on
+                                    demand.  0 → 1<<26 */
 } kuq_config;
 
 /* One run of the Kraken hit list: `code:count` (classify.cpp:826-861). code = taxid, 0 (miss) or KUQ_CODE_AMBIG */
@@ -353,6 +356,24 @@ int kuq_sparse_export(kuq_ctx *ctx, uint64_t *d_keys_out, uint64_t cap, uint64_t
  * records into (taxon, encoded hash) keys, growing the set first when it would pass a load factor of 0.7. */
 int kuq_sparse_tier_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *keys, uint64_t *times_grown, double *last_harvest_ms);
 int kuq_sparse_import(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n);
+/* ---- the exact k-mer set (KUQ_HLL_EXACT) ----------------------------------------------------------------------------
+ * One open-addressing table of (taxon, canonical k-mer) pairs holds the k-mer sets of all taxa.  Before each batch the
+ * library bounds the pairs it could add (one per window); when the bound could take the table past a load factor of 0.8
+ * it reads the real fill back, and only when that does not fit either does it re-allocate the table at a load of at most
+ * 0.6 (all slots drained first).  A growth that finds no device memory fails with KUQ_E_NOMEM.
+ * kuq_exact_info: the table's capacity in slots, the pairs it holds (= the sum of the per-taxon set sizes) and how often
+ * it grew.  Not KUQ_HLL_EXACT: 0 slots, 0 pairs. */
+int kuq_exact_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *pairs, uint64_t *times_grown);
+/* Pair layout of kuq_exact_export / kuq_exact_import: 16 bytes, 16-byte aligned,
+ *     { uint64_t kmer_plus_1;    canonical k-mer + 1
+ *       uint64_t taxon_plus_1; } dense taxon id + 1 (kuq_dense_taxids numbers them)
+ * kuq_exact_export writes every pair of the table to d_pairs_out (HBM, order unspecified; pass NULL / cap 0 to query *n
+ * first).  kuq_exact_import inserts pairs into this context's table, growing it first when they need room; a pair the
+ * table holds already is not counted again, so importing is set union.  Dense ids only mean the same taxon in two
+ * contexts that number their taxa identically: the same database ranges' taxids (kuq_set_db_taxid_universe) and the same
+ * taxonomy, which kuq_merge_into checks and callers of these two calls must ensure. */
+int kuq_exact_export(kuq_ctx *ctx, void *d_pairs_out, uint64_t cap, uint64_t *n);
+int kuq_exact_import(kuq_ctx *ctx, const void *d_pairs, uint64_t n);
 /* ---- database sharded by minimizer range over the GPUs of a node (SURVEY.md §8(e).2) ------------------------------
  * Who counts: with kuq_set_shard_counting(on) the GPU that FINDS a hit does that hit's sketch work inside the lookup
  * half (kuq_lookup_device / kuq_lookup_device_peers): HLL register update and the record flag behind the sparse tier;

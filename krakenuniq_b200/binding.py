@@ -162,6 +162,9 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_sparse_import": (C.c_int, [vp, vp, C.c_uint64]),
         "kuq_reset_counts": (C.c_int, [vp]),
         "kuq_sparse_tier_info": (C.c_int, [vp, u64p, u64p, u64p, C.POINTER(C.c_double)]),
+        "kuq_exact_info": (C.c_int, [vp, u64p, u64p, u64p]),
+        "kuq_exact_export": (C.c_int, [vp, vp, C.c_uint64, u64p]),
+        "kuq_exact_import": (C.c_int, [vp, vp, C.c_uint64]),
         "kuq_set_shard_counting": (C.c_int, [vp, C.c_int]),
         "kuq_set_stats": (C.c_int, [vp, C.c_int]),
         "kuq_merge_into": (C.c_int, [vp, vp]),
@@ -604,6 +607,21 @@ class Classifier:
         a, b, c, d = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_double()
         self._ck(self.L.kuq_sparse_tier_info(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return {"slots": a.value, "keys": b.value, "times_grown": c.value, "last_harvest_ms": d.value}
+
+    def exact_info(self):
+        """kuq_exact_info: capacity, pairs held and growths of the exact k-mer set (HLL_EXACT)"""
+        a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        self._ck(self.L.kuq_exact_info(self.h, C.byref(a), C.byref(b), C.byref(c)))
+        return {"slots": a.value, "pairs": b.value, "times_grown": c.value}
+
+    def exact_export(self, d_out=None, cap=0):
+        """kuq_exact_export: pairs (16 B: k-mer + 1, dense taxon + 1) into device memory; without a buffer → their number"""
+        n = C.c_uint64(0)
+        self._ck(self.L.kuq_exact_export(self.h, d_out, cap, C.byref(n)))
+        return n.value
+
+    def exact_import(self, d_pairs, n):
+        self._ck(self.L.kuq_exact_import(self.h, d_pairs, n))
 
     def layout_experiment(self, slot, n_positions, reps=5):
         """kuq_layout_experiment: record layout x search shape of the bin search, timed on the windows of the slot's

@@ -1676,19 +1676,14 @@ int main(int argc, char **argv) {
   // is also the reference's rule for several databases (resident, streamed or sharded)
   cfg.hll_mode = (Populate_memory_size > 0 || ((chunk_budget || want_shards) && n_db == 1)) ? KUQ_HLL_CHUNKED : KUQ_HLL_PRELOAD;
 #ifdef EXACT_COUNTING
-  // classifyExact (classify.cpp:46-49): sets of k-mers instead of sketches; work units and chunks make no difference
+  // classifyExact (classify.cpp:46-49): sets of k-mers instead of sketches.  Work units, chunks and devices make no
+  // difference to a union of sets, so replicas and shards run as for classify and kuq_merge_into unites the sets.
   cfg.hll_mode = KUQ_HLL_EXACT;
-  if (want_shards) {                           // exact sets are not merged across devices
-    want_shards = false;
-    chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30);
-    if (n_db > 1) cerr << "classify: classifyExact streams several databases through one GPU instead of sharding them "
-                          "(exact k-mer sets are not merged across devices)" << endl;
-  }
   if (Quick_mode) die(EX_USAGE, "-q is not supported by the GPU classifyExact");
 #endif
   if ((chunk_budget || want_shards) && !Populate_memory_size && n_db == 1)
     cerr << "classify: database larger than one GPU's HBM budget: " << (want_shards ? "sharding it over the GPUs" : "processing it in ranges")
-         << " (unique k-mer counts follow the -x rule)" << endl;
+         << (cfg.hll_mode == KUQ_HLL_EXACT ? "" : " (unique k-mer counts follow the -x rule)") << endl;
   if (getenv("KUQ_SPARSE_SLOTS")) cfg.sparse_set_slots = strtoull(getenv("KUQ_SPARSE_SLOTS"), NULL, 10);
   if (getenv("KUQ_DEVICE")) cfg.device = atoi(getenv("KUQ_DEVICE"));
   // devices: KUQ_DEVICES=0,2,3 (or "all"); default = every visible sm_90 GPU when the databases are replicated (they fit
@@ -1696,8 +1691,7 @@ int main(int argc, char **argv) {
   vector<int> devices;
   {
     const char *dl = getenv("KUQ_DEVICES");
-    const bool replicable = !chunk_budget && cfg.hll_mode != KUQ_HLL_EXACT;   // exact k-mer sets are not merged across devices
-    // (replicas when the database fits a card, shards when it only fits the cards together)
+    const bool replicable = !chunk_budget;   // replicas when the database fits a card, shards when it only fits the cards together
     if (dl && strcmp(dl, "all") != 0) {
       for (const char *q = dl; *q;) { devices.push_back(atoi(q)); while (*q && *q != ',') q++; if (*q) q++; }
     } else if ((dl || !getenv("KUQ_DEVICE")) && replicable) {
@@ -1796,8 +1790,20 @@ int main(int argc, char **argv) {
   else if (chunk_budget) run_streamed(ctx, kdbs, idxs, chunk_budget, hbm_budget, argc, argv, db_counts);
   else for (int i = optind; i < argc; i++) process_file(ctx, argv[i]);
   // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
-  for (size_t g = 1; g < All_ctx.size(); g++)
-    if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+  {
+    double T0__ = now_s();
+    for (size_t g = 1; g < All_ctx.size(); g++)
+      if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+    if (All_ctx.size() > 1) TICK("merge");
+#ifdef EXACT_COUNTING
+    for (size_t g = 0; g < All_ctx.size() && Timing; g++) {
+      uint64_t slots = 0, pairs = 0, grown = 0;
+      if (kuq_exact_info(All_ctx[g], &slots, &pairs, &grown)) die(EX_SOFTWARE, kuq_last_error(All_ctx[g]));
+      fprintf(stderr, "[timing] exact set of context %zu: %llu slots, %llu pairs, grown %llu times\n", g, (unsigned long long)slots,
+              (unsigned long long)pairs, (unsigned long long)grown);
+    }
+#endif
+  }
   gettimeofday(&tv2, NULL);
   {                                                                 // report_stats, classify.cpp:361-375
     double seconds = get_seconds(tv1, tv2);

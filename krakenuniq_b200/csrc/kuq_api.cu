@@ -143,6 +143,8 @@ struct kuq_ctx {
   ExactPair *d_exact = nullptr;           // KUQ_HLL_EXACT: the (taxon, k-mer) table and the per-taxon set sizes
   unsigned long long *d_exact_count = nullptr;
   uint64_t exact_cap = 0;
+  uint64_t exact_upper = 0;               // upper bound of the pairs in that table (reserve_exact_inserts)
+  uint64_t exact_grown = 0;               // times it was re-allocated
 
   // database streamed through HBM range by range (kuq_stream_*): two device buffers, one copy stream
   struct StreamBuf {
@@ -485,7 +487,8 @@ int finalize(kuq_ctx *ctx) {
   CU(cudaMemset(ctx->d_n_kmers, 0, ctx->n_sketch * 8ull));
   CU(cudaMemset(ctx->d_n_reads, 0, ctx->n_taxa * 8ull));
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
-    ctx->exact_cap = ctx->cfg.sparse_set_slots;            // entries of 16 B
+    ctx->exact_cap = ctx->cfg.sparse_set_slots;            // entries of 16 B; grows before batches that could fill it
+    ctx->exact_upper = 0;
     CU(dmalloc(&ctx->d_exact, ctx->exact_cap));
     CU(dmalloc(&ctx->d_exact_count, ctx->n_sketch));
     CU(cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull));
@@ -571,32 +574,174 @@ int grow_sparse_set(kuq_ctx *ctx, uint64_t cap) {
   return KUQ_OK;
 }
 
-// Misses and the resolve half insert (taxon, code) pairs straight into the set — at most one per window of the batch.  Make room
-// BEFORE the batch instead of failing in the middle of it: `direct_upper` bounds the keys inserted that way since the
-// last exact count; when the bound says the set could pass a load factor of 0.8 the exact fill is read back, and only
-// if that still does not fit the set doubles (all slots drained first).
-int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
-  if (!ctx->d_sparse_slots) return KUQ_OK;
-  if ((ctx->direct_upper + windows) * 10 <= ctx->sparse_cap * 8) { ctx->direct_upper += windows; return KUQ_OK; }
+// Room for `incoming` more keys in an open-addressing table of `cap` slots, made BEFORE a batch instead of failing in the
+// middle of it: `upper` bounds the keys in the table since the last exact count; when the bound says the table could
+// pass a load factor of 0.8, `fill` reads the exact count back (all slots drained first), and only if that still does
+// not fit does `grow` re-allocate the table at a load factor of at most 0.6.  The sparse-tier set and the exact set
+// both grow by this rule.
+template <typename Fill, typename Grow>
+int reserve_room(kuq_ctx *ctx, uint64_t &upper, uint64_t cap, uint64_t incoming, Fill fill, Grow grow) {
+  if ((upper + incoming) * 10 <= cap * 8) { upper += incoming; return KUQ_OK; }
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  std::vector<uint32_t> distinct(ctx->n_sketch);
-  CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
   uint64_t used = 0;
-  for (uint32_t v : distinct) used += v;
-  // keys of kept records live in the records, not in the set; those of keep-mode calls since the last settle_kept are
-  // counted in distinct[] and in d_harvest_stat[2] alike (duplicates of collision groups included)
-  unsigned long long pending = 0;
-  if (ctx->keep_dirty) CU(cudaMemcpy(&pending, ctx->d_harvest_stat + 2, 8, cudaMemcpyDeviceToHost));
-  used -= std::min<uint64_t>(used, ctx->kept_keys + pending);
-  ctx->direct_upper = used;
-  if ((used + windows) * 10 > ctx->sparse_cap * 8) {
-    uint64_t cap = ctx->sparse_cap;
-    while ((used + windows) * 10 > cap * 6) cap <<= 1;
-    int rc = grow_sparse_set(ctx, cap);
+  int rc = fill(&used);
+  if (rc) return rc;
+  upper = used;
+  if ((used + incoming) * 10 > cap * 8) {
+    uint64_t c = cap;
+    while ((used + incoming) * 10 > c * 6) c <<= 1;
+    rc = grow(c);
     if (rc) return rc;
   }
-  ctx->direct_upper += windows;
+  upper += incoming;
   return KUQ_OK;
+}
+
+// Misses and the resolve half insert (taxon, code) pairs straight into the set — at most one per window of the batch.
+int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
+  if (!ctx->d_sparse_slots) return KUQ_OK;
+  auto fill = [ctx](uint64_t *used) -> int {
+    std::vector<uint32_t> distinct(ctx->n_sketch);
+    CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
+    uint64_t n = 0;
+    for (uint32_t v : distinct) n += v;
+    // keys of kept records live in the records, not in the set; those of keep-mode calls since the last settle_kept are
+    // counted in distinct[] and in d_harvest_stat[2] alike (duplicates of collision groups included)
+    unsigned long long pending = 0;
+    if (ctx->keep_dirty) CU(cudaMemcpy(&pending, ctx->d_harvest_stat + 2, 8, cudaMemcpyDeviceToHost));
+    *used = n - std::min<uint64_t>(n, ctx->kept_keys + pending);
+    return KUQ_OK;
+  };
+  return reserve_room(ctx, ctx->direct_upper, ctx->sparse_cap, windows, fill, [ctx](uint64_t cap) { return grow_sparse_set(ctx, cap); });
+}
+
+// ---- the exact k-mer set (KUQ_HLL_EXACT) grows like the sparse-tier set ---------------------------------------------
+// Re-allocate the (taxon, k-mer) table with `cap` slots and move its pairs over (not counted again).  All slots must be idle.
+int grow_exact_set(kuq_ctx *ctx, uint64_t cap) {
+  ExactPair *bigger = nullptr;
+  if (dmalloc(&bigger, cap) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no room to grow from %llu to %llu slots (%.2f GiB)", (unsigned long long)ctx->exact_cap,
+                (unsigned long long)cap, cap * 16.0 / (1ull << 30));
+  }
+  uint32_t *d_err = nullptr;
+  CU(dmalloc(&d_err, 1));
+  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
+  CU(cudaMemsetAsync(bigger, 0, cap * 16ull, ctx->aux));
+  const ExactSet nb{bigger, cap - 1, ctx->d_exact_count};
+  launch_exact_rehash(ctx->d_exact, ctx->exact_cap, nb, d_err, ctx->aux);
+  ctx->launches++;
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_err);
+  if (err) { cudaFree(bigger); return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated while growing to %llu slots", (unsigned long long)cap); }
+  cudaFree(ctx->d_exact);
+  ctx->d_exact = bigger;
+  ctx->exact_cap = cap;
+  ctx->exact_grown++;
+  return KUQ_OK;
+}
+
+// pairs in the table: every pair was counted once, under its taxon
+int exact_pairs(kuq_ctx *ctx, uint64_t *n) {
+  std::vector<unsigned long long> count(ctx->n_sketch);
+  CU(cudaMemcpy(count.data(), ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+  *n = 0;
+  for (unsigned long long v : count) *n += v;
+  return KUQ_OK;
+}
+
+// A batch adds at most one pair per non-ambiguous window; an import at most one per incoming pair.
+int reserve_exact_inserts(kuq_ctx *ctx, uint64_t incoming) {
+  if (!ctx->d_exact) return KUQ_OK;
+  return reserve_room(ctx, ctx->exact_upper, ctx->exact_cap, incoming, [ctx](uint64_t *used) { return exact_pairs(ctx, used); },
+                      [ctx](uint64_t cap) { return grow_exact_set(ctx, cap); });
+}
+
+// Occupied slots [lo, hi) of the table into out (cap pairs; cap 0 only counts); *n = their number.  All slots idle.
+int exact_export_range(kuq_ctx *ctx, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t cap, uint64_t *n) {
+  unsigned long long *d_n = nullptr;
+  CU(dmalloc(&d_n, 1));
+  CU(cudaMemsetAsync(d_n, 0, 8, ctx->aux));
+  launch_exact_export(ctx->d_exact, lo, hi, out, out ? cap : 0, d_n, ctx->aux);
+  ctx->launches++;
+  unsigned long long cnt = 0;
+  CU(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_n);
+  *n = cnt;
+  if (out && cnt > cap) return fail(ctx, KUQ_E_CAPACITY, "need room for %llu pairs", cnt);
+  return KUQ_OK;
+}
+
+// pairs of another context (ExactPair layout) into the table, grown first when they need room.  All slots idle.
+int exact_import(kuq_ctx *ctx, const ExactPair *d_pairs, uint64_t n) {
+  int rc = reserve_exact_inserts(ctx, n);
+  if (rc) return rc;
+  ctx->snap_valid = false;
+  uint32_t *d_err = nullptr;
+  CU(dmalloc(&d_err, 1));
+  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
+  const ExactSet es{ctx->d_exact, ctx->exact_cap - 1, ctx->d_exact_count};
+  launch_exact_import(d_pairs, n, es, d_err, ctx->aux);
+  ctx->launches++;
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_err);
+  if (err) return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated while importing (%llu slots)", (unsigned long long)ctx->exact_cap);
+  return KUQ_OK;
+}
+
+// a batch's kernels found the set they insert into full (error code 4)
+int batch_set_saturated(kuq_ctx *ctx) {
+  if (ctx->cfg.hll_mode == KUQ_HLL_EXACT)
+    return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated (%llu slots)", (unsigned long long)ctx->exact_cap);
+  return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated: raise kuq_config.sparse_set_slots (now %llu)", (unsigned long long)ctx->sparse_cap);
+}
+
+// kuq_merge_into under KUQ_HLL_EXACT: src's pairs move to dst in rounds over at most 2^22 slots of src's table (64 MiB
+// of pairs per round on each side; KUQ_EXACT_MERGE_SLOTS overrides it, so that tests of the rounds can use small tables)
+// — compacted on src's device, copied peer to peer when the devices differ, imported on dst's (count[] grows by the pairs
+// dst did not hold yet).  Union does not depend on order, so dst ends with the set one context would have built.
+// The slots of both contexts must be idle.
+int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
+  kuq_ctx *ctx = dst;
+  if (!src->d_exact || !dst->d_exact) return KUQ_OK;
+  uint64_t round_slots = 1ull << 22;
+  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+  const uint64_t chunk = std::min(round_slots, src->exact_cap);
+  const bool same_device = src->device == dst->device;
+  ExactPair *d_src = nullptr, *d_dst = nullptr;
+  CU(cudaSetDevice(src->device));
+  if (dmalloc(&d_src, chunk) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set merge: no room for %llu pairs on device %d", (unsigned long long)chunk, src->device);
+  }
+  int rc = KUQ_OK;
+  if (!same_device) {
+    CU(cudaSetDevice(dst->device));
+    if (dmalloc(&d_dst, chunk) != cudaSuccess) {
+      (void)cudaGetLastError();
+      rc = fail(ctx, KUQ_E_NOMEM, "exact k-mer set merge: no room for %llu pairs on device %d", (unsigned long long)chunk, dst->device);
+    }
+  }
+  for (uint64_t lo = 0; lo < src->exact_cap && !rc; lo += chunk) {
+    uint64_t n = 0;
+    CU(cudaSetDevice(src->device));
+    rc = exact_export_range(src, lo, std::min(lo + chunk, src->exact_cap), d_src, chunk, &n);
+    if (rc) { dst->err = src->err; break; }
+    if (!n) continue;
+    CU(cudaSetDevice(dst->device));
+    if (!same_device) CU(cudaMemcpyPeer(d_dst, dst->device, d_src, src->device, n * 16));
+    rc = exact_import(dst, same_device ? d_src : d_dst, n);
+  }
+  cudaSetDevice(src->device);
+  cudaFree(d_src);
+  cudaSetDevice(dst->device);
+  if (d_dst) cudaFree(d_dst);
+  return rc;
 }
 
 // Build the collision table of the staged range once, the first time keep mode or a harvest can use the record tier.
@@ -1025,6 +1170,14 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
     // the set may have moved
     p.sparse.slots = ctx->d_sparse_slots;
     p.sparse.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0;
+  }
+  // exact counting: the batch's windows go into the (taxon, k-mer) table, which grows before the batch when they could
+  // fill it
+  if ((mode == MODE_RESOLVE || mode == MODE_FUSED) && !(p.flags & 4u) && ctx->cfg.hll_mode == KUQ_HLL_EXACT && p.n_reads) {
+    int rrc = reserve_exact_inserts(ctx, s.total_bases);
+    if (rrc) return rrc;
+    p.exact.slots = ctx->d_exact;
+    p.exact.mask = ctx->exact_cap - 1;
   }
   const bool units = mode != MODE_LOOKUP && ctx->cfg.hll_mode == KUQ_HLL_PRELOAD && p.unit_id && !(p.flags & 4u);
   if (units) {
@@ -1594,7 +1747,7 @@ int kuq_wait_batch(kuq_ctx *ctx, uint32_t slot, kuq_batch_result *out) {
   s.kernel_ms = ms;
   const uint32_t err = (uint32_t)(s.h_scalars[3] & 0xFFFFFFFFu);
   if (err == 1) return fail(ctx, KUQ_E_TAXA_OVERFLOW, "the batch exhausted the hit-table pool for reads with more than 32 distinct taxa: use smaller batches");
-  if (err == 4) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated: raise kuq_config.sparse_set_slots (now %llu)", (unsigned long long)ctx->sparse_cap);
+  if (err == 4) return batch_set_saturated(ctx);
   if (err == 5) return fail(ctx, KUQ_E_CAPACITY, "the hit lists of the batch need more run slots than the slot holds (%llu): use smaller batches", (unsigned long long)s.runs_cap);
   if (err) return fail(ctx, KUQ_E_CAPACITY, "per-batch work-unit bookkeeping overflowed (code %u): use smaller batches", err);
   const uint64_t n_runs = (s.flags & KUQ_F_NO_RUNS) ? 0 : s.h_scalars[0];
@@ -1812,7 +1965,7 @@ int kuq_sync_slot(kuq_ctx *ctx, uint32_t slot) {
   }
   CU(cudaMemcpy(&err, reinterpret_cast<uint32_t *>(s.d_scalars + 3), 4, cudaMemcpyDeviceToHost));
   if (err == 1) return fail(ctx, KUQ_E_TAXA_OVERFLOW, "the batch exhausted the hit-table pool for reads with more than 32 distinct taxa: use smaller batches");
-  if (err == 4) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated: raise kuq_config.sparse_set_slots (now %llu)", (unsigned long long)ctx->sparse_cap);
+  if (err == 4) return batch_set_saturated(ctx);
   if (err == 5) return fail(ctx, KUQ_E_CAPACITY, "the hit lists of the batch need more run slots than the slot holds (%llu): use smaller batches", (unsigned long long)s.runs_cap);
   if (err) return fail(ctx, KUQ_E_CAPACITY, "per-batch work-unit bookkeeping overflowed (code %u): use smaller batches", err);
   return KUQ_OK;
@@ -2601,14 +2754,14 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
   if (dst->n_taxa != src->n_taxa || dst->n_sketch != src->n_sketch || dst->raw_of_dense != src->raw_of_dense ||
       dst->cfg.hll_mode != src->cfg.hll_mode)
     return fail(ctx, KUQ_E_STATE, "the contexts number their taxa differently (different database / taxonomy / HLL mode)");
-  if (dst->cfg.hll_mode == KUQ_HLL_EXACT) return fail(ctx, KUQ_E_STATE, "kuq_merge_into does not merge exact k-mer sets");
+  const bool exact = dst->cfg.hll_mode == KUQ_HLL_EXACT;
   // src: flagged records → its set (skipping what dst already knows to be dense is a refinement left out)
   CU(cudaSetDevice(src->device));
   for (auto &s : src->slots) CU(cudaStreamSynchronize(s.stream));
   { int rc = harvest_seen(src, false); if (rc) { dst->err = src->err; return rc; } }
   uint64_t n_keys = 0;
   uint64_t *d_keys_src = nullptr;
-  if (src->d_sparse_slots) {
+  if (src->d_sparse_slots && !exact) {
     int rc = kuq_sparse_export(src, nullptr, 0, &n_keys);
     if (rc) { dst->err = src->err; return rc; }
     if (n_keys) {
@@ -2640,6 +2793,7 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
   dst->launches++;
   CU(cudaStreamSynchronize(dst->aux));
   cudaFree(t_regs); cudaFree(t_dense); cudaFree(t_nk); cudaFree(t_nr);
+  if (exact) return merge_exact_pairs(dst, src);
   int rc = KUQ_OK;
   if (n_keys && dst->d_sparse_slots) {
     uint64_t *d_keys_dst = nullptr;
@@ -2962,6 +3116,47 @@ int kuq_sparse_import(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   return KUQ_OK;
 }
 
+int kuq_exact_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *pairs, uint64_t *times_grown) {
+  if (!ctx) return KUQ_E_INVALID_ARG;
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  if (slots) *slots = ctx->exact_cap;
+  if (times_grown) *times_grown = ctx->exact_grown;
+  if (pairs) {
+    *pairs = 0;
+    if (ctx->d_exact) {
+      CU(cudaSetDevice(ctx->device));
+      for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+      rc = exact_pairs(ctx, pairs);
+      if (rc) return rc;
+    }
+  }
+  return KUQ_OK;
+}
+
+int kuq_exact_export(kuq_ctx *ctx, void *d_pairs_out, uint64_t cap, uint64_t *n) {
+  if (!ctx || !n) return KUQ_E_INVALID_ARG;
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  *n = 0;
+  if (!ctx->d_exact) return KUQ_OK;                           // not KUQ_HLL_EXACT
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  return exact_export_range(ctx, 0, ctx->exact_cap, static_cast<ExactPair *>(d_pairs_out), d_pairs_out ? cap : 0, n);
+}
+
+int kuq_exact_import(kuq_ctx *ctx, const void *d_pairs, uint64_t n) {
+  if (!ctx || (!d_pairs && n)) return KUQ_E_INVALID_ARG;
+  if ((uintptr_t)d_pairs & 15) return fail(ctx, KUQ_E_INVALID_ARG, "d_pairs must be 16-byte aligned");
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_import needs a KUQ_HLL_EXACT context");
+  if (!n) return KUQ_OK;
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  return exact_import(ctx, static_cast<const ExactPair *>(d_pairs), n);
+}
+
 int kuq_dense_taxids(kuq_ctx *ctx, uint32_t *taxid_of_dense, uint32_t cap, uint32_t *n) {
   if (!ctx || !n) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
@@ -2994,6 +3189,7 @@ int kuq_reset_counts(kuq_ctx *ctx) {
   if (ctx->d_exact) {
     CU(cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull));
     CU(cudaMemset(ctx->d_exact_count, 0, ctx->n_sketch * 8ull));
+    ctx->exact_upper = 0;
   }
   ctx->unit_nt = 0;
   ctx->unit_next = 0;

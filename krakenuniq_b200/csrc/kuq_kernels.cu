@@ -1448,6 +1448,55 @@ __global__ void __launch_bounds__(256) k_exact_insert(const __grid_constant__ Pa
   }
 }
 
+// the pairs of a table that is being replaced, into the bigger one with exact_insert's probe sequence; every pair is
+// counted already, so count[] stays as it is
+__global__ void k_exact_rehash(const ExactPair *old_slots, uint64_t old_cap, ExactSet e, uint32_t *error_flag) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x) {
+    const ExactPair pr = old_slots[i];
+    if (!pr.kmer1) continue;
+    if (exact_insert(e, (uint32_t)(pr.taxon1 - 1), pr.kmer1 - 1) < 0) atomicExch(error_flag, 4u);
+  }
+}
+void launch_exact_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream) {
+  if (old_cap) k_exact_rehash<<<(int)min((uint64_t)device_sm_count() * 16, (old_cap + 255) / 256), 256, 0, stream>>>(old_slots, old_cap, e, error_flag);
+}
+
+// occupied slots [lo, hi) → dense pairs: one cursor atomic per warp (out_cap 0 only counts them)
+__global__ void k_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t out_cap,
+                               unsigned long long *n_out) {
+  for (uint64_t i = lo + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (uint64_t)gridDim.x * blockDim.x) {
+    const ExactPair pr = slots[i];
+    const bool keep = pr.kmer1 != 0;
+    const uint32_t m = __ballot_sync(__activemask(), keep);
+    if (!keep) continue;
+    const uint32_t lane = threadIdx.x & 31;
+    unsigned long long base = 0;
+    const int leader = __ffs(m) - 1;
+    if ((int)lane == leader) base = atomicAdd(n_out, (unsigned long long)__popc(m));
+    base = __shfl_sync(m, base, leader);
+    const unsigned long long pos = base + __popc(m & ((1u << lane) - 1));
+    if (pos < out_cap) out[pos] = pr;
+  }
+}
+// pairs of another context into this table: only the ones it did not hold yet add to count[]
+__global__ void k_exact_import(const ExactPair *pairs, uint64_t n, ExactSet e, uint32_t *error_flag) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const ExactPair pr = pairs[i];
+    if (!pr.kmer1 || !pr.taxon1) continue;
+    const uint32_t taxon = (uint32_t)(pr.taxon1 - 1);
+    const int ins = exact_insert(e, taxon, pr.kmer1 - 1);
+    if (ins > 0) atomicAdd(e.count + taxon, 1ull);
+    else if (ins < 0) atomicExch(error_flag, 4u);
+  }
+}
+void launch_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t out_cap,
+                         unsigned long long *n_out, cudaStream_t stream) {
+  if (hi > lo) k_exact_export<<<(int)min((uint64_t)device_sm_count() * 16, (hi - lo + 255) / 256), 256, 0, stream>>>(slots, lo, hi, out, out_cap, n_out);
+}
+void launch_exact_import(const ExactPair *pairs, uint64_t n, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream) {
+  if (n) k_exact_import<<<(int)min((uint64_t)device_sm_count() * 16, (n + 255) / 256), 256, 0, stream>>>(pairs, n, e, error_flag);
+}
+
 // distinct k-mers among the pairs whose taxon is a clade member
 __global__ void k_exact_union(ExactSet e, const uint8_t *member, unsigned long long *scratch, uint64_t smask,
                               unsigned long long *n_distinct, uint32_t *overflow) {

@@ -331,6 +331,13 @@ void launch_sparse_histograms(const KeySource &src, const uint8_t *dense_flag, u
 // exact mode: distinct k-mers over the member taxa (set union of ReadCounts::operator+=, readcounts.hpp:76-81)
 void launch_exact_union(const ExactSet &e, const uint8_t *member, unsigned long long *scratch_set, uint64_t scratch_mask,
                         unsigned long long *n_distinct, uint32_t *overflow, cudaStream_t stream);
+// the pairs of old_slots[0, old_cap) into e without counting them again (growth of the exact set)
+void launch_exact_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
+// occupied slots [lo, hi) compacted into out (order unspecified); *n_out += their number, also beyond out_cap
+void launch_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t out_cap,
+                         unsigned long long *n_out, cudaStream_t stream);
+// pairs (layout of ExactPair) into e; count[taxon] grows by the pairs that were new
+void launch_exact_import(const ExactPair *pairs, uint64_t n, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
 void launch_sparse_union(const KeySource &src, const uint8_t *member,
                          unsigned long long *scratch_set, uint64_t scratch_mask, uint32_t *hist64, uint32_t *overflow,
                          cudaStream_t stream);
