@@ -62,7 +62,8 @@ extern "C" {
                                `unique` of kuq_read_counts / kuq_clade_counts is the exact set / union size.  The
                                (taxon, k-mer) table starts with kuq_config.sparse_set_slots entries of 16 bytes and
                                grows before a batch whose windows could take it past a load factor of 0.8
-                               (kuq_exact_info); kuq_merge_into unites the sets of two contexts. */
+                               (kuq_exact_info); kuq_merge_into unites the sets of two contexts, kuq_exact_partition
+                               and the kuq_exact_*partitioned calls spread them over contexts by k-mer. */
 
 /* flags of the classify calls */
 #define KUQ_F_WANT_CODES 1u     /* also return the per-window codes (4 B per base position) */
@@ -331,8 +332,10 @@ int kuq_clade_counts(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t 
  * one pass up the tree; dense clades (a member's sketch is dense: register-wise max, hyperloglogplus.cpp:604-621) by
  * one launch per 8192 clades; sparse clades (union of the members' code sets, :600-603) from ONE sort of the sparse
  * tier's keys by (code, preorder of the taxon) — a subtree is a preorder interval, so its distinct codes are its
- * keys minus the adjacent equal-code pairs whose lowest common ancestor lies inside it.  Results equal
- * kuq_clade_counts() of the member list, clade by clade.  Unknown taxids and taxa without counted descendants give 0. */
+ * keys minus the adjacent equal-code pairs whose lowest common ancestor lies inside it.  KUQ_HLL_EXACT: the same
+ * identity over the (k-mer, taxon) pairs, from ONE sort of the table (the books of kuq_exact_summary), or from the
+ * books summed over the parts once kuq_set_exact_summary installed them.  Results equal kuq_clade_counts() of the
+ * member list, clade by clade.  Unknown taxids and taxa without counted descendants give 0. */
 int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t *n_reads, uint64_t *n_kmers,
                           uint64_t *unique);
 /* The 4096 p=12 registers of one taxon (all zero if it received no k-mer). */
@@ -374,6 +377,39 @@ int kuq_exact_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *pairs, uint64_t *tim
  * taxonomy, which kuq_merge_into checks and callers of these two calls must ensure. */
 int kuq_exact_export(kuq_ctx *ctx, void *d_pairs_out, uint64_t cap, uint64_t *n);
 int kuq_exact_import(kuq_ctx *ctx, const void *d_pairs, uint64_t n);
+/* ---- the exact set partitioned by k-mer over GPUs / processes ---------------------------------------------------------
+ * Distinct counts are additive over any partition of the k-mer space: all pairs of one k-mer live in one part, so a
+ * taxon's set size and a clade's union size are sums over the parts.  The owner of a canonical k-mer among n_parts
+ * parts (1..64) is kuq_exact_owner:
+ *     x = kmer ^ 0x2545F4914F6CDD1D;  x ^= x >> 30;  x *= 0xbf58476d1ce4e5b9;  x ^= x >> 27;  x *= 0x94d049bb133111eb;
+ *     x ^= x >> 31;                   owner = ((x >> 32) * n_parts) >> 32
+ * (splitmix64's finalizer; the table's slot hash is a different function of (k-mer, taxon), so a part never crowds
+ * into a subset of a table's slots).  The recipe for G processes (krakenuniq_b200/dist.py, merge_exact_partitioned):
+ *   1. all-reduce SUM of the counters (kuq_state_ptrs: n_kmers, n_reads);
+ *   2. kuq_exact_export_partitioned(G): the table's pairs grouped by owner, parts back to back, counts[part] pairs each
+ *      (NULL / cap 0: counts only); _alloc sizes and allocates the buffer itself (release with kuq_device_free);
+ *   3. an all-to-all of the parts (two int64 words per pair);
+ *   4. kuq_exact_replace(received pairs): the context's table is rebuilt from them at a load of at most 0.6 (its old
+ *      pairs are dropped, duplicates across senders collapse, count[] is recounted); it now holds only its part, and
+ *      kuq_clade_counts refuses (KUQ_E_STATE) rather than return a partial union;
+ *   5. kuq_exact_summary: the part's per-taxon set sizes ([n_sketch] uint64) and roll-up books ([n_taxa] int64, dense
+ *      ids of kuq_dense_taxids) into device buffers → all-reduce SUM → kuq_set_exact_summary.  Until the next batch,
+ *      kuq_read_counts' `unique` and kuq_clade_counts_tree then report the union over all parts.
+ * books[d] = pairs of taxon d − pairs adjacent in (k-mer, preorder of the taxon) order with one k-mer whose lowest
+ * common ancestor is d; summed over a subtree they give the subtree's distinct k-mers (kuq_clade_counts_tree computes
+ * them on one context too, with one sort of the pairs in passes over the k-mer space sized to free device memory;
+ * KUQ_EXACT_ROLLUP_BUDGET=<bytes> sets the sort's scratch budget, kuq_exact_rollup_passes reports the passes taken).
+ * kuq_exact_partition does steps 2–5 for the contexts of one process: pairs move to their owner in rounds over slot
+ * ranges with peer copies, each owner builds its part beside its old table (peak per device: old table + part + one
+ * round of pairs each way), and the summed summary is installed on ctxs[0].  Step 1 there is kuq_merge_counters_into. */
+uint32_t kuq_exact_owner(uint64_t kmer, uint32_t n_parts);
+int kuq_exact_export_partitioned(kuq_ctx *ctx, uint32_t n_parts, void *d_pairs_out, uint64_t cap, uint64_t *counts);
+int kuq_exact_export_partitioned_alloc(kuq_ctx *ctx, uint32_t n_parts, void **d_pairs_out, uint64_t *counts);
+int kuq_exact_replace(kuq_ctx *ctx, const void *d_pairs, uint64_t n);
+int kuq_exact_summary(kuq_ctx *ctx, uint64_t *d_count_out, int64_t *d_books_out);
+int kuq_set_exact_summary(kuq_ctx *ctx, const uint64_t *d_count, const int64_t *d_books);
+int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n);
+int kuq_exact_rollup_passes(kuq_ctx *ctx, uint32_t *passes);
 /* ---- database sharded by minimizer range over the GPUs of a node (SURVEY.md §8(e).2) ------------------------------
  * Who counts: with kuq_set_shard_counting(on) the GPU that FINDS a hit does that hit's sketch work inside the lookup
  * half (kuq_lookup_device / kuq_lookup_device_peers): HLL register update and the record flag behind the sparse tier;
@@ -450,6 +486,9 @@ int kuq_host_unregister(void *p);
  * anywhere = dense, sparse-tier keys united (classify.cpp:542-544 across devices; cudaMemcpyPeer, no NCCL).  Both
  * contexts must have been given the same database and taxonomy.  `src` keeps its state. */
 int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src);
+/* kuq_merge_into without the sets: counters add, registers max, dense flags or; the sparse-tier keys and the exact
+ * pairs stay where they are (the partitioned merges move them: kuq_exact_partition, kuq_sparse_export_partitioned). */
+int kuq_merge_counters_into(kuq_ctx *dst, kuq_ctx *src);
 /* In one process the GPUs of a sharded database need no CUDA IPC: after kuq_enable_peer_access(ctx, peer) the device
  * pointers of `peer` (kuq_device_alloc) can be handed to kuq_lookup_device_peers / kuq_signal_peers of `ctx` as they are. */
 int kuq_enable_peer_access(kuq_ctx *ctx, kuq_ctx *peer);

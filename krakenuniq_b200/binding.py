@@ -165,6 +165,15 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_exact_info": (C.c_int, [vp, u64p, u64p, u64p]),
         "kuq_exact_export": (C.c_int, [vp, vp, C.c_uint64, u64p]),
         "kuq_exact_import": (C.c_int, [vp, vp, C.c_uint64]),
+        "kuq_exact_owner": (C.c_uint32, [C.c_uint64, C.c_uint32]),
+        "kuq_exact_export_partitioned": (C.c_int, [vp, C.c_uint32, vp, C.c_uint64, u64p]),
+        "kuq_exact_export_partitioned_alloc": (C.c_int, [vp, C.c_uint32, C.POINTER(vp), u64p]),
+        "kuq_exact_replace": (C.c_int, [vp, vp, C.c_uint64]),
+        "kuq_exact_summary": (C.c_int, [vp, vp, vp]),
+        "kuq_set_exact_summary": (C.c_int, [vp, vp, vp]),
+        "kuq_exact_partition": (C.c_int, [C.POINTER(vp), C.c_uint32]),
+        "kuq_exact_rollup_passes": (C.c_int, [vp, u32p]),
+        "kuq_merge_counters_into": (C.c_int, [vp, vp]),
         "kuq_set_shard_counting": (C.c_int, [vp, C.c_int]),
         "kuq_set_stats": (C.c_int, [vp, C.c_int]),
         "kuq_merge_into": (C.c_int, [vp, vp]),
@@ -622,6 +631,49 @@ class Classifier:
 
     def exact_import(self, d_pairs, n):
         self._ck(self.L.kuq_exact_import(self.h, d_pairs, n))
+
+    def exact_owner(self, kmer, n_parts):
+        """kuq_exact_owner: the part (0..n_parts-1) that owns a canonical k-mer in the partitioned exact set"""
+        return int(self.L.kuq_exact_owner(int(kmer), n_parts))
+
+    def exact_export_partitioned(self, n_parts, d_out=None, cap=0):
+        """kuq_exact_export_partitioned: pairs grouped by owner, parts back to back; → pairs per part"""
+        counts = np.zeros(n_parts, np.uint64)
+        self._ck(self.L.kuq_exact_export_partitioned(self.h, n_parts, d_out, cap, _p(counts, u64p)))
+        return counts
+
+    def exact_export_partitioned_alloc(self, n_parts):
+        """→ (device pointer of the pairs grouped by owner — release with device_free —, pairs per part)"""
+        counts = np.zeros(n_parts, np.uint64)
+        ptr = C.c_void_p()
+        self._ck(self.L.kuq_exact_export_partitioned_alloc(self.h, n_parts, C.byref(ptr), _p(counts, u64p)))
+        return ptr.value, counts
+
+    def exact_replace(self, d_pairs, n):
+        self._ck(self.L.kuq_exact_replace(self.h, d_pairs, n))
+
+    def exact_summary(self, d_count, d_books):
+        """kuq_exact_summary: per-taxon set sizes ([n_sketch] uint64) and roll-up books ([n_taxa] int64) of this part"""
+        self._ck(self.L.kuq_exact_summary(self.h, d_count, d_books))
+
+    def set_exact_summary(self, d_count, d_books):
+        self._ck(self.L.kuq_set_exact_summary(self.h, d_count, d_books))
+
+    def exact_rollup_passes(self):
+        n = np.zeros(1, np.uint32)
+        self._ck(self.L.kuq_exact_rollup_passes(self.h, _p(n, u32p)))
+        return int(n[0])
+
+    def merge_counters_from(self, other):
+        """kuq_merge_counters_into(self, other): kuq_merge_into without the sparse-tier keys and the exact pairs"""
+        self._ck(self.L.kuq_merge_counters_into(self.h, other.h))
+
+    @staticmethod
+    def exact_partition(classifiers):
+        """kuq_exact_partition: the exact sets of these contexts (one process) spread over them by k-mer owner; the summed
+        summary is installed on the first one"""
+        arr = (C.c_void_p * len(classifiers))(*[c.h for c in classifiers])
+        classifiers[0]._ck(classifiers[0].L.kuq_exact_partition(arr, len(classifiers)))
 
     def layout_experiment(self, slot, n_positions, reps=5):
         """kuq_layout_experiment: record layout x search shape of the bin search, timed on the windows of the slot's

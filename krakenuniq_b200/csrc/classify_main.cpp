@@ -400,6 +400,8 @@ struct TaxDB {
 
 struct Clade { uint64_t reads = 0, kmers = 0, unique = 0; };
 
+static bool Exact_partitioned = false;   // classifyExact: the contexts hold the exact set's k-mer parts (kuq_exact_partition)
+
 static void print_report(kuq_ctx *ctx, TaxDB &tax, ostream &out) {
   uint32_t n = 0;
   if (kuq_counts_size(ctx, &n)) die(EX_SOFTWARE, kuq_last_error(ctx));
@@ -426,6 +428,9 @@ static void print_report(kuq_ctx *ctx, TaxDB &tax, ostream &out) {
     auto z = tax.idx.find(0);
     if (z != tax.idx.end() && !tax.e[z->second].children.empty()) batch = false;
   }
+  // an exact set partitioned over contexts has no member-list unions: every clade comes from the roll-up (the run kept
+  // the union when taxon 0 has children, so the library's tree is this one)
+  if (Exact_partitioned) batch = true;
   if (batch) {
     vector<uint32_t> ids;
     vector<int> node;
@@ -1792,7 +1797,22 @@ int main(int argc, char **argv) {
   // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
   {
     double T0__ = now_s();
-    for (size_t g = 1; g < All_ctx.size(); g++)
+#ifdef EXACT_COUNTING
+    // classifyExact on several contexts: the counters join the first context, and the exact k-mer sets are spread over
+    // all contexts by k-mer instead of united on one card, so no card has to hold the union.  The report's clades come
+    // from the roll-up books summed over the parts.  A taxonomy with entries below taxon 0 keeps the union on the first
+    // context: print_report counts those clades one by one, which needs every pair in one place.
+    {
+      auto z = tax.idx.find(0);
+      Exact_partitioned = All_ctx.size() > 1 && !(z != tax.idx.end() && !tax.e[z->second].children.empty());
+    }
+    if (Exact_partitioned) {
+      for (size_t g = 1; g < All_ctx.size(); g++)
+        if (kuq_merge_counters_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+      if (kuq_exact_partition(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
+    }
+#endif
+    for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned; g++)
       if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
     if (All_ctx.size() > 1) TICK("merge");
 #ifdef EXACT_COUNTING

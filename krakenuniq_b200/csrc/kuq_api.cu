@@ -145,6 +145,13 @@ struct kuq_ctx {
   uint64_t exact_cap = 0;
   uint64_t exact_upper = 0;               // upper bound of the pairs in that table (reserve_exact_inserts)
   uint64_t exact_grown = 0;               // times it was re-allocated
+  bool exact_partitioned = false;         // kuq_exact_replace / kuq_exact_partition: the table holds one owner's part
+  bool merged_exact = false;              // kuq_set_exact_summary: merged_exact_count / merged_books hold sums over parts
+  std::vector<unsigned long long> merged_exact_count;
+  std::vector<long long> merged_books;
+  std::vector<uint32_t> exact_pre;        // preorder of every sketch taxon in the taxonomy (exact roll-up), built once
+  uint32_t *d_exact_pre = nullptr;
+  uint32_t exact_rollup_passes = 0;       // k-mer passes of the last exact roll-up
 
   // database streamed through HBM range by range (kuq_stream_*): two device buffers, one copy stream
   struct StreamBuf {
@@ -264,8 +271,9 @@ void free_tax_state(kuq_ctx *ctx) {
   cudaFree(ctx->d_parent); cudaFree(ctx->d_raw); cudaFree(ctx->d_depth);
   cudaFree(ctx->d_regs); cudaFree(ctx->d_dense_flag); cudaFree(ctx->d_n_kmers); cudaFree(ctx->d_n_reads);
   cudaFree(ctx->d_sparse_slots); cudaFree(ctx->d_sparse_used); cudaFree(ctx->d_sparse_distinct);
-  cudaFree(ctx->d_exact); cudaFree(ctx->d_exact_count);
-  ctx->d_exact = nullptr; ctx->d_exact_count = nullptr;
+  cudaFree(ctx->d_exact); cudaFree(ctx->d_exact_count); cudaFree(ctx->d_exact_pre);
+  ctx->d_exact = nullptr; ctx->d_exact_count = nullptr; ctx->d_exact_pre = nullptr;
+  ctx->exact_pre.clear();
   ctx->d_parent = ctx->d_raw = nullptr; ctx->d_depth = nullptr; ctx->d_regs = ctx->d_dense_flag = nullptr;
   ctx->d_n_kmers = ctx->d_n_reads = nullptr; ctx->d_sparse_slots = ctx->d_sparse_used = nullptr;
   ctx->d_sparse_distinct = nullptr;
@@ -617,9 +625,17 @@ int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
 
 // ---- the exact k-mer set (KUQ_HLL_EXACT) grows like the sparse-tier set ---------------------------------------------
 // Re-allocate the (taxon, k-mer) table with `cap` slots and move its pairs over (not counted again).  All slots must be idle.
+// KUQ_EXACT_MAX_SLOTS caps the slots a table may grow to, as if the device had no room for more: tests use it to build,
+// on one card, runs whose union exceeds one context's table (0 / unset = no cap)
+uint64_t exact_max_slots() {
+  const char *e = getenv("KUQ_EXACT_MAX_SLOTS");
+  return e ? strtoull(e, nullptr, 10) : 0;
+}
+
 int grow_exact_set(kuq_ctx *ctx, uint64_t cap) {
   ExactPair *bigger = nullptr;
-  if (dmalloc(&bigger, cap) != cudaSuccess) {
+  const uint64_t max_slots = exact_max_slots();
+  if ((max_slots && cap > max_slots) || dmalloc(&bigger, cap) != cudaSuccess) {
     (void)cudaGetLastError();
     return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no room to grow from %llu to %llu slots (%.2f GiB)", (unsigned long long)ctx->exact_cap,
                 (unsigned long long)cap, cap * 16.0 / (1ull << 30));
@@ -742,6 +758,171 @@ int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
   cudaSetDevice(dst->device);
   if (d_dst) cudaFree(d_dst);
   return rc;
+}
+
+// ---- the exact set partitioned by k-mer over contexts (kuq_exact_export_partitioned / _replace / _partition) ---------
+// Slots [lo, hi) of the table grouped by owner (exact_owner) into out, parts back to back; counts[part] = their number.
+// out == nullptr only counts.  All slots idle.
+int exact_parts_range(kuq_ctx *ctx, uint64_t lo, uint64_t hi, uint32_t n_parts, ExactPair *out, uint64_t cap, uint64_t *counts) {
+  unsigned long long *d_cnt = nullptr;
+  const uint32_t P = EXACT_MAX_PARTS;
+  CU(dmalloc(&d_cnt, 2 * P + 1));                // [0, P) counts / cursors, [P, 2P) part ends, [2P] error word
+  CU(cudaMemsetAsync(d_cnt, 0, (2 * P + 1) * 8ull, ctx->aux));
+  uint32_t *d_err = reinterpret_cast<uint32_t *>(d_cnt + 2 * P);
+  launch_exact_parts(ctx->d_exact, lo, hi, n_parts, d_cnt, nullptr, nullptr, d_err, 0, ctx->aux);
+  ctx->launches++;
+  std::vector<unsigned long long> h(2 * P, 0);
+  CU(cudaMemcpyAsync(h.data(), d_cnt, P * 8ull, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  uint64_t total = 0;
+  for (uint32_t j = 0; j < n_parts; j++) { counts[j] = h[j]; total += h[j]; }
+  if (!out) { cudaFree(d_cnt); return KUQ_OK; }
+  if (total > cap) { cudaFree(d_cnt); return fail(ctx, KUQ_E_CAPACITY, "need room for %llu pairs", (unsigned long long)total); }
+  unsigned long long at = 0;
+  for (uint32_t j = 0; j < P; j++) {
+    const unsigned long long c = j < n_parts ? h[j] : 0;
+    h[j] = at;
+    h[P + j] = at + c;
+    at += c;
+  }
+  CU(cudaMemcpyAsync(d_cnt, h.data(), 2 * P * 8ull, cudaMemcpyHostToDevice, ctx->aux));
+  launch_exact_parts(ctx->d_exact, lo, hi, n_parts, d_cnt, out, d_cnt + P, d_err, 1, ctx->aux);
+  ctx->launches++;
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_cnt);
+  if (err) return fail(ctx, KUQ_E_CAPACITY, "internal: partitioned export overran a part");
+  return KUQ_OK;
+}
+
+// A fresh table for `incoming` pairs at a load of at most 0.6 (KUQ_EXACT_MAX_SLOTS applies as to growth), zeroed, with
+// zeroed per-taxon counters.  On ctx's device.
+struct ExactTable {
+  ExactPair *slots = nullptr;
+  unsigned long long *count = nullptr;
+  uint64_t cap = 0;
+};
+int exact_table_alloc(kuq_ctx *ctx, uint64_t incoming, ExactTable &t) {
+  uint64_t cap = 1024;
+  while (incoming * 10 > cap * 6) cap <<= 1;
+  const uint64_t max_slots = exact_max_slots();
+  if ((max_slots && cap > max_slots) || dmalloc(&t.slots, cap) != cudaSuccess ||
+      dmalloc(&t.count, ctx->n_sketch) != cudaSuccess) {
+    (void)cudaGetLastError();
+    cudaFree(t.slots);
+    t = ExactTable{};
+    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no room for a part of %llu pairs (%llu slots, %.2f GiB) on device %d",
+                (unsigned long long)incoming, (unsigned long long)cap, cap * 16.0 / (1ull << 30), ctx->device);
+  }
+  t.cap = cap;
+  CU(cudaMemsetAsync(t.slots, 0, cap * 16ull, ctx->aux));
+  CU(cudaMemsetAsync(t.count, 0, ctx->n_sketch * 8ull, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  return KUQ_OK;
+}
+void exact_table_free(ExactTable &t) { cudaFree(t.slots); cudaFree(t.count); t = ExactTable{}; }
+
+// pairs into a table that is being built; count[] grows by the pairs that are new, so duplicates across senders collapse
+int exact_table_import(kuq_ctx *ctx, ExactTable &t, const ExactPair *d_pairs, uint64_t n) {
+  if (!n) return KUQ_OK;
+  uint32_t *d_err = nullptr;
+  CU(dmalloc(&d_err, 1));
+  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
+  launch_exact_import(d_pairs, n, ExactSet{t.slots, t.cap - 1, t.count}, d_err, ctx->aux);
+  ctx->launches++;
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_err);
+  if (err) return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated while building a part (%llu slots)", (unsigned long long)t.cap);
+  return KUQ_OK;
+}
+
+// the built table replaces the context's: from now on it holds one owner's part
+void exact_table_install(kuq_ctx *ctx, ExactTable &t, uint64_t upper) {
+  cudaFree(ctx->d_exact);
+  cudaFree(ctx->d_exact_count);
+  ctx->d_exact = t.slots;
+  ctx->d_exact_count = t.count;
+  if (t.cap != ctx->exact_cap) ctx->exact_grown++;
+  ctx->exact_cap = t.cap;
+  ctx->exact_upper = upper;
+  ctx->exact_partitioned = true;
+  ctx->merged_exact = false;
+  ctx->snap_valid = false;
+  t = ExactTable{};
+}
+
+// Preorder of the context's taxonomy (roots: taxa whose parent is 0, as in kuq_clade_counts_tree), kept for the sketch
+// taxa on host and device.  Taxa no root reaches (a malformed chain) stay NONE and are left out of the roll-up.
+int exact_preorder(kuq_ctx *ctx) {
+  if (ctx->d_exact_pre) return KUQ_OK;
+  const uint32_t NT = ctx->n_taxa, NONE = 0xFFFFFFFFu;
+  const std::vector<uint32_t> &par = ctx->parent_dense;
+  std::vector<uint32_t> first(NT + 1, 0), child(NT), pre(NT, NONE), stack;
+  for (uint32_t x = 1; x < NT; x++) if (par[x]) first[par[x] + 1]++;
+  for (uint32_t x = 0; x < NT; x++) first[x + 1] += first[x];
+  {
+    std::vector<uint32_t> fill(first.begin(), first.end() - 1);
+    for (uint32_t x = 1; x < NT; x++) if (par[x]) child[fill[par[x]]++] = x;
+  }
+  uint32_t counter = 0;
+  for (uint32_t r = 0; r < NT; r++) {
+    if (r != 0 && par[r] != 0) continue;
+    stack.push_back(r);
+    while (!stack.empty()) {
+      const uint32_t x = stack.back();
+      stack.pop_back();
+      if (pre[x] != NONE) continue;
+      pre[x] = counter++;
+      if (x == 0) continue;                      // dense 0 ("no taxon") is a root of its own
+      for (uint32_t i = first[x]; i < first[x + 1]; i++) stack.push_back(child[i]);
+    }
+  }
+  pre.resize(ctx->n_sketch);
+  CU(dmalloc(&ctx->d_exact_pre, ctx->n_sketch));
+  CU(cudaMemcpy(ctx->d_exact_pre, pre.data(), ctx->n_sketch * 4ull, cudaMemcpyHostToDevice));
+  ctx->exact_pre.swap(pre);
+  return KUQ_OK;
+}
+
+// Books of the exact roll-up, one signed counter per taxon of the taxonomy: books[d] = pairs of taxon d − the adjacent
+// equal-k-mer pairs (sorted by (k-mer, preorder)) whose LCA is d.  Summed over a subtree they give its distinct k-mers;
+// summed over contexts that hold disjoint parts of the k-mer space they give the books of the union.  The +1 per pair
+// comes from count[] instead of one atomic per pair on the device (most pairs of a run go to a few taxa: the misses to
+// taxon 0).  Scratch: KUQ_EXACT_ROLLUP_BUDGET bytes, else 80 % of the free device memory.  All slots idle.
+int exact_books(kuq_ctx *ctx, std::vector<long long> &books) {
+  int rc = exact_preorder(ctx);
+  if (rc) return rc;
+  std::vector<unsigned long long> count(ctx->n_sketch);
+  CU(cudaMemcpy(count.data(), ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+  uint64_t n_pairs = 0;
+  for (unsigned long long v : count) n_pairs += v;
+  unsigned long long *d_books = nullptr;
+  CU(dmalloc(&d_books, ctx->n_taxa));
+  CU(cudaMemsetAsync(d_books, 0, ctx->n_taxa * 8ull, ctx->aux));
+  uint64_t budget = 0;
+  if (const char *e = getenv("KUQ_EXACT_ROLLUP_BUDGET")) budget = strtoull(e, nullptr, 10);
+  if (!budget) {
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    budget = (uint64_t)(free_b * 0.8);
+  }
+  const int src = exact_clade_dups(ctx->d_exact, ctx->exact_cap, n_pairs, ctx->d_exact_pre, ctx->d_parent, ctx->d_depth, d_books,
+                                   std::max<uint64_t>(budget, 1), ctx->n_sm, ctx->aux, &ctx->exact_rollup_passes);
+  ctx->launches += 3ull * std::max<uint32_t>(ctx->exact_rollup_passes, 1);
+  std::vector<unsigned long long> dups(ctx->n_taxa, 0);
+  cudaError_t ce = cudaSuccess;
+  if (src == 0) ce = cudaMemcpy(dups.data(), d_books, ctx->n_taxa * 8ull, cudaMemcpyDeviceToHost);
+  cudaFree(d_books);
+  if (src == 1) return fail(ctx, KUQ_E_NOMEM, "exact clade roll-up: no device memory for one pass of the sort (budget %llu bytes)", (unsigned long long)budget);
+  if (src == 2 || ce != cudaSuccess) return fail(ctx, KUQ_E_CUDA, "exact clade roll-up failed: %s", cudaGetErrorString(cudaGetLastError()));
+  books.assign(ctx->n_taxa, 0);
+  for (uint32_t d = 0; d < ctx->n_taxa; d++) books[d] = (long long)dups[d];
+  for (uint32_t d = 0; d < ctx->n_sketch; d++)
+    if (ctx->exact_pre[d] != 0xFFFFFFFFu) books[d] += (long long)count[d];
+  return KUQ_OK;
 }
 
 // Build the collision table of the staged range once, the first time keep mode or a harvest can use the record tier.
@@ -1150,6 +1331,7 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
     if (mode == MODE_LOOKUP && p.n_reads && ctx->cfg.hll_mode <= KUQ_HLL_CHUNKED) ctx->seen_dirty = true;
   }
   ctx->merged_summary = false;
+  ctx->merged_exact = false;
   if (mode != MODE_LOOKUP && ctx->quick_min) {           // "Q:hits" replaces the hit list (classify.cpp:989-990)
     p.quick_min = ctx->quick_min;
     p.quick_stop = ctx->quick_stop;
@@ -2058,6 +2240,7 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
     h.exact.resize(ctx->n_sketch);
     CU(cudaMemcpy(h.exact.data(), ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+    if (ctx->merged_exact) h.exact = ctx->merged_exact_count;   // sums over the k-mer parts (kuq_set_exact_summary)
   } else if (ctx->cfg.hll_mode != KUQ_HLL_DENSE_ONLY) {
     if (ctx->cfg.hll_mode == KUQ_HLL_CHUNKED) {
       launch_flag_dense_global(ctx->d_sparse_distinct, ctx->d_dense_flag, ctx->n_sketch, ctx->aux);
@@ -2215,6 +2398,10 @@ int kuq_clade_counts(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t 
   }
   uint64_t u = 0;
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
+    if (ctx->exact_partitioned)
+      return fail(ctx, KUQ_E_STATE, "the exact k-mer set is partitioned by k-mer over contexts and this one holds one part: "
+                                    "a union over a member list would be partial (use kuq_clade_counts_tree after "
+                                    "kuq_set_exact_summary)");
     // the clade's container is the union of the members' k-mer sets (readcounts.hpp:76-81)
     uint64_t sum = 0;
     for (uint32_t d : members) sum += h.exact[d];
@@ -2361,10 +2548,29 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
     if (it != ctx->dense_of_raw.end() && cid[it->second] != NONE) { req[i] = cid[it->second]; wanted[req[i]] = 1; }
   }
   std::vector<uint64_t> c_unique(NC, 0);
-  const bool per_clade = ctx->cfg.hll_mode == KUQ_HLL_EXACT || ctx->merged_summary;
+  const bool exact = ctx->cfg.hll_mode == KUQ_HLL_EXACT;
+  const bool per_clade = !exact && ctx->merged_summary;
   bool sparse_fallback = false;
   std::vector<uint32_t> dense_list, sparse_multi;          // compact ids
-  if (!per_clade) {
+  // ---- exact counting: every clade from the books of one sort (exact_books), or from their sums over the parts ------
+  if (exact) {
+    std::vector<long long> own;
+    const std::vector<long long> *books = &ctx->merged_books;
+    if (!ctx->merged_exact) {
+      if (ctx->exact_partitioned)
+        return fail(ctx, KUQ_E_STATE, "the exact k-mer set is partitioned by k-mer over contexts: install the books summed "
+                                      "over all parts first (kuq_exact_summary, kuq_set_exact_summary)");
+      int rc = exact_books(ctx, own);
+      if (rc) return rc;
+      books = &own;
+    }
+    std::vector<long long> acc(NC, 0);
+    for (uint32_t c = 0; c < NC; c++) acc[c] = (*books)[nodes[c]];
+    for (uint32_t c : order)
+      if (parent_c[c] != NONE) acc[parent_c[c]] += acc[c];
+    for (uint32_t c = 0; c < NC; c++) c_unique[c] = (uint64_t)std::max<long long>(acc[c], 0);
+  }
+  if (!per_clade && !exact) {
     for (uint32_t c = 0; c < NC; c++) {
       if (c_members[c] == 0) continue;
       if (c_members[c] == 1) {
@@ -2746,7 +2952,12 @@ int kuq_host_unregister(void *p) {
 }
 
 // Several GPUs in ONE process (the drop-in `classify` with replicas): fold the per-taxon state of `src` into `dst`.
-int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
+// sets = false folds the counters, registers and dense flags only (kuq_merge_counters_into).
+static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets);
+int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) { return merge_into(dst, src, true); }
+int kuq_merge_counters_into(kuq_ctx *dst, kuq_ctx *src) { return merge_into(dst, src, false); }
+
+static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets) {
   kuq_ctx *ctx = dst;
   if (!dst || !src || dst == src) return KUQ_E_INVALID_ARG;
   if (!src->finalized) return KUQ_OK;                       // src never classified anything: nothing to add
@@ -2761,7 +2972,7 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
   { int rc = harvest_seen(src, false); if (rc) { dst->err = src->err; return rc; } }
   uint64_t n_keys = 0;
   uint64_t *d_keys_src = nullptr;
-  if (src->d_sparse_slots && !exact) {
+  if (src->d_sparse_slots && !exact && sets) {
     int rc = kuq_sparse_export(src, nullptr, 0, &n_keys);
     if (rc) { dst->err = src->err; return rc; }
     if (n_keys) {
@@ -2778,6 +2989,7 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
   { int rc = harvest_seen(dst, false, true); if (rc) return rc; }
   dst->snap_valid = false;
   dst->merged_summary = false;
+  dst->merged_exact = false;
   uint8_t *t_regs, *t_dense; unsigned long long *t_nk, *t_nr;
   const uint64_t reg_bytes = (uint64_t)dst->n_sketch * HLL_M;
   CU(cudaMalloc((void **)&t_regs, reg_bytes));
@@ -2793,7 +3005,7 @@ int kuq_merge_into(kuq_ctx *dst, kuq_ctx *src) {
   dst->launches++;
   CU(cudaStreamSynchronize(dst->aux));
   cudaFree(t_regs); cudaFree(t_dense); cudaFree(t_nk); cudaFree(t_nr);
-  if (exact) return merge_exact_pairs(dst, src);
+  if (exact) return sets ? merge_exact_pairs(dst, src) : KUQ_OK;
   int rc = KUQ_OK;
   if (n_keys && dst->d_sparse_slots) {
     uint64_t *d_keys_dst = nullptr;
@@ -3157,6 +3369,229 @@ int kuq_exact_import(kuq_ctx *ctx, const void *d_pairs, uint64_t n) {
   return exact_import(ctx, static_cast<const ExactPair *>(d_pairs), n);
 }
 
+uint32_t kuq_exact_owner(uint64_t kmer, uint32_t n_parts) { return n_parts ? exact_owner(kmer, n_parts) : 0; }
+
+static int exact_export_partitioned(kuq_ctx *ctx, uint32_t n_parts, void *d_pairs_out, uint64_t cap, uint64_t *counts, void **alloc_out) {
+  if (!ctx || !counts || n_parts == 0 || n_parts > EXACT_MAX_PARTS) return KUQ_E_INVALID_ARG;
+  if (d_pairs_out && ((uintptr_t)d_pairs_out & 15)) return fail(ctx, KUQ_E_INVALID_ARG, "d_pairs_out must be 16-byte aligned");
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  for (uint32_t j = 0; j < n_parts; j++) counts[j] = 0;
+  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_export_partitioned needs a KUQ_HLL_EXACT context");
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  rc = exact_parts_range(ctx, 0, ctx->exact_cap, n_parts, nullptr, 0, counts);
+  if (rc || (!d_pairs_out && !alloc_out)) return rc;
+  uint64_t total = 0;
+  for (uint32_t j = 0; j < n_parts; j++) total += counts[j];
+  ExactPair *out = static_cast<ExactPair *>(d_pairs_out);
+  if (alloc_out) {                                         // the library sizes the buffer after its counting pass
+    if (dmalloc(&out, std::max<uint64_t>(total, 1)) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return fail(ctx, KUQ_E_NOMEM, "no room for %llu exported pairs", (unsigned long long)total);
+    }
+    cap = total;
+  }
+  rc = exact_parts_range(ctx, 0, ctx->exact_cap, n_parts, out, cap, counts);
+  if (alloc_out) {
+    if (rc) cudaFree(out); else *alloc_out = out;
+  }
+  return rc;
+}
+
+int kuq_exact_export_partitioned(kuq_ctx *ctx, uint32_t n_parts, void *d_pairs_out, uint64_t cap, uint64_t *counts) {
+  return exact_export_partitioned(ctx, n_parts, d_pairs_out, cap, counts, nullptr);
+}
+int kuq_exact_export_partitioned_alloc(kuq_ctx *ctx, uint32_t n_parts, void **d_pairs_out, uint64_t *counts) {
+  if (!d_pairs_out) return KUQ_E_INVALID_ARG;
+  *d_pairs_out = nullptr;
+  return exact_export_partitioned(ctx, n_parts, nullptr, 0, counts, d_pairs_out);
+}
+
+int kuq_exact_replace(kuq_ctx *ctx, const void *d_pairs, uint64_t n) {
+  if (!ctx || (!d_pairs && n)) return KUQ_E_INVALID_ARG;
+  if ((uintptr_t)d_pairs & 15) return fail(ctx, KUQ_E_INVALID_ARG, "d_pairs must be 16-byte aligned");
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_replace needs a KUQ_HLL_EXACT context");
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  // the old pairs were exported before: its table goes first, so the peak is the received pairs and the new table
+  cudaFree(ctx->d_exact);
+  ctx->d_exact = nullptr;
+  ExactTable t;
+  rc = exact_table_alloc(ctx, n, t);
+  if (!rc) rc = exact_table_import(ctx, t, static_cast<const ExactPair *>(d_pairs), n);
+  if (rc) {                                      // leave an empty table of the old size behind, not a dangling one
+    exact_table_free(t);
+    if (dmalloc(&ctx->d_exact, ctx->exact_cap) == cudaSuccess) {
+      cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull);
+      cudaMemset(ctx->d_exact_count, 0, ctx->n_sketch * 8ull);
+    } else {
+      (void)cudaGetLastError();
+      ctx->exact_cap = 0;
+    }
+    ctx->exact_upper = 0;
+    return rc;
+  }
+  exact_table_install(ctx, t, n);
+  return KUQ_OK;
+}
+
+int kuq_exact_summary(kuq_ctx *ctx, uint64_t *d_count_out, int64_t *d_books_out) {
+  if (!ctx || !d_count_out || !d_books_out) return KUQ_E_INVALID_ARG;
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_summary needs a KUQ_HLL_EXACT context");
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  std::vector<long long> books;
+  rc = exact_books(ctx, books);
+  if (rc) return rc;
+  CU(cudaMemcpy(d_count_out, ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToDevice));
+  CU(cudaMemcpy(d_books_out, books.data(), ctx->n_taxa * 8ull, cudaMemcpyHostToDevice));
+  return KUQ_OK;
+}
+
+static int set_exact_summary(kuq_ctx *ctx, std::vector<unsigned long long> &count, std::vector<long long> &books) {
+  ctx->merged_exact_count.swap(count);
+  ctx->merged_books.swap(books);
+  ctx->merged_exact = true;
+  ctx->snap_valid = false;
+  return KUQ_OK;
+}
+
+int kuq_set_exact_summary(kuq_ctx *ctx, const uint64_t *d_count, const int64_t *d_books) {
+  if (!ctx || !d_count || !d_books) return KUQ_E_INVALID_ARG;
+  int rc = ensure_ready(ctx);
+  if (rc) return rc;
+  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_set_exact_summary needs a KUQ_HLL_EXACT context");
+  CU(cudaSetDevice(ctx->device));
+  std::vector<unsigned long long> count(ctx->n_sketch);
+  std::vector<long long> books(ctx->n_taxa);
+  CU(cudaMemcpy(count.data(), d_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(books.data(), d_books, ctx->n_taxa * 8ull, cudaMemcpyDeviceToHost));
+  return set_exact_summary(ctx, count, books);
+}
+
+// In one process: every context's pairs go to the context that owns their k-mer, in rounds over slot ranges of each
+// source table (KUQ_EXACT_MERGE_SLOTS, as kuq_merge_into), peer to peer between devices.  Each owner builds its part
+// in a new table beside its old one, sized to the pairs all sources send it; the old tables go when every round is done.
+// Peak per device: its old table + its new part + one round of pairs on each side.  Then the books and counters of
+// the parts are summed on the host and installed on ctxs[0] (kuq_set_exact_summary).
+int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
+  if (!ctxs || n == 0 || n > EXACT_MAX_PARTS) return KUQ_E_INVALID_ARG;
+  kuq_ctx *ctx = ctxs[0];
+  for (uint32_t g = 0; g < n; g++) {
+    if (!ctxs[g]) return KUQ_E_INVALID_ARG;
+    for (uint32_t h = 0; h < g; h++) if (ctxs[h] == ctxs[g]) return KUQ_E_INVALID_ARG;
+  }
+  for (uint32_t g = 0; g < n; g++) {
+    kuq_ctx *c = ctxs[g];
+    int rc = ensure_ready(c);
+    if (rc) { if (g) ctx->err = c->err; return rc; }
+    if (!c->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_partition needs KUQ_HLL_EXACT contexts");
+    if (c->n_taxa != ctx->n_taxa || c->n_sketch != ctx->n_sketch || c->raw_of_dense != ctx->raw_of_dense)
+      return fail(ctx, KUQ_E_STATE, "the contexts number their taxa differently (different database / taxonomy)");
+    CU(cudaSetDevice(c->device));
+    for (auto &s : c->slots) CU(cudaStreamSynchronize(s.stream));
+  }
+  // 1. pairs per (source, owner): the owner's part is at most their sum (pairs held by several sources collapse)
+  std::vector<uint64_t> want(n, 0), counts(n);
+  for (uint32_t g = 0; g < n; g++) {
+    CU(cudaSetDevice(ctxs[g]->device));
+    int rc = exact_parts_range(ctxs[g], 0, ctxs[g]->exact_cap, n, nullptr, 0, counts.data());
+    if (rc) { if (g) ctx->err = ctxs[g]->err; return rc; }
+    for (uint32_t o = 0; o < n; o++) want[o] += counts[o];
+  }
+  // 2. the new tables and the round buffers
+  uint64_t round_slots = 1ull << 22;
+  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+  std::vector<ExactTable> part(n);
+  std::vector<ExactPair *> round(n, nullptr), recv(n, nullptr);
+  std::vector<uint64_t> round_cap(n, 0);
+  auto cleanup = [&]() {
+    for (uint32_t g = 0; g < n; g++) {
+      cudaSetDevice(ctxs[g]->device);
+      exact_table_free(part[g]);
+      cudaFree(round[g]);
+      cudaFree(recv[g]);
+    }
+    cudaSetDevice(ctx->device);
+  };
+  int rc = KUQ_OK;
+  for (uint32_t g = 0; g < n && !rc; g++) {
+    kuq_ctx *c = ctxs[g];
+    CU(cudaSetDevice(c->device));
+    rc = exact_table_alloc(c, want[g], part[g]);
+    if (rc) { ctx->err = c->err; break; }
+    round_cap[g] = std::min(round_slots, c->exact_cap);
+    bool needs_recv = false;
+    for (uint32_t h = 0; h < n; h++) needs_recv |= ctxs[h]->device != c->device;
+    uint64_t recv_cap = 0;
+    for (uint32_t h = 0; h < n; h++) if (ctxs[h]->device != c->device) recv_cap = std::max(recv_cap, std::min(round_slots, ctxs[h]->exact_cap));
+    if (dmalloc(&round[g], std::max<uint64_t>(round_cap[g], 1)) != cudaSuccess ||
+        (needs_recv && dmalloc(&recv[g], std::max<uint64_t>(recv_cap, 1)) != cudaSuccess)) {
+      (void)cudaGetLastError();
+      rc = fail(ctx, KUQ_E_NOMEM, "exact k-mer set partition: no room for a round of %llu pairs on device %d",
+                (unsigned long long)round_cap[g], c->device);
+    }
+  }
+  if (rc) { cleanup(); return rc; }
+  // 3. rounds: a slot range of one source, grouped by owner, each group imported by its owner
+  for (uint32_t g = 0; g < n && !rc; g++) {
+    kuq_ctx *src = ctxs[g];
+    for (uint64_t lo = 0; lo < src->exact_cap && !rc; lo += round_cap[g]) {
+      CU(cudaSetDevice(src->device));
+      rc = exact_parts_range(src, lo, std::min(lo + round_cap[g], src->exact_cap), n, round[g], round_cap[g], counts.data());
+      if (rc) { ctx->err = src->err; break; }
+      uint64_t off = 0;
+      for (uint32_t o = 0; o < n && !rc; o++) {
+        const uint64_t m = counts[o];
+        const ExactPair *from = round[g] + off;
+        off += m;
+        if (!m) continue;
+        kuq_ctx *dst = ctxs[o];
+        CU(cudaSetDevice(dst->device));
+        if (dst->device != src->device) {
+          CU(cudaMemcpyPeer(recv[o], dst->device, from, src->device, m * 16));
+          from = recv[o];
+        }
+        rc = exact_table_import(dst, part[o], from, m);
+        if (rc) ctx->err = dst->err;
+      }
+    }
+  }
+  if (rc) { cleanup(); return rc; }
+  // 4. the parts replace the tables
+  for (uint32_t g = 0; g < n; g++) {
+    CU(cudaSetDevice(ctxs[g]->device));
+    cudaFree(round[g]); cudaFree(recv[g]);
+    round[g] = recv[g] = nullptr;
+    exact_table_install(ctxs[g], part[g], want[g]);
+  }
+  // 5. counters and books summed over the parts, installed on the first context
+  std::vector<unsigned long long> count_sum(ctx->n_sketch, 0), cnt(ctx->n_sketch);
+  std::vector<long long> books_sum(ctx->n_taxa, 0), books;
+  for (uint32_t g = 0; g < n; g++) {
+    kuq_ctx *c = ctxs[g];
+    CU(cudaSetDevice(c->device));
+    rc = exact_books(c, books);
+    if (rc) { ctx->err = c->err; cudaSetDevice(ctx->device); return rc; }
+    CU(cudaMemcpy(cnt.data(), c->d_exact_count, c->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+    for (uint32_t d = 0; d < ctx->n_sketch; d++) count_sum[d] += cnt[d];
+    for (uint32_t d = 0; d < ctx->n_taxa; d++) books_sum[d] += books[d];
+  }
+  CU(cudaSetDevice(ctx->device));
+  return set_exact_summary(ctx, count_sum, books_sum);
+}
+
+int kuq_exact_rollup_passes(kuq_ctx *ctx, uint32_t *passes) {
+  if (!ctx || !passes) return KUQ_E_INVALID_ARG;
+  *passes = ctx->exact_rollup_passes;
+  return KUQ_OK;
+}
+
 int kuq_dense_taxids(kuq_ctx *ctx, uint32_t *taxid_of_dense, uint32_t cap, uint32_t *n) {
   if (!ctx || !n) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
@@ -3190,6 +3625,8 @@ int kuq_reset_counts(kuq_ctx *ctx) {
     CU(cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull));
     CU(cudaMemset(ctx->d_exact_count, 0, ctx->n_sketch * 8ull));
     ctx->exact_upper = 0;
+    ctx->exact_partitioned = false;
+    ctx->merged_exact = false;
   }
   ctx->unit_nt = 0;
   ctx->unit_next = 0;

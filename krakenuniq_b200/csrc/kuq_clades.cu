@@ -11,10 +11,15 @@
 //      and a pair lies inside u exactly when its taxa's lowest common ancestor does.  The kernel books every
 //      adjacent pair at its LCA (per encoded rank, because the estimator wants the rank histogram of the union);
 //      the host sums the books up the tree.
+//  exact mode (KUQ_HLL_EXACT): the same identity over the (k-mer, taxon) pairs of the exact table, sorted by
+//      (k-mer, preorder), in passes over parts of the k-mer space when scratch is short (exact_clade_dups).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include <cub/cub.cuh>
+#include <cuda/std/tuple>
 
 #include "kuq_kernels.cuh"
 
@@ -95,7 +100,125 @@ __global__ void __launch_bounds__(256) k_clade_dups(const unsigned long long *__
   }
 }
 
+// ---- exact mode: the same identity over (k-mer, taxon) pairs --------------------------------------------------------
+// distinct(subtree u) = pairs of taxa in u − adjacent equal-k-mer pairs whose LCA lies in u, with the pairs sorted by
+// (k-mer, preorder of the taxon).  The pairs of one k-mer all fall in one pass of the k-mer space, so passes add up.
+struct ExactItem {
+  unsigned long long kmer;     // canonical k-mer (62 bits at most): sort key, most significant
+  uint32_t pre;                // preorder of the taxon: sort key
+  uint32_t taxon;              // dense taxon id, carried along
+};
+struct ExactItemDecomposer {
+  __host__ __device__ cuda::std::tuple<unsigned long long &, uint32_t &> operator()(ExactItem &it) const { return {it.kmer, it.pre}; }
+};
+
+// the occupied slots whose k-mer falls in this pass and whose taxon lies in the tree → items; one cursor atomic per warp
+__global__ void __launch_bounds__(256) k_exact_sort_items(const ExactPair *__restrict__ slots, uint64_t n_slots, uint32_t n_pass,
+                                                          uint32_t pass, const uint32_t *__restrict__ pre_of_taxon,
+                                                          ExactItem *__restrict__ out, uint64_t out_cap, unsigned long long *cursor) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  const uint64_t n_round = (n_slots + stride - 1) / stride * stride;      // whole warps stay in the loop (ballot below)
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+    ExactItem it{0ull, NONE32, 0u};
+    bool have = false;
+    if (i < n_slots) {
+      const ExactPair pr = slots[i];
+      if (pr.kmer1 && (n_pass == 1 || exact_pass(pr.kmer1 - 1, n_pass) == pass)) {
+        it.kmer = pr.kmer1 - 1;
+        it.taxon = (uint32_t)(pr.taxon1 - 1);
+        it.pre = pre_of_taxon[it.taxon];
+        have = it.pre != NONE32;
+      }
+    }
+    const uint32_t vote = __ballot_sync(0xFFFFFFFFu, have);
+    if (vote) {
+      const uint32_t lane = threadIdx.x & 31;
+      unsigned long long base = 0;
+      if (lane == 0) base = atomicAdd(cursor, (unsigned long long)__popc(vote));
+      base = __shfl_sync(0xFFFFFFFFu, base, 0);
+      if (have) {
+        const unsigned long long at = base + __popc(vote & ((1u << lane) - 1));
+        if (at < out_cap) out[at] = it;
+      }
+    }
+  }
+}
+
+// adjacent items with one k-mer: −1 at the LCA of their taxa in the context's taxonomy (parent 0 = none; the walk is
+// bounded by the depth, so a malformed chain cannot hold it)
+__global__ void __launch_bounds__(256) k_exact_dups(const ExactItem *__restrict__ sorted, uint64_t n, const uint32_t *__restrict__ parent,
+                                                    const uint16_t *__restrict__ depth, unsigned long long *books) {
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x + 1; i < n; i += stride) {
+    const ExactItem a = sorted[i - 1], b = sorted[i];
+    if (a.kmer != b.kmer) continue;
+    uint32_t x = a.taxon, y = b.taxon, dx = depth[x], dy = depth[y];
+    while (dx > dy) { x = parent[x]; dx--; }
+    while (dy > dx) { y = parent[y]; dy--; }
+    for (uint32_t s = 0; x != y && s <= dx; s++) { x = parent[x]; y = parent[y]; }
+    if (x == y && x != 0) atomicAdd(books + x, ~0ull);                  // two's complement −1
+  }
+}
+
 }  // namespace
+
+int exact_clade_dups(const ExactPair *slots, uint64_t n_slots, uint64_t n_pairs, const uint32_t *d_pre_of_taxon,
+                     const uint32_t *d_parent, const uint16_t *d_depth, unsigned long long *d_books, uint64_t budget, int n_sm,
+                     cudaStream_t stream, uint32_t *passes_out) {
+  *passes_out = 0;
+  if (n_pairs < 2) return 0;
+  // scratch per item: two sort buffers of 16 B and CUB's temporary storage (a few bytes per item); 48 B with margin
+  const uint64_t per_item = 48;
+  uint64_t n_pass = std::max<uint64_t>(1, (n_pairs * per_item + budget - 1) / std::max<uint64_t>(budget, 1));
+  if (n_pass > (1ull << 20)) return 1;
+  auto pass_cap = [&](uint64_t want) { return std::min<uint64_t>(n_pairs, want + want / 16 + 4096); };
+  uint64_t cap = pass_cap((n_pairs + n_pass - 1) / n_pass);
+  ExactItem *buf[2] = {nullptr, nullptr};
+  unsigned long long *cursor = nullptr;
+  void *temp = nullptr;
+  size_t temp_bytes = 0;
+  auto release = [&]() { cudaFree(buf[0]); cudaFree(buf[1]); cudaFree(temp); buf[0] = buf[1] = nullptr; temp = nullptr; };
+  auto reserve = [&](uint64_t c) -> int {                                // 0 ok, 1 no memory, 2 CUDA error
+    release();
+    cub::DoubleBuffer<ExactItem> keys(nullptr, nullptr);
+    temp_bytes = 0;
+    if (cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, keys, (int64_t)c, ExactItemDecomposer{}, 0, 94, stream) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return 2;
+    }
+    if (cudaMalloc((void **)&buf[0], c * sizeof(ExactItem)) != cudaSuccess || cudaMalloc((void **)&buf[1], c * sizeof(ExactItem)) != cudaSuccess ||
+        cudaMalloc(&temp, temp_bytes ? temp_bytes : 1) != cudaSuccess) {
+      (void)cudaGetLastError();
+      release();
+      return 1;
+    }
+    cap = c;
+    return 0;
+  };
+  if (cudaMalloc((void **)&cursor, 8) != cudaSuccess) { (void)cudaGetLastError(); return 1; }
+  int rc = reserve(cap);
+  const int grid = n_sm * 8;
+  for (uint32_t pass = 0; pass < n_pass && !rc; pass++) {
+    unsigned long long n = 0;
+    for (int attempt = 0; attempt < 2 && !rc; attempt++) {
+      cudaMemsetAsync(cursor, 0, 8, stream);
+      k_exact_sort_items<<<grid, 256, 0, stream>>>(slots, n_slots, (uint32_t)n_pass, pass, d_pre_of_taxon, buf[0], cap, cursor);
+      cudaMemcpyAsync(&n, cursor, 8, cudaMemcpyDeviceToHost, stream);
+      if (cudaStreamSynchronize(stream) != cudaSuccess) { (void)cudaGetLastError(); rc = 2; break; }
+      if (n <= cap) break;
+      rc = attempt ? 2 : reserve(n);                                     // an unlucky pass: room for all of its items
+    }
+    if (rc || n < 2) continue;
+    cub::DoubleBuffer<ExactItem> keys(buf[0], buf[1]);
+    if (cub::DeviceRadixSort::SortKeys(temp, temp_bytes, keys, (int64_t)n, ExactItemDecomposer{}, 0, 94, stream) != cudaSuccess) rc = 2;
+    if (!rc) k_exact_dups<<<grid, 256, 0, stream>>>(keys.Current(), n, d_parent, d_depth, d_books);
+    if (cudaStreamSynchronize(stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) rc = 2;
+  }
+  release();
+  cudaFree(cursor);
+  *passes_out = (uint32_t)n_pass;
+  return rc;
+}
 
 void launch_clade_max_batch(const uint8_t *regs, const uint32_t *d_offs, const uint32_t *d_members, uint32_t n_clades,
                             uint8_t *d_out, cudaStream_t stream) {

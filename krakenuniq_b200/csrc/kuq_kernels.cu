@@ -1497,6 +1497,65 @@ void launch_exact_import(const ExactPair *pairs, uint64_t n, const ExactSet &e, 
   if (n) k_exact_import<<<(int)min((uint64_t)device_sm_count() * 16, (n + 255) / 256), 256, 0, stream>>>(pairs, n, e, error_flag);
 }
 
+// Pairs of the slots [lo, hi) grouped by the owner of their k-mer, as k_keys_parts groups sparse-tier keys: the pairs of
+// a tile are ranked on shared-memory counters per part (only occupied slots touch them), and one thread per part and
+// CTA bumps the global cursor once per tile.  pass 0 only counts.
+constexpr int XP_E = 4;      // pairs per thread and tile (16 B each)
+__global__ void __launch_bounds__(256) k_exact_parts(const ExactPair *slots, uint64_t lo, uint64_t hi, uint32_t n_parts,
+                                                     unsigned long long *counters, ExactPair *out,
+                                                     const unsigned long long *part_end, uint32_t *error_flag, int pass) {
+  __shared__ uint32_t s_cnt[EXACT_MAX_PARTS];
+  __shared__ unsigned long long s_base[EXACT_MAX_PARTS];
+  const uint32_t tid = threadIdx.x;
+  if (tid < EXACT_MAX_PARTS) s_cnt[tid] = 0;
+  __syncthreads();
+  const uint64_t tile = (uint64_t)blockDim.x * XP_E;
+  for (uint64_t base = lo + (uint64_t)blockIdx.x * tile; base < hi; base += (uint64_t)gridDim.x * tile) {
+    ExactPair pr[XP_E];
+    uint32_t where[XP_E];                        // part << 24 | rank inside the tile's group of that part
+#pragma unroll
+    for (int j = 0; j < XP_E; j++) {
+      const uint64_t i = base + (uint64_t)j * blockDim.x + tid;
+      pr[j] = ExactPair{0ull, 0ull};
+      if (i < hi) pr[j] = slots[i];
+    }
+#pragma unroll
+    for (int j = 0; j < XP_E; j++) {
+      where[j] = 0;
+      if (pr[j].kmer1) {
+        const uint32_t part = exact_owner(pr[j].kmer1 - 1, n_parts);
+        const uint32_t r = atomicAdd(&s_cnt[part], 1u);
+        where[j] = (part << 24) | r;
+      }
+    }
+    if (pass == 1) {
+      __syncthreads();
+      if (tid < n_parts && s_cnt[tid]) s_base[tid] = atomicAdd(counters + tid, (unsigned long long)s_cnt[tid]);
+      __syncthreads();
+#pragma unroll
+      for (int j = 0; j < XP_E; j++) {
+        if (!pr[j].kmer1) continue;
+        const uint32_t part = where[j] >> 24;
+        const unsigned long long at = s_base[part] + (where[j] & 0xFFFFFFu);
+        if (at < part_end[part]) out[at] = pr[j]; else atomicExch(error_flag, 7u);
+      }
+      __syncthreads();
+      if (tid < EXACT_MAX_PARTS) s_cnt[tid] = 0;
+      __syncthreads();
+    }
+  }
+  if (pass == 0) {
+    __syncthreads();
+    if (tid < n_parts && s_cnt[tid]) atomicAdd(counters + tid, (unsigned long long)s_cnt[tid]);
+  }
+}
+void launch_exact_parts(const ExactPair *slots, uint64_t lo, uint64_t hi, uint32_t n_parts, unsigned long long *counters,
+                        ExactPair *out, const unsigned long long *part_end, uint32_t *error_flag, int pass, cudaStream_t stream) {
+  if (hi <= lo) return;
+  const int grid = (int)min((uint64_t)device_sm_count() * 8, (hi - lo + 256 * XP_E - 1) / (256 * XP_E));
+  k_exact_parts<<<grid, 256, 0, stream>>>(slots, lo, hi, n_parts, counters, out, part_end, error_flag, pass);
+}
+
 // distinct k-mers among the pairs whose taxon is a clade member
 __global__ void k_exact_union(ExactSet e, const uint8_t *member, unsigned long long *scratch, uint64_t smask,
                               unsigned long long *n_distinct, uint32_t *overflow) {

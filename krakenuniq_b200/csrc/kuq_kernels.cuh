@@ -95,6 +95,26 @@ struct KeySource {
 };
 
 #ifdef __CUDACC__
+// Owner and roll-up pass of a canonical k-mer of the exact set (kuq.h, kuq_exact_owner): a splitmix64 finalizer of the
+// k-mer alone.  The table's slot hash mixes (k-mer, taxon) with another function, so an owner's part of a table does
+// not crowd into a subset of its slots; the owner takes the high word, the roll-up passes the low word, so a context
+// that holds one owner's part still splits evenly over the passes.
+__host__ __device__ __forceinline__ uint64_t exact_kmer_hash(uint64_t kmer) {
+  uint64_t x = kmer ^ 0x2545F4914F6CDD1Dull;
+  x ^= x >> 30;
+  x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27;
+  x *= 0x94d049bb133111ebull;
+  x ^= x >> 31;
+  return x;
+}
+__host__ __device__ __forceinline__ uint32_t exact_owner(uint64_t kmer, uint32_t n_parts) {
+  return (uint32_t)(((exact_kmer_hash(kmer) >> 32) * n_parts) >> 32);
+}
+__host__ __device__ __forceinline__ uint32_t exact_pass(uint64_t kmer, uint32_t n_pass) {
+  return (uint32_t)(((exact_kmer_hash(kmer) & 0xFFFFFFFFull) * n_pass) >> 32);
+}
+
 // murmurhash3_finalizer (hyperloglogplus.cpp:830-838)
 __device__ __forceinline__ uint64_t fmix64(uint64_t key) {
   key += 1;
@@ -338,6 +358,11 @@ void launch_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, Exact
                          unsigned long long *n_out, cudaStream_t stream);
 // pairs (layout of ExactPair) into e; count[taxon] grows by the pairs that were new
 void launch_exact_import(const ExactPair *pairs, uint64_t n, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
+// occupied slots [lo, hi) grouped by the owner of their k-mer (exact_owner, at most EXACT_MAX_PARTS parts): pass 0 adds
+// the pairs per part to counters[part]; pass 1 scatters them through the cursors counters[part], bounded by part_end
+constexpr uint32_t EXACT_MAX_PARTS = 64;
+void launch_exact_parts(const ExactPair *slots, uint64_t lo, uint64_t hi, uint32_t n_parts, unsigned long long *counters,
+                        ExactPair *out, const unsigned long long *part_end, uint32_t *error_flag, int pass, cudaStream_t stream);
 void launch_sparse_union(const KeySource &src, const uint8_t *member,
                          unsigned long long *scratch_set, uint64_t scratch_mask, uint32_t *hist64, uint32_t *overflow,
                          cudaStream_t stream);
@@ -367,6 +392,13 @@ void launch_clade_max_batch(const uint8_t *regs, const uint32_t *d_offs, const u
 int sparse_clade_dups(const KeySource &set_keys, const KeySource &kept_keys, const uint8_t *dense_flag, uint64_t n_keys_upper,
                       const uint32_t *d_pre_of_taxon, const uint32_t *d_node_of_pre, const uint32_t *d_parent_c,
                       const uint32_t *d_depth_c, const int32_t *d_sid_of_node, uint32_t *d_dup, int n_sm, cudaStream_t stream);
+// exact mode: d_books[lca] -= 1 for every two pairs of the table with one k-mer that are adjacent in (k-mer, preorder)
+// order, their LCA in the taxonomy (d_parent / d_depth of the context, 0 = none).  Taxa with pre_of_taxon NONE are left
+// out.  In passes over parts of the k-mer space (exact_pass) sized to `budget` bytes of scratch.  0 = ok, 1 = not
+// enough device memory for one pass, 2 = CUDA error.
+int exact_clade_dups(const ExactPair *slots, uint64_t n_slots, uint64_t n_pairs, const uint32_t *d_pre_of_taxon,
+                     const uint32_t *d_parent, const uint16_t *d_depth, unsigned long long *d_books, uint64_t budget, int n_sm,
+                     cudaStream_t stream, uint32_t *passes_out);
 // kuq_layout_exp.cu: record-layout / search-shape experiment (0 ok, 1 no memory, 2 CUDA error, 3 taxon ids > 24 bits);
 // `product` = parameters of a k_lookup<MODE_LOOKUP> launch on the same database (scratch / output pointers are set there)
 int layout_experiment(const Params &product, uint64_t n_records, const uint64_t *canon, const uint32_t *bins, const uint32_t *ref,

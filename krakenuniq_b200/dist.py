@@ -206,6 +206,42 @@ def merge_classifier_state_partitioned(clf, device, group=None, timings: dict | 
             prev = t
 
 
+def merge_exact_partitioned(clf, device, group=None):
+    """End-of-run merge of exact k-mer sets (KUQ_HLL_EXACT) in O(pairs / world) per rank; no rank holds the union:
+      1. all-reduce SUM of the counters;
+      2. the (k-mer, taxon) pairs grouped by the rank owning their k-mer (kuq_exact_export_partitioned);
+      3. one all-to-all of the pairs (two int64 words each);
+      4. each rank rebuilds its table from what it received (kuq_exact_replace; duplicates collapse);
+      5. all-reduce SUM of the per-taxon set sizes and roll-up books (kuq_exact_summary / kuq_set_exact_summary).
+    Afterwards `counts()` and `clade_counts_tree()` report the union on every rank (until its next batch)."""
+    c = collectives(group)
+    world = c.world_size()
+    sp = clf.state_ptrs()
+    nk = device_view(sp.d_n_kmers, sp.n_sketch * 8, torch.int64, device)
+    nr = device_view(sp.d_n_reads, sp.n_taxa * 8, torch.int64, device)
+    c.all_reduce(nk, "sum")
+    c.all_reduce(nr, "sum")
+    torch.cuda.synchronize()
+    ptr, counts = clf.exact_export_partitioned_alloc(world)
+    n = int(counts.sum())
+    pairs = device_view(ptr, max(n, 1) * 16, torch.int64, device)[:2 * n]
+    recv = exchange_partitioned_keys(pairs, [2 * int(x) for x in counts], c)
+    torch.cuda.synchronize()
+    del pairs
+    clf.device_free(ptr)
+    recv = recv.contiguous()
+    clf.exact_replace(recv.data_ptr() if recv.numel() else None, recv.numel() // 2)
+    del recv
+    count = torch.zeros(sp.n_sketch, dtype=torch.int64, device=device)
+    books = torch.zeros(sp.n_taxa, dtype=torch.int64, device=device)
+    torch.cuda.synchronize()
+    clf.exact_summary(count.data_ptr(), books.data_ptr())
+    c.all_reduce(count, "sum")
+    c.all_reduce(books, "sum")
+    torch.cuda.synchronize()
+    clf.set_exact_summary(count.data_ptr(), books.data_ptr())
+
+
 def clade_counts_distributed(clf, clades, device, group=None):
     """(unique, reads, kmers) per clade (list of taxid lists) after merge_classifier_state_partitioned: the union
     histograms of the code partitions add up; one all-reduce for all clades."""
