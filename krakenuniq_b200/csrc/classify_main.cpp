@@ -9,6 +9,10 @@
 //   stats / progress lines         src/classify.cpp:361-375, 555-558
 //   taxDB reader, genome sizes     src/taxdb.hpp:563-605, 850-885
 //   report (clades, sorting, cols) src/taxdb.hpp:928-1123, src/classify.cpp:286-328
+//   --paired / --check-names       scripts/read_merger.pl (what scripts/krakenuniq:230-237 runs before classify): the
+//                                  mates are merged during the ingest; the one deviation is the exit status, EX_DATAERR
+//                                  where the merger stopped at a malformed record or a name mismatch (the wrapper
+//                                  ignores the merger's status and exits 0)
 // Not supported (exit with a message): -I uid mapping, -x together with several -d databases (the reference's own loop
 // for that combination queries database 0 in every pass, classify.cpp:585-632).
 #include <fcntl.h>
@@ -52,6 +56,8 @@ static vector<string> DB_filenames, Index_filenames;
 static uint32_t Minimum_hit_count = 1;        // -m (classify.cpp:45)
 static bool Quick_mode = false, Print_classified = false, Print_unclassified = false, Print_kraken = true;
 static bool Populate_memory = false, Only_classified_kraken_output = false, Print_sequence = false, Map_UIDs = false;
+static bool Paired = false, Check_names = false;  // --paired / --check-names: argv holds one pair of mate files
+static string Pair_error;                         // what read_merger.pl would have died with (the run exits EX_DATAERR)
 static uint64_t Populate_memory_size = 0;
 static string Classified_output_file, Unclassified_output_file, Kraken_output_file, Report_output_file, TaxDB_file;
 static size_t Work_unit_size = 500000;      // DEF_WORK_UNIT_SIZE, classify.cpp:38
@@ -90,6 +96,9 @@ static void usage(int exit_code = EX_USAGE) {
        << "  -M               Preload database files" << endl
        << "  -x size          Preload database files using x amount of RAM (e.g. 10G)" << endl
        << "  -s               Print read sequence in Kraken output" << endl
+       << "  --paired         The two files are mates of paired-end reads: each pair is classified as one" << endl
+       << "                   sequence mate1 + 'N' + mate2, named after mate 1 (what read_merger.pl writes)" << endl
+       << "  --check-names    With --paired: stop at the first pair whose names differ (exit status 65)" << endl
        << "  -h               Print this message" << endl
        << endl
        << "Kraken output is to standard output by default." << endl;
@@ -118,8 +127,13 @@ static void parse_command_line(int argc, char **argv) {
   int opt;
   long long sig;
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
-  while ((opt = getopt(argc, argv, "d:i:t:u:n:m:o:qcC:U:Ma:r:sI:p:x:")) != -1) {
+  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES };
+  static const struct option long_opts[] = {{"paired", no_argument, NULL, OPT_PAIRED},
+                                            {"check-names", no_argument, NULL, OPT_CHECK_NAMES}, {NULL, 0, NULL, 0}};
+  while ((opt = getopt_long(argc, argv, "d:i:t:u:n:m:o:qcC:U:Ma:r:sI:p:x:", long_opts, NULL)) != -1) {
     switch (opt) {
+      case OPT_PAIRED: Paired = true; break;
+      case OPT_CHECK_NAMES: Check_names = true; break;           // ignored without --paired (krakenuniq:281-283)
       case 'd': DB_filenames.push_back(optarg); break;
       case 'i': Index_filenames.push_back(optarg); break;
       case 't':
@@ -155,8 +169,13 @@ static void parse_command_line(int argc, char **argv) {
   }
   if (DB_filenames.empty()) { cerr << "Missing mandatory option -d" << endl; usage(); }
   if (Index_filenames.empty()) { cerr << "Missing mandatory option -i" << endl; usage(); }
+  if (Paired && argc - optind != 2) die(EX_USAGE, "--paired requires exactly two filenames");   // krakenuniq:160-161
   if (optind == argc && !Populate_memory) cerr << "No sequence data files specified" << endl;
 }
+
+// argv[i] is an input; with --paired it is mate file 1 and argv[i + 1] mate file 2
+static int input_step() { return Paired ? 2 : 1; }
+static const char *mate_of(char **argv, int i) { return Paired ? argv[i + 1] : NULL; }
 
 // ---- output streams: plain file, ".gz" → gzip, "-" → stdout (cout_or_file, classify.cpp:133-148) ---------------
 struct OutStream {
@@ -335,6 +354,159 @@ struct SeqReader {
     r.seq_len = bases.size() - r.seq_off;
     return true;
   }
+};
+
+// ---- paired-end input (--paired): the records scripts/read_merger.pl writes, merged during the ingest ------------
+// Both readers (MateFile + PairReader for the serial path, process_file_parallel for plain files) take their record
+// order from MergeOrder and their ids from mate_id, so the merger's rules live here.
+
+// The length of a mate's id: the run of non-space characters right after the '>' / '@' (h is the header line without
+// it), -1 when there is none (malformed, read_merger.pl:145-148,162-170); then s/[\/_.][12]$// (:182).  The id is a
+// prefix of h.
+static long mate_id(const char *h, size_t n) {
+  size_t k = 0;
+  while (k < n && !isspace((unsigned char)h[k])) k++;
+  if (k == 0) return -1;
+  if (k >= 2 && (h[k - 2] == '/' || h[k - 2] == '_' || h[k - 2] == '.') && (h[k - 1] == '1' || h[k - 1] == '2')) k -= 2;
+  return (long)k;
+}
+
+// The order of the merged records (read_merger.pl:102-127).  `read(k)` takes the next record of mate file k: 1 a
+// record, 0 the file has ended, -1 malformed.  `same()` compares the ids of the last record of each file.
+struct MergeOrder {
+  enum Kind { END, PAIR, ONLY1, ONLY2, EMPTY_N, MALFORMED, MISMATCH };
+  enum { PAIRS, REST1, REST2, DONE } phase = PAIRS;
+  template <class ReadMate, class Same> Kind next(ReadMate read, Same same) {
+    int a, b;
+    switch (phase) {
+      case PAIRS:
+        if ((a = read(0)) < 0) return fail(MALFORMED);
+        if ((b = read(1)) < 0) return fail(MALFORMED);
+        if (a == 0 && b == 0) { phase = DONE; return END; }
+        if (a == 0) { warn(2); phase = REST2; return ONLY2; }
+        if (b == 0) { warn(1); phase = REST1; return ONLY1; }
+        if (Check_names && !same()) return fail(MISMATCH);
+        return PAIR;
+      case REST1:
+        // after the rest of file 1 the loop falls through with both mates undefined and writes ">" + "N" (:104-118)
+        if ((a = read(0)) < 0) return fail(MALFORMED);
+        if (a == 0) { phase = DONE; return EMPTY_N; }
+        return ONLY1;
+      case REST2:
+        if ((b = read(1)) < 0) return fail(MALFORMED);
+        if (b == 0) { phase = DONE; return END; }
+        return ONLY2;
+      default:
+        return END;
+    }
+  }
+  Kind fail(Kind k) { phase = DONE; return k; }
+  static void warn(int longer) {
+    fprintf(stderr, "classify: mismatched sequence counts - file %d has more reads\n\n  Outputting the further reads unpaired\n", longer);
+  }
+};
+
+static string mismatch_message(const char *a, size_t na, const char *b, size_t nb) {     // :114-116
+  return "mismatched mate pair names ('" + string(a, na) + "' & '" + string(b, nb) + "')";
+}
+
+// read_sequence (read_merger.pl:136-183) over one mate file: the format is file 1's, whatever this file holds
+struct MateFile {
+  LineReader in;
+  bool fasta = false;
+  string buffer, id, seq;                  // buffer: the next record's header line, when have_line
+  bool have_line = false, line_nl = false, ended = false;
+  int read(string &err) {
+    if (ended) return 0;
+    if (!have_line) {
+      if (!in.getline(buffer)) { ended = true; return 0; }
+      have_line = true;
+      line_nl = !in.eofbit;
+    }
+    const long k = buffer.empty() || buffer[0] != (fasta ? '>' : '@') ? -1 : mate_id(buffer.data() + 1, buffer.size() - 1);
+    if (k < 0) {
+      if (!fasta && buffer.empty()) { ended = true; return 0; }    // a blank line ends a FASTQ file (:165-167)
+      err = string(fasta ? "malformed fasta file" : "malformed fastq file") + " (line = '" + buffer + (line_nl ? "\n" : "") + "')";
+      return -1;
+    }
+    id.assign(buffer, 1, (size_t)k);
+    have_line = false;
+    seq.clear();
+    if (fasta) {                                                   // every line up to the next '>' line, '\n' removed
+      string line;
+      while (in.getline(line)) {
+        if (!line.empty() && line[0] == '>') { buffer.swap(line); have_line = true; line_nl = !in.eofbit; break; }
+        seq += line;
+      }
+    } else {                                                       // line 2; lines 3 and 4 are skipped unchecked
+      string skip;
+      in.getline(seq);
+      in.getline(skip);
+      in.getline(skip);
+    }
+    return 1;
+  }
+};
+
+// The merged records of two mate files, with SeqReader::next's interface (the serial path: compressed files and pipes)
+struct PairReader {
+  MateFile m[2];
+  MergeOrder order;
+  bool valid = true;
+  void open(const char *f1, const char *f2) {
+    const char *names[2] = {f1, f2};
+    for (int k = 0; k < 2; k++) {
+      struct stat sb;
+      const bool regular = stat(names[k], &sb) == 0 && S_ISREG(sb.st_mode);
+      unsigned char magic[3] = {0, 0, 0};
+      if (regular)                                                 // determine_file_type (:199-216)
+        if (FILE *f = fopen(names[k], "rb")) { size_t got = fread(magic, 1, 3, f); (void)got; fclose(f); }
+      if (!m[k].in.open(names[k])) die(EX_NOINPUT, string("can't open ") + names[k]);
+      const bool known = magic[0] == '@' || magic[0] == '>' || is_bzip2(magic) || (magic[0] == 0x1f && magic[1] == 0x8b && magic[2] == 8);
+      if (regular && !known) { stop(string("Unknown input file type for ") + names[k]); return; }
+    }
+    const int c = m[0].in.peek();                                  // the format: file 1's first line (:66-75)
+    if (c != '>' && c != '@') { stop(string("Unknown file format for ") + f1); return; }
+    m[0].fasta = m[1].fasta = c == '>';
+  }
+  void stop(const string &why) { Pair_error = why; valid = false; }
+  void close() { m[0].in.close(); m[1].in.close(); }
+  bool next(Read &r, string &bases) {
+    if (!valid) return false;
+    string err;
+    auto kind = order.next([&](int k) { return m[k].read(err); }, [&] { return m[0].id == m[1].id; });
+    r.quals.clear();
+    r.seq_off = bases.size();
+    switch (kind) {
+      case MergeOrder::PAIR: r.id = m[0].id; bases += m[0].seq; bases += 'N'; bases += m[1].seq; break;
+      case MergeOrder::ONLY1: r.id = m[0].id; bases += m[0].seq; break;
+      case MergeOrder::ONLY2: r.id = m[1].id; bases += m[1].seq; break;
+      case MergeOrder::EMPTY_N: r.id.clear(); bases += 'N'; break;
+      case MergeOrder::MALFORMED: stop(err); return false;
+      case MergeOrder::MISMATCH: stop(mismatch_message(m[0].id.data(), m[0].id.size(), m[1].id.data(), m[1].id.size())); return false;
+      case MergeOrder::END: valid = false; return false;
+    }
+    r.header_line = r.id;
+    r.seq_len = bases.size() - r.seq_off;
+    return true;
+  }
+};
+
+// The records of one input of process_file / BatchReader: a FASTA / FASTQ file, or two mate files merged (--paired)
+struct InputReader {
+  SeqReader single;
+  PairReader pair;
+  bool paired = false;
+  void open(const char *filename, const char *mate2) {
+    paired = mate2 != NULL;
+    if (paired) { pair.open(filename, mate2); return; }
+    if (!single.in.open(filename)) die(EX_NOINPUT, string("can't open ") + filename);
+    single.fastq = single.in.peek() == '@';                        // determine_input_file_type, :377-388
+  }
+  bool fastq() const { return !paired && single.fastq; }          // merged records are FASTA
+  bool valid() const { return paired ? pair.valid : single.valid; }
+  bool next(Read &r, string &bases) { return paired ? pair.next(r, bases) : single.next(r, bases); }
+  void close() { if (paired) pair.close(); else single.in.close(); }
 };
 
 // ---- taxonomy (taxdb.hpp:563-605) + report (taxdb.hpp:928-1123) ------------------------------------------------
@@ -762,43 +934,180 @@ static void prepare_stage(Stage &s, uint64_t bases, size_t reads) {
 // Several GPUs (replicas: every device holds the database): batches go round-robin over the contexts; results come back
 // in submission order, so the Kraken output stays in file order whatever the number of devices.
 static vector<kuq_ctx *> All_ctx;
-static bool process_file_parallel(kuq_ctx *ctx0, const char *filename) {
+
+// A plain file (regular, uncompressed) mapped and cut into chunks at record boundaries, every chunk parsed by its own
+// thread
+struct PlainInput {
+  const char *base = NULL, *fend = NULL;
+  size_t size = 0;
+  vector<const char *> cut;
+  vector<ChunkParse> parsed;
+  bool map(const char *filename) {
+    int fd = ::open(filename, O_RDONLY);
+    if (fd < 0) return false;
+    struct stat sb;
+    if (fstat(fd, &sb) < 0 || !S_ISREG(sb.st_mode) || sb.st_size < 2) { ::close(fd); return false; }
+    size = sb.st_size;
+    base = (const char *)mmap(0, size, PROT_READ, MAP_PRIVATE, fd, 0);
+    ::close(fd);
+    if (base == MAP_FAILED) { base = NULL; return false; }
+    if (((unsigned char)base[0] == 0x1f && (unsigned char)base[1] == 0x8b) || (size >= 3 && is_bzip2((const unsigned char *)base))) {
+      unmap();                                                      // gzip / bzip2: the serial reader decompresses
+      return false;
+    }
+    madvise((void *)base, size, MADV_WILLNEED);
+    fend = base + size;
+    return true;
+  }
+  void unmap() { if (base) munmap((void *)base, size); base = NULL; }
+  void parse(bool fastq, int T) {
+    const int n_chunks = (int)std::min<size_t>((size_t)T * 4, std::max<size_t>(1, size / (1 << 20)));
+    cut.assign(n_chunks + 1, NULL);
+    cut[0] = base; cut[n_chunks] = fend;
+    for (int c = 1; c < n_chunks; c++) cut[c] = next_record_start(base + size * c / n_chunks, base, fend, fastq);
+    for (int c = 1; c <= n_chunks; c++) if (cut[c] < cut[c - 1]) cut[c] = cut[c - 1];
+    parsed.assign(n_chunks, ChunkParse());
+#pragma omp parallel for schedule(dynamic, 1) num_threads(T)
+    for (int c = 0; c < n_chunks; c++) {
+      if (cut[c] >= cut[c + 1]) continue;
+      if (fastq) parse_fastq_chunk(cut[c], cut[c + 1], fend, parsed[c]);
+      else parse_fasta_chunk(cut[c], cut[c + 1], fend, parsed[c]);
+    }
+  }
+};
+
+static string malformed_message(bool fasta, char marker, const char *line, size_t n, bool newline) {   // :149,170
+  return string(fasta ? "malformed fasta file" : "malformed fastq file") + " (line = '" + (marker ? string(1, marker) : "") +
+         string(line, n) + (newline ? "\n" : "") + "')";
+}
+
+// Where a merged record's bases come from: s1, then 'N' and s2 when the record joins two mates
+struct MateSeqs { const char *s1, *s2; uint32_t n1, n2; bool joined; };
+
+// The records of two parsed mate files, merged (MergeOrder, mate_id): each view is named by the stripped id of its mate
+// (a prefix of that mate's header).  False where the chunk parsers and read_merger.pl part ways (a FASTQ record without
+// its '+' line, a file that does not start with a header, a FASTA header on the last line without a newline): the
+// serial PairReader then reads the pair.
+static bool merge_parsed(const PlainInput (&in)[2], bool fastq, int T, vector<View> &merged, vector<MateSeqs> &mates) {
+  struct Rec { const View *v; const char *seq; long id; };
+  vector<Rec> recs[2];
+  for (int k = 0; k < 2; k++) {
+    const vector<ChunkParse> &parsed = in[k].parsed;
+    int last_chunk = (int)parsed.size();
+    for (int c = 0; c < (int)parsed.size(); c++) {
+      if (!parsed[c].stopped) continue;
+      // a blank line where a FASTQ header should be ends the file for both; any other stop differs
+      const vector<View> &rs = parsed[c].reads;
+      const char *p = rs.empty() ? in[k].cut[c] : rs.back().qual + rs.back().qual_len + 1;
+      if (!fastq || p >= in[k].fend || *p != '\n') return false;
+      last_chunk = c + 1;
+      break;
+    }
+    vector<size_t> first_of(last_chunk + 1, 0);
+    for (int c = 0; c < last_chunk; c++) first_of[c + 1] = first_of[c] + parsed[c].reads.size();
+    recs[k].resize(first_of[last_chunk]);
+#pragma omp parallel for schedule(dynamic, 1) num_threads(T)
+    for (int c = 0; c < last_chunk; c++) {
+      size_t i = first_of[c];
+      for (const View &v : parsed[c].reads)
+        recs[k][i++] = {&v, v.owned >= 0 ? parsed[c].arena[v.owned].data() : v.seq, mate_id(v.hdr, v.hdr_len)};
+    }
+  }
+  auto pair_view = [](const Rec &a, const Rec &b, View &m, MateSeqs &s) {
+    m.hdr = a.v->hdr; m.hdr_len = (uint32_t)a.id;
+    m.qual = NULL; m.qual_len = 0; m.owned = -1; m.seq = NULL;
+    s = {a.seq, b.seq, a.v->seq_len, b.v->seq_len, true};
+    const uint64_t len = (uint64_t)s.n1 + 1 + s.n2;
+    m.seq_len = (uint32_t)std::min<uint64_t>(len, UINT32_MAX);
+    return len;
+  };
+  // Every pair before the first one that stops the merger (a malformed header, a name mismatch) is merged as a pair
+  // (PAIRS in MergeOrder): those are merged in parallel, and MergeOrder goes on from the first stop.
+  const size_t n_pair = std::min(recs[0].size(), recs[1].size());
+  size_t first_stop = n_pair;
+#pragma omp parallel for schedule(static) num_threads(T) reduction(min : first_stop)
+  for (size_t i = 0; i < n_pair; i++) {
+    const Rec &a = recs[0][i], &b = recs[1][i];
+    if (a.id < 0 || b.id < 0 || (Check_names && (a.id != b.id || memcmp(a.v->hdr, b.v->hdr, a.id) != 0))) first_stop = std::min(first_stop, i);
+  }
+  merged.resize(first_stop);
+  mates.resize(first_stop);
+  uint64_t longest = 0;
+#pragma omp parallel for schedule(static) num_threads(T) reduction(max : longest)
+  for (size_t i = 0; i < first_stop; i++) longest = std::max(longest, pair_view(recs[0][i], recs[1][i], merged[i], mates[i]));
+  if (longest > (280ull << 20)) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
+  size_t next_of[2] = {first_stop, first_stop};
+  const Rec *cur[2] = {NULL, NULL};
+  int last_read = 0;
+  auto read = [&](int k) {
+    if (next_of[k] >= recs[k].size()) return 0;
+    cur[k] = &recs[k][next_of[k]++];
+    last_read = k;
+    return cur[k]->id < 0 ? -1 : 1;
+  };
+  auto same = [&] { return cur[0]->id == cur[1]->id && memcmp(cur[0]->v->hdr, cur[1]->v->hdr, cur[0]->id) == 0; };
+  MergeOrder order;
+  for (;;) {
+    const MergeOrder::Kind kind = order.next(read, same);
+    if (kind == MergeOrder::END) break;
+    if (kind == MergeOrder::MALFORMED) {
+      const View &v = *cur[last_read]->v;
+      Pair_error = malformed_message(!fastq, fastq ? '@' : '>', v.hdr, v.hdr_len, v.hdr + v.hdr_len < in[last_read].fend);
+      break;
+    }
+    if (kind == MergeOrder::MISMATCH) {
+      Pair_error = mismatch_message(cur[0]->v->hdr, cur[0]->id, cur[1]->v->hdr, cur[1]->id);
+      break;
+    }
+    View m;
+    MateSeqs s;
+    uint64_t len;
+    if (kind == MergeOrder::PAIR) {
+      len = pair_view(*cur[0], *cur[1], m, s);
+    } else {
+      const Rec *a = kind == MergeOrder::ONLY2 ? cur[1] : cur[0];
+      m.hdr = kind == MergeOrder::EMPTY_N ? "" : a->v->hdr;
+      m.hdr_len = kind == MergeOrder::EMPTY_N ? 0 : (uint32_t)a->id;
+      m.qual = NULL; m.qual_len = 0; m.owned = -1; m.seq = NULL;
+      s = kind == MergeOrder::EMPTY_N ? MateSeqs{NULL, NULL, 0, 0, true} : MateSeqs{a->seq, NULL, a->v->seq_len, 0, false};
+      len = m.seq_len = s.n1 + s.joined;
+    }
+    if (len > (280ull << 20)) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
+    merged.push_back(m);
+    mates.push_back(s);
+  }
+  return true;
+}
+
+static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const char *mate2) {
   const vector<kuq_ctx *> ctxs = All_ctx.empty() ? vector<kuq_ctx *>{ctx0} : All_ctx;
   const int G = (int)ctxs.size();
-  int fd = ::open(filename, O_RDONLY);
-  if (fd < 0) return false;
-  struct stat sb;
-  if (fstat(fd, &sb) < 0 || !S_ISREG(sb.st_mode) || sb.st_size < 2) { ::close(fd); return false; }
-  const size_t size = sb.st_size;
-  const char *base = (const char *)mmap(0, size, PROT_READ, MAP_PRIVATE, fd, 0);
-  ::close(fd);
-  if (base == MAP_FAILED) return false;
-  if (((unsigned char)base[0] == 0x1f && (unsigned char)base[1] == 0x8b) || (size >= 3 && is_bzip2((const unsigned char *)base))) {
-    munmap((void *)base, size);                                     // gzip / bzip2: the serial reader decompresses
+  PlainInput in[2];
+  if (!in[0].map(filename)) return false;
+  // mate files: both plain, both starting with a header (determine_file_type, read_merger.pl:199-216)
+  auto header_first = [](const PlainInput &f) { return f.base[0] == '>' || f.base[0] == '@'; };
+  if (mate2 && (!in[1].map(mate2) || !header_first(in[0]) || !header_first(in[1]))) {
+    in[0].unmap(); in[1].unmap();
     return false;
   }
-  madvise((void *)base, size, MADV_WILLNEED);
-  const char *fend = base + size;
-  const bool fastq = Fastq_input = base[0] == '@';                                  // determine_input_file_type
+  const bool fastq_records = in[0].base[0] == '@';                   // determine_input_file_type; mate files: :66-75
+  const bool fastq = Fastq_input = fastq_records && !mate2;          // merged records are FASTA
   const int T = std::max(1, Num_threads);
-  const int n_chunks = (int)std::min<size_t>((size_t)T * 4, std::max<size_t>(1, size / (1 << 20)));
-  vector<const char *> cut(n_chunks + 1);
-  cut[0] = base; cut[n_chunks] = fend;
-  for (int c = 1; c < n_chunks; c++) cut[c] = next_record_start(base + size * c / n_chunks, base, fend, fastq);
-  for (int c = 1; c <= n_chunks; c++) if (cut[c] < cut[c - 1]) cut[c] = cut[c - 1];
   double T0__ = now_s();
-  vector<ChunkParse> parsed(n_chunks);
-#pragma omp parallel for schedule(dynamic, 1) num_threads(T)
-  for (int c = 0; c < n_chunks; c++) {
-    if (cut[c] >= cut[c + 1]) continue;
-    if (fastq) parse_fastq_chunk(cut[c], cut[c + 1], fend, parsed[c]);
-    else parse_fasta_chunk(cut[c], cut[c + 1], fend, parsed[c]);
-  }
+  for (int k = 0; k < (mate2 ? 2 : 1); k++) in[k].parse(fastq_records, T);
+  vector<ChunkParse> &parsed = in[0].parsed;
+  const int n_chunks = (int)parsed.size();
   TICK("parse");
+  vector<View> merged;
+  vector<MateSeqs> mates;
+  if (mate2 && !merge_parsed(in, fastq_records, T, merged, mates)) {
+    in[0].unmap(); in[1].unmap();
+    return false;
+  }
   // the reference stops at the first record its reader rejects
   size_t n_total = 0;
-  int last_chunk = n_chunks;
-  for (int c = 0; c < n_chunks; c++) {
+  int last_chunk = mate2 ? 0 : n_chunks;
+  for (int c = 0; c < last_chunk; c++) {
     n_total += parsed[c].reads.size();
     if (parsed[c].stopped) {
       if (!parsed[c].warning.empty()) fprintf(stderr, "classify: %s\n", parsed[c].warning.c_str());
@@ -808,11 +1117,14 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename) {
   }
   vector<size_t> first_of(last_chunk + 1, 0);
   for (int c = 0; c < last_chunk; c++) first_of[c + 1] = first_of[c] + parsed[c].reads.size();
-  n_total = first_of[last_chunk];
+  n_total = mate2 ? merged.size() : first_of[last_chunk];
   // flat views of all reads + cumulative sequence length (parallel per chunk, chunk bases from a short serial scan)
   vector<const View *> rv(n_total);
   vector<uint64_t> cum(n_total + 1);
-  {
+  if (mate2) {
+    cum[0] = 0;
+    for (size_t i = 0; i < n_total; i++) { rv[i] = &merged[i]; cum[i + 1] = cum[i] + merged[i].seq_len; }
+  } else {
     vector<uint64_t> chunk_nt(last_chunk + 1, 0);
 #pragma omp parallel for schedule(dynamic, 1) num_threads(T)
     for (int c = 0; c < last_chunk; c++) {
@@ -885,6 +1197,13 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename) {
     for (size_t i = 0; i < n; i++) {
       const View &v = *rv[b.begin + i];
       s.offs[i] = cum[b.begin + i] - c0;
+      if (mate2) {                                                   // seq1 . "N" . seq2 (read_merger.pl:187-191)
+        const MateSeqs &m = mates[b.begin + i];
+        char *d = s.bases + s.offs[i];
+        memcpy(d, m.s1, m.n1);
+        if (m.joined) { d[m.n1] = 'N'; memcpy(d + m.n1 + 1, m.s2, m.n2); }
+        continue;
+      }
       const char *src = v.owned >= 0 ? parsed[chunk_of(b.begin + i)].arena[v.owned].data() : v.seq;
       memcpy(s.bases + s.offs[i], src, v.seq_len);
     }
@@ -1016,17 +1335,20 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename) {
   for (kuq_ctx *c : ctxs) if (kuq_finish(c)) die(EX_SOFTWARE, kuq_last_error(c));
   TICK("kuq_finish (harvest)");
   // tearing down a multi-GB mapping takes ~0.1 s of page-table work nobody has to wait for
-  std::thread([base, size] { munmap((void *)base, size); }).detach();
+  std::thread([b0 = in[0].base, s0 = in[0].size, b1 = in[1].base, s1 = in[1].size] {
+    munmap((void *)b0, s0);
+    if (b1) munmap((void *)b1, s1);
+  }).detach();
   TICK("unmap (detached)");
   (void)ctx0;
   return true;
 }
 
-static void process_file(kuq_ctx *ctx, const char *filename) {
-  if (!getenv("KUQ_SERIAL_INGEST") && process_file_parallel(ctx, filename)) return;   // plain files: parallel path
-  SeqReader reader;
-  if (!reader.in.open(filename)) die(EX_NOINPUT, string("can't open ") + filename);
-  Fastq_input = reader.fastq = reader.in.peek() == '@';            // determine_input_file_type, :377-388
+static void process_file(kuq_ctx *ctx, const char *filename, const char *mate2) {
+  if (!getenv("KUQ_SERIAL_INGEST") && process_file_parallel(ctx, filename, mate2)) return;   // plain files: parallel path
+  InputReader reader;
+  reader.open(filename, mate2);
+  Fastq_input = reader.fastq();
   const uint64_t BATCH_NT = 96ull << 20;
   Batch batches[2];
   int cur = 0, inflight = -1;
@@ -1054,7 +1376,7 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
     batch_units = 0;
   };
   Read r;
-  while (reader.valid) {
+  while (reader.valid()) {
     Batch &b = batches[cur];
     if (!reader.next(r, b.bases)) break;
     if (r.seq_len > (280ull << 20)) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
@@ -1105,7 +1427,7 @@ static void process_file(kuq_ctx *ctx, const char *filename) {
   }
   if (inflight >= 0) wait_emit(inflight);
   if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));     // work units do not span input files
-  reader.in.close();
+  reader.close();
 }
 
 // ---- chunked mode: `-x size` with a database that does not fit (process_file_with_db_chunk, classify.cpp:566-791) --
@@ -1121,13 +1443,13 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 // sketch rule of the preloaded path needs.  The -x path of the reference reads sequence by sequence without work units
 // (:566-791): unit_aligned = false.  A batch closes (at a unit boundary when aligned) once it holds max_nt bases.
 struct BatchReader {
-  SeqReader reader;
+  InputReader reader;
   bool fq = false, unit_aligned = false, done = false;
   uint64_t max_nt = 96ull << 20;
   uint64_t unit_nt = 0;
-  BatchReader(const char *filename, bool aligned) : unit_aligned(aligned) {
-    if (!reader.in.open(filename)) die(EX_NOINPUT, string("can't open ") + filename);
-    fq = reader.fastq = reader.in.peek() == '@';
+  BatchReader(const char *filename, const char *mate2, bool aligned) : unit_aligned(aligned) {
+    reader.open(filename, mate2);
+    fq = reader.fastq();
   }
   bool next(Batch &b) {
     b.clear();
@@ -1136,7 +1458,7 @@ struct BatchReader {
     Read r;
     size_t unit_first_read = 0;        // first read of the open work unit inside this batch
     size_t batch_units = 0;
-    while (reader.valid) {
+    while (reader.valid()) {
       if (!reader.next(r, b.bases)) break;
       b.reads.push_back(r);
       b.offs.push_back(b.bases.size());
@@ -1158,13 +1480,13 @@ struct BatchReader {
       b.offs.resize(unit_first_read + 1);
     }
     done = true;
-    reader.in.close();
+    reader.close();
     return !b.reads.empty();
   }
 };
 
-static void load_file_batches(const char *filename, vector<Batch> &out, bool unit_aligned) {
-  BatchReader br(filename, unit_aligned);
+static void load_file_batches(const char *filename, const char *mate2, vector<Batch> &out, bool unit_aligned) {
+  BatchReader br(filename, mate2, unit_aligned);
   Batch b;
   while (br.next(b)) out.push_back(std::move(b));
 }
@@ -1264,12 +1586,12 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     for (;;) {
       if (!br) {
         if (fi >= argc) return false;
-        br.reset(new BatchReader(argv[fi], unit_rule));
+        br.reset(new BatchReader(argv[fi], mate_of(argv, fi), unit_rule));
         br->max_nt = batch_nt;
       }
       if (br->next(b)) { b.file = fi; return true; }
       br.reset();
-      fi++;
+      fi += input_step();
     }
   };
   // work-unit ids of the per-work-unit rule: process_file's cutting (classify.cpp:506-521), units end with their file
@@ -1405,9 +1727,9 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
   const int G = (int)ctxs.size();
   const uint64_t R = n_phases;
   vector<Batch> batches;
-  for (int i = optind; i < argc; i++) {
+  for (int i = optind; i < argc; i += input_step()) {
     const size_t from = batches.size();
-    load_file_batches(argv[i], batches, /*unit_aligned=*/true);
+    load_file_batches(argv[i], mate_of(argv, i), batches, /*unit_aligned=*/true);
     for (size_t j = from; j < batches.size(); j++) batches[j].file = i;
   }
   uint64_t max_bases = 64, max_reads = 4;
@@ -1793,7 +2115,7 @@ int main(int argc, char **argv) {
   if (want_shards && n_db == 1) run_sharded(All_ctx, kdb, idx, argc, argv, db_counts[0]);
   else if (want_shards) run_sharded_multi(All_ctx, kdbs, idxs, argc, argv, db_counts);
   else if (chunk_budget) run_streamed(ctx, kdbs, idxs, chunk_budget, hbm_budget, argc, argv, db_counts);
-  else for (int i = optind; i < argc; i++) process_file(ctx, argv[i]);
+  else for (int i = optind; i < argc; i += input_step()) process_file(ctx, argv[i], mate_of(argv, i));
   // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
   {
     double T0__ = now_s();
@@ -1893,5 +2215,7 @@ int main(int argc, char **argv) {
   Classified_out.close();
   Unclassified_out.close();
   for (kuq_ctx *c : All_ctx) kuq_destroy(c);
+  // the records before the merger's stop are classified and written, like the wrapper's run on its partial output
+  if (!Pair_error.empty()) { cerr << "classify: " << Pair_error << endl; return EX_DATAERR; }
   return 0;
 }
