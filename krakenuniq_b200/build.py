@@ -12,7 +12,8 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "lib", "libkuq.so")
 SOURCES = ["kuq_kernels.cu", "kuq_api.cu", "kuq_dbbuild.cu", "kuq_microbench.cu", "kuq_layout_exp.cu", "kuq_clades.cu",
            "kuq_collisions.cu", "kuq_kmerset.cu"]
-HEADERS = ["kuq_kernels.cuh", "kuq_minimizer.cuh", "kuq_bounce.cuh", "kuq_ranges.h", os.path.join(ROOT, "include", "kuq.h")]
+HEADERS = ["kuq_kernels.cuh", "kuq_minimizer.cuh", "kuq_bounce.cuh", "kuq_ranges.h", "kuq_batches.h",
+           os.path.join(ROOT, "include", "kuq.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--compiler-bindir", "/usr/bin/g++", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared", "-cudart", "shared"]
 
@@ -56,7 +57,7 @@ def build_classify(force: bool = False) -> str:
     src = os.path.join(CSRC, "classify_main.cpp")
     build(force=force)
     exact = CLASSIFY + "Exact"
-    newest = max(os.path.getmtime(src), os.path.getmtime(LIB))
+    newest = max(os.path.getmtime(p) for p in (src, LIB, os.path.join(CSRC, "kuq_batches.h"), os.path.join(CSRC, "kuq_ranges.h")))
     if not force and all(os.path.exists(x) and os.path.getmtime(x) >= newest for x in (CLASSIFY, exact)):
         return CLASSIFY
     os.makedirs(os.path.dirname(CLASSIFY), exist_ok=True)

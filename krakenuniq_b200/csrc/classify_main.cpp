@@ -4,7 +4,7 @@
 // scripts/krakenuniq:240-248 can call it unchanged; the per-read work (classify_sequence, :897-1012) happens on the
 // GPU behind include/kuq.h.  Host-side pieces restated here, each citing what it mirrors:
 //   FASTA/FASTQ readers            src/seqreader.cpp:34-129 (gz through zlib instead of bxzstr)
-//   work-unit loop                 src/classify.cpp:506-559 (batches hold whole work units, DESIGN.md §4)
+//   work-unit loop                 src/classify.cpp:506-559 (batches hold whole work units, DESIGN.md §4): kuq_batches.h
 //   Kraken output lines            src/classify.cpp:980-1010, hitlist_string :826-861
 //   stats / progress lines         src/classify.cpp:361-375, 555-558
 //   taxDB reader, genome sizes     src/taxdb.hpp:563-605, 850-885
@@ -40,7 +40,6 @@
 #include <iomanip>
 #include <iostream>
 #include <map>
-#include <memory>
 #include <set>
 #include <sstream>
 #include <string>
@@ -48,6 +47,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_batches.h"
 #include "kuq_ranges.h"
 
 using namespace std;
@@ -173,10 +173,6 @@ static void parse_command_line(int argc, char **argv) {
   if (optind == argc && !Populate_memory) cerr << "No sequence data files specified" << endl;
 }
 
-// argv[i] is an input; with --paired it is mate file 1 and argv[i + 1] mate file 2
-static int input_step() { return Paired ? 2 : 1; }
-static const char *mate_of(char **argv, int i) { return Paired ? argv[i + 1] : NULL; }
-
 // ---- output streams: plain file, ".gz" → gzip, "-" → stdout (cout_or_file, classify.cpp:133-148) ---------------
 struct OutStream {
   FILE *f = NULL;
@@ -207,7 +203,7 @@ struct OutStream {
 
 // ---- input: FASTA / FASTQ through zlib (plain or gzip), semantics of src/seqreader.cpp -------------------------
 struct Read {
-  string id, header_line, quals;
+  string header_line, quals;
   uint64_t seq_off, seq_len;          // into the batch's bases buffer
 };
 
@@ -292,14 +288,6 @@ struct LineReader {     // std::ifstream + std::getline state semantics (eofbit 
   }
 };
 
-static string first_token(const string &s) {            // istringstream >> id
-  size_t a = 0;
-  while (a < s.size() && isspace((unsigned char)s[a])) a++;
-  size_t b = a;
-  while (b < s.size() && !isspace((unsigned char)s[b])) b++;
-  return s.substr(a, b - a);
-}
-
 struct SeqReader {
   LineReader in;
   bool fastq = false, valid = true;
@@ -319,7 +307,6 @@ struct SeqReader {
         return false;
       }
       r.header_line = line.substr(1);
-      r.id = first_token(r.header_line);
       string seq;
       in.getline(seq);
       in.getline(line);
@@ -344,7 +331,6 @@ struct SeqReader {
       return false;
     }
     r.header_line = line.substr(1);
-    r.id = first_token(r.header_line);
     r.seq_off = bases.size();
     while (in.good()) {
       in.getline(line);
@@ -478,15 +464,14 @@ struct PairReader {
     r.quals.clear();
     r.seq_off = bases.size();
     switch (kind) {
-      case MergeOrder::PAIR: r.id = m[0].id; bases += m[0].seq; bases += 'N'; bases += m[1].seq; break;
-      case MergeOrder::ONLY1: r.id = m[0].id; bases += m[0].seq; break;
-      case MergeOrder::ONLY2: r.id = m[1].id; bases += m[1].seq; break;
-      case MergeOrder::EMPTY_N: r.id.clear(); bases += 'N'; break;
+      case MergeOrder::PAIR: r.header_line = m[0].id; bases += m[0].seq; bases += 'N'; bases += m[1].seq; break;
+      case MergeOrder::ONLY1: r.header_line = m[0].id; bases += m[0].seq; break;
+      case MergeOrder::ONLY2: r.header_line = m[1].id; bases += m[1].seq; break;
+      case MergeOrder::EMPTY_N: r.header_line.clear(); bases += 'N'; break;
       case MergeOrder::MALFORMED: stop(err); return false;
       case MergeOrder::MISMATCH: stop(mismatch_message(m[0].id.data(), m[0].id.size(), m[1].id.data(), m[1].id.size())); return false;
       case MergeOrder::END: valid = false; return false;
     }
-    r.header_line = r.id;
     r.seq_len = bases.size() - r.seq_off;
     return true;
   }
@@ -688,73 +673,133 @@ static double get_seconds(struct timeval a, struct timeval b) {
   return (b.tv_sec - a.tv_sec) + (b.tv_usec - a.tv_usec) / 1e6;
 }
 
-// ---- the work-unit loop ---------------------------------------------------------------------------------------
+// ---- batches and their output ------------------------------------------------------------------------------------
 struct Batch {
   string bases;
   vector<uint64_t> offs{0};
   vector<Read> reads;
+  vector<uint32_t> units;             // the reads' work units (kuq_batches.h)
   bool fastq = false;
-  int file = 0;                       // index of the input file (work units do not span files)
-  void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); }
+  void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); units.clear(); }
 };
 
+static const uint64_t SLOT_NT = 280ull << 20;   // the longest read of the resident paths, below the slot capacity (288 MiB)
+
+// The limits of a batch (kuq_batches.h) with the work units of this run.  Resident databases: a batch fills one slot,
+// and KUQ_BATCH_READS closes it at the first unit boundary after that many reads (tests: small batches).
+static BatchLimits batch_limits(uint64_t batch_nt, bool aligned, bool resident) {
+  BatchLimits l;
+  l.batch_nt = batch_nt;
+  l.max_units = Max_units_per_batch;
+  l.unit_size = Work_unit_size;
+  l.aligned = aligned;
+  l.slot_nt = resident ? SLOT_NT : 0;
+  const char *v = getenv("KUQ_BATCH_READS");
+  if (resident && v) l.batch_reads = std::min<size_t>(l.batch_reads, std::max<size_t>(1, strtoull(v, NULL, 10)));
+  return l;
+}
+
 static OutStream Kraken_out, Classified_out, Unclassified_out;
-static bool Fastq_input = false;
 
-static void print_sequence(OutStream &o, const Read &r, const string &bases) {   // classify.cpp:794-805
-  string s;
-  if (Fastq_input) {
-    s = "@" + r.header_line + "\n";
-    s.append(bases, r.seq_off, r.seq_len);
-    s += "\n+\n" + r.quals + "\n";
-  } else {
-    s = ">" + r.header_line + "\n";
-    s.append(bases, r.seq_off, r.seq_len);
-    s += "\n";
-  }
-  o.write(s);
-}
+// One read as the output sees it: the header line without its '>' / '@', the bases and (FASTQ) the qualities
+struct ReadView {
+  const char *hdr; size_t hdr_len;
+  const char *seq; uint64_t len;
+  const char *qual; size_t qual_len;
+};
 
-// reads [first, first + n) of the batch; the result arrays are indexed from 0 (a share of the batch resolved on one GPU)
-static void emit_results(const Batch &b, const kuq_batch_result &res, size_t first = 0, size_t n = (size_t)-1) {
-  string out;
-  if (n == (size_t)-1) n = b.reads.size() - first;
-  out.reserve(n * 64);
-  char num[32];
-  for (size_t i = 0; i < n; i++) {
-    const Read &r = b.reads[first + i];
-    uint32_t call = res.call[i];
-    if (Print_unclassified && !call) print_sequence(Unclassified_out, r, b.bases);
-    if (Print_classified && call) print_sequence(Classified_out, r, b.bases);
-    if (!Print_kraken) continue;
-    if (!call && Only_classified_kraken_output) continue;           // :986-988
-    out += call ? "C\t" : "U\t";
-    out += r.id;
-    out += '\t';
-    snprintf(num, sizeof num, "%u", call); out += num;
-    out += '\t';
-    snprintf(num, sizeof num, "%" PRIu64, r.seq_len); out += num;
-    out += '\t';
-    if (Quick_mode) { snprintf(num, sizeof num, "Q:%u", res.run_count[i]); out += num; }   // :989-990
-    else if (res.run_count[i] == 0) out += "0:0";                    // :994-995
-    for (uint32_t j = 0; !Quick_mode && j < res.run_count[i]; j++) {   // hitlist_string, :826-861
-      const kuq_run &run = res.runs[res.run_start[i] + j];
-      if (j) out += ' ';
-      if (run.code == KUQ_CODE_AMBIG) snprintf(num, sizeof num, "A:%u", run.count);
-      else snprintf(num, sizeof num, "%u:%u", run.code, run.count);
-      out += num;
+// The Kraken lines (classify.cpp:980-1010, hitlist_string :826-861) and the -C / -U records (print_sequence, :794-805)
+// of reads [a, b); read i's results are at i - res0 of `res`.  The Kraken text goes into one buffer sized up front.
+template <class ViewOf>
+static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_result &res, size_t res0, bool fastq,
+                         string &kraken, string &classified, string &unclassified) {
+  const size_t at = kraken.size();
+  if (Print_kraken) {
+    size_t need = 0;
+    for (size_t i = a; i < b; i++) {
+      const ReadView v = view_of(i);
+      need += 2 + v.hdr_len + 1 + 10 + 1 + 20 + 1 + 4 + 22ull * res.run_count[i - res0] + 1 + (Print_sequence ? v.len + 1 : 0);
     }
-    if (Print_sequence) { out += '\t'; out.append(b.bases, r.seq_off, r.seq_len); }
-    out += '\n';
+    kraken.resize(at + need);
   }
-  if (Print_kraken) Kraken_out.write(out);
+  char *o = Print_kraken ? &kraken[at] : NULL;
+  auto put = [&](auto v) {
+    char buf[20];
+    int k = 0;
+    do { buf[k++] = (char)('0' + v % 10); v /= 10; } while (v);
+    while (k) *o++ = buf[--k];
+  };
+  for (size_t i = a; i < b; i++) {
+    const ReadView v = view_of(i);
+    const size_t r = i - res0;
+    const uint32_t call = res.call[r];
+    if ((Print_unclassified && !call) || (Print_classified && call)) {
+      string &oo = call ? classified : unclassified;
+      oo += fastq ? '@' : '>';
+      oo.append(v.hdr, v.hdr_len); oo += '\n';
+      oo.append(v.seq, v.len); oo += '\n';
+      if (fastq) { oo += "+\n"; oo.append(v.qual, v.qual_len); oo += '\n'; }
+    }
+    if (!Print_kraken) continue;
+    if (!call && Only_classified_kraken_output) continue;            // :986-988
+    *o++ = call ? 'C' : 'U'; *o++ = '\t';
+    {   // id = first whitespace-delimited token of the header line
+      size_t x = 0;
+      while (x < v.hdr_len && isspace((unsigned char)v.hdr[x])) x++;
+      size_t y = x;
+      while (y < v.hdr_len && !isspace((unsigned char)v.hdr[y])) y++;
+      memcpy(o, v.hdr + x, y - x); o += y - x;
+    }
+    *o++ = '\t';
+    put(call);
+    *o++ = '\t';
+    put(v.len);
+    *o++ = '\t';
+    if (Quick_mode) { *o++ = 'Q'; *o++ = ':'; put(res.run_count[r]); }   // :989-990
+    else if (res.run_count[r] == 0) { *o++ = '0'; *o++ = ':'; *o++ = '0'; }   // :994-995
+    for (uint32_t j = 0; !Quick_mode && j < res.run_count[r]; j++) {
+      const kuq_run &run = res.runs[res.run_start[r] + j];
+      if (j) *o++ = ' ';
+      if (run.code == KUQ_CODE_AMBIG) *o++ = 'A'; else put(run.code);
+      *o++ = ':';
+      put(run.count);
+    }
+    if (Print_sequence) { *o++ = '\t'; memcpy(o, v.seq, v.len); o += v.len; }
+    *o++ = '\n';
+  }
+  if (Print_kraken) kraken.resize(o - &kraken[0]);
 }
 
-static inline void append_u32(string &o, uint32_t v) {       // decimal without snprintf
-  char buf[10];
-  int n = 0;
-  do { buf[n++] = (char)('0' + v % 10); v /= 10; } while (v);
-  while (n) o += buf[--n];
+// The output of reads [a, b) of a batch, whose results start at read a (the whole batch, or a GPU's share of it)
+static void write_reads(const Batch &bt, const kuq_batch_result &res, size_t a, size_t b) {
+  string kraken, classified, unclassified;
+  auto view_of = [&](size_t i) {
+    const Read &r = bt.reads[i];
+    return ReadView{r.header_line.data(), r.header_line.size(), bt.bases.data() + r.seq_off, r.seq_len, r.quals.data(), r.quals.size()};
+  };
+  format_reads(view_of, a, b, res, a, bt.fastq, kraken, classified, unclassified);
+  Kraken_out.write(kraken);
+  Classified_out.write(classified);
+  Unclassified_out.write(unclassified);
+}
+
+// A batch's totals (report_stats, classify.cpp:361-375) and the progress line (:555-558)
+static void book_batch(uint64_t reads, uint64_t bases, uint64_t classified) {
+  total_classified += classified;
+  total_sequences += reads;
+  total_bases += bases;
+  fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
+}
+
+// The records per taxid of the databases `ctx` has staged, added to `into` (kuq_db_taxids: count, then fetch)
+static int db_taxids(kuq_ctx *ctx, map<uint32_t, uint64_t> &into) {
+  uint32_t m = 0;
+  int rc = kuq_db_taxids(ctx, NULL, NULL, 0, &m);
+  vector<uint32_t> t(m);
+  vector<uint64_t> c(m);
+  if (!rc && m) rc = kuq_db_taxids(ctx, t.data(), c.data(), m, &m);
+  for (uint32_t i = 0; !rc && i < m; i++) into[t[i]] += c[i];
+  return rc;
 }
 
 // background writer: formatted text is handed over batch by batch and written in order while the next batch is
@@ -1091,7 +1136,7 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
     return false;
   }
   const bool fastq_records = in[0].base[0] == '@';                   // determine_input_file_type; mate files: :66-75
-  const bool fastq = Fastq_input = fastq_records && !mate2;          // merged records are FASTA
+  const bool fastq = fastq_records && !mate2;                        // merged records are FASTA
   const int T = std::max(1, Num_threads);
   double T0__ = now_s();
   for (int k = 0; k < (mate2 ? 2 : 1); k++) in[k].parse(fastq_records, T);
@@ -1142,37 +1187,21 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
     cum[n_total] = chunk_nt[last_chunk];
   }
   auto chunk_of = [&](size_t i) { return (int)(std::upper_bound(first_of.begin(), first_of.end(), i) - first_of.begin()) - 1; };
-  // work units and batches (classify.cpp:506-521): batches end at unit boundaries
-  struct Cut { size_t begin, end; uint64_t bases; };
+  // work units and batches (kuq_batches.h): batches end at unit boundaries
+  struct Cut { size_t begin, end; };
   vector<Cut> batches;
   {
-    const uint64_t BATCH_NT = 96ull << 20;
-    // KUQ_BATCH_READS: close a batch at the first unit boundary after this many reads (tests: small batches)
-    const size_t batch_reads = getenv("KUQ_BATCH_READS") ? std::max<size_t>(1, strtoull(getenv("KUQ_BATCH_READS"), NULL, 10)) : (1u << 20) - 4096;
-    uint64_t unit_nt = 0, batch_nt = 0;
-    size_t begin = 0, unit_first = 0, batch_units = 0;
-    const uint64_t SLOT_NT = 280ull << 20;            // below the slot capacity (288 MiB)
+    BatchCutter cutter(batch_limits(96ull << 20, true, true));
+    size_t begin = 0;
     for (size_t i = 0; i < n_total; i++) {
       const uint64_t len = cum[i + 1] - cum[i];
       if (len > SLOT_NT) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
-      if (batch_nt + len > SLOT_NT && i > begin) {    // a very long sequence is coming: close the batch before it
-        batches.push_back({begin, i, batch_nt});
-        begin = i; batch_nt = 0; batch_units = 0;
-      }
-      unit_nt += len; batch_nt += len;
-      bool close_unit = unit_nt >= Work_unit_size;
-      if (close_unit) { unit_nt = 0; unit_first = i + 1; batch_units++; }
-      if ((close_unit && (batch_nt >= BATCH_NT || i + 1 - begin >= std::min<size_t>(batch_reads, (1u << 20) - 4096) ||
-                          batch_units >= Max_units_per_batch)) ||
-          (!close_unit && (i + 1 - begin >= (1u << 20) - 1 || batch_nt >= (150ull << 20)))) {
-        batches.push_back({begin, i + 1, batch_nt});
-        begin = i + 1; batch_nt = 0; batch_units = 0;
-        if (!close_unit) unit_first = i + 1;
-      }
+      const BatchCutter::Step st = cutter.next(len);
+      if (st.before) { batches.push_back({begin, i}); begin = i; }
+      if (st.after) { batches.push_back({begin, i + 1}); begin = i + 1; }
     }
-    size_t end = n_total;
-    if (unit_nt == 0 && unit_first < n_total) end = unit_first;    // last unit with zero length is dropped (:523-524)
-    if (end > begin) batches.push_back({begin, end, cum[end] - cum[begin]});
+    const size_t end = n_total - cutter.drop();
+    if (end > begin) batches.push_back({begin, end});
   }
   TICK("units+batches");
   // ---- pipeline: a filler thread gathers batch b + 2 into pinned memory and submits it while the GPUs classify batch
@@ -1191,7 +1220,7 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
   auto fill = [&](Stage &s, const Cut &b) {
     s.begin = b.begin; s.end = b.end;
     const size_t n = b.end - b.begin;
-    prepare_stage(s, b.bases, n);
+    prepare_stage(s, cum[b.end] - cum[b.begin], n);
     const uint64_t c0 = cum[b.begin];
 #pragma omp parallel for schedule(static) num_threads(Tf)
     for (size_t i = 0; i < n; i++) {
@@ -1211,76 +1240,19 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
   };
   Writer writer;
   writer.start();
-  // upper bound of the Kraken line of read i (so that a part formats into one exactly sized buffer, no growth checks)
   auto emit = [&](Stage &s, const kuq_batch_result &res) {
     const size_t n = s.end - s.begin;
     const int parts = Te;
     OutJob job = writer.take(parts);
-    vector<string> &kr = job.kraken, &cl = job.classified, &un = job.unclassified;
+    auto view_of = [&](size_t i) {
+      const View &v = *rv[s.begin + i];
+      return ReadView{v.hdr, v.hdr_len, s.bases + s.offs[i], v.seq_len, v.qual, v.qual_len};
+    };
 #pragma omp parallel for schedule(static, 1) num_threads(Te)
-    for (int pi = 0; pi < parts; pi++) {
-      const size_t a = n * pi / parts, b = n * (pi + 1) / parts;
-      string &out = kr[pi];
-      if (Print_kraken) {
-        size_t need = 0;
-        for (size_t i = a; i < b; i++) {
-          const View &v = *rv[s.begin + i];
-          need += 2 + v.hdr_len + 1 + 10 + 1 + 10 + 1 + 4 + 22ull * res.run_count[i] + 1 + (Print_sequence ? v.seq_len + 1 : 0);
-        }
-        out.resize(need);
-      }
-      char *o = Print_kraken ? &out[0] : NULL;
-      auto put_u32 = [&](uint32_t v) {
-        char buf[10];
-        int k = 0;
-        do { buf[k++] = (char)('0' + v % 10); v /= 10; } while (v);
-        while (k) *o++ = buf[--k];
-      };
-      for (size_t i = a; i < b; i++) {
-        const View &v = *rv[s.begin + i];
-        const uint32_t call = res.call[i];
-        const char *seq = s.bases + s.offs[i];
-        if ((Print_unclassified && !call) || (Print_classified && call)) {       // print_sequence, :794-805
-          string &oo = call ? cl[pi] : un[pi];
-          oo += fastq ? '@' : '>';
-          oo.append(v.hdr, v.hdr_len); oo += '\n';
-          oo.append(seq, v.seq_len); oo += '\n';
-          if (fastq) { oo += "+\n"; oo.append(v.qual, v.qual_len); oo += '\n'; }
-        }
-        if (!Print_kraken) continue;
-        if (!call && Only_classified_kraken_output) continue;
-        *o++ = call ? 'C' : 'U'; *o++ = '\t';
-        {   // id = first whitespace-delimited token of the header line
-          uint32_t x = 0;
-          while (x < v.hdr_len && isspace((unsigned char)v.hdr[x])) x++;
-          uint32_t y = x;
-          while (y < v.hdr_len && !isspace((unsigned char)v.hdr[y])) y++;
-          memcpy(o, v.hdr + x, y - x); o += y - x;
-        }
-        *o++ = '\t';
-        put_u32(call);
-        *o++ = '\t';
-        put_u32(v.seq_len);
-        *o++ = '\t';
-        if (Quick_mode) { *o++ = 'Q'; *o++ = ':'; put_u32(res.run_count[i]); }
-        else if (res.run_count[i] == 0) { *o++ = '0'; *o++ = ':'; *o++ = '0'; }
-        for (uint32_t j = 0; !Quick_mode && j < res.run_count[i]; j++) {
-          const kuq_run &run = res.runs[res.run_start[i] + j];
-          if (j) *o++ = ' ';
-          if (run.code == KUQ_CODE_AMBIG) *o++ = 'A'; else put_u32(run.code);
-          *o++ = ':';
-          put_u32(run.count);
-        }
-        if (Print_sequence) { *o++ = '\t'; memcpy(o, seq, v.seq_len); o += v.seq_len; }
-        *o++ = '\n';
-      }
-      if (Print_kraken) out.resize(o - &out[0]);
-    }
+    for (int pi = 0; pi < parts; pi++)
+      format_reads(view_of, n * pi / parts, n * (pi + 1) / parts, res, 0, fastq, job.kraken[pi], job.classified[pi], job.unclassified[pi]);
     writer.push(std::move(job));
-    total_classified += res.n_classified;
-    total_sequences += n;
-    total_bases += s.offs[n];
-    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
+    book_batch(n, s.offs[n], res.n_classified);
   };
   // batch bi: device bi % G, slot (bi / G) % NS, staging set bi % (NS * G)
   std::mutex pm;
@@ -1344,90 +1316,95 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
   return true;
 }
 
-static void process_file(kuq_ctx *ctx, const char *filename, const char *mate2) {
-  if (!getenv("KUQ_SERIAL_INGEST") && process_file_parallel(ctx, filename, mate2)) return;   // plain files: parallel path
+// The inputs of the command line: a FASTA / FASTQ file, or with --paired a pair of mate files
+static vector<pair<const char *, const char *>> inputs(int argc, char **argv) {
+  vector<pair<const char *, const char *>> in;
+  for (int i = optind; i < argc; i += Paired ? 2 : 1) in.emplace_back(argv[i], Paired ? argv[i + 1] : NULL);
+  return in;
+}
+
+// The batches of the inputs, file after file, read one at a time and cut by kuq_batches.h.  A read that closes a batch
+// before itself is held over and starts the next batch.
+struct BatchReader {
+  vector<pair<const char *, const char *>> files;
+  size_t fi = 0;
+  bool open = false, held = false;
   InputReader reader;
-  reader.open(filename, mate2);
-  Fastq_input = reader.fastq();
-  const uint64_t BATCH_NT = 96ull << 20;
-  Batch batches[2];
-  int cur = 0, inflight = -1;
-  uint64_t unit_nt = 0;
-  size_t unit_first_read = 0;       // first read of the open work unit inside the current batch
-  size_t batch_units = 0;           // units closed in the current batch
-  auto wait_emit = [&](int which) {
-    kuq_batch_result res;
-    if (kuq_wait_batch(ctx, (uint32_t)which, &res)) die(EX_SOFTWARE, kuq_last_error(ctx));
-    emit_results(batches[which], res);
-    total_classified += res.n_classified;
-    total_sequences += batches[which].reads.size();
-    total_bases += batches[which].bases.size();
-    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences,
-            total_classified * 100.0 / total_sequences);
-    batches[which].clear();
-  };
-  auto submit = [&](int which) {
-    Batch &b = batches[which];
-    if (b.reads.empty()) return;
-    if (kuq_submit_batch(ctx, (uint32_t)which, b.bases.data(), b.offs.data(), (uint32_t)b.reads.size(), NULL, 0))
-      die(EX_SOFTWARE, kuq_last_error(ctx));
-    if (inflight >= 0) wait_emit(inflight);
-    inflight = which;
-    batch_units = 0;
-  };
+  BatchCutter cutter;
   Read r;
-  while (reader.valid()) {
-    Batch &b = batches[cur];
-    if (!reader.next(r, b.bases)) break;
-    if (r.seq_len > (280ull << 20)) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
-    if (b.bases.size() > (280ull << 20) && !b.reads.empty()) {
-      // the sequence just read does not fit next to the batch: move it to the next batch
-      Batch &nb = batches[cur ^ 1];
-      string seq = b.bases.substr(r.seq_off);
-      b.bases.resize(r.seq_off);
-      submit(cur);
-      cur ^= 1;
-      unit_first_read = 0;
-      Batch &b2 = batches[cur];
-      (void)nb;
-      r.seq_off = b2.bases.size();
-      b2.bases += seq;
-      b2.reads.push_back(r);
-      b2.offs.push_back(b2.bases.size());
-      unit_nt += r.seq_len;
-      if (unit_nt >= Work_unit_size) { unit_nt = 0; unit_first_read = b2.reads.size(); batch_units++; }
-      continue;
-    }
+  BatchCutter::Step step;
+  string held_bases;
+  BatchReader(const vector<pair<const char *, const char *>> &f, const BatchLimits &lim) : files(f), cutter(lim) {}
+  void push(Batch &b) {
     b.reads.push_back(r);
     b.offs.push_back(b.bases.size());
-    unit_nt += r.seq_len;
-    if (unit_nt >= Work_unit_size) {                                 // the unit closes (classify.cpp:514-520)
-      unit_nt = 0;
-      unit_first_read = b.reads.size();
-      if (b.bases.size() >= BATCH_NT || b.reads.size() >= (1u << 20) - 4096 || ++batch_units >= Max_units_per_batch) {
-        submit(cur);
-        cur ^= 1;
-        unit_first_read = 0;
+    b.units.push_back(step.unit);
+  }
+  bool next(Batch &b) {
+    b.clear();
+    if (held) {
+      held = false;
+      b.fastq = reader.fastq();
+      r.seq_off = 0;
+      b.bases += held_bases;
+      push(b);
+      if (step.after) return true;
+    }
+    for (; fi < files.size(); fi++) {
+      if (!open) {
+        reader = InputReader();
+        reader.open(files[fi].first, files[fi].second);
+        open = true;
       }
-    } else if (b.reads.size() >= (1u << 20) - 1 || b.bases.size() >= (150ull << 20)) {
-      // a single work unit larger than a slot (huge -u): cut here; the unit is then counted as two (DESIGN §4)
-      submit(cur);
-      cur ^= 1;
-      unit_first_read = 0;
+      b.fastq = reader.fastq();
+      while (reader.valid() && reader.next(r, b.bases)) {
+        if (cutter.lim.slot_nt && r.seq_len > cutter.lim.slot_nt) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
+        step = cutter.next(r.seq_len);
+        if (step.before) {
+          held_bases.assign(b.bases, r.seq_off, r.seq_len);
+          b.bases.resize(r.seq_off);
+          held = true;
+          return true;
+        }
+        push(b);
+        if (step.after) return true;
+      }
+      const size_t keep = b.reads.size() - cutter.drop();     // the end of the file
+      b.bases.resize(b.offs[keep]);
+      b.reads.resize(keep);
+      b.offs.resize(keep + 1);
+      b.units.resize(keep);
+      cutter.next_file();
+      reader.close();
+      open = false;
+      if (keep) { fi++; return true; }
     }
+    return false;
   }
-  // end of file: a last work unit whose total length is 0 is dropped by the reference (classify.cpp:523-524)
-  {
-    Batch &b = batches[cur];
-    if (unit_nt == 0 && unit_first_read < b.reads.size()) {
-      b.reads.resize(unit_first_read);
-      b.offs.resize(unit_first_read + 1);
-    }
-    submit(cur);
+};
+
+static void process_file(kuq_ctx *ctx, const char *filename, const char *mate2) {
+  if (!getenv("KUQ_SERIAL_INGEST") && process_file_parallel(ctx, filename, mate2)) return;   // plain files: parallel path
+  BatchReader br({{filename, mate2}}, batch_limits(96ull << 20, true, true));
+  Batch batches[2];
+  int inflight = -1;
+  auto wait_write = [&](int which) {
+    const Batch &b = batches[which];
+    kuq_batch_result res;
+    if (kuq_wait_batch(ctx, (uint32_t)which, &res)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    write_reads(b, res, 0, b.reads.size());
+    book_batch(b.reads.size(), b.bases.size(), res.n_classified);
+  };
+  // batch `cur` is read while the other one is classified
+  for (int cur = 0; br.next(batches[cur]); cur ^= 1) {
+    const Batch &b = batches[cur];
+    if (kuq_submit_batch(ctx, (uint32_t)cur, b.bases.data(), b.offs.data(), (uint32_t)b.reads.size(), NULL, 0))
+      die(EX_SOFTWARE, kuq_last_error(ctx));
+    if (inflight >= 0) wait_write(inflight);
+    inflight = cur;
   }
-  if (inflight >= 0) wait_emit(inflight);
+  if (inflight >= 0) wait_write(inflight);
   if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));     // work units do not span input files
-  reader.close();
 }
 
 // ---- chunked mode: `-x size` with a database that does not fit (process_file_with_db_chunk, classify.cpp:566-791) --
@@ -1436,59 +1413,6 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
   vector<pair<uint64_t, uint64_t>> ranges;
   if (!plan_ranges(offsets, n_bins, budget, 12, ranges)) die(EX_SOFTWARE, "a single minimizer bin exceeds the chunk budget; raise -x");
   return ranges;
-}
-
-// The batches of one input file, read one at a time.  unit_aligned: batches end where a work unit of process_file ends
-// (classify.cpp:506-521) and a last unit of total length 0 is dropped like there (:523-524) — what the per-work-unit
-// sketch rule of the preloaded path needs.  The -x path of the reference reads sequence by sequence without work units
-// (:566-791): unit_aligned = false.  A batch closes (at a unit boundary when aligned) once it holds max_nt bases.
-struct BatchReader {
-  InputReader reader;
-  bool fq = false, unit_aligned = false, done = false;
-  uint64_t max_nt = 96ull << 20;
-  uint64_t unit_nt = 0;
-  BatchReader(const char *filename, const char *mate2, bool aligned) : unit_aligned(aligned) {
-    reader.open(filename, mate2);
-    fq = reader.fastq();
-  }
-  bool next(Batch &b) {
-    b.clear();
-    b.fastq = fq;
-    if (done) return false;
-    Read r;
-    size_t unit_first_read = 0;        // first read of the open work unit inside this batch
-    size_t batch_units = 0;
-    while (reader.valid()) {
-      if (!reader.next(r, b.bases)) break;
-      b.reads.push_back(r);
-      b.offs.push_back(b.bases.size());
-      bool cut;
-      if (!unit_aligned) {
-        cut = b.bases.size() >= max_nt || b.reads.size() >= (1u << 20) - 1;
-      } else {
-        unit_nt += r.seq_len;
-        const bool close_unit = unit_nt >= Work_unit_size;
-        if (close_unit) { unit_nt = 0; unit_first_read = b.reads.size(); batch_units++; }
-        cut = close_unit ? (b.bases.size() >= max_nt || b.reads.size() >= (1u << 20) - 4096 || batch_units >= Max_units_per_batch)
-                         : (b.reads.size() >= (1u << 20) - 1 || b.bases.size() >= (150ull << 20));   // one huge unit: counted as two
-      }
-      if (cut) return true;
-    }
-    if (unit_aligned && unit_nt == 0 && unit_first_read < b.reads.size()) {
-      b.bases.resize(b.offs[unit_first_read]);
-      b.reads.resize(unit_first_read);
-      b.offs.resize(unit_first_read + 1);
-    }
-    done = true;
-    reader.close();
-    return !b.reads.empty();
-  }
-};
-
-static void load_file_batches(const char *filename, const char *mate2, vector<Batch> &out, bool unit_aligned) {
-  BatchReader br(filename, mate2, unit_aligned);
-  Batch b;
-  while (br.next(b)) out.push_back(std::move(b));
 }
 
 // ---- databases that do not fit the HBM budget: streamed through two range buffers ----------------------------------
@@ -1513,7 +1437,6 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     vector<pair<uint64_t, uint64_t>> ranges;
   };
   vector<Plan> plans(n_db);
-  set<uint32_t> all;
   uint64_t max_rec = 1, max_bins = 1;
   for (size_t d = 0; d < n_db; d++) {
     Plan &pl = plans[d];
@@ -1531,17 +1454,14 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     for (auto &rg : pl.ranges) {
       max_rec = std::max<uint64_t>(max_rec, pl.offsets[rg.second] - pl.offsets[rg.first]);
       max_bins = std::max<uint64_t>(max_bins, rg.second - rg.first);
-      if (kuq_stage_db(ctx, kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, rg.first, rg.second)) die(EX_DATAERR, kuq_last_error(ctx));
-      uint32_t m = 0;
-      kuq_db_taxids(ctx, NULL, NULL, 0, &m);
-      vector<uint32_t> tt(m);
-      vector<uint64_t> cc(m);
-      if (m) kuq_db_taxids(ctx, tt.data(), cc.data(), m, &m);
-      for (uint32_t i = 0; i < m; i++) { db_counts[d][tt[i]] += cc[i]; all.insert(tt[i]); }
+      if (kuq_stage_db(ctx, kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, rg.first, rg.second) || db_taxids(ctx, db_counts[d]))
+        die(EX_DATAERR, kuq_last_error(ctx));
     }
   }
   if (n_db == 1) cerr << "Database split into " << plans[0].ranges.size() << " chunks" << endl;
   {
+    set<uint32_t> all;
+    for (auto &c : db_counts) for (auto &kv : c) all.insert(kv.first);
     vector<uint32_t> u(all.begin(), all.end());
     if (kuq_set_db_taxid_universe(ctx, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
   }
@@ -1579,25 +1499,7 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
   }
   if (Timing) fprintf(stderr, "[timing] streamed: %zu database(s), %llu MiB per round\n", n_db, (unsigned long long)(round_bytes >> 20));
 
-  // the input, batch by batch across the files
-  int fi = optind;
-  std::unique_ptr<BatchReader> br;
-  auto pull = [&](Batch &b) -> bool {
-    for (;;) {
-      if (!br) {
-        if (fi >= argc) return false;
-        br.reset(new BatchReader(argv[fi], mate_of(argv, fi), unit_rule));
-        br->max_nt = batch_nt;
-      }
-      if (br->next(b)) { b.file = fi; return true; }
-      br.reset();
-      fi += input_step();
-    }
-  };
-  // work-unit ids of the per-work-unit rule: process_file's cutting (classify.cpp:506-521), units end with their file
-  uint32_t unit_next = 0;
-  uint64_t unit_nt = 0;
-  int unit_file = -1;
+  BatchReader input(inputs(argc, argv), batch_limits(batch_nt, unit_rule, false));
   struct DevBatch { void *bases, *offs, *codes, *units; };
   vector<Batch> round;
   Batch pending;
@@ -1608,7 +1510,7 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     round.clear();
     uint64_t bytes = 0;
     for (;;) {
-      if (!have_pending) have_pending = pull(pending);
+      if (!have_pending) have_pending = input.next(pending);
       if (!have_pending) break;
       const uint64_t need = (pending.bases.size() + 64) * 5 + (pending.reads.size() + 4) * (unit_rule ? 12 : 8) + 1024;
       if (!round.empty() && bytes + need > round_bytes) break;
@@ -1634,17 +1536,7 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
           kuq_copy_to_device(ctx, 0, d.offs, offs.data(), offs.size() * 8) ||
           kuq_device_memset(ctx, 0, d.codes, 0, (b.bases.size() + 64) * 4))
         die(EX_SOFTWARE, kuq_last_error(ctx));
-      if (unit_rule) {
-        if (unit_file >= 0 && b.file != unit_file) { unit_next++; unit_nt = 0; }
-        unit_file = b.file;
-        vector<uint32_t> units(b.reads.size());
-        for (size_t i = 0; i < b.reads.size(); i++) {
-          units[i] = unit_next;
-          unit_nt += b.reads[i].seq_len;
-          if (unit_nt >= Work_unit_size) { unit_next++; unit_nt = 0; }
-        }
-        if (kuq_copy_to_device(ctx, 0, d.units, units.data(), units.size() * 4)) die(EX_SOFTWARE, kuq_last_error(ctx));
-      }
+      if (unit_rule && kuq_copy_to_device(ctx, 0, d.units, b.units.data(), b.units.size() * 4)) die(EX_SOFTWARE, kuq_last_error(ctx));
       if (kuq_sync_slot(ctx, 0)) die(EX_SOFTWARE, kuq_last_error(ctx));
     }
     for (size_t db = 0; db < n_db; db++) {
@@ -1687,12 +1579,8 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
                              b.bases.size(), (const uint32_t *)dev[bi].codes, (const uint32_t *)dev[bi].units, 0) ||
           kuq_collect_device_batch(ctx, 0, &res))
         die(EX_SOFTWARE, kuq_last_error(ctx));
-      Fastq_input = b.fastq;
-      emit_results(b, res);
-      total_classified += res.n_classified;
-      total_sequences += b.reads.size();
-      total_bases += b.bases.size();
-      fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
+      write_reads(b, res, 0, b.reads.size());
+      book_batch(b.reads.size(), b.bases.size(), res.n_classified);
     }
     for (auto &d : dev) {
       kuq_device_free(ctx, d.bases); kuq_device_free(ctx, d.offs); kuq_device_free(ctx, d.codes);
@@ -1727,10 +1615,9 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
   const int G = (int)ctxs.size();
   const uint64_t R = n_phases;
   vector<Batch> batches;
-  for (int i = optind; i < argc; i += input_step()) {
-    const size_t from = batches.size();
-    load_file_batches(argv[i], mate_of(argv, i), batches, /*unit_aligned=*/true);
-    for (size_t j = from; j < batches.size(); j++) batches[j].file = i;
+  {
+    BatchReader input(inputs(argc, argv), batch_limits(96ull << 20, true, false));
+    for (Batch b; input.next(b);) batches.push_back(std::move(b));
   }
   uint64_t max_bases = 64, max_reads = 4;
   for (auto &b : batches) { max_bases = std::max<uint64_t>(max_bases, b.bases.size()); max_reads = std::max<uint64_t>(max_reads, b.reads.size()); }
@@ -1757,25 +1644,11 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
   }
   vector<uint32_t *> peer_ids(G);
   vector<uint64_t *> peer_done(G), peer_ready(G);
-  // work-unit ids of the per-work-unit rule: process_file's cutting (classify.cpp:506-521), units end with their file
-  uint32_t unit_next = 0;
-  uint64_t unit_nt = 0;
-  int unit_file = -1;
-  vector<uint32_t> units;
   uint64_t step = 0;
   for (auto &b : batches) {
     const size_t n = b.reads.size();
     const int par = (int)(step & 1);
-    if (multi) {
-      if (unit_file >= 0 && b.file != unit_file) { unit_next++; unit_nt = 0; }
-      unit_file = b.file;
-      units.resize(n);
-      for (size_t i = 0; i < n; i++) {
-        units[i] = unit_next;
-        unit_nt += b.reads[i].seq_len;
-        if (unit_nt >= Work_unit_size) { unit_next++; unit_nt = 0; }
-      }
-    }
+    const vector<uint32_t> &units = b.units;
     // shares: contiguous; with work-unit ids a share starts where a unit starts (k_unit_decide sees every read of a unit
     // on one GPU), else anywhere (the chunked rule does not depend on units)
     vector<size_t> first(G + 1, 0);
@@ -1831,18 +1704,16 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
         die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
     }
     // results of the shares, in read order
-    Fastq_input = b.fastq;
+    uint64_t classified = 0;
     for (int g = 0; g < G; g++) {
       const size_t share = first[g + 1] - first[g];
       if (!share) { if (kuq_sync_slot(ctxs[g], 0)) die(EX_SOFTWARE, kuq_last_error(ctxs[g])); continue; }
       kuq_batch_result res;
       if (kuq_collect_device_batch(ctxs[g], 0, &res)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-      emit_results(b, res, first[g], share);
-      total_classified += res.n_classified;
+      write_reads(b, res, first[g], first[g + 1]);
+      classified += res.n_classified;
     }
-    total_sequences += n;
-    total_bases += b.bases.size();
-    fprintf(stderr, "\r Processed %llu sequences (%.2f%% classified)", total_sequences, total_classified * 100.0 / total_sequences);
+    book_batch(n, b.bases.size(), classified);
     step++;
   }
   for (int g = 0; g < G; g++) {
@@ -1873,12 +1744,7 @@ static void run_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const 
   }
   for (int g = 0; g < G; g++) {
     if (cut[g + 1] <= cut[g]) die(EX_DATAERR, "more GPUs than non-empty minimizer ranges: use fewer devices (KUQ_DEVICES)");
-    uint32_t m = 0;
-    kuq_db_taxids(ctxs[g], NULL, NULL, 0, &m);
-    vector<uint32_t> tt(m);
-    vector<uint64_t> cc(m);
-    if (m) kuq_db_taxids(ctxs[g], tt.data(), cc.data(), m, &m);
-    for (uint32_t i = 0; i < m; i++) db_counts[tt[i]] += cc[i];
+    if (db_taxids(ctxs[g], db_counts)) die(EX_DATAERR, kuq_last_error(ctxs[g]));
   }
   vector<uint32_t> all;
   for (auto &kv : db_counts) all.push_back(kv.first);
@@ -1909,12 +1775,7 @@ static void run_sharded_multi(const vector<kuq_ctx *> &ctxs, const vector<Mapped
         uint64_t lo = run.cut[g], hi = run.cut[g + 1];
         if (lo == hi) lo = hi = 1ull << (2 * sd[d].nt);             // an empty slice
         rcs[g] = kuq_stage_db_append_range(ctxs[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, lo, hi);
-        uint32_t m = 0;
-        if (!rcs[g]) rcs[g] = kuq_db_taxids(ctxs[g], NULL, NULL, 0, &m);
-        vector<uint32_t> tt(m);
-        vector<uint64_t> cc(m);
-        if (!rcs[g] && m) rcs[g] = kuq_db_taxids(ctxs[g], tt.data(), cc.data(), m, &m);
-        for (uint32_t i = 0; i < m; i++) after[g][d][tt[i]] = cc[i];
+        if (!rcs[g]) rcs[g] = db_taxids(ctxs[g], after[g][d]);
       }
   for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
   set<uint32_t> all;
@@ -2065,14 +1926,7 @@ int main(int argc, char **argv) {
       for (size_t d = 0; d < n_db && !rcs[g]; d++) {
         rcs[g] = d ? kuq_stage_db_append(All_ctx[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size)
                    : kuq_stage_db(All_ctx[g], kdb.p, kdb.size, idx.p, idx.size, 0, 0);
-        if (g == 0 && !rcs[g] && n_db > 1) {
-          uint32_t m = 0;
-          kuq_db_taxids(All_ctx[g], NULL, NULL, 0, &m);
-          vector<uint32_t> tt(m);
-          vector<uint64_t> cc(m);
-          if (m) kuq_db_taxids(All_ctx[g], tt.data(), cc.data(), m, &m);
-          for (uint32_t i = 0; i < m; i++) union_after[d][tt[i]] = cc[i];
-        }
+        if (g == 0 && !rcs[g] && n_db > 1) rcs[g] = db_taxids(All_ctx[g], union_after[d]);
       }
     }
     for (size_t g = 0; g < All_ctx.size(); g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(All_ctx[g]));
@@ -2115,7 +1969,7 @@ int main(int argc, char **argv) {
   if (want_shards && n_db == 1) run_sharded(All_ctx, kdb, idx, argc, argv, db_counts[0]);
   else if (want_shards) run_sharded_multi(All_ctx, kdbs, idxs, argc, argv, db_counts);
   else if (chunk_budget) run_streamed(ctx, kdbs, idxs, chunk_budget, hbm_budget, argc, argv, db_counts);
-  else for (int i = optind; i < argc; i += input_step()) process_file(ctx, argv[i], mate_of(argv, i));
+  else for (auto &in : inputs(argc, argv)) process_file(ctx, in.first, in.second);
   // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
   {
     double T0__ = now_s();
@@ -2173,16 +2027,8 @@ int main(int argc, char **argv) {
     if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
       cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
       ofstream ofs(fname);
-      if (n_db > 1 || chunk_budget || want_shards) {
-        for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
-      } else {
-        uint32_t m = 0;
-        kuq_db_taxids(ctx, NULL, NULL, 0, &m);
-        vector<uint32_t> tt(m);
-        vector<uint64_t> cc(m);
-        if (m) kuq_db_taxids(ctx, tt.data(), cc.data(), m, &m);
-        for (uint32_t i = 0; i < m; i++) ofs << tt[i] << '\t' << cc[i] << '\n';
-      }
+      if (n_db == 1 && !chunk_budget && !want_shards && db_taxids(ctx, db_counts[0])) die(EX_SOFTWARE, kuq_last_error(ctx));
+      for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
     }
     {
       cerr << "Reading genome sizes from " << fname << " ...";

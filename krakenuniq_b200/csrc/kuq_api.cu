@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_batches.h"
 #include "kuq_bounce.cuh"
 #include "kuq_kernels.cuh"
 
@@ -192,9 +193,7 @@ struct kuq_ctx {
   unsigned long long *d_harvest_stat = nullptr;
   cudaEvent_t harvest_ev[2] = {nullptr, nullptr};
   bool lca_mode = false;                  // kuq_set_lcas_batch ran: record values are LCA results, not classifiable
-  // work-unit cutting across batches (classify.cpp:506-521)
-  uint64_t unit_nt = 0;
-  uint32_t unit_next = 0;
+  WorkUnits units;                        // the open work unit across batches (kuq_batches.h)
 };
 
 namespace {
@@ -1169,13 +1168,11 @@ int prepare_unit_map(kuq_ctx *ctx, Slot &s) {
   return KUQ_OK;
 }
 
-// process_file's unit cutting (classify.cpp:506-521): reads join the open unit until its length reaches -u.
+// process_file's unit cutting (kuq_batches.h): reads join the open unit until its length reaches -u.
 void cut_units(kuq_ctx *ctx, const uint64_t *offsets, uint32_t n, uint32_t *unit) {
-  const uint64_t wus = ctx->cfg.work_unit_size;
   for (uint32_t i = 0; i < n; i++) {
-    unit[i] = ctx->unit_next;
-    ctx->unit_nt += offsets[i + 1] - offsets[i];
-    if (ctx->unit_nt >= wus) { ctx->unit_next++; ctx->unit_nt = 0; }
+    unit[i] = ctx->units.id;
+    ctx->units.add(offsets[i + 1] - offsets[i], ctx->cfg.work_unit_size);
   }
 }
 
@@ -2211,8 +2208,7 @@ int kuq_finish(kuq_ctx *ctx) {
   if (!ctx) return KUQ_E_INVALID_ARG;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  ctx->unit_nt = 0;
-  ctx->unit_next++;
+  ctx->units.new_file();
   return harvest_seen(ctx, false);
 }
 
@@ -3628,8 +3624,7 @@ int kuq_reset_counts(kuq_ctx *ctx) {
     ctx->exact_partitioned = false;
     ctx->merged_exact = false;
   }
-  ctx->unit_nt = 0;
-  ctx->unit_next = 0;
+  ctx->units = WorkUnits();
   return KUQ_OK;
 }
 
