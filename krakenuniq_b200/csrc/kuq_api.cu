@@ -14,6 +14,7 @@
 #include <cstring>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -70,6 +71,19 @@ struct Slot {
 };
 
 }  // namespace
+
+// One open-addressing table in HBM: the sparse-tier set (8-byte keys (taxon + 1) << 32 | code) or the exact k-mer set
+// (16-byte ExactPairs).  A context has at most one of them.
+template <typename Item, typename Count>
+struct DevTable {
+  Item *slots = nullptr;
+  Count *count = nullptr;                 // [n_sketch] items per taxon
+  uint64_t cap = 0;                       // slots, a power of two
+  uint64_t upper = 0;                     // upper bound of the items since the last exact count (reserve_room)
+  uint64_t grown = 0;                     // times the slots were re-allocated
+};
+using SparseTable = DevTable<unsigned long long, uint32_t>;
+using ExactTable = DevTable<ExactPair, unsigned long long>;
 
 struct CountsHost {
   std::vector<unsigned long long> n_kmers, n_reads;
@@ -138,14 +152,9 @@ struct kuq_ctx {
   // per-taxon state
   uint8_t *d_regs = nullptr, *d_dense_flag = nullptr;
   unsigned long long *d_n_kmers = nullptr, *d_n_reads = nullptr;
-  unsigned long long *d_sparse_slots = nullptr, *d_sparse_used = nullptr;
-  uint32_t *d_sparse_distinct = nullptr;
-  uint64_t sparse_cap = 0;
-  ExactPair *d_exact = nullptr;           // KUQ_HLL_EXACT: the (taxon, k-mer) table and the per-taxon set sizes
-  unsigned long long *d_exact_count = nullptr;
-  uint64_t exact_cap = 0;
-  uint64_t exact_upper = 0;               // upper bound of the pairs in that table (reserve_exact_inserts)
-  uint64_t exact_grown = 0;               // times it was re-allocated
+  unsigned long long *d_sparse_used = nullptr;
+  SparseTable sparse;                     // the sparse-tier set; count[] includes the keys of kept records
+  ExactTable exact;                       // KUQ_HLL_EXACT: the (taxon, k-mer) table and the per-taxon set sizes
   bool exact_partitioned = false;         // kuq_exact_replace / kuq_exact_partition: the table holds one owner's part
   bool merged_exact = false;              // kuq_set_exact_summary: merged_exact_count / merged_books hold sums over parts
   std::vector<unsigned long long> merged_exact_count;
@@ -174,7 +183,6 @@ struct kuq_ctx {
   uint32_t *d_sync_err = nullptr;         // set by a kuq_wait_flags that timed out
   bool merged_summary = false;            // kuq_set_sparse_summary: snap.sparse_hist / distinct hold cross-GPU sums
   std::vector<uint32_t> merged_hist, merged_distinct;
-  uint64_t direct_upper = 0;              // upper bound of the keys in the sparse-tier set (reserve_direct_inserts)
   bool seen_dirty = false;                // counted hits flagged records since the last harvest (SEEN_BIT)
   // record tier of the sparse HLL tier (KEPT_BIT): a resident range keeps its hits' keys in the records themselves
   uint2 *d_secondaries = nullptr;         // (secondary, primary) record pairs of the (taxon, code) groups of the range
@@ -182,10 +190,9 @@ struct kuq_ctx {
   int collisions = 0;                     // that table: 0 = not built yet, 1 = built, -1 = none (harvests fill the set)
   double collisions_ms = 0;               // time the table took to build
   bool kept = false;                      // some staged records carry KEPT_BIT
-  uint64_t kept_keys = 0;                 // keys held by kept records (included in d_sparse_distinct)
+  uint64_t kept_keys = 0;                 // keys held by kept records (included in sparse.count)
   bool set_has_hits = false;              // the set holds keys of hits, which kept records could duplicate
   bool keep_dirty = false;                // fused calls kept records at their first sighting (F_KEEP) since settle_kept
-  uint64_t sparse_grown = 0;              // times the sparse-tier set was re-allocated at a harvest
   double harvest_ms = 0;                  // device time of the last harvest
   // the harvest's counters and timing events, made at the first harvest (or keep-mode call) and kept: a cudaMalloc /
   // cudaFree pair per harvest held the device idle at the end of every run.  [0], [1]: the harvest's; [2]: records that
@@ -200,6 +207,7 @@ namespace {
 
 void stream_close(kuq_ctx *ctx);
 int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set = false);
+int settle_kept(kuq_ctx *ctx);
 
 // Records of a database with k <= 28 are shorter than the 12 bytes they take in HBM; they pass through a device landing
 // zone of this many records on their way there.  64 MiB unless KUQ_LANDING_BYTES says otherwise (a small zone cuts a
@@ -269,13 +277,13 @@ void free_db(kuq_ctx *ctx) {
 void free_tax_state(kuq_ctx *ctx) {
   cudaFree(ctx->d_parent); cudaFree(ctx->d_raw); cudaFree(ctx->d_depth);
   cudaFree(ctx->d_regs); cudaFree(ctx->d_dense_flag); cudaFree(ctx->d_n_kmers); cudaFree(ctx->d_n_reads);
-  cudaFree(ctx->d_sparse_slots); cudaFree(ctx->d_sparse_used); cudaFree(ctx->d_sparse_distinct);
-  cudaFree(ctx->d_exact); cudaFree(ctx->d_exact_count); cudaFree(ctx->d_exact_pre);
-  ctx->d_exact = nullptr; ctx->d_exact_count = nullptr; ctx->d_exact_pre = nullptr;
+  cudaFree(ctx->sparse.slots); cudaFree(ctx->d_sparse_used); cudaFree(ctx->sparse.count);
+  cudaFree(ctx->exact.slots); cudaFree(ctx->exact.count); cudaFree(ctx->d_exact_pre);
+  ctx->exact.slots = nullptr; ctx->exact.count = nullptr; ctx->d_exact_pre = nullptr;
   ctx->exact_pre.clear();
   ctx->d_parent = ctx->d_raw = nullptr; ctx->d_depth = nullptr; ctx->d_regs = ctx->d_dense_flag = nullptr;
-  ctx->d_n_kmers = ctx->d_n_reads = nullptr; ctx->d_sparse_slots = ctx->d_sparse_used = nullptr;
-  ctx->d_sparse_distinct = nullptr;
+  ctx->d_n_kmers = ctx->d_n_reads = nullptr; ctx->sparse.slots = ctx->d_sparse_used = nullptr;
+  ctx->sparse.count = nullptr;
   ctx->finalized = false;
 }
 
@@ -415,6 +423,431 @@ int collect_taxids(kuq_ctx *ctx) {
                         ctx->db_taxids, ctx->db_taxid_counts);
 }
 
+// ---- the two device tables: the sparse-tier set and the exact k-mer set ---------------------------------------------
+// What differs between them is supplied by the overloads below: the device view (whose counter the kernels add to),
+// the kernels that re-insert and import items, the slot cap and the messages.  The routines after them are written
+// once over both tables.
+// KUQ_EXACT_MAX_SLOTS caps the slots the exact set may grow to, as if the device had no room for more: tests use it to
+// build, on one card, runs whose union exceeds one context's table (0 / unset = no cap)
+uint64_t max_slots(const SparseTable &) { return 0; }
+uint64_t max_slots(const ExactTable &) {
+  const char *e = getenv("KUQ_EXACT_MAX_SLOTS");
+  return e ? strtoull(e, nullptr, 10) : 0;
+}
+SparseSet set_view(const kuq_ctx *ctx, const SparseTable &t) {
+  return SparseSet{t.slots, t.cap ? t.cap - 1 : 0, ctx->d_sparse_used, t.count};
+}
+ExactSet set_view(const kuq_ctx *, const ExactTable &t) { return ExactSet{t.slots, t.cap ? t.cap - 1 : 0, t.count}; }
+void launch_import(kuq_ctx *ctx, const unsigned long long *keys, uint64_t n, const SparseSet &s, uint32_t *err) {
+  launch_sparse_import(keys, n, s, ctx->d_dense_flag, err, ctx->aux);
+}
+void launch_import(kuq_ctx *ctx, const ExactPair *pairs, uint64_t n, const ExactSet &e, uint32_t *err) {
+  launch_exact_import(pairs, n, e, err, ctx->aux);
+}
+// The messages of each table.  printf arguments: no_room_to_grow takes (slots now, slots wanted, GiB wanted), the two
+// `saturated` messages take the slots.
+struct TableText {
+  const char *name, *items, *no_room_to_grow, *saturated_importing, *saturated_building, *overran;
+};
+const TableText SPARSE_TEXT{"sparse-tier set", "keys", "sparse-tier set: no room to grow from %llu to %llu slots",
+                            "sparse-tier set saturated while importing", "sparse-tier set saturated while importing",
+                            "internal: partitioned export overran a segment"};
+const TableText EXACT_TEXT{"exact k-mer set", "pairs", "exact k-mer set: no room to grow from %llu to %llu slots (%.2f GiB)",
+                           "exact k-mer set saturated while importing (%llu slots)",
+                           "exact k-mer set saturated while building a part (%llu slots)", "internal: partitioned export overran a part"};
+const TableText &text(const SparseTable &) { return SPARSE_TEXT; }
+const TableText &text(const ExactTable &) { return EXACT_TEXT; }
+// a table of `cap` slots for `incoming` items could not be allocated
+int no_room_for(kuq_ctx *ctx, const SparseTable &, uint64_t, uint64_t cap) {
+  (void)cudaGetLastError();
+  return fail(ctx, KUQ_E_NOMEM, "sparse-tier set: no room for %llu slots", (unsigned long long)cap);
+}
+int no_room_for(kuq_ctx *ctx, const ExactTable &, uint64_t incoming, uint64_t cap) {
+  (void)cudaGetLastError();
+  return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no room for a part of %llu pairs (%llu slots, %.2f GiB) on device %d",
+              (unsigned long long)incoming, (unsigned long long)cap, cap * 16.0 / (1ull << 30), ctx->device);
+}
+
+// Runs `launch(d_err)` on ctx->aux with a zeroed device word that its kernels set when the table they fill is full, and
+// turns a set word into KUQ_E_CAPACITY with the message (fmt, args).
+template <typename Launch, typename... Args>
+int run_saturating(kuq_ctx *ctx, Launch launch, const char *fmt, Args... args) {
+  uint32_t *d_err = nullptr;
+  CU(dmalloc(&d_err, 1));
+  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
+  launch(d_err);
+  ctx->launches++;
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_err);
+  return err ? fail(ctx, KUQ_E_CAPACITY, fmt, args...) : KUQ_OK;
+}
+
+// the table's per-taxon counter on the host, and the items in the table: every item was counted once, under its taxon
+template <typename Table, typename Count>
+int table_counts(kuq_ctx *ctx, const Table &t, std::vector<Count> &count, uint64_t *n) {
+  count.resize(ctx->n_sketch);
+  CU(cudaMemcpy(count.data(), t.count, ctx->n_sketch * sizeof count[0], cudaMemcpyDeviceToHost));
+  *n = 0;
+  for (auto v : count) *n += v;
+  return KUQ_OK;
+}
+template <typename Table>
+int table_items(kuq_ctx *ctx, const Table &t, uint64_t *n) {
+  std::vector<std::remove_pointer_t<decltype(t.count)>> count;
+  return table_counts(ctx, t, count, n);
+}
+
+// slots for n items at a load of at most tenths / 10: `cap`, doubled as often as that needs
+uint64_t slots_for(uint64_t n, uint64_t cap, uint64_t tenths) {
+  cap = std::max<uint64_t>(cap, 1);
+  while (n * 10 > cap * tenths) cap <<= 1;
+  return cap;
+}
+
+// Re-allocate the table with `cap` slots and re-insert its items (not counted again).  All slots must be idle.
+template <typename Table>
+int grow_table(kuq_ctx *ctx, Table &t, uint64_t cap) {
+  Table bigger = t;
+  bigger.slots = nullptr;
+  bigger.cap = cap;
+  const uint64_t max = max_slots(t);
+  if ((max && cap > max) || dmalloc(&bigger.slots, cap) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return fail(ctx, KUQ_E_NOMEM, text(t).no_room_to_grow, (unsigned long long)t.cap, (unsigned long long)cap,
+                cap * (double)sizeof *t.slots / (1ull << 30));
+  }
+  CU(cudaMemsetAsync(bigger.slots, 0, cap * sizeof *t.slots, ctx->aux));
+  const int rc = run_saturating(ctx, [&](uint32_t *err) { launch_rehash(t.slots, t.cap, set_view(ctx, bigger), err, ctx->aux); },
+                                "%s saturated while growing to %llu slots", text(t).name, (unsigned long long)cap);
+  if (rc) { cudaFree(bigger.slots); return rc; }
+  cudaFree(t.slots);
+  t.slots = bigger.slots;
+  t.cap = cap;
+  t.grown++;
+  return KUQ_OK;
+}
+
+// The one growth rule of both tables: `used` items in the table and `incoming` more to come; when they could pass a
+// load factor of 0.8, the table grows to a load of at most 0.6.  t.upper becomes their sum.  All slots must be idle.
+template <typename Table>
+int make_room(kuq_ctx *ctx, Table &t, uint64_t used, uint64_t incoming) {
+  t.upper = used;
+  if ((used + incoming) * 10 > t.cap * 8) {
+    int rc = grow_table(ctx, t, slots_for(used + incoming, t.cap, 6));
+    if (rc) return rc;
+  }
+  t.upper += incoming;
+  return KUQ_OK;
+}
+
+// Room for `incoming` more items, made BEFORE a batch instead of failing in the middle of it: t.upper bounds the items
+// since the last exact count, and only when the bound could pass the load of make_room does `fill` read the exact count
+// back (all slots drained first).
+template <typename Table, typename Fill>
+int reserve_room(kuq_ctx *ctx, Table &t, uint64_t incoming, Fill fill) {
+  if ((t.upper + incoming) * 10 <= t.cap * 8) { t.upper += incoming; return KUQ_OK; }
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  uint64_t used = 0;
+  int rc = fill(&used);
+  if (rc) return rc;
+  return make_room(ctx, t, used, incoming);
+}
+
+// Items (the table's layout) into the table; its counter grows by the items that were new.  The caller made room.
+template <typename Table, typename Item>
+int import_items(kuq_ctx *ctx, Table &t, const Item *items, uint64_t n, bool building = false) {
+  if (!n) return KUQ_OK;
+  return run_saturating(ctx, [&](uint32_t *err) { launch_import(ctx, items, n, set_view(ctx, t), err); },
+                        building ? text(t).saturated_building : text(t).saturated_importing, (unsigned long long)t.cap);
+}
+
+template <typename Table>
+void free_table(Table &t) {
+  cudaFree(t.slots);
+  cudaFree(t.count);
+  t = Table{};
+}
+
+template <typename Table>
+int clear_table(kuq_ctx *ctx, Table &t) {
+  CU(cudaMemsetAsync(t.slots, 0, t.cap * sizeof *t.slots, ctx->aux));
+  CU(cudaMemsetAsync(t.count, 0, ctx->n_sketch * sizeof *t.count, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  t.upper = 0;
+  return KUQ_OK;
+}
+
+// A fresh table for `incoming` items at a load of at most tenths / 10 from `start` slots up (the slot cap applies as to
+// growth), zeroed, with a zeroed per-taxon counter.  On ctx's device.
+template <typename Table>
+int alloc_table(kuq_ctx *ctx, uint64_t incoming, uint64_t start, uint64_t tenths, Table &t) {
+  const uint64_t cap = slots_for(incoming, start, tenths), max = max_slots(t);
+  if ((max && cap > max) || dmalloc(&t.slots, cap) != cudaSuccess || dmalloc(&t.count, ctx->n_sketch) != cudaSuccess) {
+    free_table(t);
+    return no_room_for(ctx, t, incoming, cap);
+  }
+  t.cap = cap;
+  return clear_table(ctx, t);
+}
+
+// the built table replaces the context's; `upper` bounds its items
+template <typename Table>
+void install_table(Table &t, Table &built, uint64_t upper) {
+  cudaFree(t.slots);
+  cudaFree(t.count);
+  built.grown = t.grown + (built.cap != t.cap);
+  built.upper = upper;
+  t = built;
+  built = Table{};
+}
+
+// The table's items become the received ones (the old ones were exported before), in a table sized for them at a load
+// of at most tenths / 10 from `start` slots up.  A table of another size replaces the old slots after they are freed,
+// so the peak is the received items and the new table.  When that fails, the context keeps an empty table of the old
+// size.  All slots must be idle.
+template <typename Table, typename Item>
+int replace_table(kuq_ctx *ctx, Table &t, const Item *items, uint64_t n, uint64_t start, uint64_t tenths) {
+  const uint64_t old_cap = t.cap, cap = slots_for(n, start, tenths), max = max_slots(t);
+  int rc = KUQ_OK;
+  if (cap != old_cap) {
+    cudaFree(t.slots);
+    t.slots = nullptr;
+    if ((max && cap > max) || dmalloc(&t.slots, cap) != cudaSuccess) {
+      t.slots = nullptr;
+      rc = no_room_for(ctx, t, n, cap);
+    }
+  }
+  t.cap = cap;
+  if (!rc) rc = clear_table(ctx, t);
+  if (!rc) rc = import_items(ctx, t, items, n, true);
+  if (!rc) {
+    t.grown += cap != old_cap;
+    t.upper = n;
+    return KUQ_OK;
+  }
+  t.cap = old_cap;
+  if (cap != old_cap) {
+    cudaFree(t.slots);
+    if (dmalloc(&t.slots, old_cap) != cudaSuccess) {
+      (void)cudaGetLastError();
+      t.slots = nullptr;
+      t.cap = t.upper = 0;
+      return rc;
+    }
+  }
+  clear_table(ctx, t);
+  return rc;
+}
+
+// The table's occupied slots compacted into out (cap items; out == nullptr only counts) by `launch(out, cap, d_n)`;
+// *n = their number.  All slots idle.
+template <typename Item, typename Launch>
+int export_items(kuq_ctx *ctx, Item *out, uint64_t cap, uint64_t *n, const char *items, Launch launch) {
+  unsigned long long *d_n = nullptr;
+  CU(dmalloc(&d_n, 1));
+  CU(cudaMemsetAsync(d_n, 0, 8, ctx->aux));
+  launch(out, out ? cap : 0, d_n);
+  unsigned long long cnt = 0;
+  CU(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  cudaFree(d_n);
+  *n = cnt;
+  if (out && cnt > cap) return fail(ctx, KUQ_E_CAPACITY, "need room for %llu %s", cnt, items);
+  return KUQ_OK;
+}
+
+// The partitioned export: items grouped by owner part into out (cap items), parts back to back; counts[part] = items per
+// part.  `scan(counters, out, part_end, err, pass)` launches the table's parts kernels: pass 0 counts per part, pass 1
+// scatters through the part cursors, bounded by the part ends.  out == nullptr only counts, unless alloc_out asks the
+// library to size the buffer after the counting pass and hand it out.  All slots idle.
+template <typename Item, typename Scan>
+int export_parts(kuq_ctx *ctx, uint32_t n_parts, uint32_t max_parts, Item *out, uint64_t cap, uint64_t *counts, Item **alloc_out,
+                 const TableText &tx, Scan scan) {
+  const uint32_t P = max_parts;
+  unsigned long long *d_cnt = nullptr;
+  CU(dmalloc(&d_cnt, 2 * P + 1));                // [0, P) counts / cursors, [P, 2P) part ends, [2P] error word
+  CU(cudaMemsetAsync(d_cnt, 0, (2 * P + 1) * 8ull, ctx->aux));
+  uint32_t *d_err = reinterpret_cast<uint32_t *>(d_cnt + 2 * P);
+  scan(d_cnt, nullptr, nullptr, d_err, 0);
+  std::vector<unsigned long long> h(2 * P, 0);
+  CU(cudaMemcpyAsync(h.data(), d_cnt, P * 8ull, cudaMemcpyDeviceToHost, ctx->aux));
+  CU(cudaStreamSynchronize(ctx->aux));
+  uint64_t total = 0;
+  for (uint32_t j = 0; j < n_parts; j++) { counts[j] = h[j]; total += h[j]; }
+  if (alloc_out) {
+    if (dmalloc(&out, std::max<uint64_t>(total, 1)) != cudaSuccess) {
+      (void)cudaGetLastError();
+      cudaFree(d_cnt);
+      return fail(ctx, KUQ_E_NOMEM, "no room for %llu exported %s", (unsigned long long)total, tx.items);
+    }
+    cap = total;
+  }
+  if (!out) { cudaFree(d_cnt); return KUQ_OK; }     // counts only: nothing was consumed
+  int rc = KUQ_OK;
+  if (total > cap) {
+    rc = fail(ctx, KUQ_E_CAPACITY, "need room for %llu %s", (unsigned long long)total, tx.items);
+  } else {
+    unsigned long long at = 0;
+    for (uint32_t j = 0; j < P; j++) {
+      const unsigned long long c = j < n_parts ? h[j] : 0;
+      h[j] = at;
+      h[P + j] = at + c;
+      at += c;
+    }
+    CU(cudaMemcpyAsync(d_cnt, h.data(), 2 * P * 8ull, cudaMemcpyHostToDevice, ctx->aux));
+    scan(d_cnt, out, d_cnt + P, d_err, 1);
+    uint32_t err = 0;
+    CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
+    CU(cudaStreamSynchronize(ctx->aux));
+    if (err) rc = fail(ctx, KUQ_E_CAPACITY, tx.overran);
+  }
+  cudaFree(d_cnt);
+  if (alloc_out) {
+    if (rc) cudaFree(out); else *alloc_out = out;
+  }
+  return rc;
+}
+
+// kuq_sparse_tier_info / kuq_exact_info: the table's slots, items and growths
+template <typename Table>
+int table_info(kuq_ctx *ctx, const Table &t, uint64_t *slots, uint64_t *items, uint64_t *times_grown) {
+  if (slots) *slots = t.cap;
+  if (times_grown) *times_grown = t.grown;
+  if (!items) return KUQ_OK;
+  *items = 0;
+  if (!t.count) return KUQ_OK;
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  if (ctx->keep_dirty) {                         // duplicates of collision groups out first
+    int rc = settle_kept(ctx);
+    if (rc) return rc;
+  }
+  return table_items(ctx, t, items);
+}
+
+// Misses and the resolve half insert (taxon, code) pairs straight into the set — at most one per window of the batch.
+int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
+  if (!ctx->sparse.slots) return KUQ_OK;
+  auto fill = [ctx](uint64_t *used) -> int {
+    uint64_t n = 0;
+    int rc = table_items(ctx, ctx->sparse, &n);
+    if (rc) return rc;
+    // keys of kept records live in the records, not in the set; those of keep-mode calls since the last settle_kept are
+    // counted in count[] and in d_harvest_stat[2] alike (duplicates of collision groups included)
+    unsigned long long pending = 0;
+    if (ctx->keep_dirty) CU(cudaMemcpy(&pending, ctx->d_harvest_stat + 2, 8, cudaMemcpyDeviceToHost));
+    *used = n - std::min<uint64_t>(n, ctx->kept_keys + pending);
+    return KUQ_OK;
+  };
+  return reserve_room(ctx, ctx->sparse, windows, fill);
+}
+
+// A batch adds at most one pair per non-ambiguous window; an import at most one per incoming pair.
+int reserve_exact_inserts(kuq_ctx *ctx, uint64_t incoming) {
+  if (!ctx->exact.slots) return KUQ_OK;
+  return reserve_room(ctx, ctx->exact, incoming, [ctx](uint64_t *used) { return table_items(ctx, ctx->exact, used); });
+}
+
+// Occupied slots [lo, hi) of the exact table into out (cap pairs; cap 0 only counts); *n = their number.  All slots idle.
+int exact_export_range(kuq_ctx *ctx, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t cap, uint64_t *n) {
+  return export_items(ctx, out, cap, n, "pairs", [&](ExactPair *o, uint64_t c, unsigned long long *d_n) {
+    launch_exact_export(ctx->exact.slots, lo, hi, o, c, d_n, ctx->aux);
+    ctx->launches++;
+  });
+}
+
+// Slots [lo, hi) of the exact table grouped by owner (exact_owner) into out, parts back to back (export_parts).
+int exact_parts(kuq_ctx *ctx, uint64_t lo, uint64_t hi, uint32_t n_parts, ExactPair *out, uint64_t cap, uint64_t *counts,
+                ExactPair **alloc_out = nullptr) {
+  return export_parts(ctx, n_parts, EXACT_MAX_PARTS, out, cap, counts, alloc_out, EXACT_TEXT,
+                      [&](unsigned long long *cnt, ExactPair *o, const unsigned long long *end, uint32_t *err, int pass) {
+                        launch_exact_parts(ctx->exact.slots, lo, hi, n_parts, cnt, o, end, err, pass, ctx->aux);
+                        ctx->launches++;
+                      });
+}
+
+// pairs of another context (ExactPair layout) into the table, grown first when they need room.  All slots idle.
+int exact_import(kuq_ctx *ctx, const ExactPair *d_pairs, uint64_t n) {
+  int rc = reserve_exact_inserts(ctx, n);
+  if (rc) return rc;
+  ctx->snap_valid = false;
+  return import_items(ctx, ctx->exact, d_pairs, n);
+}
+
+// a batch's kernels found the set they insert into full (error code 4)
+int batch_set_saturated(kuq_ctx *ctx) {
+  if (ctx->cfg.hll_mode == KUQ_HLL_EXACT)
+    return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated (%llu slots)", (unsigned long long)ctx->exact.cap);
+  return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated: raise kuq_config.sparse_set_slots (now %llu)", (unsigned long long)ctx->sparse.cap);
+}
+
+// src's exact pairs go to the tables of dsts[0, n) in rounds over at most 2^22 slots of src's table (64 MiB of pairs per
+// round on each side; KUQ_EXACT_MERGE_SLOTS overrides it, so that tests of the rounds can use small tables).
+// `gather(lo, hi, buf, cap, counts)` compacts the slots [lo, hi) into buf on src's device, grouped by destination with
+// counts[o] pairs for dsts[o]; each group is copied peer to peer when its destination is on another device and handed
+// to `take(o, pairs, m)` there.  Peak per device: one round on each side.  Errors are reported on `report`.  The slots
+// of all contexts must be idle.
+template <typename Gather, typename Take>
+int move_rounds(kuq_ctx *report, const char *no_room, kuq_ctx *src, kuq_ctx *const *dsts, uint32_t n, Gather gather, Take take) {
+  kuq_ctx *ctx = report;
+  uint64_t round_slots = 1ull << 22;
+  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+  const uint64_t chunk = std::min(round_slots, src->exact.cap);
+  ExactPair *send = nullptr;
+  std::vector<ExactPair *> recv(n, nullptr);
+  int rc = KUQ_OK;
+  for (uint32_t o = 0; o <= n && !rc; o++) {     // the round buffer on src's device, then one on each other destination's
+    kuq_ctx *c = o < n ? dsts[o] : src;
+    ExactPair *&buf = o < n ? recv[o] : send;
+    if (o < n && c->device == src->device) continue;
+    CU(cudaSetDevice(c->device));
+    if (dmalloc(&buf, std::max<uint64_t>(chunk, 1)) != cudaSuccess) {
+      (void)cudaGetLastError();
+      rc = fail(ctx, KUQ_E_NOMEM, no_room, (unsigned long long)chunk, c->device);
+    }
+  }
+  std::vector<uint64_t> counts(n);
+  for (uint64_t lo = 0; lo < src->exact.cap && !rc; lo += chunk) {
+    CU(cudaSetDevice(src->device));
+    rc = gather(lo, std::min(lo + chunk, src->exact.cap), send, chunk, counts.data());
+    if (rc) { report->err = src->err; break; }
+    uint64_t off = 0;
+    for (uint32_t o = 0; o < n && !rc; o++) {
+      const uint64_t m = counts[o];
+      const ExactPair *from = send + off;
+      off += m;
+      if (!m) continue;
+      kuq_ctx *dst = dsts[o];
+      CU(cudaSetDevice(dst->device));
+      if (recv[o]) {
+        CU(cudaMemcpyPeer(recv[o], dst->device, from, src->device, m * 16));
+        from = recv[o];
+      }
+      rc = take(o, from, m);
+      if (rc && dst != report) report->err = dst->err;
+    }
+  }
+  for (uint32_t o = 0; o < n; o++)
+    if (recv[o]) { cudaSetDevice(dsts[o]->device); cudaFree(recv[o]); }
+  cudaSetDevice(src->device);
+  cudaFree(send);
+  cudaSetDevice(report->device);
+  return rc;
+}
+
+// kuq_merge_into under KUQ_HLL_EXACT: src's pairs move to dst's table in rounds (move_rounds), imported on dst's device
+// (count[] grows by the pairs dst did not hold yet).  Union does not depend on order, so dst ends with the set one
+// context would have built.  The slots of both contexts must be idle.
+int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
+  if (!src->exact.slots || !dst->exact.slots) return KUQ_OK;
+  return move_rounds(
+      dst, "exact k-mer set merge: no room for %llu pairs on device %d", src, &dst, 1,
+      [src](uint64_t lo, uint64_t hi, ExactPair *buf, uint64_t cap, uint64_t *counts) { return exact_export_range(src, lo, hi, buf, cap, counts); },
+      [dst](uint32_t, const ExactPair *pairs, uint64_t m) { return exact_import(dst, pairs, m); });
+}
+
 // Dense numbering: 0 = "no taxon", 1 = taxid 1 (the reference's hard-wired root, krakenutil.cpp:96,106), then every
 // taxid stored in database records (these own HLL sketches), then the remaining taxonomy nodes; each group
 // ascending by taxid.  Builds the flattened Parent_map and uploads everything.
@@ -494,20 +927,19 @@ int finalize(kuq_ctx *ctx) {
   CU(cudaMemset(ctx->d_n_kmers, 0, ctx->n_sketch * 8ull));
   CU(cudaMemset(ctx->d_n_reads, 0, ctx->n_taxa * 8ull));
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
-    ctx->exact_cap = ctx->cfg.sparse_set_slots;            // entries of 16 B; grows before batches that could fill it
-    ctx->exact_upper = 0;
-    CU(dmalloc(&ctx->d_exact, ctx->exact_cap));
-    CU(dmalloc(&ctx->d_exact_count, ctx->n_sketch));
-    CU(cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull));
-    CU(cudaMemset(ctx->d_exact_count, 0, ctx->n_sketch * 8ull));
+    ctx->exact.cap = ctx->cfg.sparse_set_slots;            // entries of 16 B; grows before batches that could fill it
+    CU(dmalloc(&ctx->exact.slots, ctx->exact.cap));
+    CU(dmalloc(&ctx->exact.count, ctx->n_sketch));
+    int rc = clear_table(ctx, ctx->exact);
+    if (rc) return rc;
   } else if (ctx->cfg.hll_mode != KUQ_HLL_DENSE_ONLY) {
-    ctx->sparse_cap = ctx->cfg.sparse_set_slots;
-    CU(dmalloc(&ctx->d_sparse_slots, ctx->sparse_cap));
+    ctx->sparse.cap = ctx->cfg.sparse_set_slots;
+    CU(dmalloc(&ctx->sparse.slots, ctx->sparse.cap));
     CU(dmalloc(&ctx->d_sparse_used, 1));
-    CU(dmalloc(&ctx->d_sparse_distinct, ctx->n_sketch));
-    CU(cudaMemset(ctx->d_sparse_slots, 0, ctx->sparse_cap * 8ull));
+    CU(dmalloc(&ctx->sparse.count, ctx->n_sketch));
     CU(cudaMemset(ctx->d_sparse_used, 0, 8));
-    CU(cudaMemset(ctx->d_sparse_distinct, 0, ctx->n_sketch * 4ull));
+    int rc = clear_table(ctx, ctx->sparse);
+    if (rc) return rc;
   }
   ctx->finalized = true;
   return KUQ_OK;
@@ -553,306 +985,6 @@ int remap_db(kuq_ctx *ctx) {
   return KUQ_OK;
 }
 
-// Sparse HLL tier of the hits: the fused lookup only flags the records it counted (SEEN_BIT); here the flagged
-// records of the staged range become (taxon, encoded hash) keys of the device set — the union the reference builds
-// with `taxon_counts[t] += ...` over sparse sketches (hyperloglogplus.cpp:600-603) — and the flags are cleared.
-// The number of keys is known before they are inserted, so the set grows here instead of failing mid-batch.
-// Re-allocate the sparse-tier set with `cap` slots and re-insert its keys.  All slots must be idle.
-int grow_sparse_set(kuq_ctx *ctx, uint64_t cap) {
-  unsigned long long *bigger = nullptr;
-  uint32_t *d_err = nullptr;
-  if (dmalloc(&bigger, cap) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return fail(ctx, KUQ_E_NOMEM, "sparse-tier set: no room to grow from %llu to %llu slots", (unsigned long long)ctx->sparse_cap, (unsigned long long)cap);
-  }
-  CU(dmalloc(&d_err, 1));
-  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
-  CU(cudaMemsetAsync(bigger, 0, cap * 8ull, ctx->aux));
-  SparseSet nb;
-  nb.slots = bigger; nb.mask = cap - 1; nb.n_used = ctx->d_sparse_used; nb.distinct = ctx->d_sparse_distinct;
-  launch_sparse_rehash(ctx->d_sparse_slots, ctx->sparse_cap, nb, d_err, ctx->aux);
-  ctx->launches++;
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
-  cudaFree(ctx->d_sparse_slots);
-  ctx->d_sparse_slots = bigger;
-  ctx->sparse_cap = cap;
-  ctx->sparse_grown++;
-  return KUQ_OK;
-}
-
-// Room for `incoming` more keys in an open-addressing table of `cap` slots, made BEFORE a batch instead of failing in the
-// middle of it: `upper` bounds the keys in the table since the last exact count; when the bound says the table could
-// pass a load factor of 0.8, `fill` reads the exact count back (all slots drained first), and only if that still does
-// not fit does `grow` re-allocate the table at a load factor of at most 0.6.  The sparse-tier set and the exact set
-// both grow by this rule.
-template <typename Fill, typename Grow>
-int reserve_room(kuq_ctx *ctx, uint64_t &upper, uint64_t cap, uint64_t incoming, Fill fill, Grow grow) {
-  if ((upper + incoming) * 10 <= cap * 8) { upper += incoming; return KUQ_OK; }
-  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  uint64_t used = 0;
-  int rc = fill(&used);
-  if (rc) return rc;
-  upper = used;
-  if ((used + incoming) * 10 > cap * 8) {
-    uint64_t c = cap;
-    while ((used + incoming) * 10 > c * 6) c <<= 1;
-    rc = grow(c);
-    if (rc) return rc;
-  }
-  upper += incoming;
-  return KUQ_OK;
-}
-
-// Misses and the resolve half insert (taxon, code) pairs straight into the set — at most one per window of the batch.
-int reserve_direct_inserts(kuq_ctx *ctx, uint64_t windows) {
-  if (!ctx->d_sparse_slots) return KUQ_OK;
-  auto fill = [ctx](uint64_t *used) -> int {
-    std::vector<uint32_t> distinct(ctx->n_sketch);
-    CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
-    uint64_t n = 0;
-    for (uint32_t v : distinct) n += v;
-    // keys of kept records live in the records, not in the set; those of keep-mode calls since the last settle_kept are
-    // counted in distinct[] and in d_harvest_stat[2] alike (duplicates of collision groups included)
-    unsigned long long pending = 0;
-    if (ctx->keep_dirty) CU(cudaMemcpy(&pending, ctx->d_harvest_stat + 2, 8, cudaMemcpyDeviceToHost));
-    *used = n - std::min<uint64_t>(n, ctx->kept_keys + pending);
-    return KUQ_OK;
-  };
-  return reserve_room(ctx, ctx->direct_upper, ctx->sparse_cap, windows, fill, [ctx](uint64_t cap) { return grow_sparse_set(ctx, cap); });
-}
-
-// ---- the exact k-mer set (KUQ_HLL_EXACT) grows like the sparse-tier set ---------------------------------------------
-// Re-allocate the (taxon, k-mer) table with `cap` slots and move its pairs over (not counted again).  All slots must be idle.
-// KUQ_EXACT_MAX_SLOTS caps the slots a table may grow to, as if the device had no room for more: tests use it to build,
-// on one card, runs whose union exceeds one context's table (0 / unset = no cap)
-uint64_t exact_max_slots() {
-  const char *e = getenv("KUQ_EXACT_MAX_SLOTS");
-  return e ? strtoull(e, nullptr, 10) : 0;
-}
-
-int grow_exact_set(kuq_ctx *ctx, uint64_t cap) {
-  ExactPair *bigger = nullptr;
-  const uint64_t max_slots = exact_max_slots();
-  if ((max_slots && cap > max_slots) || dmalloc(&bigger, cap) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no room to grow from %llu to %llu slots (%.2f GiB)", (unsigned long long)ctx->exact_cap,
-                (unsigned long long)cap, cap * 16.0 / (1ull << 30));
-  }
-  uint32_t *d_err = nullptr;
-  CU(dmalloc(&d_err, 1));
-  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
-  CU(cudaMemsetAsync(bigger, 0, cap * 16ull, ctx->aux));
-  const ExactSet nb{bigger, cap - 1, ctx->d_exact_count};
-  launch_exact_rehash(ctx->d_exact, ctx->exact_cap, nb, d_err, ctx->aux);
-  ctx->launches++;
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
-  if (err) { cudaFree(bigger); return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated while growing to %llu slots", (unsigned long long)cap); }
-  cudaFree(ctx->d_exact);
-  ctx->d_exact = bigger;
-  ctx->exact_cap = cap;
-  ctx->exact_grown++;
-  return KUQ_OK;
-}
-
-// pairs in the table: every pair was counted once, under its taxon
-int exact_pairs(kuq_ctx *ctx, uint64_t *n) {
-  std::vector<unsigned long long> count(ctx->n_sketch);
-  CU(cudaMemcpy(count.data(), ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
-  *n = 0;
-  for (unsigned long long v : count) *n += v;
-  return KUQ_OK;
-}
-
-// A batch adds at most one pair per non-ambiguous window; an import at most one per incoming pair.
-int reserve_exact_inserts(kuq_ctx *ctx, uint64_t incoming) {
-  if (!ctx->d_exact) return KUQ_OK;
-  return reserve_room(ctx, ctx->exact_upper, ctx->exact_cap, incoming, [ctx](uint64_t *used) { return exact_pairs(ctx, used); },
-                      [ctx](uint64_t cap) { return grow_exact_set(ctx, cap); });
-}
-
-// Occupied slots [lo, hi) of the table into out (cap pairs; cap 0 only counts); *n = their number.  All slots idle.
-int exact_export_range(kuq_ctx *ctx, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t cap, uint64_t *n) {
-  unsigned long long *d_n = nullptr;
-  CU(dmalloc(&d_n, 1));
-  CU(cudaMemsetAsync(d_n, 0, 8, ctx->aux));
-  launch_exact_export(ctx->d_exact, lo, hi, out, out ? cap : 0, d_n, ctx->aux);
-  ctx->launches++;
-  unsigned long long cnt = 0;
-  CU(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_n);
-  *n = cnt;
-  if (out && cnt > cap) return fail(ctx, KUQ_E_CAPACITY, "need room for %llu pairs", cnt);
-  return KUQ_OK;
-}
-
-// pairs of another context (ExactPair layout) into the table, grown first when they need room.  All slots idle.
-int exact_import(kuq_ctx *ctx, const ExactPair *d_pairs, uint64_t n) {
-  int rc = reserve_exact_inserts(ctx, n);
-  if (rc) return rc;
-  ctx->snap_valid = false;
-  uint32_t *d_err = nullptr;
-  CU(dmalloc(&d_err, 1));
-  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
-  const ExactSet es{ctx->d_exact, ctx->exact_cap - 1, ctx->d_exact_count};
-  launch_exact_import(d_pairs, n, es, d_err, ctx->aux);
-  ctx->launches++;
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
-  if (err) return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated while importing (%llu slots)", (unsigned long long)ctx->exact_cap);
-  return KUQ_OK;
-}
-
-// a batch's kernels found the set they insert into full (error code 4)
-int batch_set_saturated(kuq_ctx *ctx) {
-  if (ctx->cfg.hll_mode == KUQ_HLL_EXACT)
-    return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated (%llu slots)", (unsigned long long)ctx->exact_cap);
-  return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated: raise kuq_config.sparse_set_slots (now %llu)", (unsigned long long)ctx->sparse_cap);
-}
-
-// kuq_merge_into under KUQ_HLL_EXACT: src's pairs move to dst in rounds over at most 2^22 slots of src's table (64 MiB
-// of pairs per round on each side; KUQ_EXACT_MERGE_SLOTS overrides it, so that tests of the rounds can use small tables)
-// — compacted on src's device, copied peer to peer when the devices differ, imported on dst's (count[] grows by the pairs
-// dst did not hold yet).  Union does not depend on order, so dst ends with the set one context would have built.
-// The slots of both contexts must be idle.
-int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
-  kuq_ctx *ctx = dst;
-  if (!src->d_exact || !dst->d_exact) return KUQ_OK;
-  uint64_t round_slots = 1ull << 22;
-  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
-  const uint64_t chunk = std::min(round_slots, src->exact_cap);
-  const bool same_device = src->device == dst->device;
-  ExactPair *d_src = nullptr, *d_dst = nullptr;
-  CU(cudaSetDevice(src->device));
-  if (dmalloc(&d_src, chunk) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set merge: no room for %llu pairs on device %d", (unsigned long long)chunk, src->device);
-  }
-  int rc = KUQ_OK;
-  if (!same_device) {
-    CU(cudaSetDevice(dst->device));
-    if (dmalloc(&d_dst, chunk) != cudaSuccess) {
-      (void)cudaGetLastError();
-      rc = fail(ctx, KUQ_E_NOMEM, "exact k-mer set merge: no room for %llu pairs on device %d", (unsigned long long)chunk, dst->device);
-    }
-  }
-  for (uint64_t lo = 0; lo < src->exact_cap && !rc; lo += chunk) {
-    uint64_t n = 0;
-    CU(cudaSetDevice(src->device));
-    rc = exact_export_range(src, lo, std::min(lo + chunk, src->exact_cap), d_src, chunk, &n);
-    if (rc) { dst->err = src->err; break; }
-    if (!n) continue;
-    CU(cudaSetDevice(dst->device));
-    if (!same_device) CU(cudaMemcpyPeer(d_dst, dst->device, d_src, src->device, n * 16));
-    rc = exact_import(dst, same_device ? d_src : d_dst, n);
-  }
-  cudaSetDevice(src->device);
-  cudaFree(d_src);
-  cudaSetDevice(dst->device);
-  if (d_dst) cudaFree(d_dst);
-  return rc;
-}
-
-// ---- the exact set partitioned by k-mer over contexts (kuq_exact_export_partitioned / _replace / _partition) ---------
-// Slots [lo, hi) of the table grouped by owner (exact_owner) into out, parts back to back; counts[part] = their number.
-// out == nullptr only counts.  All slots idle.
-int exact_parts_range(kuq_ctx *ctx, uint64_t lo, uint64_t hi, uint32_t n_parts, ExactPair *out, uint64_t cap, uint64_t *counts) {
-  unsigned long long *d_cnt = nullptr;
-  const uint32_t P = EXACT_MAX_PARTS;
-  CU(dmalloc(&d_cnt, 2 * P + 1));                // [0, P) counts / cursors, [P, 2P) part ends, [2P] error word
-  CU(cudaMemsetAsync(d_cnt, 0, (2 * P + 1) * 8ull, ctx->aux));
-  uint32_t *d_err = reinterpret_cast<uint32_t *>(d_cnt + 2 * P);
-  launch_exact_parts(ctx->d_exact, lo, hi, n_parts, d_cnt, nullptr, nullptr, d_err, 0, ctx->aux);
-  ctx->launches++;
-  std::vector<unsigned long long> h(2 * P, 0);
-  CU(cudaMemcpyAsync(h.data(), d_cnt, P * 8ull, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  uint64_t total = 0;
-  for (uint32_t j = 0; j < n_parts; j++) { counts[j] = h[j]; total += h[j]; }
-  if (!out) { cudaFree(d_cnt); return KUQ_OK; }
-  if (total > cap) { cudaFree(d_cnt); return fail(ctx, KUQ_E_CAPACITY, "need room for %llu pairs", (unsigned long long)total); }
-  unsigned long long at = 0;
-  for (uint32_t j = 0; j < P; j++) {
-    const unsigned long long c = j < n_parts ? h[j] : 0;
-    h[j] = at;
-    h[P + j] = at + c;
-    at += c;
-  }
-  CU(cudaMemcpyAsync(d_cnt, h.data(), 2 * P * 8ull, cudaMemcpyHostToDevice, ctx->aux));
-  launch_exact_parts(ctx->d_exact, lo, hi, n_parts, d_cnt, out, d_cnt + P, d_err, 1, ctx->aux);
-  ctx->launches++;
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_cnt);
-  if (err) return fail(ctx, KUQ_E_CAPACITY, "internal: partitioned export overran a part");
-  return KUQ_OK;
-}
-
-// A fresh table for `incoming` pairs at a load of at most 0.6 (KUQ_EXACT_MAX_SLOTS applies as to growth), zeroed, with
-// zeroed per-taxon counters.  On ctx's device.
-struct ExactTable {
-  ExactPair *slots = nullptr;
-  unsigned long long *count = nullptr;
-  uint64_t cap = 0;
-};
-int exact_table_alloc(kuq_ctx *ctx, uint64_t incoming, ExactTable &t) {
-  uint64_t cap = 1024;
-  while (incoming * 10 > cap * 6) cap <<= 1;
-  const uint64_t max_slots = exact_max_slots();
-  if ((max_slots && cap > max_slots) || dmalloc(&t.slots, cap) != cudaSuccess ||
-      dmalloc(&t.count, ctx->n_sketch) != cudaSuccess) {
-    (void)cudaGetLastError();
-    cudaFree(t.slots);
-    t = ExactTable{};
-    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no room for a part of %llu pairs (%llu slots, %.2f GiB) on device %d",
-                (unsigned long long)incoming, (unsigned long long)cap, cap * 16.0 / (1ull << 30), ctx->device);
-  }
-  t.cap = cap;
-  CU(cudaMemsetAsync(t.slots, 0, cap * 16ull, ctx->aux));
-  CU(cudaMemsetAsync(t.count, 0, ctx->n_sketch * 8ull, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  return KUQ_OK;
-}
-void exact_table_free(ExactTable &t) { cudaFree(t.slots); cudaFree(t.count); t = ExactTable{}; }
-
-// pairs into a table that is being built; count[] grows by the pairs that are new, so duplicates across senders collapse
-int exact_table_import(kuq_ctx *ctx, ExactTable &t, const ExactPair *d_pairs, uint64_t n) {
-  if (!n) return KUQ_OK;
-  uint32_t *d_err = nullptr;
-  CU(dmalloc(&d_err, 1));
-  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
-  launch_exact_import(d_pairs, n, ExactSet{t.slots, t.cap - 1, t.count}, d_err, ctx->aux);
-  ctx->launches++;
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
-  if (err) return fail(ctx, KUQ_E_CAPACITY, "exact k-mer set saturated while building a part (%llu slots)", (unsigned long long)t.cap);
-  return KUQ_OK;
-}
-
-// the built table replaces the context's: from now on it holds one owner's part
-void exact_table_install(kuq_ctx *ctx, ExactTable &t, uint64_t upper) {
-  cudaFree(ctx->d_exact);
-  cudaFree(ctx->d_exact_count);
-  ctx->d_exact = t.slots;
-  ctx->d_exact_count = t.count;
-  if (t.cap != ctx->exact_cap) ctx->exact_grown++;
-  ctx->exact_cap = t.cap;
-  ctx->exact_upper = upper;
-  ctx->exact_partitioned = true;
-  ctx->merged_exact = false;
-  ctx->snap_valid = false;
-  t = ExactTable{};
-}
-
 // Preorder of the context's taxonomy (roots: taxa whose parent is 0, as in kuq_clade_counts_tree), kept for the sketch
 // taxa on host and device.  Taxa no root reaches (a malformed chain) stay NONE and are left out of the roll-up.
 int exact_preorder(kuq_ctx *ctx) {
@@ -894,10 +1026,10 @@ int exact_preorder(kuq_ctx *ctx) {
 int exact_books(kuq_ctx *ctx, std::vector<long long> &books) {
   int rc = exact_preorder(ctx);
   if (rc) return rc;
-  std::vector<unsigned long long> count(ctx->n_sketch);
-  CU(cudaMemcpy(count.data(), ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+  std::vector<unsigned long long> count;
   uint64_t n_pairs = 0;
-  for (unsigned long long v : count) n_pairs += v;
+  rc = table_counts(ctx, ctx->exact, count, &n_pairs);
+  if (rc) return rc;
   unsigned long long *d_books = nullptr;
   CU(dmalloc(&d_books, ctx->n_taxa));
   CU(cudaMemsetAsync(d_books, 0, ctx->n_taxa * 8ull, ctx->aux));
@@ -908,7 +1040,7 @@ int exact_books(kuq_ctx *ctx, std::vector<long long> &books) {
     CU(cudaMemGetInfo(&free_b, &total_b));
     budget = (uint64_t)(free_b * 0.8);
   }
-  const int src = exact_clade_dups(ctx->d_exact, ctx->exact_cap, n_pairs, ctx->d_exact_pre, ctx->d_parent, ctx->d_depth, d_books,
+  const int src = exact_clade_dups(ctx->exact.slots, ctx->exact.cap, n_pairs, ctx->d_exact_pre, ctx->d_parent, ctx->d_depth, d_books,
                                    std::max<uint64_t>(budget, 1), ctx->n_sm, ctx->aux, &ctx->exact_rollup_passes);
   ctx->launches += 3ull * std::max<uint32_t>(ctx->exact_rollup_passes, 1);
   std::vector<unsigned long long> dups(ctx->n_taxa, 0);
@@ -959,7 +1091,7 @@ int harvest_state(kuq_ctx *ctx) {
 // runs and tests compare both in one build).
 int use_keep_mode(kuq_ctx *ctx, int mode, const Params &p, bool *keep) {
   *keep = false;
-  if (mode != MODE_FUSED || !p.n_reads || (p.flags & 4u) || ctx->cfg.hll_mode != KUQ_HLL_PRELOAD || !ctx->d_sparse_slots ||
+  if (mode != MODE_FUSED || !p.n_reads || (p.flags & 4u) || ctx->cfg.hll_mode != KUQ_HLL_PRELOAD || !ctx->sparse.slots ||
       ctx->set_has_hits || ctx->stream_open || ctx->seen_dirty || (ctx->quick_min && ctx->quick_stop))
     return KUQ_OK;
   const char *env = getenv("KUQ_KEEP_AT_HARVEST");
@@ -981,7 +1113,7 @@ int settle_kept(kuq_ctx *ctx) {
   unsigned long long *d_stat = ctx->d_harvest_stat;
   CU(cudaMemsetAsync(d_stat, 0, 8, ctx->aux));
   CU(cudaEventRecord(ctx->harvest_ev[0], ctx->aux));
-  launch_settle_kept(ctx->d_pairs, ctx->d_secondaries, ctx->n_secondaries, ctx->d_sparse_distinct, d_stat, ctx->aux);
+  launch_settle_kept(ctx->d_pairs, ctx->d_secondaries, ctx->n_secondaries, ctx->sparse.count, d_stat, ctx->aux);
   if (ctx->n_secondaries) ctx->launches++;
   CU(cudaEventRecord(ctx->harvest_ev[1], ctx->aux));
   unsigned long long st[3] = {0, 0, 0};
@@ -1003,35 +1135,19 @@ int settle_kept(kuq_ctx *ctx) {
 // to leave HBM, or the set is about to receive keys of hits that kept records could duplicate.  All slots must be idle.
 int spill_kept(kuq_ctx *ctx) {
   if (!ctx->kept) return KUQ_OK;
-  std::vector<uint32_t> distinct(ctx->n_sketch);
-  CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
   uint64_t used = 0;
-  for (uint32_t v : distinct) used += v;
-  if (used * 10 > ctx->sparse_cap * 8) {
-    uint64_t cap = ctx->sparse_cap;
-    while (used * 10 > cap * 6) cap <<= 1;
-    int grc = grow_sparse_set(ctx, cap);
-    if (grc) return grc;
-  }
-  SparseSet ss;
-  ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1; ss.n_used = ctx->d_sparse_used; ss.distinct = ctx->d_sparse_distinct;
-  uint32_t *d_err;
-  CU(dmalloc(&d_err, 1));
-  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
-  launch_harvest_seen(ctx->d_pairs, ctx->key_ct, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), ctx->d_dense_flag, ss, nullptr,
-                      d_err, 3, ctx->aux);
-  ctx->launches++;
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
+  int rc = table_items(ctx, ctx->sparse, &used);
+  if (!rc) rc = make_room(ctx, ctx->sparse, used, 0);
+  if (rc) return rc;
+  const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
+  rc = run_saturating(
+      ctx, [&](uint32_t *err) { launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, set_view(ctx, ctx->sparse), nullptr, err, 3, ctx->aux); },
+      "sparse-tier set saturated while taking over the kept records (%llu slots)", (unsigned long long)ctx->sparse.cap);
   ctx->kept = false;
   ctx->kept_keys = 0;
   ctx->set_has_hits = true;
-  ctx->direct_upper = used;
   ctx->snap_valid = false;
-  if (err) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated while taking over the kept records (%llu slots)", (unsigned long long)ctx->sparse_cap);
-  return KUQ_OK;
+  return rc;
 }
 
 // Sparse HLL tier of the hits: the fused lookup only flags the records it counted (SEEN_BIT); here the flags of the
@@ -1058,49 +1174,40 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   if (!ctx->seen_dirty && !(ctx->kept && discard)) return KUQ_OK;
   ctx->seen_dirty = false;
   if (!ctx->d_pairs || !ctx->key_ct) return KUQ_OK;
-  bool keep = !discard && !to_set && ctx->d_sparse_slots && !ctx->set_has_hits && !ctx->stream_open;
+  bool keep = !discard && !to_set && ctx->sparse.slots && !ctx->set_has_hits && !ctx->stream_open;
   if (keep) {
     int rc = ensure_collisions(ctx);
     if (rc) return rc;
     keep = ctx->collisions == 1;
   }
   const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
-  SparseSet ss;
-  ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0; ss.n_used = ctx->d_sparse_used;
-  ss.distinct = ctx->d_sparse_distinct;
+  SparseSet ss = set_view(ctx, ctx->sparse);
   { int rc = harvest_state(ctx); if (rc) return rc; }
   unsigned long long *d_stat = ctx->d_harvest_stat;
   cudaEvent_t e0 = ctx->harvest_ev[0], e1 = ctx->harvest_ev[1];
   CU(cudaMemsetAsync(d_stat, 0, 16, ctx->aux));
   CU(cudaEventRecord(e0, ctx->aux));
-  if (discard || !ctx->d_sparse_slots) {
+  if (discard || !ctx->sparse.slots) {
     launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 2, ctx->aux);
     ctx->launches++;
     ctx->kept = false;
     ctx->kept_keys = 0;
   } else if (keep) {
     launch_harvest_keep(ctx->d_pairs, ctx->key_ct, ctx->d_secondaries, ctx->n_secondaries, ctx->d_dense_flag, ctx->n_sketch,
-                        ctx->d_sparse_distinct, d_stat, ctx->aux);
+                        ctx->sparse.count, d_stat, ctx->aux);
     ctx->launches += ctx->n_secondaries ? 2 : 1;
     ctx->kept = true;
   } else {
     launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 0, ctx->aux);
     ctx->launches++;
     unsigned long long n_new = 0;
-    CU(cudaMemcpyAsync(&n_new, d_stat, 8, cudaMemcpyDeviceToHost, ctx->aux));
-    std::vector<uint32_t> distinct(ctx->n_sketch);
-    CU(cudaMemcpyAsync(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost, ctx->aux));
-    CU(cudaStreamSynchronize(ctx->aux));
     uint64_t used = 0;
-    for (uint32_t v : distinct) used += v;
-    if ((used + n_new) * 10 > ctx->sparse_cap * 8) {             // keep the load factor below 0.8
-      uint64_t cap = ctx->sparse_cap;
-      while ((used + n_new) * 10 > cap * 6) cap <<= 1;
-      int grc = grow_sparse_set(ctx, cap);
-      if (grc) return grc;
-      ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1;
-    }
-    ctx->direct_upper = used + n_new;
+    CU(cudaMemcpyAsync(&n_new, d_stat, 8, cudaMemcpyDeviceToHost, ctx->aux));
+    CU(cudaStreamSynchronize(ctx->aux));
+    int grc = table_items(ctx, ctx->sparse, &used);
+    if (!grc) grc = make_room(ctx, ctx->sparse, used, n_new);
+    if (grc) return grc;
+    ss = set_view(ctx, ctx->sparse);
     if (n_new) ctx->set_has_hits = true;
     // Insert in record order.  (Round 2 also tried staging the keys by table slice so that the inserts of a slice are
     // L2-resident: read-only probes got faster, but NEW keys did not (each one still costs a DRAM sector fetch and a
@@ -1108,7 +1215,7 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
     launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 1, ctx->aux);
     ctx->launches++;
     CU(cudaStreamSynchronize(ctx->aux));
-    if (getenv("KUQ_TIMING")) fprintf(stderr, "[timing] harvest: %llu flagged records, %llu slots\n", n_new, (unsigned long long)ctx->sparse_cap);
+    if (getenv("KUQ_TIMING")) fprintf(stderr, "[timing] harvest: %llu flagged records, %llu slots\n", n_new, (unsigned long long)ctx->sparse.cap);
   }
   CU(cudaEventRecord(e1, ctx->aux));
   unsigned long long st[2] = {0, 0};
@@ -1123,12 +1230,12 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
     if (getenv("KUQ_TIMING")) fprintf(stderr, "[timing] harvest: %llu records became kept (%llu kept), %.2f ms\n", st[0], (unsigned long long)ctx->kept_keys, ms);
     return KUQ_OK;
   }
-  if ((uint32_t)st[1]) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated during the harvest (%llu slots)", (unsigned long long)ctx->sparse_cap);
+  if ((uint32_t)st[1]) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated during the harvest (%llu slots)", (unsigned long long)ctx->sparse.cap);
   return KUQ_OK;
 }
 
 KeySource set_keys(const kuq_ctx *ctx) {
-  KeySource k{ctx->d_sparse_slots, nullptr, ctx->d_sparse_slots ? ctx->sparse_cap : 0, 0};
+  KeySource k{ctx->sparse.slots, nullptr, ctx->sparse.slots ? ctx->sparse.cap : 0, 0};
   return k;
 }
 KeySource kept_keys(const kuq_ctx *ctx) {
@@ -1245,13 +1352,8 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   p.n_kmers = ctx->d_n_kmers;
   p.n_reads_ctr = ctx->d_n_reads;
   p.dense_flag = ctx->d_dense_flag;
-  p.sparse.slots = ctx->d_sparse_slots;
-  p.sparse.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0;
-  p.sparse.n_used = ctx->d_sparse_used;
-  p.sparse.distinct = ctx->d_sparse_distinct;
-  p.exact.slots = ctx->d_exact;
-  p.exact.mask = ctx->exact_cap ? ctx->exact_cap - 1 : 0;
-  p.exact.count = ctx->d_exact_count;
+  p.sparse = set_view(ctx, ctx->sparse);
+  p.exact = set_view(ctx, ctx->exact);
   set_unit_ptrs(p, s);
 }
 
@@ -1346,17 +1448,14 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
     }
     int rrc = reserve_direct_inserts(ctx, s.total_bases);
     if (rrc) return rrc;
-    // the set may have moved
-    p.sparse.slots = ctx->d_sparse_slots;
-    p.sparse.mask = ctx->sparse_cap ? ctx->sparse_cap - 1 : 0;
+    p.sparse = set_view(ctx, ctx->sparse);             // the set may have moved
   }
   // exact counting: the batch's windows go into the (taxon, k-mer) table, which grows before the batch when they could
   // fill it
   if ((mode == MODE_RESOLVE || mode == MODE_FUSED) && !(p.flags & 4u) && ctx->cfg.hll_mode == KUQ_HLL_EXACT && p.n_reads) {
     int rrc = reserve_exact_inserts(ctx, s.total_bases);
     if (rrc) return rrc;
-    p.exact.slots = ctx->d_exact;
-    p.exact.mask = ctx->exact_cap - 1;
+    p.exact = set_view(ctx, ctx->exact);
   }
   const bool units = mode != MODE_LOOKUP && ctx->cfg.hll_mode == KUQ_HLL_PRELOAD && p.unit_id && !(p.flags & 4u);
   if (units) {
@@ -1398,7 +1497,7 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
   if (p.n_reads && mode != MODE_LOOKUP && !(p.flags & 4u)) {
     if (units) ctx->launches += launch_unit_accounting(p, ctx->n_sm, s.stream);
     else if (ctx->cfg.hll_mode == KUQ_HLL_CHUNKED) {
-      launch_flag_dense_global(ctx->d_sparse_distinct, ctx->d_dense_flag, ctx->n_sketch, s.stream);
+      launch_flag_dense_global(ctx->sparse.count, ctx->d_dense_flag, ctx->n_sketch, s.stream);
       ctx->launches++;
     }
   }
@@ -2235,11 +2334,11 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
   cudaFree(d_hist);
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
     h.exact.resize(ctx->n_sketch);
-    CU(cudaMemcpy(h.exact.data(), ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(h.exact.data(), ctx->exact.count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
     if (ctx->merged_exact) h.exact = ctx->merged_exact_count;   // sums over the k-mer parts (kuq_set_exact_summary)
   } else if (ctx->cfg.hll_mode != KUQ_HLL_DENSE_ONLY) {
     if (ctx->cfg.hll_mode == KUQ_HLL_CHUNKED) {
-      launch_flag_dense_global(ctx->d_sparse_distinct, ctx->d_dense_flag, ctx->n_sketch, ctx->aux);
+      launch_flag_dense_global(ctx->sparse.count, ctx->d_dense_flag, ctx->n_sketch, ctx->aux);
       ctx->launches++;
     }
     uint32_t *d_sh;
@@ -2251,7 +2350,7 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
     h.sparse_hist.resize((size_t)ctx->n_sketch * 64);
     CU(cudaMemcpyAsync(h.sparse_hist.data(), d_sh, (uint64_t)ctx->n_sketch * 64 * 4, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaMemcpyAsync(h.dense_flag.data(), ctx->d_dense_flag, ctx->n_sketch, cudaMemcpyDeviceToHost, ctx->aux));
-    CU(cudaMemcpyAsync(h.distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost, ctx->aux));
+    CU(cudaMemcpyAsync(h.distinct.data(), ctx->sparse.count, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaStreamSynchronize(ctx->aux));
     cudaFree(d_sh);
     if (ctx->merged_summary) {             // sums over the code partitions of all GPUs (kuq_set_sparse_summary)
@@ -2415,8 +2514,7 @@ int kuq_clade_counts(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t 
       CU(cudaMemcpyAsync(d_member, member.data(), ctx->n_sketch, cudaMemcpyHostToDevice, ctx->aux));
       CU(cudaMemsetAsync(d_set, 0, cap * 8, ctx->aux));
       CU(cudaMemsetAsync(d_cnt, 0, 16, ctx->aux));
-      ExactSet es{ctx->d_exact, ctx->exact_cap - 1, ctx->d_exact_count};
-      launch_exact_union(es, d_member, d_set, cap - 1, d_cnt, reinterpret_cast<uint32_t *>(d_cnt + 1), ctx->aux);
+      launch_exact_union(set_view(ctx, ctx->exact), d_member, d_set, cap - 1, d_cnt, reinterpret_cast<uint32_t *>(d_cnt + 1), ctx->aux);
       ctx->launches++;
       unsigned long long out[2];
       CU(cudaMemcpyAsync(out, d_cnt, 16, cudaMemcpyDeviceToHost, ctx->aux));
@@ -2760,24 +2858,16 @@ int kuq_sparse_export(kuq_ctx *ctx, uint64_t *d_keys_out, uint64_t cap, uint64_t
   int rc = ensure_ready(ctx);
   if (rc) return rc;
   *n = 0;
-  if (!ctx->d_sparse_slots) return KUQ_OK;                    // KUQ_HLL_DENSE_ONLY: no sparse tier
+  if (!ctx->sparse.slots) return KUQ_OK;                    // KUQ_HLL_DENSE_ONLY: no sparse tier
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   rc = harvest_seen(ctx, false);
   if (rc) return rc;
-  unsigned long long *d_n;
-  CU(dmalloc(&d_n, 1));
-  CU(cudaMemsetAsync(d_n, 0, 8, ctx->aux));
-  for (const KeySource &src : {set_keys(ctx), kept_keys(ctx)})
-    launch_sparse_export(src, ctx->d_dense_flag, reinterpret_cast<unsigned long long *>(d_keys_out), d_keys_out ? cap : 0, d_n, ctx->aux);
-  ctx->launches += ctx->kept ? 2 : 1;
-  unsigned long long cnt = 0;
-  CU(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_n);
-  *n = cnt;
-  if (d_keys_out && cnt > cap) return fail(ctx, KUQ_E_CAPACITY, "need room for %llu keys", cnt);
-  return KUQ_OK;
+  return export_items(ctx, reinterpret_cast<unsigned long long *>(d_keys_out), cap, n, "keys",
+                      [ctx](unsigned long long *out, uint64_t c, unsigned long long *d_n) {
+                        for (const KeySource &src : {set_keys(ctx), kept_keys(ctx)}) launch_sparse_export(src, ctx->d_dense_flag, out, c, d_n, ctx->aux);
+                        ctx->launches += ctx->kept ? 2 : 1;
+                      });
 }
 
 // ---- database sharded over GPUs: who counts, step flags, partitioned merge of the sparse tier ---------------------
@@ -2968,7 +3058,7 @@ static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets) {
   { int rc = harvest_seen(src, false); if (rc) { dst->err = src->err; return rc; } }
   uint64_t n_keys = 0;
   uint64_t *d_keys_src = nullptr;
-  if (src->d_sparse_slots && !exact && sets) {
+  if (src->sparse.slots && !exact && sets) {
     int rc = kuq_sparse_export(src, nullptr, 0, &n_keys);
     if (rc) { dst->err = src->err; return rc; }
     if (n_keys) {
@@ -3003,7 +3093,7 @@ static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets) {
   cudaFree(t_regs); cudaFree(t_dense); cudaFree(t_nk); cudaFree(t_nr);
   if (exact) return sets ? merge_exact_pairs(dst, src) : KUQ_OK;
   int rc = KUQ_OK;
-  if (n_keys && dst->d_sparse_slots) {
+  if (n_keys && dst->sparse.slots) {
     uint64_t *d_keys_dst = nullptr;
     if (cudaMalloc((void **)&d_keys_dst, n_keys * 8) != cudaSuccess) { (void)cudaGetLastError(); cudaSetDevice(src->device); cudaFree(d_keys_src); return fail(ctx, KUQ_E_NOMEM, "no room for %llu keys", (unsigned long long)n_keys); }
     CU(cudaMemcpyPeer(d_keys_dst, dst->device, d_keys_src, src->device, n_keys * 8));
@@ -3077,7 +3167,7 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
   int rc = ensure_ready(ctx);
   if (rc) return rc;
   for (uint32_t j = 0; j < n_parts; j++) counts[j] = 0;
-  if (!ctx->d_sparse_slots) return KUQ_OK;
+  if (!ctx->sparse.slots) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   if (ctx->keep_dirty) { rc = settle_kept(ctx); if (rc) return rc; }   // one kept record per key
@@ -3087,83 +3177,36 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
   // owner.
   const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
   const bool records = (ctx->seen_dirty || ctx->kept) && ctx->d_pairs && ctx->key_ct;
-  unsigned long long *d_cnt;
-  CU(dmalloc(&d_cnt, 24));                       // [0:8) counts / cursors, [8:16) part ends, [16] error word
-  CU(cudaMemsetAsync(d_cnt, 0, 24 * 8, ctx->aux));
-  uint32_t *d_err = reinterpret_cast<uint32_t *>(d_cnt + 16);
-  launch_keys_parts(0, ctx->d_sparse_slots, nullptr, ctx->sparse_cap, key_mask, ctx->d_dense_flag, n_parts, d_cnt, nullptr, nullptr, d_err, 0, ctx->aux);
-  ctx->launches++;
-  if (records) {
-    launch_keys_parts(1, nullptr, ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, n_parts, d_cnt, nullptr, nullptr, d_err, 0, ctx->aux);
-    ctx->launches++;
-  }
-  unsigned long long h[8];
-  CU(cudaMemcpyAsync(h, d_cnt, 64, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  uint64_t total = 0;
-  for (uint32_t j = 0; j < n_parts; j++) { counts[j] = h[j]; total += h[j]; }
-  if (alloc_out) {                                         // the library sizes the buffer (one counting pass instead of two)
-    if (cudaMalloc((void **)&d_keys_out, (total ? total : 1) * 8) != cudaSuccess) {
-      (void)cudaGetLastError();
-      cudaFree(d_cnt);
-      return fail(ctx, KUQ_E_NOMEM, "no room for %llu exported keys", (unsigned long long)total);
-    }
-    *alloc_out = d_keys_out;
-    cap = total;
-  }
-  if (!d_keys_out) { cudaFree(d_cnt); return KUQ_OK; }     // counts only: nothing was consumed
-  if (total > cap) { cudaFree(d_cnt); return fail(ctx, KUQ_E_CAPACITY, "need room for %llu keys", (unsigned long long)total); }
-  unsigned long long lay[16];
-  lay[0] = 0;
-  for (uint32_t j = 1; j < 8; j++) lay[j] = lay[j - 1] + (j - 1 < n_parts ? h[j - 1] : 0);
-  for (uint32_t j = 0; j < 8; j++) lay[8 + j] = lay[j] + (j < n_parts ? h[j] : 0);
-  CU(cudaMemcpyAsync(d_cnt, lay, 128, cudaMemcpyHostToDevice, ctx->aux));
-  launch_keys_parts(0, ctx->d_sparse_slots, nullptr, ctx->sparse_cap, key_mask, ctx->d_dense_flag, n_parts, d_cnt,
-                    reinterpret_cast<unsigned long long *>(d_keys_out), d_cnt + 8, d_err, 1, ctx->aux);
-  ctx->launches++;
-  if (records) {
-    launch_keys_parts(1, nullptr, ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, n_parts, d_cnt,
-                      reinterpret_cast<unsigned long long *>(d_keys_out), d_cnt + 8, d_err, 1, ctx->aux);
-    ctx->launches++;
-    ctx->seen_dirty = false;                     // the flags are gone: their keys live in the export buffer now (the kept
-                                                 // records drop their flag when the merged keys replace the set)
-  }
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_cnt);
-  if (err) return fail(ctx, KUQ_E_CAPACITY, "internal: partitioned export overran a segment");
-  return KUQ_OK;
+  return export_parts(ctx, n_parts, 8, reinterpret_cast<unsigned long long *>(d_keys_out), cap, counts,
+                      reinterpret_cast<unsigned long long **>(alloc_out), SPARSE_TEXT,
+                      [&](unsigned long long *cnt, unsigned long long *out, const unsigned long long *end, uint32_t *err, int pass) {
+                        launch_keys_parts(0, ctx->sparse.slots, nullptr, ctx->sparse.cap, key_mask, ctx->d_dense_flag, n_parts, cnt, out,
+                                          end, err, pass, ctx->aux);
+                        ctx->launches++;
+                        if (!records) return;
+                        launch_keys_parts(1, nullptr, ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, n_parts, cnt, out, end,
+                                          err, pass, ctx->aux);
+                        ctx->launches++;
+                        // the flags are gone: their keys live in the export buffer now (the kept records drop their flag
+                        // when the merged keys replace the set)
+                        if (pass == 1) ctx->seen_dirty = false;
+                      });
 }
 
 int kuq_sparse_replace(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   if (!ctx || (!d_keys && n)) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->d_sparse_slots) return KUQ_OK;
+  if (!ctx->sparse.slots) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   rc = harvest_seen(ctx, true);                  // anything still flagged or kept was exported before; drop the flags
   if (rc) return rc;
   ctx->snap_valid = false;
-  uint64_t cap = ctx->sparse_cap;
-  while (n * 10 > cap * 7) cap <<= 1;
-  if (cap != ctx->sparse_cap) {
-    cudaFree(ctx->d_sparse_slots);
-    ctx->d_sparse_slots = nullptr;
-    if (dmalloc(&ctx->d_sparse_slots, cap) != cudaSuccess) {
-      (void)cudaGetLastError();
-      ctx->sparse_cap = 0;
-      return fail(ctx, KUQ_E_NOMEM, "sparse-tier set: no room for %llu slots", (unsigned long long)cap);
-    }
-    ctx->sparse_cap = cap;
-    ctx->sparse_grown++;
-  }
-  CU(cudaMemsetAsync(ctx->d_sparse_slots, 0, ctx->sparse_cap * 8ull, ctx->aux));
-  CU(cudaMemsetAsync(ctx->d_sparse_distinct, 0, ctx->n_sketch * 4ull, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  ctx->direct_upper = n;
-  return kuq_sparse_import(ctx, d_keys, n);
+  // at a load of at most 0.7, from the current size up
+  rc = replace_table(ctx, ctx->sparse, reinterpret_cast<const unsigned long long *>(d_keys), n, ctx->sparse.cap, 7);
+  if (!rc && n) ctx->set_has_hits = true;
+  return rc;
 }
 
 int kuq_sparse_summary(kuq_ctx *ctx, uint32_t *d_hist_out, uint32_t *d_distinct_out) {
@@ -3175,11 +3218,11 @@ int kuq_sparse_summary(kuq_ctx *ctx, uint32_t *d_hist_out, uint32_t *d_distinct_
   rc = harvest_seen(ctx, false);
   if (rc) return rc;
   CU(cudaMemsetAsync(d_hist_out, 0, (uint64_t)ctx->n_sketch * 64 * 4, ctx->aux));
-  if (ctx->d_sparse_slots) {
+  if (ctx->sparse.slots) {
     launch_sparse_histograms(set_keys(ctx), ctx->d_dense_flag, d_hist_out, ctx->aux);
     launch_sparse_histograms(kept_keys(ctx), ctx->d_dense_flag, d_hist_out, ctx->aux);
     ctx->launches += ctx->kept ? 2 : 1;
-    CU(cudaMemcpyAsync(d_distinct_out, ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToDevice, ctx->aux));
+    CU(cudaMemcpyAsync(d_distinct_out, ctx->sparse.count, ctx->n_sketch * 4ull, cudaMemcpyDeviceToDevice, ctx->aux));
   } else {
     CU(cudaMemsetAsync(d_distinct_out, 0, ctx->n_sketch * 4ull, ctx->aux));
   }
@@ -3267,28 +3310,15 @@ int kuq_sparse_tier_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *keys, uint64_t
   if (!ctx) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (slots) *slots = ctx->sparse_cap;
-  if (times_grown) *times_grown = ctx->sparse_grown;
   if (last_harvest_ms) *last_harvest_ms = ctx->harvest_ms;
-  if (keys) {
-    *keys = 0;
-    if (ctx->d_sparse_distinct) {
-      CU(cudaSetDevice(ctx->device));
-      for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-      if (ctx->keep_dirty) { rc = settle_kept(ctx); if (rc) return rc; }     // duplicates of collision groups out
-      std::vector<uint32_t> d(ctx->n_sketch);
-      CU(cudaMemcpy(d.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
-      for (uint32_t v : d) *keys += v;
-    }
-  }
-  return KUQ_OK;
+  return table_info(ctx, ctx->sparse, slots, keys, times_grown);
 }
 
 int kuq_sparse_import(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   if (!ctx || (!d_keys && n)) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->d_sparse_slots || !n) return KUQ_OK;
+  if (!ctx->sparse.slots || !n) return KUQ_OK;
   ctx->snap_valid = false;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
@@ -3296,50 +3326,19 @@ int kuq_sparse_import(kuq_ctx *ctx, const uint64_t *d_keys, uint64_t n) {
   if (rc) return rc;
   // make room first: the import kernel cannot grow the set (a context that classified few reads or none has a small
   // set and may receive the keys of all the others)
-  std::vector<uint32_t> distinct(ctx->n_sketch);
-  CU(cudaMemcpy(distinct.data(), ctx->d_sparse_distinct, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost));
   uint64_t used = 0;
-  for (uint32_t v : distinct) used += v;
-  if ((used + n) * 10 > ctx->sparse_cap * 8) {
-    uint64_t cap = ctx->sparse_cap;
-    while ((used + n) * 10 > cap * 6) cap <<= 1;
-    rc = grow_sparse_set(ctx, cap);
-    if (rc) return rc;
-  }
-  ctx->direct_upper = used + n;
+  rc = table_items(ctx, ctx->sparse, &used);
+  if (!rc) rc = make_room(ctx, ctx->sparse, used, n);
+  if (rc) return rc;
   ctx->set_has_hits = true;
-  SparseSet ss;
-  ss.slots = ctx->d_sparse_slots; ss.mask = ctx->sparse_cap - 1; ss.n_used = ctx->d_sparse_used;
-  ss.distinct = ctx->d_sparse_distinct;
-  uint32_t *d_err;
-  CU(dmalloc(&d_err, 1));
-  CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
-  launch_sparse_import(reinterpret_cast<const unsigned long long *>(d_keys), n, ss, ctx->d_dense_flag, d_err, ctx->aux);
-  ctx->launches++;
-  uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
-  if (err) return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated while importing");
-  return KUQ_OK;
+  return import_items(ctx, ctx->sparse, reinterpret_cast<const unsigned long long *>(d_keys), n);
 }
 
 int kuq_exact_info(kuq_ctx *ctx, uint64_t *slots, uint64_t *pairs, uint64_t *times_grown) {
   if (!ctx) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (slots) *slots = ctx->exact_cap;
-  if (times_grown) *times_grown = ctx->exact_grown;
-  if (pairs) {
-    *pairs = 0;
-    if (ctx->d_exact) {
-      CU(cudaSetDevice(ctx->device));
-      for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-      rc = exact_pairs(ctx, pairs);
-      if (rc) return rc;
-    }
-  }
-  return KUQ_OK;
+  return table_info(ctx, ctx->exact, slots, pairs, times_grown);
 }
 
 int kuq_exact_export(kuq_ctx *ctx, void *d_pairs_out, uint64_t cap, uint64_t *n) {
@@ -3347,10 +3346,10 @@ int kuq_exact_export(kuq_ctx *ctx, void *d_pairs_out, uint64_t cap, uint64_t *n)
   int rc = ensure_ready(ctx);
   if (rc) return rc;
   *n = 0;
-  if (!ctx->d_exact) return KUQ_OK;                           // not KUQ_HLL_EXACT
+  if (!ctx->exact.slots) return KUQ_OK;                           // not KUQ_HLL_EXACT
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  return exact_export_range(ctx, 0, ctx->exact_cap, static_cast<ExactPair *>(d_pairs_out), d_pairs_out ? cap : 0, n);
+  return exact_export_range(ctx, 0, ctx->exact.cap, static_cast<ExactPair *>(d_pairs_out), d_pairs_out ? cap : 0, n);
 }
 
 int kuq_exact_import(kuq_ctx *ctx, const void *d_pairs, uint64_t n) {
@@ -3358,7 +3357,7 @@ int kuq_exact_import(kuq_ctx *ctx, const void *d_pairs, uint64_t n) {
   if ((uintptr_t)d_pairs & 15) return fail(ctx, KUQ_E_INVALID_ARG, "d_pairs must be 16-byte aligned");
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_import needs a KUQ_HLL_EXACT context");
+  if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_import needs a KUQ_HLL_EXACT context");
   if (!n) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
@@ -3373,26 +3372,11 @@ static int exact_export_partitioned(kuq_ctx *ctx, uint32_t n_parts, void *d_pair
   int rc = ensure_ready(ctx);
   if (rc) return rc;
   for (uint32_t j = 0; j < n_parts; j++) counts[j] = 0;
-  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_export_partitioned needs a KUQ_HLL_EXACT context");
+  if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_export_partitioned needs a KUQ_HLL_EXACT context");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  rc = exact_parts_range(ctx, 0, ctx->exact_cap, n_parts, nullptr, 0, counts);
-  if (rc || (!d_pairs_out && !alloc_out)) return rc;
-  uint64_t total = 0;
-  for (uint32_t j = 0; j < n_parts; j++) total += counts[j];
-  ExactPair *out = static_cast<ExactPair *>(d_pairs_out);
-  if (alloc_out) {                                         // the library sizes the buffer after its counting pass
-    if (dmalloc(&out, std::max<uint64_t>(total, 1)) != cudaSuccess) {
-      (void)cudaGetLastError();
-      return fail(ctx, KUQ_E_NOMEM, "no room for %llu exported pairs", (unsigned long long)total);
-    }
-    cap = total;
-  }
-  rc = exact_parts_range(ctx, 0, ctx->exact_cap, n_parts, out, cap, counts);
-  if (alloc_out) {
-    if (rc) cudaFree(out); else *alloc_out = out;
-  }
-  return rc;
+  return exact_parts(ctx, 0, ctx->exact.cap, n_parts, static_cast<ExactPair *>(d_pairs_out), cap, counts,
+                     reinterpret_cast<ExactPair **>(alloc_out));
 }
 
 int kuq_exact_export_partitioned(kuq_ctx *ctx, uint32_t n_parts, void *d_pairs_out, uint64_t cap, uint64_t *counts) {
@@ -3409,28 +3393,15 @@ int kuq_exact_replace(kuq_ctx *ctx, const void *d_pairs, uint64_t n) {
   if ((uintptr_t)d_pairs & 15) return fail(ctx, KUQ_E_INVALID_ARG, "d_pairs must be 16-byte aligned");
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_replace needs a KUQ_HLL_EXACT context");
+  if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_replace needs a KUQ_HLL_EXACT context");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  // the old pairs were exported before: its table goes first, so the peak is the received pairs and the new table
-  cudaFree(ctx->d_exact);
-  ctx->d_exact = nullptr;
-  ExactTable t;
-  rc = exact_table_alloc(ctx, n, t);
-  if (!rc) rc = exact_table_import(ctx, t, static_cast<const ExactPair *>(d_pairs), n);
-  if (rc) {                                      // leave an empty table of the old size behind, not a dangling one
-    exact_table_free(t);
-    if (dmalloc(&ctx->d_exact, ctx->exact_cap) == cudaSuccess) {
-      cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull);
-      cudaMemset(ctx->d_exact_count, 0, ctx->n_sketch * 8ull);
-    } else {
-      (void)cudaGetLastError();
-      ctx->exact_cap = 0;
-    }
-    ctx->exact_upper = 0;
-    return rc;
-  }
-  exact_table_install(ctx, t, n);
+  // a part of its own size: at a load of at most 0.6, from 1024 slots up
+  rc = replace_table(ctx, ctx->exact, static_cast<const ExactPair *>(d_pairs), n, 1024, 6);
+  if (rc) return rc;
+  ctx->exact_partitioned = true;                 // from now on the table holds one owner's part
+  ctx->merged_exact = false;
+  ctx->snap_valid = false;
   return KUQ_OK;
 }
 
@@ -3438,13 +3409,13 @@ int kuq_exact_summary(kuq_ctx *ctx, uint64_t *d_count_out, int64_t *d_books_out)
   if (!ctx || !d_count_out || !d_books_out) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_summary needs a KUQ_HLL_EXACT context");
+  if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_summary needs a KUQ_HLL_EXACT context");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   std::vector<long long> books;
   rc = exact_books(ctx, books);
   if (rc) return rc;
-  CU(cudaMemcpy(d_count_out, ctx->d_exact_count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToDevice));
+  CU(cudaMemcpy(d_count_out, ctx->exact.count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToDevice));
   CU(cudaMemcpy(d_books_out, books.data(), ctx->n_taxa * 8ull, cudaMemcpyHostToDevice));
   return KUQ_OK;
 }
@@ -3461,7 +3432,7 @@ int kuq_set_exact_summary(kuq_ctx *ctx, const uint64_t *d_count, const int64_t *
   if (!ctx || !d_count || !d_books) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_set_exact_summary needs a KUQ_HLL_EXACT context");
+  if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_set_exact_summary needs a KUQ_HLL_EXACT context");
   CU(cudaSetDevice(ctx->device));
   std::vector<unsigned long long> count(ctx->n_sketch);
   std::vector<long long> books(ctx->n_taxa);
@@ -3486,7 +3457,7 @@ int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
     kuq_ctx *c = ctxs[g];
     int rc = ensure_ready(c);
     if (rc) { if (g) ctx->err = c->err; return rc; }
-    if (!c->d_exact) return fail(ctx, KUQ_E_STATE, "kuq_exact_partition needs KUQ_HLL_EXACT contexts");
+    if (!c->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_partition needs KUQ_HLL_EXACT contexts");
     if (c->n_taxa != ctx->n_taxa || c->n_sketch != ctx->n_sketch || c->raw_of_dense != ctx->raw_of_dense)
       return fail(ctx, KUQ_E_STATE, "the contexts number their taxa differently (different database / taxonomy)");
     CU(cudaSetDevice(c->device));
@@ -3496,75 +3467,41 @@ int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
   std::vector<uint64_t> want(n, 0), counts(n);
   for (uint32_t g = 0; g < n; g++) {
     CU(cudaSetDevice(ctxs[g]->device));
-    int rc = exact_parts_range(ctxs[g], 0, ctxs[g]->exact_cap, n, nullptr, 0, counts.data());
+    int rc = exact_parts(ctxs[g], 0, ctxs[g]->exact.cap, n, nullptr, 0, counts.data());
     if (rc) { if (g) ctx->err = ctxs[g]->err; return rc; }
     for (uint32_t o = 0; o < n; o++) want[o] += counts[o];
   }
-  // 2. the new tables and the round buffers
-  uint64_t round_slots = 1ull << 22;
-  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+  // 2. the new parts, at a load of at most 0.6 from 1024 slots up
   std::vector<ExactTable> part(n);
-  std::vector<ExactPair *> round(n, nullptr), recv(n, nullptr);
-  std::vector<uint64_t> round_cap(n, 0);
   auto cleanup = [&]() {
     for (uint32_t g = 0; g < n; g++) {
       cudaSetDevice(ctxs[g]->device);
-      exact_table_free(part[g]);
-      cudaFree(round[g]);
-      cudaFree(recv[g]);
+      free_table(part[g]);
     }
     cudaSetDevice(ctx->device);
   };
   int rc = KUQ_OK;
   for (uint32_t g = 0; g < n && !rc; g++) {
-    kuq_ctx *c = ctxs[g];
-    CU(cudaSetDevice(c->device));
-    rc = exact_table_alloc(c, want[g], part[g]);
-    if (rc) { ctx->err = c->err; break; }
-    round_cap[g] = std::min(round_slots, c->exact_cap);
-    bool needs_recv = false;
-    for (uint32_t h = 0; h < n; h++) needs_recv |= ctxs[h]->device != c->device;
-    uint64_t recv_cap = 0;
-    for (uint32_t h = 0; h < n; h++) if (ctxs[h]->device != c->device) recv_cap = std::max(recv_cap, std::min(round_slots, ctxs[h]->exact_cap));
-    if (dmalloc(&round[g], std::max<uint64_t>(round_cap[g], 1)) != cudaSuccess ||
-        (needs_recv && dmalloc(&recv[g], std::max<uint64_t>(recv_cap, 1)) != cudaSuccess)) {
-      (void)cudaGetLastError();
-      rc = fail(ctx, KUQ_E_NOMEM, "exact k-mer set partition: no room for a round of %llu pairs on device %d",
-                (unsigned long long)round_cap[g], c->device);
-    }
+    CU(cudaSetDevice(ctxs[g]->device));
+    rc = alloc_table(ctxs[g], want[g], 1024, 6, part[g]);
+    if (rc) ctx->err = ctxs[g]->err;
   }
-  if (rc) { cleanup(); return rc; }
   // 3. rounds: a slot range of one source, grouped by owner, each group imported by its owner
   for (uint32_t g = 0; g < n && !rc; g++) {
     kuq_ctx *src = ctxs[g];
-    for (uint64_t lo = 0; lo < src->exact_cap && !rc; lo += round_cap[g]) {
-      CU(cudaSetDevice(src->device));
-      rc = exact_parts_range(src, lo, std::min(lo + round_cap[g], src->exact_cap), n, round[g], round_cap[g], counts.data());
-      if (rc) { ctx->err = src->err; break; }
-      uint64_t off = 0;
-      for (uint32_t o = 0; o < n && !rc; o++) {
-        const uint64_t m = counts[o];
-        const ExactPair *from = round[g] + off;
-        off += m;
-        if (!m) continue;
-        kuq_ctx *dst = ctxs[o];
-        CU(cudaSetDevice(dst->device));
-        if (dst->device != src->device) {
-          CU(cudaMemcpyPeer(recv[o], dst->device, from, src->device, m * 16));
-          from = recv[o];
-        }
-        rc = exact_table_import(dst, part[o], from, m);
-        if (rc) ctx->err = dst->err;
-      }
-    }
+    rc = move_rounds(
+        ctx, "exact k-mer set partition: no room for a round of %llu pairs on device %d", src, ctxs, n,
+        [src, n](uint64_t lo, uint64_t hi, ExactPair *buf, uint64_t cap, uint64_t *cnt) { return exact_parts(src, lo, hi, n, buf, cap, cnt); },
+        [&](uint32_t o, const ExactPair *pairs, uint64_t m) { return import_items(ctxs[o], part[o], pairs, m, true); });
   }
   if (rc) { cleanup(); return rc; }
-  // 4. the parts replace the tables
+  // 4. the parts replace the tables: from now on each holds one owner's part
   for (uint32_t g = 0; g < n; g++) {
     CU(cudaSetDevice(ctxs[g]->device));
-    cudaFree(round[g]); cudaFree(recv[g]);
-    round[g] = recv[g] = nullptr;
-    exact_table_install(ctxs[g], part[g], want[g]);
+    install_table(ctxs[g]->exact, part[g], want[g]);
+    ctxs[g]->exact_partitioned = true;
+    ctxs[g]->merged_exact = false;
+    ctxs[g]->snap_valid = false;
   }
   // 5. counters and books summed over the parts, installed on the first context
   std::vector<unsigned long long> count_sum(ctx->n_sketch, 0), cnt(ctx->n_sketch);
@@ -3574,7 +3511,7 @@ int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
     CU(cudaSetDevice(c->device));
     rc = exact_books(c, books);
     if (rc) { ctx->err = c->err; cudaSetDevice(ctx->device); return rc; }
-    CU(cudaMemcpy(cnt.data(), c->d_exact_count, c->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(cnt.data(), c->exact.count, c->n_sketch * 8ull, cudaMemcpyDeviceToHost));
     for (uint32_t d = 0; d < ctx->n_sketch; d++) count_sum[d] += cnt[d];
     for (uint32_t d = 0; d < ctx->n_taxa; d++) books_sum[d] += books[d];
   }
@@ -3605,22 +3542,21 @@ int kuq_reset_counts(kuq_ctx *ctx) {
   if (!ctx->finalized) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  { int hrc = harvest_seen(ctx, true); if (hrc) return hrc; }
+  int rc = harvest_seen(ctx, true);
+  if (rc) return rc;
   CU(cudaMemset(ctx->d_regs, 0, (uint64_t)ctx->n_sketch * HLL_M));
   CU(cudaMemset(ctx->d_dense_flag, 0, ctx->n_sketch));
   CU(cudaMemset(ctx->d_n_kmers, 0, ctx->n_sketch * 8ull));
   CU(cudaMemset(ctx->d_n_reads, 0, ctx->n_taxa * 8ull));
-  if (ctx->d_sparse_slots) {
-    CU(cudaMemset(ctx->d_sparse_slots, 0, ctx->sparse_cap * 8ull));
+  if (ctx->sparse.slots) {
     CU(cudaMemset(ctx->d_sparse_used, 0, 8));
-    CU(cudaMemset(ctx->d_sparse_distinct, 0, ctx->n_sketch * 4ull));
-    ctx->direct_upper = 0;
+    rc = clear_table(ctx, ctx->sparse);
+    if (rc) return rc;
     ctx->set_has_hits = false;
   }
-  if (ctx->d_exact) {
-    CU(cudaMemset(ctx->d_exact, 0, ctx->exact_cap * 16ull));
-    CU(cudaMemset(ctx->d_exact_count, 0, ctx->n_sketch * 8ull));
-    ctx->exact_upper = 0;
+  if (ctx->exact.slots) {
+    rc = clear_table(ctx, ctx->exact);
+    if (rc) return rc;
     ctx->exact_partitioned = false;
     ctx->merged_exact = false;
   }

@@ -1376,21 +1376,27 @@ void launch_sparse_union(const KeySource &src, const uint8_t *member,
   if (src.n) k_sparse_union<<<device_sm_count() * 16, 256, 0, stream>>>(src, member, scratch_set, scratch_mask, hist64, overflow);
 }
 
+// The kept items of the active lanes go to out[*n_out ...]: one cursor atomic per warp.  *n_out counts them also beyond
+// out_cap.
+template <typename Item>
+__device__ __forceinline__ void warp_append(bool keep, const Item &item, Item *out, uint64_t out_cap, unsigned long long *n_out) {
+  const uint32_t m = __ballot_sync(__activemask(), keep);
+  if (!keep) return;
+  const uint32_t lane = threadIdx.x & 31;
+  unsigned long long base = 0;
+  const int leader = __ffs(m) - 1;
+  if ((int)lane == leader) base = atomicAdd(n_out, (unsigned long long)__popc(m));
+  base = __shfl_sync(m, base, leader);
+  const unsigned long long pos = base + __popc(m & ((1u << lane) - 1));
+  if (pos < out_cap) out[pos] = item;
+}
+
 // export / import of the sparse tier (cross-GPU union of the (taxon, code) sets)
 __global__ void k_sparse_export(const KeySource src, const uint8_t *dense_flag,
                                 unsigned long long *out, uint64_t out_cap, unsigned long long *n_out) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < src.n; i += (uint64_t)gridDim.x * blockDim.x) {
     const unsigned long long key = source_key(src, i);
-    const bool keep = key && !dense_flag[(uint32_t)(key >> 32) - 1];
-    const uint32_t m = __ballot_sync(__activemask(), keep);
-    if (!keep) continue;
-    const uint32_t lane = threadIdx.x & 31;
-    unsigned long long base = 0;
-    const int leader = __ffs(m) - 1;
-    if ((int)lane == leader) base = atomicAdd(n_out, (unsigned long long)__popc(m));
-    base = __shfl_sync(m, base, leader);
-    const unsigned long long pos = base + __popc(m & ((1u << lane) - 1));
-    if (pos < out_cap) out[pos] = key;
+    warp_append(key && !dense_flag[(uint32_t)(key >> 32) - 1], key, out, out_cap, n_out);
   }
 }
 __global__ void k_sparse_import(const unsigned long long *keys, uint64_t n, SparseSet s, const uint8_t *dense_flag,
@@ -1448,34 +1454,39 @@ __global__ void __launch_bounds__(256) k_exact_insert(const __grid_constant__ Pa
   }
 }
 
-// the pairs of a table that is being replaced, into the bigger one with exact_insert's probe sequence; every pair is
-// counted already, so count[] stays as it is
-__global__ void k_exact_rehash(const ExactPair *old_slots, uint64_t old_cap, ExactSet e, uint32_t *error_flag) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    const ExactPair pr = old_slots[i];
-    if (!pr.kmer1) continue;
-    if (exact_insert(e, (uint32_t)(pr.taxon1 - 1), pr.kmer1 - 1) < 0) atomicExch(error_flag, 4u);
-  }
+// Slots of the two device tables: a sparse-tier key (0 = empty) or an exact pair (kmer1 0 = empty).
+__device__ __forceinline__ bool occupied(unsigned long long key) { return key != 0; }
+__device__ __forceinline__ bool occupied(const ExactPair &pr) { return pr.kmer1 != 0; }
+__device__ __forceinline__ int reinsert(const SparseSet &s, unsigned long long key) {
+  return sparse_insert(s, (uint32_t)(key >> 32) - 1, (uint32_t)key);
 }
-void launch_exact_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream) {
-  if (old_cap) k_exact_rehash<<<(int)min((uint64_t)device_sm_count() * 16, (old_cap + 255) / 256), 256, 0, stream>>>(old_slots, old_cap, e, error_flag);
+__device__ __forceinline__ int reinsert(const ExactSet &e, const ExactPair &pr) {
+  return exact_insert(e, (uint32_t)(pr.taxon1 - 1), pr.kmer1 - 1);
 }
 
-// occupied slots [lo, hi) → dense pairs: one cursor atomic per warp (out_cap 0 only counts them)
+// the items of an outgrown table into its successor with the table's own probe sequence; every item is counted already,
+// so the per-taxon counters stay as they are
+template <typename Set, typename Item>
+__global__ void k_rehash(const Item *old_slots, uint64_t old_cap, Set s, uint32_t *error_flag) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x) {
+    const Item it = old_slots[i];
+    if (!occupied(it)) continue;
+    if (reinsert(s, it) < 0) atomicExch(error_flag, 4u);
+  }
+}
+void launch_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag, cudaStream_t stream) {
+  if (old_cap) k_rehash<<<device_sm_count() * 16, 256, 0, stream>>>(old_slots, old_cap, s, error_flag);
+}
+void launch_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream) {
+  if (old_cap) k_rehash<<<(int)min((uint64_t)device_sm_count() * 16, (old_cap + 255) / 256), 256, 0, stream>>>(old_slots, old_cap, e, error_flag);
+}
+
+// occupied slots [lo, hi) → dense pairs (out_cap 0 only counts them)
 __global__ void k_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t out_cap,
                                unsigned long long *n_out) {
   for (uint64_t i = lo + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (uint64_t)gridDim.x * blockDim.x) {
     const ExactPair pr = slots[i];
-    const bool keep = pr.kmer1 != 0;
-    const uint32_t m = __ballot_sync(__activemask(), keep);
-    if (!keep) continue;
-    const uint32_t lane = threadIdx.x & 31;
-    unsigned long long base = 0;
-    const int leader = __ffs(m) - 1;
-    if ((int)lane == leader) base = atomicAdd(n_out, (unsigned long long)__popc(m));
-    base = __shfl_sync(m, base, leader);
-    const unsigned long long pos = base + __popc(m & ((1u << lane) - 1));
-    if (pos < out_cap) out[pos] = pr;
+    warp_append(occupied(pr), pr, out, out_cap, n_out);
   }
 }
 // pairs of another context into this table: only the ones it did not hold yet add to count[]
@@ -1495,65 +1506,6 @@ void launch_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, Exact
 }
 void launch_exact_import(const ExactPair *pairs, uint64_t n, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream) {
   if (n) k_exact_import<<<(int)min((uint64_t)device_sm_count() * 16, (n + 255) / 256), 256, 0, stream>>>(pairs, n, e, error_flag);
-}
-
-// Pairs of the slots [lo, hi) grouped by the owner of their k-mer, as k_keys_parts groups sparse-tier keys: the pairs of
-// a tile are ranked on shared-memory counters per part (only occupied slots touch them), and one thread per part and
-// CTA bumps the global cursor once per tile.  pass 0 only counts.
-constexpr int XP_E = 4;      // pairs per thread and tile (16 B each)
-__global__ void __launch_bounds__(256) k_exact_parts(const ExactPair *slots, uint64_t lo, uint64_t hi, uint32_t n_parts,
-                                                     unsigned long long *counters, ExactPair *out,
-                                                     const unsigned long long *part_end, uint32_t *error_flag, int pass) {
-  __shared__ uint32_t s_cnt[EXACT_MAX_PARTS];
-  __shared__ unsigned long long s_base[EXACT_MAX_PARTS];
-  const uint32_t tid = threadIdx.x;
-  if (tid < EXACT_MAX_PARTS) s_cnt[tid] = 0;
-  __syncthreads();
-  const uint64_t tile = (uint64_t)blockDim.x * XP_E;
-  for (uint64_t base = lo + (uint64_t)blockIdx.x * tile; base < hi; base += (uint64_t)gridDim.x * tile) {
-    ExactPair pr[XP_E];
-    uint32_t where[XP_E];                        // part << 24 | rank inside the tile's group of that part
-#pragma unroll
-    for (int j = 0; j < XP_E; j++) {
-      const uint64_t i = base + (uint64_t)j * blockDim.x + tid;
-      pr[j] = ExactPair{0ull, 0ull};
-      if (i < hi) pr[j] = slots[i];
-    }
-#pragma unroll
-    for (int j = 0; j < XP_E; j++) {
-      where[j] = 0;
-      if (pr[j].kmer1) {
-        const uint32_t part = exact_owner(pr[j].kmer1 - 1, n_parts);
-        const uint32_t r = atomicAdd(&s_cnt[part], 1u);
-        where[j] = (part << 24) | r;
-      }
-    }
-    if (pass == 1) {
-      __syncthreads();
-      if (tid < n_parts && s_cnt[tid]) s_base[tid] = atomicAdd(counters + tid, (unsigned long long)s_cnt[tid]);
-      __syncthreads();
-#pragma unroll
-      for (int j = 0; j < XP_E; j++) {
-        if (!pr[j].kmer1) continue;
-        const uint32_t part = where[j] >> 24;
-        const unsigned long long at = s_base[part] + (where[j] & 0xFFFFFFu);
-        if (at < part_end[part]) out[at] = pr[j]; else atomicExch(error_flag, 7u);
-      }
-      __syncthreads();
-      if (tid < EXACT_MAX_PARTS) s_cnt[tid] = 0;
-      __syncthreads();
-    }
-  }
-  if (pass == 0) {
-    __syncthreads();
-    if (tid < n_parts && s_cnt[tid]) atomicAdd(counters + tid, (unsigned long long)s_cnt[tid]);
-  }
-}
-void launch_exact_parts(const ExactPair *slots, uint64_t lo, uint64_t hi, uint32_t n_parts, unsigned long long *counters,
-                        ExactPair *out, const unsigned long long *part_end, uint32_t *error_flag, int pass, cudaStream_t stream) {
-  if (hi <= lo) return;
-  const int grid = (int)min((uint64_t)device_sm_count() * 8, (hi - lo + 256 * XP_E - 1) / (256 * XP_E));
-  k_exact_parts<<<grid, 256, 0, stream>>>(slots, lo, hi, n_parts, counters, out, part_end, error_flag, pass);
 }
 
 // distinct k-mers among the pairs whose taxon is a clade member
@@ -2039,19 +1991,6 @@ void launch_harvest_keep(uint8_t *pairs, uint64_t n_rec, const uint2 *secondarie
   kernel<<<grid, KEEP_THREADS, smem, stream>>>(pairs, n_rec, dense_flag, n_sketch, distinct, n_kept);
 }
 
-// re-insert the keys of an outgrown table into its successor (no per-taxon counting: the keys were counted before)
-__global__ void k_sparse_rehash(const unsigned long long *old_slots, uint64_t old_cap, SparseSet s, uint32_t *error_flag) {
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    const unsigned long long key = old_slots[i];
-    if (!key) continue;
-    if (sparse_insert(s, (uint32_t)(key >> 32) - 1, (uint32_t)key) < 0) atomicExch(error_flag, 4u);
-  }
-}
-void launch_sparse_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag,
-                          cudaStream_t stream) {
-  if (old_cap) k_sparse_rehash<<<device_sm_count() * 16, 256, 0, stream>>>(old_slots, old_cap, s, error_flag);
-}
-
 // C[taxon][v] = number of registers of the taxon holding v (registerHistogram, hyperloglogplus.cpp:337-354);
 // the double-precision Ertl sum over it runs on the host.
 __global__ void k_register_histograms(const uint8_t *regs, uint32_t n_sketch, uint32_t *hist) {
@@ -2209,64 +2148,84 @@ void launch_wait_flags(const unsigned long long *flags, uint32_t n, unsigned lon
 __device__ __forceinline__ uint32_t key_part(unsigned long long key, uint32_t n_parts) {
   return (uint32_t)((mix64((uint32_t)key) >> 33) % n_parts);
 }
-// One kernel for both sources of keys — SRC 0: the slots of the local set, SRC 1: the records a counted hit flagged
-// and the kept records (pass 1 clears SEEN_BIT: the key leaves this GPU instead of entering its set; KEPT_BIT is
-// dropped when the merged keys replace the set, kuq_sparse_replace).  pass 0 counts per part, pass 1
-// scatters through the per-part cursors.  Same-address atomics would serialise hundreds of millions of keys on
-// n_parts counters, so keys are counted / ranked on shared-memory counters (only real keys touch them — most slots are
-// empty and most records unflagged, and a per-part warp vote for every item made the kernel instruction bound), and
-// only one thread per part and CTA touches the global cursor per tile.
+// Items grouped by owner part for the partitioned exports: pass 0 counts per part (counters[part]), pass 1 scatters
+// through the per-part cursors counters[part], bounded by part_end.  Same-address atomics would serialise hundreds of
+// millions of items on n_parts counters, so the items of a tile are counted / ranked on shared-memory counters (only real
+// items touch them — most slots are empty and most records unflagged, and a per-part warp vote for every item made the
+// kernel instruction bound), and only one thread per part and CTA touches the global cursor per tile.
+// A source gives the item type, E items per thread and tile, P part counters, RANK_BITS of a tile rank (the part goes
+// above them), the raw load of item i, the item it makes (an unoccupied one = none) and the item's owner.
 constexpr int KP_E = 8;      // keys per thread and tile: four block-wide barriers per 2048 items instead of per 256
-template <int SRC>
-__global__ void __launch_bounds__(256) k_keys_parts(const unsigned long long *slots, uint8_t *pairs, uint64_t n_items, uint32_t hi_mask,
-                                                    const uint8_t *dense_flag, uint32_t n_parts, unsigned long long *counters,
-                                                    unsigned long long *out, const unsigned long long *part_end, uint32_t *error_flag,
-                                                    int pass) {
-  __shared__ uint32_t s_total32[8];              // pass 0: the CTA's counts (a CTA sees far fewer than 2^32 items)
-  __shared__ uint32_t s_cnt[8];                  // pass 1: keys of the tile per part
-  __shared__ unsigned long long s_base[8];
+constexpr int XP_E = 4;      // pairs per thread and tile (16 B each)
+struct SetKeyParts {         // the slots of the local sparse-tier set
+  using Item = unsigned long long;
+  using Raw = unsigned long long;
+  static constexpr int E = KP_E, P = 8, RANK_BITS = 28;
+  const unsigned long long *slots;
+  const uint8_t *dense_flag;
+  __device__ Raw load(uint64_t i) const { return __ldg(slots + i); }
+  __device__ Item item(Raw k, uint64_t, int) const { return k && dense_flag[(uint32_t)(k >> 32) - 1] ? 0ull : k; }
+  __device__ static uint32_t owner(Item k, uint32_t n_parts) { return key_part(k, n_parts); }
+};
+// the records a counted hit flagged and the kept records: pass 1 clears SEEN_BIT (the key leaves this GPU instead of
+// entering its set); KEPT_BIT is dropped when the merged keys replace the set (kuq_sparse_replace)
+struct RecordKeyParts {
+  using Item = unsigned long long;
+  using Raw = uint32_t;      // the record's high word
+  static constexpr int E = KP_E, P = 8, RANK_BITS = 28;
+  uint8_t *pairs;
+  const uint8_t *dense_flag;
+  uint32_t hi_mask;
+  __device__ Raw load(uint64_t i) const { return __ldg(reinterpret_cast<const uint32_t *>(pairs + i * 12) + 1); }
+  __device__ Item item(Raw hiw, uint64_t i, int pass) const {
+    if (!(hiw & (SEEN_BIT | KEPT_BIT))) return 0ull;
+    uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
+    if (pass == 1 && (hiw & SEEN_BIT)) w[1] = hiw & ~SEEN_BIT;
+    return dense_flag[w[2]] ? 0ull : record_key(w, hiw, hi_mask);
+  }
+  __device__ static uint32_t owner(Item k, uint32_t n_parts) { return key_part(k, n_parts); }
+};
+struct ExactPairParts {      // the slots of the exact k-mer set, owned by exact_owner of their k-mer
+  using Item = ExactPair;
+  using Raw = ExactPair;
+  static constexpr int E = XP_E, P = EXACT_MAX_PARTS, RANK_BITS = 24;
+  const ExactPair *slots;
+  __device__ Raw load(uint64_t i) const { return slots[i]; }
+  __device__ Item item(Raw pr, uint64_t, int) const { return pr; }
+  __device__ static uint32_t owner(const Item &pr, uint32_t n_parts) { return exact_owner(pr.kmer1 - 1, n_parts); }
+};
+
+template <typename S>
+__global__ void __launch_bounds__(256) k_parts(const S src, uint64_t lo, uint64_t hi, uint32_t n_parts, unsigned long long *counters,
+                                               typename S::Item *out, const unsigned long long *part_end, uint32_t *error_flag,
+                                               int pass) {
+  __shared__ uint32_t s_cnt[S::P];               // pass 0: the CTA's items (far fewer than 2^32), pass 1: the tile's
+  __shared__ unsigned long long s_base[S::P];
+  constexpr uint32_t RANK_MASK = (1u << S::RANK_BITS) - 1;
   const uint32_t tid = threadIdx.x;
-  if (tid < 8) { s_total32[tid] = 0; s_cnt[tid] = 0; }
+  if (tid < S::P) s_cnt[tid] = 0;
   __syncthreads();
-  const uint64_t tile = (uint64_t)blockDim.x * KP_E;
-  for (uint64_t base = (uint64_t)blockIdx.x * tile; base < n_items; base += (uint64_t)gridDim.x * tile) {
-    unsigned long long key[KP_E];
-    uint32_t where[KP_E];                        // part << 28 | rank inside the tile's group of that part
-    // all loads of the tile first (KP_E independent requests per thread in flight: the scan is bandwidth work), then
-    // the per-key arithmetic
-    uint32_t hiws[KP_E];
+  const uint64_t tile = (uint64_t)blockDim.x * S::E;
+  for (uint64_t base = lo + (uint64_t)blockIdx.x * tile; base < hi; base += (uint64_t)gridDim.x * tile) {
+    typename S::Raw raw[S::E];
+    typename S::Item item[S::E];
+    uint32_t where[S::E];                        // part << RANK_BITS | rank inside the tile's group of that part
+    // all loads of the tile first (E independent requests per thread in flight: the scan is bandwidth work), then the
+    // per-item arithmetic
 #pragma unroll
-    for (int j = 0; j < KP_E; j++) {
+    for (int j = 0; j < S::E; j++) {
       const uint64_t i = base + (uint64_t)j * blockDim.x + tid;
-      key[j] = 0; hiws[j] = 0;
-      if (i < n_items) {
-        if (SRC == 0) key[j] = __ldg(slots + i);
-        else hiws[j] = __ldg(reinterpret_cast<const uint32_t *>(pairs + i * 12) + 1);
-      }
+      raw[j] = typename S::Raw{};
+      if (i < hi) raw[j] = src.load(i);
     }
 #pragma unroll
-    for (int j = 0; j < KP_E; j++) {
-      const uint64_t i = base + (uint64_t)j * blockDim.x + tid;
-      unsigned long long k = 0;
-      if (i < n_items) {
-        if (SRC == 0) {
-          k = key[j];
-          if (k && dense_flag[(uint32_t)(k >> 32) - 1]) k = 0;
-        } else {
-          uint32_t *w = reinterpret_cast<uint32_t *>(pairs + i * 12);
-          const uint32_t hiw = hiws[j];
-          if (hiw & (SEEN_BIT | KEPT_BIT)) {
-            if (pass == 1 && (hiw & SEEN_BIT)) w[1] = hiw & ~SEEN_BIT;
-            if (!dense_flag[w[2]]) k = record_key(w, hiw, hi_mask);
-          }
-        }
-      }
-      key[j] = k;
+    for (int j = 0; j < S::E; j++) {
+      item[j] = src.item(raw[j], base + (uint64_t)j * blockDim.x + tid, pass);
       where[j] = 0;
-      if (k) {                                   // only real keys cost anything: one shared-memory atomic on the part's counter
-        const uint32_t part = key_part(k, n_parts);
-        if (pass == 0) atomicAdd(&s_total32[part], 1u);
-        else where[j] = (part << 28) | atomicAdd(&s_cnt[part], 1u);
+      if (occupied(item[j])) {                   // only real items cost anything: one shared-memory atomic on the part's counter
+        const uint32_t part = S::owner(item[j], n_parts);
+        if (pass == 0) atomicAdd(&s_cnt[part], 1u);
+        else where[j] = (part << S::RANK_BITS) | atomicAdd(&s_cnt[part], 1u);
       }
     }
     if (pass == 1) {
@@ -2274,29 +2233,39 @@ __global__ void __launch_bounds__(256) k_keys_parts(const unsigned long long *sl
       if (tid < n_parts && s_cnt[tid]) s_base[tid] = atomicAdd(counters + tid, (unsigned long long)s_cnt[tid]);
       __syncthreads();
 #pragma unroll
-      for (int j = 0; j < KP_E; j++) {
-        if (!key[j]) continue;
-        const uint32_t part = where[j] >> 28;
-        const unsigned long long at = s_base[part] + (where[j] & 0x0FFFFFFFu);
-        if (at < part_end[part]) out[at] = key[j]; else atomicExch(error_flag, 7u);
+      for (int j = 0; j < S::E; j++) {
+        if (!occupied(item[j])) continue;
+        const uint32_t part = where[j] >> S::RANK_BITS;
+        const unsigned long long at = s_base[part] + (where[j] & RANK_MASK);
+        if (at < part_end[part]) out[at] = item[j]; else atomicExch(error_flag, 7u);
       }
       __syncthreads();
-      if (tid < 8) s_cnt[tid] = 0;
+      if (tid < S::P) s_cnt[tid] = 0;
       __syncthreads();
     }
   }
   if (pass == 0) {
     __syncthreads();
-    if (tid < n_parts && s_total32[tid]) atomicAdd(counters + tid, (unsigned long long)s_total32[tid]);
+    if (tid < n_parts && s_cnt[tid]) atomicAdd(counters + tid, (unsigned long long)s_cnt[tid]);
   }
+}
+template <typename S>
+void launch_parts(const S &src, uint64_t lo, uint64_t hi, uint32_t n_parts, unsigned long long *counters, typename S::Item *out,
+                  const unsigned long long *part_end, uint32_t *error_flag, int pass, cudaStream_t stream) {
+  if (hi <= lo) return;
+  const int grid = (int)min((uint64_t)device_sm_count() * 8, (hi - lo + 256 * S::E - 1) / (256 * S::E));
+  k_parts<<<grid, 256, 0, stream>>>(src, lo, hi, n_parts, counters, out, part_end, error_flag, pass);
 }
 void launch_keys_parts(int src, const unsigned long long *slots, uint8_t *pairs, uint64_t n_items, uint64_t key_mask,
                        const uint8_t *dense_flag, uint32_t n_parts, unsigned long long *counters, unsigned long long *out,
                        const unsigned long long *part_end, uint32_t *error_flag, int pass, cudaStream_t stream) {
-  if (!n_items) return;
-  const int grid = (int)min((uint64_t)device_sm_count() * 8, (n_items + 256 * KP_E - 1) / (256 * KP_E));
-  if (src == 0) k_keys_parts<0><<<grid, 256, 0, stream>>>(slots, pairs, n_items, (uint32_t)(key_mask >> 32), dense_flag, n_parts, counters, out, part_end, error_flag, pass);
-  else k_keys_parts<1><<<grid, 256, 0, stream>>>(slots, pairs, n_items, (uint32_t)(key_mask >> 32), dense_flag, n_parts, counters, out, part_end, error_flag, pass);
+  if (src == 0) launch_parts(SetKeyParts{slots, dense_flag}, 0, n_items, n_parts, counters, out, part_end, error_flag, pass, stream);
+  else launch_parts(RecordKeyParts{pairs, dense_flag, (uint32_t)(key_mask >> 32)}, 0, n_items, n_parts, counters, out, part_end,
+                    error_flag, pass, stream);
+}
+void launch_exact_parts(const ExactPair *slots, uint64_t lo, uint64_t hi, uint32_t n_parts, unsigned long long *counters,
+                        ExactPair *out, const unsigned long long *part_end, uint32_t *error_flag, int pass, cudaStream_t stream) {
+  launch_parts(ExactPairParts{slots}, lo, hi, n_parts, counters, out, part_end, error_flag, pass, stream);
 }
 
 }  // namespace kuq

@@ -333,8 +333,9 @@ void launch_settle_kept(uint8_t *pairs, const uint2 *secondaries, uint64_t n_sec
 // kuq_collisions.cu: (secondary, primary) record pairs of every (taxon, code) group of the staged records
 int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint64_t *records_of_taxon, uint32_t n_sketch,
                      uint64_t max_entries, uint2 **list_out, uint64_t *n_out, int n_sm, cudaStream_t stream);
-void launch_sparse_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag,
-                          cudaStream_t stream);
+// the items of old_slots[0, old_cap) into a grown table without counting them again
+void launch_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag, cudaStream_t stream);
+void launch_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
 void launch_register_histograms(const uint8_t *regs, uint32_t n_sketch, uint32_t *hist /*[n_sketch][64]*/,
                                 cudaStream_t stream);
 void launch_clade_max(const uint8_t *regs, const uint32_t *members, uint32_t n_members, uint8_t *out4096,
@@ -351,8 +352,6 @@ void launch_sparse_histograms(const KeySource &src, const uint8_t *dense_flag, u
 // exact mode: distinct k-mers over the member taxa (set union of ReadCounts::operator+=, readcounts.hpp:76-81)
 void launch_exact_union(const ExactSet &e, const uint8_t *member, unsigned long long *scratch_set, uint64_t scratch_mask,
                         unsigned long long *n_distinct, uint32_t *overflow, cudaStream_t stream);
-// the pairs of old_slots[0, old_cap) into e without counting them again (growth of the exact set)
-void launch_exact_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
 // occupied slots [lo, hi) compacted into out (order unspecified); *n_out += their number, also beyond out_cap
 void launch_exact_export(const ExactPair *slots, uint64_t lo, uint64_t hi, ExactPair *out, uint64_t out_cap,
                          unsigned long long *n_out, cudaStream_t stream);
