@@ -495,6 +495,14 @@ int kuq_enable_peer_access(kuq_ctx *ctx, kuq_ctx *peer);
 
 /* Dense id ↔ taxid tables (n_taxa entries) for callers that exchange dense ids between GPUs. */
 int kuq_dense_taxids(kuq_ctx *ctx, uint32_t *taxid_of_dense, uint32_t cap, uint32_t *n);
+/* Start a new run on the staged database(s): afterwards the context gives the same results for any later batches and
+ * readouts as a context that was just staged and given the same taxonomy and quick-mode settings (one staging serves
+ * many samples, `classify --sample-sheet`).  Cleared: registers, dense flags, per-taxon k-mer and read counters, the
+ * sparse-tier set (keys, used counter) and the exact k-mer set, the summaries and partitions installed by
+ * kuq_set_sparse_summary / kuq_set_exact_summary / kuq_exact_partition, the SEEN and KEPT bits of every staged record
+ * (one streaming pass over the records, skipped when no record can carry one), the open work unit and the host
+ * snapshot.  Kept, being functions of the staged database alone: the records, the collision table of the record tier
+ * and the grown table capacities (results do not depend on table size).  All slots must be idle. */
 int kuq_reset_counts(kuq_ctx *ctx);
 
 /* Host-side estimator (no device needed): ertlCardinality over 4096 dense registers (hyperloglogplus.cpp:

@@ -691,6 +691,7 @@ class Classifier:
         return out
 
     def reset_counts(self):
+        """Start a new run on the staged database: the context then answers like a freshly staged one (kuq.h)"""
         self._ck(self.L.kuq_reset_counts(self.h))
 
 

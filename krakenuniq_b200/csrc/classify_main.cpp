@@ -13,6 +13,8 @@
 //                                  mates are merged during the ingest; the one deviation is the exit status, EX_DATAERR
 //                                  where the merger stopped at a malformed record or a name mismatch (the wrapper
 //                                  ignores the merger's status and exits 0)
+//   --sample-sheet                 no counterpart: one process stages the database(s) once and classifies every row of
+//                                  the sheet as a separate run would, with kuq_reset_counts between the samples
 // Not supported (exit with a message): -I uid mapping, -x together with several -d databases (the reference's own loop
 // for that combination queries database 0 in every pass, classify.cpp:585-632).
 #include <fcntl.h>
@@ -58,6 +60,8 @@ static bool Quick_mode = false, Print_classified = false, Print_unclassified = f
 static bool Populate_memory = false, Only_classified_kraken_output = false, Print_sequence = false, Map_UIDs = false;
 static bool Paired = false, Check_names = false;  // --paired / --check-names: argv holds one pair of mate files
 static string Pair_error;                         // what read_merger.pl would have died with (the run exits EX_DATAERR)
+static string Sample_sheet;                       // --sample-sheet: the samples of the run, each with its own outputs
+static string Sample_label;                       // the sample being classified (sheet runs), named in error messages
 static uint64_t Populate_memory_size = 0;
 static string Classified_output_file, Unclassified_output_file, Kraken_output_file, Report_output_file, TaxDB_file;
 static size_t Work_unit_size = 500000;      // DEF_WORK_UNIT_SIZE, classify.cpp:38
@@ -71,7 +75,7 @@ static int HLL_PRECISION = 14;              // readcounts.hpp:29 (only selects r
 static unsigned long long total_classified = 0, total_sequences = 0, total_bases = 0;
 
 [[noreturn]] static void die(int code, const string &msg) {
-  cerr << "classify: " << msg << endl;
+  cerr << "classify: " << (Sample_label.empty() ? "" : "sample " + Sample_label + ": ") << msg << endl;
   exit(code);
 }
 
@@ -99,6 +103,9 @@ static void usage(int exit_code = EX_USAGE) {
        << "  --paired         The two files are mates of paired-end reads: each pair is classified as one" << endl
        << "                   sequence mate1 + 'N' + mate2, named after mate 1 (what read_merger.pl writes)" << endl
        << "  --check-names    With --paired: stop at the first pair whose names differ (exit status 65)" << endl
+       << "  --sample-sheet f Classify every sample of the tab-separated sheet f against one staging of the database:" << endl
+       << "                   columns input (files separated by ','), input2 (the mates, with --paired), output," << endl
+       << "                   report, classified_out, unclassified_out (as -o -r -C -U; empty = not written), name" << endl
        << "  -h               Print this message" << endl
        << endl
        << "Kraken output is to standard output by default." << endl;
@@ -127,13 +134,15 @@ static void parse_command_line(int argc, char **argv) {
   int opt;
   long long sig;
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
-  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES };
+  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES, OPT_SAMPLE_SHEET };
   static const struct option long_opts[] = {{"paired", no_argument, NULL, OPT_PAIRED},
-                                            {"check-names", no_argument, NULL, OPT_CHECK_NAMES}, {NULL, 0, NULL, 0}};
+                                            {"check-names", no_argument, NULL, OPT_CHECK_NAMES},
+                                            {"sample-sheet", required_argument, NULL, OPT_SAMPLE_SHEET}, {NULL, 0, NULL, 0}};
   while ((opt = getopt_long(argc, argv, "d:i:t:u:n:m:o:qcC:U:Ma:r:sI:p:x:", long_opts, NULL)) != -1) {
     switch (opt) {
       case OPT_PAIRED: Paired = true; break;
       case OPT_CHECK_NAMES: Check_names = true; break;           // ignored without --paired (krakenuniq:281-283)
+      case OPT_SAMPLE_SHEET: Sample_sheet = optarg; break;
       case 'd': DB_filenames.push_back(optarg); break;
       case 'i': Index_filenames.push_back(optarg); break;
       case 't':
@@ -169,8 +178,116 @@ static void parse_command_line(int argc, char **argv) {
   }
   if (DB_filenames.empty()) { cerr << "Missing mandatory option -d" << endl; usage(); }
   if (Index_filenames.empty()) { cerr << "Missing mandatory option -i" << endl; usage(); }
+  if (!Sample_sheet.empty()) {                      // the sheet names every sample's inputs and outputs
+    if (optind < argc) die(EX_USAGE, "--sample-sheet takes the inputs from the sheet: no input files on the command line");
+    if (!Kraken_output_file.empty() || !Report_output_file.empty() || Print_classified || Print_unclassified)
+      die(EX_USAGE, "--sample-sheet takes the outputs from the sheet: -o, -r, -C and -U are its columns");
+    return;
+  }
   if (Paired && argc - optind != 2) die(EX_USAGE, "--paired requires exactly two filenames");   // krakenuniq:160-161
   if (optind == argc && !Populate_memory) cerr << "No sequence data files specified" << endl;
+}
+
+// ---- samples: the command line's one, or the rows of --sample-sheet ---------------------------------------------
+// A sample's inputs are classified as one run, the inputs of a separate `classify` call: each a file, or with --paired
+// a pair of mate files.  The outputs are the values of -o -r -C -U ("" = the option was not given).
+struct Sample {
+  string name;
+  vector<pair<string, string>> inputs;
+  string kraken, report, classified, unclassified;
+};
+
+static vector<pair<const char *, const char *>> files_of(const Sample &s) {
+  vector<pair<const char *, const char *>> in;
+  for (auto &f : s.inputs) in.emplace_back(f.first.c_str(), f.second.empty() ? NULL : f.second.c_str());
+  return in;
+}
+
+static vector<string> split(const string &s, char sep) {
+  vector<string> v;
+  for (size_t a = 0;;) {
+    const size_t b = s.find(sep, a);
+    v.push_back(s.substr(a, b == string::npos ? string::npos : b - a));
+    if (b == string::npos) return v;
+    a = b + 1;
+  }
+}
+
+// What two paths share when they name one file: device and inode of an existing file, else the absolute path
+static string path_key(const string &p) {
+  struct stat sb;
+  if (stat(p.c_str(), &sb) == 0) return "i" + to_string(sb.st_dev) + ":" + to_string(sb.st_ino);
+  const size_t slash = p.rfind('/');
+  const string dir = slash == string::npos ? "." : slash == 0 ? "/" : p.substr(0, slash);
+  char *real = realpath(dir.c_str(), NULL);
+  const string key = "p" + (real ? string(real) : dir) + "/" + p.substr(slash == string::npos ? 0 : slash + 1);
+  free(real);
+  return key;
+}
+
+// The sheet: tab-separated, a header line naming the columns, then one sample per line; blank lines and lines that start
+// with '#' are skipped.  Every check runs here, before a database is opened, so a bad sheet writes nothing.
+static vector<Sample> read_sample_sheet(const string &path) {
+  ifstream in(path);
+  if (!in.is_open()) die(EX_NOINPUT, "can't open the sample sheet " + path);
+  static const set<string> known = {"input", "input2", "output", "report", "classified_out", "unclassified_out", "name"};
+  map<string, size_t> col;
+  vector<Sample> samples;
+  map<string, string> written;                     // path_key -> which sample writes it
+  set<string> read_keys{path_key(path)};
+  string line;
+  for (size_t line_no = 1; getline(in, line); line_no++) {
+    if (!line.empty() && line.back() == '\r') line.pop_back();
+    if (line.empty() || line[0] == '#') continue;
+    const vector<string> f = split(line, '\t');
+    const string at = path + ":" + to_string(line_no) + ": ";
+    if (col.empty()) {
+      for (size_t i = 0; i < f.size(); i++) {
+        if (!known.count(f[i])) die(EX_USAGE, at + "unknown column '" + f[i] + "' (columns: input input2 output report classified_out unclassified_out name)");
+        if (!col.emplace(f[i], i).second) die(EX_USAGE, at + "column '" + f[i] + "' named twice");
+      }
+      if (!col.count("input")) die(EX_USAGE, at + "the header has no input column");
+      if (Paired && !col.count("input2")) die(EX_USAGE, at + "--paired needs an input2 column with the second mates");
+      if (!Paired && col.count("input2")) die(EX_USAGE, at + "an input2 column needs --paired");
+      continue;
+    }
+    if (f.size() > col.size()) die(EX_USAGE, at + "more cells than the header has columns");
+    auto cell = [&](const char *c) { auto it = col.find(c); return it != col.end() && it->second < f.size() ? f[it->second] : string(); };
+    Sample s;
+    s.name = cell("name").empty() ? to_string(samples.size() + 1) : cell("name");
+    const vector<string> in1 = split(cell("input"), ','), in2 = split(cell("input2"), ',');
+    if (cell("input").empty()) die(EX_USAGE, at + "sample " + s.name + " has no input");
+    if (Paired && (in1.size() != 1 || in2.size() != 1 || in2[0].empty()))
+      die(EX_USAGE, at + "sample " + s.name + ": with --paired, input and input2 each hold one file");
+    for (size_t i = 0; i < in1.size(); i++) {
+      vector<string> files{in1[i]};
+      if (Paired) files.push_back(in2[i]);
+      for (const string &p : files) {
+        if (p.empty()) die(EX_USAGE, at + "sample " + s.name + ": an empty input file name");
+        struct stat sb;
+        if (access(p.c_str(), R_OK) != 0 || stat(p.c_str(), &sb) != 0 || S_ISDIR(sb.st_mode))
+          die(EX_NOINPUT, at + "sample " + s.name + ": can't read input " + p);
+        read_keys.insert(path_key(p));
+      }
+      s.inputs.emplace_back(in1[i], Paired ? in2[i] : string());
+    }
+    // an empty cell: that output is not written (-o off); Kraken lines never go to standard output
+    s.kraken = cell("output").empty() || cell("output") == "-" ? "off" : cell("output");
+    s.report = cell("report");
+    s.classified = cell("classified_out");
+    s.unclassified = cell("unclassified_out");
+    for (const string *o : {&s.kraken, &s.report, &s.classified, &s.unclassified}) {
+      if (o->empty() || *o == "off" || *o == "-") continue;
+      auto w = written.emplace(path_key(*o), s.name);
+      if (!w.second) die(EX_USAGE, at + "samples " + w.first->second + " and " + s.name + " both write " + *o);
+    }
+    samples.push_back(s);
+  }
+  if (col.empty()) die(EX_USAGE, path + ": no header line");
+  if (samples.empty()) die(EX_USAGE, path + ": no samples");
+  for (auto &w : written)
+    if (read_keys.count(w.first)) die(EX_USAGE, "sample " + w.second + " writes to one of the inputs");
+  return samples;
 }
 
 // ---- output streams: plain file, ".gz" → gzip, "-" → stdout (cout_or_file, classify.cpp:133-148) ---------------
@@ -1316,13 +1433,6 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
   return true;
 }
 
-// The inputs of the command line: a FASTA / FASTQ file, or with --paired a pair of mate files
-static vector<pair<const char *, const char *>> inputs(int argc, char **argv) {
-  vector<pair<const char *, const char *>> in;
-  for (int i = optind; i < argc; i += Paired ? 2 : 1) in.emplace_back(argv[i], Paired ? argv[i + 1] : NULL);
-  return in;
-}
-
 // The batches of the inputs, file after file, read one at a time and cut by kuq_batches.h.  A read that closes a batch
 // before itself is held over and starts the next batch.
 struct BatchReader {
@@ -1425,10 +1535,9 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 // windows that no earlier database answered (KUQ_LOOKUP_FILL_EMPTY).  Then the round's batches are resolved and written
 // in input order.  One database keeps the -x rule (one sketch per taxon; batches need not hold whole work units);
 // several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b` without -x.
-static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, uint64_t range_budget,
-                         uint64_t hbm_budget, int argc, char **argv, vector<map<uint32_t, uint64_t>> &db_counts) {
-  const size_t n_db = kdbs.size();
-  const bool unit_rule = n_db > 1;
+// stage_streamed runs once per process: the ranges, the taxids of every record and the pinned registration of the mapped
+// files.  classify_streamed runs once per sample: its rounds of reads, each through every range.
+struct Streamed {
   struct Plan {
     const uint8_t *rec0;
     const uint64_t *offsets;
@@ -1436,10 +1545,22 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     uint32_t k, nt, idx_type;
     vector<pair<uint64_t, uint64_t>> ranges;
   };
-  vector<Plan> plans(n_db);
-  uint64_t max_rec = 1, max_bins = 1;
+  vector<Plan> plans;
+  bool unit_rule = false;
+  uint64_t max_rec = 1, max_bins = 1, round_bytes = 0, batch_nt = 1;
+  vector<const void *> pinned;                                     // registered mappings, unregistered at the end
+  uint32_t open_nt = 0, open_type = 0;                             // parameters the range buffers are open for
+};
+
+static void stage_streamed(Streamed &sm, kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, uint64_t range_budget,
+                           uint64_t hbm_budget, vector<map<uint32_t, uint64_t>> &db_counts) {
+  const size_t n_db = kdbs.size();
+  const bool unit_rule = sm.unit_rule = n_db > 1;
+  vector<Streamed::Plan> &plans = sm.plans;
+  plans.resize(n_db);
+  uint64_t &max_rec = sm.max_rec, &max_bins = sm.max_bins;
   for (size_t d = 0; d < n_db; d++) {
-    Plan &pl = plans[d];
+    Streamed::Plan &pl = plans[d];
     const uint8_t *q = (const uint8_t *)idxs[d].p;
     uint64_t key_bits;
     memcpy(&key_bits, (const uint8_t *)kdbs[d].p + 8, 8);
@@ -1475,8 +1596,8 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
   const uint64_t range_bytes = 2 * (max_rec * 12 + (max_bins + 1) * 8 + 4096);     // 12 B per record in HBM
   const uint64_t free_b = kuq_device_free_bytes(ctx);
   const uint64_t cap = std::min<uint64_t>(hbm_budget, free_b > (2ull << 30) ? free_b - (2ull << 30) : 0);
-  const uint64_t round_bytes = cap > range_bytes ? cap - range_bytes : 0;
-  const uint64_t batch_nt = std::max<uint64_t>(1, std::min<uint64_t>(96ull << 20, round_bytes / 6));
+  const uint64_t round_bytes = sm.round_bytes = cap > range_bytes ? cap - range_bytes : 0;
+  sm.batch_nt = std::max<uint64_t>(1, std::min<uint64_t>(96ull << 20, round_bytes / 6));
   uint64_t db_bytes = 0;                                           // what every round copies to the device
   for (size_t d = 0; d < n_db; d++) db_bytes += kdbs[d].size + idxs[d].size;
   if (round_bytes < db_bytes)
@@ -1486,25 +1607,28 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
   // Mappings registered as pinned memory (the range copies overlap the lookups only from pinned memory), in command-line
   // order while they take at most half of the host's physical memory together: the rest streams from pageable memory
   // rather than page-locking what the reads and the rest of the host need.
-  vector<int> pinned;
   {
     const uint64_t phys = (uint64_t)sysconf(_SC_PHYS_PAGES) * (uint64_t)sysconf(_SC_PAGESIZE);
     uint64_t locked = 0;
     for (size_t d = 0; d < n_db; d++)
-      for (const Mapped *m : {&kdbs[d], &idxs[d]}) {
-        const bool ok = locked + m->size <= phys / 2 && kuq_host_register(m->p, m->size) == KUQ_OK;
-        if (ok) locked += m->size;
-        pinned.push_back(ok);
-      }
+      for (const Mapped *m : {&kdbs[d], &idxs[d]})
+        if (locked + m->size <= phys / 2 && kuq_host_register(m->p, m->size) == KUQ_OK) {
+          locked += m->size;
+          sm.pinned.push_back(m->p);
+        }
   }
   if (Timing) fprintf(stderr, "[timing] streamed: %zu database(s), %llu MiB per round\n", n_db, (unsigned long long)(round_bytes >> 20));
+}
 
-  BatchReader input(inputs(argc, argv), batch_limits(batch_nt, unit_rule, false));
+static void classify_streamed(Streamed &sm, kuq_ctx *ctx, const vector<pair<const char *, const char *>> &files) {
+  const size_t n_db = sm.plans.size();
+  const bool unit_rule = sm.unit_rule;
+  const uint64_t round_bytes = sm.round_bytes;
+  BatchReader input(files, batch_limits(sm.batch_nt, unit_rule, false));
   struct DevBatch { void *bases, *offs, *codes, *units; };
   vector<Batch> round;
   Batch pending;
   bool have_pending = false;
-  uint32_t open_nt = 0, open_type = 0;                             // parameters the range buffers are open for
   size_t n_rounds = 0;
   for (;;) {
     round.clear();
@@ -1540,14 +1664,14 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
       if (kuq_sync_slot(ctx, 0)) die(EX_SOFTWARE, kuq_last_error(ctx));
     }
     for (size_t db = 0; db < n_db; db++) {
-      const Plan &pl = plans[db];
+      const Streamed::Plan &pl = sm.plans[db];
       if (pl.ranges.empty()) continue;                             // a database without records answers nothing
-      if (pl.nt != open_nt || pl.idx_type != open_type) {
+      if (pl.nt != sm.open_nt || pl.idx_type != sm.open_type) {
         // taxonomy and universe are known before the stream opens (the dense numbering is fixed there)
-        if ((open_nt && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, max_rec, max_bins))
+        if ((sm.open_nt && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, sm.max_rec, sm.max_bins))
           die(EX_DATAERR, kuq_last_error(ctx));
-        open_nt = pl.nt;
-        open_type = pl.idx_type;
+        sm.open_nt = pl.nt;
+        sm.open_type = pl.idx_type;
       }
       auto load = [&](uint32_t buf, size_t c) {
         const uint64_t lo = pl.ranges[c].first, hi = pl.ranges[c].second;
@@ -1588,13 +1712,9 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
     }
   }
   if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
-  for (size_t d = 0; d < n_db; d++) {
-    if (pinned[2 * d]) kuq_host_unregister(kdbs[d].p);
-    if (pinned[2 * d + 1]) kuq_host_unregister(idxs[d].p);
-  }
   if (n_db > 1) {
     string per;
-    for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(plans[d].ranges.size());
+    for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(sm.plans[d].ranges.size());
     fprintf(stderr, "\nclassify: %zu databases streamed: %zu rounds, ranges per database %s\n", n_db, n_rounds, per.c_str());
   }
 }
@@ -1611,12 +1731,12 @@ static void run_streamed(kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<
 //   half, with the work-unit ids of the per-work-unit rule (the reference's rule for -d a -d b), so shares hold whole
 //   work units.
 // shard_loop is what both share: batches, id buffers, flags, shares, phases, resolve and output.
-static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool multi, int argc, char **argv) {
+static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool multi, const vector<pair<const char *, const char *>> &files) {
   const int G = (int)ctxs.size();
   const uint64_t R = n_phases;
   vector<Batch> batches;
   {
-    BatchReader input(inputs(argc, argv), batch_limits(96ull << 20, true, false));
+    BatchReader input(files, batch_limits(96ull << 20, true, false));
     for (Batch b; input.next(b);) batches.push_back(std::move(b));
   }
   uint64_t max_bases = 64, max_reads = 4;
@@ -1730,8 +1850,8 @@ static ShardDb shard_db(const Mapped &idx) {
   return ShardDb{(const uint64_t *)(q + 8), q[7], memcmp(q, "KRAKIDX", 7) == 0 ? 1u : 2u};
 }
 
-static void run_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const Mapped &idx, int argc, char **argv,
-                        map<uint32_t, uint64_t> &db_counts) {
+// Staging, once per process; every sample then runs shard_loop with one phase (one database) or one per lookup run
+static void stage_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const Mapped &idx, map<uint32_t, uint64_t> &db_counts) {
   const int G = (int)ctxs.size();
   const vector<uint64_t> cut = plan_shards({shard_db(idx)}, G)[0].cut;
   cerr << "Database sharded over " << G << " GPUs by minimizer range" << endl;
@@ -1753,13 +1873,12 @@ static void run_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const 
       die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
     for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
   }
-  shard_loop(ctxs, 1, false, argc, argv);
 }
 
 // Several databases: every GPU stages, in command-line order, the bins of its range of each database's run (a range may
 // be empty); each database's records per taxid (.counts) are the growth of the staged union it causes, summed over GPUs.
-static void run_sharded_multi(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, int argc,
-                              char **argv, vector<map<uint32_t, uint64_t>> &db_counts) {
+static uint32_t stage_sharded_multi(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs,
+                                    vector<map<uint32_t, uint64_t>> &db_counts) {
   const int G = (int)ctxs.size();
   const size_t n_db = kdbs.size();
   vector<ShardDb> sd;
@@ -1796,7 +1915,7 @@ static void run_sharded_multi(const vector<kuq_ctx *> &ctxs, const vector<Mapped
   uint32_t rows = 0;
   if (kuq_unit_table_rows(ctxs[0], &rows)) die(EX_SOFTWARE, kuq_last_error(ctxs[0]));
   if (rows) Max_units_per_batch = rows;
-  shard_loop(ctxs, (uint32_t)runs.size(), true, argc, argv);
+  return (uint32_t)runs.size();
 }
 
 // What a staged database takes in HBM: 12 bytes per record whatever the file's record size (records of k <= 28 databases
@@ -1813,6 +1932,15 @@ int main(int argc, char **argv) {
   if (DB_filenames.size() != Index_filenames.size()) die(EX_USAGE, "Must specify a index file for each database file");
   const size_t n_db = DB_filenames.size();
   if (n_db > 1 && Populate_memory_size > 0) die(EX_USAGE, "-x with several databases is not supported by the GPU classify");
+  const bool sheet = !Sample_sheet.empty();
+  vector<Sample> samples;
+  if (sheet) {
+    samples = read_sample_sheet(Sample_sheet);
+  } else {
+    Sample s;
+    for (int i = optind; i < argc; i += Paired ? 2 : 1) s.inputs.emplace_back(argv[i], Paired ? argv[i + 1] : "");
+    samples.push_back(s);
+  }
   if (Populate_memory && Populate_memory_size == 0) cerr << "Loading database(s)... " << endl;
   vector<Mapped> kdbs(n_db), idxs(n_db);
   for (size_t i = 0; i < n_db; i++) {
@@ -1828,7 +1956,7 @@ int main(int argc, char **argv) {
       exit(1);
     }
   }
-  if (optind == argc) {                                            // `-M` without inputs: page-cache warm-up idiom
+  if (!sheet && optind == argc) {                                  // `-M` without inputs: page-cache warm-up idiom
     if (Populate_memory && Populate_memory_size == 0) cerr << "\ncomplete." << endl;
     return 0;
   }
@@ -1955,113 +2083,152 @@ int main(int argc, char **argv) {
     if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
     if (rows) Max_units_per_batch = rows;
   }
-  if (Print_classified) Classified_out.open(Classified_output_file);
-  if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);
-  if (!Kraken_output_file.empty()) {
-    if (Kraken_output_file == "off" || Kraken_output_file == "-") Print_kraken = false;   // classify.cpp:233-235
-    else { cerr << "Writing Kraken output to " << Kraken_output_file << endl; Kraken_out.open(Kraken_output_file); }
-  } else {
-    Kraken_out.open("-");
-  }
-
-  struct timeval tv1, tv2;
-  gettimeofday(&tv1, NULL);
-  if (want_shards && n_db == 1) run_sharded(All_ctx, kdb, idx, argc, argv, db_counts[0]);
-  else if (want_shards) run_sharded_multi(All_ctx, kdbs, idxs, argc, argv, db_counts);
-  else if (chunk_budget) run_streamed(ctx, kdbs, idxs, chunk_budget, hbm_budget, argc, argv, db_counts);
-  else for (auto &in : inputs(argc, argv)) process_file(ctx, in.first, in.second);
-  // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
+  // staging of the layouts that stage in pieces (the resident layouts staged above)
+  Streamed streamed;
+  uint32_t shard_phases = 0;
+  if (want_shards && n_db == 1) stage_sharded(All_ctx, kdb, idx, db_counts[0]);
+  else if (want_shards) shard_phases = stage_sharded_multi(All_ctx, kdbs, idxs, db_counts);
+  else if (chunk_budget) stage_streamed(streamed, ctx, kdbs, idxs, chunk_budget, hbm_budget, db_counts);
+#ifdef EXACT_COUNTING
+  // classifyExact on several contexts: the counters join the first context, and the exact k-mer sets are spread over
+  // all contexts by k-mer instead of united on one card, so no card has to hold the union.  The report's clades come
+  // from the roll-up books summed over the parts.  A taxonomy with entries below taxon 0 keeps the union on the first
+  // context: print_report counts those clades one by one, which needs every pair in one place.
   {
-    double T0__ = now_s();
-#ifdef EXACT_COUNTING
-    // classifyExact on several contexts: the counters join the first context, and the exact k-mer sets are spread over
-    // all contexts by k-mer instead of united on one card, so no card has to hold the union.  The report's clades come
-    // from the roll-up books summed over the parts.  A taxonomy with entries below taxon 0 keeps the union on the first
-    // context: print_report counts those clades one by one, which needs every pair in one place.
-    {
-      auto z = tax.idx.find(0);
-      Exact_partitioned = All_ctx.size() > 1 && !(z != tax.idx.end() && !tax.e[z->second].children.empty());
-    }
-    if (Exact_partitioned) {
-      for (size_t g = 1; g < All_ctx.size(); g++)
-        if (kuq_merge_counters_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
-      if (kuq_exact_partition(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
-    }
-#endif
-    for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned; g++)
-      if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
-    if (All_ctx.size() > 1) TICK("merge");
-#ifdef EXACT_COUNTING
-    for (size_t g = 0; g < All_ctx.size() && Timing; g++) {
-      uint64_t slots = 0, pairs = 0, grown = 0;
-      if (kuq_exact_info(All_ctx[g], &slots, &pairs, &grown)) die(EX_SOFTWARE, kuq_last_error(All_ctx[g]));
-      fprintf(stderr, "[timing] exact set of context %zu: %llu slots, %llu pairs, grown %llu times\n", g, (unsigned long long)slots,
-              (unsigned long long)pairs, (unsigned long long)grown);
-    }
-#endif
+    auto z = tax.idx.find(0);
+    Exact_partitioned = All_ctx.size() > 1 && !(z != tax.idx.end() && !tax.e[z->second].children.empty());
   }
-  gettimeofday(&tv2, NULL);
-  {                                                                 // report_stats, classify.cpp:361-375
-    double seconds = get_seconds(tv1, tv2);
-    cerr << "\r";
-    fprintf(stderr, "%llu sequences (%.2f Mbp) processed in %.3fs (%.1f Kseq/m, %.2f Mbp/m).\n", total_sequences,
-            total_bases / 1.0e6, seconds, total_sequences / 1.0e3 / (seconds / 60), total_bases / 1.0e6 / (seconds / 60));
-    fprintf(stderr, "  %llu sequences classified (%.2f%%)\n", total_classified, total_classified * 100.0 / total_sequences);
-    fprintf(stderr, "  %llu sequences unclassified (%.2f%%)\n", total_sequences - total_classified,
-            (total_sequences - total_classified) * 100.0 / total_sequences);
-  }
+#endif
+  bool genome_sizes_read = false;
+  int status = 0;
+  for (size_t si = 0; si < samples.size(); si++) {
+    const Sample &sample = samples[si];
+    if (sheet) {
+      cerr << "classify: sample " << sample.name << " (" << si + 1 << " of " << samples.size() << ")" << endl;
+      Sample_label = sample.name;
+      Kraken_output_file = sample.kraken;
+      Report_output_file = sample.report;
+      Classified_output_file = sample.classified;
+      Unclassified_output_file = sample.unclassified;
+      Print_classified = !sample.classified.empty();
+      Print_unclassified = !sample.unclassified.empty();
+      Print_kraken = true;
+    }
+    if (si) {                                                       // the staged database(s) serve the next sample
+      double T0__ = now_s();
+      for (kuq_ctx *c : All_ctx) if (kuq_reset_counts(c)) die(EX_SOFTWARE, kuq_last_error(c));
+      TICK("reset_counts");
+    }
+    total_classified = total_sequences = total_bases = 0;
+    if (Print_classified) Classified_out.open(Classified_output_file);
+    if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);
+    if (!Kraken_output_file.empty()) {
+      if (Kraken_output_file == "off" || Kraken_output_file == "-") Print_kraken = false;   // classify.cpp:233-235
+      else { cerr << "Writing Kraken output to " << Kraken_output_file << endl; Kraken_out.open(Kraken_output_file); }
+    } else {
+      Kraken_out.open("-");
+    }
 
-  if (!Report_output_file.empty() && Report_output_file != "off") {
+    struct timeval tv1, tv2;
     gettimeofday(&tv1, NULL);
-    cerr << "Writing report file to " << Report_output_file << "  ..\n";
-    for (size_t d = 0; d < n_db; d++) {                             // classify.cpp:262-285, once per database
-    const string fname = DB_filenames[d] + ".counts";
-    bool counts_ok = false;
+    const vector<pair<const char *, const char *>> files = files_of(sample);
+    if (want_shards) shard_loop(All_ctx, n_db == 1 ? 1 : shard_phases, n_db > 1, files);
+    else if (chunk_budget) classify_streamed(streamed, ctx, files);
+    else for (auto &in : files) process_file(ctx, in.first, in.second);
+    // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
     {
-      ifstream ifs(fname);
-      if (ifs.good()) {
-        if (ifs.peek() == ifstream::traits_type::eof()) cerr << "Kmer counts file is empty - trying to regenerate ..." << endl;
-        else counts_ok = true;
+      double T0__ = now_s();
+#ifdef EXACT_COUNTING
+      if (Exact_partitioned) {
+        for (size_t g = 1; g < All_ctx.size(); g++)
+          if (kuq_merge_counters_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+        if (kuq_exact_partition(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
       }
-    }
-    if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
-      cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
-      ofstream ofs(fname);
-      if (n_db == 1 && !chunk_budget && !want_shards && db_taxids(ctx, db_counts[0])) die(EX_SOFTWARE, kuq_last_error(ctx));
-      for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
-    }
-    {
-      cerr << "Reading genome sizes from " << fname << " ...";
-      ifstream in(fname);
-      // readGenomeSizes, taxdb.hpp:868-885, loop kept literally: `while (!eof) { in >> id >> size; set(...) }` counts
-      // the last line of a newline-terminated file twice (the failed extraction leaves the variables unchanged);
-      // the reference's `cov` column depends on it, so the drop-in reproduces it.
-      uint32_t taxid = 0;
-      uint64_t size = 0;
-      while (!in.eof()) {
-        in >> taxid >> size;
-        tax.set_genome_size(taxid, size);
+#endif
+      for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned; g++)
+        if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+      if (All_ctx.size() > 1) TICK("merge");
+#ifdef EXACT_COUNTING
+      for (size_t g = 0; g < All_ctx.size() && Timing; g++) {
+        uint64_t slots = 0, pairs = 0, grown = 0;
+        if (kuq_exact_info(All_ctx[g], &slots, &pairs, &grown)) die(EX_SOFTWARE, kuq_last_error(All_ctx[g]));
+        fprintf(stderr, "[timing] exact set of context %zu: %llu slots, %llu pairs, grown %llu times\n", g, (unsigned long long)slots,
+                (unsigned long long)pairs, (unsigned long long)grown);
       }
-      cerr << " done" << endl;
+#endif
     }
-    }
-    ostringstream rep;
-    double T0__ = now_s();
-    print_report(ctx, tax, rep);
-    TICK("print_report");
-    OutStream ro;
-    ro.open(Report_output_file, true);                              // appended to the wrapper's 2 header lines
-    ro.write(rep.str());
-    ro.close();
     gettimeofday(&tv2, NULL);
-    fprintf(stderr, "Report finished in %.3f seconds.\n", get_seconds(tv1, tv2));
+    {                                                                 // report_stats, classify.cpp:361-375
+      double seconds = get_seconds(tv1, tv2);
+      cerr << "\r";
+      fprintf(stderr, "%llu sequences (%.2f Mbp) processed in %.3fs (%.1f Kseq/m, %.2f Mbp/m).\n", total_sequences,
+              total_bases / 1.0e6, seconds, total_sequences / 1.0e3 / (seconds / 60), total_bases / 1.0e6 / (seconds / 60));
+      fprintf(stderr, "  %llu sequences classified (%.2f%%)\n", total_classified, total_classified * 100.0 / total_sequences);
+      fprintf(stderr, "  %llu sequences unclassified (%.2f%%)\n", total_sequences - total_classified,
+              (total_sequences - total_classified) * 100.0 / total_sequences);
+    }
+
+    if (!Report_output_file.empty() && Report_output_file != "off") {
+      gettimeofday(&tv1, NULL);
+      cerr << "Writing report file to " << Report_output_file << "  ..\n";
+      // the genome sizes are read (and .counts written) once per process, as by the first separate run
+      for (size_t d = 0; d < n_db && !genome_sizes_read; d++) {     // classify.cpp:262-285, once per database
+        const string fname = DB_filenames[d] + ".counts";
+        bool counts_ok = false;
+        {
+          ifstream ifs(fname);
+          if (ifs.good()) {
+            if (ifs.peek() == ifstream::traits_type::eof()) cerr << "Kmer counts file is empty - trying to regenerate ..." << endl;
+            else counts_ok = true;
+          }
+        }
+        if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
+          cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
+          ofstream ofs(fname);
+          if (n_db == 1 && !chunk_budget && !want_shards && db_taxids(ctx, db_counts[0])) die(EX_SOFTWARE, kuq_last_error(ctx));
+          for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
+        }
+        {
+          cerr << "Reading genome sizes from " << fname << " ...";
+          ifstream in(fname);
+          // readGenomeSizes, taxdb.hpp:868-885, loop kept literally: `while (!eof) { in >> id >> size; set(...) }` counts
+          // the last line of a newline-terminated file twice (the failed extraction leaves the variables unchanged);
+          // the reference's `cov` column depends on it, so the drop-in reproduces it.
+          uint32_t taxid = 0;
+          uint64_t size = 0;
+          while (!in.eof()) {
+            in >> taxid >> size;
+            tax.set_genome_size(taxid, size);
+          }
+          cerr << " done" << endl;
+        }
+      }
+      genome_sizes_read = true;
+      ostringstream rep;
+      double T0__ = now_s();
+      print_report(ctx, tax, rep);
+      TICK("print_report");
+      OutStream ro;
+      ro.open(Report_output_file, true);                              // appended to the wrapper's 2 header lines
+      ro.write(rep.str());
+      ro.close();
+      gettimeofday(&tv2, NULL);
+      fprintf(stderr, "Report finished in %.3f seconds.\n", get_seconds(tv1, tv2));
+    }
+    cerr << "Finishing up ..." << endl;
+    Kraken_out.close();
+    Classified_out.close();
+    Unclassified_out.close();
+    // the records before the merger's stop are classified and written, like the wrapper's run on its partial output; the
+    // samples after it still run
+    if (!Pair_error.empty()) {
+      cerr << "classify: " << (sheet ? "sample " + sample.name + ": " : "") << Pair_error << endl;
+      status = EX_DATAERR;
+      Pair_error.clear();
+    }
   }
-  cerr << "Finishing up ..." << endl;
-  Kraken_out.close();
-  Classified_out.close();
-  Unclassified_out.close();
+  Sample_label.clear();
+  for (const void *p : streamed.pinned) kuq_host_unregister((void *)p);
   for (kuq_ctx *c : All_ctx) kuq_destroy(c);
-  // the records before the merger's stop are classified and written, like the wrapper's run on its partial output
-  if (!Pair_error.empty()) { cerr << "classify: " << Pair_error << endl; return EX_DATAERR; }
-  return 0;
+  return status;
 }

@@ -1165,6 +1165,10 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   double settle_ms = 0;
+  if (discard && ctx->keep_dirty) {              // the flags are dropped below (kept is set): settle_kept would be wasted,
+    ctx->keep_dirty = false;                     // only its counter of records kept since then starts over
+    CU(cudaMemsetAsync(ctx->d_harvest_stat + 2, 0, 8, ctx->aux));
+  }
   if (ctx->keep_dirty) {
     int rc = settle_kept(ctx);
     if (rc) return rc;
@@ -3542,8 +3546,11 @@ int kuq_reset_counts(kuq_ctx *ctx) {
   if (!ctx->finalized) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+  // the SEEN / KEPT bits of the records go in one discarding pass, skipped when no record can carry one
   int rc = harvest_seen(ctx, true);
   if (rc) return rc;
+  ctx->kept = false;
+  ctx->kept_keys = 0;
   CU(cudaMemset(ctx->d_regs, 0, (uint64_t)ctx->n_sketch * HLL_M));
   CU(cudaMemset(ctx->d_dense_flag, 0, ctx->n_sketch));
   CU(cudaMemset(ctx->d_n_kmers, 0, ctx->n_sketch * 8ull));
@@ -3552,14 +3559,19 @@ int kuq_reset_counts(kuq_ctx *ctx) {
     CU(cudaMemset(ctx->d_sparse_used, 0, 8));
     rc = clear_table(ctx, ctx->sparse);
     if (rc) return rc;
-    ctx->set_has_hits = false;
   }
   if (ctx->exact.slots) {
     rc = clear_table(ctx, ctx->exact);
     if (rc) return rc;
-    ctx->exact_partitioned = false;
-    ctx->merged_exact = false;
   }
+  ctx->set_has_hits = false;
+  ctx->merged_summary = false;
+  ctx->merged_hist.clear();
+  ctx->merged_distinct.clear();
+  ctx->exact_partitioned = false;
+  ctx->merged_exact = false;
+  ctx->merged_exact_count.clear();
+  ctx->merged_books.clear();
   ctx->units = WorkUnits();
   return KUQ_OK;
 }
