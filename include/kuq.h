@@ -107,6 +107,10 @@ typedef struct kuq_batch_result {
                                   read_offsets[0] + i]; NULL otherwise */
   uint64_t n_classified;       /* reads with call != 0 (total_classified, classify.cpp:541) */
   double kernel_ms;            /* device time of the batch's kernels (CUDA events on the slot's stream) */
+  /* kuq_set_threshold (krakenuniq-filter): NULL when no threshold is set */
+  const uint32_t *filtered_call; /* [n_reads] taxid the call moves up to; 0 = unclassified */
+  const uint32_t *filter_hits;   /* [n_reads] P = filter_hits / filter_total of the last node the walk weighed ... */
+  const uint32_t *filter_total;  /* [n_reads] ... (filter_total = the read's unambiguous k-mers); 0 / 0 = none, P 0 */
 } kuq_batch_result;
 
 /* Device-side view of a slot's outputs after kuq_classify_device / kuq_resolve_device (HBM pointers). */
@@ -206,6 +210,16 @@ int kuq_set_quick_mode(kuq_ctx *ctx, uint32_t min_hits, int stop_at_last_hit);
 
 /* ---- taxonomy: Parent_map (taxdb.hpp:383-398): taxid → parent taxid, 0 for the root / unknown parent --------- */
 int kuq_set_taxonomy(kuq_ctx *ctx, const uint32_t *taxid, const uint32_t *parent_taxid, uint32_t n);
+/* The confidence filter of krakenuniq-filter (scripts/krakenuniq-filter:87-132) on every read of later batches.  taxid /
+ * parent are the taxDB rows in file order; they make the script's parent map F: F[t] = p unless p == t, a later row
+ * with another parent overwrites, and p = 0 is a parent like any other.  A read's call moves up F until the hits at or
+ * below the node (hit taxa whose F-chain passes through it, the node itself included) reach a fraction of at least
+ * threshold - 1e-5 of its unambiguous k-mers (misses count); a node without an F entry ends the walk unweighed.
+ * Quick mode weighs "Q:<hits>" as hits that lie below no node.  The results come in kuq_batch_result's filtered_call /
+ * filter_hits / filter_total; nothing else a batch computes changes.  Call after kuq_set_taxonomy, before the first
+ * batch.  KUQ_E_INVALID_ARG for a threshold outside [0, 1]; KUQ_E_TAXONOMY when F has a cycle (the script would never
+ * end) or gives taxid 0 a parent (the script divides by zero on reads without unambiguous k-mers). */
+int kuq_set_threshold(kuq_ctx *ctx, double threshold, const uint32_t *taxid, const uint32_t *parent, uint32_t n);
 
 /* ---- classification, host buffers (the call a user makes) ----------------------------------------------- */
 /* bases: concatenated sequences exactly as DNASequence::seq holds them (seqreader.hpp:27-32), read r =

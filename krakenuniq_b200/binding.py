@@ -43,7 +43,8 @@ class Run(C.Structure):
 class BatchResult(C.Structure):
     _fields_ = [("n_reads", C.c_uint32), ("reserved0", C.c_uint32), ("call", u32p), ("n_windows", u32p),
                 ("run_start", u32p), ("run_count", u32p), ("runs", C.POINTER(Run)), ("n_runs", C.c_uint64),
-                ("codes", u32p), ("n_classified", C.c_uint64), ("kernel_ms", C.c_double)]
+                ("codes", u32p), ("n_classified", C.c_uint64), ("kernel_ms", C.c_double),
+                ("filtered_call", u32p), ("filter_hits", u32p), ("filter_total", u32p)]
 
 
 class DeviceResult(C.Structure):
@@ -119,6 +120,7 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_export_db_values": (C.c_int, [vp, vp, C.c_uint64]),
         "kuq_set_quick_mode": (C.c_int, [vp, C.c_uint32, C.c_int]),
         "kuq_set_taxonomy": (C.c_int, [vp, u32p, u32p, C.c_uint32]),
+        "kuq_set_threshold": (C.c_int, [vp, C.c_double, u32p, u32p, C.c_uint32]),
         "kuq_classify_batch": (C.c_int, [vp, vp, u64p, C.c_uint32, u32p, C.c_uint32, C.POINTER(BatchResult)]),
         "kuq_submit_batch": (C.c_int, [vp, C.c_uint32, vp, u64p, C.c_uint32, u32p, C.c_uint32]),
         "kuq_wait_batch": (C.c_int, [vp, C.c_uint32, C.POINTER(BatchResult)]),
@@ -336,6 +338,13 @@ class Classifier:
         p = np.ascontiguousarray(parent, np.uint32)
         self._ck(self.L.kuq_set_taxonomy(self.h, _p(t, u32p), _p(p, u32p), len(t)))
 
+    def set_threshold(self, threshold, taxid, parent):
+        """krakenuniq-filter --threshold on every later batch, from the taxDB rows in file order (kuq_set_threshold);
+        results gain filtered_call, filter_hits and filter_total"""
+        t = np.ascontiguousarray(taxid, np.uint32)
+        p = np.ascontiguousarray(parent, np.uint32)
+        self._ck(self.L.kuq_set_threshold(self.h, float(threshold), _p(t, u32p), _p(p, u32p), len(t)))
+
     # ---- host-buffer classification ---------------------------------------------------------------------------
     def _result(self, res: BatchResult, offsets, copy=True):
         n = res.n_reads
@@ -348,6 +357,10 @@ class Classifier:
             runs = np.ctypeslib.as_array(C.cast(res.runs, u32p), shape=(int(res.n_runs) * 2,)) if res.n_runs else \
                 np.zeros(0, np.uint32)
             out["runs"] = runs.reshape(-1, 2)
+        if res.filtered_call:
+            out["filtered_call"] = as_np(res.filtered_call, n, np.uint32)
+            out["filter_hits"] = as_np(res.filter_hits, n, np.uint32)
+            out["filter_total"] = as_np(res.filter_total, n, np.uint32)
         if res.codes:
             total = int(offsets[-1] - offsets[0])
             out["codes"] = as_np(res.codes, total, np.uint32)

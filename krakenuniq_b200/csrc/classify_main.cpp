@@ -62,6 +62,8 @@ static bool Paired = false, Check_names = false;  // --paired / --check-names: a
 static string Pair_error;                         // what read_merger.pl would have died with (the run exits EX_DATAERR)
 static string Sample_sheet;                       // --sample-sheet: the samples of the run, each with its own outputs
 static string Sample_label;                       // the sample being classified (sheet runs), named in error messages
+static bool Filter = false;                       // --threshold: the Kraken lines krakenuniq-filter makes of ours
+static double Threshold = 0;
 static uint64_t Populate_memory_size = 0;
 static string Classified_output_file, Unclassified_output_file, Kraken_output_file, Report_output_file, TaxDB_file;
 static size_t Work_unit_size = 500000;      // DEF_WORK_UNIT_SIZE, classify.cpp:38
@@ -106,6 +108,9 @@ static void usage(int exit_code = EX_USAGE) {
        << "  --sample-sheet f Classify every sample of the tab-separated sheet f against one staging of the database:" << endl
        << "                   columns input (files separated by ','), input2 (the mates, with --paired), output," << endl
        << "                   report, classified_out, unclassified_out (as -o -r -C -U; empty = not written), name" << endl
+       << "  --threshold T    Write the Kraken lines that krakenuniq-filter --threshold T makes of them: each call moves" << endl
+       << "                   up the taxonomy until a fraction T of the read's unambiguous k-mers lies in the clade," << endl
+       << "                   with that fraction as a P= column (-a's taxDB is the filter's taxonomy)" << endl
        << "  -h               Print this message" << endl
        << endl
        << "Kraken output is to standard output by default." << endl;
@@ -134,15 +139,24 @@ static void parse_command_line(int argc, char **argv) {
   int opt;
   long long sig;
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
-  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES, OPT_SAMPLE_SHEET };
+  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES, OPT_SAMPLE_SHEET, OPT_THRESHOLD };
   static const struct option long_opts[] = {{"paired", no_argument, NULL, OPT_PAIRED},
                                             {"check-names", no_argument, NULL, OPT_CHECK_NAMES},
-                                            {"sample-sheet", required_argument, NULL, OPT_SAMPLE_SHEET}, {NULL, 0, NULL, 0}};
+                                            {"sample-sheet", required_argument, NULL, OPT_SAMPLE_SHEET},
+                                            {"threshold", required_argument, NULL, OPT_THRESHOLD}, {NULL, 0, NULL, 0}};
   while ((opt = getopt_long(argc, argv, "d:i:t:u:n:m:o:qcC:U:Ma:r:sI:p:x:", long_opts, NULL)) != -1) {
     switch (opt) {
       case OPT_PAIRED: Paired = true; break;
       case OPT_CHECK_NAMES: Check_names = true; break;           // ignored without --paired (krakenuniq:281-283)
       case OPT_SAMPLE_SHEET: Sample_sheet = optarg; break;
+      case OPT_THRESHOLD: {
+        char *end = NULL;
+        Threshold = strtod(optarg, &end);
+        if (end == optarg || *end) die(EX_USAGE, string("--threshold: not a number: '") + optarg + "'");
+        if (!(Threshold >= 0 && Threshold <= 1)) die(EX_USAGE, "threshold must be in the interval [0,1].");   // krakenuniq-filter:55-58
+        Filter = true;
+        break;
+      }
       case 'd': DB_filenames.push_back(optarg); break;
       case 'i': Index_filenames.push_back(optarg); break;
       case 't':
@@ -176,6 +190,8 @@ static void parse_command_line(int argc, char **argv) {
       default: usage(); break;
     }
   }
+  // the filter keeps five columns of a Kraken line (krakenuniq-filter:131): the sequence column would silently go
+  if (Filter && Print_sequence) die(EX_USAGE, "--threshold cannot be combined with -s");
   if (DB_filenames.empty()) { cerr << "Missing mandatory option -d" << endl; usage(); }
   if (Index_filenames.empty()) { cerr << "Missing mandatory option -i" << endl; usage(); }
   if (!Sample_sheet.empty()) {                      // the sheet names every sample's inputs and outputs
@@ -622,6 +638,7 @@ struct TaxEntry {
 struct TaxDB {
   vector<TaxEntry> e;
   unordered_map<uint32_t, int> idx;
+  vector<uint32_t> row_ids, row_parents;   // every row in file order (krakenuniq-filter's parent map, kuq_set_threshold)
   void read(const string &path) {
     ifstream in(path);
     if (!in.is_open()) die(EX_NOINPUT, "unable to open taxonomy index file " + path);
@@ -636,6 +653,8 @@ struct TaxDB {
       t.id = (uint32_t)strtoul(line.substr(0, a).c_str(), NULL, 10);
       uint32_t par = (uint32_t)strtoul(line.substr(a + 1, b - a - 1).c_str(), NULL, 10);
       if (t.id > 1 && t.id == par) die(1, "ERROR: the parent of " + to_string(t.id) + " is itself. Should not happend for taxa other than the root.");
+      row_ids.push_back(t.id);
+      row_parents.push_back(par);
       t.name = line.substr(b + 1, c == string::npos ? string::npos : c - b - 1);
       t.rank = c == string::npos ? "" : line.substr(c + 1);
       if (idx.count(t.id)) continue;                                // entries.insert keeps the first
@@ -835,7 +854,8 @@ static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_res
     size_t need = 0;
     for (size_t i = a; i < b; i++) {
       const ReadView v = view_of(i);
-      need += 2 + v.hdr_len + 1 + 10 + 1 + 20 + 1 + 4 + 22ull * res.run_count[i - res0] + 1 + (Print_sequence ? v.len + 1 : 0);
+      need += 2 + v.hdr_len + 1 + 10 + 1 + 20 + 1 + 4 + 22ull * res.run_count[i - res0] + 1 + (Print_sequence ? v.len + 1 : 0) +
+              (Filter ? 16 : 0);
     }
     kraken.resize(at + need);
   }
@@ -859,7 +879,9 @@ static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_res
     }
     if (!Print_kraken) continue;
     if (!call && Only_classified_kraken_output) continue;            // :986-988
-    *o++ = call ? 'C' : 'U'; *o++ = '\t';
+    // --threshold: krakenuniq-filter's line (:131-133), "%s\t<id>\t<new taxon>\t<len>\tP=%0.3f\t<hit list>\n"
+    const uint32_t shown = Filter ? res.filtered_call[r] : call;
+    *o++ = shown ? 'C' : 'U'; *o++ = '\t';
     {   // id = first whitespace-delimited token of the header line
       size_t x = 0;
       while (x < v.hdr_len && isspace((unsigned char)v.hdr[x])) x++;
@@ -868,10 +890,14 @@ static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_res
       memcpy(o, v.hdr + x, y - x); o += y - x;
     }
     *o++ = '\t';
-    put(call);
+    put(shown);
     *o++ = '\t';
     put(v.len);
     *o++ = '\t';
+    if (Filter) {
+      const uint32_t den = res.filter_total[r];
+      o += snprintf(o, 12, "P=%.3f\t", den ? (double)res.filter_hits[r] / den : 0.0);
+    }
     if (Quick_mode) { *o++ = 'Q'; *o++ = ':'; put(res.run_count[r]); }   // :989-990
     else if (res.run_count[r] == 0) { *o++ = '0'; *o++ = ':'; *o++ = '0'; }   // :994-995
     for (uint32_t j = 0; !Quick_mode && j < res.run_count[r]; j++) {
@@ -2077,6 +2103,9 @@ int main(int argc, char **argv) {
     tax.parent_map(ids, parents);
     for (kuq_ctx *c : All_ctx)
       if (kuq_set_taxonomy(c, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(c));
+    for (kuq_ctx *c : All_ctx)
+      if (Filter && kuq_set_threshold(c, Threshold, tax.row_ids.data(), tax.row_parents.data(), (uint32_t)tax.row_ids.size()))
+        die(EX_DATAERR, kuq_last_error(c));
   }
   if (cfg.hll_mode == KUQ_HLL_PRELOAD && !chunk_budget && !want_shards) {   // (streamed / sharded runs ask once their taxa are known)
     uint32_t rows = 0;

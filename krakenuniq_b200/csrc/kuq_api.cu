@@ -57,6 +57,9 @@ struct Slot {
   // pinned host
   uint32_t *h_call = nullptr, *h_nwin = nullptr, *h_run_start = nullptr, *h_run_count = nullptr, *h_codes = nullptr;
   uint32_t *h_unit = nullptr;
+  // confidence filter (kuq_set_threshold): filtered call, hits and total per read, allocated when it is set
+  uint32_t *d_fcall = nullptr, *d_fhits = nullptr, *d_ftotal = nullptr;
+  uint32_t *h_fcall = nullptr, *h_fhits = nullptr, *h_ftotal = nullptr;
   kuq_run *h_runs = nullptr;
   uint64_t h_runs_cap = 0;
   unsigned long long *h_scalars = nullptr;
@@ -148,6 +151,12 @@ struct kuq_ctx {
   uint32_t n_taxa = 0, n_sketch = 0;
   uint32_t *d_parent = nullptr, *d_raw = nullptr;
   uint16_t *d_depth = nullptr;
+  // kuq_set_threshold: krakenuniq-filter's parent map F (taxid → parent) with the F-depth of every node; uploaded in
+  // filter ids (Params::fparent) once the dense numbering exists
+  bool filter_set = false;
+  double threshold = 0;
+  std::unordered_map<uint32_t, uint32_t> f_parent, f_depth;
+  uint32_t *d_fparent = nullptr, *d_fdepth = nullptr, *d_fextra = nullptr;
 
   // per-taxon state
   uint8_t *d_regs = nullptr, *d_dense_flag = nullptr;
@@ -251,6 +260,8 @@ void free_slot(Slot &s) {
   cudaFree(s.u_codes);
   cudaFreeHost(s.h_call); cudaFreeHost(s.h_nwin); cudaFreeHost(s.h_run_start); cudaFreeHost(s.h_run_count);
   cudaFreeHost(s.h_codes); cudaFreeHost(s.h_runs); cudaFreeHost(s.h_scalars); cudaFreeHost(s.h_unit);
+  cudaFree(s.d_fcall); cudaFree(s.d_fhits); cudaFree(s.d_ftotal);
+  cudaFreeHost(s.h_fcall); cudaFreeHost(s.h_fhits); cudaFreeHost(s.h_ftotal);
   if (s.ev_k0) cudaEventDestroy(s.ev_k0);
   if (s.ev_k1) cudaEventDestroy(s.ev_k1);
   if (s.ev_stage[0]) cudaEventDestroy(s.ev_stage[0]);
@@ -279,7 +290,9 @@ void free_tax_state(kuq_ctx *ctx) {
   cudaFree(ctx->d_regs); cudaFree(ctx->d_dense_flag); cudaFree(ctx->d_n_kmers); cudaFree(ctx->d_n_reads);
   cudaFree(ctx->sparse.slots); cudaFree(ctx->d_sparse_used); cudaFree(ctx->sparse.count);
   cudaFree(ctx->exact.slots); cudaFree(ctx->exact.count); cudaFree(ctx->d_exact_pre);
+  cudaFree(ctx->d_fparent); cudaFree(ctx->d_fdepth); cudaFree(ctx->d_fextra);
   ctx->exact.slots = nullptr; ctx->exact.count = nullptr; ctx->d_exact_pre = nullptr;
+  ctx->d_fparent = ctx->d_fdepth = ctx->d_fextra = nullptr;
   ctx->exact_pre.clear();
   ctx->d_parent = ctx->d_raw = nullptr; ctx->d_depth = nullptr; ctx->d_regs = ctx->d_dense_flag = nullptr;
   ctx->d_n_kmers = ctx->d_n_reads = nullptr; ctx->sparse.slots = ctx->d_sparse_used = nullptr;
@@ -848,6 +861,36 @@ int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
       [dst](uint32_t, const ExactPair *pairs, uint64_t m) { return exact_import(dst, pairs, m); });
 }
 
+// krakenuniq-filter's parent map in filter ids: a taxon's dense id, or for taxa of F without one (parents without a
+// taxonomy row, taxa the taxonomy does not have) n_taxa + their index in d_fextra.
+int upload_filter(kuq_ctx *ctx) {
+  std::unordered_map<uint32_t, uint32_t> extra;
+  std::vector<uint32_t> extra_raw;
+  auto id_of = [&](uint32_t t) {
+    auto it = ctx->dense_of_raw.find(t);
+    if (it != ctx->dense_of_raw.end()) return it->second;
+    auto ins = extra.emplace(t, ctx->n_taxa + (uint32_t)extra_raw.size());
+    if (ins.second) extra_raw.push_back(t);
+    return ins.first->second;
+  };
+  for (auto &kv : ctx->f_parent) { id_of(kv.first); id_of(kv.second); }
+  const uint64_t n = (uint64_t)ctx->n_taxa + extra_raw.size();
+  std::vector<uint32_t> parent(n, 0), depth(n, 0);
+  for (auto &kv : ctx->f_parent) {
+    const uint32_t i = id_of(kv.first);
+    parent[i] = id_of(kv.second);
+    depth[i] = ctx->f_depth[kv.first];
+  }
+  extra_raw.push_back(0);                             // never an empty allocation
+  CU(dmalloc(&ctx->d_fparent, n));
+  CU(dmalloc(&ctx->d_fdepth, n));
+  CU(dmalloc(&ctx->d_fextra, extra_raw.size()));
+  CU(cudaMemcpy(ctx->d_fparent, parent.data(), n * 4, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(ctx->d_fdepth, depth.data(), n * 4, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(ctx->d_fextra, extra_raw.data(), extra_raw.size() * 4, cudaMemcpyHostToDevice));
+  return KUQ_OK;
+}
+
 // Dense numbering: 0 = "no taxon", 1 = taxid 1 (the reference's hard-wired root, krakenutil.cpp:96,106), then every
 // taxid stored in database records (these own HLL sketches), then the remaining taxonomy nodes; each group
 // ascending by taxid.  Builds the flattened Parent_map and uploads everything.
@@ -942,7 +985,7 @@ int finalize(kuq_ctx *ctx) {
     if (rc) return rc;
   }
   ctx->finalized = true;
-  return KUQ_OK;
+  return ctx->filter_set ? upload_filter(ctx) : KUQ_OK;
 }
 
 // rewrite the staged record values taxid → dense id (once per staged range or appended database)
@@ -1359,6 +1402,15 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   p.sparse = set_view(ctx, ctx->sparse);
   p.exact = set_view(ctx, ctx->exact);
   set_unit_ptrs(p, s);
+  if (ctx->filter_set) {
+    p.fparent = ctx->d_fparent;
+    p.fdepth = ctx->d_fdepth;
+    p.fextra = ctx->d_fextra;
+    p.fmin = ctx->threshold - 1e-5;                  // krakenuniq-filter:126, in double like the script
+    p.fcall = s.d_fcall;
+    p.fhits = s.d_fhits;
+    p.ftotal = s.d_ftotal;
+  }
 }
 
 // The staged databases in the order they are asked, each with its own minimizer range.  A run = consecutive databases
@@ -1882,8 +1934,72 @@ int kuq_set_taxonomy(kuq_ctx *ctx, const uint32_t *taxid, const uint32_t *parent
   return KUQ_OK;
 }
 
+int kuq_set_threshold(kuq_ctx *ctx, double threshold, const uint32_t *taxid, const uint32_t *parent, uint32_t n) {
+  if (!ctx || ((!taxid || !parent) && n)) return KUQ_E_INVALID_ARG;
+  if (!(threshold >= 0 && threshold <= 1)) return fail(ctx, KUQ_E_INVALID_ARG, "threshold must be in the interval [0,1]");
+  if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "kuq_set_threshold: set the taxonomy first");
+  if (ctx->filter_set) return fail(ctx, KUQ_E_STATE, "the threshold is already set");
+  for (auto &s : ctx->slots)
+    if (s.busy) return fail(ctx, KUQ_E_STATE, "the threshold cannot be set while a batch is in flight");
+  // F (krakenuniq-filter:136-146): rows in file order, `$parent_map{$taxID} = $parentTaxID unless $parentTaxID == $taxID`
+  std::unordered_map<uint32_t, uint32_t> F, depth;
+  for (uint32_t i = 0; i < n; i++)
+    if (parent[i] != taxid[i]) F[taxid[i]] = parent[i];
+  if (F.count(0)) return fail(ctx, KUQ_E_TAXONOMY, "taxid 0 has parent %u in the taxonomy: the filter would divide by zero", F[0]);
+  // F-depth = steps until a node without an F entry; a cycle would keep the script's loops going forever
+  std::vector<uint32_t> stack;
+  std::unordered_map<uint32_t, bool> on_stack;
+  for (auto &kv : F) {
+    uint32_t x = kv.first;
+    stack.clear();
+    while (F.count(x) && !depth.count(x)) {
+      if (on_stack[x]) return fail(ctx, KUQ_E_TAXONOMY, "cycle in the parents of the taxonomy at taxid %u", x);
+      on_stack[x] = true;
+      stack.push_back(x);
+      x = F[x];
+    }
+    uint32_t d = F.count(x) ? depth[x] : 0;
+    while (!stack.empty()) { depth[stack.back()] = ++d; on_stack[stack.back()] = false; stack.pop_back(); }
+  }
+  CU(cudaSetDevice(ctx->device));
+  const uint64_t mr = ctx->cfg.max_reads_per_batch;
+  for (auto &s : ctx->slots) {
+    CU(dmalloc(&s.d_fcall, mr));
+    CU(dmalloc(&s.d_fhits, mr));
+    CU(dmalloc(&s.d_ftotal, mr));
+    CU(hmalloc(&s.h_fcall, mr));
+    CU(hmalloc(&s.h_fhits, mr));
+    CU(hmalloc(&s.h_ftotal, mr));
+  }
+  ctx->f_parent.swap(F);
+  ctx->f_depth.swap(depth);
+  ctx->threshold = threshold;
+  ctx->filter_set = true;
+  return ctx->finalized ? upload_filter(ctx) : KUQ_OK;
+}
+
 // ---- classification -------------------------------------------------------------------------------------------
 namespace {
+// D2H of a batch's fixed-size results; the variable-size hit lists follow in kuq_wait_batch
+int copy_results(kuq_ctx *ctx, Slot &s) {
+  const uint64_t n = s.n_reads;
+  if (n) {
+    CU(cudaMemcpyAsync(s.h_call, s.d_call, n * 4, cudaMemcpyDeviceToHost, s.stream));
+    CU(cudaMemcpyAsync(s.h_nwin, s.d_nwin, n * 4, cudaMemcpyDeviceToHost, s.stream));
+    if (!(s.flags & KUQ_F_NO_RUNS) || ctx->quick_min) {
+      CU(cudaMemcpyAsync(s.h_run_start, s.d_run_start, n * 4, cudaMemcpyDeviceToHost, s.stream));
+      CU(cudaMemcpyAsync(s.h_run_count, s.d_run_count, n * 4, cudaMemcpyDeviceToHost, s.stream));
+    }
+    if (ctx->filter_set) {
+      CU(cudaMemcpyAsync(s.h_fcall, s.d_fcall, n * 4, cudaMemcpyDeviceToHost, s.stream));
+      CU(cudaMemcpyAsync(s.h_fhits, s.d_fhits, n * 4, cudaMemcpyDeviceToHost, s.stream));
+      CU(cudaMemcpyAsync(s.h_ftotal, s.d_ftotal, n * 4, cudaMemcpyDeviceToHost, s.stream));
+    }
+  }
+  CU(cudaMemcpyAsync(s.h_scalars, s.d_scalars, 8 * 8, cudaMemcpyDeviceToHost, s.stream));
+  return KUQ_OK;
+}
+
 // copy one batch of reads (host) into the slot; returns the total number of bases
 int upload_reads(kuq_ctx *ctx, Slot &s, const char *bases, const uint64_t *read_offsets, uint32_t n_reads, uint64_t *total_out) {
   if (n_reads > ctx->cfg.max_reads_per_batch) return fail(ctx, KUQ_E_CAPACITY, "%u reads > slot capacity %u", n_reads, ctx->cfg.max_reads_per_batch);
@@ -1962,15 +2078,8 @@ int kuq_resolve_batch(kuq_ctx *ctx, const char *bases, const uint64_t *read_offs
   p.codes_in = s.d_codes_in;
   rc = launch_on_slot(ctx, s, MODE_RESOLVE, p);
   if (rc) return rc;
-  if (n_reads) {
-    CU(cudaMemcpyAsync(s.h_call, s.d_call, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    CU(cudaMemcpyAsync(s.h_nwin, s.d_nwin, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    if (!(flags & KUQ_F_NO_RUNS) || ctx->quick_min) {
-      CU(cudaMemcpyAsync(s.h_run_start, s.d_run_start, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-      CU(cudaMemcpyAsync(s.h_run_count, s.d_run_count, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    }
-  }
-  CU(cudaMemcpyAsync(s.h_scalars, s.d_scalars, 8 * 8, cudaMemcpyDeviceToHost, s.stream));
+  rc = copy_results(ctx, s);
+  if (rc) return rc;
   s.busy = true;
   return kuq_wait_batch(ctx, 0, out);
 }
@@ -2001,15 +2110,8 @@ int kuq_submit_batch(kuq_ctx *ctx, uint32_t slot, const char *bases, const uint6
   rc = launch_on_slot(ctx, s, MODE_FUSED, p);
   if (rc) return rc;
   // D2H of the fixed-size results; the variable-size hit lists follow in kuq_wait_batch
-  if (n_reads) {
-    CU(cudaMemcpyAsync(s.h_call, s.d_call, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    CU(cudaMemcpyAsync(s.h_nwin, s.d_nwin, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    if (!(flags & KUQ_F_NO_RUNS) || ctx->quick_min) {
-      CU(cudaMemcpyAsync(s.h_run_start, s.d_run_start, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-      CU(cudaMemcpyAsync(s.h_run_count, s.d_run_count, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    }
-  }
-  CU(cudaMemcpyAsync(s.h_scalars, s.d_scalars, 8 * 8, cudaMemcpyDeviceToHost, s.stream));
+  rc = copy_results(ctx, s);
+  if (rc) return rc;
   s.busy = true;
   return KUQ_OK;
 }
@@ -2058,6 +2160,11 @@ int kuq_wait_batch(kuq_ctx *ctx, uint32_t slot, kuq_batch_result *out) {
   out->codes = (s.flags & KUQ_F_WANT_CODES) ? s.h_codes : nullptr;
   out->n_classified = s.h_scalars[1];
   out->kernel_ms = s.kernel_ms;
+  if (ctx->filter_set) {
+    out->filtered_call = s.h_fcall;
+    out->filter_hits = s.h_fhits;
+    out->filter_total = s.h_ftotal;
+  }
   return KUQ_OK;
 }
 
@@ -2218,16 +2325,8 @@ int kuq_collect_device_batch(kuq_ctx *ctx, uint32_t slot, kuq_batch_result *out)
   CU(cudaSetDevice(ctx->device));
   Slot &s = ctx->slots[slot];
   if (s.busy) return fail(ctx, KUQ_E_STATE, "slot %u still has an unread batch", slot);
-  const uint32_t n_reads = s.n_reads;
-  if (n_reads) {
-    CU(cudaMemcpyAsync(s.h_call, s.d_call, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    CU(cudaMemcpyAsync(s.h_nwin, s.d_nwin, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    if (!(s.flags & KUQ_F_NO_RUNS) || ctx->quick_min) {
-      CU(cudaMemcpyAsync(s.h_run_start, s.d_run_start, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-      CU(cudaMemcpyAsync(s.h_run_count, s.d_run_count, n_reads * 4ull, cudaMemcpyDeviceToHost, s.stream));
-    }
-  }
-  CU(cudaMemcpyAsync(s.h_scalars, s.d_scalars, 8 * 8, cudaMemcpyDeviceToHost, s.stream));
+  rc = copy_results(ctx, s);
+  if (rc) return rc;
   s.busy = true;
   return kuq_wait_batch(ctx, slot, out);
 }

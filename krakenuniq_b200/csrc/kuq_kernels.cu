@@ -789,8 +789,11 @@ struct OverflowPool {
   uint64_t capacity;              // entries
 };
 
+// FILTER: *tab_out / *cap_out = the read's table (nullptr when the pool is exhausted), which the filter walks next
+template <bool FILTER = false>
 __device__ uint32_t resolve_overflow(const Params &p, const OverflowPool &pool, const uint32_t *codes_src, uint64_t out_base,
-                                     uint32_t nwin, uint32_t unit, bool counting, bool units, uint32_t lane) {
+                                     uint32_t nwin, uint32_t unit, bool counting, bool units, uint32_t lane,
+                                     unsigned long long **tab_out = nullptr, uint32_t *cap_out = nullptr) {
   // capacity: next power of two >= 2 * (upper bound of distinct taxa); distinct taxa <= windows
   // (and <= taxa that own a sketch: only database values can be hits)
   const uint32_t most = min(nwin, p.tax.n_sketch);
@@ -804,6 +807,7 @@ __device__ uint32_t resolve_overflow(const Params &p, const OverflowPool &pool, 
     return 0;
   }
   unsigned long long *tab = pool.mem + 2 * start;
+  if constexpr (FILTER) { *tab_out = tab; *cap_out = cap; }
   for (uint32_t i = lane; i < cap; i += 32) { tab[2 * i] = 0; tab[2 * i + 1] = 0; }
   __syncwarp();
   auto find = [&](uint32_t t) -> int {              // slot of taxon t or -1
@@ -887,6 +891,66 @@ __device__ uint32_t resolve_overflow(const Params &p, const OverflowPool &pool, 
   return acc;
 }
 
+// ---- confidence filter (krakenuniq-filter, scripts/krakenuniq-filter:88-133) ----------------------------------
+// The deepest node that the F-chains of filter ids a and b (F-depths da, db) share, as its F-depth + 1; 0 = none.
+__device__ __forceinline__ uint32_t f_common(const Params &p, uint32_t a, uint32_t da, uint32_t b, uint32_t db) {
+  for (; da > db; da--) a = __ldg(p.fparent + a);
+  for (; db > da; db--) b = __ldg(p.fparent + b);
+  for (; a != b; da--) {
+    if (!da) return 0;
+    a = __ldg(p.fparent + a);
+    b = __ldg(p.fparent + b);
+  }
+  return da + 1;
+}
+
+// Read r's filtered call, warp-collective.  The hit taxa are lane j's (my_t, my_c) for j < n_hits plus the entries of
+// the overflow table tab (cap slots; nullptr = none); `total` starts as the misses (QUICK: the "Q:<hits>" value, with
+// no taxa at all).  hit_sums[a] of a node a on the call's F-chain is the sum of the counts of the hit taxa whose chain
+// shares a node with the call's at a's depth or above: their common node, found once per taxon, decides every step.
+template <bool QUICK>
+__device__ void filter_read(const Params &p, uint32_t r, uint32_t call, uint32_t lane, uint32_t my_t, uint32_t my_c,
+                            uint32_t n_hits, uint32_t total, unsigned long long *tab, uint32_t cap) {
+  const uint32_t dc = __ldg(p.fdepth + call);
+  uint32_t mine = 0;                                            // lane's register entry: common depth + 1
+  if (!QUICK) {
+    uint32_t sum = lane < n_hits ? my_c : 0;
+    if (dc && lane < n_hits) mine = f_common(p, my_t, __ldg(p.fdepth + my_t), call, dc);
+    if (tab) {
+      for (uint32_t s = lane; s < cap; s += 32) {
+        const unsigned long long e = tab[2 * s];
+        if (!e) continue;
+        const uint32_t t = (uint32_t)(e >> 32) - 1;
+        sum += (uint32_t)e;
+        if (dc) tab[2 * s + 1] = f_common(p, t, __ldg(p.fdepth + t), call, dc);   // the score is no longer needed
+      }
+    }
+    total += __reduce_add_sync(0xFFFFFFFFu, sum);
+  }
+  uint32_t node = call, hits = 0, den = 0;
+  for (uint32_t d = dc; d; d--) {                               // while F[node] is defined
+    uint32_t h = 0;
+    if (!QUICK) {
+      h = mine > d ? my_c : 0;
+      if (tab)
+        for (uint32_t s = lane; s < cap; s += 32) {
+          const unsigned long long e = tab[2 * s];
+          if (e && (uint32_t)tab[2 * s + 1] > d) h += (uint32_t)e;
+        }
+      h = __reduce_add_sync(0xFFFFFFFFu, h);
+    }
+    hits = h;
+    den = total;
+    if ((double)h / (double)total >= p.fmin) break;
+    node = __ldg(p.fparent + node);
+  }
+  if (lane == 0) {
+    p.fcall[r] = node < p.tax.n_taxa ? __ldg(p.tax.raw + node) : __ldg(p.fextra + node - p.tax.n_taxa);
+    p.fhits[r] = hits;
+    p.ftotal[r] = den;
+  }
+}
+
 // Stage 3: one warp per read.  hit_counts (classify.cpp:941-942), resolve_tree / lca (krakenutil.cpp:90-118,
 // 149-200), the per-taxon counters (classify.cpp:939,968) and the run-length encoded hit list (:826-861).
 constexpr int RUN_BUF = 96;      // runs buffered per warp before they are flushed to global memory
@@ -895,7 +959,9 @@ constexpr uint32_t RUN_BLOCK = 256;   // run slots a warp takes from the global 
 // QUICK (classify -q): no resolve_tree; hits = min(#hits, quick_min) goes to run_count[] ("Q:hits", :989-990) and the
 // call is the taxon of the last unambiguous window once quick_min hits were seen (:963-964 after k_quick_cut ended
 // the read at that hit; :705-721,737-738 on the -x path, where the last window of the whole read decides).
-template <bool QUICK>
+// FILTER: also the confidence filter of every read (filter_read), a separate instantiation so that runs without one
+// execute the kernels they always did.
+template <bool QUICK, bool FILTER = false>
 __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Params p) {
   __shared__ uint2 s_runs[CTA_WARPS][RUN_BUF];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1031,9 +1097,12 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
 
     // ---- resolve_tree (krakenutil.cpp:149-200) ------------------------------------------------------------
     uint32_t call = 0;
+    unsigned long long *ovf_tab = nullptr;                      // FILTER: the overflow table of the read
+    uint32_t ovf_cap = 0;
     if (overflow) {
       OverflowPool pool{p.ovf_mem, p.ovf_cursor, p.ovf_capacity};
-      call = resolve_overflow(p, pool, codes_src, out_base, nwin, unit, counting, units, lane);
+      if constexpr (FILTER) call = resolve_overflow<true>(p, pool, codes_src, out_base, nwin, unit, counting, units, lane, &ovf_tab, &ovf_cap);
+      else call = resolve_overflow(p, pool, codes_src, out_base, nwin, unit, counting, units, lane);
       n_hits = 0;                                               // counters were booked from the table
     } else if (!QUICK && n_hits == 1) {
       call = __shfl_sync(0xFFFFFFFFu, my_t, 0);                 // a single hit taxon is its own best path
@@ -1077,6 +1146,8 @@ __global__ void __launch_bounds__(256, 4) k_resolve(const __grid_constant__ Para
     }
     const uint32_t call_raw = call ? __ldg(p.tax.raw + call) : 0;
     if (lane == 0) p.call[r] = call_raw;
+    if constexpr (FILTER)
+      filter_read<QUICK>(p, r, call, lane, my_t, my_c, n_hits, QUICK ? min(q_hits, p.quick_min) : n_miss, ovf_tab, ovf_cap);
     // ---- counters: n_kmers per hit taxon (+ misses on taxon 0), n_reads of the call (classify.cpp:939,968) ---
     if (units) {
       // inserts per (work unit, taxon): the necessary condition for a per-unit sketch to convert
@@ -1644,7 +1715,9 @@ int launch_classify(int mode, const Params &p, int n_sm, cudaStream_t stream, cu
   if (stage_events) cudaEventRecord(stage_events[1], stream);
   if (mode != MODE_LOOKUP) {
     const int rgrid = (int)min((uint32_t)n_sm * 4 * 2, (p.n_reads + CTA_WARPS - 1) / CTA_WARPS);
-    if (quick) k_resolve<true><<<rgrid, 256, 0, stream>>>(p);
+    if (p.fcall && quick) k_resolve<true, true><<<rgrid, 256, 0, stream>>>(p);
+    else if (p.fcall) k_resolve<false, true><<<rgrid, 256, 0, stream>>>(p);
+    else if (quick) k_resolve<true><<<rgrid, 256, 0, stream>>>(p);
     else k_resolve<false><<<rgrid, 256, 0, stream>>>(p);
     launches++;
   }

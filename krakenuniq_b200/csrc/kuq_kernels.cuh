@@ -286,6 +286,15 @@ struct Params {
   // set_lcas: 1 = -T (values lca_keep[] stick, pieces with such a taxid overwrite), 2 = -R (values become 0)
   uint32_t lca_flags;
   uint32_t lca_keep[2];         // dense ids of taxids 32630 / 81077 (0 = not in the taxonomy)
+  // confidence filter (kuq_set_threshold; fcall == nullptr = off).  Filter ids: the dense ids, then taxa of the
+  // filter's parent map F that have no dense id (fextra[id - tax.n_taxa] = their taxids)
+  const uint32_t *fparent;      // filter id → filter id of F[t]; meaningful where fdepth > 0
+  const uint32_t *fdepth;       // filter id → F-steps to the end of its chain (0 = no F entry)
+  const uint32_t *fextra;
+  double fmin;                  // threshold - 1e-5
+  uint32_t *fcall;              // [n_reads] taxid the call moves up to
+  uint32_t *fhits;              // [n_reads] hits at or below the last weighed node ...
+  uint32_t *ftotal;             // [n_reads] ... and the read's unambiguous k-mers (0 / 0: no node weighed)
 };
 
 // The fused lookup computes its windows itself from the packed copy of the batch; exact counting and quick-stop runs
