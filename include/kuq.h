@@ -125,7 +125,9 @@ typedef struct kuq_device_result {
 } kuq_device_result;
 
 /* Raw device pointers to the per-taxon state, for the cross-GPU merge the caller performs with NCCL
- * (allreduce MAX over regs, SUM over the counters) when reads or DB ranges are spread over GPUs (SURVEY §8(e)). */
+ * (allreduce MAX over regs, SUM over the counters) when reads or DB ranges are spread over GPUs (SURVEY §8(e)).
+ * Write through them only while no call of the context is in flight: each counting launch takes a lower bound of every
+ * sketch's registers when it starts and relies on the registers not shrinking until it ends. */
 typedef struct kuq_state_ptrs {
   uint8_t *d_regs;             /* [n_sketch][4096] HLL registers, p = 12 (readcounts.hpp:40) */
   uint64_t regs_bytes;
@@ -554,10 +556,14 @@ int kuq_harvest_keep_device(int device, void *d_pairs, uint64_t n_rec, const voi
  * k_lookup<MODE_FUSED> (search + register update) with / without those switches — these two run only on a
  * KUQ_HLL_DENSE_ONLY context (they count the batch's windows into its sketches once per launch; use a throwaway
  * context) and are reported as 0 ms otherwise; 11 = shape 0 with the narrowing step as an if / else-if chain instead
- * of a count of the pivots <= key, 12 = shape 0 fed through the product's parameter block.
- * Needs 8 bytes per record + 4 bytes per position of free device memory.
+ * of a count of the pivots <= key, 12 = shape 0 fed through the product's parameter block, 13 = shape 0 with the
+ * first round's pivots loaded with the L2::256B prefetch-size qualifier, 14 / 15 = shape 0 on a copy of the records
+ * with every bin laid out as a two-level search tree (its pivots at the bin's head, then the leaves in key order;
+ * tree_ms times the copy, tree_unordered counts bins whose keys do not strictly increase) with the tree's header
+ * loaded plainly / with the L2::256B qualifier.
+ * Needs 20 bytes per record + 4 bytes per position of free device memory.
  * Times: CUDA events on the slot's stream, one warm-up launch then `reps` timed ones per variant. */
-#define KUQ_LAYOUT_VARIANTS 22
+#define KUQ_LAYOUT_VARIANTS 25
 typedef struct kuq_layout_result {
   uint64_t n_records, n_positions;
   uint64_t n_windows;                         /* windows looked up in the staged range */
@@ -569,6 +575,8 @@ typedef struct kuq_layout_result {
   uint32_t shape[KUQ_LAYOUT_VARIANTS];        /* see below */
   double best_ms[KUQ_LAYOUT_VARIANTS], mean_ms[KUQ_LAYOUT_VARIANTS];
   uint64_t mismatches[KUQ_LAYOUT_VARIANTS];
+  double tree_ms;
+  uint64_t tree_unordered;
 } kuq_layout_result;
 int kuq_layout_experiment(kuq_ctx *ctx, uint32_t slot, uint64_t n_positions, uint32_t reps, kuq_layout_result *out);
 

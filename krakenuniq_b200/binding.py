@@ -53,12 +53,13 @@ class DeviceResult(C.Structure):
                 ("d_n_runs", C.c_void_p)]
 
 
-LAYOUT_VARIANTS = 22
+LAYOUT_VARIANTS = 25
 LAYOUT_SHAPES = ["thread per window", "product k_lookup<MODE_LOOKUP>", "index prefetch, 8 CTAs/SM", "index prefetch, 6 CTAs/SM",
                  "2 windows per thread, 8 CTAs/SM", "2 windows per thread, 6 CTAs/SM", "2 windows per thread, 4 CTAs/SM",
                  "4 windows per thread, 4 CTAs/SM", "product k_lookup<MODE_LOOKUP>, lean", "product k_lookup<MODE_FUSED>",
                  "product k_lookup<MODE_FUSED>, lean", "thread per window, if-chain narrowing",
-                 "thread per window, product parameter block"]
+                 "thread per window, product parameter block", "thread per window, L2::256B on round 1",
+                 "tree layout", "tree layout, L2::256B on the header"]
 
 
 class LayoutResult(C.Structure):                     # kuq_layout_result
@@ -68,7 +69,7 @@ class LayoutResult(C.Structure):                     # kuq_layout_result
                 ("arity", C.c_uint32 * LAYOUT_VARIANTS), ("window", C.c_uint32 * LAYOUT_VARIANTS),
                 ("shape", C.c_uint32 * LAYOUT_VARIANTS),
                 ("best_ms", C.c_double * LAYOUT_VARIANTS), ("mean_ms", C.c_double * LAYOUT_VARIANTS),
-                ("mismatches", C.c_uint64 * LAYOUT_VARIANTS)]
+                ("mismatches", C.c_uint64 * LAYOUT_VARIANTS), ("tree_ms", C.c_double), ("tree_unordered", C.c_uint64)]
 
 
 class StatePtrs(C.Structure):
@@ -695,6 +696,7 @@ class Classifier:
         self._ck(self.L.kuq_layout_experiment(self.h, slot, n_positions, reps, C.byref(r)))
         out = {"n_records": r.n_records, "n_positions": r.n_positions, "n_windows": r.n_windows,
                "probes_per_window": r.sum_probes / max(r.n_windows, 1), "transcode_ms": r.transcode_ms,
+               "tree_ms": r.tree_ms, "tree_unordered_bins": r.tree_unordered,
                "windows_by_bin_size": dict(zip(["<=8", "<=16", "<=64", "<=256", "<=1024", ">1024"], list(r.bin_class))),
                "variants": []}
         for v in range(r.n_variants):

@@ -160,6 +160,7 @@ struct kuq_ctx {
 
   // per-taxon state
   uint8_t *d_regs = nullptr, *d_dense_flag = nullptr;
+  uint8_t *d_reg_floor = nullptr;         // [n_sketch]: lower bound of each sketch's registers (refresh_reg_floor)
   unsigned long long *d_n_kmers = nullptr, *d_n_reads = nullptr;
   unsigned long long *d_sparse_used = nullptr;
   SparseTable sparse;                     // the sparse-tier set; count[] includes the keys of kept records
@@ -288,13 +289,14 @@ void free_db(kuq_ctx *ctx) {
 void free_tax_state(kuq_ctx *ctx) {
   cudaFree(ctx->d_parent); cudaFree(ctx->d_raw); cudaFree(ctx->d_depth);
   cudaFree(ctx->d_regs); cudaFree(ctx->d_dense_flag); cudaFree(ctx->d_n_kmers); cudaFree(ctx->d_n_reads);
+  cudaFree(ctx->d_reg_floor);
   cudaFree(ctx->sparse.slots); cudaFree(ctx->d_sparse_used); cudaFree(ctx->sparse.count);
   cudaFree(ctx->exact.slots); cudaFree(ctx->exact.count); cudaFree(ctx->d_exact_pre);
   cudaFree(ctx->d_fparent); cudaFree(ctx->d_fdepth); cudaFree(ctx->d_fextra);
   ctx->exact.slots = nullptr; ctx->exact.count = nullptr; ctx->d_exact_pre = nullptr;
   ctx->d_fparent = ctx->d_fdepth = ctx->d_fextra = nullptr;
   ctx->exact_pre.clear();
-  ctx->d_parent = ctx->d_raw = nullptr; ctx->d_depth = nullptr; ctx->d_regs = ctx->d_dense_flag = nullptr;
+  ctx->d_parent = ctx->d_raw = nullptr; ctx->d_depth = nullptr; ctx->d_regs = ctx->d_dense_flag = ctx->d_reg_floor = nullptr;
   ctx->d_n_kmers = ctx->d_n_reads = nullptr; ctx->sparse.slots = ctx->d_sparse_used = nullptr;
   ctx->sparse.count = nullptr;
   ctx->finalized = false;
@@ -963,10 +965,12 @@ int finalize(kuq_ctx *ctx) {
   CU(cudaMemcpy(ctx->d_depth, depth.data(), ctx->n_taxa * 2ull, cudaMemcpyHostToDevice));
   CU(dmalloc(&ctx->d_regs, (uint64_t)ctx->n_sketch * HLL_M));
   CU(dmalloc(&ctx->d_dense_flag, ctx->n_sketch));
+  CU(dmalloc(&ctx->d_reg_floor, ctx->n_sketch));
   CU(dmalloc(&ctx->d_n_kmers, ctx->n_sketch));
   CU(dmalloc(&ctx->d_n_reads, ctx->n_taxa));
   CU(cudaMemset(ctx->d_regs, 0, (uint64_t)ctx->n_sketch * HLL_M));
   CU(cudaMemset(ctx->d_dense_flag, 0, ctx->n_sketch));
+  CU(cudaMemset(ctx->d_reg_floor, 0, ctx->n_sketch));
   CU(cudaMemset(ctx->d_n_kmers, 0, ctx->n_sketch * 8ull));
   CU(cudaMemset(ctx->d_n_reads, 0, ctx->n_taxa * 8ull));
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
@@ -1125,6 +1129,23 @@ int harvest_state(kuq_ctx *ctx) {
   CU(dmalloc(&ctx->d_harvest_stat, 3));
   CU(cudaMemset(ctx->d_harvest_stat, 0, 3 * 8));
   CU(cudaEventCreate(&ctx->harvest_ev[0])); CU(cudaEventCreate(&ctx->harvest_ev[1]));
+  return KUQ_OK;
+}
+
+// Params::reg_floor for a counting launch about to run on `stream`: every sketch's smallest register, so that windows
+// whose hash rank cannot raise a register skip the register load (hll_update).  Registers only grow while kernels
+// run, so a floor taken before the launch stays a lower bound through it, whichever slot refreshed it last; between
+// launches they may be cleared (kuq_reset_counts) or rewritten through kuq_state_ptrs_get, hence a refresh per launch.
+// The pass reads every register: when that is more bytes than the launch's bases the floor is 0 instead (no skip).
+int refresh_reg_floor(kuq_ctx *ctx, uint64_t total_bases, cudaStream_t stream) {
+  if (!ctx->d_reg_floor) return KUQ_OK;
+  if ((uint64_t)ctx->n_sketch * HLL_M <= total_bases) {
+    launch_reg_floor(ctx->d_regs, ctx->n_sketch, ctx->d_reg_floor, stream);
+    ctx->launches++;
+  } else {
+    CU(cudaMemsetAsync(ctx->d_reg_floor, 0, ctx->n_sketch, stream));
+  }
+  CU(cudaGetLastError());
   return KUQ_OK;
 }
 
@@ -1399,6 +1420,7 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
   p.n_kmers = ctx->d_n_kmers;
   p.n_reads_ctr = ctx->d_n_reads;
   p.dense_flag = ctx->d_dense_flag;
+  p.reg_floor = ctx->d_reg_floor;
   p.sparse = set_view(ctx, ctx->sparse);
   p.exact = set_view(ctx, ctx->exact);
   set_unit_ptrs(p, s);
@@ -1531,6 +1553,10 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
   }
   p.packed = windows_packed(mode, p) ? 1u : 0u;
   if (p.n_reads) s.windows_packed = p.packed != 0;
+  if (p.n_reads && !(p.flags & 4u)) {
+    int frc = refresh_reg_floor(ctx, s.total_bases, s.stream);
+    if (frc) return frc;
+  }
   CU(cudaMemsetAsync(s.d_scalars, 0, 8 * 8, s.stream));
   CU(cudaEventRecord(s.ev_k0, s.stream));
   CU(cudaEventRecord(s.ev_stage[0], s.stream));
@@ -3399,11 +3425,13 @@ int kuq_layout_experiment(kuq_ctx *ctx, uint32_t slot, uint64_t n_positions, uin
   fill_params(ctx, s, p, nullptr, nullptr, nullptr, 0, 0);
   // a fused call leaves its windows packed: the variants read scratch
   if (s.windows_packed) launch_unpack_windows(p, n_positions, ctx->n_sm, s.stream);
+  rc = refresh_reg_floor(ctx, s.total_bases, s.stream);     // the fused variants count
+  if (rc) return rc;
   const int erc = layout_experiment(p, ctx->key_ct, s.d_canon, s.d_bins, s.d_dense, n_positions, ctx->n_sm, s.stream, reps,
                                     ctx->cfg.hll_mode == KUQ_HLL_DENSE_ONLY && s.windows_packed, out);
   ctx->snap_valid = false;
-  ctx->launches += 2 + (s.windows_packed ? 1 : 0) + (uint64_t)KUQ_LAYOUT_VARIANTS * (reps + 2ull);
-  if (erc == 1) return fail(ctx, KUQ_E_NOMEM, "not enough free device memory for the transcoded records");
+  ctx->launches += 3 + (s.windows_packed ? 1 : 0) + (uint64_t)KUQ_LAYOUT_VARIANTS * (reps + 2ull);
+  if (erc == 1) return fail(ctx, KUQ_E_NOMEM, "not enough free device memory for the transcoded and tree-ordered records");
   if (erc == 3) return fail(ctx, KUQ_E_CAPACITY, "dense taxon ids need more than 24 bits");
   if (erc) return fail(ctx, KUQ_E_CUDA, "layout experiment: %s", cudaGetErrorString(cudaGetLastError()));
   return KUQ_OK;
@@ -3651,6 +3679,7 @@ int kuq_reset_counts(kuq_ctx *ctx) {
   ctx->kept = false;
   ctx->kept_keys = 0;
   CU(cudaMemset(ctx->d_regs, 0, (uint64_t)ctx->n_sketch * HLL_M));
+  CU(cudaMemset(ctx->d_reg_floor, 0, ctx->n_sketch));
   CU(cudaMemset(ctx->d_dense_flag, 0, ctx->n_sketch));
   CU(cudaMemset(ctx->d_n_kmers, 0, ctx->n_sketch * 8ull));
   CU(cudaMemset(ctx->d_n_reads, 0, ctx->n_taxa * 8ull));

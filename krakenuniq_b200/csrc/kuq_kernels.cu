@@ -65,10 +65,15 @@ __device__ __forceinline__ uint32_t load_val(const uint8_t *pairs, uint64_t pos)
 // Registers are bytes; a byte-wide max is a CAS on the enclosing word, reached only when the plain load says the
 // register would grow (after warm-up almost never: P[grow] ~ 1/n).  A stale load can only be too small, which
 // costs a redundant CAS, never a lost update.
-__device__ __forceinline__ void hll_update(uint8_t *regs, uint32_t taxon, uint64_t hash) {
+// floor[taxon] is at most every register of the sketch (refreshed before each counting launch, registers only grow
+// during one): a rank that low cannot raise any register, so most windows skip the register load, a dependent L2
+// trip once the taxon is known.  Once a sketch has seen a few hashes per register that is most windows (rank <= 3 for
+// 7 in 8 of them).
+__device__ __forceinline__ void hll_update(uint8_t *regs, const uint8_t *floor, uint32_t taxon, uint64_t hash) {
   uint32_t idx = (uint32_t)(hash >> (64 - HLL_P));
   uint64_t rest = hash << HLL_P;
   uint32_t rank = rest ? (uint32_t)__clzll((long long)rest) + 1 : (64 - HLL_P + 1);   // getRank, :140-147
+  if (rank <= __ldg(floor + taxon)) return;
   uint8_t *reg = regs + (size_t)taxon * HLL_M + idx;
   if (*reinterpret_cast<volatile uint8_t *>(reg) >= rank) return;
   uint32_t *word = reinterpret_cast<uint32_t *>(reinterpret_cast<uintptr_t>(reg) & ~(uintptr_t)3);
@@ -622,10 +627,10 @@ __device__ __forceinline__ void lookup_window(const Params &p, uint64_t g, uint3
       p.codes_dense[g] = taxon | kept_new;
     }
     if (MODE == MODE_LOOKUP && shard_counting) {
-      if (taxon != 0 && taxon != FOUND_ZERO) hll_update(p.regs, taxon, fmix64(canon));
+      if (taxon != 0 && taxon != FOUND_ZERO) hll_update(p.regs, p.reg_floor, taxon, fmix64(canon));
     } else if ((counting || (MODE == MODE_RESOLVE && !(flags & 4u))) && !(MODE == MODE_RESOLVE && shard_counting && taxon != 0)) {
       const uint64_t h = fmix64(canon);
-      hll_update(p.regs, taxon, h);
+      hll_update(p.regs, p.reg_floor, taxon, h);
       // direct set insert: misses (taxon 0 has no record to flag) and the resolve half, which only sees merged ids
       if (p.hll_mode != 2u && !(mark_seen && taxon != 0) && !p.dense_flag[taxon]) {
         const int ins = sparse_insert(p.sparse, taxon, encode_hash32(h));
@@ -2143,6 +2148,28 @@ void launch_widen_records(const uint8_t *narrow, uint64_t n_rec, uint32_t key_le
   int grid = (int)min((uint64_t)device_sm_count() * 8, (n_rec + 255) / 256);
   k_widen_records<<<grid, 256, 0, stream>>>(narrow, n_rec, key_len, wide12);
 }
+// one warp per sketch: byte-wise minimum of its 4096 registers
+__global__ void __launch_bounds__(256) k_reg_floor(const uint8_t *__restrict__ regs, uint32_t n_sketch, uint8_t *__restrict__ floor) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < n_sketch; t += warps) {   // warp-uniform
+    const uint4 *r = reinterpret_cast<const uint4 *>(regs + t * HLL_M);
+    uint32_t m = 0xFFFFFFFFu;
+    for (uint32_t i = lane; i < HLL_M / 16; i += 32) {
+      const uint4 v = __ldcg(r + i);
+      m = __vminu4(m, __vminu4(__vminu4(v.x, v.y), __vminu4(v.z, v.w)));
+    }
+    m = min(min(m & 0xFFu, (m >> 8) & 0xFFu), min((m >> 16) & 0xFFu, m >> 24));
+    m = __reduce_min_sync(0xFFFFFFFFu, m);
+    if (lane == 0) floor[t] = (uint8_t)m;
+  }
+}
+
+void launch_reg_floor(const uint8_t *regs, uint32_t n_sketch, uint8_t *floor, cudaStream_t stream) {
+  if (!n_sketch) return;
+  k_reg_floor<<<min((n_sketch + 7) / 8, (uint32_t)device_sm_count() * 8), 256, 0, stream>>>(regs, n_sketch, floor);
+}
+
 void launch_register_histograms(const uint8_t *regs, uint32_t n_sketch, uint32_t *hist, cudaStream_t stream) {
   if (!n_sketch) return;
   k_register_histograms<<<min(n_sketch, (uint32_t)device_sm_count() * 16), 256, 0, stream>>>(regs, n_sketch, hist);

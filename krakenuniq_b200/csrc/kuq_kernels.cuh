@@ -271,6 +271,7 @@ struct Params {
   unsigned long long *n_kmers;  // [n_sketch]
   unsigned long long *n_reads_ctr; // [n_taxa]
   uint8_t *dense_flag;          // [n_sketch]
+  const uint8_t *reg_floor;     // [n_sketch]: at most the smallest register of each sketch (launch_reg_floor)
   SparseSet sparse;
   unsigned long long *n_new_kept;  // F_KEEP: records the batch made kept (k_resolve adds them)
   UnitMap units;
@@ -345,6 +346,8 @@ int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, co
 // the items of old_slots[0, old_cap) into a grown table without counting them again
 void launch_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag, cudaStream_t stream);
 void launch_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
+// floor[t] = the smallest of sketch t's registers
+void launch_reg_floor(const uint8_t *regs, uint32_t n_sketch, uint8_t *floor, cudaStream_t stream);
 void launch_register_histograms(const uint8_t *regs, uint32_t n_sketch, uint32_t *hist /*[n_sketch][64]*/,
                                 cudaStream_t stream);
 void launch_clade_max(const uint8_t *regs, const uint32_t *members, uint32_t n_members, uint8_t *out4096,
