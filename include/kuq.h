@@ -111,6 +111,10 @@ typedef struct kuq_batch_result {
   const uint32_t *filtered_call; /* [n_reads] taxid the call moves up to; 0 = unclassified */
   const uint32_t *filter_hits;   /* [n_reads] P = filter_hits / filter_total of the last node the walk weighed ... */
   const uint32_t *filter_total;  /* [n_reads] ... (filter_total = the read's unambiguous k-mers); 0 / 0 = none, P 0 */
+  /* kuq_set_extract (krakenuniq-extract-reads): NULL / 0 when no extraction is set */
+  const uint8_t *extract_sel;    /* [n_reads] bit 0: the read's Kraken line is selected, XOR KUQ_EXTRACT_INVERT; bit 1: the
+                                    read has no Kraken line (call 0 under KUQ_EXTRACT_CLASSIFIED_ONLY) */
+  uint64_t n_extract;            /* reads of the batch whose Kraken line is selected (before the inversion) */
 } kuq_batch_result;
 
 /* Device-side view of a slot's outputs after kuq_classify_device / kuq_resolve_device (HBM pointers). */
@@ -222,6 +226,26 @@ int kuq_set_taxonomy(kuq_ctx *ctx, const uint32_t *taxid, const uint32_t *parent
  * batch.  KUQ_E_INVALID_ARG for a threshold outside [0, 1]; KUQ_E_TAXONOMY when F has a cycle (the script would never
  * end) or gives taxid 0 a parent (the script divides by zero on reads without unambiguous k-mers). */
 int kuq_set_threshold(kuq_ctx *ctx, double threshold, const uint32_t *taxid, const uint32_t *parent, uint32_t n);
+/* The read selection of krakenuniq-extract-reads (scripts/krakenuniq-extract-reads:60-127) on every read of later
+ * batches.  A read is selected when its Kraken line's taxid (the call, or filtered_call with a threshold) is one of
+ * list[0, n_list), or, with KUQ_EXTRACT_SUBTREE, is reachable from one of them through the taxDB's child graph: taxid /
+ * parent are the taxDB rows in file order, and every row with taxid != parent is an edge parent -> taxid (a taxid with
+ * two rows sits under both parents).  KUQ_EXTRACT_OTHERS (the script's "-1") selects every read that has a Kraken line.
+ * KUQ_EXTRACT_CLASSIFIED_ONLY (`classify -c`): reads with call 0 have no line and are never selected.
+ * KUQ_EXTRACT_INVERT flips bit 0 of extract_sel, not n_extract.  Results in kuq_batch_result's extract_sel /
+ * n_extract; nothing else a batch computes changes.  Call after kuq_set_taxonomy (and kuq_set_threshold, if used),
+ * before the first batch.  KUQ_E_TAXONOMY when KUQ_EXTRACT_SUBTREE is given and a cycle of the child graph is
+ * reachable from a listed taxon (the script's recursion would never end). */
+#define KUQ_EXTRACT_SUBTREE 1u
+#define KUQ_EXTRACT_INVERT 2u
+#define KUQ_EXTRACT_OTHERS 4u
+#define KUQ_EXTRACT_CLASSIFIED_ONLY 8u
+int kuq_set_extract(kuq_ctx *ctx, const uint32_t *list, uint32_t n_list, uint32_t flags, const uint32_t *taxid,
+                    const uint32_t *parent, uint32_t n_rows);
+/* The taxa kuq_set_extract would select (flags: KUQ_EXTRACT_SUBTREE matters), ascending, without a context or a device:
+ * *n_out of them, the first cap written to out (cap = 0: count only).  KUQ_E_TAXONOMY on a reachable cycle. */
+int kuq_extract_taxa(const uint32_t *list, uint32_t n_list, uint32_t flags, const uint32_t *taxid, const uint32_t *parent,
+                     uint32_t n_rows, uint32_t *out, uint32_t cap, uint32_t *n_out);
 
 /* ---- classification, host buffers (the call a user makes) ----------------------------------------------- */
 /* bases: concatenated sequences exactly as DNASequence::seq holds them (seqreader.hpp:27-32), read r =

@@ -20,6 +20,7 @@ CODE_FOUND_ZERO = 0xFFFFFFFD      # KUQ_CODE_FOUND_ZERO: the first database hold
 LOOKUP_FILL_EMPTY = 2             # KUQ_LOOKUP_FILL_EMPTY (lookup_device only_hits)
 HLL_PRELOAD, HLL_CHUNKED, HLL_DENSE_ONLY, HLL_EXACT = 0, 1, 2, 3
 F_WANT_CODES, F_NO_RUNS, F_NO_COUNTS, F_STATS = 1, 2, 4, 8
+EXTRACT_SUBTREE, EXTRACT_INVERT, EXTRACT_OTHERS, EXTRACT_CLASSIFIED_ONLY = 1, 2, 4, 8     # kuq_set_extract flags
 
 u8p, u32p, u64p = C.POINTER(C.c_uint8), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)
 
@@ -44,7 +45,8 @@ class BatchResult(C.Structure):
     _fields_ = [("n_reads", C.c_uint32), ("reserved0", C.c_uint32), ("call", u32p), ("n_windows", u32p),
                 ("run_start", u32p), ("run_count", u32p), ("runs", C.POINTER(Run)), ("n_runs", C.c_uint64),
                 ("codes", u32p), ("n_classified", C.c_uint64), ("kernel_ms", C.c_double),
-                ("filtered_call", u32p), ("filter_hits", u32p), ("filter_total", u32p)]
+                ("filtered_call", u32p), ("filter_hits", u32p), ("filter_total", u32p),
+                ("extract_sel", C.POINTER(C.c_uint8)), ("n_extract", C.c_uint64)]
 
 
 class DeviceResult(C.Structure):
@@ -122,6 +124,8 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_set_quick_mode": (C.c_int, [vp, C.c_uint32, C.c_int]),
         "kuq_set_taxonomy": (C.c_int, [vp, u32p, u32p, C.c_uint32]),
         "kuq_set_threshold": (C.c_int, [vp, C.c_double, u32p, u32p, C.c_uint32]),
+        "kuq_set_extract": (C.c_int, [vp, u32p, C.c_uint32, C.c_uint32, u32p, u32p, C.c_uint32]),
+        "kuq_extract_taxa": (C.c_int, [u32p, C.c_uint32, C.c_uint32, u32p, u32p, C.c_uint32, u32p, C.c_uint32, u32p]),
         "kuq_classify_batch": (C.c_int, [vp, vp, u64p, C.c_uint32, u32p, C.c_uint32, C.POINTER(BatchResult)]),
         "kuq_submit_batch": (C.c_int, [vp, C.c_uint32, vp, u64p, C.c_uint32, u32p, C.c_uint32]),
         "kuq_wait_batch": (C.c_int, [vp, C.c_uint32, C.POINTER(BatchResult)]),
@@ -224,6 +228,23 @@ def exported_symbols():
     hdr = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "kuq.h")).read()
     hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     return sorted(set(re.findall(r"\b(kuq_[a-z0-9_]+)\s*\(", hdr)))
+
+
+def extract_taxa(taxa, flags, taxid=(), parent=()):
+    """the taxa kuq_set_extract selects (kuq_extract_taxa; no device needed), ascending"""
+    L = load_library()
+    l = np.ascontiguousarray(taxa, np.uint32)
+    t = np.ascontiguousarray(taxid, np.uint32)
+    p = np.ascontiguousarray(parent, np.uint32)
+    n = C.c_uint32(0)
+    rc = L.kuq_extract_taxa(_p(l, u32p), len(l), int(flags), _p(t, u32p), _p(p, u32p), len(t), None, 0, C.byref(n))
+    if rc:
+        raise KuqError(rc, "kuq_extract_taxa: " + L.kuq_strerror(rc).decode())
+    out = np.zeros(max(1, n.value), np.uint32)
+    rc = L.kuq_extract_taxa(_p(l, u32p), len(l), int(flags), _p(t, u32p), _p(p, u32p), len(t), _p(out, u32p), n.value, C.byref(n))
+    if rc:
+        raise KuqError(rc, "kuq_extract_taxa: " + L.kuq_strerror(rc).decode())
+    return out[:n.value]
 
 
 def _p(a, t):
@@ -346,6 +367,14 @@ class Classifier:
         p = np.ascontiguousarray(parent, np.uint32)
         self._ck(self.L.kuq_set_threshold(self.h, float(threshold), _p(t, u32p), _p(p, u32p), len(t)))
 
+    def set_extract(self, taxa, flags, taxid=(), parent=()):
+        """krakenuniq-extract-reads' read selection on every later batch (kuq_set_extract; flags: EXTRACT_*); results gain
+        extract_sel and n_extract"""
+        l = np.ascontiguousarray(taxa, np.uint32)
+        t = np.ascontiguousarray(taxid, np.uint32)
+        p = np.ascontiguousarray(parent, np.uint32)
+        self._ck(self.L.kuq_set_extract(self.h, _p(l, u32p), len(l), int(flags), _p(t, u32p), _p(p, u32p), len(t)))
+
     # ---- host-buffer classification ---------------------------------------------------------------------------
     def _result(self, res: BatchResult, offsets, copy=True):
         n = res.n_reads
@@ -358,6 +387,9 @@ class Classifier:
             runs = np.ctypeslib.as_array(C.cast(res.runs, u32p), shape=(int(res.n_runs) * 2,)) if res.n_runs else \
                 np.zeros(0, np.uint32)
             out["runs"] = runs.reshape(-1, 2)
+        if res.extract_sel:
+            out["extract_sel"] = as_np(res.extract_sel, n, np.uint8)
+            out["n_extract"] = int(res.n_extract)
         if res.filtered_call:
             out["filtered_call"] = as_np(res.filtered_call, n, np.uint32)
             out["filter_hits"] = as_np(res.filter_hits, n, np.uint32)

@@ -13,6 +13,8 @@
 //                                  mates are merged during the ingest; the one deviation is the exit status, EX_DATAERR
 //                                  where the merger stopped at a malformed record or a name mismatch (the wrapper
 //                                  ignores the merger's status and exits 0)
+//   --extract                      scripts/krakenuniq-extract-reads run on our Kraken lines and inputs: the reads of the
+//                                  chosen taxa are written while the batch is formatted (INTEGRATION.md)
 //   --sample-sheet                 no counterpart: one process stages the database(s) once and classifies every row of
 //                                  the sheet as a separate run would, with kuq_reset_counts between the samples
 // Not supported (exit with a message): -I uid mapping, -x together with several -d databases (the reference's own loop
@@ -64,6 +66,11 @@ static string Sample_sheet;                       // --sample-sheet: the samples
 static string Sample_label;                       // the sample being classified (sheet runs), named in error messages
 static bool Filter = false;                       // --threshold: the Kraken lines krakenuniq-filter makes of ours
 static double Threshold = 0;
+// --extract: the reads krakenuniq-extract-reads [-t taxDB] [-i] [-f] [-p] TAXIDS out.kraken reads would print
+static bool Extract = false, Extract_subtree = false, Extract_invert = false, Extract_fasta = false, Extract_others = false;
+static bool Extract_now = false;                  // this sample writes an extraction (a sheet row may leave it out)
+static string Extract_list, Extract_output_file;
+static vector<uint32_t> Extract_taxa;             // the list's decimal taxids ("-1" is Extract_others)
 static uint64_t Populate_memory_size = 0;
 static string Classified_output_file, Unclassified_output_file, Kraken_output_file, Report_output_file, TaxDB_file;
 static size_t Work_unit_size = 500000;      // DEF_WORK_UNIT_SIZE, classify.cpp:38
@@ -111,10 +118,25 @@ static void usage(int exit_code = EX_USAGE) {
        << "  --threshold T    Write the Kraken lines that krakenuniq-filter --threshold T makes of them: each call moves" << endl
        << "                   up the taxonomy until a fraction T of the read's unambiguous k-mers lies in the clade," << endl
        << "                   with that fraction as a P= column (-a's taxDB is the filter's taxonomy)" << endl
+       << "  --extract L      Write the reads that krakenuniq-extract-reads L <Kraken output> <input> prints: L is a" << endl
+       << "                   comma-separated taxid list (-1 = every other line, 0 = unclassified), to --extract-out f" << endl
+       << "                   ('-' = stdout, .gz = gzip; a --sample-sheet column extract_out instead)" << endl
+       << "  --extract-subtree  with the children of the taxa in -a's taxDB (the script's -t)" << endl
+       << "  --extract-invert   every read not selected (-i)       --extract-fasta  FASTQ reads as FASTA (-f)" << endl
        << "  -h               Print this message" << endl
        << endl
        << "Kraken output is to standard output by default." << endl;
   exit(exit_code);
+}
+
+static vector<string> split(const string &s, char sep) {
+  vector<string> v;
+  for (size_t a = 0;;) {
+    const size_t b = s.find(sep, a);
+    v.push_back(s.substr(a, b == string::npos ? string::npos : b - a));
+    if (b == string::npos) return v;
+    a = b + 1;
+  }
 }
 
 // parse_human_readable_size, krakenutil.cpp:30-55
@@ -139,11 +161,17 @@ static void parse_command_line(int argc, char **argv) {
   int opt;
   long long sig;
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
-  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES, OPT_SAMPLE_SHEET, OPT_THRESHOLD };
+  enum { OPT_PAIRED = 256, OPT_CHECK_NAMES, OPT_SAMPLE_SHEET, OPT_THRESHOLD, OPT_EXTRACT, OPT_EXTRACT_OUT, OPT_EXTRACT_SUBTREE,
+         OPT_EXTRACT_INVERT, OPT_EXTRACT_FASTA };
   static const struct option long_opts[] = {{"paired", no_argument, NULL, OPT_PAIRED},
                                             {"check-names", no_argument, NULL, OPT_CHECK_NAMES},
                                             {"sample-sheet", required_argument, NULL, OPT_SAMPLE_SHEET},
-                                            {"threshold", required_argument, NULL, OPT_THRESHOLD}, {NULL, 0, NULL, 0}};
+                                            {"threshold", required_argument, NULL, OPT_THRESHOLD},
+                                            {"extract", required_argument, NULL, OPT_EXTRACT},
+                                            {"extract-out", required_argument, NULL, OPT_EXTRACT_OUT},
+                                            {"extract-subtree", no_argument, NULL, OPT_EXTRACT_SUBTREE},
+                                            {"extract-invert", no_argument, NULL, OPT_EXTRACT_INVERT},
+                                            {"extract-fasta", no_argument, NULL, OPT_EXTRACT_FASTA}, {NULL, 0, NULL, 0}};
   while ((opt = getopt_long(argc, argv, "d:i:t:u:n:m:o:qcC:U:Ma:r:sI:p:x:", long_opts, NULL)) != -1) {
     switch (opt) {
       case OPT_PAIRED: Paired = true; break;
@@ -157,6 +185,11 @@ static void parse_command_line(int argc, char **argv) {
         Filter = true;
         break;
       }
+      case OPT_EXTRACT: Extract = true; Extract_list = optarg; break;
+      case OPT_EXTRACT_OUT: Extract_output_file = optarg; break;
+      case OPT_EXTRACT_SUBTREE: Extract_subtree = true; break;
+      case OPT_EXTRACT_INVERT: Extract_invert = true; break;
+      case OPT_EXTRACT_FASTA: Extract_fasta = true; break;
       case 'd': DB_filenames.push_back(optarg); break;
       case 'i': Index_filenames.push_back(optarg); break;
       case 't':
@@ -192,6 +225,21 @@ static void parse_command_line(int argc, char **argv) {
   }
   // the filter keeps five columns of a Kraken line (krakenuniq-filter:131): the sequence column would silently go
   if (Filter && Print_sequence) die(EX_USAGE, "--threshold cannot be combined with -s");
+  if (!Extract && (!Extract_output_file.empty() || Extract_subtree || Extract_invert || Extract_fasta))
+    die(EX_USAGE, "--extract-out, --extract-subtree, --extract-invert and --extract-fasta need --extract");
+  if (Extract) {
+    // the script's list (:62): entries compare as strings with the line's decimal taxid, so only canonical decimals
+    // can match; "-1" takes every line no other entry matched (:116-118)
+    for (const string &e : split(Extract_list, ',')) {
+      if (e == "-1") { Extract_others = true; continue; }
+      const bool canonical = !e.empty() && e.size() <= 10 && all_of(e.begin(), e.end(), ::isdigit) && (e == "0" || e[0] != '0');
+      if (canonical && strtoull(e.c_str(), NULL, 10) <= UINT32_MAX) Extract_taxa.push_back((uint32_t)strtoull(e.c_str(), NULL, 10));
+    }
+    if (Extract_subtree && TaxDB_file.empty()) die(EX_USAGE, "--extract-subtree takes the children from the taxDB: give it with -a");
+    if (!Sample_sheet.empty() && !Extract_output_file.empty())
+      die(EX_USAGE, "--sample-sheet takes the extraction's file from the sheet: --extract-out is its column extract_out");
+    if (Sample_sheet.empty() && Extract_output_file.empty()) die(EX_USAGE, "--extract needs --extract-out");
+  }
   if (DB_filenames.empty()) { cerr << "Missing mandatory option -d" << endl; usage(); }
   if (Index_filenames.empty()) { cerr << "Missing mandatory option -i" << endl; usage(); }
   if (!Sample_sheet.empty()) {                      // the sheet names every sample's inputs and outputs
@@ -210,23 +258,13 @@ static void parse_command_line(int argc, char **argv) {
 struct Sample {
   string name;
   vector<pair<string, string>> inputs;
-  string kraken, report, classified, unclassified;
+  string kraken, report, classified, unclassified, extract;
 };
 
 static vector<pair<const char *, const char *>> files_of(const Sample &s) {
   vector<pair<const char *, const char *>> in;
   for (auto &f : s.inputs) in.emplace_back(f.first.c_str(), f.second.empty() ? NULL : f.second.c_str());
   return in;
-}
-
-static vector<string> split(const string &s, char sep) {
-  vector<string> v;
-  for (size_t a = 0;;) {
-    const size_t b = s.find(sep, a);
-    v.push_back(s.substr(a, b == string::npos ? string::npos : b - a));
-    if (b == string::npos) return v;
-    a = b + 1;
-  }
 }
 
 // What two paths share when they name one file: device and inode of an existing file, else the absolute path
@@ -246,7 +284,8 @@ static string path_key(const string &p) {
 static vector<Sample> read_sample_sheet(const string &path) {
   ifstream in(path);
   if (!in.is_open()) die(EX_NOINPUT, "can't open the sample sheet " + path);
-  static const set<string> known = {"input", "input2", "output", "report", "classified_out", "unclassified_out", "name"};
+  static const set<string> known = {"input", "input2", "output", "report", "classified_out", "unclassified_out", "name",
+                                    "extract_out"};
   map<string, size_t> col;
   vector<Sample> samples;
   map<string, string> written;                     // path_key -> which sample writes it
@@ -259,12 +298,14 @@ static vector<Sample> read_sample_sheet(const string &path) {
     const string at = path + ":" + to_string(line_no) + ": ";
     if (col.empty()) {
       for (size_t i = 0; i < f.size(); i++) {
-        if (!known.count(f[i])) die(EX_USAGE, at + "unknown column '" + f[i] + "' (columns: input input2 output report classified_out unclassified_out name)");
+        if (!known.count(f[i])) die(EX_USAGE, at + "unknown column '" + f[i] + "' (columns: input input2 output report classified_out unclassified_out name extract_out)");
         if (!col.emplace(f[i], i).second) die(EX_USAGE, at + "column '" + f[i] + "' named twice");
       }
       if (!col.count("input")) die(EX_USAGE, at + "the header has no input column");
       if (Paired && !col.count("input2")) die(EX_USAGE, at + "--paired needs an input2 column with the second mates");
       if (!Paired && col.count("input2")) die(EX_USAGE, at + "an input2 column needs --paired");
+      if (Extract && !col.count("extract_out")) die(EX_USAGE, at + "--extract needs an extract_out column");
+      if (!Extract && col.count("extract_out")) die(EX_USAGE, at + "an extract_out column needs --extract");
       continue;
     }
     if (f.size() > col.size()) die(EX_USAGE, at + "more cells than the header has columns");
@@ -292,7 +333,8 @@ static vector<Sample> read_sample_sheet(const string &path) {
     s.report = cell("report");
     s.classified = cell("classified_out");
     s.unclassified = cell("unclassified_out");
-    for (const string *o : {&s.kraken, &s.report, &s.classified, &s.unclassified}) {
+    s.extract = cell("extract_out");                // empty: nothing is extracted from this sample
+    for (const string *o : {&s.kraken, &s.report, &s.classified, &s.unclassified, &s.extract}) {
       if (o->empty() || *o == "off" || *o == "-") continue;
       auto w = written.emplace(path_key(*o), s.name);
       if (!w.second) die(EX_USAGE, at + "samples " + w.first->second + " and " + s.name + " both write " + *o);
@@ -421,11 +463,20 @@ struct LineReader {     // std::ifstream + std::getline state semantics (eofbit 
   }
 };
 
+// --extract: a record's lines as they are in the file (a FASTQ record's four lines, a FASTA record's sequence lines), each
+// with its '\n' where the file has one
+static void keep_line(string *raw, const string &line, const LineReader &in) {
+  if (!raw) return;
+  raw->append(line);
+  if (!in.eofbit) *raw += '\n';
+}
+
 struct SeqReader {
   LineReader in;
   bool fastq = false, valid = true;
   string linebuffer;
   bool have_linebuffer = false;
+  string *raw = NULL;                    // --extract: the record's lines are appended here
   // next_sequence(): FASTA seqreader.cpp:34-79, FASTQ :93-129.  Appends the sequence to `bases`.
   bool next(Read &r, string &bases) {
     r.quals.clear();
@@ -440,15 +491,19 @@ struct SeqReader {
         return false;
       }
       r.header_line = line.substr(1);
+      keep_line(raw, line, in);
       string seq;
       in.getline(seq);
+      keep_line(raw, seq, in);
       in.getline(line);
       if (line.empty() || line[0] != '+') {
         if (line.empty() || line[0] != '\r') fprintf(stderr, "classify: malformed fastq file - quality header (%s)\n", line.c_str());
         valid = false;
         return false;
       }
+      keep_line(raw, line, in);
       in.getline(r.quals);
+      keep_line(raw, r.quals, in);
       r.seq_off = bases.size();
       r.seq_len = seq.size();
       bases += seq;
@@ -469,6 +524,7 @@ struct SeqReader {
       in.getline(line);
       if (!line.empty() && line[0] == '>') { linebuffer = line; have_linebuffer = true; break; }
       bases += line;
+      keep_line(raw, line, in);
     }
     r.seq_len = bases.size() - r.seq_off;
     return true;
@@ -535,6 +591,8 @@ struct MateFile {
   bool fasta = false;
   string buffer, id, seq;                  // buffer: the next record's header line, when have_line
   bool have_line = false, line_nl = false, ended = false;
+  bool keep = false;                       // --extract: raw = the record's four FASTQ lines as in the file
+  string raw;
   int read(string &err) {
     if (ended) return 0;
     if (!have_line) {
@@ -559,9 +617,14 @@ struct MateFile {
       }
     } else {                                                       // line 2; lines 3 and 4 are skipped unchecked
       string skip;
+      string *r = keep ? &raw : NULL;
+      if (r) { raw.assign(buffer); if (line_nl) raw += '\n'; }
       in.getline(seq);
+      keep_line(r, seq, in);
       in.getline(skip);
+      keep_line(r, skip, in);
       in.getline(skip);
+      keep_line(r, skip, in);
     }
     return 1;
   }
@@ -572,6 +635,9 @@ struct PairReader {
   MateFile m[2];
   MergeOrder order;
   bool valid = true;
+  string *raw = NULL;                      // --extract: mate 1's lines, then mate 2's (raw_n2 bytes)
+  uint32_t raw_n2 = 0;
+  bool raw_visited = true;                 // the script reads the record: it has a mate 1 (PAIR, ONLY1)
   void open(const char *f1, const char *f2) {
     const char *names[2] = {f1, f2};
     for (int k = 0; k < 2; k++) {
@@ -593,7 +659,14 @@ struct PairReader {
   bool next(Read &r, string &bases) {
     if (!valid) return false;
     string err;
+    m[0].keep = m[1].keep = raw != NULL;
     auto kind = order.next([&](int k) { return m[k].read(err); }, [&] { return m[0].id == m[1].id; });
+    if (raw) {
+      raw_visited = kind == MergeOrder::PAIR || kind == MergeOrder::ONLY1;
+      raw_n2 = kind == MergeOrder::PAIR ? (uint32_t)m[1].raw.size() : 0;
+      if (raw_visited) *raw += m[0].raw;
+      if (raw_n2) *raw += m[1].raw;
+    }
     r.quals.clear();
     r.seq_off = bases.size();
     switch (kind) {
@@ -625,6 +698,9 @@ struct InputReader {
   bool valid() const { return paired ? pair.valid : single.valid; }
   bool next(Read &r, string &bases) { return paired ? pair.next(r, bases) : single.next(r, bases); }
   void close() { if (paired) pair.close(); else single.in.close(); }
+  void keep_raw(string *raw) { single.raw = pair.raw = raw; }
+  uint32_t raw_n2() const { return paired ? pair.raw_n2 : 0; }
+  bool raw_visited() const { return !paired || pair.raw_visited; }
 };
 
 // ---- taxonomy (taxdb.hpp:563-605) + report (taxdb.hpp:928-1123) ------------------------------------------------
@@ -810,13 +886,18 @@ static double get_seconds(struct timeval a, struct timeval b) {
 }
 
 // ---- batches and their output ------------------------------------------------------------------------------------
+// --extract: where a read's lines lie in Batch::raw (mate 1's or the only record's n1 bytes, then mate 2's n2)
+struct RawRec { uint64_t off; uint32_t n1, n2; bool visited; };
+
 struct Batch {
   string bases;
   vector<uint64_t> offs{0};
   vector<Read> reads;
   vector<uint32_t> units;             // the reads' work units (kuq_batches.h)
   bool fastq = false;
-  void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); units.clear(); }
+  string raw;                         // --extract only: the reads' lines as in the file
+  vector<RawRec> raw_recs;
+  void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); units.clear(); raw.clear(); raw_recs.clear(); }
 };
 
 static const uint64_t SLOT_NT = 280ull << 20;   // the longest read of the resident paths, below the slot capacity (288 MiB)
@@ -835,7 +916,7 @@ static BatchLimits batch_limits(uint64_t batch_nt, bool aligned, bool resident) 
   return l;
 }
 
-static OutStream Kraken_out, Classified_out, Unclassified_out;
+static OutStream Kraken_out, Classified_out, Unclassified_out, Extract_out;
 
 // One read as the output sees it: the header line without its '>' / '@', the bases and (FASTQ) the qualities
 struct ReadView {
@@ -913,6 +994,84 @@ static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_res
   if (Print_kraken) kraken.resize(o - &kraken[0]);
 }
 
+// ---- --extract: krakenuniq-extract-reads (:139-217) over the records as they are in the input ---------------------
+// One record as the script reads it: `hdr` the header line without its '@' / '>' (the FASTQ record's first line for
+// paired reads), `kid` the header our Kraken line takes its id from, m1 / m2 the lines the script prints (a FASTQ
+// record's four lines, a FASTA record's sequence lines; m2 = the second mate's four lines).  visited: the script reaches
+// the record (records of mate file 2 that have no mate 1 are never read).
+struct XRec {
+  const char *hdr; size_t hdr_len;
+  const char *kid; size_t kid_len;
+  const char *m1; size_t n1;
+  const char *m2; size_t n2;
+  bool visited;
+};
+
+// the length of the id the script looks up (:142-150): the line's first word without its '@' / '>' (a prefix of h),
+// and one trailing /1 /2 .1 .2
+static size_t script_id(const char *h, size_t n) {
+  size_t k = 0;
+  while (k < n && h[k] != '\n' && !isspace((unsigned char)h[k])) k++;
+  if (k >= 2 && (h[k - 2] == '/' || h[k - 2] == '.') && (h[k - 1] == '1' || h[k - 1] == '2')) k -= 2;
+  return k;
+}
+
+// whether our Kraken line's id (format_reads: the header's first whitespace-delimited token) is id[0, k)
+static bool kraken_id_is(const char *h, size_t n, const char *id, size_t k) {
+  size_t x = 0;
+  while (x < n && isspace((unsigned char)h[x])) x++;
+  size_t y = x;
+  while (y < n && !isspace((unsigned char)h[y])) y++;
+  return y - x == k && memcmp(h + x, id, k) == 0;
+}
+
+// the second line of a FASTQ record's text, with its '\n' when it has one
+static void append_line2(string &o, const char *m, size_t n) {
+  const char *nl = (const char *)memchr(m, '\n', n);
+  if (!nl) return;
+  const char *s = nl + 1, *e = (const char *)memchr(s, '\n', m + n - s);
+  o.append(s, e ? e + 1 - s : m + n - s);
+}
+
+// What the script prints for reads [a, b): a read is printed when its Kraken line is selected (extract_sel bit 0 holds
+// selected XOR --extract-invert) and the script's id of the record is that line's id; where the ids differ (a header
+// ending in /1 .1 ...), the script finds no line for the record, so it prints the record only with --extract-invert.
+template <class XOf>
+static void extract_reads(XOf x_of, size_t a, size_t b, const kuq_batch_result &res, size_t res0, bool fasta, string &out) {
+  for (size_t i = a; i < b; i++) {
+    // a read whose line is not selected is written exactly with --extract-invert, whichever id it has; one whose line
+    // is selected is written when the script finds the line under the record's id, and with --extract-invert when not
+    const bool selected = ((res.extract_sel[i - res0] & 1) != 0) != Extract_invert;
+    if (!selected && !Extract_invert) continue;
+    const XRec x = x_of(i);
+    if (!x.visited) continue;
+    const size_t k = script_id(x.hdr, x.hdr_len);
+    if (selected && kraken_id_is(x.kid, x.kid_len, x.hdr, k) == Extract_invert) continue;
+    const string id(x.hdr, k);
+    if (fasta) {                                                   // -a (:162-177)
+      out += '>'; out += id; out += '\n';
+      out.append(x.m1, x.n1);
+    } else if (Extract_fasta) {                                    // -f (:162-190)
+      out += '>'; out += id; out += '\n';
+      append_line2(out, x.m1, x.n1);
+      if (Paired) { out += '>'; out += id; out += '\n'; append_line2(out, x.m2, x.n2); }
+    } else {                                                       // the four lines, then mate 2's (:191-204)
+      out.append(x.m1, x.n1);
+      out.append(x.m2, x.n2);
+    }
+  }
+}
+
+// The script prints nothing when no line is selected (:127), even with -i.  Text written before the sample's first
+// selected read is held back (only --extract-invert writes such text) and dropped if no read is ever selected.
+static string Extract_pending;
+static uint64_t Extract_selected = 0;      // selected reads of the sample so far
+static void write_extract(const string &text, bool selected_so_far) {
+  if (!selected_so_far) { Extract_pending += text; return; }
+  if (!Extract_pending.empty()) { Extract_out.write(Extract_pending); string().swap(Extract_pending); }
+  Extract_out.write(text);
+}
+
 // The output of reads [a, b) of a batch, whose results start at read a (the whole batch, or a GPU's share of it)
 static void write_reads(const Batch &bt, const kuq_batch_result &res, size_t a, size_t b) {
   string kraken, classified, unclassified;
@@ -924,6 +1083,21 @@ static void write_reads(const Batch &bt, const kuq_batch_result &res, size_t a, 
   Kraken_out.write(kraken);
   Classified_out.write(classified);
   Unclassified_out.write(unclassified);
+  if (!Extract_now) return;
+  Extract_selected += res.n_extract;
+  if (!res.n_extract && !Extract_invert) return;
+  const bool fasta = !bt.fastq && !Paired;
+  auto x_of = [&](size_t i) {
+    const Read &r = bt.reads[i];
+    const RawRec &q = bt.raw_recs[i];
+    const char *m1 = bt.raw.data() + q.off;
+    const char *h = fasta ? r.header_line.data() : m1 + 1;
+    const size_t hn = fasta ? r.header_line.size() : (q.n1 ? q.n1 - 1 : 0);
+    return XRec{h, hn, r.header_line.data(), r.header_line.size(), m1, q.n1, m1 + q.n1, q.n2, q.visited && (fasta || q.n1)};
+  };
+  string x;
+  extract_reads(x_of, a, b, res, a, fasta, x);
+  write_extract(x, Extract_selected > 0);
 }
 
 // A batch's totals (report_stats, classify.cpp:361-375) and the progress line (:555-558)
@@ -947,7 +1121,7 @@ static int db_taxids(kuq_ctx *ctx, map<uint32_t, uint64_t> &into) {
 
 // background writer: formatted text is handed over batch by batch and written in order while the next batch is
 // being gathered / classified / formatted
-struct OutJob { vector<string> kraken, classified, unclassified; };
+struct OutJob { vector<string> kraken, classified, unclassified, extract; bool extract_selected = false; };
 struct Writer {
   std::mutex m;
   std::condition_variable cv;
@@ -960,10 +1134,11 @@ struct Writer {
   OutJob take(size_t parts) {
     OutJob j;
     { std::lock_guard<std::mutex> l(m); if (!spare.empty()) { j = std::move(spare.front()); spare.pop_front(); } }
-    j.kraken.resize(parts); j.classified.resize(parts); j.unclassified.resize(parts);
+    j.kraken.resize(parts); j.classified.resize(parts); j.unclassified.resize(parts); j.extract.resize(parts);
     for (auto &x : j.kraken) x.clear();
     for (auto &x : j.classified) x.clear();
     for (auto &x : j.unclassified) x.clear();
+    for (auto &x : j.extract) x.clear();
     return j;
   }
   void finish() { { std::lock_guard<std::mutex> l(m); done = true; } cv.notify_one(); if (th.joinable()) th.join(); }
@@ -983,6 +1158,7 @@ void Writer::run() {
     for (auto &x : j.kraken) Kraken_out.write(x);
     for (auto &x : j.classified) Classified_out.write(x);
     for (auto &x : j.unclassified) Unclassified_out.write(x);
+    if (Extract_now) for (auto &x : j.extract) write_extract(x, j.extract_selected);
     { std::lock_guard<std::mutex> l(m); if (spare.size() < 3) spare.push_back(std::move(j)); }
   }
 }
@@ -1267,6 +1443,37 @@ static bool merge_parsed(const PlainInput (&in)[2], bool fastq, int T, vector<Vi
   return true;
 }
 
+// --extract over the mapped files: the lines of the FASTQ record whose sequence line starts at `seq`
+static void fastq_record_at(const char *seq, const PlainInput &f, const char *&m, size_t &n) {
+  const char *a = seq - 1;                                         // the header line's '\n'
+  while (a > f.base && a[-1] != '\n') a--;
+  const char *e = seq;
+  for (int k = 0; k < 3 && e < f.fend; k++) { e = line_end(e, f.fend); if (e < f.fend) e++; }
+  m = a; n = (size_t)(e - a);
+}
+
+// One mapped record as extract_reads reads it.  Merged mates (pair != NULL) take both records from the mapped files; a
+// record with no mate 1 (mate file 2's rest, the lone "N") is never visited.
+static XRec mapped_record(const View &v, const MateSeqs *pair, const PlainInput (&in)[2], bool fastq) {
+  XRec x{v.hdr, v.hdr_len, v.hdr, v.hdr_len, NULL, 0, NULL, 0, true};
+  const PlainInput &f = in[0];
+  if (pair) {
+    if (!pair->s1 || pair->s1 < f.base || pair->s1 >= f.fend + 1) { x.visited = false; return x; }
+    fastq_record_at(pair->s1, f, x.m1, x.n1);
+    if (pair->joined) fastq_record_at(pair->s2, in[1], x.m2, x.n2);
+    x.hdr = x.m1 + 1; x.hdr_len = x.n1 - 1;
+  } else if (fastq) {
+    x.m1 = v.hdr - 1;
+    const char *e = v.qual + v.qual_len;
+    x.n1 = (size_t)((e < f.fend ? e + 1 : e) - x.m1);
+  } else {                                                         // the sequence lines up to the next '>' line
+    const char *a = v.hdr + v.hdr_len < f.fend ? v.hdr + v.hdr_len + 1 : f.fend, *e = a;
+    while (e < f.fend && *e != '>') { e = line_end(e, f.fend); if (e < f.fend) e++; }
+    x.m1 = a; x.n1 = (size_t)(e - a);
+  }
+  return x;
+}
+
 static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const char *mate2) {
   const vector<kuq_ctx *> ctxs = All_ctx.empty() ? vector<kuq_ctx *>{ctx0} : All_ctx;
   const int G = (int)ctxs.size();
@@ -1391,9 +1598,15 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
       const View &v = *rv[s.begin + i];
       return ReadView{v.hdr, v.hdr_len, s.bases + s.offs[i], v.seq_len, v.qual, v.qual_len};
     };
+    if (Extract_now) Extract_selected += res.n_extract;
+    const bool extract = Extract_now && (res.n_extract || Extract_invert);
+    job.extract_selected = Extract_selected > 0;
+    auto x_of = [&](size_t i) { return mapped_record(*rv[s.begin + i], mate2 ? &mates[s.begin + i] : NULL, in, fastq_records); };
 #pragma omp parallel for schedule(static, 1) num_threads(Te)
-    for (int pi = 0; pi < parts; pi++)
+    for (int pi = 0; pi < parts; pi++) {
       format_reads(view_of, n * pi / parts, n * (pi + 1) / parts, res, 0, fastq, job.kraken[pi], job.classified[pi], job.unclassified[pi]);
+      if (extract) extract_reads(x_of, n * pi / parts, n * (pi + 1) / parts, res, 0, !fastq_records, job.extract[pi]);
+    }
     writer.push(std::move(job));
     book_batch(n, s.offs[n], res.n_classified);
   };
@@ -1469,12 +1682,14 @@ struct BatchReader {
   BatchCutter cutter;
   Read r;
   BatchCutter::Step step;
-  string held_bases;
+  string held_bases, held_raw;
+  RawRec rr{0, 0, 0, true};
   BatchReader(const vector<pair<const char *, const char *>> &f, const BatchLimits &lim) : files(f), cutter(lim) {}
   void push(Batch &b) {
     b.reads.push_back(r);
     b.offs.push_back(b.bases.size());
     b.units.push_back(step.unit);
+    if (Extract_now) b.raw_recs.push_back(rr);
   }
   bool next(Batch &b) {
     b.clear();
@@ -1483,6 +1698,8 @@ struct BatchReader {
       b.fastq = reader.fastq();
       r.seq_off = 0;
       b.bases += held_bases;
+      b.raw += held_raw;
+      rr.off = 0;
       push(b);
       if (step.after) return true;
     }
@@ -1493,12 +1710,18 @@ struct BatchReader {
         open = true;
       }
       b.fastq = reader.fastq();
-      while (reader.valid() && reader.next(r, b.bases)) {
+      reader.keep_raw(Extract_now ? &b.raw : NULL);
+      for (;;) {
+        const size_t x0 = b.raw.size();
+        if (!reader.valid() || !reader.next(r, b.bases)) break;
+        rr = RawRec{x0, (uint32_t)(b.raw.size() - x0 - reader.raw_n2()), reader.raw_n2(), reader.raw_visited()};
         if (cutter.lim.slot_nt && r.seq_len > cutter.lim.slot_nt) die(EX_DATAERR, "a single sequence is longer than 280 Mbp: not supported");
         step = cutter.next(r.seq_len);
         if (step.before) {
           held_bases.assign(b.bases, r.seq_off, r.seq_len);
           b.bases.resize(r.seq_off);
+          held_raw.assign(b.raw, rr.off, string::npos);
+          b.raw.resize(rr.off);
           held = true;
           return true;
         }
@@ -1510,6 +1733,7 @@ struct BatchReader {
       b.reads.resize(keep);
       b.offs.resize(keep + 1);
       b.units.resize(keep);
+      if (Extract_now) b.raw_recs.resize(keep);
       cutter.next_file();
       reader.close();
       open = false;
@@ -1952,6 +2176,49 @@ static uint64_t hbm_bytes(const Mapped &kdb, const Mapped &idx) {
   return key_ct * 12 + idx.size;
 }
 
+static uint32_t extract_flags() {
+  return (Extract_subtree ? KUQ_EXTRACT_SUBTREE : 0) | (Extract_invert ? KUQ_EXTRACT_INVERT : 0) |
+         (Extract_others ? KUQ_EXTRACT_OTHERS : 0) | (Only_classified_kraken_output ? KUQ_EXTRACT_CLASSIFIED_ONLY : 0);
+}
+
+// The checks of --extract that need the inputs or the taxonomy, before any device call: an extraction file that is an
+// input or another output, FASTA mates (the script dies on -a -p at the first read it prints), and a cycle below the
+// listed taxa (the script's get_children recursion never ends).  The taxonomy is read here for the last one.
+static void check_extract(const vector<Sample> &samples, TaxDB &tax, bool &tax_read) {
+  for (const Sample &s : samples) {
+    if (s.extract.empty()) continue;
+    set<string> in_keys;
+    for (auto &f : s.inputs) {
+      in_keys.insert(path_key(f.first));
+      if (!f.second.empty()) in_keys.insert(path_key(f.second));
+      if (f.second.empty()) continue;
+      LineReader lr;
+      if (lr.open(f.first.c_str()) && lr.peek() == '>')
+        die(EX_USAGE, "--extract with --paired needs FASTQ mates: krakenuniq-extract-reads cannot print FASTA mates (" + f.first + ")");
+      lr.close();
+    }
+    if (s.extract == "-") {
+      if (Sample_sheet.empty() && (Kraken_output_file.empty() || Kraken_output_file == "-"))
+        die(EX_USAGE, "--extract-out - : the Kraken output goes to standard output (give -o)");
+      if (Classified_output_file == "-" || Unclassified_output_file == "-")
+        die(EX_USAGE, "--extract-out - : -C or -U writes to standard output");
+      continue;
+    }
+    const string key = path_key(s.extract);
+    if (in_keys.count(key)) die(EX_USAGE, "--extract-out " + s.extract + " is one of the inputs");
+    if (Sample_sheet.empty())
+      for (const string *o : {&Kraken_output_file, &Report_output_file, &Classified_output_file, &Unclassified_output_file})
+        if (!o->empty() && *o != "-" && *o != "off" && path_key(*o) == key) die(EX_USAGE, "--extract-out " + s.extract + " is another output");
+  }
+  if (!Extract_subtree) return;
+  tax.read(TaxDB_file);
+  tax_read = true;
+  uint32_t n = 0;
+  if (kuq_extract_taxa(Extract_taxa.data(), (uint32_t)Extract_taxa.size(), KUQ_EXTRACT_SUBTREE, tax.row_ids.data(),
+                       tax.row_parents.data(), (uint32_t)tax.row_ids.size(), NULL, 0, &n))
+    die(EX_USAGE, "--extract-subtree: the children of the listed taxa in " + TaxDB_file + " form a cycle");
+}
+
 int main(int argc, char **argv) {
   parse_command_line(argc, argv);
   if (Map_UIDs) die(EX_USAGE, "-I (UID mapping) is not supported by the GPU classify");
@@ -1965,8 +2232,12 @@ int main(int argc, char **argv) {
   } else {
     Sample s;
     for (int i = optind; i < argc; i += Paired ? 2 : 1) s.inputs.emplace_back(argv[i], Paired ? argv[i + 1] : "");
+    s.extract = Extract_output_file;
     samples.push_back(s);
   }
+  TaxDB tax;
+  bool tax_read = false;
+  if (Extract) check_extract(samples, tax, tax_read);
   if (Populate_memory && Populate_memory_size == 0) cerr << "Loading database(s)... " << endl;
   vector<Mapped> kdbs(n_db), idxs(n_db);
   for (size_t i = 0; i < n_db; i++) {
@@ -2094,9 +2365,8 @@ int main(int argc, char **argv) {
   }
   if (Populate_memory && Populate_memory_size == 0) cerr << "\ncomplete." << endl;
 
-  TaxDB tax;
   cerr << "Reading taxonomy index from " << TaxDB_file;
-  tax.read(TaxDB_file);
+  if (!tax_read) tax.read(TaxDB_file);
   cerr << ". Done.\n";
   {
     vector<uint32_t> ids, parents;
@@ -2105,6 +2375,10 @@ int main(int argc, char **argv) {
       if (kuq_set_taxonomy(c, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(c));
     for (kuq_ctx *c : All_ctx)
       if (Filter && kuq_set_threshold(c, Threshold, tax.row_ids.data(), tax.row_parents.data(), (uint32_t)tax.row_ids.size()))
+        die(EX_DATAERR, kuq_last_error(c));
+    for (kuq_ctx *c : All_ctx)
+      if (Extract && kuq_set_extract(c, Extract_taxa.data(), (uint32_t)Extract_taxa.size(), extract_flags(), tax.row_ids.data(),
+                                     tax.row_parents.data(), (uint32_t)tax.row_ids.size()))
         die(EX_DATAERR, kuq_last_error(c));
   }
   if (cfg.hll_mode == KUQ_HLL_PRELOAD && !chunk_budget && !want_shards) {   // (streamed / sharded runs ask once their taxa are known)
@@ -2149,6 +2423,9 @@ int main(int argc, char **argv) {
       TICK("reset_counts");
     }
     total_classified = total_sequences = total_bases = 0;
+    Extract_now = Extract && !sample.extract.empty();
+    Extract_selected = 0;
+    if (Extract_now) Extract_out.open(sample.extract);
     if (Print_classified) Classified_out.open(Classified_output_file);
     if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);
     if (!Kraken_output_file.empty()) {
@@ -2248,6 +2525,8 @@ int main(int argc, char **argv) {
     Kraken_out.close();
     Classified_out.close();
     Unclassified_out.close();
+    string().swap(Extract_pending);                                  // no read was selected: nothing is written
+    Extract_out.close();
     // the records before the merger's stop are classified and written, like the wrapper's run on its partial output; the
     // samples after it still run
     if (!Pair_error.empty()) {

@@ -16,6 +16,7 @@
 #include <thread>
 #include <type_traits>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/kuq.h"
@@ -60,6 +61,8 @@ struct Slot {
   // confidence filter (kuq_set_threshold): filtered call, hits and total per read, allocated when it is set
   uint32_t *d_fcall = nullptr, *d_fhits = nullptr, *d_ftotal = nullptr;
   uint32_t *h_fcall = nullptr, *h_fhits = nullptr, *h_ftotal = nullptr;
+  // read selection (kuq_set_extract): one byte per read, then the batch's selected reads (u32 at extract_count_at)
+  uint8_t *d_xsel = nullptr, *h_xsel = nullptr;
   kuq_run *h_runs = nullptr;
   uint64_t h_runs_cap = 0;
   unsigned long long *h_scalars = nullptr;
@@ -157,6 +160,10 @@ struct kuq_ctx {
   double threshold = 0;
   std::unordered_map<uint32_t, uint32_t> f_parent, f_depth;
   uint32_t *d_fparent = nullptr, *d_fdepth = nullptr, *d_fextra = nullptr;
+  // kuq_set_extract: the selected taxids, ascending, and the KUQ_EXTRACT_* flags
+  bool extract_set = false;
+  uint32_t extract_flags = 0, n_members = 0;
+  uint32_t *d_members = nullptr;
 
   // per-taxon state
   uint8_t *d_regs = nullptr, *d_dense_flag = nullptr;
@@ -263,6 +270,7 @@ void free_slot(Slot &s) {
   cudaFreeHost(s.h_codes); cudaFreeHost(s.h_runs); cudaFreeHost(s.h_scalars); cudaFreeHost(s.h_unit);
   cudaFree(s.d_fcall); cudaFree(s.d_fhits); cudaFree(s.d_ftotal);
   cudaFreeHost(s.h_fcall); cudaFreeHost(s.h_fhits); cudaFreeHost(s.h_ftotal);
+  cudaFree(s.d_xsel); cudaFreeHost(s.h_xsel);
   if (s.ev_k0) cudaEventDestroy(s.ev_k0);
   if (s.ev_k1) cudaEventDestroy(s.ev_k1);
   if (s.ev_stage[0]) cudaEventDestroy(s.ev_stage[0]);
@@ -862,6 +870,9 @@ int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
       [src](uint64_t lo, uint64_t hi, ExactPair *buf, uint64_t cap, uint64_t *counts) { return exact_export_range(src, lo, hi, buf, cap, counts); },
       [dst](uint32_t, const ExactPair *pairs, uint64_t m) { return exact_import(dst, pairs, m); });
 }
+
+// kuq_set_extract's slot buffer: one selection byte per read, then the batch's count of selected reads (u32)
+uint64_t extract_count_at(const kuq_ctx *ctx) { return (ctx->cfg.max_reads_per_batch + 15ull) & ~15ull; }
 
 // krakenuniq-filter's parent map in filter ids: a taxon's dense id, or for taxa of F without one (parents without a
 // taxonomy row, taxa the taxonomy does not have) n_taxa + their index in d_fextra.
@@ -1569,6 +1580,12 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
     if (mode != MODE_LOOKUP) CU(cudaMemsetAsync(p.chunk_counter, 0, 4, s.stream));   // k_scan of the resolve half
   }
   if (p.n_reads && !(multi && mode == MODE_LOOKUP)) ctx->launches += launch_classify(mode, p, ctx->n_sm, s.stream, s.ev_stage);
+  if (p.n_reads && mode != MODE_LOOKUP && ctx->extract_set) {          // after whichever resolve wrote the calls
+    CU(cudaMemsetAsync(s.d_xsel + extract_count_at(ctx), 0, 4, s.stream));
+    launch_extract_select(p.call, p.fcall, p.n_reads, ctx->d_members, ctx->n_members, ctx->extract_flags, s.d_xsel,
+                          reinterpret_cast<uint32_t *>(s.d_xsel + extract_count_at(ctx)), s.stream);
+    ctx->launches++;
+  }
   // the fused path flags the records of its counted hits (k_lookup); quick / exact runs go through the other halves
   if (p.n_reads && mode == MODE_FUSED && !(p.flags & 4u) && ctx->cfg.hll_mode <= KUQ_HLL_CHUNKED &&
       !(ctx->quick_min && ctx->quick_stop) && !keep)
@@ -1688,6 +1705,7 @@ void kuq_destroy(kuq_ctx *ctx) {
   stream_close(ctx);
   free_db(ctx);
   free_tax_state(ctx);
+  cudaFree(ctx->d_members);                  // raw taxids: kept when finalize renumbers the taxonomy
   cudaFree(ctx->d_sync_err);
   cudaFree(ctx->d_harvest_stat);
   for (cudaEvent_t e : ctx->harvest_ev) if (e) cudaEventDestroy(e);
@@ -2004,6 +2022,83 @@ int kuq_set_threshold(kuq_ctx *ctx, double threshold, const uint32_t *taxid, con
   return ctx->finalized ? upload_filter(ctx) : KUQ_OK;
 }
 
+namespace {
+// get_children (krakenuniq-extract-reads:48-58,65-76) over the child multigraph of the rows: the listed taxa and, with
+// KUQ_EXTRACT_SUBTREE, everything reachable from them, ascending.  A depth-first walk that meets a node still on its
+// path has found a cycle: KUQ_E_TAXONOMY, *cycle_at = that node.
+int extract_members(const uint32_t *list, uint32_t n_list, uint32_t flags, const uint32_t *taxid, const uint32_t *parent,
+                    uint32_t n_rows, std::vector<uint32_t> &out, uint32_t *cycle_at) {
+  std::unordered_set<uint32_t> members(list, list + n_list);
+  if (flags & KUQ_EXTRACT_SUBTREE) {
+    std::unordered_map<uint32_t, std::vector<uint32_t>> children;
+    for (uint32_t i = 0; i < n_rows; i++)
+      if (taxid[i] != parent[i]) children[parent[i]].push_back(taxid[i]);
+    std::unordered_map<uint32_t, uint8_t> state;          // 1 = on the walk's path, 2 = done
+    std::vector<std::pair<uint32_t, size_t>> path;
+    for (uint32_t i = 0; i < n_list; i++) {
+      if (state[list[i]]) continue;
+      path.assign(1, {list[i], 0});
+      state[list[i]] = 1;
+      while (!path.empty()) {
+        const uint32_t node = path.back().first;
+        auto it = children.find(node);
+        if (it == children.end() || path.back().second == it->second.size()) { state[node] = 2; path.pop_back(); continue; }
+        const uint32_t c = it->second[path.back().second++];
+        uint8_t &st = state[c];
+        if (st == 1) { *cycle_at = c; return KUQ_E_TAXONOMY; }
+        if (st == 2) continue;
+        st = 1;
+        members.insert(c);
+        path.push_back({c, 0});
+      }
+    }
+  }
+  out.assign(members.begin(), members.end());
+  std::sort(out.begin(), out.end());
+  return KUQ_OK;
+}
+}  // namespace
+
+int kuq_extract_taxa(const uint32_t *list, uint32_t n_list, uint32_t flags, const uint32_t *taxid, const uint32_t *parent,
+                     uint32_t n_rows, uint32_t *out, uint32_t cap, uint32_t *n_out) {
+  if ((!list && n_list) || ((!taxid || !parent) && n_rows) || !n_out || (!out && cap)) return KUQ_E_INVALID_ARG;
+  std::vector<uint32_t> m;
+  uint32_t at = 0;
+  const int rc = extract_members(list, n_list, flags, taxid, parent, n_rows, m, &at);
+  if (rc) return rc;
+  *n_out = (uint32_t)m.size();
+  if (cap) std::copy(m.begin(), m.begin() + std::min<size_t>(cap, m.size()), out);
+  return KUQ_OK;
+}
+
+int kuq_set_extract(kuq_ctx *ctx, const uint32_t *list, uint32_t n_list, uint32_t flags, const uint32_t *taxid,
+                    const uint32_t *parent, uint32_t n_rows) {
+  if (!ctx || (!list && n_list) || ((!taxid || !parent) && n_rows)) return KUQ_E_INVALID_ARG;
+  if (flags & ~(KUQ_EXTRACT_SUBTREE | KUQ_EXTRACT_INVERT | KUQ_EXTRACT_OTHERS | KUQ_EXTRACT_CLASSIFIED_ONLY))
+    return fail(ctx, KUQ_E_INVALID_ARG, "unknown kuq_set_extract flags 0x%x", flags);
+  if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "kuq_set_extract: set the taxonomy first");
+  if (ctx->extract_set) return fail(ctx, KUQ_E_STATE, "the extraction is already set");
+  for (auto &s : ctx->slots)
+    if (s.busy) return fail(ctx, KUQ_E_STATE, "the extraction cannot be set while a batch is in flight");
+  std::vector<uint32_t> sorted;
+  uint32_t at = 0;
+  if (extract_members(list, n_list, flags, taxid, parent, n_rows, sorted, &at))
+    return fail(ctx, KUQ_E_TAXONOMY, "cycle in the children of the taxonomy at taxid %u", at);
+  const uint32_t n_members = (uint32_t)sorted.size();
+  sorted.push_back(0);                                  // never an empty allocation
+  CU(cudaSetDevice(ctx->device));
+  CU(dmalloc(&ctx->d_members, sorted.size()));
+  CU(cudaMemcpy(ctx->d_members, sorted.data(), sorted.size() * 4, cudaMemcpyHostToDevice));
+  for (auto &s : ctx->slots) {
+    CU(dmalloc(&s.d_xsel, extract_count_at(ctx) + 16));
+    CU(hmalloc(&s.h_xsel, extract_count_at(ctx) + 16));
+  }
+  ctx->n_members = n_members;
+  ctx->extract_flags = flags;
+  ctx->extract_set = true;
+  return KUQ_OK;
+}
+
 // ---- classification -------------------------------------------------------------------------------------------
 namespace {
 // D2H of a batch's fixed-size results; the variable-size hit lists follow in kuq_wait_batch
@@ -2020,6 +2115,10 @@ int copy_results(kuq_ctx *ctx, Slot &s) {
       CU(cudaMemcpyAsync(s.h_fcall, s.d_fcall, n * 4, cudaMemcpyDeviceToHost, s.stream));
       CU(cudaMemcpyAsync(s.h_fhits, s.d_fhits, n * 4, cudaMemcpyDeviceToHost, s.stream));
       CU(cudaMemcpyAsync(s.h_ftotal, s.d_ftotal, n * 4, cudaMemcpyDeviceToHost, s.stream));
+    }
+    if (ctx->extract_set) {
+      CU(cudaMemcpyAsync(s.h_xsel, s.d_xsel, n, cudaMemcpyDeviceToHost, s.stream));
+      CU(cudaMemcpyAsync(s.h_xsel + extract_count_at(ctx), s.d_xsel + extract_count_at(ctx), 4, cudaMemcpyDeviceToHost, s.stream));
     }
   }
   CU(cudaMemcpyAsync(s.h_scalars, s.d_scalars, 8 * 8, cudaMemcpyDeviceToHost, s.stream));
@@ -2190,6 +2289,12 @@ int kuq_wait_batch(kuq_ctx *ctx, uint32_t slot, kuq_batch_result *out) {
     out->filtered_call = s.h_fcall;
     out->filter_hits = s.h_fhits;
     out->filter_total = s.h_ftotal;
+  }
+  if (ctx->extract_set) {
+    out->extract_sel = s.h_xsel;
+    uint32_t n_sel = 0;
+    if (s.n_reads) memcpy(&n_sel, s.h_xsel + extract_count_at(ctx), 4);
+    out->n_extract = n_sel;
   }
   return KUQ_OK;
 }

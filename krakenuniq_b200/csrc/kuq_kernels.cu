@@ -4,6 +4,7 @@
 // each keep a small register footprint.  The lookup and resolve halves hand windows over through HBM scratch (12 B per
 // window, streamed); the fused call hands over a 2-bit packed copy of the batch (16 B per 32 positions) and the
 // thread-per-window lookup computes its window from it.
+#include "../../include/kuq.h"
 #include "kuq_kernels.cuh"
 
 namespace kuq {
@@ -1398,6 +1399,41 @@ __global__ void k_flag_dense_global(const uint32_t *distinct, uint8_t *dense_fla
 }
 void launch_flag_dense_global(const uint32_t *distinct, uint8_t *dense_flag, uint32_t n_sketch, cudaStream_t stream) {
   if (n_sketch) k_flag_dense_global<<<(n_sketch + 255) / 256, 256, 0, stream>>>(distinct, dense_flag, n_sketch);
+}
+
+// krakenuniq-extract-reads' selection (:107-119) of each read's Kraken line: the line's taxid (the filtered call when a
+// threshold is set) is looked up in the sorted member taxids; KUQ_EXTRACT_OTHERS takes every line.  One thread per read;
+// each warp adds its selected reads to *count with one atomic.
+__global__ void __launch_bounds__(256) k_extract_select(const uint32_t *__restrict__ call, const uint32_t *__restrict__ fcall,
+                                                        uint32_t n_reads, const uint32_t *__restrict__ members,
+                                                        uint32_t n_members, uint32_t flags, uint8_t *__restrict__ sel,
+                                                        uint32_t *count) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  bool selected = false;
+  if (r < n_reads) {
+    const uint32_t c = __ldg(call + r);
+    const bool line = c != 0 || !(flags & KUQ_EXTRACT_CLASSIFIED_ONLY);
+    if (line) {
+      if (flags & KUQ_EXTRACT_OTHERS) {
+        selected = true;
+      } else {
+        const uint32_t t = fcall ? __ldg(fcall + r) : c;
+        uint32_t lo = 0, hi = n_members;                 // first member >= t
+        while (lo < hi) {
+          const uint32_t mid = (lo + hi) >> 1;
+          if (__ldg(members + mid) < t) lo = mid + 1; else hi = mid;
+        }
+        selected = lo < n_members && __ldg(members + lo) == t;
+      }
+    }
+    sel[r] = (uint8_t)((selected != ((flags & KUQ_EXTRACT_INVERT) != 0)) | (line ? 0 : 2));
+  }
+  const unsigned m = __ballot_sync(0xFFFFFFFFu, selected);
+  if ((threadIdx.x & 31) == 0 && m) atomicAdd(count, (uint32_t)__popc(m));
+}
+void launch_extract_select(const uint32_t *call, const uint32_t *fcall, uint32_t n_reads, const uint32_t *members,
+                           uint32_t n_members, uint32_t flags, uint8_t *sel, uint32_t *count, cudaStream_t stream) {
+  if (n_reads) k_extract_select<<<(n_reads + 255) / 256, 256, 0, stream>>>(call, fcall, n_reads, members, n_members, flags, sel, count);
 }
 
 // getEncodedRank(enc, 25, 12), hyperloglogplus.cpp:152-161

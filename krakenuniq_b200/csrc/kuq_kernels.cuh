@@ -358,6 +358,10 @@ int launch_unit_accounting(const Params &p, int n_sm, cudaStream_t stream);
 void launch_unit_clear(const UnitMap &u, uint32_t n_sketch, int n_sm, cudaStream_t stream);
 // chunked rule: one global sketch per taxon converts once it holds >= 1025 distinct codes
 void launch_flag_dense_global(const uint32_t *distinct, uint8_t *dense_flag, uint32_t n_sketch, cudaStream_t stream);
+// kuq_set_extract: one byte per read (bit 0 selected XOR invert, bit 1 no Kraken line) and the batch's selected reads
+// added to *count; members = the selected taxids, ascending
+void launch_extract_select(const uint32_t *call, const uint32_t *fcall, uint32_t n_reads, const uint32_t *members,
+                           uint32_t n_members, uint32_t flags, uint8_t *sel, uint32_t *count, cudaStream_t stream);
 // histogram of encoded ranks over one source of the sparse tier, per taxon: hist[t][64] (+ hist[t][63] unused)
 void launch_sparse_histograms(const KeySource &src, const uint8_t *dense_flag, uint32_t *hist, cudaStream_t stream);
 // distinct codes of the union of the member taxa (member[t] != 0): rank histogram hist64 via a scratch set
