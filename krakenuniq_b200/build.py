@@ -12,7 +12,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "lib", "libkuq.so")
 SOURCES = ["kuq_kernels.cu", "kuq_api.cu", "kuq_dbbuild.cu", "kuq_microbench.cu", "kuq_layout_exp.cu", "kuq_clades.cu",
            "kuq_collisions.cu", "kuq_kmerset.cu"]
-HEADERS = ["kuq_kernels.cuh", "kuq_minimizer.cuh", "kuq_bounce.cuh", "kuq_ranges.h", "kuq_batches.h",
+HEADERS = ["kuq_kernels.cuh", "kuq_buffers.cuh", "kuq_minimizer.cuh", "kuq_bounce.cuh", "kuq_ranges.h", "kuq_batches.h",
            os.path.join(ROOT, "include", "kuq.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--compiler-bindir", "/usr/bin/g++", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared", "-cudart", "shared"]

@@ -33,39 +33,40 @@ constexpr uint32_t SLACK = 64;                                // bytes readable 
 constexpr uint32_t UMAP_CAP = 1u << 21;                       // (unit, taxon) pairs per batch
 
 struct Slot {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr, ev_stage[2] = {nullptr, nullptr}, ev_sync = nullptr;
+  Stream stream;
+  Event ev_k0, ev_k1, ev_stage[2], ev_sync;
   double stage_ms[3] = {0, 0, 0};
   // device
-  char *d_bases = nullptr, *d_clean = nullptr;
-  uint64_t *d_offsets = nullptr;
-  uint32_t *d_unit = nullptr, *d_call = nullptr, *d_nwin = nullptr, *d_codes = nullptr;
+  DevBuf<char> d_bases, d_clean;
+  DevBuf<uint64_t> d_offsets;
+  DevBuf<uint32_t> d_unit, d_call, d_nwin, d_codes;
   // HLL mode rule bookkeeping (KUQ_HLL_PRELOAD), allocated on first use
-  unsigned long long *u_keys = nullptr;
-  uint32_t *u_inserts = nullptr, *u_cand = nullptr, *u_ncand = nullptr, *u_direct = nullptr, *u_codes = nullptr;
+  DevBuf<unsigned long long> u_keys;
+  DevBuf<uint32_t> u_inserts, u_cand, u_ncand, u_direct, u_codes;
   uint32_t u_direct_rows = 0;
-  uint64_t *d_canon = nullptr;                 // scratch between the stages
-  uint32_t *d_bins = nullptr, *d_dense = nullptr, *d_codes_in = nullptr;
-  PackedBlock *d_pack = nullptr;               // the fused path's 2-bit copy of the batch (k_pack)
-  uint32_t *d_side = nullptr;
+  DevBuf<uint64_t> d_canon;                    // scratch between the stages
+  DevBuf<uint32_t> d_bins, d_dense, d_codes_in;
+  DevBuf<PackedBlock> d_pack;                  // the fused path's 2-bit copy of the batch (k_pack)
+  DevBuf<uint32_t> d_side;
   bool windows_packed = false;                 // the last call's windows are in d_pack, not in d_canon / d_bins
-  unsigned long long *d_ovf = nullptr;          // hit-table pool for reads with > 32 distinct taxa
+  DevBuf<unsigned long long> d_ovf;            // hit-table pool for reads with > 32 distinct taxa
   uint64_t ovf_entries = 0;
-  uint32_t *d_run_start = nullptr, *d_run_count = nullptr;
-  uint2 *d_runs = nullptr;
+  DevBuf<uint32_t> d_run_start, d_run_count;
+  DevBuf<uint2> d_runs;
   uint64_t runs_cap = 0;
-  unsigned long long *d_scalars = nullptr;   // [0] run cursor, [1] n_classified, [2] chunk counter(u32) [3] error(u32)
+  DevBuf<unsigned long long> d_scalars;        // [0] run cursor, [1] n_classified, [2] chunk counter(u32) [3] error(u32)
   // pinned host
-  uint32_t *h_call = nullptr, *h_nwin = nullptr, *h_run_start = nullptr, *h_run_count = nullptr, *h_codes = nullptr;
-  uint32_t *h_unit = nullptr;
+  HostBuf<uint32_t> h_call, h_nwin, h_run_start, h_run_count, h_codes;
+  HostBuf<uint32_t> h_unit;
   // confidence filter (kuq_set_threshold): filtered call, hits and total per read, allocated when it is set
-  uint32_t *d_fcall = nullptr, *d_fhits = nullptr, *d_ftotal = nullptr;
-  uint32_t *h_fcall = nullptr, *h_fhits = nullptr, *h_ftotal = nullptr;
+  DevBuf<uint32_t> d_fcall, d_fhits, d_ftotal;
+  HostBuf<uint32_t> h_fcall, h_fhits, h_ftotal;
   // read selection (kuq_set_extract): one byte per read, then the batch's selected reads (u32 at extract_count_at)
-  uint8_t *d_xsel = nullptr, *h_xsel = nullptr;
-  kuq_run *h_runs = nullptr;
+  DevBuf<uint8_t> d_xsel;
+  HostBuf<uint8_t> h_xsel;
+  HostBuf<kuq_run> h_runs;
   uint64_t h_runs_cap = 0;
-  unsigned long long *h_scalars = nullptr;
+  HostBuf<unsigned long long> h_scalars;
   // in-flight batch
   bool busy = false;
   bool timed = false;      // the timing events of this slot have been recorded at least once
@@ -82,8 +83,8 @@ struct Slot {
 // (16-byte ExactPairs).  A context has at most one of them.
 template <typename Item, typename Count>
 struct DevTable {
-  Item *slots = nullptr;
-  Count *count = nullptr;                 // [n_sketch] items per taxon
+  DevBuf<Item> slots;
+  DevBuf<Count> count;                    // [n_sketch] items per taxon
   uint64_t cap = 0;                       // slots, a power of two
   uint64_t upper = 0;                     // upper bound of the items since the last exact count (reserve_room)
   uint64_t grown = 0;                     // times the slots were re-allocated
@@ -109,12 +110,14 @@ struct kuq_ctx {
   std::string err;
   std::vector<Slot> slots;
   uint64_t launches = 0;
-  cudaStream_t aux = nullptr;
+  Stream aux;
 
-  // database
+  // database: d_pairs / d_offsets are the records in use, owned here (db_owned), by the caller
+  // (kuq_attach_db_device) or by a stream buffer
   bool db_owned = false;
   uint8_t *d_pairs = nullptr;
-  uint64_t *d_offsets_owned = nullptr;
+  DevBuf<uint8_t> d_pairs_owned;
+  DevBuf<uint64_t> d_offsets_owned;
   const uint64_t *d_offsets = nullptr;
   uint64_t key_ct = 0, rec_base = 0;
   uint32_t k = 0, nt = 0, idx_type = 0;
@@ -124,17 +127,17 @@ struct kuq_ctx {
   std::vector<uint64_t> db_taxid_counts;
   std::vector<uint32_t> universe;         // taxids of all records of the database (optional)
   // device hash of the staged taxids (keys = taxid + 1)
-  uint32_t *d_tx_keys = nullptr, *d_tx_dense = nullptr;
-  unsigned long long *d_tx_counts = nullptr;
+  DevBuf<uint32_t> d_tx_keys, d_tx_dense;
+  DevBuf<unsigned long long> d_tx_counts;
   uint32_t tx_cap = 0;
   // databases (or minimizer ranges of them) asked after the one above, in this order (kuq_stage_db_append_range); same k
   struct ExtraDb {
-    uint8_t *d_pairs = nullptr;
-    uint64_t *d_offsets = nullptr;
+    DevBuf<uint8_t> d_pairs;
+    DevBuf<uint64_t> d_offsets;
     uint64_t key_ct = 0, rec_base = 0, bin_lo = 0, bin_hi = 0;
     uint32_t nt = 0, idx_type = 0;
-    uint32_t *d_tx_keys = nullptr, *d_tx_dense = nullptr;
-    unsigned long long *d_tx_counts = nullptr;
+    DevBuf<uint32_t> d_tx_keys, d_tx_dense;
+    DevBuf<unsigned long long> d_tx_counts;
     uint32_t tx_cap = 0;
     std::vector<uint32_t> taxids;
     std::vector<uint64_t> counts;
@@ -152,24 +155,24 @@ struct kuq_ctx {
   std::vector<uint32_t> parent_dense;     // host copy of d_parent (dense id of the parent, 0 = none)
   std::unordered_map<uint32_t, uint32_t> dense_of_raw;
   uint32_t n_taxa = 0, n_sketch = 0;
-  uint32_t *d_parent = nullptr, *d_raw = nullptr;
-  uint16_t *d_depth = nullptr;
+  DevBuf<uint32_t> d_parent, d_raw;
+  DevBuf<uint16_t> d_depth;
   // kuq_set_threshold: krakenuniq-filter's parent map F (taxid → parent) with the F-depth of every node; uploaded in
   // filter ids (Params::fparent) once the dense numbering exists
   bool filter_set = false;
   double threshold = 0;
   std::unordered_map<uint32_t, uint32_t> f_parent, f_depth;
-  uint32_t *d_fparent = nullptr, *d_fdepth = nullptr, *d_fextra = nullptr;
+  DevBuf<uint32_t> d_fparent, d_fdepth, d_fextra;
   // kuq_set_extract: the selected taxids, ascending, and the KUQ_EXTRACT_* flags
   bool extract_set = false;
   uint32_t extract_flags = 0, n_members = 0;
-  uint32_t *d_members = nullptr;
+  DevBuf<uint32_t> d_members;
 
   // per-taxon state
-  uint8_t *d_regs = nullptr, *d_dense_flag = nullptr;
-  uint8_t *d_reg_floor = nullptr;         // [n_sketch]: lower bound of each sketch's registers (refresh_reg_floor)
-  unsigned long long *d_n_kmers = nullptr, *d_n_reads = nullptr;
-  unsigned long long *d_sparse_used = nullptr;
+  DevBuf<uint8_t> d_regs, d_dense_flag;
+  DevBuf<uint8_t> d_reg_floor;            // [n_sketch]: lower bound of each sketch's registers (refresh_reg_floor)
+  DevBuf<unsigned long long> d_n_kmers, d_n_reads;
+  DevBuf<unsigned long long> d_sparse_used;
   SparseTable sparse;                     // the sparse-tier set; count[] includes the keys of kept records
   ExactTable exact;                       // KUQ_HLL_EXACT: the (taxon, k-mer) table and the per-taxon set sizes
   bool exact_partitioned = false;         // kuq_exact_replace / kuq_exact_partition: the table holds one owner's part
@@ -177,32 +180,32 @@ struct kuq_ctx {
   std::vector<unsigned long long> merged_exact_count;
   std::vector<long long> merged_books;
   std::vector<uint32_t> exact_pre;        // preorder of every sketch taxon in the taxonomy (exact roll-up), built once
-  uint32_t *d_exact_pre = nullptr;
+  DevBuf<uint32_t> d_exact_pre;
   uint32_t exact_rollup_passes = 0;       // k-mer passes of the last exact roll-up
 
   // database streamed through HBM range by range (kuq_stream_*): two device buffers, one copy stream
   struct StreamBuf {
-    uint8_t *d_pairs = nullptr;
-    uint64_t *d_offsets = nullptr;
-    cudaEvent_t ready = nullptr;
+    DevBuf<uint8_t> d_pairs;
+    DevBuf<uint64_t> d_offsets;
+    Event ready;
     uint64_t key_ct = 0, rec_base = 0, bin_lo = 0, bin_hi = 0;
     bool loaded = false;
   } sbuf[2];
   bool stream_open = false;
   uint64_t stream_cap_records = 0, stream_cap_bins = 0;
-  cudaStream_t copy_stream = nullptr;
-  uint32_t *d_stream_missing = nullptr;
+  Stream copy_stream;
+  DevBuf<uint32_t> d_stream_missing;
   uint64_t stream_pair_sz = 12;           // record size of the streamed database's file (key_len + 4)
-  uint8_t *d_stream_land = nullptr;       // k <= 28: landing zone of stream_land_rec file records, widened from there
+  DevBuf<uint8_t> d_stream_land;          // k <= 28: landing zone of stream_land_rec file records, widened from there
   uint64_t stream_land_rec = 0;
   bool shard_counting = false;            // kuq_set_shard_counting: hits are counted by the GPU that finds them
   uint32_t extra_flags = 0;               // kuq_set_stats: KUQ_F_STATS for calls that take no flags
-  uint32_t *d_sync_err = nullptr;         // set by a kuq_wait_flags that timed out
+  DevBuf<uint32_t> d_sync_err;            // set by a kuq_wait_flags that timed out
   bool merged_summary = false;            // kuq_set_sparse_summary: snap.sparse_hist / distinct hold cross-GPU sums
   std::vector<uint32_t> merged_hist, merged_distinct;
   bool seen_dirty = false;                // counted hits flagged records since the last harvest (SEEN_BIT)
   // record tier of the sparse HLL tier (KEPT_BIT): a resident range keeps its hits' keys in the records themselves
-  uint2 *d_secondaries = nullptr;         // (secondary, primary) record pairs of the (taxon, code) groups of the range
+  DevBuf<uint2> d_secondaries;            // (secondary, primary) record pairs of the (taxon, code) groups of the range
   uint64_t n_secondaries = 0;
   int collisions = 0;                     // that table: 0 = not built yet, 1 = built, -1 = none (harvests fill the set)
   double collisions_ms = 0;               // time the table took to build
@@ -214,8 +217,8 @@ struct kuq_ctx {
   // the harvest's counters and timing events, made at the first harvest (or keep-mode call) and kept: a cudaMalloc /
   // cudaFree pair per harvest held the device idle at the end of every run.  [0], [1]: the harvest's; [2]: records that
   // keep-mode calls made kept since settle_kept (k_resolve counts them)
-  unsigned long long *d_harvest_stat = nullptr;
-  cudaEvent_t harvest_ev[2] = {nullptr, nullptr};
+  DevBuf<unsigned long long> d_harvest_stat;
+  Event harvest_ev[2];
   bool lca_mode = false;                  // kuq_set_lcas_batch ran: record values are LCA results, not classifiable
   WorkUnits units;                        // the open work unit across batches (kuq_batches.h)
 };
@@ -254,60 +257,14 @@ int fail(kuq_ctx *c, int code, const char *fmt, ...) {
       return fail(ctx, KUQ_E_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
 
-template <typename T>
-cudaError_t dmalloc(T **p, uint64_t n) { return cudaMalloc((void **)p, n * sizeof(T)); }
-template <typename T>
-cudaError_t hmalloc(T **p, uint64_t n) { return cudaMallocHost((void **)p, n * sizeof(T)); }
-
-void free_slot(Slot &s) {
-  cudaFree(s.d_bases); cudaFree(s.d_clean); cudaFree(s.d_offsets); cudaFree(s.d_unit); cudaFree(s.d_call);
-  cudaFree(s.d_nwin); cudaFree(s.d_codes); cudaFree(s.d_run_start); cudaFree(s.d_run_count); cudaFree(s.d_runs);
-  cudaFree(s.d_scalars); cudaFree(s.d_canon); cudaFree(s.d_bins); cudaFree(s.d_dense); cudaFree(s.d_codes_in); cudaFree(s.d_ovf);
-  cudaFree(s.d_pack); cudaFree(s.d_side);
-  cudaFree(s.u_keys); cudaFree(s.u_inserts); cudaFree(s.u_ncand); cudaFree(s.u_cand); cudaFree(s.u_direct);
-  cudaFree(s.u_codes);
-  cudaFreeHost(s.h_call); cudaFreeHost(s.h_nwin); cudaFreeHost(s.h_run_start); cudaFreeHost(s.h_run_count);
-  cudaFreeHost(s.h_codes); cudaFreeHost(s.h_runs); cudaFreeHost(s.h_scalars); cudaFreeHost(s.h_unit);
-  cudaFree(s.d_fcall); cudaFree(s.d_fhits); cudaFree(s.d_ftotal);
-  cudaFreeHost(s.h_fcall); cudaFreeHost(s.h_fhits); cudaFreeHost(s.h_ftotal);
-  cudaFree(s.d_xsel); cudaFreeHost(s.h_xsel);
-  if (s.ev_k0) cudaEventDestroy(s.ev_k0);
-  if (s.ev_k1) cudaEventDestroy(s.ev_k1);
-  if (s.ev_stage[0]) cudaEventDestroy(s.ev_stage[0]);
-  if (s.ev_stage[1]) cudaEventDestroy(s.ev_stage[1]);
-  if (s.ev_sync) cudaEventDestroy(s.ev_sync);
-  if (s.stream) cudaStreamDestroy(s.stream);
-  s = Slot();
-}
-
 void free_db(kuq_ctx *ctx) {
-  if (ctx->db_owned) { cudaFree(ctx->d_pairs); cudaFree(ctx->d_offsets_owned); }
-  ctx->d_pairs = nullptr; ctx->d_offsets_owned = nullptr; ctx->d_offsets = nullptr;
-  cudaFree(ctx->d_tx_keys); cudaFree(ctx->d_tx_dense); cudaFree(ctx->d_tx_counts);
-  ctx->d_tx_keys = ctx->d_tx_dense = nullptr; ctx->d_tx_counts = nullptr;
-  cudaFree(ctx->d_secondaries);
-  ctx->d_secondaries = nullptr; ctx->n_secondaries = 0; ctx->collisions = 0;
+  ctx->d_pairs_owned.reset(); ctx->d_offsets_owned.reset();
+  ctx->d_pairs = nullptr; ctx->d_offsets = nullptr;
+  ctx->d_tx_keys.reset(); ctx->d_tx_dense.reset(); ctx->d_tx_counts.reset();
+  ctx->d_secondaries.reset();
+  ctx->n_secondaries = 0; ctx->collisions = 0;
   ctx->db_staged = false; ctx->db_remapped = false;
-  for (auto &e : ctx->more) {
-    cudaFree(e.d_pairs); cudaFree(e.d_offsets); cudaFree(e.d_tx_keys); cudaFree(e.d_tx_dense); cudaFree(e.d_tx_counts);
-  }
   ctx->more.clear();
-}
-
-void free_tax_state(kuq_ctx *ctx) {
-  cudaFree(ctx->d_parent); cudaFree(ctx->d_raw); cudaFree(ctx->d_depth);
-  cudaFree(ctx->d_regs); cudaFree(ctx->d_dense_flag); cudaFree(ctx->d_n_kmers); cudaFree(ctx->d_n_reads);
-  cudaFree(ctx->d_reg_floor);
-  cudaFree(ctx->sparse.slots); cudaFree(ctx->d_sparse_used); cudaFree(ctx->sparse.count);
-  cudaFree(ctx->exact.slots); cudaFree(ctx->exact.count); cudaFree(ctx->d_exact_pre);
-  cudaFree(ctx->d_fparent); cudaFree(ctx->d_fdepth); cudaFree(ctx->d_fextra);
-  ctx->exact.slots = nullptr; ctx->exact.count = nullptr; ctx->d_exact_pre = nullptr;
-  ctx->d_fparent = ctx->d_fdepth = ctx->d_fextra = nullptr;
-  ctx->exact_pre.clear();
-  ctx->d_parent = ctx->d_raw = nullptr; ctx->d_depth = nullptr; ctx->d_regs = ctx->d_dense_flag = ctx->d_reg_floor = nullptr;
-  ctx->d_n_kmers = ctx->d_n_reads = nullptr; ctx->sparse.slots = ctx->d_sparse_used = nullptr;
-  ctx->sparse.count = nullptr;
-  ctx->finalized = false;
 }
 
 // ---- Ertl estimator (hyperloglogplus.cpp:373-422,738-752), same operation order as the reference ----------
@@ -350,44 +307,44 @@ uint64_t ertl_sparse_hist(const uint32_t *hist64, uint64_t n_codes, uint64_t n_o
 
 int alloc_slot(kuq_ctx *ctx, Slot &s) {
   const uint64_t mr = ctx->cfg.max_reads_per_batch, mb = ctx->cfg.max_bases_per_batch;
-  CU(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-  CU(cudaEventCreate(&s.ev_k0));
-  CU(cudaEventCreate(&s.ev_k1));
-  CU(cudaEventCreate(&s.ev_stage[0]));
-  CU(cudaEventCreate(&s.ev_stage[1]));
-  CU(cudaEventCreateWithFlags(&s.ev_sync, cudaEventDisableTiming));
-  CU(dmalloc(&s.d_bases, mb + SLACK));
-  CU(dmalloc(&s.d_clean, mb + SLACK));
-  CU(dmalloc(&s.d_offsets, mr + 4));   // + slack: offsets slices are bulk-copied in 16-byte units
-  CU(dmalloc(&s.d_unit, mr));
-  CU(dmalloc(&s.d_call, mr));
-  CU(dmalloc(&s.d_nwin, mr));
-  CU(dmalloc(&s.d_codes, mb + SLACK));
-  CU(dmalloc(&s.d_canon, mb + SLACK));
-  CU(dmalloc(&s.d_bins, mb + SLACK));
-  CU(dmalloc(&s.d_pack, (mb + SLACK) / 32 + 3));   // blocks up to the one after the last text position
-  CU(dmalloc(&s.d_side, (mb + SLACK) / 32 + 3));
-  CU(dmalloc(&s.d_dense, mb + SLACK));
+  CU(s.stream.alloc(cudaStreamNonBlocking));
+  CU(s.ev_k0.alloc(cudaEventDefault));
+  CU(s.ev_k1.alloc(cudaEventDefault));
+  CU(s.ev_stage[0].alloc(cudaEventDefault));
+  CU(s.ev_stage[1].alloc(cudaEventDefault));
+  CU(s.ev_sync.alloc(cudaEventDisableTiming));
+  CU(s.d_bases.alloc(mb + SLACK));
+  CU(s.d_clean.alloc(mb + SLACK));
+  CU(s.d_offsets.alloc(mr + 4));   // + slack: offsets slices are bulk-copied in 16-byte units
+  CU(s.d_unit.alloc(mr));
+  CU(s.d_call.alloc(mr));
+  CU(s.d_nwin.alloc(mr));
+  CU(s.d_codes.alloc(mb + SLACK));
+  CU(s.d_canon.alloc(mb + SLACK));
+  CU(s.d_bins.alloc(mb + SLACK));
+  CU(s.d_pack.alloc((mb + SLACK) / 32 + 3));   // blocks up to the one after the last text position
+  CU(s.d_side.alloc((mb + SLACK) / 32 + 3));
+  CU(s.d_dense.alloc(mb + SLACK));
   // worst case one table of < 4 * windows entries per read: 4 entries (64 B) per base always suffices, but reads that
   // need it are rare: a pool of max(bases / 4, 1 Mi) entries + the largest single table
   s.ovf_entries = std::max<uint64_t>(mb / 4, 1ull << 20);
-  CU(dmalloc(&s.d_ovf, 2 * s.ovf_entries));
-  CU(dmalloc(&s.d_run_start, mr));
-  CU(dmalloc(&s.d_run_count, mr));
+  CU(s.d_ovf.alloc(2 * s.ovf_entries));
+  CU(s.d_run_start.alloc(mr));
+  CU(s.d_run_count.alloc(mr));
   // every resolving warp may leave one partly used block of 256 run slots behind (k_resolve)
   s.runs_cap = mb + SLACK + 256ull * (uint64_t)ctx->n_sm * 64;
   if (s.runs_cap > 0xFFFFFF00ull) s.runs_cap = 0xFFFFFF00ull;   // run indices are 32-bit
-  CU(dmalloc(&s.d_runs, s.runs_cap));
-  CU(dmalloc(&s.d_scalars, 8));
+  CU(s.d_runs.alloc(s.runs_cap));
+  CU(s.d_scalars.alloc(8));
   CU(cudaMemset(s.d_scalars, 0, 8 * 8));           // kuq_sync_slot reads the error word even before the first batch
-  CU(hmalloc(&s.h_call, mr));
-  CU(hmalloc(&s.h_nwin, mr));
-  CU(hmalloc(&s.h_run_start, mr));
-  CU(hmalloc(&s.h_run_count, mr));
-  CU(hmalloc(&s.h_unit, mr));
-  CU(hmalloc(&s.h_scalars, 8));
+  CU(s.h_call.alloc(mr));
+  CU(s.h_nwin.alloc(mr));
+  CU(s.h_run_start.alloc(mr));
+  CU(s.h_run_count.alloc(mr));
+  CU(s.h_unit.alloc(mr));
+  CU(s.h_scalars.alloc(8));
   s.h_runs_cap = std::max<uint64_t>(mr * 8, 1024);
-  CU(hmalloc(&s.h_runs, s.h_runs_cap));
+  CU(s.h_runs.alloc(s.h_runs_cap));
   return KUQ_OK;
 }
 
@@ -399,26 +356,25 @@ int check_slot(kuq_ctx *ctx, uint32_t slot) {
 
 // Scan the staged records for their distinct taxids (+counts): count_taxons (krakendb.cpp:90-113) on the GPU.  The
 // device hash (keys, dense ids to be filled, counts) and the sorted taxids / counts go to the caller's fields.
-int collect_taxids(kuq_ctx *ctx, const uint8_t *pairs, uint64_t key_ct, uint32_t *&d_keys, uint32_t *&d_dense,
-                   unsigned long long *&d_counts, uint32_t &tx_cap, std::vector<uint32_t> &taxids, std::vector<uint64_t> &tcounts) {
+int collect_taxids(kuq_ctx *ctx, const uint8_t *pairs, uint64_t key_ct, DevBuf<uint32_t> &d_keys, DevBuf<uint32_t> &d_dense,
+                   DevBuf<unsigned long long> &d_counts, uint32_t &tx_cap, std::vector<uint32_t> &taxids, std::vector<uint64_t> &tcounts) {
   uint32_t cap = 1u << 16;
   for (;;) {
-    cudaFree(d_keys); cudaFree(d_counts); cudaFree(d_dense);
-    d_keys = d_dense = nullptr; d_counts = nullptr;
-    CU(dmalloc(&d_keys, cap));
-    CU(dmalloc(&d_counts, cap));
-    CU(dmalloc(&d_dense, cap));
+    d_keys.reset(); d_counts.reset(); d_dense.reset();
+    CU(d_keys.alloc(cap));
+    CU(d_counts.alloc(cap));
+    CU(d_dense.alloc(cap));
     CU(cudaMemsetAsync(d_keys, 0, cap * 4ull, ctx->aux));
     CU(cudaMemsetAsync(d_counts, 0, cap * 8ull, ctx->aux));
-    uint32_t *d_over;
-    CU(dmalloc(&d_over, 1));
+    DevBuf<uint32_t> d_over;
+    CU(d_over.alloc(1));
     CU(cudaMemsetAsync(d_over, 0, 4, ctx->aux));
     launch_collect_taxids(pairs, key_ct, d_keys, d_counts, cap - 1, d_over, ctx->aux);
     ctx->launches++;
     uint32_t over = 0;
     CU(cudaMemcpyAsync(&over, d_over, 4, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaStreamSynchronize(ctx->aux));
-    cudaFree(d_over);
+    d_over.reset();
     if (over == 2) return fail(ctx, KUQ_E_DB_FORMAT, "taxid 0xFFFFFFFF is reserved");
     std::vector<uint32_t> keys(cap);
     std::vector<unsigned long long> counts(cap);
@@ -495,15 +451,14 @@ int no_room_for(kuq_ctx *ctx, const ExactTable &, uint64_t incoming, uint64_t ca
 // turns a set word into KUQ_E_CAPACITY with the message (fmt, args).
 template <typename Launch, typename... Args>
 int run_saturating(kuq_ctx *ctx, Launch launch, const char *fmt, Args... args) {
-  uint32_t *d_err = nullptr;
-  CU(dmalloc(&d_err, 1));
+  DevBuf<uint32_t> d_err;
+  CU(d_err.alloc(1));
   CU(cudaMemsetAsync(d_err, 0, 4, ctx->aux));
   launch(d_err);
   ctx->launches++;
   uint32_t err = 0;
   CU(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, ctx->aux));
   CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_err);
   return err ? fail(ctx, KUQ_E_CAPACITY, fmt, args...) : KUQ_OK;
 }
 
@@ -518,7 +473,7 @@ int table_counts(kuq_ctx *ctx, const Table &t, std::vector<Count> &count, uint64
 }
 template <typename Table>
 int table_items(kuq_ctx *ctx, const Table &t, uint64_t *n) {
-  std::vector<std::remove_pointer_t<decltype(t.count)>> count;
+  std::vector<std::remove_pointer_t<decltype(t.count.get())>> count;
   return table_counts(ctx, t, count, n);
 }
 
@@ -532,22 +487,24 @@ uint64_t slots_for(uint64_t n, uint64_t cap, uint64_t tenths) {
 // Re-allocate the table with `cap` slots and re-insert its items (not counted again).  All slots must be idle.
 template <typename Table>
 int grow_table(kuq_ctx *ctx, Table &t, uint64_t cap) {
-  Table bigger = t;
-  bigger.slots = nullptr;
-  bigger.cap = cap;
-  const uint64_t max = max_slots(t);
-  if ((max && cap > max) || dmalloc(&bigger.slots, cap) != cudaSuccess) {
+  decltype(t.slots) bigger;
+  const uint64_t max = max_slots(t), old_cap = t.cap;
+  if ((max && cap > max) || bigger.alloc(cap) != cudaSuccess) {
     (void)cudaGetLastError();
     return fail(ctx, KUQ_E_NOMEM, text(t).no_room_to_grow, (unsigned long long)t.cap, (unsigned long long)cap,
-                cap * (double)sizeof *t.slots / (1ull << 30));
+                cap * (double)sizeof *t.slots.get() / (1ull << 30));
   }
-  CU(cudaMemsetAsync(bigger.slots, 0, cap * sizeof *t.slots, ctx->aux));
-  const int rc = run_saturating(ctx, [&](uint32_t *err) { launch_rehash(t.slots, t.cap, set_view(ctx, bigger), err, ctx->aux); },
-                                "%s saturated while growing to %llu slots", text(t).name, (unsigned long long)cap);
-  if (rc) { cudaFree(bigger.slots); return rc; }
-  cudaFree(t.slots);
-  t.slots = bigger.slots;
+  CU(cudaMemsetAsync(bigger, 0, cap * sizeof *t.slots.get(), ctx->aux));
+  decltype(t.slots) old = std::move(t.slots);
+  t.slots = std::move(bigger);
   t.cap = cap;
+  const int rc = run_saturating(ctx, [&](uint32_t *err) { launch_rehash(old, old_cap, set_view(ctx, t), err, ctx->aux); },
+                                "%s saturated while growing to %llu slots", text(t).name, (unsigned long long)cap);
+  if (rc) {
+    t.slots = std::move(old);
+    t.cap = old_cap;
+    return rc;
+  }
   t.grown++;
   return KUQ_OK;
 }
@@ -587,13 +544,6 @@ int import_items(kuq_ctx *ctx, Table &t, const Item *items, uint64_t n, bool bui
 }
 
 template <typename Table>
-void free_table(Table &t) {
-  cudaFree(t.slots);
-  cudaFree(t.count);
-  t = Table{};
-}
-
-template <typename Table>
 int clear_table(kuq_ctx *ctx, Table &t) {
   CU(cudaMemsetAsync(t.slots, 0, t.cap * sizeof *t.slots, ctx->aux));
   CU(cudaMemsetAsync(t.count, 0, ctx->n_sketch * sizeof *t.count, ctx->aux));
@@ -607,8 +557,8 @@ int clear_table(kuq_ctx *ctx, Table &t) {
 template <typename Table>
 int alloc_table(kuq_ctx *ctx, uint64_t incoming, uint64_t start, uint64_t tenths, Table &t) {
   const uint64_t cap = slots_for(incoming, start, tenths), max = max_slots(t);
-  if ((max && cap > max) || dmalloc(&t.slots, cap) != cudaSuccess || dmalloc(&t.count, ctx->n_sketch) != cudaSuccess) {
-    free_table(t);
+  if ((max && cap > max) || t.slots.alloc(cap) != cudaSuccess || t.count.alloc(ctx->n_sketch) != cudaSuccess) {
+    t = Table{};
     return no_room_for(ctx, t, incoming, cap);
   }
   t.cap = cap;
@@ -618,12 +568,9 @@ int alloc_table(kuq_ctx *ctx, uint64_t incoming, uint64_t start, uint64_t tenths
 // the built table replaces the context's; `upper` bounds its items
 template <typename Table>
 void install_table(Table &t, Table &built, uint64_t upper) {
-  cudaFree(t.slots);
-  cudaFree(t.count);
   built.grown = t.grown + (built.cap != t.cap);
   built.upper = upper;
-  t = built;
-  built = Table{};
+  t = std::move(built);
 }
 
 // The table's items become the received ones (the old ones were exported before), in a table sized for them at a load
@@ -635,12 +582,8 @@ int replace_table(kuq_ctx *ctx, Table &t, const Item *items, uint64_t n, uint64_
   const uint64_t old_cap = t.cap, cap = slots_for(n, start, tenths), max = max_slots(t);
   int rc = KUQ_OK;
   if (cap != old_cap) {
-    cudaFree(t.slots);
-    t.slots = nullptr;
-    if ((max && cap > max) || dmalloc(&t.slots, cap) != cudaSuccess) {
-      t.slots = nullptr;
-      rc = no_room_for(ctx, t, n, cap);
-    }
+    t.slots.reset();
+    if ((max && cap > max) || t.slots.alloc(cap) != cudaSuccess) rc = no_room_for(ctx, t, n, cap);
   }
   t.cap = cap;
   if (!rc) rc = clear_table(ctx, t);
@@ -651,14 +594,10 @@ int replace_table(kuq_ctx *ctx, Table &t, const Item *items, uint64_t n, uint64_
     return KUQ_OK;
   }
   t.cap = old_cap;
-  if (cap != old_cap) {
-    cudaFree(t.slots);
-    if (dmalloc(&t.slots, old_cap) != cudaSuccess) {
-      (void)cudaGetLastError();
-      t.slots = nullptr;
-      t.cap = t.upper = 0;
-      return rc;
-    }
+  if (cap != old_cap && t.slots.alloc(old_cap) != cudaSuccess) {
+    (void)cudaGetLastError();
+    t.cap = t.upper = 0;
+    return rc;
   }
   clear_table(ctx, t);
   return rc;
@@ -668,14 +607,13 @@ int replace_table(kuq_ctx *ctx, Table &t, const Item *items, uint64_t n, uint64_
 // *n = their number.  All slots idle.
 template <typename Item, typename Launch>
 int export_items(kuq_ctx *ctx, Item *out, uint64_t cap, uint64_t *n, const char *items, Launch launch) {
-  unsigned long long *d_n = nullptr;
-  CU(dmalloc(&d_n, 1));
+  DevBuf<unsigned long long> d_n;
+  CU(d_n.alloc(1));
   CU(cudaMemsetAsync(d_n, 0, 8, ctx->aux));
   launch(out, out ? cap : 0, d_n);
   unsigned long long cnt = 0;
   CU(cudaMemcpyAsync(&cnt, d_n, 8, cudaMemcpyDeviceToHost, ctx->aux));
   CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_n);
   *n = cnt;
   if (out && cnt > cap) return fail(ctx, KUQ_E_CAPACITY, "need room for %llu %s", cnt, items);
   return KUQ_OK;
@@ -689,8 +627,8 @@ template <typename Item, typename Scan>
 int export_parts(kuq_ctx *ctx, uint32_t n_parts, uint32_t max_parts, Item *out, uint64_t cap, uint64_t *counts, Item **alloc_out,
                  const TableText &tx, Scan scan) {
   const uint32_t P = max_parts;
-  unsigned long long *d_cnt = nullptr;
-  CU(dmalloc(&d_cnt, 2 * P + 1));                // [0, P) counts / cursors, [P, 2P) part ends, [2P] error word
+  DevBuf<unsigned long long> d_cnt;
+  CU(d_cnt.alloc(2 * P + 1));                    // [0, P) counts / cursors, [P, 2P) part ends, [2P] error word
   CU(cudaMemsetAsync(d_cnt, 0, (2 * P + 1) * 8ull, ctx->aux));
   uint32_t *d_err = reinterpret_cast<uint32_t *>(d_cnt + 2 * P);
   scan(d_cnt, nullptr, nullptr, d_err, 0);
@@ -699,15 +637,16 @@ int export_parts(kuq_ctx *ctx, uint32_t n_parts, uint32_t max_parts, Item *out, 
   CU(cudaStreamSynchronize(ctx->aux));
   uint64_t total = 0;
   for (uint32_t j = 0; j < n_parts; j++) { counts[j] = h[j]; total += h[j]; }
+  DevBuf<Item> owned;                            // alloc_out's buffer until it is handed out
   if (alloc_out) {
-    if (dmalloc(&out, std::max<uint64_t>(total, 1)) != cudaSuccess) {
+    if (owned.alloc(std::max<uint64_t>(total, 1)) != cudaSuccess) {
       (void)cudaGetLastError();
-      cudaFree(d_cnt);
       return fail(ctx, KUQ_E_NOMEM, "no room for %llu exported %s", (unsigned long long)total, tx.items);
     }
+    out = owned;
     cap = total;
   }
-  if (!out) { cudaFree(d_cnt); return KUQ_OK; }     // counts only: nothing was consumed
+  if (!out) return KUQ_OK;                       // counts only: nothing was consumed
   int rc = KUQ_OK;
   if (total > cap) {
     rc = fail(ctx, KUQ_E_CAPACITY, "need room for %llu %s", (unsigned long long)total, tx.items);
@@ -726,10 +665,7 @@ int export_parts(kuq_ctx *ctx, uint32_t n_parts, uint32_t max_parts, Item *out, 
     CU(cudaStreamSynchronize(ctx->aux));
     if (err) rc = fail(ctx, KUQ_E_CAPACITY, tx.overran);
   }
-  cudaFree(d_cnt);
-  if (alloc_out) {
-    if (rc) cudaFree(out); else *alloc_out = out;
-  }
+  if (alloc_out && !rc) *alloc_out = owned.release();
   return rc;
 }
 
@@ -818,15 +754,15 @@ int move_rounds(kuq_ctx *report, const char *no_room, kuq_ctx *src, kuq_ctx *con
   uint64_t round_slots = 1ull << 22;
   if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
   const uint64_t chunk = std::min(round_slots, src->exact.cap);
-  ExactPair *send = nullptr;
-  std::vector<ExactPair *> recv(n, nullptr);
+  DevBuf<ExactPair> send;
+  std::vector<DevBuf<ExactPair>> recv(n);
   int rc = KUQ_OK;
   for (uint32_t o = 0; o <= n && !rc; o++) {     // the round buffer on src's device, then one on each other destination's
     kuq_ctx *c = o < n ? dsts[o] : src;
-    ExactPair *&buf = o < n ? recv[o] : send;
+    DevBuf<ExactPair> &buf = o < n ? recv[o] : send;
     if (o < n && c->device == src->device) continue;
     CU(cudaSetDevice(c->device));
-    if (dmalloc(&buf, std::max<uint64_t>(chunk, 1)) != cudaSuccess) {
+    if (buf.alloc(std::max<uint64_t>(chunk, 1)) != cudaSuccess) {
       (void)cudaGetLastError();
       rc = fail(ctx, KUQ_E_NOMEM, no_room, (unsigned long long)chunk, c->device);
     }
@@ -852,10 +788,6 @@ int move_rounds(kuq_ctx *report, const char *no_room, kuq_ctx *src, kuq_ctx *con
       if (rc && dst != report) report->err = dst->err;
     }
   }
-  for (uint32_t o = 0; o < n; o++)
-    if (recv[o]) { cudaSetDevice(dsts[o]->device); cudaFree(recv[o]); }
-  cudaSetDevice(src->device);
-  cudaFree(send);
   cudaSetDevice(report->device);
   return rc;
 }
@@ -895,9 +827,9 @@ int upload_filter(kuq_ctx *ctx) {
     depth[i] = ctx->f_depth[kv.first];
   }
   extra_raw.push_back(0);                             // never an empty allocation
-  CU(dmalloc(&ctx->d_fparent, n));
-  CU(dmalloc(&ctx->d_fdepth, n));
-  CU(dmalloc(&ctx->d_fextra, extra_raw.size()));
+  CU(ctx->d_fparent.alloc(n));
+  CU(ctx->d_fdepth.alloc(n));
+  CU(ctx->d_fextra.alloc(extra_raw.size()));
   CU(cudaMemcpy(ctx->d_fparent, parent.data(), n * 4, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(ctx->d_fdepth, depth.data(), n * 4, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(ctx->d_fextra, extra_raw.data(), extra_raw.size() * 4, cudaMemcpyHostToDevice));
@@ -966,19 +898,18 @@ int finalize(kuq_ctx *ctx) {
       depth[y] = (uint16_t)d; state[y] = 2;
     }
   }
-  free_tax_state(ctx);
   ctx->parent_dense = parent;
-  CU(dmalloc(&ctx->d_parent, ctx->n_taxa));
-  CU(dmalloc(&ctx->d_raw, ctx->n_taxa));
-  CU(dmalloc(&ctx->d_depth, ctx->n_taxa));
+  CU(ctx->d_parent.alloc(ctx->n_taxa));
+  CU(ctx->d_raw.alloc(ctx->n_taxa));
+  CU(ctx->d_depth.alloc(ctx->n_taxa));
   CU(cudaMemcpy(ctx->d_parent, parent.data(), ctx->n_taxa * 4ull, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(ctx->d_raw, raw.data(), ctx->n_taxa * 4ull, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(ctx->d_depth, depth.data(), ctx->n_taxa * 2ull, cudaMemcpyHostToDevice));
-  CU(dmalloc(&ctx->d_regs, (uint64_t)ctx->n_sketch * HLL_M));
-  CU(dmalloc(&ctx->d_dense_flag, ctx->n_sketch));
-  CU(dmalloc(&ctx->d_reg_floor, ctx->n_sketch));
-  CU(dmalloc(&ctx->d_n_kmers, ctx->n_sketch));
-  CU(dmalloc(&ctx->d_n_reads, ctx->n_taxa));
+  CU(ctx->d_regs.alloc((uint64_t)ctx->n_sketch * HLL_M));
+  CU(ctx->d_dense_flag.alloc(ctx->n_sketch));
+  CU(ctx->d_reg_floor.alloc(ctx->n_sketch));
+  CU(ctx->d_n_kmers.alloc(ctx->n_sketch));
+  CU(ctx->d_n_reads.alloc(ctx->n_taxa));
   CU(cudaMemset(ctx->d_regs, 0, (uint64_t)ctx->n_sketch * HLL_M));
   CU(cudaMemset(ctx->d_dense_flag, 0, ctx->n_sketch));
   CU(cudaMemset(ctx->d_reg_floor, 0, ctx->n_sketch));
@@ -986,15 +917,15 @@ int finalize(kuq_ctx *ctx) {
   CU(cudaMemset(ctx->d_n_reads, 0, ctx->n_taxa * 8ull));
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
     ctx->exact.cap = ctx->cfg.sparse_set_slots;            // entries of 16 B; grows before batches that could fill it
-    CU(dmalloc(&ctx->exact.slots, ctx->exact.cap));
-    CU(dmalloc(&ctx->exact.count, ctx->n_sketch));
+    CU(ctx->exact.slots.alloc(ctx->exact.cap));
+    CU(ctx->exact.count.alloc(ctx->n_sketch));
     int rc = clear_table(ctx, ctx->exact);
     if (rc) return rc;
   } else if (ctx->cfg.hll_mode != KUQ_HLL_DENSE_ONLY) {
     ctx->sparse.cap = ctx->cfg.sparse_set_slots;
-    CU(dmalloc(&ctx->sparse.slots, ctx->sparse.cap));
-    CU(dmalloc(&ctx->d_sparse_used, 1));
-    CU(dmalloc(&ctx->sparse.count, ctx->n_sketch));
+    CU(ctx->sparse.slots.alloc(ctx->sparse.cap));
+    CU(ctx->d_sparse_used.alloc(1));
+    CU(ctx->sparse.count.alloc(ctx->n_sketch));
     CU(cudaMemset(ctx->d_sparse_used, 0, 8));
     int rc = clear_table(ctx, ctx->sparse);
     if (rc) return rc;
@@ -1015,8 +946,8 @@ int remap_values(kuq_ctx *ctx, uint8_t *pairs, uint64_t key_ct, const uint32_t *
       dense[i] = it->second;
     }
   CU(cudaMemcpy(d_dense, dense.data(), tx_cap * 4ull, cudaMemcpyHostToDevice));
-  uint32_t *d_missing;
-  CU(dmalloc(&d_missing, 1));
+  DevBuf<uint32_t> d_missing;
+  CU(d_missing.alloc(1));
   CU(cudaMemset(d_missing, 0, 4));
   launch_remap_values(pairs, key_ct, d_keys, d_dense, tx_cap - 1, d_missing, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1),
                       ctx->aux);
@@ -1024,7 +955,6 @@ int remap_values(kuq_ctx *ctx, uint8_t *pairs, uint64_t key_ct, const uint32_t *
   uint32_t missing = 0;
   CU(cudaMemcpyAsync(&missing, d_missing, 4, cudaMemcpyDeviceToHost, ctx->aux));
   CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_missing);
   if (missing) return fail(ctx, KUQ_E_STATE, "internal: a record value was missing from the taxid table");
   return KUQ_OK;
 }
@@ -1070,7 +1000,7 @@ int exact_preorder(kuq_ctx *ctx) {
     }
   }
   pre.resize(ctx->n_sketch);
-  CU(dmalloc(&ctx->d_exact_pre, ctx->n_sketch));
+  CU(ctx->d_exact_pre.alloc(ctx->n_sketch));
   CU(cudaMemcpy(ctx->d_exact_pre, pre.data(), ctx->n_sketch * 4ull, cudaMemcpyHostToDevice));
   ctx->exact_pre.swap(pre);
   return KUQ_OK;
@@ -1088,8 +1018,8 @@ int exact_books(kuq_ctx *ctx, std::vector<long long> &books) {
   uint64_t n_pairs = 0;
   rc = table_counts(ctx, ctx->exact, count, &n_pairs);
   if (rc) return rc;
-  unsigned long long *d_books = nullptr;
-  CU(dmalloc(&d_books, ctx->n_taxa));
+  DevBuf<unsigned long long> d_books;
+  CU(d_books.alloc(ctx->n_taxa));
   CU(cudaMemsetAsync(d_books, 0, ctx->n_taxa * 8ull, ctx->aux));
   uint64_t budget = 0;
   if (const char *e = getenv("KUQ_EXACT_ROLLUP_BUDGET")) budget = strtoull(e, nullptr, 10);
@@ -1104,7 +1034,7 @@ int exact_books(kuq_ctx *ctx, std::vector<long long> &books) {
   std::vector<unsigned long long> dups(ctx->n_taxa, 0);
   cudaError_t ce = cudaSuccess;
   if (src == 0) ce = cudaMemcpy(dups.data(), d_books, ctx->n_taxa * 8ull, cudaMemcpyDeviceToHost);
-  cudaFree(d_books);
+  d_books.reset();
   if (src == 1) return fail(ctx, KUQ_E_NOMEM, "exact clade roll-up: no device memory for one pass of the sort (budget %llu bytes)", (unsigned long long)budget);
   if (src == 2 || ce != cudaSuccess) return fail(ctx, KUQ_E_CUDA, "exact clade roll-up failed: %s", cudaGetErrorString(cudaGetLastError()));
   books.assign(ctx->n_taxa, 0);
@@ -1124,7 +1054,7 @@ int ensure_collisions(kuq_ctx *ctx) {
   const auto t0 = std::chrono::steady_clock::now();
   // a table above 1/32 of the records (a taxon far above 2^25 records) is not worth it: the set path stays
   const int rc = build_collisions(ctx->d_pairs, ctx->key_ct, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), per_taxon.data(),
-                                  ctx->n_sketch, ctx->key_ct / 32 + 1024, &ctx->d_secondaries, &ctx->n_secondaries, ctx->n_sm, ctx->aux);
+                                  ctx->n_sketch, ctx->key_ct / 32 + 1024, ctx->d_secondaries, &ctx->n_secondaries, ctx->n_sm, ctx->aux);
   ctx->launches += 3;
   ctx->collisions_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   if (rc == 2) return fail(ctx, KUQ_E_CUDA, "building the collision table of the record tier failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -1137,9 +1067,9 @@ int ensure_collisions(kuq_ctx *ctx) {
 
 int harvest_state(kuq_ctx *ctx) {
   if (ctx->d_harvest_stat) return KUQ_OK;
-  CU(dmalloc(&ctx->d_harvest_stat, 3));
+  CU(ctx->d_harvest_stat.alloc(3));
   CU(cudaMemset(ctx->d_harvest_stat, 0, 3 * 8));
-  CU(cudaEventCreate(&ctx->harvest_ev[0])); CU(cudaEventCreate(&ctx->harvest_ev[1]));
+  CU(ctx->harvest_ev[0].alloc(cudaEventDefault)); CU(ctx->harvest_ev[1].alloc(cudaEventDefault));
   return KUQ_OK;
 }
 
@@ -1338,14 +1268,14 @@ void set_unit_ptrs(Params &p, Slot &s);
 int prepare_unit_map(kuq_ctx *ctx, Slot &s) {
   if (ctx->cfg.hll_mode != KUQ_HLL_PRELOAD) return KUQ_OK;
   if (!s.u_keys) {
-    CU(dmalloc(&s.u_keys, UMAP_CAP));
-    CU(dmalloc(&s.u_inserts, UMAP_CAP));
-    CU(dmalloc(&s.u_cand, UMAP_CAP));         // every candidate is a distinct map slot
-    CU(dmalloc(&s.u_ncand, 2));
-    CU(dmalloc(&s.u_codes, (size_t)ctx->n_sm * UNIT_DECIDE_CTAS_PER_SM * 2 * UNIT_CODES));
+    CU(s.u_keys.alloc(UMAP_CAP));
+    CU(s.u_inserts.alloc(UMAP_CAP));
+    CU(s.u_cand.alloc(UMAP_CAP));             // every candidate is a distinct map slot
+    CU(s.u_ncand.alloc(2));
+    CU(s.u_codes.alloc((size_t)ctx->n_sm * UNIT_DECIDE_CTAS_PER_SM * 2 * UNIT_CODES));
     const uint64_t rows = unit_table_rows(ctx);
     s.u_direct_rows = (uint32_t)rows;
-    if (rows) CU(dmalloc(&s.u_direct, rows * ctx->n_sketch));
+    if (rows) CU(s.u_direct.alloc(rows * ctx->n_sketch));
   }
   Params tmp;
   set_unit_ptrs(tmp, s);
@@ -1579,7 +1509,10 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
     if (mrc) return mrc;
     if (mode != MODE_LOOKUP) CU(cudaMemsetAsync(p.chunk_counter, 0, 4, s.stream));   // k_scan of the resolve half
   }
-  if (p.n_reads && !(multi && mode == MODE_LOOKUP)) ctx->launches += launch_classify(mode, p, ctx->n_sm, s.stream, s.ev_stage);
+  if (p.n_reads && !(multi && mode == MODE_LOOKUP)) {
+    cudaEvent_t stage[2] = {s.ev_stage[0], s.ev_stage[1]};
+    ctx->launches += launch_classify(mode, p, ctx->n_sm, s.stream, stage);
+  }
   if (p.n_reads && mode != MODE_LOOKUP && ctx->extract_set) {          // after whichever resolve wrote the calls
     CU(cudaMemsetAsync(s.d_xsel + extract_count_at(ctx), 0, 4, s.stream));
     launch_extract_select(p.call, p.fcall, p.n_reads, ctx->d_members, ctx->n_members, ctx->extract_flags, s.d_xsel,
@@ -1683,7 +1616,7 @@ int kuq_create(const kuq_config *cfg_in, kuq_ctx **out) {
   ctx->cfg = cfg;
   ctx->device = cfg.device;
   ctx->n_sm = prop.multiProcessorCount;
-  if (cudaStreamCreateWithFlags(&ctx->aux, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return KUQ_E_CUDA; }
+  if (ctx->aux.alloc(cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return KUQ_E_CUDA; }
   ctx->slots.resize(cfg.n_slots);
   for (auto &s : ctx->slots) {
     int rc = alloc_slot(ctx, s);
@@ -1701,15 +1634,6 @@ void kuq_destroy(kuq_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
-  for (auto &s : ctx->slots) free_slot(s);
-  stream_close(ctx);
-  free_db(ctx);
-  free_tax_state(ctx);
-  cudaFree(ctx->d_members);                  // raw taxids: kept when finalize renumbers the taxonomy
-  cudaFree(ctx->d_sync_err);
-  cudaFree(ctx->d_harvest_stat);
-  for (cudaEvent_t e : ctx->harvest_ev) if (e) cudaEventDestroy(e);
-  if (ctx->aux) cudaStreamDestroy(ctx->aux);
   delete ctx;
 }
 
@@ -1774,9 +1698,9 @@ int upload_db(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi, u
   {
     PinnedBounce bounce;
     CU(bounce.init());
-    uint8_t *d_land = nullptr;
+    DevBuf<uint8_t> d_land;
     const uint64_t land_rec = pair_sz == 12 ? 0 : std::min(landing_records(pair_sz), PinnedBounce::CH / pair_sz);
-    if (land_rec && n_rec) CU(cudaMalloc((void **)&d_land, land_rec * pair_sz + SLACK));
+    if (land_rec && n_rec) CU(d_land.alloc(land_rec * pair_sz + SLACK));
     // rec_sz = 0: bytes are copied to d_dst as they are; else they are records of rec_sz bytes, widened into d_dst
     auto piece_copy = [&](uint8_t *d_dst, const uint8_t *h_src, uint64_t bytes, uint64_t rec_sz) -> int {
       if (!rec_sz) {
@@ -1796,7 +1720,6 @@ int upload_db(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi, u
     int crc = piece_copy(d_pairs, f.records + rec_lo * pair_sz, n_rec * pair_sz, pair_sz == 12 ? 0 : pair_sz);
     if (!crc) crc = piece_copy(reinterpret_cast<uint8_t *>(d_offsets), reinterpret_cast<const uint8_t *>(f.offsets + bin_lo),
                                (bin_hi - bin_lo + 1) * 8, 0);
-    cudaFree(d_land);
     if (crc) return crc;
   }
   return KUQ_OK;
@@ -1818,8 +1741,9 @@ int stage_first(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi)
   ctx->rec_base = rec_lo;
   ctx->key_ct = rec_hi - rec_lo;
   ctx->db_owned = true;
-  CU(cudaMalloc((void **)&ctx->d_pairs, ctx->key_ct * 12 + SLACK));
-  CU(dmalloc(&ctx->d_offsets_owned, bin_hi - bin_lo + 1));
+  CU(ctx->d_pairs_owned.alloc(ctx->key_ct * 12 + SLACK));
+  CU(ctx->d_offsets_owned.alloc(bin_hi - bin_lo + 1));
+  ctx->d_pairs = ctx->d_pairs_owned;
   ctx->d_offsets = ctx->d_offsets_owned;
   int rc = upload_db(ctx, f, bin_lo, bin_hi, ctx->d_pairs, ctx->d_offsets_owned);
   if (rc) return rc;
@@ -1867,17 +1791,13 @@ int kuq_stage_db_append_range(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_
   e.bin_lo = bin_lo; e.bin_hi = bin_hi;
   e.nt = f.nt; e.idx_type = f.idx_type;
   auto drop = [&](int code) { ctx->more.pop_back(); return code; };
-  if (dmalloc(&e.d_pairs, e.key_ct * 12 + SLACK) != cudaSuccess || dmalloc(&e.d_offsets, bin_hi - bin_lo + 1) != cudaSuccess) {
+  if (e.d_pairs.alloc(e.key_ct * 12 + SLACK) != cudaSuccess || e.d_offsets.alloc(bin_hi - bin_lo + 1) != cudaSuccess) {
     (void)cudaGetLastError();
-    cudaFree(e.d_pairs); cudaFree(e.d_offsets);
     return drop(fail(ctx, KUQ_E_NOMEM, "no room for database %zu (%llu records)", ctx->more.size() + 1, (unsigned long long)e.key_ct));
   }
   rc = upload_db(ctx, f, bin_lo, bin_hi, e.d_pairs, e.d_offsets);
   if (!rc) rc = collect_taxids(ctx, e.d_pairs, e.key_ct, e.d_tx_keys, e.d_tx_dense, e.d_tx_counts, e.tx_cap, e.taxids, e.counts);
-  if (rc) {
-    cudaFree(e.d_pairs); cudaFree(e.d_offsets); cudaFree(e.d_tx_keys); cudaFree(e.d_tx_dense); cudaFree(e.d_tx_counts);
-    return drop(rc);
-  }
+  if (rc) return drop(rc);
   if (ctx->finalized) return remap_db(ctx);
   return KUQ_OK;
 }
@@ -2008,12 +1928,12 @@ int kuq_set_threshold(kuq_ctx *ctx, double threshold, const uint32_t *taxid, con
   CU(cudaSetDevice(ctx->device));
   const uint64_t mr = ctx->cfg.max_reads_per_batch;
   for (auto &s : ctx->slots) {
-    CU(dmalloc(&s.d_fcall, mr));
-    CU(dmalloc(&s.d_fhits, mr));
-    CU(dmalloc(&s.d_ftotal, mr));
-    CU(hmalloc(&s.h_fcall, mr));
-    CU(hmalloc(&s.h_fhits, mr));
-    CU(hmalloc(&s.h_ftotal, mr));
+    CU(s.d_fcall.alloc(mr));
+    CU(s.d_fhits.alloc(mr));
+    CU(s.d_ftotal.alloc(mr));
+    CU(s.h_fcall.alloc(mr));
+    CU(s.h_fhits.alloc(mr));
+    CU(s.h_ftotal.alloc(mr));
   }
   ctx->f_parent.swap(F);
   ctx->f_depth.swap(depth);
@@ -2087,11 +2007,11 @@ int kuq_set_extract(kuq_ctx *ctx, const uint32_t *list, uint32_t n_list, uint32_
   const uint32_t n_members = (uint32_t)sorted.size();
   sorted.push_back(0);                                  // never an empty allocation
   CU(cudaSetDevice(ctx->device));
-  CU(dmalloc(&ctx->d_members, sorted.size()));
+  CU(ctx->d_members.alloc(sorted.size()));
   CU(cudaMemcpy(ctx->d_members, sorted.data(), sorted.size() * 4, cudaMemcpyHostToDevice));
   for (auto &s : ctx->slots) {
-    CU(dmalloc(&s.d_xsel, extract_count_at(ctx) + 16));
-    CU(hmalloc(&s.h_xsel, extract_count_at(ctx) + 16));
+    CU(s.d_xsel.alloc(extract_count_at(ctx) + 16));
+    CU(s.h_xsel.alloc(extract_count_at(ctx) + 16));
   }
   ctx->n_members = n_members;
   ctx->extract_flags = flags;
@@ -2188,7 +2108,7 @@ int kuq_resolve_batch(kuq_ctx *ctx, const char *bases, const uint64_t *read_offs
   uint64_t total = 0;
   rc = upload_reads(ctx, s, bases, read_offsets, n_reads, &total);
   if (rc) return rc;
-  if (!s.d_codes_in) CU(dmalloc(&s.d_codes_in, ctx->cfg.max_bases_per_batch + SLACK));
+  if (!s.d_codes_in) CU(s.d_codes_in.alloc(ctx->cfg.max_bases_per_batch + SLACK));
   if (n_reads) CU(cudaMemcpyAsync(s.d_codes_in, codes_in, total * 4, cudaMemcpyHostToDevice, s.stream));
   s.n_reads = n_reads; s.flags = flags; s.total_bases = total; s.external = false;
   const uint32_t *d_unit = nullptr;
@@ -2262,15 +2182,13 @@ int kuq_wait_batch(kuq_ctx *ctx, uint32_t slot, kuq_batch_result *out) {
   const uint64_t n_runs = (s.flags & KUQ_F_NO_RUNS) ? 0 : s.h_scalars[0];
   if (n_runs) {
     if (n_runs > s.h_runs_cap) {
-      cudaFreeHost(s.h_runs);
-      s.h_runs = nullptr;
       s.h_runs_cap = n_runs + n_runs / 2;
-      CU(hmalloc(&s.h_runs, s.h_runs_cap));
+      CU(s.h_runs.alloc(s.h_runs_cap));
     }
     CU(cudaMemcpyAsync(s.h_runs, s.d_runs, n_runs * 8, cudaMemcpyDeviceToHost, s.stream));
   }
   if ((s.flags & KUQ_F_WANT_CODES) && s.total_bases) {
-    if (!s.h_codes) CU(hmalloc(&s.h_codes, ctx->cfg.max_bases_per_batch));
+    if (!s.h_codes) CU(s.h_codes.alloc(ctx->cfg.max_bases_per_batch));
     CU(cudaMemcpyAsync(s.h_codes, s.d_codes, s.total_bases * 4, cudaMemcpyDeviceToHost, s.stream));
   }
   CU(cudaStreamSynchronize(s.stream));
@@ -2282,7 +2200,7 @@ int kuq_wait_batch(kuq_ctx *ctx, uint32_t slot, kuq_batch_result *out) {
   out->run_count = s.h_run_count;
   out->runs = s.h_runs;
   out->n_runs = n_runs;
-  out->codes = (s.flags & KUQ_F_WANT_CODES) ? s.h_codes : nullptr;
+  out->codes = (s.flags & KUQ_F_WANT_CODES) ? s.h_codes.get() : nullptr;
   out->n_classified = s.h_scalars[1];
   out->kernel_ms = s.kernel_ms;
   if (ctx->filter_set) {
@@ -2493,8 +2411,8 @@ int kuq_slot_device_result(kuq_ctx *ctx, uint32_t slot, kuq_device_result *out) 
   out->d_codes = s.d_codes;
   out->d_run_start = s.d_run_start;
   out->d_run_count = s.d_run_count;
-  out->d_runs = reinterpret_cast<const kuq_run *>(s.d_runs);
-  out->d_n_runs = reinterpret_cast<const uint64_t *>(s.d_scalars);
+  out->d_runs = reinterpret_cast<const kuq_run *>(s.d_runs.get());
+  out->d_n_runs = reinterpret_cast<const uint64_t *>(s.d_scalars.get());
   return KUQ_OK;
 }
 
@@ -2512,7 +2430,7 @@ int kuq_slot_stats(kuq_ctx *ctx, uint32_t slot, uint64_t *n_lookups, uint64_t *s
 
 void *kuq_slot_stream(kuq_ctx *ctx, uint32_t slot) {
   if (!ctx || slot >= ctx->slots.size()) return nullptr;
-  return (void *)ctx->slots[slot].stream;
+  return (void *)ctx->slots[slot].stream.get();
 }
 uint64_t kuq_launch_count(const kuq_ctx *ctx) { return ctx ? ctx->launches : 0; }
 double kuq_last_kernel_ms(kuq_ctx *ctx, uint32_t slot) {
@@ -2559,13 +2477,14 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
   h.distinct.assign(ctx->n_sketch, 0);
   CU(cudaMemcpy(h.n_kmers.data(), ctx->d_n_kmers, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
   CU(cudaMemcpy(h.n_reads.data(), ctx->d_n_reads, ctx->n_taxa * 8ull, cudaMemcpyDeviceToHost));
-  uint32_t *d_hist;
-  CU(dmalloc(&d_hist, (uint64_t)ctx->n_sketch * 64));
-  launch_register_histograms(ctx->d_regs, ctx->n_sketch, d_hist, ctx->aux);
-  ctx->launches++;
-  CU(cudaMemcpyAsync(h.hist.data(), d_hist, (uint64_t)ctx->n_sketch * 64 * 4, cudaMemcpyDeviceToHost, ctx->aux));
-  CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_hist);
+  {
+    DevBuf<uint32_t> d_hist;
+    CU(d_hist.alloc((uint64_t)ctx->n_sketch * 64));
+    launch_register_histograms(ctx->d_regs, ctx->n_sketch, d_hist, ctx->aux);
+    ctx->launches++;
+    CU(cudaMemcpyAsync(h.hist.data(), d_hist, (uint64_t)ctx->n_sketch * 64 * 4, cudaMemcpyDeviceToHost, ctx->aux));
+    CU(cudaStreamSynchronize(ctx->aux));
+  }
   if (ctx->cfg.hll_mode == KUQ_HLL_EXACT) {
     h.exact.resize(ctx->n_sketch);
     CU(cudaMemcpy(h.exact.data(), ctx->exact.count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
@@ -2575,8 +2494,8 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
       launch_flag_dense_global(ctx->sparse.count, ctx->d_dense_flag, ctx->n_sketch, ctx->aux);
       ctx->launches++;
     }
-    uint32_t *d_sh;
-    CU(dmalloc(&d_sh, (uint64_t)ctx->n_sketch * 64));
+    DevBuf<uint32_t> d_sh;
+    CU(d_sh.alloc((uint64_t)ctx->n_sketch * 64));
     CU(cudaMemsetAsync(d_sh, 0, (uint64_t)ctx->n_sketch * 64 * 4, ctx->aux));
     launch_sparse_histograms(set_keys(ctx), ctx->d_dense_flag, d_sh, ctx->aux);
     launch_sparse_histograms(kept_keys(ctx), ctx->d_dense_flag, d_sh, ctx->aux);
@@ -2586,7 +2505,6 @@ int fetch_counts(kuq_ctx *ctx, CountsHost &h) {
     CU(cudaMemcpyAsync(h.dense_flag.data(), ctx->d_dense_flag, ctx->n_sketch, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaMemcpyAsync(h.distinct.data(), ctx->sparse.count, ctx->n_sketch * 4ull, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaStreamSynchronize(ctx->aux));
-    cudaFree(d_sh);
     if (ctx->merged_summary) {             // sums over the code partitions of all GPUs (kuq_set_sparse_summary)
       h.sparse_hist = ctx->merged_hist;
       h.distinct = ctx->merged_distinct;
@@ -2623,10 +2541,12 @@ int clade_hist(kuq_ctx *ctx, const std::vector<uint32_t> &members, uint32_t *his
     for (uint32_t d : members) member[d] = 1;
     uint64_t cap = 1024;
     while (cap < 2 * sum_distinct + 16) cap <<= 1;
-    uint8_t *d_member; unsigned long long *d_set; uint32_t *d_hist;
-    CU(dmalloc(&d_member, ctx->n_sketch));
-    CU(dmalloc(&d_set, cap));
-    CU(dmalloc(&d_hist, 65));
+    DevBuf<uint8_t> d_member;
+    DevBuf<unsigned long long> d_set;
+    DevBuf<uint32_t> d_hist;
+    CU(d_member.alloc(ctx->n_sketch));
+    CU(d_set.alloc(cap));
+    CU(d_hist.alloc(65));
     CU(cudaMemcpyAsync(d_member, member.data(), ctx->n_sketch, cudaMemcpyHostToDevice, ctx->aux));
     CU(cudaMemsetAsync(d_set, 0, cap * 8, ctx->aux));
     CU(cudaMemsetAsync(d_hist, 0, 65 * 4, ctx->aux));
@@ -2636,22 +2556,21 @@ int clade_hist(kuq_ctx *ctx, const std::vector<uint32_t> &members, uint32_t *his
     uint32_t hist[65];
     CU(cudaMemcpyAsync(hist, d_hist, sizeof hist, cudaMemcpyDeviceToHost, ctx->aux));
     CU(cudaStreamSynchronize(ctx->aux));
-    cudaFree(d_member); cudaFree(d_set); cudaFree(d_hist);
     if (hist[64]) return fail(ctx, KUQ_E_CAPACITY, "internal: clade union scratch overflow");
     memcpy(hist64, hist, 64 * sizeof(uint32_t));
     return KUQ_OK;
   }
-  uint32_t *d_members; uint8_t *d_out; uint32_t *d_hist;
-  CU(dmalloc(&d_members, members.size()));
-  CU(dmalloc(&d_out, HLL_M));
-  CU(dmalloc(&d_hist, 64));
+  DevBuf<uint32_t> d_members, d_hist;
+  DevBuf<uint8_t> d_out;
+  CU(d_members.alloc(members.size()));
+  CU(d_out.alloc(HLL_M));
+  CU(d_hist.alloc(64));
   CU(cudaMemcpyAsync(d_members, members.data(), members.size() * 4, cudaMemcpyHostToDevice, ctx->aux));
   launch_clade_max(ctx->d_regs, d_members, (uint32_t)members.size(), d_out, ctx->aux);
   launch_register_histograms(d_out, 1, d_hist, ctx->aux);
   ctx->launches += 2;
   CU(cudaMemcpyAsync(hist64, d_hist, 64 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->aux));
   CU(cudaStreamSynchronize(ctx->aux));
-  cudaFree(d_members); cudaFree(d_out); cudaFree(d_hist);
   return KUQ_OK;
 }
 }  // namespace
@@ -2741,10 +2660,11 @@ int kuq_clade_counts(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t 
       for (uint32_t d : members) member[d] = 1;
       uint64_t cap = 1024;
       while (cap < 2 * sum + 16) cap <<= 1;
-      uint8_t *d_member; unsigned long long *d_set; unsigned long long *d_cnt;
-      CU(dmalloc(&d_member, ctx->n_sketch));
-      CU(dmalloc(&d_set, cap));
-      CU(dmalloc(&d_cnt, 2));
+      DevBuf<uint8_t> d_member;
+      DevBuf<unsigned long long> d_set, d_cnt;
+      CU(d_member.alloc(ctx->n_sketch));
+      CU(d_set.alloc(cap));
+      CU(d_cnt.alloc(2));
       CU(cudaMemcpyAsync(d_member, member.data(), ctx->n_sketch, cudaMemcpyHostToDevice, ctx->aux));
       CU(cudaMemsetAsync(d_set, 0, cap * 8, ctx->aux));
       CU(cudaMemsetAsync(d_cnt, 0, 16, ctx->aux));
@@ -2753,7 +2673,6 @@ int kuq_clade_counts(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t 
       unsigned long long out[2];
       CU(cudaMemcpyAsync(out, d_cnt, 16, cudaMemcpyDeviceToHost, ctx->aux));
       CU(cudaStreamSynchronize(ctx->aux));
-      cudaFree(d_member); cudaFree(d_set); cudaFree(d_cnt);
       if (out[1]) return fail(ctx, KUQ_E_CAPACITY, "internal: clade union scratch overflow");
       u = out[0];
     }
@@ -2927,13 +2846,13 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
       if (pass == 0) { for (size_t i = 1; i < offs.size(); i++) offs[i] += offs[i - 1]; mem.resize(offs.back()); }
     }
     const uint32_t CH = 8192;                                // clades per launch: 32 MB of folded registers
-    uint32_t *d_offs = nullptr, *d_mem = nullptr, *d_hist = nullptr;
-    uint8_t *d_out = nullptr;
+    DevBuf<uint32_t> d_offs, d_mem, d_hist;
+    DevBuf<uint8_t> d_out;
     std::vector<uint32_t> hist((size_t)CH * 64), loc;
-    CU(dmalloc(&d_offs, CH + 1));
-    CU(dmalloc(&d_mem, std::max<size_t>(mem.size(), 1)));
-    CU(dmalloc(&d_out, (uint64_t)CH * HLL_M));
-    CU(dmalloc(&d_hist, (uint64_t)CH * 64));
+    CU(d_offs.alloc(CH + 1));
+    CU(d_mem.alloc(std::max<size_t>(mem.size(), 1)));
+    CU(d_out.alloc((uint64_t)CH * HLL_M));
+    CU(d_hist.alloc((uint64_t)CH * 64));
     CU(cudaMemcpyAsync(d_mem, mem.data(), mem.size() * 4, cudaMemcpyHostToDevice, ctx->aux));
     for (uint32_t a = 0; a < dense_list.size(); a += CH) {
       const uint32_t m = std::min<uint32_t>(CH, (uint32_t)dense_list.size() - a);
@@ -2949,7 +2868,6 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
         c_unique[c] = ertl_dense_hist(&hist[(size_t)i * 64], c_kmers[c]);
       }
     }
-    cudaFree(d_offs); cudaFree(d_mem); cudaFree(d_out); cudaFree(d_hist);
   }
   // ---- sparse clades with several members: distinct codes of every subtree from one sort ------------------------------
   if (!sparse_multi.empty()) {
@@ -2982,26 +2900,28 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
       const uint32_t d = nodes[c];
       if (d < NS) { pre_of_taxon[d] = pre[c]; if (has_kmers(d) && !h.dense_flag[d]) n_keys += h.distinct[d]; }
     }
-    uint32_t *d_pre = nullptr, *d_nop = nullptr, *d_par = nullptr, *d_dep = nullptr, *d_dup = nullptr;
-    int32_t *d_sid = nullptr;
-    CU(dmalloc(&d_pre, NS)); CU(dmalloc(&d_nop, NC)); CU(dmalloc(&d_par, NC)); CU(dmalloc(&d_dep, NC)); CU(dmalloc(&d_sid, NC));
-    CU(dmalloc(&d_dup, sparse_multi.size() * 64));
-    CU(cudaMemcpyAsync(d_pre, pre_of_taxon.data(), NS * 4ull, cudaMemcpyHostToDevice, ctx->aux));
-    CU(cudaMemcpyAsync(d_nop, node_of_pre.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
-    CU(cudaMemcpyAsync(d_par, parent_c.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
-    CU(cudaMemcpyAsync(d_dep, depth_c.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
-    CU(cudaMemcpyAsync(d_sid, sid.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
-    CU(cudaMemsetAsync(d_dup, 0, sparse_multi.size() * 64 * 4ull, ctx->aux));
-    const int src = sparse_clade_dups(set_keys(ctx), kept_keys(ctx), ctx->d_dense_flag, n_keys, d_pre, d_nop, d_par, d_dep,
-                                      d_sid, d_dup, ctx->n_sm, ctx->aux);
-    ctx->launches += 3;
     std::vector<uint32_t> dup(sparse_multi.size() * 64, 0);
+    int src = 0;
     cudaError_t ce = cudaSuccess;
-    if (src == 0) {
-      ce = cudaMemcpyAsync(dup.data(), d_dup, dup.size() * 4, cudaMemcpyDeviceToHost, ctx->aux);
-      if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->aux);
+    {
+      DevBuf<uint32_t> d_pre, d_nop, d_par, d_dep, d_dup;
+      DevBuf<int32_t> d_sid;
+      CU(d_pre.alloc(NS)); CU(d_nop.alloc(NC)); CU(d_par.alloc(NC)); CU(d_dep.alloc(NC)); CU(d_sid.alloc(NC));
+      CU(d_dup.alloc(sparse_multi.size() * 64));
+      CU(cudaMemcpyAsync(d_pre, pre_of_taxon.data(), NS * 4ull, cudaMemcpyHostToDevice, ctx->aux));
+      CU(cudaMemcpyAsync(d_nop, node_of_pre.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
+      CU(cudaMemcpyAsync(d_par, parent_c.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
+      CU(cudaMemcpyAsync(d_dep, depth_c.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
+      CU(cudaMemcpyAsync(d_sid, sid.data(), NC * 4ull, cudaMemcpyHostToDevice, ctx->aux));
+      CU(cudaMemsetAsync(d_dup, 0, sparse_multi.size() * 64 * 4ull, ctx->aux));
+      src = sparse_clade_dups(set_keys(ctx), kept_keys(ctx), ctx->d_dense_flag, n_keys, d_pre, d_nop, d_par, d_dep, d_sid, d_dup,
+                              ctx->n_sm, ctx->aux);
+      ctx->launches += 3;
+      if (src == 0) {
+        ce = cudaMemcpyAsync(dup.data(), d_dup, dup.size() * 4, cudaMemcpyDeviceToHost, ctx->aux);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->aux);
+      }
     }
-    cudaFree(d_pre); cudaFree(d_nop); cudaFree(d_par); cudaFree(d_dep); cudaFree(d_sid); cudaFree(d_dup);
     if (src == 2 || ce != cudaSuccess) return fail(ctx, KUQ_E_CUDA, "clade roll-up (sparse tier) failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (src == 1) {
       sparse_fallback = true;                                // no room for the sort: one union per clade instead
@@ -3071,8 +2991,8 @@ int kuq_state_ptrs_get(kuq_ctx *ctx, kuq_state_ptrs *out) {
   if (rc) return rc;
   out->d_regs = ctx->d_regs;
   out->regs_bytes = (uint64_t)ctx->n_sketch * HLL_M;
-  out->d_n_kmers = reinterpret_cast<uint64_t *>(ctx->d_n_kmers);
-  out->d_n_reads = reinterpret_cast<uint64_t *>(ctx->d_n_reads);
+  out->d_n_kmers = reinterpret_cast<uint64_t *>(ctx->d_n_kmers.get());
+  out->d_n_reads = reinterpret_cast<uint64_t *>(ctx->d_n_reads.get());
   out->d_dense_flag = ctx->d_dense_flag;
   out->n_sketch = ctx->n_sketch;
   out->n_taxa = ctx->n_taxa;
@@ -3121,17 +3041,10 @@ uint32_t host_hash_u32(uint32_t x) {                        // == hash_u32 of ku
   return x;
 }
 void stream_close(kuq_ctx *ctx) {
-  for (auto &b : ctx->sbuf) {
-    cudaFree(b.d_pairs); cudaFree(b.d_offsets);
-    if (b.ready) cudaEventDestroy(b.ready);
-    b = kuq_ctx::StreamBuf();
-  }
-  if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  ctx->copy_stream = nullptr;
-  cudaFree(ctx->d_stream_missing);
-  ctx->d_stream_missing = nullptr;
-  cudaFree(ctx->d_stream_land);
-  ctx->d_stream_land = nullptr;
+  for (auto &b : ctx->sbuf) b = kuq_ctx::StreamBuf();
+  ctx->copy_stream.reset();
+  ctx->d_stream_missing.reset();
+  ctx->d_stream_land.reset();
   if (ctx->stream_open) { ctx->d_pairs = nullptr; ctx->d_offsets = nullptr; ctx->db_staged = false; }
   ctx->stream_open = false;
 }
@@ -3168,25 +3081,25 @@ int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, ui
     keys[slot] = t + 1;
     dense[slot] = ctx->dense_of_raw[t];
   }
-  CU(dmalloc(&ctx->d_tx_keys, cap));
-  CU(dmalloc(&ctx->d_tx_dense, cap));
+  CU(ctx->d_tx_keys.alloc(cap));
+  CU(ctx->d_tx_dense.alloc(cap));
   CU(cudaMemcpy(ctx->d_tx_keys, keys.data(), cap * 4ull, cudaMemcpyHostToDevice));
   CU(cudaMemcpy(ctx->d_tx_dense, dense.data(), cap * 4ull, cudaMemcpyHostToDevice));
   ctx->tx_cap = cap;
   ctx->db_remapped = true;                       // each range is remapped as it arrives
-  CU(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-  CU(dmalloc(&ctx->d_stream_missing, 1));
+  CU(ctx->copy_stream.alloc(cudaStreamNonBlocking));
+  CU(ctx->d_stream_missing.alloc(1));
   CU(cudaMemset(ctx->d_stream_missing, 0, 4));
   for (auto &b : ctx->sbuf) {
-    CU(cudaMalloc((void **)&b.d_pairs, max_records * 12 + SLACK));
-    CU(dmalloc(&b.d_offsets, max_bins + 1));
-    CU(cudaEventCreateWithFlags(&b.ready, cudaEventDisableTiming));
+    CU(b.d_pairs.alloc(max_records * 12 + SLACK));
+    CU(b.d_offsets.alloc(max_bins + 1));
+    CU(b.ready.alloc(cudaEventDisableTiming));
   }
   ctx->stream_pair_sz = (2 * k + 7) / 8 + 4;     // the file's record size: key_len + 4 (krakendb.cpp:76,176)
   ctx->stream_land_rec = 0;
   if (ctx->stream_pair_sz != 12) {               // k <= 28: one landing zone, the pieces of both buffers pass through in turn
     ctx->stream_land_rec = std::min(landing_records(ctx->stream_pair_sz), max_records);
-    CU(cudaMalloc((void **)&ctx->d_stream_land, ctx->stream_land_rec * ctx->stream_pair_sz + SLACK));
+    CU(ctx->d_stream_land.alloc(ctx->stream_land_rec * ctx->stream_pair_sz + SLACK));
   }
   ctx->stream_cap_records = max_records;
   ctx->stream_cap_bins = max_bins;
@@ -3291,15 +3204,15 @@ static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets) {
   for (auto &s : src->slots) CU(cudaStreamSynchronize(s.stream));
   { int rc = harvest_seen(src, false); if (rc) { dst->err = src->err; return rc; } }
   uint64_t n_keys = 0;
-  uint64_t *d_keys_src = nullptr;
+  DevBuf<uint64_t> d_keys_src;                   // on src's device
   if (src->sparse.slots && !exact && sets) {
     int rc = kuq_sparse_export(src, nullptr, 0, &n_keys);
     if (rc) { dst->err = src->err; return rc; }
     if (n_keys) {
-      if (cudaMalloc((void **)&d_keys_src, n_keys * 8) != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, KUQ_E_NOMEM, "no room for %llu keys", (unsigned long long)n_keys); }
+      if (d_keys_src.alloc(n_keys) != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, KUQ_E_NOMEM, "no room for %llu keys", (unsigned long long)n_keys); }
       uint64_t n2 = 0;
       rc = kuq_sparse_export(src, d_keys_src, n_keys, &n2);
-      if (rc) { cudaFree(d_keys_src); dst->err = src->err; return rc; }
+      if (rc) { dst->err = src->err; return rc; }
       n_keys = n2;
     }
   }
@@ -3310,31 +3223,31 @@ static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets) {
   dst->snap_valid = false;
   dst->merged_summary = false;
   dst->merged_exact = false;
-  uint8_t *t_regs, *t_dense; unsigned long long *t_nk, *t_nr;
-  const uint64_t reg_bytes = (uint64_t)dst->n_sketch * HLL_M;
-  CU(cudaMalloc((void **)&t_regs, reg_bytes));
-  CU(dmalloc(&t_dense, dst->n_sketch));
-  CU(dmalloc(&t_nk, dst->n_sketch));
-  CU(dmalloc(&t_nr, dst->n_taxa));
-  CU(cudaMemcpyPeer(t_regs, dst->device, src->d_regs, src->device, reg_bytes));
-  CU(cudaMemcpyPeer(t_dense, dst->device, src->d_dense_flag, src->device, dst->n_sketch));
-  CU(cudaMemcpyPeer(t_nk, dst->device, src->d_n_kmers, src->device, dst->n_sketch * 8ull));
-  CU(cudaMemcpyPeer(t_nr, dst->device, src->d_n_reads, src->device, dst->n_taxa * 8ull));
-  launch_merge_state(dst->d_regs, t_regs, dst->d_n_kmers, t_nk, dst->n_sketch, dst->d_n_reads, t_nr, dst->n_taxa, dst->d_dense_flag,
-                     t_dense, dst->aux);
-  dst->launches++;
-  CU(cudaStreamSynchronize(dst->aux));
-  cudaFree(t_regs); cudaFree(t_dense); cudaFree(t_nk); cudaFree(t_nr);
+  {
+    DevBuf<uint8_t> t_regs, t_dense;
+    DevBuf<unsigned long long> t_nk, t_nr;
+    const uint64_t reg_bytes = (uint64_t)dst->n_sketch * HLL_M;
+    CU(t_regs.alloc(reg_bytes));
+    CU(t_dense.alloc(dst->n_sketch));
+    CU(t_nk.alloc(dst->n_sketch));
+    CU(t_nr.alloc(dst->n_taxa));
+    CU(cudaMemcpyPeer(t_regs, dst->device, src->d_regs, src->device, reg_bytes));
+    CU(cudaMemcpyPeer(t_dense, dst->device, src->d_dense_flag, src->device, dst->n_sketch));
+    CU(cudaMemcpyPeer(t_nk, dst->device, src->d_n_kmers, src->device, dst->n_sketch * 8ull));
+    CU(cudaMemcpyPeer(t_nr, dst->device, src->d_n_reads, src->device, dst->n_taxa * 8ull));
+    launch_merge_state(dst->d_regs, t_regs, dst->d_n_kmers, t_nk, dst->n_sketch, dst->d_n_reads, t_nr, dst->n_taxa, dst->d_dense_flag,
+                       t_dense, dst->aux);
+    dst->launches++;
+    CU(cudaStreamSynchronize(dst->aux));
+  }
   if (exact) return sets ? merge_exact_pairs(dst, src) : KUQ_OK;
   int rc = KUQ_OK;
   if (n_keys && dst->sparse.slots) {
-    uint64_t *d_keys_dst = nullptr;
-    if (cudaMalloc((void **)&d_keys_dst, n_keys * 8) != cudaSuccess) { (void)cudaGetLastError(); cudaSetDevice(src->device); cudaFree(d_keys_src); return fail(ctx, KUQ_E_NOMEM, "no room for %llu keys", (unsigned long long)n_keys); }
+    DevBuf<uint64_t> d_keys_dst;
+    if (d_keys_dst.alloc(n_keys) != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, KUQ_E_NOMEM, "no room for %llu keys", (unsigned long long)n_keys); }
     CU(cudaMemcpyPeer(d_keys_dst, dst->device, d_keys_src, src->device, n_keys * 8));
     rc = kuq_sparse_import(dst, d_keys_dst, n_keys);        // grows dst's set first when the keys need room
-    cudaFree(d_keys_dst);
   }
-  if (d_keys_src) { cudaSetDevice(src->device); cudaFree(d_keys_src); cudaSetDevice(dst->device); }
   return rc;
 }
 
@@ -3375,7 +3288,7 @@ int kuq_wait_flags(kuq_ctx *ctx, uint32_t slot, const uint64_t *d_flags, uint32_
   if (!d_flags || n == 0 || n > 32) return fail(ctx, KUQ_E_INVALID_ARG, "1..32 flags");
   CU(cudaSetDevice(ctx->device));
   if (!ctx->d_sync_err) {
-    CU(dmalloc(&ctx->d_sync_err, 1));
+    CU(ctx->d_sync_err.alloc(1));
     CU(cudaMemset(ctx->d_sync_err, 0, 4));
   }
   launch_wait_flags(reinterpret_cast<const unsigned long long *>(d_flags), n, value, (unsigned long long)(timeout_ms ? timeout_ms : 20000) * 1000000ull,
@@ -3709,13 +3622,6 @@ int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
   }
   // 2. the new parts, at a load of at most 0.6 from 1024 slots up
   std::vector<ExactTable> part(n);
-  auto cleanup = [&]() {
-    for (uint32_t g = 0; g < n; g++) {
-      cudaSetDevice(ctxs[g]->device);
-      free_table(part[g]);
-    }
-    cudaSetDevice(ctx->device);
-  };
   int rc = KUQ_OK;
   for (uint32_t g = 0; g < n && !rc; g++) {
     CU(cudaSetDevice(ctxs[g]->device));
@@ -3730,7 +3636,10 @@ int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
         [src, n](uint64_t lo, uint64_t hi, ExactPair *buf, uint64_t cap, uint64_t *cnt) { return exact_parts(src, lo, hi, n, buf, cap, cnt); },
         [&](uint32_t o, const ExactPair *pairs, uint64_t m) { return import_items(ctxs[o], part[o], pairs, m, true); });
   }
-  if (rc) { cleanup(); return rc; }
+  if (rc) {
+    cudaSetDevice(ctx->device);
+    return rc;
+  }
   // 4. the parts replace the tables: from now on each holds one owner's part
   for (uint32_t g = 0; g < n; g++) {
     CU(cudaSetDevice(ctxs[g]->device));

@@ -173,29 +173,26 @@ int exact_clade_dups(const ExactPair *slots, uint64_t n_slots, uint64_t n_pairs,
   if (n_pass > (1ull << 20)) return 1;
   auto pass_cap = [&](uint64_t want) { return std::min<uint64_t>(n_pairs, want + want / 16 + 4096); };
   uint64_t cap = pass_cap((n_pairs + n_pass - 1) / n_pass);
-  ExactItem *buf[2] = {nullptr, nullptr};
-  unsigned long long *cursor = nullptr;
-  void *temp = nullptr;
+  DevBuf<ExactItem> buf[2];
+  DevBuf<unsigned long long> cursor;
+  DevBuf<uint8_t> temp;
   size_t temp_bytes = 0;
-  auto release = [&]() { cudaFree(buf[0]); cudaFree(buf[1]); cudaFree(temp); buf[0] = buf[1] = nullptr; temp = nullptr; };
   auto reserve = [&](uint64_t c) -> int {                                // 0 ok, 1 no memory, 2 CUDA error
-    release();
+    buf[0].reset(); buf[1].reset(); temp.reset();
     cub::DoubleBuffer<ExactItem> keys(nullptr, nullptr);
     temp_bytes = 0;
     if (cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, keys, (int64_t)c, ExactItemDecomposer{}, 0, 94, stream) != cudaSuccess) {
       (void)cudaGetLastError();
       return 2;
     }
-    if (cudaMalloc((void **)&buf[0], c * sizeof(ExactItem)) != cudaSuccess || cudaMalloc((void **)&buf[1], c * sizeof(ExactItem)) != cudaSuccess ||
-        cudaMalloc(&temp, temp_bytes ? temp_bytes : 1) != cudaSuccess) {
+    if (buf[0].alloc(c) != cudaSuccess || buf[1].alloc(c) != cudaSuccess || temp.alloc(temp_bytes ? temp_bytes : 1) != cudaSuccess) {
       (void)cudaGetLastError();
-      release();
       return 1;
     }
     cap = c;
     return 0;
   };
-  if (cudaMalloc((void **)&cursor, 8) != cudaSuccess) { (void)cudaGetLastError(); return 1; }
+  if (cursor.alloc(1) != cudaSuccess) { (void)cudaGetLastError(); return 1; }
   int rc = reserve(cap);
   const int grid = n_sm * 8;
   for (uint32_t pass = 0; pass < n_pass && !rc; pass++) {
@@ -210,12 +207,10 @@ int exact_clade_dups(const ExactPair *slots, uint64_t n_slots, uint64_t n_pairs,
     }
     if (rc || n < 2) continue;
     cub::DoubleBuffer<ExactItem> keys(buf[0], buf[1]);
-    if (cub::DeviceRadixSort::SortKeys(temp, temp_bytes, keys, (int64_t)n, ExactItemDecomposer{}, 0, 94, stream) != cudaSuccess) rc = 2;
+    if (cub::DeviceRadixSort::SortKeys(temp.get(), temp_bytes, keys, (int64_t)n, ExactItemDecomposer{}, 0, 94, stream) != cudaSuccess) rc = 2;
     if (!rc) k_exact_dups<<<grid, 256, 0, stream>>>(keys.Current(), n, d_parent, d_depth, d_books);
     if (cudaStreamSynchronize(stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) rc = 2;
   }
-  release();
-  cudaFree(cursor);
   *passes_out = (uint32_t)n_pass;
   return rc;
 }
@@ -230,20 +225,18 @@ int sparse_clade_dups(const KeySource &set_keys, const KeySource &kept_keys, con
                       const uint32_t *d_pre_of_taxon, const uint32_t *d_node_of_pre, const uint32_t *d_parent_c,
                       const uint32_t *d_depth_c, const int32_t *d_sid_of_node, uint32_t *d_dup, int n_sm, cudaStream_t stream) {
   if (n_keys_upper < 2 || set_keys.n + kept_keys.n == 0) return 0;
-  unsigned long long *buf[2] = {nullptr, nullptr}, *cursor = nullptr;
-  void *temp = nullptr;
+  DevBuf<unsigned long long> buf[2], cursor;
+  DevBuf<uint8_t> temp;
   size_t temp_bytes = 0;
   int rc = 0;
-  auto cleanup = [&]() { cudaFree(buf[0]); cudaFree(buf[1]); cudaFree(cursor); cudaFree(temp); };
   cub::DoubleBuffer<unsigned long long> keys(nullptr, nullptr);
   if (cub::DeviceRadixSort::SortKeys(nullptr, temp_bytes, keys, (int64_t)n_keys_upper, 0, 64, stream) != cudaSuccess) {
     (void)cudaGetLastError();
     return 2;
   }
-  if (cudaMalloc((void **)&buf[0], n_keys_upper * 8) != cudaSuccess || cudaMalloc((void **)&buf[1], n_keys_upper * 8) != cudaSuccess ||
-      cudaMalloc((void **)&cursor, 8) != cudaSuccess || cudaMalloc(&temp, temp_bytes ? temp_bytes : 1) != cudaSuccess) {
+  if (buf[0].alloc(n_keys_upper) != cudaSuccess || buf[1].alloc(n_keys_upper) != cudaSuccess || cursor.alloc(1) != cudaSuccess ||
+      temp.alloc(temp_bytes ? temp_bytes : 1) != cudaSuccess) {
     (void)cudaGetLastError();
-    cleanup();
     return 1;
   }
   cudaMemsetAsync(cursor, 0, 8, stream);
@@ -251,15 +244,14 @@ int sparse_clade_dups(const KeySource &set_keys, const KeySource &kept_keys, con
     if (src->n) k_clade_sort_keys<<<n_sm * 8, 256, 0, stream>>>(*src, dense_flag, d_pre_of_taxon, buf[0], n_keys_upper, cursor);
   unsigned long long n = 0;
   cudaMemcpyAsync(&n, cursor, 8, cudaMemcpyDeviceToHost, stream);
-  if (cudaStreamSynchronize(stream) != cudaSuccess) { (void)cudaGetLastError(); cleanup(); return 2; }
-  if (n > n_keys_upper) { cleanup(); return 2; }                       // more keys than the per-taxon counters promised
+  if (cudaStreamSynchronize(stream) != cudaSuccess) { (void)cudaGetLastError(); return 2; }
+  if (n > n_keys_upper) return 2;                                      // more keys than the per-taxon counters promised
   if (n >= 2) {
     keys = cub::DoubleBuffer<unsigned long long>(buf[0], buf[1]);
-    if (cub::DeviceRadixSort::SortKeys(temp, temp_bytes, keys, (int64_t)n, 0, 64, stream) != cudaSuccess) rc = 2;
+    if (cub::DeviceRadixSort::SortKeys(temp.get(), temp_bytes, keys, (int64_t)n, 0, 64, stream) != cudaSuccess) rc = 2;
     if (!rc) k_clade_dups<<<n_sm * 8, 256, 0, stream>>>(keys.Current(), n, d_node_of_pre, d_parent_c, d_depth_c, d_sid_of_node, d_dup);
     if (cudaStreamSynchronize(stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) rc = 2;
   }
-  cleanup();
   return rc;
 }
 

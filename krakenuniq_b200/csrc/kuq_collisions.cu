@@ -68,11 +68,11 @@ __global__ void __launch_bounds__(256) k_collide_emit(const unsigned long long *
 
 }  // namespace
 
-// 0 = ok (*list_out / *n_out: device list of (secondary, primary), nullptr when empty), 1 = no table (more than 2^32
+// 0 = ok (list_out / *n_out: device list of (secondary, primary), empty when there is none), 1 = no table (more than 2^32
 // records, no memory for the sort, a taxon too large for one pass, or more than `max_entries` secondaries), 2 = CUDA error
 int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint64_t *records_of_taxon, uint32_t n_sketch,
-                     uint64_t max_entries, uint2 **list_out, uint64_t *n_out, int n_sm, cudaStream_t stream) {
-  *list_out = nullptr;
+                     uint64_t max_entries, DevBuf<uint2> &list_out, uint64_t *n_out, int n_sm, cudaStream_t stream) {
+  list_out.reset();
   *n_out = 0;
   if (n_rec >= (1ull << 32)) return 1;
   const uint32_t hi_mask = (uint32_t)(key_mask >> 32);
@@ -95,52 +95,48 @@ int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, co
   biggest = std::max(biggest, in_pass);
   cuts.push_back(n_sketch);
   if (biggest == 0) return 0;
-  unsigned long long *kbuf[2] = {nullptr, nullptr}, *cnt = nullptr;
-  uint32_t *ibuf[2] = {nullptr, nullptr};
-  uint2 *list = nullptr;
-  void *temp = nullptr;
+  DevBuf<unsigned long long> kbuf[2], cnt;
+  DevBuf<uint32_t> ibuf[2];
+  DevBuf<uint2> list;
+  DevBuf<uint8_t> temp;
   size_t temp_bytes = 0;
-  auto cleanup = [&](int rc) {
-    cudaFree(kbuf[0]); cudaFree(kbuf[1]); cudaFree(ibuf[0]); cudaFree(ibuf[1]); cudaFree(cnt); cudaFree(temp);
-    if (rc) cudaFree(list);
+  auto error = [](int rc) {
     (void)cudaGetLastError();
     return rc;
   };
   {
     cub::DoubleBuffer<unsigned long long> k(nullptr, nullptr);
     cub::DoubleBuffer<uint32_t> v(nullptr, nullptr);
-    if (cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, k, v, (int64_t)biggest, 0, 64, stream) != cudaSuccess) return cleanup(2);
+    if (cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, k, v, (int64_t)biggest, 0, 64, stream) != cudaSuccess) return error(2);
   }
-  if (cudaMalloc((void **)&kbuf[0], biggest * 8) != cudaSuccess || cudaMalloc((void **)&kbuf[1], biggest * 8) != cudaSuccess ||
-      cudaMalloc((void **)&ibuf[0], biggest * 4) != cudaSuccess || cudaMalloc((void **)&ibuf[1], biggest * 4) != cudaSuccess ||
-      cudaMalloc((void **)&cnt, 16) != cudaSuccess || cudaMalloc(&temp, temp_bytes ? temp_bytes : 1) != cudaSuccess ||
-      cudaMalloc((void **)&list, list_bytes) != cudaSuccess)
-    return cleanup(1);
-  if (cudaMemsetAsync(cnt + 1, 0, 8, stream) != cudaSuccess) return cleanup(2);
+  if (kbuf[0].alloc(biggest) != cudaSuccess || kbuf[1].alloc(biggest) != cudaSuccess || ibuf[0].alloc(biggest) != cudaSuccess ||
+      ibuf[1].alloc(biggest) != cudaSuccess || cnt.alloc(2) != cudaSuccess || temp.alloc(temp_bytes ? temp_bytes : 1) != cudaSuccess ||
+      list.alloc(max_entries + 1) != cudaSuccess)
+    return error(1);
+  if (cudaMemsetAsync(cnt + 1, 0, 8, stream) != cudaSuccess) return error(2);
   const int grid = n_sm * 8;
   for (size_t p = 0; p + 1 < cuts.size(); p++) {
     const uint32_t t_lo = cuts[p], t_hi = cuts[p + 1];
     unsigned long long n = 0;
-    if (cudaMemsetAsync(cnt, 0, 8, stream) != cudaSuccess) return cleanup(2);
+    if (cudaMemsetAsync(cnt, 0, 8, stream) != cudaSuccess) return error(2);
     k_collide_gather<<<grid, 256, 0, stream>>>(pairs, n_rec, hi_mask, t_lo, t_hi, kbuf[0], ibuf[0], cnt);
     if (cudaMemcpyAsync(&n, cnt, 8, cudaMemcpyDeviceToHost, stream) != cudaSuccess || cudaStreamSynchronize(stream) != cudaSuccess)
-      return cleanup(2);
-    if (n > biggest) return cleanup(2);                    // more records than the per-taxon counts promised
+      return error(2);
+    if (n > biggest) return error(2);                      // more records than the per-taxon counts promised
     if (n < 2) continue;
     const int end_bit = 32 + (32 - __builtin_clz(std::max<uint32_t>(t_hi - t_lo - 1, 1)));
     cub::DoubleBuffer<unsigned long long> k(kbuf[0], kbuf[1]);
     cub::DoubleBuffer<uint32_t> v(ibuf[0], ibuf[1]);
-    if (cub::DeviceRadixSort::SortPairs(temp, temp_bytes, k, v, (int64_t)n, 0, end_bit, stream) != cudaSuccess) return cleanup(2);
+    if (cub::DeviceRadixSort::SortPairs(temp.get(), temp_bytes, k, v, (int64_t)n, 0, end_bit, stream) != cudaSuccess) return error(2);
     k_collide_emit<<<grid, 256, 0, stream>>>(k.Current(), v.Current(), n, list, max_entries, cnt + 1);
   }
   unsigned long long n_list = 0;
   if (cudaMemcpyAsync(&n_list, cnt + 1, 8, cudaMemcpyDeviceToHost, stream) != cudaSuccess ||
       cudaStreamSynchronize(stream) != cudaSuccess || cudaGetLastError() != cudaSuccess)
-    return cleanup(2);
-  if (n_list > max_entries) return cleanup(1);
-  cleanup(0);
-  if (n_list == 0) { cudaFree(list); list = nullptr; }
-  *list_out = list;
+    return error(2);
+  if (n_list > max_entries) return error(1);
+  if (n_list == 0) list.reset();
+  list_out = std::move(list);
   *n_out = n_list;
   return 0;
 }

@@ -104,17 +104,9 @@ int seterr(int code, char *err, size_t cap, const char *fmt, ...) {
   return code;
 }
 
-struct Buffers {                    // frees on scope exit whatever was allocated
-  void *p[16];
-  int n = 0;
-  template <typename T>
-  cudaError_t get(T **out, uint64_t count) {
-    cudaError_t e = cudaMalloc((void **)out, count * sizeof(T) + 16);
-    if (e == cudaSuccess) p[n++] = *out;
-    return e;
-  }
-  ~Buffers() { for (int i = 0; i < n; i++) cudaFree(p[i]); }
-};
+// count items and 16 bytes more
+template <typename T>
+cudaError_t get(DevBuf<T> &b, uint64_t count) { return b.alloc(count + 16 / sizeof(T)); }
 
 #define DB_CU(call)                                                                                      \
   do {                                                                                                   \
@@ -141,9 +133,9 @@ const uint64_t PASS_C_REC = CORE_REC + 20;
 const uint64_t RESERVE = 1ull << 18; // budget kept back from the pass-C plan for CUB's fixed-size state
 
 struct Core {
-  uint8_t *in = nullptr, *out = nullptr, *tmp = nullptr;
-  ull *keys = nullptr, *keys2 = nullptr, *idx = nullptr, *idx2 = nullptr;
-  uint32_t *bins = nullptr, *bins2 = nullptr, *bins3 = nullptr;
+  DevBuf<uint8_t> in, out, tmp;
+  DevBuf<ull> keys, keys2, idx, idx2;
+  DevBuf<uint32_t> bins, bins2, bins3;
   size_t tmp_bytes = 0;
 };
 
@@ -163,11 +155,11 @@ cudaError_t core_tmp(uint64_t n, int key_bits, int bin_bits, size_t *bytes) {
 
 uint64_t core_bytes(uint64_t n, uint64_t pair_sz, size_t tmp) { return n * (2 * pair_sz + CORE_REC) + tmp + 10 * 16; }
 
-cudaError_t core_alloc(Buffers &buf, Core &c, uint64_t n, uint64_t pair_sz, size_t tmp) {
+cudaError_t core_alloc(Core &c, uint64_t n, uint64_t pair_sz, size_t tmp) {
   cudaError_t rc;
-  if ((rc = buf.get(&c.in, n * pair_sz)) || (rc = buf.get(&c.out, n * pair_sz)) || (rc = buf.get(&c.keys, n)) ||
-      (rc = buf.get(&c.keys2, n)) || (rc = buf.get(&c.idx, n)) || (rc = buf.get(&c.idx2, n)) || (rc = buf.get(&c.bins, n)) ||
-      (rc = buf.get(&c.bins2, n)) || (rc = buf.get(&c.bins3, n)) || (rc = buf.get(&c.tmp, tmp)))
+  if ((rc = get(c.in, n * pair_sz)) || (rc = get(c.out, n * pair_sz)) || (rc = get(c.keys, n)) || (rc = get(c.keys2, n)) ||
+      (rc = get(c.idx, n)) || (rc = get(c.idx2, n)) || (rc = get(c.bins, n)) || (rc = get(c.bins2, n)) || (rc = get(c.bins3, n)) ||
+      (rc = get(c.tmp, tmp)))
     return rc;
   c.tmp_bytes = tmp;
   return cudaSuccess;
@@ -182,12 +174,13 @@ cudaError_t core_sort(Core &c, uint64_t n, const Geometry &g, uint32_t bin_lo, i
   k_dbs_keys<<<grid, 256, 0, st>>>(c.in, n, g.key_len, g.k, g.nt, bin_lo, c.keys, c.bins, c.idx, hist);
   // by key (pair_cmp, db_sort.cpp:118-128) ...
   size_t need = c.tmp_bytes;
-  cudaError_t rc = cub::DeviceRadixSort::SortPairs(c.tmp, need, c.keys, c.keys2, c.idx, c.idx2, (int64_t)n, 0, (int)g.key_bits, st);
+  cudaError_t rc = cub::DeviceRadixSort::SortPairs(c.tmp.get(), need, c.keys.get(), c.keys2.get(), c.idx.get(), c.idx2.get(), (int64_t)n, 0,
+                                                   (int)g.key_bits, st);
   if (rc != cudaSuccess) return rc;
   // ... then, stably, by bin (:96-107): the order inside a bin stays the key order
   k_dbs_gather_bins<<<grid, 256, 0, st>>>(c.bins, c.idx2, n, c.bins2);
   need = c.tmp_bytes;
-  rc = cub::DeviceRadixSort::SortPairs(c.tmp, need, c.bins2, c.bins3, c.idx2, c.idx, (int64_t)n, 0, bin_bits, st);
+  rc = cub::DeviceRadixSort::SortPairs(c.tmp.get(), need, c.bins2.get(), c.bins3.get(), c.idx2.get(), c.idx.get(), (int64_t)n, 0, bin_bits, st);
   if (rc != cudaSuccess) return rc;
   k_dbs_emit<<<grid, 256, 0, st>>>(c.in, c.idx, n, g.key_len, zero_vals, c.out);
   return cudaGetLastError();
@@ -252,17 +245,16 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
 
   // ---- in one piece: the whole input and the index on the device ----
   if (core_bytes(n, pair_sz, std::max(tmp, scan_tmp)) + idx_dev <= budget) {
-    Buffers buf;
     Core c;
-    ull *d_off = nullptr;
-    DB_CU(core_alloc(buf, c, n, pair_sz, std::max(tmp, scan_tmp)));
-    DB_CU(buf.get(&d_off, entries + 1));
+    DevBuf<ull> d_off;
+    DB_CU(core_alloc(c, n, pair_sz, std::max(tmp, scan_tmp)));
+    DB_CU(get(d_off, entries + 1));
     DB_CU(bounce.to_device(c.in, body, n * pair_sz, st));
     DB_CU(cudaMemsetAsync(d_off, 0, (entries + 1) * 8, st));
     DB_CU(core_sort(c, n, g, 0, 2 * nt, zero_vals, d_off, st));
     // offsets = running sum of the bin sizes (make_index :136-139)
     size_t need = c.tmp_bytes;
-    DB_CU(cub::DeviceScan::InclusiveSum(c.tmp, need, d_off, d_off, (int64_t)(entries + 1), st));
+    DB_CU(cub::DeviceScan::InclusiveSum(c.tmp.get(), need, d_off.get(), d_off.get(), (int64_t)(entries + 1), st));
     DB_CU(bounce.to_host(obody, c.out, n * pair_sz, st));
     DB_CU(bounce.to_host(idx_out + 8, d_off, (entries + 1) * 8, st));
     return KUQ_OK;
@@ -275,12 +267,11 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
     if (idx_dev + scan_tmp + chunk * pair_sz + 32 > budget)
       return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: the bin histogram of -n %u (%llu bytes) does not fit KUQ_DB_SORT_BUDGET = %llu bytes",
                     nt, (unsigned long long)idx_dev, (unsigned long long)budget);
-    Buffers buf;
-    uint8_t *d_chunk = nullptr, *d_tmp = nullptr;
-    ull *d_off = nullptr;
-    DB_CU(buf.get(&d_chunk, chunk * pair_sz));
-    DB_CU(buf.get(&d_off, entries + 1));
-    DB_CU(buf.get(&d_tmp, scan_tmp));
+    DevBuf<uint8_t> d_chunk, d_tmp;
+    DevBuf<ull> d_off;
+    DB_CU(get(d_chunk, chunk * pair_sz));
+    DB_CU(get(d_off, entries + 1));
+    DB_CU(get(d_tmp, scan_tmp));
     DB_CU(cudaMemsetAsync(d_off, 0, (entries + 1) * 8, st));
     for (uint64_t s = 0; s < n; s += chunk) {
       const uint64_t m = std::min(chunk, n - s);
@@ -289,7 +280,7 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
       DB_CU(cudaGetLastError());
     }
     size_t need = scan_tmp;
-    DB_CU(cub::DeviceScan::InclusiveSum(d_tmp, need, d_off, d_off, (int64_t)(entries + 1), st));
+    DB_CU(cub::DeviceScan::InclusiveSum(d_tmp.get(), need, d_off.get(), d_off.get(), (int64_t)(entries + 1), st));
     DB_CU(bounce.to_host(idx_out + 8, d_off, (entries + 1) * 8, st));
   }
   const uint64_t *offsets = reinterpret_cast<const uint64_t *>(idx_out + 8);
@@ -337,19 +328,18 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
     if (!fits(chunk, stmp))
       return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: %u ranges do not fit KUQ_DB_SORT_BUDGET = %llu bytes", R,
                     (unsigned long long)budget);
-    Buffers buf;
-    uint8_t *d_chunk = nullptr, *d_grp = nullptr, *d_tmp = nullptr;
-    uint32_t *d_rid = nullptr, *d_rid2 = nullptr, *d_starts = nullptr;
-    ull *d_idx = nullptr, *d_idx2 = nullptr, *d_cnt = nullptr;
-    DB_CU(buf.get(&d_chunk, chunk * pair_sz));
-    DB_CU(buf.get(&d_grp, chunk * pair_sz));
-    DB_CU(buf.get(&d_rid, chunk));
-    DB_CU(buf.get(&d_rid2, chunk));
-    DB_CU(buf.get(&d_idx, chunk));
-    DB_CU(buf.get(&d_idx2, chunk));
-    DB_CU(buf.get(&d_starts, R));
-    DB_CU(buf.get(&d_cnt, R));
-    DB_CU(buf.get(&d_tmp, stmp));
+    DevBuf<uint8_t> d_chunk, d_grp, d_tmp;
+    DevBuf<uint32_t> d_rid, d_rid2, d_starts;
+    DevBuf<ull> d_idx, d_idx2, d_cnt;
+    DB_CU(get(d_chunk, chunk * pair_sz));
+    DB_CU(get(d_grp, chunk * pair_sz));
+    DB_CU(get(d_rid, chunk));
+    DB_CU(get(d_rid2, chunk));
+    DB_CU(get(d_idx, chunk));
+    DB_CU(get(d_idx2, chunk));
+    DB_CU(get(d_starts, R));
+    DB_CU(get(d_cnt, R));
+    DB_CU(get(d_tmp, stmp));
     std::vector<uint32_t> starts(R);
     std::vector<uint64_t> cursor(R), cnt(R), pos(R);
     for (uint32_t r = 0; r < R; r++) { starts[r] = (uint32_t)ranges[r].first; cursor[r] = offsets[ranges[r].first]; }
@@ -360,7 +350,7 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
       DB_CU(cudaMemsetAsync(d_cnt, 0, R * 8ull, st));
       k_dbs_range_of<<<grid, 256, 0, st>>>(d_chunk, m, g.key_len, g.k, nt, d_starts, R, d_rid, d_idx, d_cnt);
       size_t need = stmp;
-      DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp, need, d_rid, d_rid2, d_idx, d_idx2, (int64_t)m, 0, rbits, st));
+      DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp.get(), need, d_rid.get(), d_rid2.get(), d_idx.get(), d_idx2.get(), (int64_t)m, 0, rbits, st));
       k_dbs_emit<<<grid, 256, 0, st>>>(d_chunk, d_idx2, m, g.key_len, 0, d_grp);
       DB_CU(cudaGetLastError());
       if (s + m < n)                                                 // the host copy of the next chunk overlaps these kernels
@@ -384,9 +374,8 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
 
   // ---- pass C: sort each range in place ----
   {
-    Buffers buf;
     Core c;
-    DB_CU(core_alloc(buf, c, max_rec, pair_sz, ctmp));
+    DB_CU(core_alloc(c, max_rec, pair_sz, ctmp));
     for (auto &r : ranges) {
       const uint64_t a = offsets[r.first], m = offsets[r.second] - a;
       DB_CU(bounce.to_device(c.in, obody + a * pair_sz, m * pair_sz, st));

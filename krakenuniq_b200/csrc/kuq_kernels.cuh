@@ -27,6 +27,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "kuq_buffers.cuh"
+
 struct kuq_layout_result;
 
 namespace kuq {
@@ -342,7 +344,7 @@ void launch_settle_kept(uint8_t *pairs, const uint2 *secondaries, uint64_t n_sec
                         unsigned long long *n_dup, cudaStream_t stream);
 // kuq_collisions.cu: (secondary, primary) record pairs of every (taxon, code) group of the staged records
 int build_collisions(const uint8_t *pairs, uint64_t n_rec, uint64_t key_mask, const uint64_t *records_of_taxon, uint32_t n_sketch,
-                     uint64_t max_entries, uint2 **list_out, uint64_t *n_out, int n_sm, cudaStream_t stream);
+                     uint64_t max_entries, DevBuf<uint2> &list_out, uint64_t *n_out, int n_sm, cudaStream_t stream);
 // the items of old_slots[0, old_cap) into a grown table without counting them again
 void launch_rehash(const unsigned long long *old_slots, uint64_t old_cap, const SparseSet &s, uint32_t *error_flag, cudaStream_t stream);
 void launch_rehash(const ExactPair *old_slots, uint64_t old_cap, const ExactSet &e, uint32_t *error_flag, cudaStream_t stream);
