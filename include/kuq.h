@@ -511,7 +511,19 @@ int kuq_scan_device(kuq_ctx *ctx, uint32_t slot, uint32_t k, uint32_t nt, uint32
  * rewritten to dense ids on arrival; kuq_stream_check reports a taxid outside the declared universe.  The buffers hold
  * max_records records of 12 bytes; records shorter than that (k <= 28) are widened on arrival, in pieces that pass
  * through one landing zone of 64 MiB (KUQ_LANDING_BYTES) on the copy stream.  kuq_stream_open may be called again once
- * the slots are idle (it waits for them): the next database of a streamed run may have another nt or index type. */
+ * the slots are idle (it waits for them): the next database of a streamed run may have another nt or index type.
+ * Several GPUs of a node (one context each, the same universe and taxonomy, kuq_enable_peer_access between all of them):
+ * GPU g streams a contiguous group of the ranges, every GPU holds every batch, and each batch has one owner whose
+ * zero-initialised id buffer takes every GPU's hits (a peer pointer for the others):
+ *     the owners zero their buffers; host barrier
+ *     for each database d, in command-line order:
+ *         every GPU g at once: the loop above over g's group of d's ranges, kuq_lookup_device(... owner's buffer,
+ *                              only_hits = d == 0 ? 1 : KUQ_LOOKUP_FILL_EMPTY);  kuq_sync_slot(0), (1);  kuq_stream_check
+ *         host barrier — KUQ_LOOKUP_FILL_EMPTY reads the owner's word with a plain load, which sees another GPU's stores
+ *         only once that GPU has finished and a new launch has begun
+ *     every owner: kuq_resolve_device(...) for its batches; at the end kuq_finish on every context and kuq_merge_into
+ * kuq_host_register pins with cudaHostRegisterPortable, so one registered mapping counts as pinned for every device and
+ * every GPU's copies from it overlap its lookups. */
 int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, uint64_t max_records, uint64_t max_bins);
 int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64_t n_records, const uint64_t *host_offsets,
                     uint64_t bin_lo, uint64_t bin_hi);

@@ -1787,6 +1787,9 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 // several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b` without -x.
 // stage_streamed runs once per process: the ranges, the taxids of every record and the pinned registration of the mapped
 // files.  classify_streamed runs once per sample: its rounds of reads, each through every range.
+//   Several GPUs (classify_streamed_gpus): every database keeps the same ranges, and GPU g streams a contiguous group of
+//   them (kuq_ranges.h, group_ranges) over its own host link.  Every GPU holds every batch of a round; each batch has one
+//   owner that holds its id buffer, and every GPU stores its hits straight into the owner's buffer (peer stores).
 struct Streamed {
   struct Plan {
     const uint8_t *rec0;
@@ -1794,18 +1797,25 @@ struct Streamed {
     uint64_t pair_sz;
     uint32_t k, nt, idx_type;
     vector<pair<uint64_t, uint64_t>> ranges;
+    vector<size_t> group;                                          // GPU g streams ranges [group[g], group[g + 1])
   };
   vector<Plan> plans;
+  vector<kuq_ctx *> ctxs;
   bool unit_rule = false;
   uint64_t max_rec = 1, max_bins = 1, round_bytes = 0, batch_nt = 1;
   vector<const void *> pinned;                                     // registered mappings, unregistered at the end
-  uint32_t open_nt = 0, open_type = 0;                             // parameters the range buffers are open for
+  vector<uint32_t> open_nt, open_type;                             // per context: what its range buffers are open for
 };
 
-static void stage_streamed(Streamed &sm, kuq_ctx *ctx, const vector<Mapped> &kdbs, const vector<Mapped> &idxs, uint64_t range_budget,
-                           uint64_t hbm_budget, vector<map<uint32_t, uint64_t>> &db_counts) {
+static void stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vector<int> &ctx_devices, const vector<Mapped> &kdbs,
+                           const vector<Mapped> &idxs, uint64_t range_budget, uint64_t hbm_budget,
+                           vector<map<uint32_t, uint64_t>> &db_counts) {
   const size_t n_db = kdbs.size();
+  const int G = (int)ctxs.size();
   const bool unit_rule = sm.unit_rule = n_db > 1;
+  sm.ctxs = ctxs;
+  sm.open_nt.assign(G, 0);
+  sm.open_type.assign(G, 0);
   vector<Streamed::Plan> &plans = sm.plans;
   plans.resize(n_db);
   uint64_t &max_rec = sm.max_rec, &max_bins = sm.max_bins;
@@ -1821,33 +1831,69 @@ static void stage_streamed(Streamed &sm, kuq_ctx *ctx, const vector<Mapped> &kdb
     pl.rec0 = (const uint8_t *)kdbs[d].p + 72 + 2 * (4 + 8 * key_bits);
     pl.offsets = (const uint64_t *)(q + 8);
     pl.ranges = plan_ranges(pl.offsets, 1ull << (2 * pl.nt), range_budget);
-    // pass 0: the taxids of all records, so that every range numbers taxa identically (also database.kdb.counts)
+    pl.group = group_ranges(pl.offsets, pl.ranges, G, 12);
     for (auto &rg : pl.ranges) {
       max_rec = std::max<uint64_t>(max_rec, pl.offsets[rg.second] - pl.offsets[rg.first]);
       max_bins = std::max<uint64_t>(max_bins, rg.second - rg.first);
-      if (kuq_stage_db(ctx, kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, rg.first, rg.second) || db_taxids(ctx, db_counts[d]))
-        die(EX_DATAERR, kuq_last_error(ctx));
     }
   }
+  // pass 0: the taxids of all records, so that every range numbers taxa identically (also database.kdb.counts); every
+  // GPU reads those of its own group
+  {
+    vector<vector<map<uint32_t, uint64_t>>> found(G, vector<map<uint32_t, uint64_t>>(n_db));
+    vector<int> rcs(G, 0);
+#pragma omp parallel for num_threads(G) schedule(static, 1)
+    for (int g = 0; g < G; g++)
+      for (size_t d = 0; d < n_db; d++)
+        for (size_t c = plans[d].group[g]; c < plans[d].group[g + 1] && !rcs[g]; c++) {
+          const auto &rg = plans[d].ranges[c];
+          rcs[g] = kuq_stage_db(ctxs[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, rg.first, rg.second);
+          if (!rcs[g]) rcs[g] = db_taxids(ctxs[g], found[g][d]);
+        }
+    for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
+    for (int g = 0; g < G; g++)
+      for (size_t d = 0; d < n_db; d++)
+        for (auto &kv : found[g][d]) db_counts[d][kv.first] += kv.second;
+  }
   if (n_db == 1) cerr << "Database split into " << plans[0].ranges.size() << " chunks" << endl;
+  if (G > 1) {
+    string per;
+    for (size_t d = 0; d < n_db; d++) {
+      per += d ? ", " : "";
+      for (int g = 0; g < G; g++) per += (g ? "/" : "") + std::to_string(plans[d].group[g + 1] - plans[d].group[g]);
+    }
+    fprintf(stderr, "classify: %s streamed over %d GPUs: ranges per GPU %s\n",
+            n_db == 1 ? "database" : (std::to_string(n_db) + " databases").c_str(), G, per.c_str());
+  }
   {
     set<uint32_t> all;
     for (auto &c : db_counts) for (auto &kv : c) all.insert(kv.first);
     vector<uint32_t> u(all.begin(), all.end());
-    if (kuq_set_db_taxid_universe(ctx, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
+    for (kuq_ctx *c : ctxs)
+      if (kuq_set_db_taxid_universe(c, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(c));
   }
+  for (int g = 0; g < G; g++)
+    for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
   if (unit_rule) {
-    if (kuq_mark_zero_hits(ctx, 1)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    for (kuq_ctx *c : ctxs)
+      if (kuq_mark_zero_hits(c, 1)) die(EX_SOFTWARE, kuq_last_error(c));
+    int g0 = 0;                                                    // a context that staged a range (a group may be empty)
+    while (g0 + 1 < G && std::all_of(plans.begin(), plans.end(), [&](const Streamed::Plan &pl) { return pl.group[g0] == pl.group[g0 + 1]; }))
+      g0++;
     uint32_t rows = 0;
-    if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
+    if (kuq_unit_table_rows(ctxs[g0], &rows)) die(EX_SOFTWARE, kuq_last_error(ctxs[g0]));
     if (rows) Max_units_per_batch = rows;
   }
-  // device memory of a round: the budget (and what the card has free) minus the two range buffers
+  // device memory of a round: the budget (and what the card has free, shared among its contexts) minus the two range
+  // buffers, on the tightest context (stream_round_bytes)
   const uint64_t range_bytes = 2 * (max_rec * 12 + (max_bins + 1) * 8 + 4096);     // 12 B per record in HBM
-  const uint64_t free_b = kuq_device_free_bytes(ctx);
-  const uint64_t cap = std::min<uint64_t>(hbm_budget, free_b > (2ull << 30) ? free_b - (2ull << 30) : 0);
-  const uint64_t round_bytes = sm.round_bytes = cap > range_bytes ? cap - range_bytes : 0;
-  sm.batch_nt = std::max<uint64_t>(1, std::min<uint64_t>(96ull << 20, round_bytes / 6));
+  vector<uint64_t> free_b;
+  for (kuq_ctx *c : ctxs) free_b.push_back(kuq_device_free_bytes(c));
+  const uint64_t round_bytes = sm.round_bytes = stream_round_bytes(ctx_devices, free_b, hbm_budget, range_bytes);
+  // A batch of b bases takes b bytes on every GPU and 4 b more on its owner (batch_shared_bytes / batch_id_bytes), so G
+  // batches, one per owner, take about (G + 4) b per GPU: batches of round / (G + 5) bases let a round give every GPU a
+  // batch to resolve.  One GPU: round / 6.
+  sm.batch_nt = std::max<uint64_t>(1, std::min<uint64_t>(96ull << 20, round_bytes / (G + 5)));
   uint64_t db_bytes = 0;                                           // what every round copies to the device
   for (size_t d = 0; d < n_db; d++) db_bytes += kdbs[d].size + idxs[d].size;
   if (round_bytes < db_bytes)
@@ -1870,7 +1916,11 @@ static void stage_streamed(Streamed &sm, kuq_ctx *ctx, const vector<Mapped> &kdb
   if (Timing) fprintf(stderr, "[timing] streamed: %zu database(s), %llu MiB per round\n", n_db, (unsigned long long)(round_bytes >> 20));
 }
 
-static void classify_streamed(Streamed &sm, kuq_ctx *ctx, const vector<pair<const char *, const char *>> &files) {
+static void classify_streamed_gpus(Streamed &sm, const vector<pair<const char *, const char *>> &files);
+
+static void classify_streamed(Streamed &sm, const vector<pair<const char *, const char *>> &files) {
+  if (sm.ctxs.size() > 1) return classify_streamed_gpus(sm, files);
+  kuq_ctx *ctx = sm.ctxs[0];
   const size_t n_db = sm.plans.size();
   const bool unit_rule = sm.unit_rule;
   const uint64_t round_bytes = sm.round_bytes;
@@ -1916,12 +1966,12 @@ static void classify_streamed(Streamed &sm, kuq_ctx *ctx, const vector<pair<cons
     for (size_t db = 0; db < n_db; db++) {
       const Streamed::Plan &pl = sm.plans[db];
       if (pl.ranges.empty()) continue;                             // a database without records answers nothing
-      if (pl.nt != sm.open_nt || pl.idx_type != sm.open_type) {
+      if (pl.nt != sm.open_nt[0] || pl.idx_type != sm.open_type[0]) {
         // taxonomy and universe are known before the stream opens (the dense numbering is fixed there)
-        if ((sm.open_nt && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, sm.max_rec, sm.max_bins))
+        if ((sm.open_nt[0] && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, sm.max_rec, sm.max_bins))
           die(EX_DATAERR, kuq_last_error(ctx));
-        sm.open_nt = pl.nt;
-        sm.open_type = pl.idx_type;
+        sm.open_nt[0] = pl.nt;
+        sm.open_type[0] = pl.idx_type;
       }
       auto load = [&](uint32_t buf, size_t c) {
         const uint64_t lo = pl.ranges[c].first, hi = pl.ranges[c].second;
@@ -1962,6 +2012,176 @@ static void classify_streamed(Streamed &sm, kuq_ctx *ctx, const vector<pair<cons
     }
   }
   if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
+  if (n_db > 1) {
+    string per;
+    for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(sm.plans[d].ranges.size());
+    fprintf(stderr, "\nclassify: %zu databases streamed: %zu rounds, ranges per database %s\n", n_db, n_rounds, per.c_str());
+  }
+}
+
+// The rounds of classify_streamed on G GPUs, each streaming its group of every database's ranges over its own link:
+//   1. every GPU receives every batch of the round; each batch has one owner (contiguous blocks balanced by bases,
+//      round_peak_bytes), which alone holds the batch's id buffer and zeroes it;
+//   2. host barrier;
+//   3. database by database, in command-line order, one host thread per GPU streams the GPU's group of the database's
+//      ranges through its two range buffers and looks every batch up into the owner's id buffer (a peer pointer when the
+//      owner is another GPU): the first database stores hits only, the later ones fill the windows still empty;
+//   4. host barrier after each database: both slots of every GPU synced, the stream checked;
+//   5. the owners resolve their batches, one in flight per owner, and the results are written in input order.
+// The barrier of step 4 is what makes KUQ_LOOKUP_FILL_EMPTY correct here: lookup_window_multi reads the owner's word with
+// a plain load, which sees the words other GPUs stored over the peer link only because a host barrier and a kernel
+// boundary separate the two databases' lookups.  The sharded layout orders its phases with device flags and no host
+// barrier, and reads the word with a system-scope load (load_relaxed_sys).  Do not drop this barrier without switching
+// to that load.
+static void classify_streamed_gpus(Streamed &sm, const vector<pair<const char *, const char *>> &files) {
+  const vector<kuq_ctx *> &ctxs = sm.ctxs;
+  const int G = (int)ctxs.size();
+  const size_t n_db = sm.plans.size();
+  const bool unit_rule = sm.unit_rule;
+  BatchReader input(files, batch_limits(sm.batch_nt, unit_rule, false));
+  struct DevBatch { void *bases, *offs, *units; };
+  vector<Batch> round;
+  Batch pending;
+  bool have_pending = false;
+  size_t n_rounds = 0;
+  for (;;) {
+    round.clear();
+    vector<uint64_t> bases, reads;
+    for (;;) {
+      if (!have_pending) have_pending = input.next(pending);
+      if (!have_pending) break;
+      bases.push_back(pending.bases.size());
+      reads.push_back(pending.reads.size());
+      if (!round.empty() && round_peak_bytes(bases, reads, unit_rule, G) > sm.round_bytes) {
+        bases.pop_back();
+        reads.pop_back();
+        break;
+      }
+      round.push_back(std::move(pending));
+      have_pending = false;
+    }
+    if (round.empty()) break;
+    n_rounds++;
+    const size_t nb = round.size();
+    vector<size_t> first;                                          // GPU g owns batches [first[g], first[g + 1])
+    round_peak_bytes(bases, reads, unit_rule, G, &first);
+    vector<int> owner(nb);
+    for (int g = 0; g < G; g++) for (size_t bi = first[g]; bi < first[g + 1]; bi++) owner[bi] = g;
+    // 1. (a pageable copy has left the source once it returns)
+    vector<vector<DevBatch>> dev(G, vector<DevBatch>(nb));
+    vector<uint32_t *> ids(nb);
+    for (size_t bi = 0; bi < nb; bi++) {
+      const Batch &b = round[bi];
+      vector<uint64_t> offs(b.offs);
+      offs.push_back(offs.back()); offs.push_back(offs.back());
+      for (int g = 0; g < G; g++) {
+        kuq_ctx *c = ctxs[g];
+        DevBatch &d = dev[g][bi];
+        d.bases = kuq_device_alloc(c, b.bases.size() + 64);
+        d.offs = kuq_device_alloc(c, (b.reads.size() + 4) * 8);
+        d.units = unit_rule ? kuq_device_alloc(c, (b.reads.size() + 4) * 4) : NULL;
+        if (!d.bases || !d.offs || (unit_rule && !d.units)) die(EX_OSERR, "device allocation for the read batches failed");
+        if (kuq_device_memset(c, 0, (char *)d.bases + b.bases.size(), 'N', 64) ||
+            kuq_copy_to_device(c, 0, d.bases, b.bases.data(), b.bases.size()) ||
+            kuq_copy_to_device(c, 0, d.offs, offs.data(), offs.size() * 8) ||
+            (unit_rule && kuq_copy_to_device(c, 0, d.units, b.units.data(), b.units.size() * 4)))
+          die(EX_SOFTWARE, kuq_last_error(c));
+      }
+      kuq_ctx *o = ctxs[owner[bi]];
+      ids[bi] = (uint32_t *)kuq_device_alloc(o, batch_id_bytes(b.bases.size()));
+      if (!ids[bi]) die(EX_OSERR, "device allocation for the read batches failed");
+      if (kuq_device_memset(o, 0, ids[bi], 0, batch_id_bytes(b.bases.size()))) die(EX_SOFTWARE, kuq_last_error(o));
+    }
+    // 2.
+    for (kuq_ctx *c : ctxs) if (kuq_sync_slot(c, 0)) die(EX_SOFTWARE, kuq_last_error(c));
+    uint64_t seqs = 0;
+    for (const Batch &b : round) seqs += b.reads.size();
+    vector<double> stream_s(G, 0.0);
+    for (size_t db = 0; db < n_db; db++) {
+      const Streamed::Plan &pl = sm.plans[db];
+      if (pl.ranges.empty()) continue;                             // a database without records answers nothing
+      const uint32_t only_hits = db == 0 ? 1 : KUQ_LOOKUP_FILL_EMPTY;
+      // 3. and 4.: every GPU's part returns with its slots and copies synced; the join is the host barrier
+      vector<int> ex(G, 0);
+#pragma omp parallel for num_threads(G) schedule(static, 1)
+      for (int g = 0; g < G; g++) {
+        const double t0 = now_s();
+        kuq_ctx *c = ctxs[g];
+        const size_t lo = pl.group[g], hi = pl.group[g + 1];
+        auto part = [&]() -> int {
+          // every context opens the stream, an empty group too: the open numbers the taxa, which its resolves need
+          if (pl.nt != sm.open_nt[g] || pl.idx_type != sm.open_type[g]) {
+            if ((sm.open_nt[g] && kuq_stream_check(c)) || kuq_stream_open(c, pl.k, pl.nt, pl.idx_type, sm.max_rec, sm.max_bins))
+              return EX_DATAERR;
+            sm.open_nt[g] = pl.nt;
+            sm.open_type[g] = pl.idx_type;
+          }
+          if (lo == hi) return 0;
+          auto load = [&](uint32_t buf, size_t r) {
+            const uint64_t blo = pl.ranges[r].first, bhi = pl.ranges[r].second;
+            return kuq_stream_load(c, buf, pl.rec0 + pl.offsets[blo] * pl.pair_sz, pl.offsets[bhi] - pl.offsets[blo], pl.offsets + blo,
+                                   blo, bhi);
+          };
+          if (load(0, lo)) return EX_DATAERR;
+          for (size_t r = lo; r < hi; r++) {
+            if (kuq_stream_use(c, (uint32_t)((r - lo) & 1))) return EX_SOFTWARE;
+            if (r + 1 < hi && load((uint32_t)((r + 1 - lo) & 1), r + 1)) return EX_DATAERR;
+            for (size_t bi = 0; bi < nb; bi++) {
+              const Batch &b = round[bi];
+              if (kuq_lookup_device(c, (uint32_t)(bi & 1), (const char *)dev[g][bi].bases, (const uint64_t *)dev[g][bi].offs,
+                                    (uint32_t)b.reads.size(), b.bases.size(), ids[bi], only_hits))
+                return EX_SOFTWARE;
+            }
+          }
+          return kuq_sync_slot(c, 0) || kuq_sync_slot(c, 1) || kuq_stream_check(c) ? EX_SOFTWARE : 0;
+        };
+        ex[g] = part();
+        stream_s[g] += now_s() - t0;
+      }
+      for (int g = 0; g < G; g++) if (ex[g]) die(ex[g], kuq_last_error(ctxs[g]));
+      for (size_t c = 0; c < pl.ranges.size(); c++) {
+        if (n_db == 1) fprintf(stderr, "\r Processed %llu sequences (database chunk %zu of %zu)\n", (unsigned long long)seqs, c + 1, pl.ranges.size());
+        else fprintf(stderr, "\r Processed %llu sequences (database %zu of %zu, chunk %zu of %zu)", (unsigned long long)seqs, db + 1, n_db,
+                     c + 1, pl.ranges.size());
+      }
+    }
+    // 5. the owner's next batch is queued before this one is written: the results stay in the slot's host buffers until
+    // the slot's next collect
+    const double t1 = now_s();
+    vector<size_t> next(first.begin(), first.end() - 1);
+    auto resolve_next = [&](int g) {
+      if (next[g] == first[g + 1]) return;
+      const size_t bi = next[g]++;
+      const Batch &b = round[bi];
+      if (kuq_resolve_device(ctxs[g], 0, (const char *)dev[g][bi].bases, (const uint64_t *)dev[g][bi].offs, (uint32_t)b.reads.size(),
+                             b.bases.size(), ids[bi], (const uint32_t *)dev[g][bi].units, 0))
+        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    };
+    for (int g = 0; g < G; g++) resolve_next(g);
+    for (size_t bi = 0; bi < nb; bi++) {
+      const int g = owner[bi];
+      Batch &b = round[bi];
+      kuq_batch_result res;
+      if (kuq_collect_device_batch(ctxs[g], 0, &res)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      resolve_next(g);
+      write_reads(b, res, 0, b.reads.size());
+      book_batch(b.reads.size(), b.bases.size(), res.n_classified);
+    }
+    if (Timing) {
+      string per;
+      for (int g = 0; g < G; g++) {
+        char s[64];
+        snprintf(s, sizeof s, "%s%.3f s (%zu batches)", g ? ", " : "", stream_s[g], first[g + 1] - first[g]);
+        per += s;
+      }
+      fprintf(stderr, "\n[timing] streamed round %zu: stream per GPU %s; resolve %.3f s\n", n_rounds, per.c_str(), now_s() - t1);
+    }
+    for (int g = 0; g < G; g++)
+      for (size_t bi = 0; bi < nb; bi++)
+        for (void *p : {dev[g][bi].bases, dev[g][bi].offs, dev[g][bi].units}) if (p) kuq_device_free(ctxs[g], p);
+    for (size_t bi = 0; bi < nb; bi++) kuq_device_free(ctxs[owner[bi]], ids[bi]);
+  }
+  for (kuq_ctx *c : ctxs) if (kuq_finish(c)) die(EX_SOFTWARE, kuq_last_error(c));
   if (n_db > 1) {
     string per;
     for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(sm.plans[d].ranges.size());
@@ -2266,7 +2486,7 @@ int main(int argc, char **argv) {
   if (getenv("KUQ_HBM_BUDGET")) hbm_budget = strtoull(getenv("KUQ_HBM_BUDGET"), NULL, 10);
   uint64_t chunk_budget = 0;
   // The databases (one, or several together) larger than one card: sharded over the visible GPUs when they hold them
-  // together (run_sharded / run_sharded_multi), else streamed through one GPU in ranges of at most 40 GB (two range
+  // together (run_sharded / run_sharded_multi), else streamed through the GPUs in ranges of at most 40 GB (two range
   // buffers + a round of reads have to fit, run_streamed).  Several databases that fit the budget together are resident.
   bool want_shards = false;
   uint64_t all_hbm = 0;
@@ -2299,24 +2519,26 @@ int main(int argc, char **argv) {
          << (cfg.hll_mode == KUQ_HLL_EXACT ? "" : " (unique k-mer counts follow the -x rule)") << endl;
   if (getenv("KUQ_SPARSE_SLOTS")) cfg.sparse_set_slots = strtoull(getenv("KUQ_SPARSE_SLOTS"), NULL, 10);
   if (getenv("KUQ_DEVICE")) cfg.device = atoi(getenv("KUQ_DEVICE"));
-  // devices: KUQ_DEVICES=0,2,3 (or "all"); default = every visible sm_90 GPU when the databases are replicated (they fit
-  // a card together), else one device (KUQ_DEVICE).  Streamed ranges run on the first device.
+  // devices: KUQ_DEVICES=0,2,3 (or "all"); default = every visible sm_90 GPU, whether the databases are replicated (they
+  // fit a card), sharded (they fit the cards together) or streamed in ranges (each GPU streams its share of the ranges);
+  // KUQ_DEVICE=n: that one device.
   vector<int> devices;
   {
     const char *dl = getenv("KUQ_DEVICES");
-    const bool replicable = !chunk_budget;   // replicas when the database fits a card, shards when it only fits the cards together
     if (dl && strcmp(dl, "all") != 0) {
       for (const char *q = dl; *q;) { devices.push_back(atoi(q)); while (*q && *q != ',') q++; if (*q) q++; }
-    } else if ((dl || !getenv("KUQ_DEVICE")) && replicable) {
+    } else if (dl || !getenv("KUQ_DEVICE")) {
       for (int d = 0; d < kuq_device_count(); d++) devices.push_back(d);
     }
-    if (devices.empty() || !replicable) devices.assign(1, devices.empty() ? cfg.device : devices[0]);
+    if (devices.empty()) devices.assign(1, cfg.device);
     cfg.device = devices[0];
   }
+  if (chunk_budget && devices.size() > 1) cfg.n_slots = 2;     // streamed over several GPUs: slots 0 and 1, as shards
   kuq_ctx *ctx = NULL;
   int rc = kuq_create(&cfg, &ctx);
   if (rc) die(EX_UNAVAILABLE, string("libkuq: ") + kuq_strerror(rc));
   All_ctx.assign(1, ctx);
+  vector<int> ctx_devices(1, cfg.device);
   for (size_t g = 1; g < devices.size(); g++) {
     kuq_config c2 = cfg;
     c2.device = devices[g];
@@ -2324,9 +2546,12 @@ int main(int argc, char **argv) {
     int r2 = kuq_create(&c2, &cx);
     if (r2) { fprintf(stderr, "classify: device %d not usable (%s): continuing without it\n", devices[g], kuq_strerror(r2)); continue; }
     All_ctx.push_back(cx);
+    ctx_devices.push_back(devices[g]);
   }
+  // shards on fewer than two contexts: streamed instead, over the contexts there are
   if (want_shards && All_ctx.size() < 2) { want_shards = false; chunk_budget = std::min<uint64_t>(hbm_budget / 4, 40ull << 30); }
-  if (All_ctx.size() > 1 && !want_shards && n_db == 1) fprintf(stderr, "classify: %zu GPUs, database replicated, batches round-robin\n", All_ctx.size());
+  if (All_ctx.size() > 1 && !want_shards && !chunk_budget && n_db == 1)
+    fprintf(stderr, "classify: %zu GPUs, database replicated, batches round-robin\n", All_ctx.size());
   if (n_db > 1 && !chunk_budget && !want_shards) fprintf(stderr, "classify: %zu databases resident on %zu GPU(s)\n", n_db, All_ctx.size());
   // -q: the preloaded path leaves a read at its -m'th hit; with -x every k-mer is counted (classify.cpp:943-944 / :701-738)
   for (kuq_ctx *c : All_ctx)
@@ -2391,7 +2616,7 @@ int main(int argc, char **argv) {
   uint32_t shard_phases = 0;
   if (want_shards && n_db == 1) stage_sharded(All_ctx, kdb, idx, db_counts[0]);
   else if (want_shards) shard_phases = stage_sharded_multi(All_ctx, kdbs, idxs, db_counts);
-  else if (chunk_budget) stage_streamed(streamed, ctx, kdbs, idxs, chunk_budget, hbm_budget, db_counts);
+  else if (chunk_budget) stage_streamed(streamed, All_ctx, ctx_devices, kdbs, idxs, chunk_budget, hbm_budget, db_counts);
 #ifdef EXACT_COUNTING
   // classifyExact on several contexts: the counters join the first context, and the exact k-mer sets are spread over
   // all contexts by k-mer instead of united on one card, so no card has to hold the union.  The report's clades come
@@ -2439,7 +2664,7 @@ int main(int argc, char **argv) {
     gettimeofday(&tv1, NULL);
     const vector<pair<const char *, const char *>> files = files_of(sample);
     if (want_shards) shard_loop(All_ctx, n_db == 1 ? 1 : shard_phases, n_db > 1, files);
-    else if (chunk_budget) classify_streamed(streamed, ctx, files);
+    else if (chunk_budget) classify_streamed(streamed, files);
     else for (auto &in : files) process_file(ctx, in.first, in.second);
     // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
     {

@@ -3171,10 +3171,12 @@ int kuq_stream_check(kuq_ctx *ctx) {
 
 int kuq_host_register(void *p, uint64_t bytes) {
   if (!p || !bytes) return KUQ_E_INVALID_ARG;
-  if (cudaHostRegister(p, bytes, cudaHostRegisterDefault) == cudaSuccess) return KUQ_OK;
+  // portable: the memory counts as pinned for every device, so each GPU streaming its ranges from one mapping overlaps
+  // its copies with its lookups
+  if (cudaHostRegister(p, bytes, cudaHostRegisterPortable) == cudaSuccess) return KUQ_OK;
   (void)cudaGetLastError();
   // a read-only mapping (mmap PROT_READ of database.kdb) can only be pinned read-only
-  if (cudaHostRegister(p, bytes, cudaHostRegisterReadOnly) == cudaSuccess) return KUQ_OK;
+  if (cudaHostRegister(p, bytes, cudaHostRegisterPortable | cudaHostRegisterReadOnly) == cudaSuccess) return KUQ_OK;
   (void)cudaGetLastError();
   return KUQ_E_CUDA;
 }
