@@ -15,6 +15,8 @@
 //                                  ignores the merger's status and exits 0)
 //   --extract                      scripts/krakenuniq-extract-reads run on our Kraken lines and inputs: the reads of the
 //                                  chosen taxa are written while the batch is formatted (INTEGRATION.md)
+//   --mpa-report / --translate-out scripts/krakenuniq-mpa-report and scripts/krakenuniq-translate run on our Kraken
+//                                  lines: booked while the batch is formatted, the table written after the last sample
 //   --sample-sheet                 no counterpart: one process stages the database(s) once and classifies every row of
 //                                  the sheet as a separate run would, with kuq_reset_counts between the samples
 // Not supported (exit with a message): -I uid mapping, -x together with several -d databases (the reference's own loop
@@ -30,6 +32,7 @@
 
 #include <dlfcn.h>
 #include <omp.h>
+#include <atomic>
 #include <condition_variable>
 #include <deque>
 #include <mutex>
@@ -44,10 +47,12 @@
 #include <iomanip>
 #include <iostream>
 #include <map>
+#include <memory>
 #include <set>
 #include <sstream>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/kuq.h"
@@ -71,6 +76,11 @@ static bool Extract = false, Extract_subtree = false, Extract_invert = false, Ex
 static bool Extract_now = false;                  // this sample writes an extraction (a sheet row may leave it out)
 static string Extract_list, Extract_output_file;
 static vector<uint32_t> Extract_taxa;             // the list's decimal taxids ("-1" is Extract_others)
+// --mpa-report: one krakenuniq-mpa-report table over the Kraken lines of every sample of the run; --translate-out: the
+// lines krakenuniq-translate [--mpa-format] prints from a sample's Kraken lines (both with -a's taxDB)
+static bool Mpa = false, Mpa_show_zeros = false, Mpa_header_line = false, Mpa_intermediate = false, Translate_mpa = false;
+static bool Translate_now = false;                // this sample writes a translation (a sheet row may leave it out)
+static string Mpa_output_file, Translate_output_file;
 static uint64_t Populate_memory_size = 0;
 static string Classified_output_file, Unclassified_output_file, Kraken_output_file, Report_output_file, TaxDB_file;
 static size_t Work_unit_size = 500000;      // DEF_WORK_UNIT_SIZE, classify.cpp:38
@@ -123,7 +133,14 @@ static void usage(int exit_code = EX_USAGE) {
        << "                   ('-' = stdout, .gz = gzip; a --sample-sheet column extract_out instead)" << endl
        << "  --extract-subtree  with the children of the taxa in -a's taxDB (the script's -t)" << endl
        << "  --extract-invert   every read not selected (-i)       --extract-fasta  FASTQ reads as FASTA (-f)" << endl
-       << "  -h               Print this message" << endl
+       << "  --mpa-report f   Write the table krakenuniq-mpa-report prints from the Kraken lines to f, one count column" << endl
+       << "                   per sample ('-' = stdout, .gz = gzip; needs -a; a --sample-sheet writes one table)" << endl
+       << "  --mpa-show-zeros, --mpa-header-line, --mpa-intermediate-ranks   the script's --show-zeros," << endl
+       << "                   --header-line (sample ids = the Kraken output files) and --intermediate-ranks" << endl
+       << "  --translate-out f  Write what krakenuniq-translate prints from the Kraken lines (read id, lineage) to f" << endl
+       << "                   ('-' = stdout, .gz = gzip; needs -a; a --sample-sheet column translate_out instead)" << endl
+       << "  --translate-mpa-format  lineages in the script's --mpa-format" << endl
+       << "  -h              Print this message" << endl
        << endl
        << "Kraken output is to standard output by default." << endl;
   exit(exit_code);
@@ -162,7 +179,8 @@ static void parse_command_line(int argc, char **argv) {
   long long sig;
   if (argc > 1 && strcmp(argv[1], "-h") == 0) usage(0);
   enum { OPT_PAIRED = 256, OPT_CHECK_NAMES, OPT_SAMPLE_SHEET, OPT_THRESHOLD, OPT_EXTRACT, OPT_EXTRACT_OUT, OPT_EXTRACT_SUBTREE,
-         OPT_EXTRACT_INVERT, OPT_EXTRACT_FASTA };
+         OPT_EXTRACT_INVERT, OPT_EXTRACT_FASTA, OPT_MPA_REPORT, OPT_MPA_SHOW_ZEROS, OPT_MPA_HEADER_LINE, OPT_MPA_INTERMEDIATE,
+         OPT_TRANSLATE_OUT, OPT_TRANSLATE_MPA };
   static const struct option long_opts[] = {{"paired", no_argument, NULL, OPT_PAIRED},
                                             {"check-names", no_argument, NULL, OPT_CHECK_NAMES},
                                             {"sample-sheet", required_argument, NULL, OPT_SAMPLE_SHEET},
@@ -171,7 +189,13 @@ static void parse_command_line(int argc, char **argv) {
                                             {"extract-out", required_argument, NULL, OPT_EXTRACT_OUT},
                                             {"extract-subtree", no_argument, NULL, OPT_EXTRACT_SUBTREE},
                                             {"extract-invert", no_argument, NULL, OPT_EXTRACT_INVERT},
-                                            {"extract-fasta", no_argument, NULL, OPT_EXTRACT_FASTA}, {NULL, 0, NULL, 0}};
+                                            {"extract-fasta", no_argument, NULL, OPT_EXTRACT_FASTA},
+                                            {"mpa-report", required_argument, NULL, OPT_MPA_REPORT},
+                                            {"mpa-show-zeros", no_argument, NULL, OPT_MPA_SHOW_ZEROS},
+                                            {"mpa-header-line", no_argument, NULL, OPT_MPA_HEADER_LINE},
+                                            {"mpa-intermediate-ranks", no_argument, NULL, OPT_MPA_INTERMEDIATE},
+                                            {"translate-out", required_argument, NULL, OPT_TRANSLATE_OUT},
+                                            {"translate-mpa-format", no_argument, NULL, OPT_TRANSLATE_MPA}, {NULL, 0, NULL, 0}};
   while ((opt = getopt_long(argc, argv, "d:i:t:u:n:m:o:qcC:U:Ma:r:sI:p:x:", long_opts, NULL)) != -1) {
     switch (opt) {
       case OPT_PAIRED: Paired = true; break;
@@ -190,6 +214,12 @@ static void parse_command_line(int argc, char **argv) {
       case OPT_EXTRACT_SUBTREE: Extract_subtree = true; break;
       case OPT_EXTRACT_INVERT: Extract_invert = true; break;
       case OPT_EXTRACT_FASTA: Extract_fasta = true; break;
+      case OPT_MPA_REPORT: Mpa = true; Mpa_output_file = optarg; break;
+      case OPT_MPA_SHOW_ZEROS: Mpa_show_zeros = true; break;
+      case OPT_MPA_HEADER_LINE: Mpa_header_line = true; break;
+      case OPT_MPA_INTERMEDIATE: Mpa_intermediate = true; break;
+      case OPT_TRANSLATE_OUT: Translate_output_file = optarg; break;
+      case OPT_TRANSLATE_MPA: Translate_mpa = true; break;
       case 'd': DB_filenames.push_back(optarg); break;
       case 'i': Index_filenames.push_back(optarg); break;
       case 't':
@@ -240,6 +270,11 @@ static void parse_command_line(int argc, char **argv) {
       die(EX_USAGE, "--sample-sheet takes the extraction's file from the sheet: --extract-out is its column extract_out");
     if (Sample_sheet.empty() && Extract_output_file.empty()) die(EX_USAGE, "--extract needs --extract-out");
   }
+  if (!Mpa && (Mpa_show_zeros || Mpa_header_line || Mpa_intermediate))
+    die(EX_USAGE, "--mpa-show-zeros, --mpa-header-line and --mpa-intermediate-ranks need --mpa-report");
+  if (!Sample_sheet.empty() && !Translate_output_file.empty())
+    die(EX_USAGE, "--sample-sheet takes the translation's file from the sheet: --translate-out is its column translate_out");
+  if (Sample_sheet.empty() && Translate_mpa && Translate_output_file.empty()) die(EX_USAGE, "--translate-mpa-format needs --translate-out");
   if (DB_filenames.empty()) { cerr << "Missing mandatory option -d" << endl; usage(); }
   if (Index_filenames.empty()) { cerr << "Missing mandatory option -i" << endl; usage(); }
   if (!Sample_sheet.empty()) {                      // the sheet names every sample's inputs and outputs
@@ -258,7 +293,7 @@ static void parse_command_line(int argc, char **argv) {
 struct Sample {
   string name;
   vector<pair<string, string>> inputs;
-  string kraken, report, classified, unclassified, extract;
+  string kraken, report, classified, unclassified, extract, translate;
 };
 
 static vector<pair<const char *, const char *>> files_of(const Sample &s) {
@@ -285,7 +320,7 @@ static vector<Sample> read_sample_sheet(const string &path) {
   ifstream in(path);
   if (!in.is_open()) die(EX_NOINPUT, "can't open the sample sheet " + path);
   static const set<string> known = {"input", "input2", "output", "report", "classified_out", "unclassified_out", "name",
-                                    "extract_out"};
+                                    "extract_out", "translate_out"};
   map<string, size_t> col;
   vector<Sample> samples;
   map<string, string> written;                     // path_key -> which sample writes it
@@ -298,7 +333,7 @@ static vector<Sample> read_sample_sheet(const string &path) {
     const string at = path + ":" + to_string(line_no) + ": ";
     if (col.empty()) {
       for (size_t i = 0; i < f.size(); i++) {
-        if (!known.count(f[i])) die(EX_USAGE, at + "unknown column '" + f[i] + "' (columns: input input2 output report classified_out unclassified_out name extract_out)");
+        if (!known.count(f[i])) die(EX_USAGE, at + "unknown column '" + f[i] + "' (columns: input input2 output report classified_out unclassified_out name extract_out translate_out)");
         if (!col.emplace(f[i], i).second) die(EX_USAGE, at + "column '" + f[i] + "' named twice");
       }
       if (!col.count("input")) die(EX_USAGE, at + "the header has no input column");
@@ -306,6 +341,7 @@ static vector<Sample> read_sample_sheet(const string &path) {
       if (!Paired && col.count("input2")) die(EX_USAGE, at + "an input2 column needs --paired");
       if (Extract && !col.count("extract_out")) die(EX_USAGE, at + "--extract needs an extract_out column");
       if (!Extract && col.count("extract_out")) die(EX_USAGE, at + "an extract_out column needs --extract");
+      if (Translate_mpa && !col.count("translate_out")) die(EX_USAGE, at + "--translate-mpa-format needs a translate_out column");
       continue;
     }
     if (f.size() > col.size()) die(EX_USAGE, at + "more cells than the header has columns");
@@ -334,7 +370,8 @@ static vector<Sample> read_sample_sheet(const string &path) {
     s.classified = cell("classified_out");
     s.unclassified = cell("unclassified_out");
     s.extract = cell("extract_out");                // empty: nothing is extracted from this sample
-    for (const string *o : {&s.kraken, &s.report, &s.classified, &s.unclassified, &s.extract}) {
+    s.translate = cell("translate_out");            // empty: this sample's reads are not translated
+    for (const string *o : {&s.kraken, &s.report, &s.classified, &s.unclassified, &s.extract, &s.translate}) {
       if (o->empty() || *o == "off" || *o == "-") continue;
       auto w = written.emplace(path_key(*o), s.name);
       if (!w.second) die(EX_USAGE, at + "samples " + w.first->second + " and " + s.name + " both write " + *o);
@@ -715,6 +752,8 @@ struct TaxDB {
   vector<TaxEntry> e;
   unordered_map<uint32_t, int> idx;
   vector<uint32_t> row_ids, row_parents;   // every row in file order (krakenuniq-filter's parent map, kuq_set_threshold)
+  bool keep_text = false;                  // also every row's name and rank (krakenuniq-mpa-report / -translate's maps)
+  vector<string> row_names, row_ranks;
   void read(const string &path) {
     ifstream in(path);
     if (!in.is_open()) die(EX_NOINPUT, "unable to open taxonomy index file " + path);
@@ -733,6 +772,10 @@ struct TaxDB {
       row_parents.push_back(par);
       t.name = line.substr(b + 1, c == string::npos ? string::npos : c - b - 1);
       t.rank = c == string::npos ? "" : line.substr(c + 1);
+      if (keep_text) {                                              // split(/\t/): the rank is the fourth field
+        row_names.push_back(t.name);
+        row_ranks.push_back(c == string::npos ? "" : line.substr(c + 1, line.find('\t', c + 1) - c - 1));
+      }
       if (idx.count(t.id)) continue;                                // entries.insert keeps the first
       idx[t.id] = (int)e.size();
       e.push_back(t);
@@ -861,6 +904,198 @@ static void print_report(kuq_ctx *ctx, TaxDB &tax, ostream &out) {
   cerr << " done" << endl;
 }
 
+// ---- --mpa-report / --translate-out: the rules of scripts/krakenuniq-mpa-report and scripts/krakenuniq-translate ----
+// Both scripts read the taxDB the same way (load_taxonomy): every row split on tabs, the name and the rank of a taxid
+// from its last row.  mpa-report's child lists get one entry per row whose parent differs from its taxid, in file order
+// (a taxid with two rows is listed, summed and printed twice); translate's parent map F is the one of krakenuniq-filter.
+// Both take a Kraken line's fields as Perl's split on whitespace does: a line with an empty read id ("C\t\t562\t150...")
+// has the taxon as its second field and the length as its third, which the scripts read as read id and taxid.
+static char rank_code(const string &rank) {        // rank_code, mpa-report:168-182 / translate:115-128
+  static const char *const ranks[] = {"species", "genus", "family", "order", "class", "phylum", "superkingdom", "kingdom"};
+  static const char codes[] = "SGFOCPDK";
+  for (int i = 0; i < 8; i++) if (rank == ranks[i]) return codes[i];
+  return '-';
+}
+
+struct ScriptTax {
+  unordered_map<uint32_t, uint32_t> last_row;     // name_map / rank_map: the taxid's last row
+  vector<string> names, ranks;                    // per row
+  unordered_map<uint32_t, vector<uint32_t>> children;
+  unordered_map<uint32_t, uint32_t> F;
+  // translate's lineage of every taxid with an F entry, computed the first time a line needs it (by any formatting
+  // thread: `ready` 0 = not yet, 1 = being computed, 2 = done), and the node where its walk stops
+  unordered_map<uint32_t, uint32_t> node;          // taxid -> slot
+  vector<uint32_t> node_taxid, stop;
+  vector<string> lineage;
+  std::unique_ptr<std::atomic<uint8_t>[]> ready;
+  bool mpa_format = false;
+
+  const string &name(uint32_t t) const { static const string none; auto it = last_row.find(t); return it == last_row.end() ? none : names[it->second]; }
+  const string &rank(uint32_t t) const { static const string none; auto it = last_row.find(t); return it == last_row.end() ? none : ranks[it->second]; }
+
+  // false when F has a cycle (the script's walk never ends)
+  bool build(const TaxDB &tax, bool translate) {
+    names = tax.row_names;
+    ranks = tax.row_ranks;
+    for (uint32_t i = 0; i < tax.row_ids.size(); i++) {
+      const uint32_t t = tax.row_ids[i], p = tax.row_parents[i];
+      last_row[t] = i;
+      if (p != t) { children[p].push_back(t); F[t] = p; }
+    }
+    if (!translate) return true;
+    for (auto &kv : F) { node.emplace(kv.first, (uint32_t)node_taxid.size()); node_taxid.push_back(kv.first); }
+    const size_t n = node_taxid.size();
+    stop.assign(n, 0);
+    lineage.assign(n, string());
+    ready.reset(new std::atomic<uint8_t>[n]);
+    vector<uint8_t> state(n, 0);                   // 1 = on the current walk, 2 = its stop is known
+    vector<uint32_t> path;
+    for (uint32_t i = 0; i < n; i++) {
+      ready[i].store(0, std::memory_order_relaxed);
+      path.clear();
+      uint32_t x = node_taxid[i];
+      for (auto it = node.find(x); it != node.end() && state[it->second] != 2; it = node.find(x)) {
+        if (state[it->second] == 1) return false;
+        state[it->second] = 1;
+        path.push_back(it->second);
+        x = F[x];
+      }
+      auto it = node.find(x);
+      const uint32_t end = it == node.end() ? x : stop[it->second];
+      for (uint32_t k : path) { stop[k] = end; state[k] = 2; }
+    }
+    return true;
+  }
+
+  // get_taxonomy_str's walk (translate:89-113): the names from the taxon up to the first node without an F entry,
+  // which is left out; with --mpa-format only nodes with a rank code, as code__name with spaces turned into '_'
+  string walk(uint32_t x) const {
+    vector<string> parts;
+    for (auto it = F.find(x); it != F.end(); x = it->second, it = F.find(x)) {
+      if (!mpa_format) { parts.push_back(name(x)); continue; }
+      const char code = rank_code(rank(x));
+      if (code == '-') continue;
+      string s = string(1, (char)tolower(code)) + "__" + name(x);
+      replace(s.begin(), s.end(), ' ', '_');
+      parts.push_back(s);
+    }
+    if (parts.empty()) return mpa_format ? "root" : "";
+    string out;
+    for (size_t k = parts.size(); k-- > 0;) { out += parts[k]; if (k) out += mpa_format ? '|' : ';'; }
+    return out;
+  }
+  const string &lineage_at(uint32_t i) {
+    if (ready[i].load(std::memory_order_acquire) == 2) return lineage[i];
+    uint8_t z = 0;
+    if (ready[i].compare_exchange_strong(z, 1, std::memory_order_acq_rel)) {
+      lineage[i] = walk(node_taxid[i]);
+      ready[i].store(2, std::memory_order_release);
+    }
+    while (ready[i].load(std::memory_order_acquire) != 2) std::this_thread::yield();
+    return lineage[i];
+  }
+  const string &empty_lineage() const { static const string root = "root", none; return mpa_format ? root : none; }
+
+  // krakenuniq-mpa-report (:95-125) over the lines per taxid of each sample, in sample order
+  string mpa_table(const vector<unordered_map<uint64_t, uint64_t>> &taxo_counts, const vector<string> &ids,
+                   bool show_zeros, bool header_line, bool intermediate) const {
+    vector<unordered_map<uint64_t, uint64_t>> clade(taxo_counts);
+    unordered_set<uint64_t> hit;
+    for (auto &counts : clade) {
+      // dfs_summation(1) (:184-194): after each child's own summation, the child's sum is added to the node's
+      struct Frame { uint64_t node; size_t next; };
+      vector<Frame> st{{1, 0}};
+      while (!st.empty()) {
+        const uint64_t x = st.back().node;
+        auto it = x <= UINT32_MAX ? children.find((uint32_t)x) : children.end();
+        if (it == children.end() || st.back().next == it->second.size()) {
+          st.pop_back();
+          if (!st.empty()) { auto c = counts.find(x); counts[st.back().node] += c == counts.end() ? 0 : c->second; }
+          continue;
+        }
+        st.push_back({it->second[st.back().next++], 0});
+      }
+      for (auto &kv : counts) if (kv.second) hit.insert(kv.first);
+    }
+    // dfs_report(1) (:127-158): rows grouped by rank code in the order D K P C O F G S (X)
+    const string order = intermediate ? "DKPCOFGSX" : "DKPCOFGS";
+    vector<string> rows(order.size());
+    struct Visit { uint32_t node; bool named; string name; };
+    vector<Visit> st{{1, false, ""}};
+    while (!st.empty()) {
+      Visit v = std::move(st.back());
+      st.pop_back();
+      if (!show_zeros && !hit.count(v.node)) continue;
+      char code = rank_code(rank(v.node));
+      if (code != '-' || intermediate) {
+        if (code == '-') code = 'X';
+        string nm = name(v.node);
+        nm.erase(remove_if(nm.begin(), nm.end(), [](char c) { return c == '|' || c == '.'; }), nm.end());
+        replace(nm.begin(), nm.end(), ' ', '_');
+        v.name = (v.named ? v.name + "|" : string()) + (char)tolower(code) + "__" + nm;
+        v.named = true;
+        string &out = rows[order.find(code)];
+        out += v.name;
+        for (auto &counts : clade) {
+          auto c = counts.find(v.node);
+          out += '\t';
+          out += to_string(c == counts.end() ? 0 : c->second);
+        }
+        out += '\n';
+      }
+      auto it = children.find(v.node);
+      if (it != children.end())
+        for (auto k = it->second.rbegin(); k != it->second.rend(); ++k) st.push_back({*k, v.named, v.name});
+    }
+    string table;
+    if (header_line) {
+      table = "#Sample ID";
+      for (auto &id : ids) table += "\t" + id;
+      table += '\n';
+    }
+    for (auto &r : rows) table += r;
+    return table;
+  }
+};
+static ScriptTax Script_tax;
+
+// What one formatting part adds to the two scripts' outputs.  Translate lines whose taxon has an F entry are written
+// with their lineage; a line whose taxon has none prints the lineage most recently stored under that taxon (the script
+// stores each lineage under the node where its walk stopped): when this part stored one earlier, it is written here,
+// else the line is a hole that book_script fills from what the earlier parts stored.
+struct ScriptPart {
+  unordered_map<uint64_t, uint64_t> counts;        // mpa-report: lines per (script) taxid
+  string translate;
+  vector<pair<size_t, uint64_t>> holes;            // (offset in translate, taxid)
+  unordered_map<uint64_t, uint32_t> last;          // stopping node -> slot of the last lineage stored under it
+  void clear() { counts.clear(); translate.clear(); holes.clear(); last.clear(); }
+};
+
+// One Kraken line of the run (written or not): its code is 'C' when `shown` is not 0, its id is the header's first
+// whitespace-delimited token
+static void book_line(ScriptPart &p, const char *hdr, size_t hdr_len, uint64_t len, uint32_t shown) {
+  size_t x = 0;
+  while (x < hdr_len && isspace((unsigned char)hdr[x])) x++;
+  size_t y = x;
+  while (y < hdr_len && !isspace((unsigned char)hdr[y])) y++;
+  const uint64_t taxid = y > x ? shown : len;       // split: an empty id moves the fields left
+  if (Mpa) p.counts[taxid]++;
+  if (!Translate_now || !shown) return;             // translate prints the lines that start with C
+  if (y > x) p.translate.append(hdr + x, y - x);
+  else p.translate += to_string(shown);
+  p.translate += '\t';
+  auto it = taxid <= UINT32_MAX ? Script_tax.node.find((uint32_t)taxid) : Script_tax.node.end();
+  if (it != Script_tax.node.end()) {
+    p.translate += Script_tax.lineage_at(it->second);
+    p.last[Script_tax.stop[it->second]] = it->second;
+  } else {
+    auto l = p.last.find(taxid);
+    if (l != p.last.end()) p.translate += Script_tax.lineage_at(l->second);
+    else p.holes.emplace_back(p.translate.size(), taxid);
+  }
+  p.translate += '\n';
+}
+
 // ---- mmap helper ----------------------------------------------------------------------------------------------
 struct Mapped {
   void *p = NULL;
@@ -916,7 +1151,7 @@ static BatchLimits batch_limits(uint64_t batch_nt, bool aligned, bool resident) 
   return l;
 }
 
-static OutStream Kraken_out, Classified_out, Unclassified_out, Extract_out;
+static OutStream Kraken_out, Classified_out, Unclassified_out, Extract_out, Translate_out;
 
 // One read as the output sees it: the header line without its '>' / '@', the bases and (FASTQ) the qualities
 struct ReadView {
@@ -927,9 +1162,10 @@ struct ReadView {
 
 // The Kraken lines (classify.cpp:980-1010, hitlist_string :826-861) and the -C / -U records (print_sequence, :794-805)
 // of reads [a, b); read i's results are at i - res0 of `res`.  The Kraken text goes into one buffer sized up front.
+// `sp` (--mpa-report / --translate-out only) books every line the run writes, or would write with -o FILE.
 template <class ViewOf>
 static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_result &res, size_t res0, bool fastq,
-                         string &kraken, string &classified, string &unclassified) {
+                         string &kraken, string &classified, string &unclassified, ScriptPart *sp = NULL) {
   const size_t at = kraken.size();
   if (Print_kraken) {
     size_t need = 0;
@@ -958,6 +1194,7 @@ static void format_reads(ViewOf view_of, size_t a, size_t b, const kuq_batch_res
       oo.append(v.seq, v.len); oo += '\n';
       if (fastq) { oo += "+\n"; oo.append(v.qual, v.qual_len); oo += '\n'; }
     }
+    if (sp && (call || !Only_classified_kraken_output)) book_line(*sp, v.hdr, v.hdr_len, v.len, Filter ? res.filtered_call[r] : call);
     if (!Print_kraken) continue;
     if (!call && Only_classified_kraken_output) continue;            // :986-988
     // --threshold: krakenuniq-filter's line (:131-133), "%s\t<id>\t<new taxon>\t<len>\tP=%0.3f\t<hit list>\n"
@@ -1072,6 +1309,29 @@ static void write_extract(const string &text, bool selected_so_far) {
   Extract_out.write(text);
 }
 
+// A part's booking, in output order: its counts join the sample's column, its translate text is written with the holes
+// filled from what the sample's earlier parts stored (batches and input files included), then its own stores are added.
+static vector<unordered_map<uint64_t, uint64_t>> Mpa_counts;   // per sample of the run
+static vector<string> Mpa_ids;                                  // the samples' ids (--mpa-header-line)
+static unordered_map<uint64_t, uint32_t> Translate_stored;      // the sample's last lineage per stopping node
+static bool scripts_now() { return Mpa || Translate_now; }
+static void book_script(const ScriptPart &p) {
+  if (Mpa) {
+    auto &c = Mpa_counts.back();
+    for (auto &kv : p.counts) c[kv.first] += kv.second;
+  }
+  if (!Translate_now) return;
+  size_t at = 0;
+  for (auto &h : p.holes) {
+    Translate_out.write(p.translate.data() + at, h.first - at);
+    auto it = Translate_stored.find(h.second);
+    Translate_out.write(it == Translate_stored.end() ? Script_tax.empty_lineage() : Script_tax.lineage_at(it->second));
+    at = h.first;
+  }
+  Translate_out.write(p.translate.data() + at, p.translate.size() - at);
+  for (auto &kv : p.last) Translate_stored[kv.first] = kv.second;
+}
+
 // The output of reads [a, b) of a batch, whose results start at read a (the whole batch, or a GPU's share of it)
 static void write_reads(const Batch &bt, const kuq_batch_result &res, size_t a, size_t b) {
   string kraken, classified, unclassified;
@@ -1079,7 +1339,10 @@ static void write_reads(const Batch &bt, const kuq_batch_result &res, size_t a, 
     const Read &r = bt.reads[i];
     return ReadView{r.header_line.data(), r.header_line.size(), bt.bases.data() + r.seq_off, r.seq_len, r.quals.data(), r.quals.size()};
   };
-  format_reads(view_of, a, b, res, a, bt.fastq, kraken, classified, unclassified);
+  static ScriptPart sp;
+  sp.clear();
+  format_reads(view_of, a, b, res, a, bt.fastq, kraken, classified, unclassified, scripts_now() ? &sp : NULL);
+  if (scripts_now()) book_script(sp);
   Kraken_out.write(kraken);
   Classified_out.write(classified);
   Unclassified_out.write(unclassified);
@@ -1121,7 +1384,7 @@ static int db_taxids(kuq_ctx *ctx, map<uint32_t, uint64_t> &into) {
 
 // background writer: formatted text is handed over batch by batch and written in order while the next batch is
 // being gathered / classified / formatted
-struct OutJob { vector<string> kraken, classified, unclassified, extract; bool extract_selected = false; };
+struct OutJob { vector<string> kraken, classified, unclassified, extract; vector<ScriptPart> script; bool extract_selected = false; };
 struct Writer {
   std::mutex m;
   std::condition_variable cv;
@@ -1139,6 +1402,8 @@ struct Writer {
     for (auto &x : j.classified) x.clear();
     for (auto &x : j.unclassified) x.clear();
     for (auto &x : j.extract) x.clear();
+    j.script.resize(scripts_now() ? parts : 0);
+    for (auto &x : j.script) x.clear();
     return j;
   }
   void finish() { { std::lock_guard<std::mutex> l(m); done = true; } cv.notify_one(); if (th.joinable()) th.join(); }
@@ -1159,6 +1424,7 @@ void Writer::run() {
     for (auto &x : j.classified) Classified_out.write(x);
     for (auto &x : j.unclassified) Unclassified_out.write(x);
     if (Extract_now) for (auto &x : j.extract) write_extract(x, j.extract_selected);
+    for (auto &x : j.script) book_script(x);
     { std::lock_guard<std::mutex> l(m); if (spare.size() < 3) spare.push_back(std::move(j)); }
   }
 }
@@ -1604,7 +1870,8 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
     auto x_of = [&](size_t i) { return mapped_record(*rv[s.begin + i], mate2 ? &mates[s.begin + i] : NULL, in, fastq_records); };
 #pragma omp parallel for schedule(static, 1) num_threads(Te)
     for (int pi = 0; pi < parts; pi++) {
-      format_reads(view_of, n * pi / parts, n * (pi + 1) / parts, res, 0, fastq, job.kraken[pi], job.classified[pi], job.unclassified[pi]);
+      format_reads(view_of, n * pi / parts, n * (pi + 1) / parts, res, 0, fastq, job.kraken[pi], job.classified[pi], job.unclassified[pi],
+                   job.script.empty() ? NULL : &job.script[pi]);
       if (extract) extract_reads(x_of, n * pi / parts, n * (pi + 1) / parts, res, 0, !fastq_records, job.extract[pi]);
     }
     writer.push(std::move(job));
@@ -2431,12 +2698,64 @@ static void check_extract(const vector<Sample> &samples, TaxDB &tax, bool &tax_r
         if (!o->empty() && *o != "-" && *o != "off" && path_key(*o) == key) die(EX_USAGE, "--extract-out " + s.extract + " is another output");
   }
   if (!Extract_subtree) return;
-  tax.read(TaxDB_file);
+  if (!tax_read) tax.read(TaxDB_file);                             // (check_scripts may have read it)
   tax_read = true;
   uint32_t n = 0;
   if (kuq_extract_taxa(Extract_taxa.data(), (uint32_t)Extract_taxa.size(), KUQ_EXTRACT_SUBTREE, tax.row_ids.data(),
                        tax.row_parents.data(), (uint32_t)tax.row_ids.size(), NULL, 0, &n))
     die(EX_USAGE, "--extract-subtree: the children of the listed taxa in " + TaxDB_file + " form a cycle");
+}
+
+// The checks of --mpa-report and --translate-out, before any database file is opened: -a, where the outputs go (not
+// onto an input or another output, one writer of standard output), and the taxonomy's cycles that keep the scripts
+// going forever: a cycle of the child lists reachable from 1 (mpa-report's recursion) or of F (translate's walk).  The
+// taxonomy is read here.
+static void check_scripts(const vector<Sample> &samples, TaxDB &tax, bool &tax_read) {
+  bool translate = false;
+  for (const Sample &s : samples) translate = translate || !s.translate.empty();
+  if (!Mpa && !translate) return;
+  if (TaxDB_file.empty()) die(EX_USAGE, "--mpa-report and --translate-out take the taxonomy from the taxDB: give it with -a");
+  set<string> in_keys;
+  if (!Sample_sheet.empty()) in_keys.insert(path_key(Sample_sheet));
+  vector<pair<string, bool>> outs;                 // every output of the run; true: one of this feature's
+  for (const Sample &s : samples) {
+    for (auto &f : s.inputs) {
+      in_keys.insert(path_key(f.first));
+      if (!f.second.empty()) in_keys.insert(path_key(f.second));
+    }
+    if (Sample_sheet.empty()) {
+      outs.emplace_back(Kraken_output_file.empty() ? "-" : Kraken_output_file == "-" ? "off" : Kraken_output_file, false);
+      for (const string *o : {&Report_output_file, &Classified_output_file, &Unclassified_output_file}) outs.emplace_back(*o, false);
+    } else {
+      for (const string *o : {&s.kraken, &s.report, &s.classified, &s.unclassified}) outs.emplace_back(*o, false);
+    }
+    outs.emplace_back(s.extract, false);
+    outs.emplace_back(s.translate, true);
+  }
+  if (Mpa) outs.emplace_back(Mpa_output_file, true);
+  for (size_t i = 0; i < outs.size(); i++) {
+    const string &o = outs[i].first;
+    if (!outs[i].second || o.empty() || o == "off") continue;
+    for (size_t j = 0; j < outs.size(); j++) {
+      const string &q = outs[j].first;
+      if (j == i || q.empty() || q == "off") continue;
+      if (o == "-" && q == "-") die(EX_USAGE, "two outputs go to standard output (--mpa-report / --translate-out -)");
+      if (o != "-" && q != "-" && path_key(o) == path_key(q)) die(EX_USAGE, o + " is written twice");
+    }
+    if (o != "-" && in_keys.count(path_key(o))) die(EX_USAGE, o + " is one of the inputs");
+  }
+  tax.keep_text = true;
+  tax.read(TaxDB_file);
+  tax_read = true;
+  if (Mpa) {
+    const uint32_t root = 1;
+    uint32_t n = 0;
+    if (kuq_extract_taxa(&root, 1, KUQ_EXTRACT_SUBTREE, tax.row_ids.data(), tax.row_parents.data(), (uint32_t)tax.row_ids.size(),
+                         NULL, 0, &n))
+      die(EX_USAGE, "--mpa-report: the children of taxon 1 in " + TaxDB_file + " form a cycle");
+  }
+  Script_tax.mpa_format = Translate_mpa;
+  if (!Script_tax.build(tax, translate)) die(EX_USAGE, "--translate-out: the parents in " + TaxDB_file + " form a cycle");
 }
 
 int main(int argc, char **argv) {
@@ -2453,10 +2772,12 @@ int main(int argc, char **argv) {
     Sample s;
     for (int i = optind; i < argc; i += Paired ? 2 : 1) s.inputs.emplace_back(argv[i], Paired ? argv[i + 1] : "");
     s.extract = Extract_output_file;
+    s.translate = Translate_output_file;
     samples.push_back(s);
   }
   TaxDB tax;
   bool tax_read = false;
+  check_scripts(samples, tax, tax_read);
   if (Extract) check_extract(samples, tax, tax_read);
   if (Populate_memory && Populate_memory_size == 0) cerr << "Loading database(s)... " << endl;
   vector<Mapped> kdbs(n_db), idxs(n_db);
@@ -2651,6 +2972,14 @@ int main(int argc, char **argv) {
     Extract_now = Extract && !sample.extract.empty();
     Extract_selected = 0;
     if (Extract_now) Extract_out.open(sample.extract);
+    Translate_now = !sample.translate.empty();
+    Translate_stored.clear();
+    if (Translate_now) Translate_out.open(sample.translate);
+    if (Mpa) {                                                      // the script names a column after its Kraken file
+      Mpa_counts.emplace_back();
+      const string &k = sheet ? sample.kraken : Kraken_output_file;
+      Mpa_ids.push_back(!k.empty() && k != "off" && k != "-" ? k : sheet ? sample.name : "-");
+    }
     if (Print_classified) Classified_out.open(Classified_output_file);
     if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);
     if (!Kraken_output_file.empty()) {
@@ -2752,6 +3081,7 @@ int main(int argc, char **argv) {
     Unclassified_out.close();
     string().swap(Extract_pending);                                  // no read was selected: nothing is written
     Extract_out.close();
+    Translate_out.close();
     // the records before the merger's stop are classified and written, like the wrapper's run on its partial output; the
     // samples after it still run
     if (!Pair_error.empty()) {
@@ -2761,6 +3091,12 @@ int main(int argc, char **argv) {
     }
   }
   Sample_label.clear();
+  if (Mpa) {                                                        // one table for every sample of the run
+    OutStream mo;
+    mo.open(Mpa_output_file);
+    mo.write(Script_tax.mpa_table(Mpa_counts, Mpa_ids, Mpa_show_zeros, Mpa_header_line, Mpa_intermediate));
+    mo.close();
+  }
   for (const void *p : streamed.pinned) kuq_host_unregister((void *)p);
   for (kuq_ctx *c : All_ctx) kuq_destroy(c);
   return status;

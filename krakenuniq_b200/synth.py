@@ -216,6 +216,22 @@ def make_taxonomy(n_species: int, n_genera: int = 0, n_families: int = 0, first_
     return Taxonomy(rows)
 
 
+def add_upper_ranks(rows):
+    """rows with superkingdom, kingdom, phylum, class and order nodes (ids 2..17) between the root and the families that
+    hang from it, so that every rank code of the MetaPhlAn-style report occurs"""
+    upper = [(2, 1, "Bacteria", "superkingdom"), (3, 2, "Kingdom one", "kingdom"), (4, 3, "Phylum a", "phylum"),
+             (5, 3, "Phylum b", "phylum")]
+    upper += [(6 + i, 4 + i % 2, f"Class {i}", "class") for i in range(4)]
+    upper += [(10 + i, 6 + i % 4, f"Order {i}", "order") for i in range(8)]
+    out, n_fam = [], 0
+    for t, p, name, rank in rows:
+        if rank == "family" and p == 1:
+            p = 10 + n_fam % 8
+            n_fam += 1
+        out.append((t, p, name, rank))
+    return out[:1] + upper + out[1:]
+
+
 def species_ids(tax: Taxonomy):
     return [r[0] for r in tax.rows if r[3] == "species"]
 
