@@ -2044,19 +2044,19 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 
 // ---- databases that do not fit the HBM budget: streamed through two range buffers ----------------------------------
 // One database larger than the budget (the -x path, process_file_with_db_chunk, classify.cpp:566-791), or several
-// databases that do not fit it together (`-d a -d b`, classify.cpp:928-936).  The input is read in rounds: a round's
-// reads and per-window ids stay in HBM (5 bytes per base + 8 per read, + 4 per read of unit ids) next to the two range
-// buffers, as many batches as fit the budget and at least one.  Each round goes through the databases in command-line
-// order and each database through its minimizer ranges (kuq_stream_*: the next range travels while the current one is
-// looked up).  The first database writes its hits, a stored zero as KUQ_CODE_FOUND_ZERO; the later ones only fill the
-// windows that no earlier database answered (KUQ_LOOKUP_FILL_EMPTY).  Then the round's batches are resolved and written
-// in input order.  One database keeps the -x rule (one sketch per taxon; batches need not hold whole work units);
-// several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b` without -x.
-// stage_streamed runs once per process: the ranges, the taxids of every record and the pinned registration of the mapped
-// files.  classify_streamed runs once per sample: its rounds of reads, each through every range.
-//   Several GPUs (classify_streamed_gpus): every database keeps the same ranges, and GPU g streams a contiguous group of
-//   them (kuq_ranges.h, group_ranges) over its own host link.  Every GPU holds every batch of a round; each batch has one
-//   owner that holds its id buffer, and every GPU stores its hits straight into the owner's buffer (peer stores).
+// databases that do not fit it together (`-d a -d b`, classify.cpp:928-936), on the run's G >= 1 contexts.  Every
+// database keeps the ranges plan_ranges cuts at the chunk budget, whatever G, and GPU g streams a contiguous group of
+// them (kuq_ranges.h, group_ranges) over its own host link (kuq_stream_*: the next range travels while the current one is
+// looked up).  The input is read in rounds that stay in HBM next to the two range buffers: every GPU holds every batch
+// of a round, and each batch has one owner that alone holds its per-window ids (5 bytes per base + 8 per read, + 4 per
+// read of unit ids, on one GPU), as many batches as fit the tightest context and at least one.  Each round goes through
+// the databases in command-line order, and every GPU stores its hits straight into the owner's buffer (peer stores when
+// the owner is another GPU).  The first database writes its hits, a stored zero as KUQ_CODE_FOUND_ZERO; the later ones
+// only fill the windows that no earlier database answered (KUQ_LOOKUP_FILL_EMPTY).  Then the owners resolve the round's
+// batches, written in input order.  One database keeps the -x rule (one sketch per taxon; batches need not hold whole
+// work units); several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b`
+// without -x.  stage_streamed runs once per process: the ranges, the taxids of every record and the pinned registration
+// of the mapped files.  classify_streamed runs once per sample: its rounds of reads, each through every range.
 struct Streamed {
   struct Plan {
     const uint8_t *rec0;
@@ -2183,112 +2183,9 @@ static void stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const ve
   if (Timing) fprintf(stderr, "[timing] streamed: %zu database(s), %llu MiB per round\n", n_db, (unsigned long long)(round_bytes >> 20));
 }
 
-static void classify_streamed_gpus(Streamed &sm, const vector<pair<const char *, const char *>> &files);
-
-static void classify_streamed(Streamed &sm, const vector<pair<const char *, const char *>> &files) {
-  if (sm.ctxs.size() > 1) return classify_streamed_gpus(sm, files);
-  kuq_ctx *ctx = sm.ctxs[0];
-  const size_t n_db = sm.plans.size();
-  const bool unit_rule = sm.unit_rule;
-  const uint64_t round_bytes = sm.round_bytes;
-  BatchReader input(files, batch_limits(sm.batch_nt, unit_rule, false));
-  struct DevBatch { void *bases, *offs, *codes, *units; };
-  vector<Batch> round;
-  Batch pending;
-  bool have_pending = false;
-  size_t n_rounds = 0;
-  for (;;) {
-    round.clear();
-    uint64_t bytes = 0;
-    for (;;) {
-      if (!have_pending) have_pending = input.next(pending);
-      if (!have_pending) break;
-      const uint64_t need = (pending.bases.size() + 64) * 5 + (pending.reads.size() + 4) * (unit_rule ? 12 : 8) + 1024;
-      if (!round.empty() && bytes + need > round_bytes) break;
-      bytes += need;
-      round.push_back(std::move(pending));
-      have_pending = false;
-    }
-    if (round.empty()) break;
-    n_rounds++;
-    vector<DevBatch> dev(round.size());
-    for (size_t bi = 0; bi < round.size(); bi++) {
-      Batch &b = round[bi];
-      DevBatch &d = dev[bi];
-      d.bases = kuq_device_alloc(ctx, b.bases.size() + 64);
-      d.offs = kuq_device_alloc(ctx, (b.reads.size() + 4) * 8);
-      d.codes = kuq_device_alloc(ctx, (b.bases.size() + 64) * 4);
-      d.units = unit_rule ? kuq_device_alloc(ctx, (b.reads.size() + 4) * 4) : NULL;
-      if (!d.bases || !d.offs || !d.codes || (unit_rule && !d.units)) die(EX_OSERR, "device allocation for the read batches failed");
-      vector<uint64_t> offs(b.offs);
-      offs.push_back(offs.back()); offs.push_back(offs.back());
-      if (kuq_device_memset(ctx, 0, (char *)d.bases + b.bases.size(), 'N', 64) ||
-          kuq_copy_to_device(ctx, 0, d.bases, b.bases.data(), b.bases.size()) ||
-          kuq_copy_to_device(ctx, 0, d.offs, offs.data(), offs.size() * 8) ||
-          kuq_device_memset(ctx, 0, d.codes, 0, (b.bases.size() + 64) * 4))
-        die(EX_SOFTWARE, kuq_last_error(ctx));
-      if (unit_rule && kuq_copy_to_device(ctx, 0, d.units, b.units.data(), b.units.size() * 4)) die(EX_SOFTWARE, kuq_last_error(ctx));
-      if (kuq_sync_slot(ctx, 0)) die(EX_SOFTWARE, kuq_last_error(ctx));
-    }
-    for (size_t db = 0; db < n_db; db++) {
-      const Streamed::Plan &pl = sm.plans[db];
-      if (pl.ranges.empty()) continue;                             // a database without records answers nothing
-      if (pl.nt != sm.open_nt[0] || pl.idx_type != sm.open_type[0]) {
-        // taxonomy and universe are known before the stream opens (the dense numbering is fixed there)
-        if ((sm.open_nt[0] && kuq_stream_check(ctx)) || kuq_stream_open(ctx, pl.k, pl.nt, pl.idx_type, sm.max_rec, sm.max_bins))
-          die(EX_DATAERR, kuq_last_error(ctx));
-        sm.open_nt[0] = pl.nt;
-        sm.open_type[0] = pl.idx_type;
-      }
-      auto load = [&](uint32_t buf, size_t c) {
-        const uint64_t lo = pl.ranges[c].first, hi = pl.ranges[c].second;
-        if (kuq_stream_load(ctx, buf, pl.rec0 + pl.offsets[lo] * pl.pair_sz, pl.offsets[hi] - pl.offsets[lo], pl.offsets + lo, lo, hi))
-          die(EX_DATAERR, kuq_last_error(ctx));
-      };
-      load(0, 0);
-      for (size_t c = 0; c < pl.ranges.size(); c++) {
-        if (kuq_stream_use(ctx, (uint32_t)(c & 1))) die(EX_SOFTWARE, kuq_last_error(ctx));
-        if (c + 1 < pl.ranges.size()) load((uint32_t)((c + 1) & 1), c + 1);
-        uint64_t seqs = 0;
-        for (size_t bi = 0; bi < round.size(); bi++) {
-          Batch &b = round[bi];
-          if (kuq_lookup_device(ctx, (uint32_t)(bi & 1), (const char *)dev[bi].bases, (const uint64_t *)dev[bi].offs,
-                                (uint32_t)b.reads.size(), b.bases.size(), (uint32_t *)dev[bi].codes, db == 0 ? 1 : KUQ_LOOKUP_FILL_EMPTY))
-            die(EX_SOFTWARE, kuq_last_error(ctx));
-          seqs += b.reads.size();
-        }
-        if (n_db == 1) fprintf(stderr, "\r Processed %llu sequences (database chunk %zu of %zu)\n", (unsigned long long)seqs, c + 1, pl.ranges.size());
-        else fprintf(stderr, "\r Processed %llu sequences (database %zu of %zu, chunk %zu of %zu)", (unsigned long long)seqs, db + 1, n_db,
-                     c + 1, pl.ranges.size());
-      }
-    }
-    if (kuq_sync_slot(ctx, 0) || kuq_sync_slot(ctx, 1) || kuq_stream_check(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
-    for (size_t bi = 0; bi < round.size(); bi++) {                 // final pass (classify.cpp:663-791)
-      Batch &b = round[bi];
-      kuq_batch_result res;
-      if (kuq_resolve_device(ctx, 0, (const char *)dev[bi].bases, (const uint64_t *)dev[bi].offs, (uint32_t)b.reads.size(),
-                             b.bases.size(), (const uint32_t *)dev[bi].codes, (const uint32_t *)dev[bi].units, 0) ||
-          kuq_collect_device_batch(ctx, 0, &res))
-        die(EX_SOFTWARE, kuq_last_error(ctx));
-      write_reads(b, res, 0, b.reads.size());
-      book_batch(b.reads.size(), b.bases.size(), res.n_classified);
-    }
-    for (auto &d : dev) {
-      kuq_device_free(ctx, d.bases); kuq_device_free(ctx, d.offs); kuq_device_free(ctx, d.codes);
-      if (d.units) kuq_device_free(ctx, d.units);
-    }
-  }
-  if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));
-  if (n_db > 1) {
-    string per;
-    for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(sm.plans[d].ranges.size());
-    fprintf(stderr, "\nclassify: %zu databases streamed: %zu rounds, ranges per database %s\n", n_db, n_rounds, per.c_str());
-  }
-}
-
-// The rounds of classify_streamed on G GPUs, each streaming its group of every database's ranges over its own link:
+// The rounds on G >= 1 GPUs, each streaming its group of every database's ranges over its own link:
 //   1. every GPU receives every batch of the round; each batch has one owner (contiguous blocks balanced by bases,
-//      round_peak_bytes), which alone holds the batch's id buffer and zeroes it;
+//      round_peak_bytes; with one GPU, GPU 0 owns every batch), which alone holds the batch's id buffer and zeroes it;
 //   2. host barrier;
 //   3. database by database, in command-line order, one host thread per GPU streams the GPU's group of the database's
 //      ranges through its two range buffers and looks every batch up into the owner's id buffer (a peer pointer when the
@@ -2299,8 +2196,9 @@ static void classify_streamed(Streamed &sm, const vector<pair<const char *, cons
 // a plain load, which sees the words other GPUs stored over the peer link only because a host barrier and a kernel
 // boundary separate the two databases' lookups.  The sharded layout orders its phases with device flags and no host
 // barrier, and reads the word with a system-scope load (load_relaxed_sys).  Do not drop this barrier without switching
-// to that load.
-static void classify_streamed_gpus(Streamed &sm, const vector<pair<const char *, const char *>> &files) {
+// to that load.  With one GPU it costs a host sync per database and round but no overlap: kuq_stream_load makes the
+// next database's first copy wait on the device for every lookup queued before it anyway.
+static void classify_streamed(Streamed &sm, const vector<pair<const char *, const char *>> &files) {
   const vector<kuq_ctx *> &ctxs = sm.ctxs;
   const int G = (int)ctxs.size();
   const size_t n_db = sm.plans.size();
@@ -2808,7 +2706,8 @@ int main(int argc, char **argv) {
   uint64_t chunk_budget = 0;
   // The databases (one, or several together) larger than one card: sharded over the visible GPUs when they hold them
   // together (run_sharded / run_sharded_multi), else streamed through the GPUs in ranges of at most 40 GB (two range
-  // buffers + a round of reads have to fit, run_streamed).  Several databases that fit the budget together are resident.
+  // buffers + a round of reads have to fit, classify_streamed).  Several databases that fit the budget together are
+  // resident.
   bool want_shards = false;
   uint64_t all_hbm = 0;
   for (size_t i = 0; i < n_db; i++) all_hbm += hbm_bytes(kdbs[i], idxs[i]);
@@ -2823,7 +2722,8 @@ int main(int argc, char **argv) {
   kuq_config cfg;
   kuq_config_default(&cfg);
   cfg.n_slots = 3;                             // classify b + 1 on the GPU, format b, gather b + 2 (process_file_parallel)
-  if (want_shards) cfg.n_slots = 2;            // shards use slot 0, and slots 0 and 1 if they fall back to streaming
+  // shards use slot 0; streamed runs (shards that fall back to streaming too) use slots 0 and 1
+  if (want_shards || chunk_budget) cfg.n_slots = 2;
   cfg.max_bases_per_batch = 288ull << 20;      // one read may be a whole chromosome (the largest human one is 248 Mbp)
   cfg.work_unit_size = Work_unit_size;
   // -x (or a database that has to be split) → one global sketch per taxon (classify.cpp:719); else per work unit, which
@@ -2854,7 +2754,6 @@ int main(int argc, char **argv) {
     if (devices.empty()) devices.assign(1, cfg.device);
     cfg.device = devices[0];
   }
-  if (chunk_budget && devices.size() > 1) cfg.n_slots = 2;     // streamed over several GPUs: slots 0 and 1, as shards
   kuq_ctx *ctx = NULL;
   int rc = kuq_create(&cfg, &ctx);
   if (rc) die(EX_UNAVAILABLE, string("libkuq: ") + kuq_strerror(rc));
