@@ -1382,6 +1382,57 @@ static int db_taxids(kuq_ctx *ctx, map<uint32_t, uint64_t> &into) {
   return rc;
 }
 
+// A piece of database `db` staged on a context: bins [bin_lo, bin_hi); (0, 0) is the whole database, lo == hi != 0 an
+// empty slice
+struct Slice { size_t db; uint64_t bin_lo, bin_hi; };
+
+// Context g stages slices[g] in order, one thread per context.  join: each slice joins what the context holds
+// (kuq_stage_db_append_range); else each replaces the last (kuq_stage_db), for a group of ranges that does not fit at
+// once.  db_counts[d] (the .counts files) gets the records per taxid that database d's slices add: the context's
+// db_taxids after a slice minus those before it (none before it when slices replace).  replicas: every context stages
+// the same slices, so context 0 alone counts.
+static void stage_slices(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs,
+                         const vector<vector<Slice>> &slices, bool join, bool replicas, vector<map<uint32_t, uint64_t>> &db_counts) {
+  const int G = (int)ctxs.size();
+  vector<vector<map<uint32_t, uint64_t>>> added(G, vector<map<uint32_t, uint64_t>>(db_counts.size()));
+  vector<int> rcs(G, 0);
+#pragma omp parallel for num_threads(G) schedule(static, 1)
+  for (int g = 0; g < G; g++) {
+    map<uint32_t, uint64_t> before, after;
+    for (size_t i = 0; i < slices[g].size() && !rcs[g]; i++) {
+      const Slice &s = slices[g][i];
+      const Mapped &kdb = kdbs[s.db], &idx = idxs[s.db];
+      rcs[g] = join ? kuq_stage_db_append_range(ctxs[g], kdb.p, kdb.size, idx.p, idx.size, s.bin_lo, s.bin_hi)
+                    : kuq_stage_db(ctxs[g], kdb.p, kdb.size, idx.p, idx.size, s.bin_lo, s.bin_hi);
+      if (rcs[g] || (replicas && g)) continue;
+      after.clear();
+      if ((rcs[g] = db_taxids(ctxs[g], after))) continue;
+      for (auto &kv : after) {
+        const auto b = before.find(kv.first);
+        const uint64_t was = b == before.end() ? 0 : b->second;
+        if (kv.second > was) added[g][s.db][kv.first] += kv.second - was;
+      }
+      if (join) before.swap(after);
+    }
+  }
+  for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
+  for (int g = 0; g < G; g++)
+    for (size_t d = 0; d < db_counts.size(); d++)
+      for (auto &kv : added[g][d]) db_counts[d][kv.first] += kv.second;
+}
+
+// Contexts that each hold a part of the databases (shards, streamed groups): every one numbers the taxids of every
+// database and range (kuq_set_db_taxid_universe), and may store into the others' id buffers (peer access)
+static void share_taxa(const vector<kuq_ctx *> &ctxs, const vector<map<uint32_t, uint64_t>> &db_counts) {
+  set<uint32_t> all;
+  for (auto &c : db_counts) for (auto &kv : c) all.insert(kv.first);
+  const vector<uint32_t> u(all.begin(), all.end());
+  for (kuq_ctx *c : ctxs)
+    if (kuq_set_db_taxid_universe(c, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(c));
+  for (kuq_ctx *c : ctxs)
+    for (kuq_ctx *p : ctxs) if (p != c && kuq_enable_peer_access(c, p)) die(EX_SOFTWARE, kuq_last_error(c));
+}
+
 // background writer: formatted text is handed over batch by batch and written in order while the next batch is
 // being gathered / classified / formatted
 struct OutJob { vector<string> kraken, classified, unclassified, extract; vector<ScriptPart> script; bool extract_selected = false; };
@@ -2056,7 +2107,8 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 // batches, written in input order.  One database keeps the -x rule (one sketch per taxon; batches need not hold whole
 // work units); several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b`
 // without -x.  stage_streamed runs once per process: the ranges, the taxids of every record and the pinned registration
-// of the mapped files.  classify_streamed runs once per sample: its rounds of reads, each through every range.
+// of the mapped files; it returns the first context that staged a range (a GPU's group may be empty).
+// classify_streamed runs once per sample: its rounds of reads, each through every range.
 struct Streamed {
   struct Plan {
     const uint8_t *rec0;
@@ -2074,9 +2126,9 @@ struct Streamed {
   vector<uint32_t> open_nt, open_type;                             // per context: what its range buffers are open for
 };
 
-static void stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vector<int> &ctx_devices, const vector<Mapped> &kdbs,
-                           const vector<Mapped> &idxs, uint64_t range_budget, uint64_t hbm_budget,
-                           vector<map<uint32_t, uint64_t>> &db_counts) {
+static int stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vector<int> &ctx_devices, const vector<Mapped> &kdbs,
+                          const vector<Mapped> &idxs, uint64_t range_budget, uint64_t hbm_budget,
+                          vector<map<uint32_t, uint64_t>> &db_counts) {
   const size_t n_db = kdbs.size();
   const int G = (int)ctxs.size();
   const bool unit_rule = sm.unit_rule = n_db > 1;
@@ -2106,22 +2158,12 @@ static void stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const ve
   }
   // pass 0: the taxids of all records, so that every range numbers taxa identically (also database.kdb.counts); every
   // GPU reads those of its own group
-  {
-    vector<vector<map<uint32_t, uint64_t>>> found(G, vector<map<uint32_t, uint64_t>>(n_db));
-    vector<int> rcs(G, 0);
-#pragma omp parallel for num_threads(G) schedule(static, 1)
-    for (int g = 0; g < G; g++)
-      for (size_t d = 0; d < n_db; d++)
-        for (size_t c = plans[d].group[g]; c < plans[d].group[g + 1] && !rcs[g]; c++) {
-          const auto &rg = plans[d].ranges[c];
-          rcs[g] = kuq_stage_db(ctxs[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, rg.first, rg.second);
-          if (!rcs[g]) rcs[g] = db_taxids(ctxs[g], found[g][d]);
-        }
-    for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
-    for (int g = 0; g < G; g++)
-      for (size_t d = 0; d < n_db; d++)
-        for (auto &kv : found[g][d]) db_counts[d][kv.first] += kv.second;
-  }
+  vector<vector<Slice>> slices(G);
+  for (int g = 0; g < G; g++)
+    for (size_t d = 0; d < n_db; d++)
+      for (size_t c = plans[d].group[g]; c < plans[d].group[g + 1]; c++)
+        slices[g].push_back(Slice{d, plans[d].ranges[c].first, plans[d].ranges[c].second});
+  stage_slices(ctxs, kdbs, idxs, slices, false, false, db_counts);
   if (n_db == 1) cerr << "Database split into " << plans[0].ranges.size() << " chunks" << endl;
   if (G > 1) {
     string per;
@@ -2132,25 +2174,10 @@ static void stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const ve
     fprintf(stderr, "classify: %s streamed over %d GPUs: ranges per GPU %s\n",
             n_db == 1 ? "database" : (std::to_string(n_db) + " databases").c_str(), G, per.c_str());
   }
-  {
-    set<uint32_t> all;
-    for (auto &c : db_counts) for (auto &kv : c) all.insert(kv.first);
-    vector<uint32_t> u(all.begin(), all.end());
-    for (kuq_ctx *c : ctxs)
-      if (kuq_set_db_taxid_universe(c, u.data(), (uint32_t)u.size())) die(EX_SOFTWARE, kuq_last_error(c));
-  }
-  for (int g = 0; g < G; g++)
-    for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-  if (unit_rule) {
+  share_taxa(ctxs, db_counts);
+  if (unit_rule)
     for (kuq_ctx *c : ctxs)
       if (kuq_mark_zero_hits(c, 1)) die(EX_SOFTWARE, kuq_last_error(c));
-    int g0 = 0;                                                    // a context that staged a range (a group may be empty)
-    while (g0 + 1 < G && std::all_of(plans.begin(), plans.end(), [&](const Streamed::Plan &pl) { return pl.group[g0] == pl.group[g0 + 1]; }))
-      g0++;
-    uint32_t rows = 0;
-    if (kuq_unit_table_rows(ctxs[g0], &rows)) die(EX_SOFTWARE, kuq_last_error(ctxs[g0]));
-    if (rows) Max_units_per_batch = rows;
-  }
   // device memory of a round: the budget (and what the card has free, shared among its contexts) minus the two range
   // buffers, on the tightest context (stream_round_bytes)
   const uint64_t range_bytes = 2 * (max_rec * 12 + (max_bins + 1) * 8 + 4096);     // 12 B per record in HBM
@@ -2181,6 +2208,9 @@ static void stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const ve
         }
   }
   if (Timing) fprintf(stderr, "[timing] streamed: %zu database(s), %llu MiB per round\n", n_db, (unsigned long long)(round_bytes >> 20));
+  int g0 = 0;
+  while (g0 + 1 < G && slices[g0].empty()) g0++;
+  return g0;
 }
 
 // The rounds on G >= 1 GPUs, each streaming its group of every database's ranges over its own link:
@@ -2359,9 +2389,9 @@ static void classify_streamed(Streamed &sm, const vector<pair<const char *, cons
 // k-mers whose minimizer it holds; each hit is stored straight into the id buffer of the GPU that resolves the read (peer
 // stores over NVLink); device flags order the phases (no host barrier between GPUs); every GPU resolves a contiguous
 // share of the batch.  One process, so peer access instead of CUDA IPC.
-//   One database (run_sharded): one lookup phase, and the GPU that finds a hit also does its sketch work; the sketches
-//   follow the chunked rule, as for any database the reference could only run with -x.
-//   Several databases (run_sharded_multi): one lookup phase per run of databases with equal (nt, index type); a later
+//   One database: one lookup phase, and the GPU that finds a hit also does its sketch work; the sketches follow the
+//   chunked rule, as for any database the reference could only run with -x.
+//   Several databases: one lookup phase per run of databases with equal (nt, index type); a later
 //   phase fills only the windows no earlier phase answered on any GPU.  The owners do all the sketch work in the resolve
 //   half, with the work-unit ids of the per-work-unit rule (the reference's rule for -d a -d b), so shares hold whole
 //   work units.
@@ -2485,71 +2515,38 @@ static ShardDb shard_db(const Mapped &idx) {
   return ShardDb{(const uint64_t *)(q + 8), q[7], memcmp(q, "KRAKIDX", 7) == 0 ? 1u : 2u};
 }
 
-// Staging, once per process; every sample then runs shard_loop with one phase (one database) or one per lookup run
-static void stage_sharded(const vector<kuq_ctx *> &ctxs, const Mapped &kdb, const Mapped &idx, map<uint32_t, uint64_t> &db_counts) {
-  const int G = (int)ctxs.size();
-  const vector<uint64_t> cut = plan_shards({shard_db(idx)}, G)[0].cut;
-  cerr << "Database sharded over " << G << " GPUs by minimizer range" << endl;
-  {
-    vector<int> rcs(G, 0);
-#pragma omp parallel for num_threads(G) schedule(static, 1)
-    for (int g = 0; g < G; g++)
-      rcs[g] = cut[g + 1] > cut[g] ? kuq_stage_db(ctxs[g], kdb.p, kdb.size, idx.p, idx.size, cut[g], cut[g + 1]) : 0;
-    for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
-  }
-  for (int g = 0; g < G; g++) {
-    if (cut[g + 1] <= cut[g]) die(EX_DATAERR, "more GPUs than non-empty minimizer ranges: use fewer devices (KUQ_DEVICES)");
-    if (db_taxids(ctxs[g], db_counts)) die(EX_DATAERR, kuq_last_error(ctxs[g]));
-  }
-  vector<uint32_t> all;
-  for (auto &kv : db_counts) all.push_back(kv.first);
-  for (int g = 0; g < G; g++) {
-    if (kuq_set_db_taxid_universe(ctxs[g], all.data(), (uint32_t)all.size()) || kuq_set_shard_counting(ctxs[g], 1))
-      die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-  }
-}
-
-// Several databases: every GPU stages, in command-line order, the bins of its range of each database's run (a range may
-// be empty); each database's records per taxid (.counts) are the growth of the staged union it causes, summed over GPUs.
-static uint32_t stage_sharded_multi(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs,
-                                    vector<map<uint32_t, uint64_t>> &db_counts) {
+// Staging, once per process: every GPU stages, in command-line order, the bins of its range of each database's run (a
+// range of several databases may be empty).  One database is one run, with a non-empty range on every GPU, and the GPU
+// that finds a hit counts it (kuq_set_shard_counting).  Returns the runs: shard_loop's lookup phases.
+static uint32_t stage_shards(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs,
+                             vector<map<uint32_t, uint64_t>> &db_counts) {
   const int G = (int)ctxs.size();
   const size_t n_db = kdbs.size();
   vector<ShardDb> sd;
   for (auto &m : idxs) sd.push_back(shard_db(m));
   const vector<ShardRun> runs = plan_shards(sd, G);
-  fprintf(stderr, "classify: %zu databases sharded over %d GPUs by minimizer range (%zu lookup phases)\n", n_db, G, runs.size());
-  vector<vector<map<uint32_t, uint64_t>>> after(G, vector<map<uint32_t, uint64_t>>(n_db));
-  vector<int> rcs(G, 0);
-#pragma omp parallel for num_threads(G) schedule(static, 1)
+  if (n_db == 1) {
+    cerr << "Database sharded over " << G << " GPUs by minimizer range" << endl;
+    for (int g = 0; g < G; g++)
+      if (runs[0].cut[g + 1] <= runs[0].cut[g]) die(EX_DATAERR, "more GPUs than non-empty minimizer ranges: use fewer devices (KUQ_DEVICES)");
+  } else {
+    fprintf(stderr, "classify: %zu databases sharded over %d GPUs by minimizer range (%zu lookup phases)\n", n_db, G, runs.size());
+  }
+  vector<vector<Slice>> slices(G);
   for (int g = 0; g < G; g++)
     for (const ShardRun &run : runs)
-      for (size_t d = run.first; d < run.end && !rcs[g]; d++) {
+      for (size_t d = run.first; d < run.end; d++) {
         uint64_t lo = run.cut[g], hi = run.cut[g + 1];
         if (lo == hi) lo = hi = 1ull << (2 * sd[d].nt);             // an empty slice
-        rcs[g] = kuq_stage_db_append_range(ctxs[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size, lo, hi);
-        if (!rcs[g]) rcs[g] = db_taxids(ctxs[g], after[g][d]);
+        slices[g].push_back(Slice{d, lo, hi});
       }
-  for (int g = 0; g < G; g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(ctxs[g]));
-  set<uint32_t> all;
-  for (int g = 0; g < G; g++)
-    for (size_t d = 0; d < n_db; d++)
-      for (auto &kv : after[g][d]) {
-        const uint64_t before = d && after[g][d - 1].count(kv.first) ? after[g][d - 1][kv.first] : 0;
-        if (kv.second > before) { db_counts[d][kv.first] += kv.second - before; all.insert(kv.first); }
-      }
-  vector<uint32_t> u(all.begin(), all.end());
+  stage_slices(ctxs, kdbs, idxs, slices, true, false, db_counts);
   for (int g = 0; g < G; g++) {
     uint32_t n_runs = 0;
-    if (kuq_db_runs(ctxs[g], &n_runs) || kuq_set_db_taxid_universe(ctxs[g], u.data(), (uint32_t)u.size()))
-      die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    if (n_runs != runs.size()) die(EX_SOFTWARE, "the library groups the databases into other lookup runs than the planner");
-    for (int h = 0; h < G; h++) if (h != g && kuq_enable_peer_access(ctxs[g], ctxs[h])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    if (n_db == 1 ? kuq_set_shard_counting(ctxs[g], 1) : kuq_db_runs(ctxs[g], &n_runs)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+    if (n_db > 1 && n_runs != runs.size()) die(EX_SOFTWARE, "the library groups the databases into other lookup runs than the planner");
   }
-  uint32_t rows = 0;
-  if (kuq_unit_table_rows(ctxs[0], &rows)) die(EX_SOFTWARE, kuq_last_error(ctxs[0]));
-  if (rows) Max_units_per_batch = rows;
+  share_taxa(ctxs, db_counts);
   return (uint32_t)runs.size();
 }
 
@@ -2684,11 +2681,10 @@ int main(int argc, char **argv) {
     kdbs[i].open(DB_filenames[i]);
     idxs[i].open(Index_filenames[i]);
   }
-  Mapped &kdb = kdbs[0], &idx = idxs[0];
   for (size_t i = 1; i < n_db; i++) {                               // classify.cpp:203-210
     auto k_of = [](const Mapped &m) { return m.size >= 16 ? (int)(((const uint64_t *)m.p)[1] / 2) : 0; };
-    if (k_of(kdbs[i]) != k_of(kdb)) {
-      fprintf(stderr, "Different k-mer sizes in databases 1 and %zu: %i vs %i!\n", i + 1, k_of(kdb), k_of(kdbs[i]));
+    if (k_of(kdbs[i]) != k_of(kdbs[0])) {
+      fprintf(stderr, "Different k-mer sizes in databases 1 and %zu: %i vs %i!\n", i + 1, k_of(kdbs[0]), k_of(kdbs[i]));
       exit(1);
     }
   }
@@ -2705,7 +2701,7 @@ int main(int argc, char **argv) {
   if (getenv("KUQ_HBM_BUDGET")) hbm_budget = strtoull(getenv("KUQ_HBM_BUDGET"), NULL, 10);
   uint64_t chunk_budget = 0;
   // The databases (one, or several together) larger than one card: sharded over the visible GPUs when they hold them
-  // together (run_sharded / run_sharded_multi), else streamed through the GPUs in ranges of at most 40 GB (two range
+  // together (stage_shards, shard_loop), else streamed through the GPUs in ranges of at most 40 GB (two range
   // buffers + a round of reads have to fit, classify_streamed).  Several databases that fit the budget together are
   // resident.
   bool want_shards = false;
@@ -2776,7 +2772,7 @@ int main(int argc, char **argv) {
   // -q: the preloaded path leaves a read at its -m'th hit; with -x every k-mer is counted (classify.cpp:943-944 / :701-738)
   for (kuq_ctx *c : All_ctx)
     if (Quick_mode && kuq_set_quick_mode(c, Minimum_hit_count, Populate_memory_size == 0)) die(EX_SOFTWARE, kuq_last_error(c));
-  // records per taxid of each database (the .counts files), when the run stages databases in pieces or several of them
+  // records per taxid of each database (the .counts files)
   vector<map<uint32_t, uint64_t>> db_counts(n_db);
   if (!chunk_budget && !want_shards) {
     double T0__ = now_s();
@@ -2787,24 +2783,10 @@ int main(int argc, char **argv) {
       for (auto &s : tmp) prepare_stage(s, 150ull << 20, 1u << 20);
       Prealloc_stages.swap(tmp);
     });
-    // every device stages the databases, in command-line order, from the same mapped files, in parallel; the first one
-    // reads each database's taxids as the difference of the staged union before and after it
-    vector<int> rcs(All_ctx.size(), 0);
-    vector<map<uint32_t, uint64_t>> union_after(n_db);
-#pragma omp parallel for num_threads((int)All_ctx.size()) schedule(static, 1)
-    for (int g = 0; g < (int)All_ctx.size(); g++) {
-      for (size_t d = 0; d < n_db && !rcs[g]; d++) {
-        rcs[g] = d ? kuq_stage_db_append(All_ctx[g], kdbs[d].p, kdbs[d].size, idxs[d].p, idxs[d].size)
-                   : kuq_stage_db(All_ctx[g], kdb.p, kdb.size, idx.p, idx.size, 0, 0);
-        if (g == 0 && !rcs[g] && n_db > 1) rcs[g] = db_taxids(All_ctx[g], union_after[d]);
-      }
-    }
-    for (size_t g = 0; g < All_ctx.size(); g++) if (rcs[g]) die(EX_DATAERR, kuq_last_error(All_ctx[g]));
-    for (size_t d = 0; d < n_db && n_db > 1; d++)
-      for (auto &kv : union_after[d]) {
-        const uint64_t before = d && union_after[d - 1].count(kv.first) ? union_after[d - 1][kv.first] : 0;
-        if (kv.second > before) db_counts[d][kv.first] = kv.second - before;
-      }
+    // every device stages every database whole, in command-line order, from the same mapped files
+    vector<Slice> whole;
+    for (size_t d = 0; d < n_db; d++) whole.push_back(Slice{d, 0, 0});
+    stage_slices(All_ctx, kdbs, idxs, vector<vector<Slice>>(All_ctx.size(), whole), true, true, db_counts);
     prealloc.join();
     TICK("stage_db");
   }
@@ -2826,17 +2808,19 @@ int main(int argc, char **argv) {
                                      tax.row_parents.data(), (uint32_t)tax.row_ids.size()))
         die(EX_DATAERR, kuq_last_error(c));
   }
-  if (cfg.hll_mode == KUQ_HLL_PRELOAD && !chunk_budget && !want_shards) {   // (streamed / sharded runs ask once their taxa are known)
-    uint32_t rows = 0;
-    if (kuq_unit_table_rows(ctx, &rows)) die(EX_SOFTWARE, kuq_last_error(ctx));
-    if (rows) Max_units_per_batch = rows;
-  }
   // staging of the layouts that stage in pieces (the resident layouts staged above)
   Streamed streamed;
-  uint32_t shard_phases = 0;
-  if (want_shards && n_db == 1) stage_sharded(All_ctx, kdb, idx, db_counts[0]);
-  else if (want_shards) shard_phases = stage_sharded_multi(All_ctx, kdbs, idxs, db_counts);
-  else if (chunk_budget) stage_streamed(streamed, All_ctx, ctx_devices, kdbs, idxs, chunk_budget, hbm_budget, db_counts);
+  uint32_t shard_runs = 0;
+  int g0 = 0;                                                       // the first context that staged a slice
+  if (want_shards) shard_runs = stage_shards(All_ctx, kdbs, idxs, db_counts);
+  else if (chunk_budget) g0 = stage_streamed(streamed, All_ctx, ctx_devices, kdbs, idxs, chunk_budget, hbm_budget, db_counts);
+  // the per-work-unit rule (resident without -x, and several databases in every layout); kuq_unit_table_rows finalizes
+  // the context, so it comes after the taxonomy and the taxid universe
+  if (want_shards || chunk_budget ? n_db > 1 : cfg.hll_mode == KUQ_HLL_PRELOAD) {
+    uint32_t rows = 0;
+    if (kuq_unit_table_rows(All_ctx[g0], &rows)) die(EX_SOFTWARE, kuq_last_error(All_ctx[g0]));
+    if (rows) Max_units_per_batch = rows;
+  }
 #ifdef EXACT_COUNTING
   // classifyExact on several contexts: the counters join the first context, and the exact k-mer sets are spread over
   // all contexts by k-mer instead of united on one card, so no card has to hold the union.  The report's clades come
@@ -2891,7 +2875,7 @@ int main(int argc, char **argv) {
     struct timeval tv1, tv2;
     gettimeofday(&tv1, NULL);
     const vector<pair<const char *, const char *>> files = files_of(sample);
-    if (want_shards) shard_loop(All_ctx, n_db == 1 ? 1 : shard_phases, n_db > 1, files);
+    if (want_shards) shard_loop(All_ctx, shard_runs, n_db > 1, files);
     else if (chunk_budget) classify_streamed(streamed, files);
     else for (auto &in : files) process_file(ctx, in.first, in.second);
     // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
@@ -2944,7 +2928,6 @@ int main(int argc, char **argv) {
         if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
           cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
           ofstream ofs(fname);
-          if (n_db == 1 && !chunk_budget && !want_shards && db_taxids(ctx, db_counts[0])) die(EX_SOFTWARE, kuq_last_error(ctx));
           for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
         }
         {

@@ -57,7 +57,7 @@ def test_cli_matches_reference_outputs(tmp_path, tag, extra, reads):
                                            ("chunked", ["-M"], {"KUQ_FORCE_SHARDS": "1"})])
 def test_cli_one_device_as_several_gpus(tmp_path, tag, extra, env):
     """one device listed twice: the multi-GPU paths of one process, with a context per listed device — replicas
-    (batches round-robin, kuq_merge_into at the end) and minimizer-range shards (run_sharded: peer stores, device
+    (batches round-robin, kuq_merge_into at the end) and minimizer-range shards (shard_loop: peer stores, device
     flags between the contexts, kuq_merge_into over shard contexts; sketches follow the -x rule).  Each context of
     the executable reserves about 33 GB of batch slots (3 slots of 288 MiB bases), so an 80 GB card holds two."""
     # small batches so that every context gets work; a small sparse set so that it has to grow
@@ -147,11 +147,12 @@ def test_cli_flags(tmp_path):
     assert r.returncode != 0 and "not supported" in r.stderr
 
 
-@pytest.mark.parametrize("size", ["40K", "16K", "100K"])
+@pytest.mark.parametrize("size", ["40K", "16K", "100K", pytest.param(None, id="shards")])
 def test_cli_database_ranges(tmp_path, size):
     """-x with a database that must be split (process_file_with_db_chunk, classify.cpp:566-791): the database is
     staged range by range, every range looks the whole input up, the merged taxa are resolved in a final pass.
-    Same Kraken output and report as the reference's `-x 40K` run, whatever the chunk size."""
+    Same Kraken output and report as the reference's `-x 40K` run, whatever the chunk size.  `shards`: the database
+    sharded by minimizer range over two contexts on one device instead, whose ranges add up to the same .counts."""
     import shutil
     db = tmp_path / "db"
     db.mkdir()
@@ -160,11 +161,15 @@ def test_cli_database_ranges(tmp_path, size):
     exe = build.build_classify()
     out, rep = tmp_path / "o.kraken", tmp_path / "o.report.tsv"
     cmd = [exe, "-d", str(db / "database.kdb"), "-i", str(db / "database.idx"), "-a", str(db / "taxDB"), "-t", "1",
-           "-r", str(rep), "-o", str(out), "-x", size, os.path.join(G, "reads.fa")]
-    env = dict(os.environ, KUQ_SPARSE_SLOTS=str(1 << 22), KUQ_FORCE_CHUNKS="1")
+           "-r", str(rep), "-o", str(out)] + (["-x", size] if size else ["-M"]) + [os.path.join(G, "reads.fa")]
+    env = dict(os.environ, KUQ_SPARSE_SLOTS=str(1 << 22),
+               **({"KUQ_FORCE_CHUNKS": "1"} if size else {"KUQ_FORCE_SHARDS": "1", "KUQ_DEVICES": "0,0"}))
     r = subprocess.run(cmd, capture_output=True, text=True, env=env)
     assert r.returncode == 0, r.stderr[-2000:]
-    assert "Database split into" in r.stderr and "split into 1 chunks" not in r.stderr
+    if size:
+        assert "Database split into" in r.stderr and "split into 1 chunks" not in r.stderr
+    else:
+        assert "Database sharded over 2 GPUs by minimizer range" in r.stderr
     assert open(out).read() == open(os.path.join(G, "chunked.kraken")).read()
     assert _report_lines(rep) == _report_lines(os.path.join(G, "chunked.report.tsv"))
     assert open(db / "database.kdb.counts").read() == open(os.path.join(G, "database.kdb.counts")).read()

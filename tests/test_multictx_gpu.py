@@ -386,8 +386,8 @@ def test_shards_merge_to_the_single_context_state(world, workload, idle, variant
 
 
 def _flag_steps(ctxs, ref, d_bases, d_offs, d_units, idle, sub, n_steps=3):
-    """(c) bench.py's and run_sharded's protocol: device flags instead of host barriers, double-buffered id buffers,
-    several steps.  Every context's phase is queued before the host waits for any of them, in run_sharded's order."""
+    """(c) bench.py's and shard_loop's protocol: device flags instead of host barriers, double-buffered id buffers,
+    several steps.  Every context's phase is queued before the host waits for any of them, in shard_loop's order."""
     world = len(ctxs)
     offs, units = ref["offs"], ref["units"]
     n, total = len(offs) - 1, int(offs[-1])
