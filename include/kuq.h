@@ -692,6 +692,36 @@ int kuq_kmer_set_stats(kuq_kmer_set *h, double *stage_ms5, uint64_t *windows, ui
 const char *kuq_kmer_set_last_error(const kuq_kmer_set *h);
 void kuq_kmer_set_destroy(kuq_kmer_set *h);
 
+/* Distinct k-mers of a FASTA library by HyperLogLog: count_unique (src/count_unique.cpp:51-79), which
+ * krakenuniq-build runs when --jellyfish-hash-size is not given (scripts/build_db.sh:125-129).  Every sequence is cut
+ * into pieces [i, i + 50000 + k - 1), i = 0, 50000, ...; a fresh KmerScanner (krakenutil.cpp:208-282) runs over each,
+ * and every window whose k bases are ACGTacgt goes into a dense HyperLogLog sketch of 2^p registers as its forward
+ * (not canonical) 2-bit k-mer: hash = murmur3 finalizer, register = top p bits, rank = leading zeros of the rest + 1
+ * (hyperloglogplus.cpp:485-523).  Pieces merge by register max; n_observed counts every valid window of every piece.
+ * Needs no context.
+ *
+ * kuq_count_unique_create: device ordinal, k = 1..31, precision p = 4..18 (KUQ_E_INVALID_ARG otherwise), batch_bases =
+ *   bases per staged batch (0 → 256 Mi), staged through two pinned buffers.  err (optional) receives a message on
+ *   failure; KUQ_E_NO_DEVICE without a GPU (there is no CPU path).
+ * kuq_count_unique_add: sequences r = bases[offsets[r] .. offsets[r + 1]) — what FastaReader::next_sequence
+ *   (seqreader.cpp:34-79) returns, a '\r' of CRLF files included.  The library cuts the pieces; a '\n' / '\r' is left
+ *   out of the k-mers but costs the window KmerScanner then skips, and near a piece's end the scanner may read into the
+ *   next piece, which can count a window twice in n_observed (sequences holding them take a slower host path).  Copies
+ *   the bases; asynchronous on the device.  May be called again after kuq_count_unique_result.
+ * kuq_count_unique_result: *estimate = what count_unique prints, ertlCardinality (hyperloglogplus.cpp:722-753) at p:
+ *   n_observed when that is below the estimate, else the rounded estimate, and 0 when no window was valid;
+ *   *n_observed = valid windows; regs_out (optional, 2^p bytes) = the registers.
+ * kuq_count_unique_stats (measurement aid): device time in ms of the sketch kernel so far, valid windows as of the last
+ *   kuq_count_unique_result, and bases staged (line breaks left out). */
+typedef struct kuq_count_unique kuq_count_unique;
+int kuq_count_unique_create(int device, uint32_t k, uint32_t p, uint64_t batch_bases, kuq_count_unique **out, char *err,
+                            uint64_t err_cap);
+int kuq_count_unique_add(kuq_count_unique *h, const char *bases, const uint64_t *offsets, uint32_t n_seqs);
+int kuq_count_unique_result(kuq_count_unique *h, uint64_t *estimate, uint64_t *n_observed, uint8_t *regs_out);
+int kuq_count_unique_stats(kuq_count_unique *h, double *sketch_ms, uint64_t *windows, uint64_t *bases);
+const char *kuq_count_unique_last_error(const kuq_count_unique *h);
+void kuq_count_unique_destroy(kuq_count_unique *h);
+
 #ifdef __cplusplus
 }
 #endif

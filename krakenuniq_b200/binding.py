@@ -214,6 +214,13 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_kmer_set_stats": (C.c_int, [vp, C.POINTER(C.c_double), u64p, u64p, u64p, C.POINTER(C.c_int)]),
         "kuq_kmer_set_last_error": (C.c_char_p, [vp]),
         "kuq_kmer_set_destroy": (None, [vp]),
+        "kuq_count_unique_create": (C.c_int, [C.c_int, C.c_uint32, C.c_uint32, C.c_uint64, C.POINTER(vp), C.c_char_p,
+                                              C.c_uint64]),
+        "kuq_count_unique_add": (C.c_int, [vp, vp, u64p, C.c_uint32]),
+        "kuq_count_unique_result": (C.c_int, [vp, u64p, u64p, vp]),
+        "kuq_count_unique_stats": (C.c_int, [vp, C.POINTER(C.c_double), u64p, u64p]),
+        "kuq_count_unique_last_error": (C.c_char_p, [vp]),
+        "kuq_count_unique_destroy": (None, [vp]),
     }
     for name, (res, args) in sigs.items():
         f = getattr(L, name)            # AttributeError here = the library does not export what kuq.h declares
@@ -892,3 +899,60 @@ def kmer_set(bases: np.ndarray, offsets: np.ndarray, k: int, budget=None, batch=
     finally:
         ks.close()
     return np.concatenate([kdb_header(k, key_ct)] + parts), passes
+
+
+class CountUnique:
+    """kuq_count_unique_*: count_unique's HyperLogLog estimate of a library's distinct forward k-mers on the GPU."""
+
+    def __init__(self, k, p=14, batch=None, device=0):
+        self.L = load_library()
+        self.k, self.p = k, p
+        h, err = C.c_void_p(), C.create_string_buffer(1024)
+        rc = self.L.kuq_count_unique_create(device, k, p, int(batch or 0), C.byref(h), err, 1024)
+        if rc != 0:
+            raise KuqError(rc, err.value.decode() or self.L.kuq_strerror(rc).decode())
+        self.h = h
+
+    def _ck(self, rc):
+        if rc != 0:
+            raise KuqError(rc, f"{self.L.kuq_strerror(rc).decode()}: {self.L.kuq_count_unique_last_error(self.h).decode()}")
+
+    def add(self, bases: np.ndarray, offsets: np.ndarray):
+        bases = np.ascontiguousarray(bases, np.uint8)
+        offsets = np.ascontiguousarray(offsets, np.uint64)
+        buf = bases if bases.size else np.zeros(1, np.uint8)
+        self._ck(self.L.kuq_count_unique_add(self.h, buf.ctypes.data, _p(offsets, u64p), len(offsets) - 1))
+
+    def result(self):
+        """(estimate count_unique prints, valid windows, registers uint8[2^p])"""
+        est, n = C.c_uint64(0), C.c_uint64(0)
+        regs = np.zeros(1 << self.p, np.uint8)
+        self._ck(self.L.kuq_count_unique_result(self.h, C.byref(est), C.byref(n), regs.ctypes.data))
+        return est.value, n.value, regs
+
+    def stats(self):
+        ms, w, b = C.c_double(), C.c_uint64(), C.c_uint64()
+        self._ck(self.L.kuq_count_unique_stats(self.h, C.byref(ms), C.byref(w), C.byref(b)))
+        return {"sketch_ms": ms.value, "windows": w.value, "bases": b.value}
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.kuq_count_unique_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def count_unique(bases: np.ndarray, offsets: np.ndarray, k: int, p: int, batch=None, device=0):
+    """What `count_unique -k k -p p` computes for the sequences bases[offsets[r]:offsets[r+1]] (FastaReader's
+    sequences): (estimate, n_observed, registers uint8[2^p]).  batch = bases per device batch (None: 256 Mi)."""
+    cu = CountUnique(k, p, batch, device)
+    try:
+        cu.add(bases, offsets)
+        return cu.result()
+    finally:
+        cu.close()

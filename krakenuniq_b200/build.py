@@ -11,8 +11,9 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "lib", "libkuq.so")
 SOURCES = ["kuq_kernels.cu", "kuq_api.cu", "kuq_dbbuild.cu", "kuq_microbench.cu", "kuq_layout_exp.cu", "kuq_clades.cu",
-           "kuq_collisions.cu", "kuq_kmerset.cu"]
+           "kuq_collisions.cu", "kuq_kmerset.cu", "kuq_countunique.cu"]
 HEADERS = ["kuq_kernels.cuh", "kuq_buffers.cuh", "kuq_minimizer.cuh", "kuq_bounce.cuh", "kuq_ranges.h", "kuq_batches.h",
+           "kuq_kmerpack.cuh",
            os.path.join(ROOT, "include", "kuq.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--compiler-bindir", "/usr/bin/g++", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared", "-cudart", "shared"]
@@ -72,27 +73,31 @@ def build_classify(force: bool = False) -> str:
 
 
 KMER_SET = os.path.join(PKG, "bin", "kmer_set")
+COUNT_UNIQUE = os.path.join(PKG, "bin", "count_unique")
 
 
 def build_dbtools(force: bool = False):
-    """The drop-in `db_sort` and `set_lcas` executables (SURVEY §8 f4; host C++ over libkuq.so), and `kmer_set`, the
-    drop-in for build_db.sh's Jellyfish 1 step (at KMER_SET).  Returns the paths of db_sort and set_lcas."""
+    """The drop-in `db_sort` and `set_lcas` executables (SURVEY §8 f4; host C++ over libkuq.so), `kmer_set`, the
+    drop-in for build_db.sh's Jellyfish 1 step (at KMER_SET), and `count_unique` (at COUNT_UNIQUE).  Returns the paths
+    of db_sort and set_lcas."""
     src = os.path.join(CSRC, "dbbuild_main.cpp")
     build(force=force)
-    outs = [(os.path.join(PKG, "bin", "db_sort"), src, []), (os.path.join(PKG, "bin", "set_lcas"), src, ["-DTOOL_SET_LCAS"]),
-            (KMER_SET, os.path.join(CSRC, "kmerset_main.cpp"), [])]
-    newest = max(os.path.getmtime(src), os.path.getmtime(outs[2][1]), os.path.getmtime(LIB))
-    if not force and all(os.path.exists(o) and os.path.getmtime(o) >= newest for o, _, _ in outs):
-        return [o for o, _, _ in outs[:2]]
+    outs = [(os.path.join(PKG, "bin", "db_sort"), src, [], []),
+            (os.path.join(PKG, "bin", "set_lcas"), src, ["-DTOOL_SET_LCAS"], []),
+            (KMER_SET, os.path.join(CSRC, "kmerset_main.cpp"), [], []),
+            (COUNT_UNIQUE, os.path.join(CSRC, "countunique_main.cpp"), [], ["-lz"])]
+    newest = max([os.path.getmtime(s) for _, s, _, _ in outs] + [os.path.getmtime(LIB)])
+    if not force and all(os.path.exists(o) and os.path.getmtime(o) >= newest for o, _, _, _ in outs):
+        return [o for o, _, _, _ in outs[:2]]
     os.makedirs(os.path.join(PKG, "bin"), exist_ok=True)
-    for out, src, defs in outs:
-        cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-Wall"] + defs + [src, "-o", out, "-L" + os.path.dirname(LIB), "-lkuq",
-               "-Wl,-rpath,$ORIGIN/../lib", "-Wl,-rpath,/usr/local/cuda/lib64"]
+    for out, src, defs, libs in outs:
+        cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-Wall"] + defs + [src, "-o", out, "-L" + os.path.dirname(LIB), "-lkuq"] + \
+              libs + ["-Wl,-rpath,$ORIGIN/../lib", "-Wl,-rpath,/usr/local/cuda/lib64"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError("g++ failed building " + os.path.basename(out))
-    return [o for o, _, _ in outs[:2]]
+    return [o for o, _, _, _ in outs[:2]]
 
 
 if __name__ == "__main__":

@@ -267,6 +267,9 @@ void free_db(kuq_ctx *ctx) {
   ctx->more.clear();
 }
 
+}  // namespace
+
+namespace kuq {
 // ---- Ertl estimator (hyperloglogplus.cpp:373-422,738-752), same operation order as the reference ----------
 double ertl_sigma(double x) {
   if (x == 1.0) return INFINITY;
@@ -288,6 +291,10 @@ uint64_t ertl_from_hist(const int *C, size_t q, size_t m, uint64_t n_observed) {
   double est = m_sq_alpha_inf / est_denominator;
   return (double(n_observed) < est) ? n_observed : (uint64_t)std::round(est);
 }
+}  // namespace kuq
+
+namespace {
+
 uint64_t ertl_dense_hist(const uint32_t *hist64, uint64_t n_observed) {
   int C[66];
   for (int i = 0; i < 64; i++) C[i] = (int)hist64[i];

@@ -311,6 +311,9 @@ int launch_classify(int mode, const Params &p, int n_sm, cudaStream_t stream, cu
 void launch_unpack_windows(const Params &p, uint64_t n_pos, int n_sm, cudaStream_t stream);
 int classify_smem_bytes();
 int device_sm_count();
+// ertlCardinality's estimator body (hyperloglogplus.cpp:738-752) from the register histogram C[0..q+1] of m registers:
+// min(n_observed, round(estimate)) in the reference's order of operations (kuq_api.cu)
+uint64_t ertl_from_hist(const int *C, size_t q, size_t m, uint64_t n_observed);
 // set_lcas: k_scan + k_set_lcas over library pieces (p.unit_id = dense taxid per piece, p.stats[0] += k-mers not found)
 int launch_set_lcas(const Params &p, int n_sm, cudaStream_t stream);
 int launch_scan_only(const Params &p, int n_sm, cudaStream_t stream);

@@ -16,6 +16,7 @@
 // The packed library stays in HBM when it fits next to the working set of a pass that holds every window; otherwise it
 // lives in pinned host memory and is streamed back once per pass on a copy stream, double-buffered against extraction.
 #include "kuq_kernels.cuh"
+#include "kuq_kmerpack.cuh"
 #include "../../include/kuq.h"
 
 #include <cub/block/block_reduce.cuh>
@@ -33,17 +34,6 @@
 #include <vector>
 
 namespace kuq {
-namespace {
-
-constexpr uint32_t HIST_BITS = 16;                 // histogram over the top 16 bits of the canonical k-mer
-constexpr uint32_t N_BUCKETS = 1u << HIST_BITS;
-constexpr int TILE_THREADS = 256, TILE_ITEMS = 8, TILE = TILE_THREADS * TILE_ITEMS;
-constexpr uint64_t CHUNK_RECORDS = 1ull << 22;     // records per device → host copy
-constexpr uint64_t DEFAULT_BATCH = 256ull << 20;   // bases per batch
-
-__host__ __device__ __forceinline__ uint32_t bucket_of(uint64_t canon, uint32_t k) {
-  return 2 * k > HIST_BITS ? (uint32_t)(canon >> (2 * k - HIST_BITS)) : (uint32_t)canon;
-}
 
 // bit of position pos[i] (relative to the batch) in mask[], i < n: sequence starts (with the end of the text), or the
 // starts of the windows the scanner skips
@@ -81,20 +71,170 @@ __global__ void __launch_bounds__(256) k_ks_pack(const char *text, uint64_t len,
   }
 }
 
-// Warp per block j < nb, lane = window start 32j + lane: valid when its k bases are ACGT, no sequence starts inside
-// (32j + lane, 32j + lane + k) — packed_window's rule — and the scanner does not skip it (drop, or nullptr).  Writes the
-// library segment (codes[0..nb], valid[0..nb)) and counts every valid window's canonical k-mer into hist.
+void ks_scanner_skips(const char *s, uint64_t len, uint32_t k, std::vector<char> &clean, std::vector<uint64_t> &drop_ends) {
+  // the automaton clean_read replays for classification
+  clean.clear();
+  drop_ends.clear();
+  int loaded = 0;
+  bool skip = false;
+  for (uint64_t i = 0; i < len; i++) {
+    const char c = s[i];
+    if (c == '\n' || c == '\r') {
+      if (skip) loaded--;
+      skip = true;
+      continue;
+    }
+    bool emit = false;
+    if (!skip && ++loaded == (int)k) { emit = true; loaded = (int)k - 1; }
+    skip = false;
+    if (!emit && clean.size() >= k - 1) drop_ends.push_back(clean.size());
+    clean.push_back(c);
+  }
+}
+
+cudaError_t KsStager::init(uint32_t k_, uint64_t batch_cap_, uint64_t max_seqs_) {
+  k = k_;
+  batch_cap = batch_cap_;
+  max_seqs = max_seqs_;
+  n_sm = device_sm_count();
+  const uint64_t nb_cap = batch_cap / 32 + 2;
+  cudaError_t e = cudaSuccess;
+  for (int b = 0; b < 2 && e == cudaSuccess; b++) {
+    if ((e = staged[b].alloc(cudaEventDisableTiming)) != cudaSuccess || (e = h_text[b].alloc(batch_cap)) != cudaSuccess) break;
+    e = h_offs[b].alloc(max_seqs + 1);
+  }
+  if (e == cudaSuccess) e = d_text.alloc(batch_cap + 32);
+  if (e == cudaSuccess) e = d_offs.alloc(max_seqs + 1);
+  if (e == cudaSuccess) e = d_codes.alloc(nb_cap + 1);
+  if (e == cudaSuccess) e = d_amb.alloc(nb_cap + 1);
+  if (e == cudaSuccess) e = d_start.alloc(nb_cap + 2);
+  if (e == cudaSuccess) e = d_drop.alloc(nb_cap + 2);
+  if (e != cudaSuccess) { (void)cudaGetLastError(); return e; }
+  h_offs[0][0] = 0;
+  return cudaSuccess;
+}
+
+void KsStager::release_device() {
+  d_text.reset(); d_offs.reset(); d_codes.reset(); d_amb.reset(); d_start.reset(); d_drop.reset(); d_drops.reset();
+  drop_cap = 0;
+  for (int b = 0; b < 2; b++) { h_text[b].reset(); h_offs[b].reset(); }
+}
+
+// Sequence boundary (seq_start .. fill is one piece): keep it when it holds a window
+void KsStager::close_piece() {
+  if (fill - seq_start >= k) h_offs[cur][++n_seqs] = fill;
+  else fill = seq_start;
+  seq_start = fill;
+}
+
+// append bases of the open sequence; a full batch cuts it, the next piece starts with the last k - 1 bases
+int KsStager::append(const char *p, uint64_t n) {
+  while (n) {
+    if (fill == batch_cap) {
+      const uint64_t piece = fill - seq_start, c = std::min<uint64_t>(piece, k - 1);
+      carry.assign(h_text[cur] + fill - c, h_text[cur] + fill);
+      close_piece();
+      int rc = flush();
+      if (rc) return rc;
+      memcpy(h_text[cur], carry.data(), c);
+      fill = c;
+    }
+    const uint64_t take = std::min(n, batch_cap - fill);
+    memcpy(h_text[cur] + fill, p, take);
+    fill += take;
+    p += take;
+    n -= take;
+  }
+  return 0;
+}
+
+int KsStager::add_clean(const char *c, uint64_t n, const std::vector<uint64_t> &ends) {
+  if (n < k) return 0;                             // no window
+  if (full()) {
+    int rc = flush();
+    if (rc) return rc;
+  }
+  seq_start = fill;
+  uint64_t done = 0;
+  for (uint64_t e : ends) {
+    int rc = append(c + done, e + 1 - done);
+    if (rc) return rc;
+    done = e + 1;
+    drops.push_back(fill - k);                     // base e sits at fill - 1 with its k - 1 predecessors in the piece
+  }
+  int rc = append(c + done, n - done);
+  if (rc) return rc;
+  close_piece();
+  return 0;
+}
+
+int KsStager::add_sequence(const char *s, uint64_t n) {
+  if (n < k) return 0;
+  if (!memchr(s, '\n', n) && !memchr(s, '\r', n)) {
+    static const std::vector<uint64_t> none;
+    return add_clean(s, n, none);
+  }
+  ks_scanner_skips(s, n, k, clean, drop_ends);
+  return add_clean(clean.data(), clean.size(), drop_ends);
+}
+
+cudaError_t KsStager::stage(cudaStream_t st) {
+  const int b = cur;
+  len = fill;
+  nb = (len + 31) / 32;
+  const uint64_t n = n_seqs;
+  cudaError_t e;
+  if ((e = cudaMemcpyAsync(d_text, h_text[b], len, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
+  if ((e = cudaMemcpyAsync(d_offs, h_offs[b], (n + 1) * 8, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;
+  if ((e = cudaEventRecord(staged[b], st)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(d_start, 0, (nb + 2) * 4, st)) != cudaSuccess) return e;
+  k_ks_mark<<<(unsigned)std::min<uint64_t>((n + 256) / 256, (uint64_t)n_sm * 8), 256, 0, st>>>(d_offs, (uint32_t)n + 1, d_start);
+  const uint64_t nd = drops.size();
+  has_drops = nd != 0;
+  if (nd) {                                         // sequences with line breaks (rare): the windows the scanner skips
+    if (nd > drop_cap) {
+      drop_cap = std::max<uint64_t>(nd, 1 << 16);
+      if ((e = d_drops.alloc(drop_cap)) != cudaSuccess) { drop_cap = 0; return e; }
+    }
+    if ((e = cudaMemcpyAsync(d_drops, drops.data(), nd * 8, cudaMemcpyHostToDevice, st)) != cudaSuccess) return e;   // pageable: staged now
+    if ((e = cudaMemsetAsync(d_drop, 0, (nb + 2) * 4, st)) != cudaSuccess) return e;
+    k_ks_mark<<<(unsigned)std::min<uint64_t>((nd + 255) / 256, (uint64_t)n_sm * 8), 256, 0, st>>>(d_drops, (uint32_t)nd, d_drop);
+    drops.clear();
+  }
+  k_ks_pack<<<(unsigned)std::min<uint64_t>((2 * (nb + 1) + 255) / 256, (uint64_t)n_sm * 16), 256, 0, st>>>(d_text, len, nb, d_codes, d_amb);
+  return cudaGetLastError();
+}
+
+cudaError_t KsStager::next() {
+  cur ^= 1;
+  const cudaError_t e = cudaEventSynchronize(staged[cur]);
+  fill = seq_start = 0;
+  n_seqs = 0;
+  h_offs[cur][0] = 0;
+  return e;
+}
+
+namespace {
+
+constexpr uint32_t HIST_BITS = 16;                 // histogram over the top 16 bits of the canonical k-mer
+constexpr uint32_t N_BUCKETS = 1u << HIST_BITS;
+constexpr int TILE_THREADS = 256, TILE_ITEMS = 8, TILE = TILE_THREADS * TILE_ITEMS;
+constexpr uint64_t CHUNK_RECORDS = 1ull << 22;     // records per device → host copy
+constexpr uint64_t DEFAULT_BATCH = 256ull << 20;   // bases per batch
+
+__host__ __device__ __forceinline__ uint32_t bucket_of(uint64_t canon, uint32_t k) {
+  return 2 * k > HIST_BITS ? (uint32_t)(canon >> (2 * k - HIST_BITS)) : (uint32_t)canon;
+}
+
+// Warp per block j < nb, lane = window start 32j + lane (valid: ks_window_ok).  Writes the library segment (codes[0..nb], valid[0..nb)) and counts every valid window's canonical k-mer into hist.
 __global__ void __launch_bounds__(256) k_ks_windows(const uint64_t *codes, const uint32_t *amb, const uint32_t *start,
                                                     const uint32_t *drop, uint64_t nb, uint32_t k, uint64_t *lib_codes,
                                                     uint32_t *lib_valid, unsigned long long *hist) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-  const uint64_t kmask = (1ull << k) - 1, smask = (1ull << (k - 1)) - 1;
   for (uint64_t j = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < nb; j += warps) {
     const uint64_t a = codes[j], b = codes[j + 1];
-    const uint64_t amb64 = ((uint64_t)amb[j + 1] << 32) | amb[j];
-    const uint64_t st64 = ((uint64_t)start[j + 1] << 32) | start[j];
-    const bool ok = !((amb64 >> lane) & kmask) && !((st64 >> (lane + 1)) & smask) && !(drop && ((drop[j] >> lane) & 1u));
+    const bool ok = ks_window_ok(amb, start, drop, j, lane, k);
     const uint32_t valid = __ballot_sync(0xFFFFFFFFu, ok);
     if (ok) atomicAdd(hist + bucket_of(canonical_kmer(window_top(a, b, lane), k), k), 1ull);
     if (lane == 0) {
@@ -204,20 +344,7 @@ struct kuq_kmer_set {
   std::map<void *, uint64_t> dev;
   uint64_t dev_bytes = 0, free0 = 0, free_min = 0;
   // batches
-  char *h_text[2] = {nullptr, nullptr};
-  uint64_t *h_offs[2] = {nullptr, nullptr};
-  cudaEvent_t staged[2] = {nullptr, nullptr};
-  int cur = 0;
-  uint64_t fill = 0, seq_start = 0;
-  uint32_t n_seqs = 0;
-  std::vector<char> carry, clean;
-  std::vector<uint64_t> drops, drop_ends;          // starts (in the batch) / ends (in `clean`) of windows the scanner skips
-  uint64_t drop_cap = 0;
-  uint64_t *d_drops = nullptr;
-  uint32_t *d_drop = nullptr;
-  char *d_text = nullptr;
-  uint64_t *d_offs = nullptr, *d_codes = nullptr;
-  uint32_t *d_amb = nullptr, *d_start = nullptr;
+  KsStager in;
   uint8_t *d_spill = nullptr;
   unsigned long long *d_hist = nullptr, *d_cursor = nullptr;
   uint64_t positions = 0;
@@ -320,31 +447,13 @@ int copy_segment_to_host(kuq_kmer_set *h, kuq_kmer_set::Segment &s) {
   return 0;
 }
 
-// the batch in h_text[cur] / h_offs[cur] → packed segment + histogram, asynchronously on h->st
+// the open batch → packed segment + histogram, asynchronously on h->st
 int flush(kuq_kmer_set *h) {
-  if (h->n_seqs == 0) { h->fill = h->seq_start = 0; return 0; }
-  const int b = h->cur;
-  const uint64_t len = h->fill, nb = (len + 31) / 32, n = h->n_seqs;
+  KsStager &in = h->in;
+  if (in.empty()) { in.fill = in.seq_start = 0; return 0; }
   h->mark(0, true);
-  KS_CU(cudaMemcpyAsync(h->d_text, h->h_text[b], len, cudaMemcpyHostToDevice, h->st));
-  KS_CU(cudaMemcpyAsync(h->d_offs, h->h_offs[b], (n + 1) * 8, cudaMemcpyHostToDevice, h->st));
-  KS_CU(cudaEventRecord(h->staged[b], h->st));
-  KS_CU(cudaMemsetAsync(h->d_start, 0, (nb + 2) * 4, h->st));
-  k_ks_mark<<<(unsigned)std::min<uint64_t>((n + 256) / 256, (uint64_t)h->n_sm * 8), 256, 0, h->st>>>(h->d_offs, (uint32_t)n + 1, h->d_start);
-  const uint64_t nd = h->drops.size();
-  if (nd) {                                         // sequences with line breaks (rare): the windows the scanner skips
-    if (nd > h->drop_cap) {
-      h->release(h->d_drops);
-      h->drop_cap = std::max<uint64_t>(nd, 1 << 16);
-      KS_ALLOC(h->d_drops, 8 * h->drop_cap);
-    }
-    KS_CU(cudaMemcpyAsync(h->d_drops, h->drops.data(), nd * 8, cudaMemcpyHostToDevice, h->st));   // pageable: staged now
-    KS_CU(cudaMemsetAsync(h->d_drop, 0, (nb + 2) * 4, h->st));
-    k_ks_mark<<<(unsigned)std::min<uint64_t>((nd + 255) / 256, (uint64_t)h->n_sm * 8), 256, 0, h->st>>>(h->d_drops, (uint32_t)nd, h->d_drop);
-    h->drops.clear();
-  }
-  k_ks_pack<<<(unsigned)std::min<uint64_t>((2 * (nb + 1) + 255) / 256, (uint64_t)h->n_sm * 16), 256, 0, h->st>>>(
-      h->d_text, len, nb, h->d_codes, h->d_amb);
+  KS_CU(in.stage(h->st));
+  const uint64_t len = in.len, nb = in.nb;
   // placement: the library stays in HBM while it fits next to a pass holding every window seen so far
   h->positions += len;
   const uint64_t sb = seg_bytes(nb);
@@ -366,8 +475,8 @@ int flush(kuq_kmer_set *h) {
     h->lib_dev_bytes += sb;
   }
   k_ks_windows<<<(unsigned)std::min<uint64_t>((nb + 7) / 8, (uint64_t)h->n_sm * 16), 256, 0, h->st>>>(
-      h->d_codes, h->d_amb, h->d_start, nd ? h->d_drop : nullptr, nb, h->k, (uint64_t *)dst, (uint32_t *)(dst + 8 * (nb + 1)),
-      h->d_hist);
+      in.d_codes, in.d_amb, in.d_start, in.has_drops ? in.d_drop.get() : nullptr, nb, h->k, (uint64_t *)dst,
+      (uint32_t *)(dst + 8 * (nb + 1)), h->d_hist);
   KS_CU(cudaGetLastError());
   if (!h->lib_on_device) {
     s.dev = h->d_spill;
@@ -378,40 +487,7 @@ int flush(kuq_kmer_set *h) {
   h->max_seg_bytes = std::max(h->max_seg_bytes, sb);
   h->segs.push_back(s);
   h->mark(0, false);
-  // the other staging buffer is refilled next: wait for its copy
-  h->cur ^= 1;
-  KS_CU(cudaEventSynchronize(h->staged[h->cur]));
-  h->fill = h->seq_start = 0;
-  h->n_seqs = 0;
-  h->h_offs[h->cur][0] = 0;
-  return 0;
-}
-
-// Sequence boundary (h->seq_start .. h->fill is one piece): keep it when it holds a window
-void close_piece(kuq_kmer_set *h) {
-  if (h->fill - h->seq_start >= h->k) h->h_offs[h->cur][++h->n_seqs] = h->fill;
-  else h->fill = h->seq_start;
-  h->seq_start = h->fill;
-}
-
-// append bases of the open sequence; a full batch cuts it, the next piece starts with the last k - 1 bases
-int append(kuq_kmer_set *h, const char *p, uint64_t n) {
-  while (n) {
-    if (h->fill == h->batch_cap) {
-      const uint64_t piece = h->fill - h->seq_start, c = std::min<uint64_t>(piece, h->k - 1);
-      h->carry.assign(h->h_text[h->cur] + h->fill - c, h->h_text[h->cur] + h->fill);
-      close_piece(h);
-      int rc = flush(h);
-      if (rc) return rc;
-      memcpy(h->h_text[h->cur], h->carry.data(), c);
-      h->fill = c;
-    }
-    const uint64_t take = std::min(n, h->batch_cap - h->fill);
-    memcpy(h->h_text[h->cur] + h->fill, p, take);
-    h->fill += take;
-    p += take;
-    n -= take;
-  }
+  KS_CU(in.next());
   return 0;
 }
 
@@ -419,20 +495,8 @@ int plan(kuq_kmer_set *h) {
   int rc = flush(h);
   if (rc) return rc;
   KS_CU(cudaStreamSynchronize(h->st));
-  h->release(h->d_text);
-  h->release(h->d_offs);
-  h->release(h->d_codes);
-  h->release(h->d_amb);
-  h->release(h->d_start);
+  h->in.release_device();
   h->release(h->d_spill);
-  h->release(h->d_drop);
-  h->release(h->d_drops);
-  for (int b = 0; b < 2; b++) {
-    cudaFreeHost(h->h_text[b]);
-    cudaFreeHost(h->h_offs[b]);
-    h->h_text[b] = nullptr;
-    h->h_offs[b] = nullptr;
-  }
   std::vector<unsigned long long> hist(N_BUCKETS);
   KS_CU(cudaMemcpy(hist.data(), h->d_hist, N_BUCKETS * 8, cudaMemcpyDeviceToHost));
   uint64_t total = 0, biggest = 0;
@@ -576,6 +640,7 @@ int kuq_kmer_set_create(int device, uint32_t k, uint64_t budget, kuq_kmer_set **
   h->budget = budget ? budget : env_u64("KUQ_KMER_SET_BUDGET", free_b / 4 * 3);
   h->batch_cap = std::max<uint64_t>(env_u64("KUQ_KMER_SET_BATCH", DEFAULT_BATCH), 2 * k + 32);
   h->max_seqs = std::min<uint64_t>(h->batch_cap / k + 2, 1ull << 22);
+  h->in.flush = [h] { return flush(h); };
   auto bail = [&](int code) {
     std::string m = h->err;
     kuq_kmer_set_destroy(h);
@@ -586,22 +651,16 @@ int kuq_kmer_set_create(int device, uint32_t k, uint64_t budget, kuq_kmer_set **
       cudaStreamCreateWithFlags(&h->cp, cudaStreamNonBlocking) != cudaSuccess)
     return bail(h->fail(KUQ_E_CUDA, "cannot create streams"));
   for (int b = 0; b < 2; b++) {
-    if (cudaEventCreateWithFlags(&h->staged[b], cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->ready[b], cudaEventDisableTiming) != cudaSuccess ||
+    if (cudaEventCreateWithFlags(&h->ready[b], cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->freed[b], cudaEventDisableTiming) != cudaSuccess)
       return bail(h->fail(KUQ_E_CUDA, "cannot create events"));
     cudaEventRecord(h->freed[b], h->cp);
-    if (cudaHostAlloc((void **)&h->h_text[b], h->batch_cap, cudaHostAllocDefault) != cudaSuccess ||
-        cudaHostAlloc((void **)&h->h_offs[b], 8 * (h->max_seqs + 1), cudaHostAllocDefault) != cudaSuccess)
-      return bail(h->fail(KUQ_E_NOMEM, "cannot allocate pinned staging buffers"));
   }
-  h->h_offs[0][0] = 0;
+  if (h->in.init(k, h->batch_cap, h->max_seqs) != cudaSuccess)
+    return bail(h->fail(KUQ_E_NOMEM, "cannot allocate the batch staging buffers"));
   if (cudaHostAlloc((void **)&h->h_scalar, 8, cudaHostAllocDefault) != cudaSuccess)
     return bail(h->fail(KUQ_E_NOMEM, "cannot allocate pinned memory"));
-  if (h->alloc(&h->d_text, h->batch_cap + 32) || h->alloc(&h->d_offs, 8 * (h->max_seqs + 1)) ||
-      h->alloc(&h->d_codes, 8 * (nb + 1)) || h->alloc(&h->d_amb, 4 * (nb + 1)) || h->alloc(&h->d_start, 4 * (nb + 2)) ||
-      h->alloc(&h->d_drop, 4 * (nb + 2)) ||
-      h->alloc(&h->d_spill, seg_bytes(nb)) || h->alloc(&h->d_hist, 8ull * N_BUCKETS) || h->alloc(&h->d_cursor, 8))
+  if (h->alloc(&h->d_spill, seg_bytes(nb)) || h->alloc(&h->d_hist, 8ull * N_BUCKETS) || h->alloc(&h->d_cursor, 8))
     return bail(h->fail(KUQ_E_NOMEM, "cannot allocate the batch buffers on the device"));
   if (cudaMemsetAsync(h->d_hist, 0, 8ull * N_BUCKETS, h->st) != cudaSuccess) return bail(h->fail(KUQ_E_CUDA, "memset failed"));
   *out = h;
@@ -615,50 +674,8 @@ int kuq_kmer_set_add(kuq_kmer_set *h, const char *bases, const uint64_t *offsets
   KS_CU(cudaSetDevice(h->device));
   for (uint32_t r = 0; r < n_seqs; r++) {
     if (offsets[r + 1] < offsets[r]) return h->fail(KUQ_E_INVALID_ARG, "offsets decrease at sequence %u", r);
-    const char *s = bases + offsets[r];
-    const uint64_t len = offsets[r + 1] - offsets[r];
-    if (len < h->k) continue;                       // no window
-    if (h->n_seqs + 1 >= h->max_seqs || h->fill == h->batch_cap) {
-      int rc = flush(h);
-      if (rc) return rc;
-    }
-    h->seq_start = h->fill;
-    if (!memchr(s, '\n', len) && !memchr(s, '\r', len)) {
-      int rc = append(h, s, len);
-      if (rc) return rc;
-    } else {
-      // KmerScanner::next_kmer (krakenutil.cpp:239-278) drops '\n' / '\r' from the k-mer but then loads the next base
-      // without counting it, and each further one of a run uncounts one more: one window per such character is never
-      // produced (the automaton clean_read replays for classification).  The bases go in without the line breaks;
-      // the start of every skipped window is recorded once its last base is in the batch.
-      h->clean.clear();
-      h->drop_ends.clear();
-      int loaded = 0;
-      bool skip = false;
-      for (uint64_t i = 0; i < len; i++) {
-        const char c = s[i];
-        if (c == '\n' || c == '\r') {
-          if (skip) loaded--;
-          skip = true;
-          continue;
-        }
-        bool emit = false;
-        if (!skip && ++loaded == (int)h->k) { emit = true; loaded = (int)h->k - 1; }
-        skip = false;
-        if (!emit && h->clean.size() >= h->k - 1) h->drop_ends.push_back(h->clean.size());
-        h->clean.push_back(c);
-      }
-      uint64_t done = 0;
-      for (uint64_t e : h->drop_ends) {
-        int rc = append(h, h->clean.data() + done, e + 1 - done);
-        if (rc) return rc;
-        done = e + 1;
-        h->drops.push_back(h->fill - h->k);           // base e sits at fill - 1 with its k - 1 predecessors in the piece
-      }
-      int rc = append(h, h->clean.data() + done, h->clean.size() - done);
-      if (rc) return rc;
-    }
-    close_piece(h);
+    int rc = h->in.add_sequence(bases + offsets[r], offsets[r + 1] - offsets[r]);
+    if (rc) return rc;
   }
   return KUQ_OK;
 }
@@ -749,12 +766,9 @@ void kuq_kmer_set_destroy(kuq_kmer_set *h) {
     if (s.host) cudaFreeHost(s.host);
   }
   for (auto &kv : h->dev) cudaFree(kv.first);
-  for (int b = 0; b < 2; b++) {
-    if (h->h_text[b]) cudaFreeHost(h->h_text[b]);
-    if (h->h_offs[b]) cudaFreeHost(h->h_offs[b]);
-    for (cudaEvent_t e : {h->staged[b], h->ready[b], h->freed[b]})
+  for (int b = 0; b < 2; b++)
+    for (cudaEvent_t e : {h->ready[b], h->freed[b]})
       if (e) cudaEventDestroy(e);
-  }
   if (h->h_chunk) cudaFreeHost(h->h_chunk);
   if (h->h_scalar) cudaFreeHost(h->h_scalar);
   if (h->st) cudaStreamDestroy(h->st);
