@@ -631,6 +631,22 @@ int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t 
  * one-piece sort, else the number of ranges.  KUQ_E_CAPACITY when the index or one minimizer bin does not fit. */
 int kuq_db_sort_budget(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
                        void *kdb_out, void *idx_out, uint32_t *n_passes, char *err, uint64_t err_cap);
+/* db_sort on several devices: kuq_db_sort_budget is its one-device case.  A sort that fits devices[0] in one piece runs
+ * there alone.  Otherwise every entry of devices[0, n_devices) is a worker (an ordinal may repeat: several workers on
+ * one card), each with its own stream and pinned bounce buffers and `budget` bytes of its device's memory (0 →
+ * KUQ_DB_SORT_BUDGET, else 3/4 of the device's free memory shared among the workers on it; the smallest share is every
+ * worker's).  The ranges are planned from that budget as on one device, so the plan does not depend on n_devices:
+ *   A. worker w streams the contiguous slice [n * w / G, n * (w + 1) / G) of the records for its bin histogram and
+ *      keeps its running sum on the device; the index is the sum over the slices;
+ *   cursors: a kernel on each device reduces the slice's counts over the ranges' bins; range r's records are laid out
+ *      slice after slice, so that they keep input order;
+ *   B. every worker groups its slice by range into the output image at its own cursors;
+ *   C. the ranges, split into contiguous groups (one per worker), are sorted in place.
+ * Workers write disjoint bytes of the host images; no peer access is needed.  The result is the bytes of the one-device
+ * sort. */
+int kuq_db_sort_devices(const int *devices, uint32_t n_devices, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt,
+                        int zero_vals, uint64_t budget, void *kdb_out, void *idx_out, uint32_t *n_passes, char *err,
+                        uint64_t err_cap);
 /* set_lcas (set_lcas.cpp:429-476): for every k-mer of the library pieces that the staged database holds,
  * value = lca(taxid of the piece, value).  A piece is a stretch of one library sequence; consecutive pieces of a
  * sequence overlap by k-1 bases (the reference's SKIP_LEN pieces, :363-364).  The context needs the database
@@ -654,6 +670,12 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
  * stride (key_len + 4 bytes), whatever the staged layout.  A staged range writes only its own records, at their
  * positions in the file. */
 int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes);
+/* Records of the staged database (or range) per value, as taxids, value 0 included: what KrakenDB::count_taxons
+ * (krakendb.cpp:90-113) writes to database.kdb.counts, for the values as they are now (kuq_db_taxids reports them as
+ * staged).  Ascending by taxid, taxids with no record left out; cap = 0 queries *n only.  Once the context has numbered
+ * its taxa (after the first kuq_set_lcas_batch or classification) one pass over the records in HBM counts them by dense
+ * id; before that the values are those staging counted.  KUQ_E_STATE with appended databases. */
+int kuq_db_value_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n);
 
 /* k-mer set of a FASTA library: step 1 of build_db.sh (scripts/build_db.sh:116-147), `jellyfish count -m k -C` of
  * Jellyfish 1, whose output database_0 becomes database.jdb.  The set holds one record per distinct canonical k-mer

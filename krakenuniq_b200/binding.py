@@ -119,6 +119,9 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_db_sort": (C.c_int, [C.c_int, vp, C.c_uint64, C.c_uint32, C.c_int, vp, vp, C.c_char_p, C.c_uint64]),
         "kuq_db_sort_budget": (C.c_int, [C.c_int, vp, C.c_uint64, C.c_uint32, C.c_int, C.c_uint64, vp, vp, u32p, C.c_char_p,
                                          C.c_uint64]),
+        "kuq_db_sort_devices": (C.c_int, [C.POINTER(C.c_int), C.c_uint32, vp, C.c_uint64, C.c_uint32, C.c_int, C.c_uint64,
+                                          vp, vp, u32p, C.c_char_p, C.c_uint64]),
+        "kuq_db_value_counts": (C.c_int, [vp, u32p, u64p, C.c_uint32, u32p]),
         "kuq_set_lcas_batch": (C.c_int, [vp, vp, u64p, C.c_uint32, u32p, C.c_uint32, u64p]),
         "kuq_export_db_values": (C.c_int, [vp, vp, C.c_uint64]),
         "kuq_set_quick_mode": (C.c_int, [vp, C.c_uint32, C.c_int]),
@@ -353,6 +356,16 @@ class Classifier:
         """kuq_export_db_values: write the device record values (taxids) into the host image `kdb` in place"""
         assert kdb.dtype == np.uint8 and kdb.flags["C_CONTIGUOUS"]
         self._ck(self.L.kuq_export_db_values(self.h, kdb.ctypes.data, kdb.size))
+
+    def db_value_counts(self):
+        """kuq_db_value_counts: (taxids ascending, records holding each) of the staged records' values as they are now"""
+        n = C.c_uint32(0)
+        self._ck(self.L.kuq_db_value_counts(self.h, None, None, 0, C.byref(n)))
+        t = np.zeros(n.value, np.uint32)
+        c = np.zeros(n.value, np.uint64)
+        if n.value:
+            self._ck(self.L.kuq_db_value_counts(self.h, _p(t, u32p), _p(c, u64p), n.value, C.byref(n)))
+        return t, c
 
     def mark_zero_hits(self, on=True):
         """several databases: lookups report a stored taxon 0 as CODE_FOUND_ZERO (kuq_mark_zero_hits)"""
@@ -791,10 +804,11 @@ def decode_runs(res, i):
     return [(int(a), int(b)) for a, b in res["runs"][s:s + c]]
 
 
-def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0, budget=0, with_passes=False):
+def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0, budget=0, with_passes=False, devices=None):
     """kuq_db_sort_budget: unsorted Jellyfish-style image → (database.kdb image, KRAKIX2 index image), on the GPU within
     `budget` bytes of device memory (0 → KUQ_DB_SORT_BUDGET, else 3/4 of the free memory).  with_passes: also return
-    the number of passes (1 = in one piece, else the number of minimizer ranges)."""
+    the number of passes (1 = in one piece, else the number of minimizer ranges).  devices: a list of device ordinals
+    (kuq_db_sort_devices; repeats allowed), each a worker of a sort in passes, instead of `device` alone."""
     L = load_library()
     jdb = np.ascontiguousarray(jdb, np.uint8)
     key_bits = int(np.frombuffer(jdb[8:16].tobytes(), np.uint64)[0])
@@ -804,8 +818,13 @@ def db_sort(jdb: np.ndarray, nt: int, zero_vals=False, device=0, budget=0, with_
     idx = np.zeros(8 + 8 * (4 ** nt + 1), np.uint8)
     err = C.create_string_buffer(512)
     passes = C.c_uint32(0)
-    rc = L.kuq_db_sort_budget(device, jdb.ctypes.data, jdb.size, nt, 1 if zero_vals else 0, budget, kdb.ctypes.data,
-                              idx.ctypes.data, C.byref(passes), err, 512)
+    if devices is None:
+        rc = L.kuq_db_sort_budget(device, jdb.ctypes.data, jdb.size, nt, 1 if zero_vals else 0, budget, kdb.ctypes.data,
+                                  idx.ctypes.data, C.byref(passes), err, 512)
+    else:
+        devs = (C.c_int * len(devices))(*devices)
+        rc = L.kuq_db_sort_devices(devs, len(devices), jdb.ctypes.data, jdb.size, nt, 1 if zero_vals else 0, budget,
+                                   kdb.ctypes.data, idx.ctypes.data, C.byref(passes), err, 512)
     if rc != 0:
         raise KuqError(rc, err.value.decode() or L.kuq_strerror(rc).decode())
     return (kdb, idx, passes.value) if with_passes else (kdb, idx)

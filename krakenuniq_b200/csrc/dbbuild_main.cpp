@@ -15,14 +15,17 @@
 
 #include <algorithm>
 #include <cctype>
+#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
 #include <iostream>
 #include <map>
+#include <mutex>
 #include <sstream>
 #include <string>
+#include <thread>
 #include <unordered_map>
 #include <vector>
 
@@ -51,6 +54,20 @@ struct Mapped {
   }
 };
 
+// The devices the tool may use, as classify picks them: KUQ_DEVICES=0,2,3 (or "all"), else KUQ_DEVICE=n alone, else
+// every visible sm_90 device.  An ordinal may repeat: several workers on one card.
+static vector<int> pick_devices() {
+  vector<int> devices;
+  const char *dl = getenv("KUQ_DEVICES");
+  if (dl && strcmp(dl, "all") != 0) {
+    for (const char *q = dl; *q;) { devices.push_back(atoi(q)); while (*q && *q != ',') q++; if (*q) q++; }
+  } else if (dl || !getenv("KUQ_DEVICE")) {
+    for (int d = 0; d < kuq_device_count(); d++) devices.push_back(d);
+  }
+  if (devices.empty()) devices.assign(1, getenv("KUQ_DEVICE") ? atoi(getenv("KUQ_DEVICE")) : 0);
+  return devices;
+}
+
 static void write_file(const string &path, const void *data, size_t size, const char *tool) {
   ofstream out(path.c_str(), ofstream::binary);
   if (!out.is_open()) die(EX_CANTCREAT, "can't write " + path, tool);
@@ -67,7 +84,8 @@ static const char *TOOL = "db_sort";
 static void usage(int exit_code = EX_USAGE) {
   cerr << "Usage: db_sort [-z] [-M] [-t threads] [-n nt] <-d input db> <-o output db> <-i output idx>\n"
        << "KUQ_DB_SORT_BUDGET (bytes of device memory; default 3/4 of the free memory): a database whose sort does not fit\n"
-       << "is sorted in passes over minimizer ranges.\n";
+       << "is sorted in passes over minimizer ranges.\n"
+       << "KUQ_DEVICES (0,2,3 or all; default: every visible GPU) or KUQ_DEVICE: the devices that share the passes.\n";
   exit(exit_code);
 }
 
@@ -109,11 +127,14 @@ int main(int argc, char **argv) {
   vector<char> kdb(header + key_ct * (key_len + 4)), idx(8 + 8 * ((1ull << (2 * nt)) + 1));
   cerr << "db_sort: Sorting ...";
   char err[512] = "";
-  int dev = getenv("KUQ_DEVICE") ? atoi(getenv("KUQ_DEVICE")) : 0;
+  const vector<int> devices = pick_devices();
   uint32_t passes = 0;                                  // budget: KUQ_DB_SORT_BUDGET, else 3/4 of free device memory
-  int rc = kuq_db_sort_budget(dev, in.p, in.size, nt, zero_vals, 0, kdb.data(), idx.data(), &passes, err, sizeof err);
+  int rc = kuq_db_sort_devices(devices.data(), (uint32_t)devices.size(), in.p, in.size, nt, zero_vals, 0, kdb.data(),
+                               idx.data(), &passes, err, sizeof err);
   if (rc) die(rc == KUQ_E_NO_DEVICE ? EX_UNAVAILABLE : EX_DATAERR, err[0] ? err : kuq_strerror(rc), TOOL);
-  cerr << "db_sort: " << passes << (passes == 1 ? " pass" : " passes") << endl;
+  cerr << "db_sort: " << passes << (passes == 1 ? " pass" : " passes");
+  if (passes > 1) cerr << " on " << devices.size() << (devices.size() == 1 ? " device" : " devices");
+  cerr << endl;
   cerr << "db_sort: Sorting complete - writing database to disk ..." << endl;
   write_file(index, idx.data(), idx.size(), TOOL);       // make_index, krakendb.cpp:141-147
   write_file(output, kdb.data(), kdb.size(), TOOL);      // db_sort.cpp:69-73
@@ -200,21 +221,59 @@ struct Batch {
   vector<uint32_t> taxids;
   uint32_t contaminant = 0;        // the one contaminant taxid (32630 / 81077) this batch holds, 0 = none yet
 };
-static kuq_ctx *Ctx = NULL;
 static uint32_t K = 0;
-static uint64_t Missing_total = 0;
 static const uint64_t BATCH_NT = 64ull << 20;
-// With the database staged in several minimizer ranges, every batch is kept to be replayed against the later ranges:
-// the library may be a pipe that can be read once (build_db.sh passes -F <(cat_library)).
+
+// One context per device entry that owns minimizer ranges: ranges[0] stays staged while the library is read, the
+// others are staged after it in turn.  missing: the library's k-mers its ranges lack; code / msg: its first failure.
+struct Context {
+  kuq_ctx *ctx = NULL;
+  vector<pair<uint64_t, uint64_t>> ranges;
+  size_t first_range = 0;                                // the plan's index of ranges[0]
+  uint64_t missing = 0, batch_missing = 0;
+  int code = 0;
+  string msg;
+  void fail(int c, const string &m) { if (!code) { code = c; msg = m; } }
+};
+static vector<Context> Ctxs;
+static uint64_t Missing_total = 0;
+// With a context that owns several ranges every batch is kept to be replayed against its later ranges: the library may
+// be a pipe that can be read once (build_db.sh passes -F <(cat_library)).  With at most one range per context the
+// library is read once and never held.
 static bool Keep_batches = false;
 static vector<Batch> Kept;
 
+// f(context) on every context at once, one host thread each (none for a single context); then the first failure ends
+// the run
+template <typename F>
+static void on_contexts(F f) {
+  if (Ctxs.size() == 1) {
+    f(Ctxs[0]);
+  } else {
+    vector<thread> th;
+    for (Context &c : Ctxs) th.emplace_back([&c, &f] { f(c); });
+    for (thread &t : th) t.join();
+  }
+  for (Context &c : Ctxs)
+    if (c.code) die(c.code, c.msg, TOOL);
+}
+
+static void lca_batch(Context &c, const Batch &b) {
+  c.batch_missing = 0;
+  if (kuq_set_lcas_batch(c.ctx, b.bases.data(), b.offs.data(), (uint32_t)b.taxids.size(), b.taxids.data(), Lca_flags, &c.batch_missing))
+    c.fail(EX_SOFTWARE, kuq_last_error(c.ctx));
+  c.missing += c.batch_missing;
+}
+
+static void check_missing() {
+  for (Context &c : Ctxs)
+    if (c.batch_missing && !Allow_extra_kmers) die(EX_DATAERR, "kmer found in sequence that is not in database", TOOL);   // :441-443
+}
+
+// every context looks the batch up in its staged range
 static void run_batch(const Batch &b) {
-  uint64_t missing = 0;
-  if (kuq_set_lcas_batch(Ctx, b.bases.data(), b.offs.data(), (uint32_t)b.taxids.size(), b.taxids.data(), Lca_flags, &missing))
-    die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
-  if (missing && !Allow_extra_kmers) die(EX_DATAERR, "kmer found in sequence that is not in database", TOOL);   // :441-443
-  Missing_total += missing;
+  on_contexts([&](Context &c) { lca_batch(c, b); });
+  check_missing();
 }
 
 static void flush(Batch &b) {
@@ -342,11 +401,11 @@ static unordered_map<string, uint32_t> read_seqid_map(const string &path) {
   return id_to_taxon;
 }
 
-// The minimizer ranges staged one at a time: as few as KUQ_SET_LCAS_BUDGET bytes of device memory allow (default: the
-// free memory less 1 GiB for the batch and the staging buffers), 12 bytes per record in HBM.  Together they cover every
-// bin, so that a k-mer whose bin holds no records is still counted as missing.  {(0, 0)} = the whole database at once;
-// so is an index that does not parse (kuq_stage_db reports it).
-static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const Mapped &kdb, const Mapped &idx) {
+// The minimizer ranges of the database, each staged on one context at a time: as few as `budget` bytes of device
+// memory allow, 12 bytes per record in HBM.  Together they cover every bin, so that a k-mer whose bin holds no records
+// is still counted as missing.  {(0, 0)} = the whole database at once; so is an index that does not parse (kuq_stage_db
+// reports it).
+static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const Mapped &kdb, const Mapped &idx, uint64_t budget) {
   const vector<pair<uint64_t, uint64_t>> whole{{0, 0}};
   const uint8_t *q = (const uint8_t *)idx.p;
   if (idx.size < 8 || kdb.size < 56) return whole;
@@ -356,11 +415,6 @@ static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const Mapped &kdb, const
   memcpy(&key_ct, (const char *)kdb.p + 48, 8);
   const uint64_t *offsets = (const uint64_t *)(q + 8);
   if (nt < 1 || nt > 15 || idx.size < 8 + 8 * (n_bins + 1) || offsets[n_bins] > key_ct) return whole;
-  uint64_t budget = getenv("KUQ_SET_LCAS_BUDGET") ? strtoull(getenv("KUQ_SET_LCAS_BUDGET"), NULL, 10) : 0;
-  if (!budget) {
-    const uint64_t free_b = kuq_device_free_bytes(Ctx);
-    budget = free_b > (2ull << 30) ? free_b - (1ull << 30) : free_b / 2;
-  }
   vector<pair<uint64_t, uint64_t>> ranges;
   if (!plan_ranges(offsets, n_bins, budget, 12, ranges)) die(EX_SOFTWARE, "a single minimizer bin exceeds KUQ_SET_LCAS_BUDGET", TOOL);
   if (ranges.size() <= 1) return whole;
@@ -370,8 +424,38 @@ static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const Mapped &kdb, const
   return ranges;
 }
 
-static void stage(const Mapped &kdb, const Mapped &idx, const pair<uint64_t, uint64_t> &range) {
-  if (kuq_stage_db(Ctx, kdb.p, kdb.size, idx.p, idx.size, range.first, range.second)) die(EX_DATAERR, kuq_last_error(Ctx), TOOL);
+// A context's default budget (KUQ_SET_LCAS_BUDGET unset): its device's free memory less 1 GiB for the batch and the
+// staging buffers, shared among the `sharing` contexts on that device
+static uint64_t default_budget(kuq_ctx *ctx, uint32_t sharing) {
+  const uint64_t free_b = kuq_device_free_bytes(ctx);
+  return (free_b > (2ull << 30) ? free_b - (1ull << 30) : free_b / 2) / sharing;
+}
+
+static kuq_ctx *create_context(int device) {
+  kuq_config cfg;
+  kuq_config_default(&cfg);
+  cfg.n_slots = 1;
+  cfg.max_bases_per_batch = BATCH_NT + (1 << 20);
+  cfg.hll_mode = KUQ_HLL_DENSE_ONLY;                      // no sketches are used here
+  cfg.device = device;
+  kuq_ctx *ctx = NULL;
+  int rc = kuq_create(&cfg, &ctx);
+  if (rc) die(EX_UNAVAILABLE, string("libkuq: ") + kuq_strerror(rc), TOOL);
+  return ctx;
+}
+
+static void stage(Context &c, const Mapped &kdb, const Mapped &idx, const pair<uint64_t, uint64_t> &range) {
+  if (kuq_stage_db(c.ctx, kdb.p, kdb.size, idx.p, idx.size, range.first, range.second)) c.fail(EX_DATAERR, kuq_last_error(c.ctx));
+}
+
+// the context's staged values, counted by taxid on the device, added to `counts`
+static void add_value_counts(Context &c, map<uint32_t, uint64_t> &counts) {
+  uint32_t m = 0;
+  if (kuq_db_value_counts(c.ctx, NULL, NULL, 0, &m)) return c.fail(EX_SOFTWARE, kuq_last_error(c.ctx));
+  vector<uint32_t> t(m);
+  vector<uint64_t> n(m);
+  if (m && kuq_db_value_counts(c.ctx, t.data(), n.data(), m, &m)) return c.fail(EX_SOFTWARE, kuq_last_error(c.ctx));
+  for (uint32_t i = 0; i < m; i++) counts[t[i]] += n[i];
 }
 
 int main(int argc, char **argv) {
@@ -418,34 +502,65 @@ int main(int argc, char **argv) {
   uint64_t key_bits;
   memcpy(&key_bits, (const char *)kdb.p + 8, 8);
   K = (uint32_t)(key_bits / 2);
-  kuq_config cfg;
-  kuq_config_default(&cfg);
-  cfg.n_slots = 1;
-  cfg.max_bases_per_batch = BATCH_NT + (1 << 20);
-  cfg.hll_mode = KUQ_HLL_DENSE_ONLY;                      // no sketches are used here
-  if (getenv("KUQ_DEVICE")) cfg.device = atoi(getenv("KUQ_DEVICE"));
-  int rc = kuq_create(&cfg, &Ctx);
-  if (rc) die(EX_UNAVAILABLE, string("libkuq: ") + kuq_strerror(rc), TOOL);
-  const vector<pair<uint64_t, uint64_t>> ranges = plan_lca_ranges(kdb, idx);
-  if (ranges.size() > 1) {
-    // one taxid numbering for every range: the values of all records (as classify -x numbers them); range 0 last, so
-    // that it stays staged for the pass that reads the library
-    cerr << "Database staged in " << ranges.size() << " minimizer ranges" << endl;
-    vector<uint32_t> all;
-    for (size_t r = ranges.size(); r-- > 0;) {
-      stage(kdb, idx, ranges[r]);
-      uint32_t m = 0;
-      kuq_db_taxids(Ctx, NULL, NULL, 0, &m);
-      vector<uint32_t> t(m);
-      if (m && kuq_db_taxids(Ctx, t.data(), NULL, m, &m)) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
-      all.insert(all.end(), t.begin(), t.end());
+  // the range plan: from KUQ_SET_LCAS_BUDGET, else from the first device's free memory; when the database takes more
+  // than one range and there are more devices, every context's share of its device (the smallest share of all)
+  const vector<int> devices = pick_devices();
+  const char *budget_env = getenv("KUQ_SET_LCAS_BUDGET");
+  const uint64_t given = budget_env ? strtoull(budget_env, NULL, 10) : 0;
+  vector<kuq_ctx *> made{create_context(devices[0])};
+  vector<pair<uint64_t, uint64_t>> ranges = plan_lca_ranges(kdb, idx, given ? given : default_budget(made[0], 1));
+  if (ranges.size() > 1 && devices.size() > 1) {
+    for (size_t g = 1; g < devices.size(); g++) made.push_back(create_context(devices[g]));
+    if (!given) {
+      uint64_t budget = UINT64_MAX;
+      for (size_t g = 0; g < devices.size(); g++)
+        budget = min(budget, default_budget(made[g], (uint32_t)count(devices.begin(), devices.end(), devices[g])));
+      ranges = plan_lca_ranges(kdb, idx, budget);
     }
+  }
+  // one range per context while there are enough contexts (the library is then never kept), else contiguous groups
+  // balanced by the bytes each range stages; a context without ranges is let go
+  vector<size_t> first{0, ranges.size()};
+  if (made.size() > 1 && ranges.size() <= made.size()) {
+    first.resize(made.size() + 1);
+    for (size_t g = 0; g <= made.size(); g++) first[g] = min(g, ranges.size());
+  } else if (made.size() > 1) {
+    first = group_ranges((const uint64_t *)((const uint8_t *)idx.p + 8), ranges, (int)made.size(), 12);
+  }
+  for (size_t g = 0; g < made.size(); g++) {
+    if (first[g] == first[g + 1]) { kuq_destroy(made[g]); continue; }
+    Ctxs.emplace_back();
+    Ctxs.back().ctx = made[g];
+    Ctxs.back().ranges.assign(ranges.begin() + first[g], ranges.begin() + first[g + 1]);
+    Ctxs.back().first_range = first[g];
+  }
+  for (Context &c : Ctxs) Keep_batches |= c.ranges.size() > 1;
+  if (ranges.size() > 1) {
+    cerr << "Database staged in " << ranges.size() << " minimizer ranges over " << Ctxs.size()
+         << (Ctxs.size() == 1 ? " context" : " contexts") << " (batches kept: " << (Keep_batches ? "yes" : "no") << ")" << endl;
+    // one taxid numbering for every range: the values of all records (as classify -x numbers them).  Each context stages
+    // its ranges last to first, so that its first range stays staged for the pass that reads the library.
+    vector<vector<uint32_t>> seen(Ctxs.size());
+    on_contexts([&](Context &c) {
+      vector<uint32_t> &all = seen[&c - Ctxs.data()];
+      for (size_t r = c.ranges.size(); r-- > 0 && !c.code;) {
+        stage(c, kdb, idx, c.ranges[r]);
+        uint32_t m = 0;
+        if (c.code) break;
+        kuq_db_taxids(c.ctx, NULL, NULL, 0, &m);
+        vector<uint32_t> t(m);
+        if (m && kuq_db_taxids(c.ctx, t.data(), NULL, m, &m)) c.fail(EX_SOFTWARE, kuq_last_error(c.ctx));
+        all.insert(all.end(), t.begin(), t.end());
+      }
+    });
+    vector<uint32_t> all;
+    for (auto &v : seen) all.insert(all.end(), v.begin(), v.end());
     sort(all.begin(), all.end());
     all.erase(unique(all.begin(), all.end()), all.end());
-    if (kuq_set_db_taxid_universe(Ctx, all.data(), (uint32_t)all.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
-    Keep_batches = true;
+    for (Context &c : Ctxs)
+      if (kuq_set_db_taxid_universe(c.ctx, all.data(), (uint32_t)all.size())) die(EX_SOFTWARE, kuq_last_error(c.ctx), TOOL);
   } else {
-    stage(kdb, idx, ranges[0]);
+    on_contexts([&](Context &c) { stage(c, kdb, idx, c.ranges[0]); });
   }
   unordered_map<string, uint32_t> id_to_taxon;
   if (one_fasta_file) id_to_taxon = read_seqid_map(ID_to_taxon_map_filename);   // may add taxa
@@ -456,7 +571,8 @@ int main(int argc, char **argv) {
       ids.push_back(kv.first);
       parents.push_back(parent_map(kv.first));
     }
-    if (kuq_set_taxonomy(Ctx, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
+    for (Context &c : Ctxs)
+      if (kuq_set_taxonomy(c.ctx, ids.data(), parents.data(), (uint32_t)ids.size())) die(EX_SOFTWARE, kuq_last_error(c.ctx), TOOL);
   }
 
   Batch batch;
@@ -541,28 +657,50 @@ int main(int argc, char **argv) {
     cerr << "\r                                                       ";
     cerr << "\rFinished processing " << seqs_processed << " sequences" << endl;
   }
+  // each context writes its ranges' records into the one image and counts their values (count_taxons,
+  // krakendb.cpp:90-113) on the device; contexts with further ranges replay the same batches in the same order against
+  // each of them
   vector<char> out((const char *)kdb.p, (const char *)kdb.p + kdb.size);
-  if (kuq_export_db_values(Ctx, out.data(), out.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
-  for (size_t r = 1; r < ranges.size(); r++) {            // the same batches in the same order against each further range
-    stage(kdb, idx, ranges[r]);
-    for (const Batch &b : Kept) run_batch(b);
-    if (kuq_export_db_values(Ctx, out.data(), out.size())) die(EX_SOFTWARE, kuq_last_error(Ctx), TOOL);
-    cerr << "Finished minimizer range " << (r + 1) << " of " << ranges.size() << endl;
-  }
-  if (verbose && Missing_total) cerr << Missing_total << " k-mers of the library are not in the database" << endl;
-  if (!Kmer_count_filename.empty()) {                     // count_taxons, krakendb.cpp:90-113 → :141-150
-    cerr << "Writing kmer counts to " << Kmer_count_filename << "..." << endl;
-    const uint64_t key_len = key_bits / 8 + !!(key_bits % 8), header = 72 + 2 * (4 + 8 * key_bits);
-    uint64_t key_ct;
-    memcpy(&key_ct, out.data() + 48, 8);
-    map<uint32_t, uint64_t> counts;
-    for (uint64_t i = 0; i < key_ct; i++) {
-      uint32_t v;
-      memcpy(&v, out.data() + header + i * (key_len + 4) + key_len, 4);
-      ++counts[v];
+  const bool want_counts = !Kmer_count_filename.empty();
+  vector<map<uint32_t, uint64_t>> counts(Ctxs.size());
+  vector<double> count_s(Ctxs.size(), 0);
+  mutex progress;
+  on_contexts([&](Context &c) {
+    const size_t g = &c - Ctxs.data();
+    for (size_t r = 0; r < c.ranges.size() && !c.code; r++) {
+      if (r) {
+        stage(c, kdb, idx, c.ranges[r]);
+        for (size_t b = 0; b < Kept.size() && !c.code; b++) {
+          lca_batch(c, Kept[b]);
+          if (c.batch_missing && !Allow_extra_kmers) c.fail(EX_DATAERR, "kmer found in sequence that is not in database");
+        }
+        if (c.code) break;
+      }
+      if (kuq_export_db_values(c.ctx, out.data(), out.size())) c.fail(EX_SOFTWARE, kuq_last_error(c.ctx));
+      if (want_counts && !c.code) {
+        const auto t0 = chrono::steady_clock::now();
+        add_value_counts(c, counts[g]);
+        count_s[g] += chrono::duration<double>(chrono::steady_clock::now() - t0).count();
+      }
+      if (r) {
+        lock_guard<mutex> hold(progress);
+        cerr << "Finished minimizer range " << (c.first_range + r + 1) << " of " << ranges.size() << endl;
+      }
     }
+  });
+  for (Context &c : Ctxs) Missing_total += c.missing;
+  if (verbose && Missing_total) cerr << Missing_total << " k-mers of the library are not in the database" << endl;
+  if (want_counts) {                                      // count_taxons → :141-150, in ascending taxid order
+    cerr << "Writing kmer counts to " << Kmer_count_filename << "..." << endl;
+    map<uint32_t, uint64_t> all;
+    double secs = 0;
+    for (size_t g = 0; g < Ctxs.size(); g++) {
+      for (auto &kv : counts[g]) all[kv.first] += kv.second;
+      secs += count_s[g];
+    }
+    if (getenv("KUQ_TIMING")) cerr << "[timing] value counts " << secs << " s" << endl;
     ofstream ofs(Kmer_count_filename.c_str());
-    for (auto &kv : counts) ofs << kv.first << '\t' << kv.second << '\n';
+    for (auto &kv : all) ofs << kv.first << '\t' << kv.second << '\n';
   }
   if (!Pretend) {
     // the reference rewrites the memory-mapped input (or the RAM copy under -M) and, with -o, copies it there
@@ -576,7 +714,7 @@ int main(int argc, char **argv) {
     cerr << "Writing new TaxDB ..." << endl;
     write_taxdb(TaxDB_filename);
   }
-  kuq_destroy(Ctx);
+  for (Context &c : Ctxs) kuq_destroy(c.ctx);
   return 0;
 }
 #endif

@@ -3747,20 +3747,29 @@ int kuq_harvest_keep_device(int device, void *d_pairs, uint64_t n_rec, const voi
 }
 
 // ---- database build (SURVEY.md §8 f4; ROUND 1: compiled, not yet run on hardware) ---------------------------------
-int kuq_db_sort_budget(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
-                       void *kdb_out, void *idx_out, uint32_t *n_passes, char *err, uint64_t err_cap) {
+int kuq_db_sort_devices(const int *devices, uint32_t n_devices, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt,
+                        int zero_vals, uint64_t budget, void *kdb_out, void *idx_out, uint32_t *n_passes, char *err,
+                        uint64_t err_cap) {
   int n_dev = 0;
   if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
     if (err && err_cap) snprintf(err, err_cap, "db_sort: no CUDA device (there is no CPU path)");
     (void)cudaGetLastError();
     return KUQ_E_NO_DEVICE;
   }
-  if (device < 0 || device >= n_dev || cudaSetDevice(device) != cudaSuccess) return KUQ_E_INVALID_ARG;
+  if (!devices || !n_devices) return KUQ_E_INVALID_ARG;
+  for (uint32_t i = 0; i < n_devices; i++)
+    if (devices[i] < 0 || devices[i] >= n_dev || cudaSetDevice(devices[i]) != cudaSuccess) return KUQ_E_INVALID_ARG;
+  if (cudaSetDevice(devices[0]) != cudaSuccess) return KUQ_E_INVALID_ARG;
   uint32_t passes = 0;
-  int rc = dbsort_device((const uint8_t *)jdb_image, jdb_bytes, nt, zero_vals, budget, (uint8_t *)kdb_out, (uint8_t *)idx_out,
-                         &passes, err, err_cap);
+  int rc = dbsort_device(devices, n_devices, (const uint8_t *)jdb_image, jdb_bytes, nt, zero_vals, budget, (uint8_t *)kdb_out,
+                         (uint8_t *)idx_out, &passes, err, err_cap);
   if (n_passes) *n_passes = passes;
   return rc;
+}
+
+int kuq_db_sort_budget(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
+                       void *kdb_out, void *idx_out, uint32_t *n_passes, char *err, uint64_t err_cap) {
+  return kuq_db_sort_devices(&device, 1, jdb_image, jdb_bytes, nt, zero_vals, budget, kdb_out, idx_out, n_passes, err, err_cap);
 }
 
 int kuq_db_sort(int device, const void *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, void *kdb_out,
@@ -3813,6 +3822,46 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
   CU(cudaMemcpyAsync(s.h_scalars, s.d_scalars, 8 * 8, cudaMemcpyDeviceToHost, s.stream));
   CU(cudaStreamSynchronize(s.stream));
   if (n_missing) *n_missing = s.h_scalars[4];
+  return KUQ_OK;
+}
+
+int kuq_db_value_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n) {
+  if (!ctx || !n) return KUQ_E_INVALID_ARG;
+  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
+  if (!ctx->more.empty()) return fail(ctx, KUQ_E_STATE, "several databases staged: count them one at a time");
+  std::vector<std::pair<uint32_t, uint64_t>> u;
+  if (!ctx->db_remapped) {
+    // the values are still the taxids they were staged with, and staging counted them (collect_taxids)
+    for (size_t i = 0; i < ctx->db_taxids.size(); i++) u.emplace_back(ctx->db_taxids[i], ctx->db_taxid_counts[i]);
+  } else {
+    CU(cudaSetDevice(ctx->device));
+    for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
+    DevBuf<unsigned long long> d_counts;
+    DevBuf<uint32_t> d_bad;
+    CU(d_counts.alloc(ctx->n_taxa));
+    CU(d_bad.alloc(1));
+    CU(cudaMemsetAsync(d_counts, 0, ctx->n_taxa * 8ull, ctx->aux));
+    CU(cudaMemsetAsync(d_bad, 0, 4, ctx->aux));
+    launch_value_counts(ctx->d_pairs, ctx->key_ct, ctx->n_taxa, d_counts, d_bad, ctx->aux);
+    CU(cudaGetLastError());
+    ctx->launches++;
+    std::vector<unsigned long long> c(ctx->n_taxa);
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(c.data(), d_counts, ctx->n_taxa * 8ull, cudaMemcpyDeviceToHost, ctx->aux));
+    CU(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, ctx->aux));
+    CU(cudaStreamSynchronize(ctx->aux));
+    if (bad) return fail(ctx, KUQ_E_STATE, "a record holds a dense id outside the %u taxa", ctx->n_taxa);
+    for (uint32_t d = 0; d < ctx->n_taxa; d++)
+      if (c[d]) u.emplace_back(ctx->raw_of_dense[d], c[d]);
+    std::sort(u.begin(), u.end());
+  }
+  *n = (uint32_t)u.size();
+  if (cap == 0) return KUQ_OK;
+  if (cap < *n) return fail(ctx, KUQ_E_CAPACITY, "need room for %u taxids", *n);
+  for (uint32_t i = 0; i < *n; i++) {
+    if (taxid) taxid[i] = u[i].first;
+    if (count) count[i] = u[i].second;
+  }
   return KUQ_OK;
 }
 

@@ -14,6 +14,9 @@
 //      from the index); each range's slice goes to that range's cursor in the output image;
 //   C. each range's records come back to the device, get the two sorts of the one-piece path, and return in place.
 // Within a range the records keep input order until C, so repeated keys come out as in the one-piece sort.
+// With several workers (devices, or one device listed more than once) A and B run on one contiguous input slice each,
+// and a range's records are laid out slice after slice (per-slice cursors from each slice's histogram), which keeps
+// that order; C sorts one contiguous group of ranges per worker.  Workers write disjoint bytes of the host images.
 #include "../../include/kuq.h"
 #include "kuq_bounce.cuh"
 #include "kuq_kernels.cuh"
@@ -75,6 +78,46 @@ __global__ void k_dbs_range_of(const uint8_t *pairs, uint64_t n, uint32_t key_le
     rid[i] = lo;
     index[i] = i;
     atomicAdd(range_counts + lo, 1ull);
+  }
+}
+
+// per-slice cursors: records of one input slice in each range, from the slice's own running bin counts (off[b] =
+// records in bins < b); range r holds bins [starts[r], starts[r + 1]), the last one up to n_bins — the bins
+// k_dbs_range_of sends to it
+__global__ void k_dbs_range_counts(const ull *off, uint64_t n_bins, const uint32_t *starts, uint32_t n_ranges, ull *counts) {
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_ranges; r += gridDim.x * blockDim.x)
+    counts[r] = off[r + 1 < n_ranges ? starts[r + 1] : n_bins] - off[starts[r]];
+}
+
+// records per value (kuq_db_value_counts): values are dense ids < n_ids.  Each warp groups its lanes by value
+// (__match_any_sync) and one lane adds the group's size, so a value most records hold (0, a dominant species) costs
+// one atomic per warp, not 32.  SHARED: the block counts into its own 32-bit counters in shared memory first (the grid
+// is sized so that no block sees 2^32 records) and adds them to the global ones at its end.  *bad = 1 when a value is
+// not below n_ids.
+template <bool SHARED>
+__global__ void k_value_counts(const uint8_t *pairs, uint64_t n, uint32_t n_ids, ull *counts, uint32_t *bad) {
+  extern __shared__ uint32_t sh_counts[];
+  if (SHARED) {
+    for (uint32_t i = threadIdx.x; i < n_ids; i += blockDim.x) sh_counts[i] = 0;
+    __syncthreads();
+  }
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;                    // a multiple of 32: whole warps loop
+  for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); w < n; w += stride) {
+    const uint64_t i = w + lane;
+    const bool ok = i < n;
+    uint32_t v = ok ? *reinterpret_cast<const uint32_t *>(pairs + i * 12 + 8) : 0xFFFFFFFFu;
+    if (ok && v >= n_ids) { *bad = 1; v = 0xFFFFFFFFu; }
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, v);
+    if (v != 0xFFFFFFFFu && lane == (uint32_t)(__ffs(peers) - 1)) {
+      if (SHARED) atomicAdd(sh_counts + v, (uint32_t)__popc(peers));
+      else atomicAdd(counts + v, (ull)__popc(peers));
+    }
+  }
+  if (SHARED) {
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < n_ids; i += blockDim.x)
+      if (sh_counts[i]) atomicAdd(counts + i, (ull)sh_counts[i]);
   }
 }
 
@@ -192,13 +235,53 @@ uint64_t largest_bin(const uint64_t *offsets, uint64_t entries) {
   return m;
 }
 
+// One worker of a sort in passes: a device, its stream and bounce buffers, and the slice [s0, s1) of the input records
+// whose histogram (pass A) and grouping (pass B) it does.  Several workers may share a device.
+struct Worker {
+  int dev = 0;
+  Stream st;
+  PinnedBounce *bounce = nullptr;
+  uint64_t s0 = 0, s1 = 0;
+  DevBuf<ull> d_off;                       // pass A → cursors: the running bin counts of the slice
+  std::vector<uint64_t> off;               // their host copy (worker 0 writes the index instead)
+  std::vector<uint64_t> cursor;            // per range: where the slice's records of the range go in the output
+  std::vector<uint64_t> cnt;               // per range: the slice's records of the range
+  size_t group_first = 0, group_end = 0;   // pass C: ranges [group_first, group_end)
+  int rc = KUQ_OK;
+  char msg[512] = "";
+  ~Worker() {                              // the bounce's events belong to the worker's device
+    int cur = dev;
+    cudaGetDevice(&cur);
+    cudaSetDevice(dev);
+    delete bounce;
+    cudaSetDevice(cur);
+  }
+};
+
+// f(worker, err, err_cap) on every worker at once, one host thread each on its device; the first failure's code and
+// message
+template <typename F>
+int on_workers(std::vector<Worker> &W, F f, char *err, size_t err_cap) {
+  std::vector<std::thread> th;
+  for (auto &w : W)
+    th.emplace_back([&w, &f] {
+      w.rc = cudaSetDevice(w.dev) == cudaSuccess ? f(w, w.msg, sizeof w.msg)
+                                                 : seterr(KUQ_E_NO_DEVICE, w.msg, sizeof w.msg, "db_sort: device %d not usable", w.dev);
+    });
+  for (auto &t : th) t.join();
+  for (auto &w : W)
+    if (w.rc) return seterr(w.rc, err, err_cap, "%s", w.msg);
+  return KUQ_OK;
+}
+
 }  // namespace
 
 // Host images in, host images out (kdb_out: header + key_ct * pair size bytes — what db_sort.cpp:70-72 writes;
-// idx_out: 8 + 8 * (4^nt + 1) bytes).  budget = bytes of device memory (0 → KUQ_DB_SORT_BUDGET, else 3/4 of the free
-// memory).  Returns KUQ_OK, KUQ_E_CAPACITY (a bin or the histogram does not fit the budget) or KUQ_E_DB_FORMAT (+ err).
-int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget, uint8_t *kdb_out,
-                  uint8_t *idx_out, uint32_t *n_passes, char *err, size_t err_cap) {
+// idx_out: 8 + 8 * (4^nt + 1) bytes), on devices[0, n_dev) (the current device is devices[0]).  budget = bytes of
+// device memory per worker (0 → KUQ_DB_SORT_BUDGET, else 3/4 of each device's free memory shared among the workers on
+// it).  Returns KUQ_OK, KUQ_E_CAPACITY (a bin or the histogram does not fit the budget) or KUQ_E_DB_FORMAT (+ err).
+int dbsort_device(const int *devices, uint32_t n_dev, const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_vals,
+                  uint64_t budget, uint8_t *kdb_out, uint8_t *idx_out, uint32_t *n_passes, char *err, size_t err_cap) {
   if (!jdb || !kdb_out || !idx_out) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: NULL image");
   if (jdb_bytes < 56 || memcmp(jdb, "JFLISTDN", 8) != 0)
     return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: not a Jellyfish-style database (krakendb.cpp:67)");
@@ -221,12 +304,25 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
   g.entries = 1ull << (2 * nt);
   if (jdb_bytes < g.header + key_ct * g.pair_sz) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: image shorter than its header says");
   const uint64_t n = g.n, pair_sz = g.pair_sz, entries = g.entries;
+  // one_budget decides whether the sort fits the first device in one piece; budget is then what every worker of the
+  // passes may use, the same for all so that the plan does not depend on the devices
+  uint64_t one_budget = budget;
   if (!budget) {
-    size_t free_b = 0, total_b = 0;
-    DB_CU(cudaMemGetInfo(&free_b, &total_b));
     const char *s = getenv("KUQ_DB_SORT_BUDGET");
-    budget = s && *s ? strtoull(s, nullptr, 10) : 0;
-    if (!budget) budget = free_b / 4 * 3;
+    one_budget = budget = s && *s ? strtoull(s, nullptr, 10) : 0;
+    if (!budget) {
+      budget = UINT64_MAX;
+      for (uint32_t w = 0; w < n_dev; w++) {
+        size_t free_b = 0, total_b = 0;
+        DB_CU(cudaSetDevice(devices[w]));
+        DB_CU(cudaMemGetInfo(&free_b, &total_b));
+        uint32_t sharing = 0;
+        for (uint32_t v = 0; v < n_dev; v++) sharing += devices[v] == devices[w];
+        if (w == 0) one_budget = free_b / 4 * 3;
+        budget = std::min<uint64_t>(budget, free_b / 4 * 3 / sharing);
+      }
+      DB_CU(cudaSetDevice(devices[0]));
+    }
   }
   memcpy(kdb_out, jdb, g.header);                                              // db_sort.cpp:56-58,71
   memcpy(idx_out, "KRAKIX2", 7);                                               // krakendb.cpp:144-147
@@ -237,14 +333,13 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
   size_t tmp = 0, scan_tmp = 0;
   DB_CU(core_tmp(n, (int)key_bits, 2 * nt, &tmp));
   DB_CU(cub::DeviceScan::InclusiveSum((void *)nullptr, scan_tmp, (ull *)nullptr, (ull *)nullptr, (int64_t)(entries + 1)));
-  PinnedBounce bounce;
-  DB_CU(bounce.init());
-  cudaStream_t st = 0;
-  const int grid = device_sm_count() * 8;
   *n_passes = 1;
 
-  // ---- in one piece: the whole input and the index on the device ----
-  if (core_bytes(n, pair_sz, std::max(tmp, scan_tmp)) + idx_dev <= budget) {
+  // ---- in one piece on the first device: the whole input and the index on the device ----
+  if (core_bytes(n, pair_sz, std::max(tmp, scan_tmp)) + idx_dev <= one_budget) {
+    PinnedBounce bounce;
+    DB_CU(bounce.init());
+    cudaStream_t st = 0;
     Core c;
     DevBuf<ull> d_off;
     DB_CU(core_alloc(c, n, pair_sz, std::max(tmp, scan_tmp)));
@@ -260,30 +355,60 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
     return KUQ_OK;
   }
 
-  // ---- pass A: the bin histogram, streamed; its running sum is the index ----
-  {
-    uint64_t chunk = std::max<uint64_t>(1, std::min(n, PinnedBounce::CH / pair_sz));
+  // ---- in passes: worker w holds the contiguous slice [n * w / G, n * (w + 1) / G) of the input records ----
+  std::vector<Worker> W(n_dev);
+  for (uint32_t w = 0; w < n_dev; w++) {
+    W[w].dev = devices[w];
+    W[w].s0 = (uint64_t)((unsigned __int128)n * w / n_dev);
+    W[w].s1 = (uint64_t)((unsigned __int128)n * (w + 1) / n_dev);
+  }
+  int rc = on_workers(W, [&](Worker &w, char *err, size_t err_cap) -> int {
+    w.bounce = new PinnedBounce;
+    DB_CU(w.bounce->init());
+    DB_CU(w.st.alloc(cudaStreamNonBlocking));
+    return KUQ_OK;
+  }, err, err_cap);
+  if (rc) return rc;
+
+  // ---- pass A: each slice's bin histogram, streamed, and its running sum; the sum over the slices is the index ----
+  rc = on_workers(W, [&](Worker &w, char *err, size_t err_cap) -> int {
+    const uint64_t m_all = w.s1 - w.s0;
+    uint64_t chunk = std::max<uint64_t>(1, std::min(m_all, PinnedBounce::CH / pair_sz));
     while (chunk > 1 && idx_dev + scan_tmp + chunk * pair_sz + 32 > budget) chunk /= 2;
     if (idx_dev + scan_tmp + chunk * pair_sz + 32 > budget)
       return seterr(KUQ_E_CAPACITY, err, err_cap, "db_sort: the bin histogram of -n %u (%llu bytes) does not fit KUQ_DB_SORT_BUDGET = %llu bytes",
                     nt, (unsigned long long)idx_dev, (unsigned long long)budget);
+    const int grid = device_sm_count() * 8;
     DevBuf<uint8_t> d_chunk, d_tmp;
-    DevBuf<ull> d_off;
     DB_CU(get(d_chunk, chunk * pair_sz));
-    DB_CU(get(d_off, entries + 1));
+    DB_CU(get(w.d_off, entries + 1));
     DB_CU(get(d_tmp, scan_tmp));
-    DB_CU(cudaMemsetAsync(d_off, 0, (entries + 1) * 8, st));
-    for (uint64_t s = 0; s < n; s += chunk) {
-      const uint64_t m = std::min(chunk, n - s);
-      DB_CU(bounce.h2d(d_chunk, body + s * pair_sz, m * pair_sz, st));   // the host copy of the next overlaps this kernel
-      k_dbs_hist<<<grid, 256, 0, st>>>(d_chunk, m, g.key_len, g.k, nt, d_off);
+    DB_CU(cudaMemsetAsync(w.d_off, 0, (entries + 1) * 8, w.st));
+    for (uint64_t s = w.s0; s < w.s1; s += chunk) {
+      const uint64_t m = std::min(chunk, w.s1 - s);
+      DB_CU(w.bounce->h2d(d_chunk, body + s * pair_sz, m * pair_sz, w.st));   // the host copy of the next overlaps this kernel
+      k_dbs_hist<<<grid, 256, 0, w.st>>>(d_chunk, m, g.key_len, g.k, nt, w.d_off);
       DB_CU(cudaGetLastError());
     }
     size_t need = scan_tmp;
-    DB_CU(cub::DeviceScan::InclusiveSum(d_tmp.get(), need, d_off.get(), d_off.get(), (int64_t)(entries + 1), st));
-    DB_CU(bounce.to_host(idx_out + 8, d_off, (entries + 1) * 8, st));
+    DB_CU(cub::DeviceScan::InclusiveSum(d_tmp.get(), need, w.d_off.get(), w.d_off.get(), (int64_t)(entries + 1), w.st));
+    if (&w != &W[0]) w.off.resize(entries + 1);
+    DB_CU(w.bounce->to_host(&w == &W[0] ? (void *)(idx_out + 8) : (void *)w.off.data(), w.d_off, (entries + 1) * 8, w.st));
+    return KUQ_OK;
+  }, err, err_cap);
+  if (rc) return rc;
+  uint64_t *offsets = reinterpret_cast<uint64_t *>(idx_out + 8);
+  if (n_dev > 1) {                                                             // the running sums add up
+    std::vector<std::thread> th;
+    const uint64_t per = (entries + 1 + PinnedBounce::NT - 1) / PinnedBounce::NT;
+    for (uint64_t a = 0; a < entries + 1; a += per)
+      th.emplace_back([&, a] {
+        for (uint32_t w = 1; w < n_dev; w++)
+          for (uint64_t b = a; b < std::min(entries + 1, a + per); b++) offsets[b] += W[w].off[b];
+      });
+    for (auto &t : th) t.join();
+    for (auto &w : W) std::vector<uint64_t>().swap(w.off);
   }
-  const uint64_t *offsets = reinterpret_cast<const uint64_t *>(idx_out + 8);
 
   // ---- the ranges of pass C: planned from the index, checked against CUB's queried temporary size ----
   std::vector<std::pair<uint64_t, uint64_t>> ranges;
@@ -311,9 +436,39 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
     }
   }
   const uint32_t R = (uint32_t)ranges.size();
+  std::vector<uint32_t> starts(R);
+  for (uint32_t r = 0; r < R; r++) starts[r] = (uint32_t)ranges[r].first;
 
-  // ---- pass B: group every chunk by range, stably; each range's slice goes to that range's cursor ----
-  if (n) {
+  // ---- cursors: each slice's records per range (on its device, from its running sums); a range's records are laid
+  // out slice after slice, so that they keep input order across the slices ----
+  if (R) {
+    rc = on_workers(W, [&](Worker &w, char *err, size_t err_cap) -> int {
+      DevBuf<uint32_t> d_starts;
+      DevBuf<ull> d_cnt;
+      DB_CU(get(d_starts, R));
+      DB_CU(get(d_cnt, R));
+      DB_CU(cudaMemcpyAsync(d_starts, starts.data(), R * 4ull, cudaMemcpyHostToDevice, w.st));
+      k_dbs_range_counts<<<(R + 255) / 256, 256, 0, w.st>>>(w.d_off, entries, d_starts, R, d_cnt);
+      DB_CU(cudaGetLastError());
+      w.cnt.resize(R);
+      DB_CU(cudaMemcpyAsync(w.cnt.data(), d_cnt, R * 8ull, cudaMemcpyDeviceToHost, w.st));
+      DB_CU(cudaStreamSynchronize(w.st));
+      w.d_off.reset();
+      return KUQ_OK;
+    }, err, err_cap);
+    if (rc) return rc;
+  }
+  for (uint32_t r = 0; r < R; r++) {
+    uint64_t at = offsets[ranges[r].first];
+    for (auto &w : W) { w.cursor.push_back(at); at += w.cnt[r]; }
+  }
+
+  // ---- pass B: each worker groups every chunk of its slice by range, stably; each range's part goes to the slice's
+  // cursor in that range ----
+  rc = on_workers(W, [&](Worker &w, char *err, size_t err_cap) -> int {
+    const uint64_t n_w = w.s1 - w.s0;
+    if (!n_w) return KUQ_OK;
+    const int grid = device_sm_count() * 8;
     const int rbits = bits_for(R);
     auto stream_need = [&](uint64_t c, size_t *sort_tmp) -> cudaError_t {
       *sort_tmp = 0;
@@ -321,7 +476,7 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
                                              (ull *)nullptr, (int64_t)c, 0, rbits);
     };
     auto fits = [&](uint64_t c, size_t t) { return c * (2 * pair_sz + 24) + t + (uint64_t)R * 12 + 8 * 16 <= budget; };
-    uint64_t chunk = std::min(n, PinnedBounce::CH / pair_sz);
+    uint64_t chunk = std::min(n_w, PinnedBounce::CH / pair_sz);
     size_t stmp = 0;
     DB_CU(stream_need(chunk, &stmp));
     while (chunk > 1 && !fits(chunk, stmp)) { chunk /= 2; DB_CU(stream_need(chunk, &stmp)); }
@@ -340,24 +495,24 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
     DB_CU(get(d_starts, R));
     DB_CU(get(d_cnt, R));
     DB_CU(get(d_tmp, stmp));
-    std::vector<uint32_t> starts(R);
-    std::vector<uint64_t> cursor(R), cnt(R), pos(R);
-    for (uint32_t r = 0; r < R; r++) { starts[r] = (uint32_t)ranges[r].first; cursor[r] = offsets[ranges[r].first]; }
-    DB_CU(cudaMemcpy(d_starts, starts.data(), R * 4ull, cudaMemcpyHostToDevice));
-    DB_CU(bounce.h2d(d_chunk, body, std::min(chunk, n) * pair_sz, st));
-    for (uint64_t s = 0; s < n; s += chunk) {
-      const uint64_t m = std::min(chunk, n - s);
-      DB_CU(cudaMemsetAsync(d_cnt, 0, R * 8ull, st));
-      k_dbs_range_of<<<grid, 256, 0, st>>>(d_chunk, m, g.key_len, g.k, nt, d_starts, R, d_rid, d_idx, d_cnt);
+    std::vector<uint64_t> &cursor = w.cursor;
+    std::vector<uint64_t> cnt(R), pos(R);
+    DB_CU(cudaMemcpyAsync(d_starts, starts.data(), R * 4ull, cudaMemcpyHostToDevice, w.st));
+    const uint8_t *in = body + w.s0 * pair_sz;
+    DB_CU(w.bounce->h2d(d_chunk, in, chunk * pair_sz, w.st));
+    for (uint64_t s = 0; s < n_w; s += chunk) {
+      const uint64_t m = std::min(chunk, n_w - s);
+      DB_CU(cudaMemsetAsync(d_cnt, 0, R * 8ull, w.st));
+      k_dbs_range_of<<<grid, 256, 0, w.st>>>(d_chunk, m, g.key_len, g.k, nt, d_starts, R, d_rid, d_idx, d_cnt);
       size_t need = stmp;
-      DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp.get(), need, d_rid.get(), d_rid2.get(), d_idx.get(), d_idx2.get(), (int64_t)m, 0, rbits, st));
-      k_dbs_emit<<<grid, 256, 0, st>>>(d_chunk, d_idx2, m, g.key_len, 0, d_grp);
+      DB_CU(cub::DeviceRadixSort::SortPairs(d_tmp.get(), need, d_rid.get(), d_rid2.get(), d_idx.get(), d_idx2.get(), (int64_t)m, 0, rbits, w.st));
+      k_dbs_emit<<<grid, 256, 0, w.st>>>(d_chunk, d_idx2, m, g.key_len, 0, d_grp);
       DB_CU(cudaGetLastError());
-      if (s + m < n)                                                 // the host copy of the next chunk overlaps these kernels
-        DB_CU(bounce.h2d(d_chunk, body + (s + m) * pair_sz, std::min(chunk, n - s - m) * pair_sz, st));
-      DB_CU(cudaMemcpyAsync(cnt.data(), d_cnt, R * 8ull, cudaMemcpyDeviceToHost, st));
+      if (s + m < n_w)                                               // the host copy of the next chunk overlaps these kernels
+        DB_CU(w.bounce->h2d(d_chunk, in + (s + m) * pair_sz, std::min(chunk, n_w - s - m) * pair_sz, w.st));
+      DB_CU(cudaMemcpyAsync(cnt.data(), d_cnt, R * 8ull, cudaMemcpyDeviceToHost, w.st));
       const uint8_t *grp = nullptr;
-      DB_CU(bounce.d2h(&grp, d_grp, m * pair_sz, st));
+      DB_CU(w.bounce->d2h(&grp, d_grp, m * pair_sz, w.st));
       uint64_t at = 0;
       for (uint32_t r = 0; r < R; r++) { pos[r] = at; at += cnt[r]; }
       std::vector<std::thread> th;
@@ -370,21 +525,44 @@ int dbsort_device(const uint8_t *jdb, uint64_t jdb_bytes, uint32_t nt, int zero_
       for (auto &x : th) x.join();
       for (uint32_t r = 0; r < R; r++) cursor[r] += cnt[r];
     }
-  }
+    return KUQ_OK;
+  }, err, err_cap);
+  if (rc) return rc;
 
-  // ---- pass C: sort each range in place ----
+  // ---- pass C: the ranges split into contiguous groups, one per worker; each range sorted in place ----
   {
+    const std::vector<size_t> first = group_ranges(offsets, ranges, (int)n_dev, 2 * pair_sz + PASS_C_REC);
+    for (uint32_t w = 0; w < n_dev; w++) { W[w].group_first = first[w]; W[w].group_end = first[w + 1]; }
+  }
+  rc = on_workers(W, [&](Worker &w, char *err, size_t err_cap) -> int {
+    if (w.group_first == w.group_end) return KUQ_OK;
     Core c;
     DB_CU(core_alloc(c, max_rec, pair_sz, ctmp));
-    for (auto &r : ranges) {
+    for (size_t i = w.group_first; i < w.group_end; i++) {
+      const auto &r = ranges[i];
       const uint64_t a = offsets[r.first], m = offsets[r.second] - a;
-      DB_CU(bounce.to_device(c.in, obody + a * pair_sz, m * pair_sz, st));
-      DB_CU(core_sort(c, m, g, (uint32_t)r.first, bits_for(r.second - r.first), zero_vals, nullptr, st));
-      DB_CU(bounce.to_host(obody + a * pair_sz, c.out, m * pair_sz, st));
+      DB_CU(w.bounce->to_device(c.in, obody + a * pair_sz, m * pair_sz, w.st));
+      DB_CU(core_sort(c, m, g, (uint32_t)r.first, bits_for(r.second - r.first), zero_vals, nullptr, w.st));
+      DB_CU(w.bounce->to_host(obody + a * pair_sz, c.out, m * pair_sz, w.st));
     }
-  }
+    return KUQ_OK;
+  }, err, err_cap);
+  if (rc) return rc;
   *n_passes = R ? R : 1;
   return KUQ_OK;
+}
+
+// records per dense id of n 12-byte records, added to counts[0, n_ids); *bad = 1 when a value is n_ids or more
+void launch_value_counts(const uint8_t *pairs, uint64_t n, uint32_t n_ids, unsigned long long *counts, uint32_t *bad,
+                         cudaStream_t st) {
+  if (!n) return;
+  const uint32_t SHARED_IDS = 12288;      // 48 KiB of 32-bit counters: as much shared memory as a block gets by default
+  uint64_t grid = std::min<uint64_t>((uint64_t)device_sm_count() * 4, (n + 255) / 256);
+  grid = std::max<uint64_t>(grid, (n >> 31) + 1);   // fewer than 2^31 records per block: its 32-bit counters hold
+  if (n_ids <= SHARED_IDS)
+    k_value_counts<true><<<(unsigned)grid, 256, n_ids * 4, st>>>(pairs, n, n_ids, counts, bad);
+  else
+    k_value_counts<false><<<(unsigned)grid, 256, 0, st>>>(pairs, n, n_ids, counts, bad);
 }
 
 }  // namespace kuq

@@ -321,9 +321,14 @@ int launch_lookup_only(const Params &p, int n_sm, cudaStream_t stream, int fused
 // several databases: [k_scan with p.db's parameters when `scan`] + the in-order lookup over p.dbs into p.codes_dense;
 // p.chunk_counter must be 0 when `scan`.  Returns #kernels launched.
 int launch_lookup_multi(const Params &p, int n_sm, cudaStream_t stream, bool scan);
-// db_sort on the device (kuq_dbbuild.cu): returns a KUQ_* code, *n_passes = per-range sorts (1 = in one piece)
-int dbsort_device(const uint8_t *jdb_image, uint64_t jdb_bytes, uint32_t nt, int zero_vals, uint64_t budget,
-                  uint8_t *kdb_out, uint8_t *idx_out, uint32_t *n_passes, char *err, size_t err_cap);
+// db_sort on devices[0, n_dev) (kuq_dbbuild.cu; the current device is devices[0]): returns a KUQ_* code, *n_passes =
+// per-range sorts (1 = in one piece)
+int dbsort_device(const int *devices, uint32_t n_dev, const uint8_t *jdb_image, uint64_t jdb_bytes, uint32_t nt,
+                  int zero_vals, uint64_t budget, uint8_t *kdb_out, uint8_t *idx_out, uint32_t *n_passes, char *err,
+                  size_t err_cap);
+// records per dense id of n 12-byte records, added to counts[0, n_ids); *bad = 1 when a value is n_ids or more
+void launch_value_counts(const uint8_t *pairs, uint64_t n, uint32_t n_ids, unsigned long long *counts, uint32_t *bad,
+                         cudaStream_t st);
 
 // database staging helpers
 void launch_collect_taxids(const uint8_t *pairs, uint64_t n_rec, uint32_t *keys, unsigned long long *counts,
