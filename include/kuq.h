@@ -523,12 +523,16 @@ int kuq_scan_device(kuq_ctx *ctx, uint32_t slot, uint32_t k, uint32_t nt, uint32
  *         only once that GPU has finished and a new launch has begun
  *     every owner: kuq_resolve_device(...) for its batches; at the end kuq_finish on every context and kuq_merge_into
  * kuq_host_register pins with cudaHostRegisterPortable, so one registered mapping counts as pinned for every device and
- * every GPU's copies from it overlap its lookups. */
+ * every GPU's copies from it overlap its lookups.
+ * kuq_stream_close releases the two range buffers and the landing zone once the slots are idle (it waits for them),
+ * so that their device memory serves other work between passes: the taxa numbering stays, kuq_resolve_device keeps
+ * resolving ids looked up before, and kuq_stream_load refuses (KUQ_E_STATE) until the next kuq_stream_open. */
 int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, uint64_t max_records, uint64_t max_bins);
 int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64_t n_records, const uint64_t *host_offsets,
                     uint64_t bin_lo, uint64_t bin_hi);
 int kuq_stream_use(kuq_ctx *ctx, uint32_t buf);
 int kuq_stream_check(kuq_ctx *ctx);
+int kuq_stream_close(kuq_ctx *ctx);
 /* Pin / unpin caller memory (e.g. an mmap'ed database.kdb) for asynchronous copies. */
 int kuq_host_register(void *p, uint64_t bytes);
 int kuq_host_unregister(void *p);

@@ -6,10 +6,12 @@ reset of the per-taxon state (kuq_reset_counts), the merge across GPUs and the r
   * each separate run's wall time, its "processed in" time (the reads' pass) and the difference, its staging;
   * the sheet run's wall time, and per sample the reset_counts / merge / print_report lines of KUQ_TIMING;
   * md5 sums of every sample's Kraken output and report, both ways (they must be equal).
+With --hbm-budget BYTES (KUQ_HBM_BUDGET) below the database's size the database streams through the GPU in ranges;
+the sheet run then shares each pass over it among the samples, and its line gives the passes ("rounds") it made.
 The database is synthetic and built on the GPU (synth_gpu, `--records` records, k = 31, nt = 15); the samples are
 `--samples` FASTQ files of `--reads` 150 bp reads sampled from its genome with different seeds.  Run from the
 repository root after `python -m krakenuniq_b200.build`:
-    python krakenuniq_b200/bench_samples.py [--records 1e9] [--samples 8] [--reads 1000000]
+    python krakenuniq_b200/bench_samples.py [--records 1e9] [--samples 8] [--reads 1000000] [--hbm-budget BYTES]
 """
 import argparse
 import hashlib
@@ -57,6 +59,16 @@ def processed(stderr):
     return [float(x) for x in re.findall(r"processed in ([0-9.]+)s", stderr.replace("\r", "\n"))]
 
 
+def passes(stderr):
+    """passes over a streamed database: its first range is looked up once per round (one database)"""
+    return stderr.count("(database chunk 1 of")
+
+
+def round_mib(stderr):
+    m = re.findall(r"\[timing\] streamed: \d+ database\(s\), (\d+) MiB per round", stderr)
+    return int(m[0]) if m else None
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--records", type=float, default=1e9)
@@ -66,6 +78,7 @@ def main():
     ap.add_argument("--threads", type=int, default=8)
     ap.add_argument("--seed", type=int, default=9)
     ap.add_argument("--classify", default=None, help="executable to time (default: this build's)")
+    ap.add_argument("--hbm-budget", type=int, default=None, help="KUQ_HBM_BUDGET: below the database's size it streams")
     a = ap.parse_args()
     exe = os.path.abspath(a.classify or build.build_classify())
     gpu = gpu_info()
@@ -81,13 +94,15 @@ def main():
         del db
         torch.cuda.empty_cache()
         common = [exe, "-d", "db.kdb", "-i", "db.idx", "-a", "taxDB", "-M", "-t", str(a.threads)]
-        env = dict(os.environ, KUQ_TIMING="1")
+        budget = {"KUQ_HBM_BUDGET": str(a.hbm_budget)} if a.hbm_budget else {}
+        env = dict(os.environ, KUQ_TIMING="1", **budget)
         # one run first, not timed: it writes db.kdb.counts (every later run reads it) and warms the page cache
-        subprocess.run(common + ["-o", "off", "-r", "warm.report", names[0] + ".fq"], cwd=tmp, capture_output=True, check=True)
+        subprocess.run(common + ["-o", "off", "-r", "warm.report", names[0] + ".fq"], cwd=tmp, capture_output=True, check=True,
+                       env=dict(os.environ, **budget))
         base = {"gpu": gpu, "records": key_ct, "samples": a.samples, "reads_per_sample": a.reads, "read_len": a.read_len,
-                "threads": a.threads, "classify": exe}
+                "threads": a.threads, "classify": exe, "hbm_budget": a.hbm_budget}
 
-        sep = {"wall_s": [], "processed_s": [], "staging_s": [], "md5": []}
+        sep = {"wall_s": [], "processed_s": [], "staging_s": [], "passes": [], "md5": []}
         t_all = time.perf_counter()
         for n in names:
             t0 = time.perf_counter()
@@ -101,6 +116,7 @@ def main():
             sep["wall_s"].append(round(wall, 3))
             sep["processed_s"].append(p)
             sep["staging_s"].append(round(wall - p, 3))
+            sep["passes"].append(passes(r.stderr))
             sep["md5"].append([md5(os.path.join(tmp, f"sep.{n}.kraken")), md5(os.path.join(tmp, f"sep.{n}.report"))])
         sep_total = time.perf_counter() - t_all
         print(json.dumps(dict(base, mode="separate runs", total_wall_s=round(sep_total, 3), **sep)), flush=True)
@@ -118,7 +134,9 @@ def main():
         md5s = [[md5(os.path.join(tmp, f"sheet.{n}.kraken")), md5(os.path.join(tmp, f"sheet.{n}.report"))] for n in names]
         reset, report, merge = timings(r.stderr, "reset_counts"), timings(r.stderr, "print_report"), timings(r.stderr, "merge")
         per_sample = [round(x + y, 4) for x, y in zip([0.0] + reset, report)]
+        rounds = re.findall(r"samples streamed in (\d+) rounds", r.stderr)       # streamed only (this build)
         print(json.dumps(dict(base, mode="sample sheet", total_wall_s=round(wall, 3), processed_s=processed(r.stderr),
+                              rounds=int(rounds[0]) if rounds else None, passes=passes(r.stderr), round_mib=round_mib(r.stderr),
                               reset_counts_s=reset, merge_s=merge, print_report_s=report,
                               fixed_per_sample_s=per_sample, md5=md5s, md5_equal=md5s == sep["md5"])), flush=True)
         return 0 if md5s == sep["md5"] else 2

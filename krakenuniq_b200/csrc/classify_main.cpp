@@ -18,7 +18,8 @@
 //   --mpa-report / --translate-out scripts/krakenuniq-mpa-report and scripts/krakenuniq-translate run on our Kraken
 //                                  lines: booked while the batch is formatted, the table written after the last sample
 //   --sample-sheet                 no counterpart: one process stages the database(s) once and classifies every row of
-//                                  the sheet as a separate run would, with kuq_reset_counts between the samples
+//                                  the sheet as a separate run would, with kuq_reset_counts between the samples; a
+//                                  streamed database's passes are shared among the rows (classify_streamed)
 // Not supported (exit with a message): -I uid mapping, -x together with several -d databases (the reference's own loop
 // for that combination queries database 0 in every pass, classify.cpp:585-632).
 #include <fcntl.h>
@@ -514,6 +515,11 @@ struct SeqReader {
   string linebuffer;
   bool have_linebuffer = false;
   string *raw = NULL;                    // --extract: the record's lines are appended here
+  string *log = NULL;                    // where the messages go (NULL: stderr at once)
+  void note(const string &msg) {
+    if (log) *log += "classify: " + msg + "\n";
+    else fprintf(stderr, "classify: %s\n", msg.c_str());
+  }
   // next_sequence(): FASTA seqreader.cpp:34-79, FASTQ :93-129.  Appends the sequence to `bases`.
   bool next(Read &r, string &bases) {
     r.quals.clear();
@@ -523,7 +529,7 @@ struct SeqReader {
       in.getline(line);
       if (line.empty()) { valid = false; return false; }            // :101-104
       if (line[0] != '@') {
-        if (line[0] != '\r') fprintf(stderr, "classify: malformed fastq file - sequence header (%s)\n", line.c_str());
+        if (line[0] != '\r') note("malformed fastq file - sequence header (" + line + ")");
         valid = false;
         return false;
       }
@@ -534,7 +540,7 @@ struct SeqReader {
       keep_line(raw, seq, in);
       in.getline(line);
       if (line.empty() || line[0] != '+') {
-        if (line.empty() || line[0] != '\r') fprintf(stderr, "classify: malformed fastq file - quality header (%s)\n", line.c_str());
+        if (line.empty() || line[0] != '\r') note("malformed fastq file - quality header (" + line + ")");
         valid = false;
         return false;
       }
@@ -551,7 +557,7 @@ struct SeqReader {
     if (have_linebuffer) { line = linebuffer; have_linebuffer = false; }
     else in.getline(line);
     if (line.empty() || line[0] != '>') {
-      fprintf(stderr, "classify: malformed fasta file - expected header char > not found\n");
+      note("malformed fasta file - expected header char > not found");
       valid = false;
       return false;
     }
@@ -675,7 +681,9 @@ struct PairReader {
   string *raw = NULL;                      // --extract: mate 1's lines, then mate 2's (raw_n2 bytes)
   uint32_t raw_n2 = 0;
   bool raw_visited = true;                 // the script reads the record: it has a mate 1 (PAIR, ONLY1)
-  void open(const char *f1, const char *f2) {
+  string *error = &Pair_error;              // where the merger's stop is recorded
+  // "" or why a mate file cannot be opened
+  string open(const char *f1, const char *f2) {
     const char *names[2] = {f1, f2};
     for (int k = 0; k < 2; k++) {
       struct stat sb;
@@ -683,15 +691,16 @@ struct PairReader {
       unsigned char magic[3] = {0, 0, 0};
       if (regular)                                                 // determine_file_type (:199-216)
         if (FILE *f = fopen(names[k], "rb")) { size_t got = fread(magic, 1, 3, f); (void)got; fclose(f); }
-      if (!m[k].in.open(names[k])) die(EX_NOINPUT, string("can't open ") + names[k]);
+      if (!m[k].in.open(names[k])) return string("can't open ") + names[k];
       const bool known = magic[0] == '@' || magic[0] == '>' || is_bzip2(magic) || (magic[0] == 0x1f && magic[1] == 0x8b && magic[2] == 8);
-      if (regular && !known) { stop(string("Unknown input file type for ") + names[k]); return; }
+      if (regular && !known) { stop(string("Unknown input file type for ") + names[k]); return ""; }
     }
     const int c = m[0].in.peek();                                  // the format: file 1's first line (:66-75)
-    if (c != '>' && c != '@') { stop(string("Unknown file format for ") + f1); return; }
+    if (c != '>' && c != '@') { stop(string("Unknown file format for ") + f1); return ""; }
     m[0].fasta = m[1].fasta = c == '>';
+    return "";
   }
-  void stop(const string &why) { Pair_error = why; valid = false; }
+  void stop(const string &why) { *error = why; valid = false; }
   void close() { m[0].in.close(); m[1].in.close(); }
   bool next(Read &r, string &bases) {
     if (!valid) return false;
@@ -725,11 +734,13 @@ struct InputReader {
   SeqReader single;
   PairReader pair;
   bool paired = false;
-  void open(const char *filename, const char *mate2) {
+  // "" or why the input cannot be opened
+  string open(const char *filename, const char *mate2) {
     paired = mate2 != NULL;
-    if (paired) { pair.open(filename, mate2); return; }
-    if (!single.in.open(filename)) die(EX_NOINPUT, string("can't open ") + filename);
+    if (paired) return pair.open(filename, mate2);
+    if (!single.in.open(filename)) return string("can't open ") + filename;
     single.fastq = single.in.peek() == '@';                        // determine_input_file_type, :377-388
+    return "";
   }
   bool fastq() const { return !paired && single.fastq; }          // merged records are FASTA
   bool valid() const { return paired ? pair.valid : single.valid; }
@@ -1132,6 +1143,7 @@ struct Batch {
   bool fastq = false;
   string raw;                         // --extract only: the reads' lines as in the file
   vector<RawRec> raw_recs;
+  size_t sample = 0;                  // the sample whose reads these are (streamed sheet runs)
   void clear() { bases.clear(); offs.assign(1, 0); reads.clear(); units.clear(); raw.clear(); raw_recs.clear(); }
 };
 
@@ -1991,23 +2003,30 @@ static bool process_file_parallel(kuq_ctx *ctx0, const char *filename, const cha
 }
 
 // The batches of the inputs, file after file, read one at a time and cut by kuq_batches.h.  A read that closes a batch
-// before itself is held over and starts the next batch.
+// before itself is held over and starts the next batch.  `extract`: the batches keep the reads' lines (--extract).  The
+// merger's stop goes to *pair_error and the messages of a malformed record to *log (NULL: stderr at once).  An input that
+// cannot be opened ends the batches: `fail` is then EX_NOINPUT, with the message in fail_msg.
 struct BatchReader {
   vector<pair<const char *, const char *>> files;
   size_t fi = 0;
-  bool open = false, held = false;
+  bool open = false, held = false, extract;
+  string *pair_error, *log;
+  int fail = 0;
+  string fail_msg;
   InputReader reader;
   BatchCutter cutter;
   Read r;
   BatchCutter::Step step;
   string held_bases, held_raw;
   RawRec rr{0, 0, 0, true};
-  BatchReader(const vector<pair<const char *, const char *>> &f, const BatchLimits &lim) : files(f), cutter(lim) {}
+  BatchReader(const vector<pair<const char *, const char *>> &f, const BatchLimits &lim, bool extract, string *pair_error = &Pair_error,
+              string *log = NULL)
+      : files(f), extract(extract), pair_error(pair_error), log(log), cutter(lim) {}
   void push(Batch &b) {
     b.reads.push_back(r);
     b.offs.push_back(b.bases.size());
     b.units.push_back(step.unit);
-    if (Extract_now) b.raw_recs.push_back(rr);
+    if (extract) b.raw_recs.push_back(rr);
   }
   bool next(Batch &b) {
     b.clear();
@@ -2024,11 +2043,18 @@ struct BatchReader {
     for (; fi < files.size(); fi++) {
       if (!open) {
         reader = InputReader();
-        reader.open(files[fi].first, files[fi].second);
+        reader.single.log = log;
+        reader.pair.error = pair_error;
+        fail_msg = reader.open(files[fi].first, files[fi].second);
+        if (!fail_msg.empty()) {
+          fail = EX_NOINPUT;
+          fi = files.size();
+          return false;
+        }
         open = true;
       }
       b.fastq = reader.fastq();
-      reader.keep_raw(Extract_now ? &b.raw : NULL);
+      reader.keep_raw(extract ? &b.raw : NULL);
       for (;;) {
         const size_t x0 = b.raw.size();
         if (!reader.valid() || !reader.next(r, b.bases)) break;
@@ -2051,7 +2077,7 @@ struct BatchReader {
       b.reads.resize(keep);
       b.offs.resize(keep + 1);
       b.units.resize(keep);
-      if (Extract_now) b.raw_recs.resize(keep);
+      if (extract) b.raw_recs.resize(keep);
       cutter.next_file();
       reader.close();
       open = false;
@@ -2063,7 +2089,7 @@ struct BatchReader {
 
 static void process_file(kuq_ctx *ctx, const char *filename, const char *mate2) {
   if (!getenv("KUQ_SERIAL_INGEST") && process_file_parallel(ctx, filename, mate2)) return;   // plain files: parallel path
-  BatchReader br({{filename, mate2}}, batch_limits(96ull << 20, true, true));
+  BatchReader br({{filename, mate2}}, batch_limits(96ull << 20, true, true), Extract_now);
   Batch batches[2];
   int inflight = -1;
   auto wait_write = [&](int which) {
@@ -2081,8 +2107,169 @@ static void process_file(kuq_ctx *ctx, const char *filename, const char *mate2) 
     if (inflight >= 0) wait_write(inflight);
     inflight = cur;
   }
+  if (br.fail) die(br.fail, br.fail_msg);
   if (inflight >= 0) wait_write(inflight);
   if (kuq_finish(ctx)) die(EX_SOFTWARE, kuq_last_error(ctx));     // work units do not span input files
+}
+
+// ---- one sample's run: begin_sample, the layout's classification of its inputs, end_sample --------------------------
+// The resident and sharded layouts run one sample at a time; the streamed layout calls both from inside its rounds,
+// which may hold the batches of several samples.
+struct SheetRun {
+  vector<Sample> samples;
+  bool sheet = false;
+  TaxDB *tax = NULL;
+  vector<map<uint32_t, uint64_t>> db_counts;     // records per taxid of each database (the .counts files)
+  bool genome_sizes_read = false;
+  int status = 0;
+  struct timeval tv1;
+};
+static SheetRun Run;
+
+// The "classify: sample" line, a clean slate on every context (the staged database(s) serve the next sample), the
+// sample's outputs and its totals
+static void begin_sample(size_t si) {
+  const Sample &sample = Run.samples[si];
+  if (Run.sheet) {
+    cerr << "classify: sample " << sample.name << " (" << si + 1 << " of " << Run.samples.size() << ")" << endl;
+    Sample_label = sample.name;
+    Kraken_output_file = sample.kraken;
+    Report_output_file = sample.report;
+    Classified_output_file = sample.classified;
+    Unclassified_output_file = sample.unclassified;
+    Print_classified = !sample.classified.empty();
+    Print_unclassified = !sample.unclassified.empty();
+    Print_kraken = true;
+  }
+  if (si) {
+    double T0__ = now_s();
+    for (kuq_ctx *c : All_ctx) if (kuq_reset_counts(c)) die(EX_SOFTWARE, kuq_last_error(c));
+    TICK("reset_counts");
+  }
+  total_classified = total_sequences = total_bases = 0;
+  Extract_now = Extract && !sample.extract.empty();
+  Extract_selected = 0;
+  if (Extract_now) Extract_out.open(sample.extract);
+  Translate_now = !sample.translate.empty();
+  Translate_stored.clear();
+  if (Translate_now) Translate_out.open(sample.translate);
+  if (Mpa) {                                                      // the script names a column after its Kraken file
+    Mpa_counts.emplace_back();
+    const string &k = Run.sheet ? sample.kraken : Kraken_output_file;
+    Mpa_ids.push_back(!k.empty() && k != "off" && k != "-" ? k : Run.sheet ? sample.name : "-");
+  }
+  if (Print_classified) Classified_out.open(Classified_output_file);
+  if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);
+  if (!Kraken_output_file.empty()) {
+    if (Kraken_output_file == "off" || Kraken_output_file == "-") Print_kraken = false;   // classify.cpp:233-235
+    else { cerr << "Writing Kraken output to " << Kraken_output_file << endl; Kraken_out.open(Kraken_output_file); }
+  } else {
+    Kraken_out.open("-");
+  }
+  gettimeofday(&Run.tv1, NULL);
+}
+
+// The per-taxon state of every context finished and joined, the stats block, the report, the outputs closed and the
+// merger's stop turned into the exit status
+static void end_sample(size_t si) {
+  const Sample &sample = Run.samples[si];
+  kuq_ctx *ctx = All_ctx[0];
+  for (kuq_ctx *c : All_ctx) if (kuq_finish(c)) die(EX_SOFTWARE, kuq_last_error(c));
+  // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
+  {
+    double T0__ = now_s();
+#ifdef EXACT_COUNTING
+    if (Exact_partitioned) {
+      for (size_t g = 1; g < All_ctx.size(); g++)
+        if (kuq_merge_counters_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+      if (kuq_exact_partition(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
+    }
+#endif
+    for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned; g++)
+      if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+    if (All_ctx.size() > 1) TICK("merge");
+#ifdef EXACT_COUNTING
+    for (size_t g = 0; g < All_ctx.size() && Timing; g++) {
+      uint64_t slots = 0, pairs = 0, grown = 0;
+      if (kuq_exact_info(All_ctx[g], &slots, &pairs, &grown)) die(EX_SOFTWARE, kuq_last_error(All_ctx[g]));
+      fprintf(stderr, "[timing] exact set of context %zu: %llu slots, %llu pairs, grown %llu times\n", g, (unsigned long long)slots,
+              (unsigned long long)pairs, (unsigned long long)grown);
+    }
+#endif
+  }
+  struct timeval tv1 = Run.tv1, tv2;
+  gettimeofday(&tv2, NULL);
+  {                                                                 // report_stats, classify.cpp:361-375
+    double seconds = get_seconds(tv1, tv2);
+    cerr << "\r";
+    fprintf(stderr, "%llu sequences (%.2f Mbp) processed in %.3fs (%.1f Kseq/m, %.2f Mbp/m).\n", total_sequences,
+            total_bases / 1.0e6, seconds, total_sequences / 1.0e3 / (seconds / 60), total_bases / 1.0e6 / (seconds / 60));
+    fprintf(stderr, "  %llu sequences classified (%.2f%%)\n", total_classified, total_classified * 100.0 / total_sequences);
+    fprintf(stderr, "  %llu sequences unclassified (%.2f%%)\n", total_sequences - total_classified,
+            (total_sequences - total_classified) * 100.0 / total_sequences);
+  }
+
+  if (!Report_output_file.empty() && Report_output_file != "off") {
+    gettimeofday(&tv1, NULL);
+    cerr << "Writing report file to " << Report_output_file << "  ..\n";
+    TaxDB &tax = *Run.tax;
+    // the genome sizes are read (and .counts written) once per process, as by the first separate run
+    for (size_t d = 0; d < DB_filenames.size() && !Run.genome_sizes_read; d++) {   // classify.cpp:262-285, once per database
+      const string fname = DB_filenames[d] + ".counts";
+      bool counts_ok = false;
+      {
+        ifstream ifs(fname);
+        if (ifs.good()) {
+          if (ifs.peek() == ifstream::traits_type::eof()) cerr << "Kmer counts file is empty - trying to regenerate ..." << endl;
+          else counts_ok = true;
+        }
+      }
+      if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
+        cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
+        ofstream ofs(fname);
+        for (auto &kv : Run.db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
+      }
+      {
+        cerr << "Reading genome sizes from " << fname << " ...";
+        ifstream in(fname);
+        // readGenomeSizes, taxdb.hpp:868-885, loop kept literally: `while (!eof) { in >> id >> size; set(...) }` counts
+        // the last line of a newline-terminated file twice (the failed extraction leaves the variables unchanged);
+        // the reference's `cov` column depends on it, so the drop-in reproduces it.
+        uint32_t taxid = 0;
+        uint64_t size = 0;
+        while (!in.eof()) {
+          in >> taxid >> size;
+          tax.set_genome_size(taxid, size);
+        }
+        cerr << " done" << endl;
+      }
+    }
+    Run.genome_sizes_read = true;
+    ostringstream rep;
+    double T0__ = now_s();
+    print_report(ctx, tax, rep);
+    TICK("print_report");
+    OutStream ro;
+    ro.open(Report_output_file, true);                              // appended to the wrapper's 2 header lines
+    ro.write(rep.str());
+    ro.close();
+    gettimeofday(&tv2, NULL);
+    fprintf(stderr, "Report finished in %.3f seconds.\n", get_seconds(tv1, tv2));
+  }
+  cerr << "Finishing up ..." << endl;
+  Kraken_out.close();
+  Classified_out.close();
+  Unclassified_out.close();
+  string().swap(Extract_pending);                                  // no read was selected: nothing is written
+  Extract_out.close();
+  Translate_out.close();
+  // the records before the merger's stop are classified and written, like the wrapper's run on its partial output; the
+  // samples after it still run
+  if (!Pair_error.empty()) {
+    cerr << "classify: " << (Run.sheet ? "sample " + sample.name + ": " : "") << Pair_error << endl;
+    Run.status = EX_DATAERR;
+    Pair_error.clear();
+  }
 }
 
 // ---- chunked mode: `-x size` with a database that does not fit (process_file_with_db_chunk, classify.cpp:566-791) --
@@ -2108,7 +2295,7 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 // work units); several take the per-work-unit rule of the preloaded path, which is the reference's rule for `-d a -d b`
 // without -x.  stage_streamed runs once per process: the ranges, the taxids of every record and the pinned registration
 // of the mapped files; it returns the first context that staged a range (a GPU's group may be empty).
-// classify_streamed runs once per sample: its rounds of reads, each through every range.
+// classify_streamed runs once per process: the rounds of reads of every sample, each through every range.
 struct Streamed {
   struct Plan {
     const uint8_t *rec0;
@@ -2122,6 +2309,7 @@ struct Streamed {
   vector<kuq_ctx *> ctxs;
   bool unit_rule = false;
   uint64_t max_rec = 1, max_bins = 1, round_bytes = 0, batch_nt = 1;
+  uint64_t tail_bytes = 0;                                         // a round's batches held past an end of a sample
   vector<const void *> pinned;                                     // registered mappings, unregistered at the end
   vector<uint32_t> open_nt, open_type;                             // per context: what its range buffers are open for
 };
@@ -2184,6 +2372,18 @@ static int stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vec
   vector<uint64_t> free_b;
   for (kuq_ctx *c : ctxs) free_b.push_back(kuq_device_free_bytes(c));
   const uint64_t round_bytes = sm.round_bytes = stream_round_bytes(ctx_devices, free_b, hbm_budget, range_bytes);
+  // An end of a sample in the middle of a round (a sheet run) finds the round's later batches in device memory, where
+  // the end of a separate run finds the range buffers, which every round releases after its lookups.  So the later
+  // batches may take the range buffers' bytes, plus what the budget keeps from every round on the tightest context:
+  // none where the card's free memory limits the round.
+  uint64_t unused = UINT64_MAX;
+  for (size_t g = 0; g < ctx_devices.size(); g++) {
+    uint64_t sharing = 0;
+    for (int d : ctx_devices) sharing += d == ctx_devices[g];
+    const uint64_t share = (free_b[g] > (2ull << 30) ? free_b[g] - (2ull << 30) : 0) / sharing;
+    unused = std::min<uint64_t>(unused, share > hbm_budget ? share - hbm_budget : 0);
+  }
+  sm.tail_bytes = range_bytes + unused;
   // A batch of b bases takes b bytes on every GPU and 4 b more on its owner (batch_shared_bytes / batch_id_bytes), so G
   // batches, one per owner, take about (G + 4) b per GPU: batches of round / (G + 5) bases let a round give every GPU a
   // batch to resolve.  One GPU: round / 6.
@@ -2213,45 +2413,90 @@ static int stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vec
   return g0;
 }
 
-// The rounds on G >= 1 GPUs, each streaming its group of every database's ranges over its own link:
+// The batches of the run's samples, sample after sample, each read by a BatchReader of its own (opened when the reading
+// reaches the sample) and tagged with its sample; a sample without reads yields one batch without reads, so that its turn
+// comes.  Reading runs ahead of the sample being written, so what it finds is kept with the sample and takes effect at
+// the sample's turn: the merger's stop, the messages of a malformed record, an input that cannot be opened (nothing is
+// read after that one).
+struct SampleBatches {
+  struct Found { string pair_error, log, fail_msg; int fail = 0; };
+  const vector<Sample> &samples;
+  BatchLimits lim;
+  vector<Found> found;
+  size_t si = 0;
+  std::unique_ptr<BatchReader> br;
+  bool any = false, stopped = false;
+  SampleBatches(const vector<Sample> &s, const BatchLimits &l) : samples(s), lim(l), found(s.size()) {}
+  bool next(Batch &b) {
+    while (si < samples.size() && !stopped) {
+      if (!br) {
+        br.reset(new BatchReader(files_of(samples[si]), lim, Extract && !samples[si].extract.empty(), &found[si].pair_error, &found[si].log));
+        any = false;
+      }
+      if (br->next(b)) { b.sample = si; any = true; return true; }
+      found[si].fail = br->fail;
+      found[si].fail_msg = br->fail_msg;
+      stopped = br->fail != 0;
+      br.reset();
+      if (!any) { b.clear(); b.sample = si++; return true; }
+      si++;
+    }
+    return false;
+  }
+};
+
+// The rounds on G >= 1 GPUs, each streaming its group of every database's ranges over its own link.  A round holds the
+// batches of one or more samples, in input order:
 //   1. every GPU receives every batch of the round; each batch has one owner (contiguous blocks balanced by bases,
 //      round_peak_bytes; with one GPU, GPU 0 owns every batch), which alone holds the batch's id buffer and zeroes it;
 //   2. host barrier;
 //   3. database by database, in command-line order, one host thread per GPU streams the GPU's group of the database's
 //      ranges through its two range buffers and looks every batch up into the owner's id buffer (a peer pointer when the
 //      owner is another GPU): the first database stores hits only, the later ones fill the windows still empty;
-//   4. host barrier after each database: both slots of every GPU synced, the stream checked;
-//   5. the owners resolve their batches, one in flight per owner, and the results are written in input order.
+//   4. host barrier after each database: both slots of every GPU synced, the stream checked; after the last database
+//      every GPU releases its range buffers (kuq_stream_close) and the next round opens the stream again;
+//   5. the round's batches, in runs of one sample: a later sample's begin_sample at its first batch, the owners resolve the
+//      run's batches, one in flight per owner, the results are written in input order and the batches freed on every
+//      GPU, and the sample's end_sample after its last batch.
+// The lookups write ids only and touch no per-taxon state (no counting in MODE_LOOKUP without shard counting), so a round
+// looks up the batches of samples that have not begun; the resolves, which count, run between the sample's
+// kuq_reset_counts and its end_sample.
 // The barrier of step 4 is what makes KUQ_LOOKUP_FILL_EMPTY correct here: lookup_window_multi reads the owner's word with
 // a plain load, which sees the words other GPUs stored over the peer link only because a host barrier and a kernel
 // boundary separate the two databases' lookups.  The sharded layout orders its phases with device flags and no host
 // barrier, and reads the word with a system-scope load (load_relaxed_sys).  Do not drop this barrier without switching
 // to that load.  With one GPU it costs a host sync per database and round but no overlap: kuq_stream_load makes the
 // next database's first copy wait on the device for every lookup queued before it anyway.
-static void classify_streamed(Streamed &sm, const vector<pair<const char *, const char *>> &files) {
+static void classify_streamed(Streamed &sm) {
   const vector<kuq_ctx *> &ctxs = sm.ctxs;
   const int G = (int)ctxs.size();
   const size_t n_db = sm.plans.size();
   const bool unit_rule = sm.unit_rule;
-  BatchReader input(files, batch_limits(sm.batch_nt, unit_rule, false));
+  const size_t S = Run.samples.size();
+  SampleBatches input(Run.samples, batch_limits(sm.batch_nt, unit_rule, false));
   struct DevBatch { void *bases, *offs, *units; };
   vector<Batch> round;
   Batch pending;
   bool have_pending = false;
-  size_t n_rounds = 0;
+  size_t n_rounds = 0, begun = 1;                                  // begun: samples whose begin_sample ran
+  begin_sample(0);                                                 // the first sample's time includes its first pass
   for (;;) {
     round.clear();
     vector<uint64_t> bases, reads;
+    uint64_t tail = 0;                                             // the batches after the round's first end of a sample
     for (;;) {
       if (!have_pending) have_pending = input.next(pending);
       if (!have_pending) break;
       bases.push_back(pending.bases.size());
       reads.push_back(pending.reads.size());
-      if (!round.empty() && round_peak_bytes(bases, reads, unit_rule, G) > sm.round_bytes) {
+      const bool past_end = !round.empty() && pending.sample != round.front().sample;
+      const uint64_t held = past_end ? batch_shared_bytes(bases.back(), reads.back(), unit_rule) + batch_id_bytes(bases.back()) : 0;
+      if (!round.empty() && (round_peak_bytes(bases, reads, unit_rule, G) > sm.round_bytes || tail + held > sm.tail_bytes)) {
         bases.pop_back();
         reads.pop_back();
         break;
       }
+      tail += held;
       round.push_back(std::move(pending));
       have_pending = false;
     }
@@ -2262,11 +2507,12 @@ static void classify_streamed(Streamed &sm, const vector<pair<const char *, cons
     round_peak_bytes(bases, reads, unit_rule, G, &first);
     vector<int> owner(nb);
     for (int g = 0; g < G; g++) for (size_t bi = first[g]; bi < first[g + 1]; bi++) owner[bi] = g;
-    // 1. (a pageable copy has left the source once it returns)
-    vector<vector<DevBatch>> dev(G, vector<DevBatch>(nb));
-    vector<uint32_t *> ids(nb);
+    // 1. (a pageable copy has left the source once it returns); a batch without reads stands for its sample's turn only
+    vector<vector<DevBatch>> dev(G, vector<DevBatch>(nb, DevBatch{NULL, NULL, NULL}));
+    vector<uint32_t *> ids(nb, NULL);
     for (size_t bi = 0; bi < nb; bi++) {
       const Batch &b = round[bi];
+      if (b.reads.empty()) continue;
       vector<uint64_t> offs(b.offs);
       offs.push_back(offs.back()); offs.push_back(offs.back());
       for (int g = 0; g < G; g++) {
@@ -2323,6 +2569,7 @@ static void classify_streamed(Streamed &sm, const vector<pair<const char *, cons
             if (r + 1 < hi && load((uint32_t)((r + 1 - lo) & 1), r + 1)) return EX_DATAERR;
             for (size_t bi = 0; bi < nb; bi++) {
               const Batch &b = round[bi];
+              if (b.reads.empty()) continue;
               if (kuq_lookup_device(c, (uint32_t)(bi & 1), (const char *)dev[g][bi].bases, (const uint64_t *)dev[g][bi].offs,
                                     (uint32_t)b.reads.size(), b.bases.size(), ids[bi], only_hits))
                 return EX_SOFTWARE;
@@ -2340,27 +2587,64 @@ static void classify_streamed(Streamed &sm, const vector<pair<const char *, cons
                      c + 1, pl.ranges.size());
       }
     }
-    // 5. the owner's next batch is queued before this one is written: the results stay in the slot's host buffers until
-    // the slot's next collect
+    for (int g = 0; g < G; g++) {
+      if (kuq_stream_close(ctxs[g])) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      sm.open_nt[g] = sm.open_type[g] = 0;
+    }
+    // 5. the owner's next batch of the run is queued before this one is written: the results stay in the slot's host
+    // buffers until the slot's next collect
     const double t1 = now_s();
-    vector<size_t> next(first.begin(), first.end() - 1);
-    auto resolve_next = [&](int g) {
-      if (next[g] == first[g + 1]) return;
-      const size_t bi = next[g]++;
-      const Batch &b = round[bi];
-      if (kuq_resolve_device(ctxs[g], 0, (const char *)dev[g][bi].bases, (const uint64_t *)dev[g][bi].offs, (uint32_t)b.reads.size(),
-                             b.bases.size(), ids[bi], (const uint32_t *)dev[g][bi].units, 0))
-        die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-    };
-    for (int g = 0; g < G; g++) resolve_next(g);
-    for (size_t bi = 0; bi < nb; bi++) {
-      const int g = owner[bi];
-      Batch &b = round[bi];
-      kuq_batch_result res;
-      if (kuq_collect_device_batch(ctxs[g], 0, &res)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
-      resolve_next(g);
-      write_reads(b, res, 0, b.reads.size());
-      book_batch(b.reads.size(), b.bases.size(), res.n_classified);
+    for (size_t a = 0; a < nb;) {
+      const size_t si = round[a].sample;
+      size_t e = a;
+      while (e < nb && round[e].sample == si) e++;
+      if (si == begun) { begin_sample(si); begun++; }
+      vector<size_t> next(G), end(G);
+      for (int g = 0; g < G; g++) {
+        next[g] = std::min(std::max(first[g], a), e);
+        end[g] = std::max(std::min(first[g + 1], e), next[g]);
+      }
+      auto resolve_next = [&](int g) {
+        while (next[g] < end[g] && round[next[g]].reads.empty()) next[g]++;
+        if (next[g] == end[g]) return;
+        const size_t bi = next[g]++;
+        const Batch &b = round[bi];
+        if (kuq_resolve_device(ctxs[g], 0, (const char *)dev[g][bi].bases, (const uint64_t *)dev[g][bi].offs, (uint32_t)b.reads.size(),
+                               b.bases.size(), ids[bi], (const uint32_t *)dev[g][bi].units, 0))
+          die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+      };
+      for (int g = 0; g < G; g++) resolve_next(g);
+      for (size_t bi = a; bi < e; bi++) {
+        Batch &b = round[bi];
+        if (b.reads.empty()) continue;
+        const int g = owner[bi];
+        kuq_batch_result res;
+        if (kuq_collect_device_batch(ctxs[g], 0, &res)) die(EX_SOFTWARE, kuq_last_error(ctxs[g]));
+        resolve_next(g);
+        write_reads(b, res, 0, b.reads.size());
+        book_batch(b.reads.size(), b.bases.size(), res.n_classified);
+      }
+      for (size_t bi = a; bi < e; bi++) {
+        for (int g = 0; g < G; g++)
+          for (void *p : {dev[g][bi].bases, dev[g][bi].offs, dev[g][bi].units}) if (p) kuq_device_free(ctxs[g], p);
+        if (ids[bi]) kuq_device_free(ctxs[owner[bi]], ids[bi]);
+        string().swap(round[bi].bases);
+        string().swap(round[bi].raw);
+      }
+      // the sample ends here unless its batches go on in the next round
+      if (e < nb || !have_pending || pending.sample != si) {
+        SampleBatches::Found &f = input.found[si];
+        cerr << f.log;
+        if (f.fail) die(f.fail, f.fail_msg);
+        Pair_error = f.pair_error;
+        if (si + 1 == S && n_db > 1) {
+          string per;
+          for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(sm.plans[d].ranges.size());
+          fprintf(stderr, "\nclassify: %zu databases streamed: %zu rounds, ranges per database %s\n", n_db, n_rounds, per.c_str());
+        }
+        end_sample(si);
+      }
+      a = e;
     }
     if (Timing) {
       string per;
@@ -2371,17 +2655,8 @@ static void classify_streamed(Streamed &sm, const vector<pair<const char *, cons
       }
       fprintf(stderr, "\n[timing] streamed round %zu: stream per GPU %s; resolve %.3f s\n", n_rounds, per.c_str(), now_s() - t1);
     }
-    for (int g = 0; g < G; g++)
-      for (size_t bi = 0; bi < nb; bi++)
-        for (void *p : {dev[g][bi].bases, dev[g][bi].offs, dev[g][bi].units}) if (p) kuq_device_free(ctxs[g], p);
-    for (size_t bi = 0; bi < nb; bi++) kuq_device_free(ctxs[owner[bi]], ids[bi]);
   }
-  for (kuq_ctx *c : ctxs) if (kuq_finish(c)) die(EX_SOFTWARE, kuq_last_error(c));
-  if (n_db > 1) {
-    string per;
-    for (size_t d = 0; d < n_db; d++) per += (d ? "/" : "") + std::to_string(sm.plans[d].ranges.size());
-    fprintf(stderr, "\nclassify: %zu databases streamed: %zu rounds, ranges per database %s\n", n_db, n_rounds, per.c_str());
-  }
+  if (Run.sheet) fprintf(stderr, "classify: %zu samples streamed in %zu rounds\n", S, n_rounds);
 }
 
 // ---- databases that fit the GPUs of the node together but not one of them: minimizer-range shards (SURVEY §8(e).2) --
@@ -2401,8 +2676,9 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
   const uint64_t R = n_phases;
   vector<Batch> batches;
   {
-    BatchReader input(files, batch_limits(96ull << 20, true, false));
+    BatchReader input(files, batch_limits(96ull << 20, true, false), Extract_now);
     for (Batch b; input.next(b);) batches.push_back(std::move(b));
+    if (input.fail) die(input.fail, input.fail_msg);
   }
   uint64_t max_bases = 64, max_reads = 4;
   for (auto &b : batches) { max_bases = std::max<uint64_t>(max_bases, b.bases.size()); max_reads = std::max<uint64_t>(max_reads, b.reads.size()); }
@@ -2831,146 +3107,18 @@ int main(int argc, char **argv) {
     Exact_partitioned = All_ctx.size() > 1 && !(z != tax.idx.end() && !tax.e[z->second].children.empty());
   }
 #endif
-  bool genome_sizes_read = false;
-  int status = 0;
-  for (size_t si = 0; si < samples.size(); si++) {
-    const Sample &sample = samples[si];
-    if (sheet) {
-      cerr << "classify: sample " << sample.name << " (" << si + 1 << " of " << samples.size() << ")" << endl;
-      Sample_label = sample.name;
-      Kraken_output_file = sample.kraken;
-      Report_output_file = sample.report;
-      Classified_output_file = sample.classified;
-      Unclassified_output_file = sample.unclassified;
-      Print_classified = !sample.classified.empty();
-      Print_unclassified = !sample.unclassified.empty();
-      Print_kraken = true;
-    }
-    if (si) {                                                       // the staged database(s) serve the next sample
-      double T0__ = now_s();
-      for (kuq_ctx *c : All_ctx) if (kuq_reset_counts(c)) die(EX_SOFTWARE, kuq_last_error(c));
-      TICK("reset_counts");
-    }
-    total_classified = total_sequences = total_bases = 0;
-    Extract_now = Extract && !sample.extract.empty();
-    Extract_selected = 0;
-    if (Extract_now) Extract_out.open(sample.extract);
-    Translate_now = !sample.translate.empty();
-    Translate_stored.clear();
-    if (Translate_now) Translate_out.open(sample.translate);
-    if (Mpa) {                                                      // the script names a column after its Kraken file
-      Mpa_counts.emplace_back();
-      const string &k = sheet ? sample.kraken : Kraken_output_file;
-      Mpa_ids.push_back(!k.empty() && k != "off" && k != "-" ? k : sheet ? sample.name : "-");
-    }
-    if (Print_classified) Classified_out.open(Classified_output_file);
-    if (Print_unclassified) Unclassified_out.open(Unclassified_output_file);
-    if (!Kraken_output_file.empty()) {
-      if (Kraken_output_file == "off" || Kraken_output_file == "-") Print_kraken = false;   // classify.cpp:233-235
-      else { cerr << "Writing Kraken output to " << Kraken_output_file << endl; Kraken_out.open(Kraken_output_file); }
-    } else {
-      Kraken_out.open("-");
-    }
-
-    struct timeval tv1, tv2;
-    gettimeofday(&tv1, NULL);
-    const vector<pair<const char *, const char *>> files = files_of(sample);
+  Run.samples = samples;
+  Run.sheet = sheet;
+  Run.tax = &tax;
+  Run.db_counts = db_counts;
+  // the streamed layout shares its passes over the database(s) among the samples: it runs every sample's lifecycle
+  if (chunk_budget) classify_streamed(streamed);
+  for (size_t si = 0; si < Run.samples.size() && !chunk_budget; si++) {
+    begin_sample(si);
+    const vector<pair<const char *, const char *>> files = files_of(Run.samples[si]);
     if (want_shards) shard_loop(All_ctx, shard_runs, n_db > 1, files);
-    else if (chunk_budget) classify_streamed(streamed, files);
     else for (auto &in : files) process_file(ctx, in.first, in.second);
-    // the other devices' per-taxon state joins the first one's (classify.cpp:542-544 across GPUs)
-    {
-      double T0__ = now_s();
-#ifdef EXACT_COUNTING
-      if (Exact_partitioned) {
-        for (size_t g = 1; g < All_ctx.size(); g++)
-          if (kuq_merge_counters_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
-        if (kuq_exact_partition(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
-      }
-#endif
-      for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned; g++)
-        if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
-      if (All_ctx.size() > 1) TICK("merge");
-#ifdef EXACT_COUNTING
-      for (size_t g = 0; g < All_ctx.size() && Timing; g++) {
-        uint64_t slots = 0, pairs = 0, grown = 0;
-        if (kuq_exact_info(All_ctx[g], &slots, &pairs, &grown)) die(EX_SOFTWARE, kuq_last_error(All_ctx[g]));
-        fprintf(stderr, "[timing] exact set of context %zu: %llu slots, %llu pairs, grown %llu times\n", g, (unsigned long long)slots,
-                (unsigned long long)pairs, (unsigned long long)grown);
-      }
-#endif
-    }
-    gettimeofday(&tv2, NULL);
-    {                                                                 // report_stats, classify.cpp:361-375
-      double seconds = get_seconds(tv1, tv2);
-      cerr << "\r";
-      fprintf(stderr, "%llu sequences (%.2f Mbp) processed in %.3fs (%.1f Kseq/m, %.2f Mbp/m).\n", total_sequences,
-              total_bases / 1.0e6, seconds, total_sequences / 1.0e3 / (seconds / 60), total_bases / 1.0e6 / (seconds / 60));
-      fprintf(stderr, "  %llu sequences classified (%.2f%%)\n", total_classified, total_classified * 100.0 / total_sequences);
-      fprintf(stderr, "  %llu sequences unclassified (%.2f%%)\n", total_sequences - total_classified,
-              (total_sequences - total_classified) * 100.0 / total_sequences);
-    }
-
-    if (!Report_output_file.empty() && Report_output_file != "off") {
-      gettimeofday(&tv1, NULL);
-      cerr << "Writing report file to " << Report_output_file << "  ..\n";
-      // the genome sizes are read (and .counts written) once per process, as by the first separate run
-      for (size_t d = 0; d < n_db && !genome_sizes_read; d++) {     // classify.cpp:262-285, once per database
-        const string fname = DB_filenames[d] + ".counts";
-        bool counts_ok = false;
-        {
-          ifstream ifs(fname);
-          if (ifs.good()) {
-            if (ifs.peek() == ifstream::traits_type::eof()) cerr << "Kmer counts file is empty - trying to regenerate ..." << endl;
-            else counts_ok = true;
-          }
-        }
-        if (!counts_ok) {                                               // classify.cpp:275-284 via kuq_db_taxids
-          cerr << "Writing kmer counts to " << fname << "... [only once for this database, may take a while] " << endl;
-          ofstream ofs(fname);
-          for (auto &kv : db_counts[d]) ofs << kv.first << '\t' << kv.second << '\n';
-        }
-        {
-          cerr << "Reading genome sizes from " << fname << " ...";
-          ifstream in(fname);
-          // readGenomeSizes, taxdb.hpp:868-885, loop kept literally: `while (!eof) { in >> id >> size; set(...) }` counts
-          // the last line of a newline-terminated file twice (the failed extraction leaves the variables unchanged);
-          // the reference's `cov` column depends on it, so the drop-in reproduces it.
-          uint32_t taxid = 0;
-          uint64_t size = 0;
-          while (!in.eof()) {
-            in >> taxid >> size;
-            tax.set_genome_size(taxid, size);
-          }
-          cerr << " done" << endl;
-        }
-      }
-      genome_sizes_read = true;
-      ostringstream rep;
-      double T0__ = now_s();
-      print_report(ctx, tax, rep);
-      TICK("print_report");
-      OutStream ro;
-      ro.open(Report_output_file, true);                              // appended to the wrapper's 2 header lines
-      ro.write(rep.str());
-      ro.close();
-      gettimeofday(&tv2, NULL);
-      fprintf(stderr, "Report finished in %.3f seconds.\n", get_seconds(tv1, tv2));
-    }
-    cerr << "Finishing up ..." << endl;
-    Kraken_out.close();
-    Classified_out.close();
-    Unclassified_out.close();
-    string().swap(Extract_pending);                                  // no read was selected: nothing is written
-    Extract_out.close();
-    Translate_out.close();
-    // the records before the merger's stop are classified and written, like the wrapper's run on its partial output; the
-    // samples after it still run
-    if (!Pair_error.empty()) {
-      cerr << "classify: " << (sheet ? "sample " + sample.name + ": " : "") << Pair_error << endl;
-      status = EX_DATAERR;
-      Pair_error.clear();
-    }
+    end_sample(si);
   }
   Sample_label.clear();
   if (Mpa) {                                                        // one table for every sample of the run
@@ -2981,5 +3129,5 @@ int main(int argc, char **argv) {
   }
   for (const void *p : streamed.pinned) kuq_host_unregister((void *)p);
   for (kuq_ctx *c : All_ctx) kuq_destroy(c);
-  return status;
+  return Run.status;
 }

@@ -3124,6 +3124,7 @@ int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64
                 (unsigned long long)(bin_hi - bin_lo));
   CU(cudaSetDevice(ctx->device));
   kuq_ctx::StreamBuf &b = ctx->sbuf[buf];
+  if (!b.d_pairs) return fail(ctx, KUQ_E_STATE, "the range buffers were released (kuq_stream_close): kuq_stream_open first");
   // whoever still reads this buffer was queued before this call: the copy waits for the slots' streams as they stand
   if (ctx->seen_dirty) { int hrc = harvest_seen(ctx, false); if (hrc) return hrc; }
   for (auto &s : ctx->slots) {
@@ -3162,6 +3163,20 @@ int kuq_stream_use(kuq_ctx *ctx, uint32_t buf) {
   for (auto &s : ctx->slots) CU(cudaStreamWaitEvent(s.stream, b.ready, 0));
   ctx->d_pairs = b.d_pairs; ctx->d_offsets = b.d_offsets;
   ctx->key_ct = b.key_ct; ctx->rec_base = b.rec_base; ctx->bin_lo = b.bin_lo; ctx->bin_hi = b.bin_hi;
+  return KUQ_OK;
+}
+
+int kuq_stream_close(kuq_ctx *ctx) {
+  if (!ctx) return KUQ_E_INVALID_ARG;
+  if (!ctx->stream_open) return KUQ_OK;
+  CU(cudaSetDevice(ctx->device));
+  for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));   // the lookups that read the buffers
+  CU(cudaStreamSynchronize(ctx->copy_stream));
+  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }  // flags in the records go before the records do
+  for (auto &b : ctx->sbuf) b = kuq_ctx::StreamBuf();
+  ctx->d_stream_land.reset();
+  ctx->d_pairs = nullptr; ctx->d_offsets = nullptr;
+  ctx->key_ct = 0;
   return KUQ_OK;
 }
 
