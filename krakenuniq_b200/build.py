@@ -13,7 +13,7 @@ LIB = os.path.join(PKG, "lib", "libkuq.so")
 SOURCES = ["kuq_kernels.cu", "kuq_api.cu", "kuq_dbbuild.cu", "kuq_microbench.cu", "kuq_layout_exp.cu", "kuq_clades.cu",
            "kuq_collisions.cu", "kuq_kmerset.cu", "kuq_countunique.cu"]
 HEADERS = ["kuq_kernels.cuh", "kuq_buffers.cuh", "kuq_minimizer.cuh", "kuq_bounce.cuh", "kuq_ranges.h", "kuq_batches.h",
-           "kuq_kmerpack.cuh",
+           "kuq_kmerpack.cuh", "kuq_dbfile.h",
            os.path.join(ROOT, "include", "kuq.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--compiler-bindir", "/usr/bin/g++", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared", "-cudart", "shared"]
@@ -58,7 +58,7 @@ def build_classify(force: bool = False) -> str:
     src = os.path.join(CSRC, "classify_main.cpp")
     build(force=force)
     exact = CLASSIFY + "Exact"
-    newest = max(os.path.getmtime(p) for p in (src, LIB, os.path.join(CSRC, "kuq_batches.h"), os.path.join(CSRC, "kuq_ranges.h")))
+    newest = max(os.path.getmtime(p) for p in [src, LIB] + [os.path.join(CSRC, h) for h in ("kuq_batches.h", "kuq_ranges.h", "kuq_dbfile.h")])
     if not force and all(os.path.exists(x) and os.path.getmtime(x) >= newest for x in (CLASSIFY, exact)):
         return CLASSIFY
     os.makedirs(os.path.dirname(CLASSIFY), exist_ok=True)
@@ -86,7 +86,8 @@ def build_dbtools(force: bool = False):
             (os.path.join(PKG, "bin", "set_lcas"), src, ["-DTOOL_SET_LCAS"], []),
             (KMER_SET, os.path.join(CSRC, "kmerset_main.cpp"), [], []),
             (COUNT_UNIQUE, os.path.join(CSRC, "countunique_main.cpp"), [], ["-lz"])]
-    newest = max([os.path.getmtime(s) for _, s, _, _ in outs] + [os.path.getmtime(LIB)])
+    newest = max([os.path.getmtime(s) for _, s, _, _ in outs] + [os.path.getmtime(LIB)] +
+                 [os.path.getmtime(os.path.join(CSRC, h)) for h in ("kuq_ranges.h", "kuq_dbfile.h")])
     if not force and all(os.path.exists(o) and os.path.getmtime(o) >= newest for o, _, _, _ in outs):
         return [o for o, _, _, _ in outs[:2]]
     os.makedirs(os.path.join(PKG, "bin"), exist_ok=True)

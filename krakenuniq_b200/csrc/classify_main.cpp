@@ -58,6 +58,7 @@
 
 #include "../../include/kuq.h"
 #include "kuq_batches.h"
+#include "kuq_dbfile.h"
 #include "kuq_ranges.h"
 
 using namespace std;
@@ -2298,10 +2299,7 @@ static vector<pair<uint64_t, uint64_t>> plan_ranges(const uint64_t *offsets, uin
 // classify_streamed runs once per process: the rounds of reads of every sample, each through every range.
 struct Streamed {
   struct Plan {
-    const uint8_t *rec0;
-    const uint64_t *offsets;
-    uint64_t pair_sz;
-    uint32_t k, nt, idx_type;
+    DbFile f;
     vector<pair<uint64_t, uint64_t>> ranges;
     vector<size_t> group;                                          // GPU g streams ranges [group[g], group[g + 1])
   };
@@ -2315,7 +2313,7 @@ struct Streamed {
 };
 
 static int stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vector<int> &ctx_devices, const vector<Mapped> &kdbs,
-                          const vector<Mapped> &idxs, uint64_t range_budget, uint64_t hbm_budget,
+                          const vector<Mapped> &idxs, const vector<DbFile> &files, uint64_t range_budget, uint64_t hbm_budget,
                           vector<map<uint32_t, uint64_t>> &db_counts) {
   const size_t n_db = kdbs.size();
   const int G = (int)ctxs.size();
@@ -2328,19 +2326,11 @@ static int stage_streamed(Streamed &sm, const vector<kuq_ctx *> &ctxs, const vec
   uint64_t &max_rec = sm.max_rec, &max_bins = sm.max_bins;
   for (size_t d = 0; d < n_db; d++) {
     Streamed::Plan &pl = plans[d];
-    const uint8_t *q = (const uint8_t *)idxs[d].p;
-    uint64_t key_bits;
-    memcpy(&key_bits, (const uint8_t *)kdbs[d].p + 8, 8);
-    pl.k = (uint32_t)(key_bits / 2);
-    pl.nt = q[7];
-    pl.idx_type = memcmp(q, "KRAKIDX", 7) == 0 ? 1 : 2;
-    pl.pair_sz = (key_bits + 7) / 8 + 4;                          // the file's record size (12 B only for k = 29..31)
-    pl.rec0 = (const uint8_t *)kdbs[d].p + 72 + 2 * (4 + 8 * key_bits);
-    pl.offsets = (const uint64_t *)(q + 8);
-    pl.ranges = plan_ranges(pl.offsets, 1ull << (2 * pl.nt), range_budget);
-    pl.group = group_ranges(pl.offsets, pl.ranges, G, 12);
+    pl.f = files[d];
+    pl.ranges = plan_ranges(pl.f.offsets, pl.f.n_bins, range_budget);
+    pl.group = group_ranges(pl.f.offsets, pl.ranges, G, 12);
     for (auto &rg : pl.ranges) {
-      max_rec = std::max<uint64_t>(max_rec, pl.offsets[rg.second] - pl.offsets[rg.first]);
+      max_rec = std::max<uint64_t>(max_rec, pl.f.offsets[rg.second] - pl.f.offsets[rg.first]);
       max_bins = std::max<uint64_t>(max_bins, rg.second - rg.first);
     }
   }
@@ -2551,16 +2541,17 @@ static void classify_streamed(Streamed &sm) {
         const size_t lo = pl.group[g], hi = pl.group[g + 1];
         auto part = [&]() -> int {
           // every context opens the stream, an empty group too: the open numbers the taxa, which its resolves need
-          if (pl.nt != sm.open_nt[g] || pl.idx_type != sm.open_type[g]) {
-            if ((sm.open_nt[g] && kuq_stream_check(c)) || kuq_stream_open(c, pl.k, pl.nt, pl.idx_type, sm.max_rec, sm.max_bins))
+          const DbFile &f = pl.f;
+          if (f.nt != sm.open_nt[g] || f.idx_type != sm.open_type[g]) {
+            if ((sm.open_nt[g] && kuq_stream_check(c)) || kuq_stream_open(c, f.k, f.nt, f.idx_type, sm.max_rec, sm.max_bins))
               return EX_DATAERR;
-            sm.open_nt[g] = pl.nt;
-            sm.open_type[g] = pl.idx_type;
+            sm.open_nt[g] = f.nt;
+            sm.open_type[g] = f.idx_type;
           }
           if (lo == hi) return 0;
           auto load = [&](uint32_t buf, size_t r) {
             const uint64_t blo = pl.ranges[r].first, bhi = pl.ranges[r].second;
-            return kuq_stream_load(c, buf, pl.rec0 + pl.offsets[blo] * pl.pair_sz, pl.offsets[bhi] - pl.offsets[blo], pl.offsets + blo,
+            return kuq_stream_load(c, buf, f.records + f.offsets[blo] * f.pair_sz, f.offsets[bhi] - f.offsets[blo], f.offsets + blo,
                                    blo, bhi);
           };
           if (load(0, lo)) return EX_DATAERR;
@@ -2786,20 +2777,15 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
   }
 }
 
-static ShardDb shard_db(const Mapped &idx) {
-  const uint8_t *q = (const uint8_t *)idx.p;
-  return ShardDb{(const uint64_t *)(q + 8), q[7], memcmp(q, "KRAKIDX", 7) == 0 ? 1u : 2u};
-}
-
 // Staging, once per process: every GPU stages, in command-line order, the bins of its range of each database's run (a
 // range of several databases may be empty).  One database is one run, with a non-empty range on every GPU, and the GPU
 // that finds a hit counts it (kuq_set_shard_counting).  Returns the runs: shard_loop's lookup phases.
 static uint32_t stage_shards(const vector<kuq_ctx *> &ctxs, const vector<Mapped> &kdbs, const vector<Mapped> &idxs,
-                             vector<map<uint32_t, uint64_t>> &db_counts) {
+                             const vector<DbFile> &files, vector<map<uint32_t, uint64_t>> &db_counts) {
   const int G = (int)ctxs.size();
   const size_t n_db = kdbs.size();
   vector<ShardDb> sd;
-  for (auto &m : idxs) sd.push_back(shard_db(m));
+  for (const DbFile &f : files) sd.push_back(ShardDb{f.offsets, f.nt, f.idx_type});
   const vector<ShardRun> runs = plan_shards(sd, G);
   if (n_db == 1) {
     cerr << "Database sharded over " << G << " GPUs by minimizer range" << endl;
@@ -2813,7 +2799,7 @@ static uint32_t stage_shards(const vector<kuq_ctx *> &ctxs, const vector<Mapped>
     for (const ShardRun &run : runs)
       for (size_t d = run.first; d < run.end; d++) {
         uint64_t lo = run.cut[g], hi = run.cut[g + 1];
-        if (lo == hi) lo = hi = 1ull << (2 * sd[d].nt);             // an empty slice
+        if (lo == hi) lo = hi = files[d].n_bins;                     // an empty slice
         slices[g].push_back(Slice{d, lo, hi});
       }
   stage_slices(ctxs, kdbs, idxs, slices, true, false, db_counts);
@@ -2828,11 +2814,7 @@ static uint32_t stage_shards(const vector<kuq_ctx *> &ctxs, const vector<Mapped>
 
 // What a staged database takes in HBM: 12 bytes per record whatever the file's record size (records of k <= 28 databases
 // are widened on the way in), plus the index.  Every decision about what fits a card counts these bytes, not the file's.
-static uint64_t hbm_bytes(const Mapped &kdb, const Mapped &idx) {
-  uint64_t key_ct = 0;
-  if (kdb.size >= 56) memcpy(&key_ct, (const uint8_t *)kdb.p + 48, 8);
-  return key_ct * 12 + idx.size;
-}
+static uint64_t hbm_bytes(const DbFile &f, const Mapped &idx) { return f.key_ct * 12 + idx.size; }
 
 static uint32_t extract_flags() {
   return (Extract_subtree ? KUQ_EXTRACT_SUBTREE : 0) | (Extract_invert ? KUQ_EXTRACT_INVERT : 0) |
@@ -2952,15 +2934,17 @@ int main(int argc, char **argv) {
   if (Extract) check_extract(samples, tax, tax_read);
   if (Populate_memory && Populate_memory_size == 0) cerr << "Loading database(s)... " << endl;
   vector<Mapped> kdbs(n_db), idxs(n_db);
+  vector<DbFile> files(n_db);                                      // every database is checked before a device is touched
   for (size_t i = 0; i < n_db; i++) {
     cerr << " Database " << DB_filenames[i] << endl;
     kdbs[i].open(DB_filenames[i]);
     idxs[i].open(Index_filenames[i]);
+    string err;
+    if (parse_db(kdbs[i].p, kdbs[i].size, idxs[i].p, idxs[i].size, files[i], err)) die(EX_DATAERR, err);
   }
   for (size_t i = 1; i < n_db; i++) {                               // classify.cpp:203-210
-    auto k_of = [](const Mapped &m) { return m.size >= 16 ? (int)(((const uint64_t *)m.p)[1] / 2) : 0; };
-    if (k_of(kdbs[i]) != k_of(kdbs[0])) {
-      fprintf(stderr, "Different k-mer sizes in databases 1 and %zu: %i vs %i!\n", i + 1, k_of(kdbs[0]), k_of(kdbs[i]));
+    if (files[i].k != files[0].k) {
+      fprintf(stderr, "Different k-mer sizes in databases 1 and %zu: %i vs %i!\n", i + 1, (int)files[0].k, (int)files[i].k);
       exit(1);
     }
   }
@@ -2982,7 +2966,7 @@ int main(int argc, char **argv) {
   // resident.
   bool want_shards = false;
   uint64_t all_hbm = 0;
-  for (size_t i = 0; i < n_db; i++) all_hbm += hbm_bytes(kdbs[i], idxs[i]);
+  for (size_t i = 0; i < n_db; i++) all_hbm += hbm_bytes(files[i], idxs[i]);
   if (all_hbm > hbm_budget || getenv("KUQ_FORCE_SHARDS")) {
     int n_vis = 0;
     if (const char *dl = getenv("KUQ_DEVICES")) { if (strcmp(dl, "all") == 0) n_vis = kuq_device_count(); else { n_vis = 1; for (const char *c = dl; *c; c++) n_vis += *c == ','; } }
@@ -3088,8 +3072,8 @@ int main(int argc, char **argv) {
   Streamed streamed;
   uint32_t shard_runs = 0;
   int g0 = 0;                                                       // the first context that staged a slice
-  if (want_shards) shard_runs = stage_shards(All_ctx, kdbs, idxs, db_counts);
-  else if (chunk_budget) g0 = stage_streamed(streamed, All_ctx, ctx_devices, kdbs, idxs, chunk_budget, hbm_budget, db_counts);
+  if (want_shards) shard_runs = stage_shards(All_ctx, kdbs, idxs, files, db_counts);
+  else if (chunk_budget) g0 = stage_streamed(streamed, All_ctx, ctx_devices, kdbs, idxs, files, chunk_budget, hbm_budget, db_counts);
   // the per-work-unit rule (resident without -x, and several databases in every layout); kuq_unit_table_rows finalizes
   // the context, so it comes after the taxonomy and the taxid universe
   if (want_shards || chunk_budget ? n_db > 1 : cfg.hll_mode == KUQ_HLL_PRELOAD) {

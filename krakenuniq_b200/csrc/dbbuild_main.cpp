@@ -30,6 +30,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_dbfile.h"
 #include "kuq_ranges.h"
 
 using namespace std;
@@ -120,11 +121,8 @@ int main(int argc, char **argv) {
   Mapped in;
   in.open(input, TOOL);
   if (in.size < 56) die(EX_DATAERR, "input database too short", TOOL);
-  uint64_t key_bits, key_ct;
-  memcpy(&key_bits, (const char *)in.p + 8, 8);
-  memcpy(&key_ct, (const char *)in.p + 48, 8);
-  const uint64_t key_len = key_bits / 8 + !!(key_bits % 8), header = 72 + 2 * (4 + 8 * key_bits);
-  vector<char> kdb(header + key_ct * (key_len + 4)), idx(8 + 8 * ((1ull << (2 * nt)) + 1));
+  const KdbFile h = kdb_view(in.p);
+  vector<char> kdb(h.header_bytes + h.key_ct * h.pair_sz), idx(8 + 8 * ((1ull << (2 * nt)) + 1));
   cerr << "db_sort: Sorting ...";
   char err[512] = "";
   const vector<int> devices = pick_devices();
@@ -403,24 +401,15 @@ static unordered_map<string, uint32_t> read_seqid_map(const string &path) {
 
 // The minimizer ranges of the database, each staged on one context at a time: as few as `budget` bytes of device
 // memory allow, 12 bytes per record in HBM.  Together they cover every bin, so that a k-mer whose bin holds no records
-// is still counted as missing.  {(0, 0)} = the whole database at once; so is an index that does not parse (kuq_stage_db
-// reports it).
-static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const Mapped &kdb, const Mapped &idx, uint64_t budget) {
+// is still counted as missing.  {(0, 0)} = the whole database at once.
+static vector<pair<uint64_t, uint64_t>> plan_lca_ranges(const DbFile &f, uint64_t budget) {
   const vector<pair<uint64_t, uint64_t>> whole{{0, 0}};
-  const uint8_t *q = (const uint8_t *)idx.p;
-  if (idx.size < 8 || kdb.size < 56) return whole;
-  const uint32_t nt = q[7];
-  const uint64_t n_bins = 1ull << (2 * (nt & 15));
-  uint64_t key_ct;
-  memcpy(&key_ct, (const char *)kdb.p + 48, 8);
-  const uint64_t *offsets = (const uint64_t *)(q + 8);
-  if (nt < 1 || nt > 15 || idx.size < 8 + 8 * (n_bins + 1) || offsets[n_bins] > key_ct) return whole;
   vector<pair<uint64_t, uint64_t>> ranges;
-  if (!plan_ranges(offsets, n_bins, budget, 12, ranges)) die(EX_SOFTWARE, "a single minimizer bin exceeds KUQ_SET_LCAS_BUDGET", TOOL);
+  if (!plan_ranges(f.offsets, f.n_bins, budget, 12, ranges)) die(EX_SOFTWARE, "a single minimizer bin exceeds KUQ_SET_LCAS_BUDGET", TOOL);
   if (ranges.size() <= 1) return whole;
   ranges.front().first = 0;                              // bins of ranges without records join the range before them
   for (size_t r = 1; r < ranges.size(); r++) ranges[r - 1].second = ranges[r].first;
-  ranges.back().second = n_bins;
+  ranges.back().second = f.n_bins;
   return ranges;
 }
 
@@ -498,24 +487,24 @@ int main(int argc, char **argv) {
   Mapped kdb, idx;
   kdb.open(DB_filename, TOOL);
   idx.open(Index_filename, TOOL);
-  if (kdb.size < 56) die(EX_DATAERR, "database too short", TOOL);
-  uint64_t key_bits;
-  memcpy(&key_bits, (const char *)kdb.p + 8, 8);
-  K = (uint32_t)(key_bits / 2);
+  DbFile file;
+  string parse_err;
+  if (parse_db(kdb.p, kdb.size, idx.p, idx.size, file, parse_err)) die(EX_DATAERR, parse_err, TOOL);
+  K = file.k;
   // the range plan: from KUQ_SET_LCAS_BUDGET, else from the first device's free memory; when the database takes more
   // than one range and there are more devices, every context's share of its device (the smallest share of all)
   const vector<int> devices = pick_devices();
   const char *budget_env = getenv("KUQ_SET_LCAS_BUDGET");
   const uint64_t given = budget_env ? strtoull(budget_env, NULL, 10) : 0;
   vector<kuq_ctx *> made{create_context(devices[0])};
-  vector<pair<uint64_t, uint64_t>> ranges = plan_lca_ranges(kdb, idx, given ? given : default_budget(made[0], 1));
+  vector<pair<uint64_t, uint64_t>> ranges = plan_lca_ranges(file, given ? given : default_budget(made[0], 1));
   if (ranges.size() > 1 && devices.size() > 1) {
     for (size_t g = 1; g < devices.size(); g++) made.push_back(create_context(devices[g]));
     if (!given) {
       uint64_t budget = UINT64_MAX;
       for (size_t g = 0; g < devices.size(); g++)
         budget = min(budget, default_budget(made[g], (uint32_t)count(devices.begin(), devices.end(), devices[g])));
-      ranges = plan_lca_ranges(kdb, idx, budget);
+      ranges = plan_lca_ranges(file, budget);
     }
   }
   // one range per context while there are enough contexts (the library is then never kept), else contiguous groups

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/kuq.h"
+#include "kuq_dbfile.h"
 
 using namespace std;
 
@@ -174,8 +175,8 @@ int main(int argc, char **argv) {
   const double input_s = chrono::duration<double>(chrono::steady_clock::now() - t1).count();
 
   // header (SURVEY App. A16): JFLISTDN, key_bits = 2k, val_len = 4, key_ct at byte 48, every other byte zero
-  const uint64_t key_bits = 2 * (uint64_t)k, key_len = (key_bits + 7) / 8, rec = key_len + 4;
-  vector<char> header(72 + 2 * (4 + 8 * key_bits), 0);
+  const uint64_t key_bits = 2 * (uint64_t)k, key_len = kdb_key_len(key_bits), rec = key_len + 4;
+  vector<char> header(kdb_header_bytes(key_bits), 0);
   memcpy(header.data(), "JFLISTDN", 8);
   const uint64_t val_len = 4;
   memcpy(header.data() + 8, &key_bits, 8);

@@ -2,7 +2,7 @@
 //
 // Owns HBM (database range, taxonomy arrays, per-taxon state), the batch slots (stream + device and pinned
 // host staging) and the host-side pieces of the path that are not data parallel: database header validation
-// (krakendb.cpp:60-78,534-544), dense taxon numbering, work-unit cutting (classify.cpp:514-520) and the
+// (kuq_dbfile.h), dense taxon numbering, work-unit cutting (classify.cpp:514-520) and the
 // double-precision Ertl estimator (hyperloglogplus.cpp:722-753).  There is no CPU classification path: without
 // an sm_90 device kuq_create fails with KUQ_E_NO_DEVICE.
 #include <algorithm>
@@ -22,6 +22,7 @@
 #include "../../include/kuq.h"
 #include "kuq_batches.h"
 #include "kuq_bounce.cuh"
+#include "kuq_dbfile.h"
 #include "kuq_kernels.cuh"
 
 using namespace kuq;
@@ -101,6 +102,29 @@ struct CountsHost {
   std::vector<unsigned long long> exact;   // KUQ_HLL_EXACT: [n_sketch] distinct k-mers per taxon
 };
 
+// The DbView inputs of one staged minimizer range: its records (12-byte layout) and index slice on the device
+struct DbRange {
+  uint8_t *pairs = nullptr;
+  const uint64_t *offsets = nullptr;
+  uint64_t key_ct = 0, rec_base = 0, bin_lo = 0, bin_hi = 0;
+  uint32_t nt = 0, idx_type = 0;
+};
+
+// One staged database or minimizer range of one.  Its records are owned here when they were staged from a host image
+// (own_pairs), else they are the caller's (kuq_attach_db_device) or a stream buffer's.
+struct StagedDb {
+  DbRange range;
+  DevBuf<uint8_t> own_pairs;
+  DevBuf<uint64_t> own_offsets;
+  // device hash of the range's taxids (keys = taxid + 1), and the distinct taxids (ascending) with their record counts
+  DevBuf<uint32_t> d_tx_keys, d_tx_dense;
+  DevBuf<unsigned long long> d_tx_counts;
+  uint32_t tx_cap = 0;
+  std::vector<uint32_t> taxids;
+  std::vector<uint64_t> counts;
+  bool remapped = false;                  // the record values are dense ids
+};
+
 struct kuq_ctx {
   kuq_config cfg;
   CountsHost snap;                 // host copy of the per-taxon state, valid until the next batch
@@ -112,38 +136,11 @@ struct kuq_ctx {
   uint64_t launches = 0;
   Stream aux;
 
-  // database: d_pairs / d_offsets are the records in use, owned here (db_owned), by the caller
-  // (kuq_attach_db_device) or by a stream buffer
-  bool db_owned = false;
-  uint8_t *d_pairs = nullptr;
-  DevBuf<uint8_t> d_pairs_owned;
-  DevBuf<uint64_t> d_offsets_owned;
-  const uint64_t *d_offsets = nullptr;
-  uint64_t key_ct = 0, rec_base = 0;
-  uint32_t k = 0, nt = 0, idx_type = 0;
-  uint64_t bin_lo = 0, bin_hi = 0;
-  bool db_staged = false, db_remapped = false;
-  std::vector<uint32_t> db_taxids;        // distinct taxids of the staged records (ascending)
-  std::vector<uint64_t> db_taxid_counts;
+  // the staged databases (or minimizer ranges of them) in the order they are asked (kuq_stage_db_append_range), all of
+  // the same k; none = no database staged.  dbs[0] is the range the record tier works on.
+  uint32_t k = 0;
+  std::vector<StagedDb> dbs;
   std::vector<uint32_t> universe;         // taxids of all records of the database (optional)
-  // device hash of the staged taxids (keys = taxid + 1)
-  DevBuf<uint32_t> d_tx_keys, d_tx_dense;
-  DevBuf<unsigned long long> d_tx_counts;
-  uint32_t tx_cap = 0;
-  // databases (or minimizer ranges of them) asked after the one above, in this order (kuq_stage_db_append_range); same k
-  struct ExtraDb {
-    DevBuf<uint8_t> d_pairs;
-    DevBuf<uint64_t> d_offsets;
-    uint64_t key_ct = 0, rec_base = 0, bin_lo = 0, bin_hi = 0;
-    uint32_t nt = 0, idx_type = 0;
-    DevBuf<uint32_t> d_tx_keys, d_tx_dense;
-    DevBuf<unsigned long long> d_tx_counts;
-    uint32_t tx_cap = 0;
-    std::vector<uint32_t> taxids;
-    std::vector<uint64_t> counts;
-    bool remapped = false;
-  };
-  std::vector<ExtraDb> more;
 
   // taxonomy
   bool tax_set = false, finalized = false;
@@ -188,7 +185,7 @@ struct kuq_ctx {
     DevBuf<uint8_t> d_pairs;
     DevBuf<uint64_t> d_offsets;
     Event ready;
-    uint64_t key_ct = 0, rec_base = 0, bin_lo = 0, bin_hi = 0;
+    DbRange range;                        // what kuq_stream_use makes dbs[0]'s range
     bool loaded = false;
   } sbuf[2];
   bool stream_open = false;
@@ -258,13 +255,15 @@ int fail(kuq_ctx *c, int code, const char *fmt, ...) {
   } while (0)
 
 void free_db(kuq_ctx *ctx) {
-  ctx->d_pairs_owned.reset(); ctx->d_offsets_owned.reset();
-  ctx->d_pairs = nullptr; ctx->d_offsets = nullptr;
-  ctx->d_tx_keys.reset(); ctx->d_tx_dense.reset(); ctx->d_tx_counts.reset();
+  ctx->dbs.clear();
   ctx->d_secondaries.reset();
   ctx->n_secondaries = 0; ctx->collisions = 0;
-  ctx->db_staged = false; ctx->db_remapped = false;
-  ctx->more.clear();
+}
+
+// the record tier's range: the first staged one, or an empty range when none is staged
+const DbRange &first_range(const kuq_ctx *ctx) {
+  static const DbRange none;
+  return ctx->dbs.empty() ? none : ctx->dbs[0].range;
 }
 
 }  // namespace
@@ -361,10 +360,11 @@ int check_slot(kuq_ctx *ctx, uint32_t slot) {
   return KUQ_OK;
 }
 
-// Scan the staged records for their distinct taxids (+counts): count_taxons (krakendb.cpp:90-113) on the GPU.  The
-// device hash (keys, dense ids to be filled, counts) and the sorted taxids / counts go to the caller's fields.
-int collect_taxids(kuq_ctx *ctx, const uint8_t *pairs, uint64_t key_ct, DevBuf<uint32_t> &d_keys, DevBuf<uint32_t> &d_dense,
-                   DevBuf<unsigned long long> &d_counts, uint32_t &tx_cap, std::vector<uint32_t> &taxids, std::vector<uint64_t> &tcounts) {
+// Scan the records of a staged range for their distinct taxids (+counts): count_taxons (krakendb.cpp:90-113) on the GPU.
+// The device hash (keys, dense ids to be filled, counts) and the sorted taxids / counts go to the range's fields.
+int collect_taxids(kuq_ctx *ctx, StagedDb &db) {
+  DevBuf<uint32_t> &d_keys = db.d_tx_keys, &d_dense = db.d_tx_dense;
+  DevBuf<unsigned long long> &d_counts = db.d_tx_counts;
   uint32_t cap = 1u << 16;
   for (;;) {
     d_keys.reset(); d_counts.reset(); d_dense.reset();
@@ -376,7 +376,7 @@ int collect_taxids(kuq_ctx *ctx, const uint8_t *pairs, uint64_t key_ct, DevBuf<u
     DevBuf<uint32_t> d_over;
     CU(d_over.alloc(1));
     CU(cudaMemsetAsync(d_over, 0, 4, ctx->aux));
-    launch_collect_taxids(pairs, key_ct, d_keys, d_counts, cap - 1, d_over, ctx->aux);
+    launch_collect_taxids(db.range.pairs, db.range.key_ct, d_keys, d_counts, cap - 1, d_over, ctx->aux);
     ctx->launches++;
     uint32_t over = 0;
     CU(cudaMemcpyAsync(&over, d_over, 4, cudaMemcpyDeviceToHost, ctx->aux));
@@ -398,15 +398,11 @@ int collect_taxids(kuq_ctx *ctx, const uint8_t *pairs, uint64_t key_ct, DevBuf<u
     v.reserve(used);
     for (uint32_t i = 0; i < cap; i++) if (keys[i]) v.emplace_back(keys[i] - 1, counts[i]);
     std::sort(v.begin(), v.end());
-    taxids.clear(); tcounts.clear();
-    for (auto &pr : v) { taxids.push_back(pr.first); tcounts.push_back(pr.second); }
-    tx_cap = cap;
+    db.taxids.clear(); db.counts.clear();
+    for (auto &pr : v) { db.taxids.push_back(pr.first); db.counts.push_back(pr.second); }
+    db.tx_cap = cap;
     return KUQ_OK;
   }
-}
-int collect_taxids(kuq_ctx *ctx) {
-  return collect_taxids(ctx, ctx->d_pairs, ctx->key_ct, ctx->d_tx_keys, ctx->d_tx_dense, ctx->d_tx_counts, ctx->tx_cap,
-                        ctx->db_taxids, ctx->db_taxid_counts);
 }
 
 // ---- the two device tables: the sparse-tier set and the exact k-mer set ---------------------------------------------
@@ -848,11 +844,11 @@ int upload_filter(kuq_ctx *ctx) {
 // ascending by taxid.  Builds the flattened Parent_map and uploads everything.
 int finalize(kuq_ctx *ctx) {
   if (ctx->finalized) return KUQ_OK;
-  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
+  if (ctx->dbs.empty()) return fail(ctx, KUQ_E_STATE, "no database staged");
   if (!ctx->tax_set) return fail(ctx, KUQ_E_STATE, "no taxonomy set");
-  std::vector<uint32_t> dbt = ctx->universe.empty() ? ctx->db_taxids : ctx->universe;
-  if (ctx->universe.empty())
-    for (auto &e : ctx->more) dbt.insert(dbt.end(), e.taxids.begin(), e.taxids.end());
+  std::vector<uint32_t> staged;
+  for (auto &e : ctx->dbs) staged.insert(staged.end(), e.taxids.begin(), e.taxids.end());
+  std::vector<uint32_t> dbt = ctx->universe.empty() ? staged : ctx->universe;
   std::sort(dbt.begin(), dbt.end());
   dbt.erase(std::unique(dbt.begin(), dbt.end()), dbt.end());
   std::vector<uint32_t> &raw = ctx->raw_of_dense;
@@ -871,8 +867,6 @@ int finalize(kuq_ctx *ctx) {
   for (uint32_t t : rest) { ctx->dense_of_raw[t] = (uint32_t)raw.size(); raw.push_back(t); }
   ctx->n_taxa = (uint32_t)raw.size();
   // staged taxids must all be numbered
-  std::vector<uint32_t> staged = ctx->db_taxids;
-  for (auto &e : ctx->more) staged.insert(staged.end(), e.taxids.begin(), e.taxids.end());
   for (uint32_t t : staged)
     if (!ctx->dense_of_raw.count(t) || ctx->dense_of_raw[t] >= ctx->n_sketch)
       return fail(ctx, KUQ_E_STATE, "staged records hold taxid %u that is not in the declared taxid universe", t);
@@ -941,10 +935,11 @@ int finalize(kuq_ctx *ctx) {
   return ctx->filter_set ? upload_filter(ctx) : KUQ_OK;
 }
 
-// rewrite the staged record values taxid → dense id (once per staged range or appended database)
-int remap_values(kuq_ctx *ctx, uint8_t *pairs, uint64_t key_ct, const uint32_t *d_keys, uint32_t *d_dense, uint32_t tx_cap) {
+// rewrite the record values of each staged range taxid → dense id, once per range
+int remap_values(kuq_ctx *ctx, StagedDb &db) {
+  const uint32_t tx_cap = db.tx_cap;
   std::vector<uint32_t> keys(tx_cap), dense(tx_cap, 0);
-  CU(cudaMemcpy(keys.data(), d_keys, tx_cap * 4ull, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(keys.data(), db.d_tx_keys, tx_cap * 4ull, cudaMemcpyDeviceToHost));
   for (uint32_t i = 0; i < tx_cap; i++)
     if (keys[i]) {
       auto it = ctx->dense_of_raw.find(keys[i] - 1);
@@ -952,12 +947,11 @@ int remap_values(kuq_ctx *ctx, uint8_t *pairs, uint64_t key_ct, const uint32_t *
         return fail(ctx, KUQ_E_STATE, "staged records hold taxid %u outside the numbered universe", keys[i] - 1);
       dense[i] = it->second;
     }
-  CU(cudaMemcpy(d_dense, dense.data(), tx_cap * 4ull, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(db.d_tx_dense, dense.data(), tx_cap * 4ull, cudaMemcpyHostToDevice));
   DevBuf<uint32_t> d_missing;
   CU(d_missing.alloc(1));
   CU(cudaMemset(d_missing, 0, 4));
-  launch_remap_values(pairs, key_ct, d_keys, d_dense, tx_cap - 1, d_missing, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1),
-                      ctx->aux);
+  launch_remap_values(db.range.pairs, db.range.key_ct, db.d_tx_keys, db.d_tx_dense, tx_cap - 1, d_missing, kmer_mask(ctx->k), ctx->aux);
   ctx->launches++;
   uint32_t missing = 0;
   CU(cudaMemcpyAsync(&missing, d_missing, 4, cudaMemcpyDeviceToHost, ctx->aux));
@@ -966,14 +960,9 @@ int remap_values(kuq_ctx *ctx, uint8_t *pairs, uint64_t key_ct, const uint32_t *
   return KUQ_OK;
 }
 int remap_db(kuq_ctx *ctx) {
-  if (!ctx->db_remapped) {
-    int rc = remap_values(ctx, ctx->d_pairs, ctx->key_ct, ctx->d_tx_keys, ctx->d_tx_dense, ctx->tx_cap);
-    if (rc) return rc;
-    ctx->db_remapped = true;
-  }
-  for (auto &e : ctx->more) {
+  for (auto &e : ctx->dbs) {
     if (e.remapped) continue;
-    int rc = remap_values(ctx, e.d_pairs, e.key_ct, e.d_tx_keys, e.d_tx_dense, e.tx_cap);
+    int rc = remap_values(ctx, e);
     if (rc) return rc;
     e.remapped = true;
   }
@@ -1055,20 +1044,21 @@ int exact_books(kuq_ctx *ctx, std::vector<long long> &books) {
 int ensure_collisions(kuq_ctx *ctx) {
   if (ctx->collisions) return KUQ_OK;
   ctx->collisions = -1;
-  if (ctx->stream_open || ctx->lca_mode || !ctx->db_remapped) return KUQ_OK;
+  if (ctx->stream_open || ctx->lca_mode || ctx->dbs.empty() || !ctx->dbs[0].remapped) return KUQ_OK;
+  const StagedDb &db = ctx->dbs[0];
   std::vector<uint64_t> per_taxon(ctx->n_sketch, 0);
-  for (size_t i = 0; i < ctx->db_taxids.size(); i++) per_taxon[ctx->dense_of_raw[ctx->db_taxids[i]]] += ctx->db_taxid_counts[i];
+  for (size_t i = 0; i < db.taxids.size(); i++) per_taxon[ctx->dense_of_raw[db.taxids[i]]] += db.counts[i];
   const auto t0 = std::chrono::steady_clock::now();
   // a table above 1/32 of the records (a taxon far above 2^25 records) is not worth it: the set path stays
-  const int rc = build_collisions(ctx->d_pairs, ctx->key_ct, ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), per_taxon.data(),
-                                  ctx->n_sketch, ctx->key_ct / 32 + 1024, ctx->d_secondaries, &ctx->n_secondaries, ctx->n_sm, ctx->aux);
+  const int rc = build_collisions(db.range.pairs, db.range.key_ct, kmer_mask(ctx->k), per_taxon.data(), ctx->n_sketch,
+                                  db.range.key_ct / 32 + 1024, ctx->d_secondaries, &ctx->n_secondaries, ctx->n_sm, ctx->aux);
   ctx->launches += 3;
   ctx->collisions_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   if (rc == 2) return fail(ctx, KUQ_E_CUDA, "building the collision table of the record tier failed: %s", cudaGetErrorString(cudaGetLastError()));
   if (rc == 0) ctx->collisions = 1;
   if (getenv("KUQ_TIMING"))
     fprintf(stderr, "[timing] collision table: %llu secondaries of %llu records, %.1f ms%s\n", (unsigned long long)ctx->n_secondaries,
-            (unsigned long long)ctx->key_ct, ctx->collisions_ms, rc ? " (not built: harvests fill the set)" : "");
+            (unsigned long long)db.range.key_ct, ctx->collisions_ms, rc ? " (not built: harvests fill the set)" : "");
   return KUQ_OK;
 }
 
@@ -1125,7 +1115,7 @@ int settle_kept(kuq_ctx *ctx) {
   unsigned long long *d_stat = ctx->d_harvest_stat;
   CU(cudaMemsetAsync(d_stat, 0, 8, ctx->aux));
   CU(cudaEventRecord(ctx->harvest_ev[0], ctx->aux));
-  launch_settle_kept(ctx->d_pairs, ctx->d_secondaries, ctx->n_secondaries, ctx->sparse.count, d_stat, ctx->aux);
+  launch_settle_kept(first_range(ctx).pairs, ctx->d_secondaries, ctx->n_secondaries, ctx->sparse.count, d_stat, ctx->aux);
   if (ctx->n_secondaries) ctx->launches++;
   CU(cudaEventRecord(ctx->harvest_ev[1], ctx->aux));
   unsigned long long st[3] = {0, 0, 0};
@@ -1151,9 +1141,9 @@ int spill_kept(kuq_ctx *ctx) {
   int rc = table_items(ctx, ctx->sparse, &used);
   if (!rc) rc = make_room(ctx, ctx->sparse, used, 0);
   if (rc) return rc;
-  const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
+  const DbRange &r = first_range(ctx);
   rc = run_saturating(
-      ctx, [&](uint32_t *err) { launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, set_view(ctx, ctx->sparse), nullptr, err, 3, ctx->aux); },
+      ctx, [&](uint32_t *err) { launch_harvest_seen(r.pairs, r.key_ct, kmer_mask(ctx->k), ctx->d_dense_flag, set_view(ctx, ctx->sparse), nullptr, err, 3, ctx->aux); },
       "sparse-tier set saturated while taking over the kept records (%llu slots)", (unsigned long long)ctx->sparse.cap);
   ctx->kept = false;
   ctx->kept_keys = 0;
@@ -1189,14 +1179,15 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   if (to_set && !discard) { int rc = spill_kept(ctx); if (rc) return rc; }
   if (!ctx->seen_dirty && !(ctx->kept && discard)) return KUQ_OK;
   ctx->seen_dirty = false;
-  if (!ctx->d_pairs || !ctx->key_ct) return KUQ_OK;
+  const DbRange &r = first_range(ctx);
+  if (!r.pairs || !r.key_ct) return KUQ_OK;
   bool keep = !discard && !to_set && ctx->sparse.slots && !ctx->set_has_hits && !ctx->stream_open;
   if (keep) {
     int rc = ensure_collisions(ctx);
     if (rc) return rc;
     keep = ctx->collisions == 1;
   }
-  const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
+  const uint64_t key_mask = kmer_mask(ctx->k);
   SparseSet ss = set_view(ctx, ctx->sparse);
   { int rc = harvest_state(ctx); if (rc) return rc; }
   unsigned long long *d_stat = ctx->d_harvest_stat;
@@ -1204,17 +1195,17 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
   CU(cudaMemsetAsync(d_stat, 0, 16, ctx->aux));
   CU(cudaEventRecord(e0, ctx->aux));
   if (discard || !ctx->sparse.slots) {
-    launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 2, ctx->aux);
+    launch_harvest_seen(r.pairs, r.key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 2, ctx->aux);
     ctx->launches++;
     ctx->kept = false;
     ctx->kept_keys = 0;
   } else if (keep) {
-    launch_harvest_keep(ctx->d_pairs, ctx->key_ct, ctx->d_secondaries, ctx->n_secondaries, ctx->d_dense_flag, ctx->n_sketch,
+    launch_harvest_keep(r.pairs, r.key_ct, ctx->d_secondaries, ctx->n_secondaries, ctx->d_dense_flag, ctx->n_sketch,
                         ctx->sparse.count, d_stat, ctx->aux);
     ctx->launches += ctx->n_secondaries ? 2 : 1;
     ctx->kept = true;
   } else {
-    launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 0, ctx->aux);
+    launch_harvest_seen(r.pairs, r.key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 0, ctx->aux);
     ctx->launches++;
     unsigned long long n_new = 0;
     uint64_t used = 0;
@@ -1228,7 +1219,7 @@ int harvest_seen(kuq_ctx *ctx, bool discard, bool to_set) {
     // Insert in record order.  (Round 2 also tried staging the keys by table slice so that the inserts of a slice are
     // L2-resident: read-only probes got faster, but NEW keys did not (each one still costs a DRAM sector fetch and a
     // dirty sector write-back), and new keys are what a harvest mostly sees.)
-    launch_harvest_seen(ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 1, ctx->aux);
+    launch_harvest_seen(r.pairs, r.key_ct, key_mask, ctx->d_dense_flag, ss, d_stat, reinterpret_cast<uint32_t *>(d_stat + 1), 1, ctx->aux);
     ctx->launches++;
     CU(cudaStreamSynchronize(ctx->aux));
     if (getenv("KUQ_TIMING")) fprintf(stderr, "[timing] harvest: %llu flagged records, %llu slots\n", n_new, (unsigned long long)ctx->sparse.cap);
@@ -1255,7 +1246,8 @@ KeySource set_keys(const kuq_ctx *ctx) {
   return k;
 }
 KeySource kept_keys(const kuq_ctx *ctx) {
-  KeySource k{nullptr, ctx->d_pairs, ctx->kept ? ctx->key_ct : 0, (uint32_t)((ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1)) >> 32)};
+  const DbRange &r = first_range(ctx);
+  KeySource k{nullptr, r.pairs, ctx->kept ? r.key_ct : 0, (uint32_t)(kmer_mask(ctx->k) >> 32)};
   return k;
 }
 
@@ -1310,26 +1302,25 @@ void set_unit_ptrs(Params &p, Slot &s) {
   p.units.direct_rows = s.u_direct_rows;
 }
 
-DbView db_view(const kuq_ctx *ctx, const uint8_t *pairs, const uint64_t *offsets, uint64_t rec_base, uint64_t bin_lo,
-                uint64_t bin_hi, uint32_t nt, uint32_t idx_type) {
+DbView db_view(const kuq_ctx *ctx, const DbRange &r) {
   DbView v;
-  v.pairs = pairs;
-  v.offsets = offsets;
-  v.rec_base = rec_base;
-  v.key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
-  v.bin_lo = (uint32_t)bin_lo;
-  v.bin_hi = (uint32_t)bin_hi;
+  v.pairs = r.pairs;
+  v.offsets = r.offsets;
+  v.rec_base = r.rec_base;
+  v.key_mask = kmer_mask(ctx->k);
+  v.bin_lo = (uint32_t)r.bin_lo;
+  v.bin_hi = (uint32_t)r.bin_hi;
   v.k = ctx->k;
-  v.nt = nt;
-  v.xor_mask = (uint32_t)((idx_type == 1 ? 0ull : INDEX2_XOR_MASK) & ((1ull << (2 * nt)) - 1));
-  v.n_mini = ctx->k - nt + 1;
+  v.nt = r.nt;
+  v.xor_mask = (uint32_t)((r.idx_type == 1 ? 0ull : INDEX2_XOR_MASK) & ((1ull << (2 * r.nt)) - 1));
+  v.n_mini = ctx->k - r.nt + 1;
   return v;
 }
 
 void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const uint64_t *d_offsets,
                  const uint32_t *d_unit, uint32_t n_reads, uint32_t flags) {
   memset(&p, 0, sizeof p);
-  p.db = db_view(ctx, ctx->d_pairs, ctx->d_offsets, ctx->rec_base, ctx->bin_lo, ctx->bin_hi, ctx->nt, ctx->idx_type);
+  p.db = db_view(ctx, first_range(ctx));
   p.tax.parent = ctx->d_parent;
   p.tax.depth = ctx->d_depth;
   p.tax.raw = ctx->d_raw;
@@ -1386,8 +1377,8 @@ void fill_params(kuq_ctx *ctx, Slot &s, Params &p, const char *d_bases, const ui
 // The staged databases in the order they are asked, each with its own minimizer range.  A run = consecutive databases
 // with the same window parameters (nt, index type).
 std::vector<DbView> db_views(const kuq_ctx *ctx) {
-  std::vector<DbView> v{db_view(ctx, ctx->d_pairs, ctx->d_offsets, ctx->rec_base, ctx->bin_lo, ctx->bin_hi, ctx->nt, ctx->idx_type)};
-  for (auto &e : ctx->more) v.push_back(db_view(ctx, e.d_pairs, e.d_offsets, e.rec_base, e.bin_lo, e.bin_hi, e.nt, e.idx_type));
+  std::vector<DbView> v;
+  for (auto &e : ctx->dbs) v.push_back(db_view(ctx, e.range));
   return v;
 }
 bool same_run(const DbView &a, const DbView &b) { return a.nt == b.nt && a.xor_mask == b.xor_mask; }
@@ -1434,7 +1425,7 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
   if (ctx->lca_mode) return fail(ctx, KUQ_E_STATE, "this context built a database (kuq_set_lcas_batch): stage it anew to classify");
   // several databases (or a fill-empty lookup): the in-order lookup, then — for a classification — the resolve half
   // over the slot's merged codes
-  const bool multi = (!ctx->more.empty() && mode != MODE_RESOLVE) || (mode == MODE_LOOKUP && p.only_hits == KUQ_LOOKUP_FILL_EMPTY) ||
+  const bool multi = (ctx->dbs.size() > 1 && mode != MODE_RESOLVE) || (mode == MODE_LOOKUP && p.only_hits == KUQ_LOOKUP_FILL_EMPTY) ||
                      run >= 0;
   if (multi && ((p.n_peers && run < 0) || ctx->shard_counting))
     return fail(ctx, KUQ_E_STATE, "shard counting and kuq_lookup_device_peers take one database (several: kuq_lookup_device_peers_run)");
@@ -1655,45 +1646,10 @@ void kuq_host_free(void *p) { if (p) cudaFreeHost(p); }
 
 // ---- database -------------------------------------------------------------------------------------------------
 namespace {
-struct DbFile {                  // a validated database.kdb + index image
-  const uint8_t *records;        // first record
-  uint64_t key_ct, pair_sz;
-  uint32_t k, nt, idx_type;
-  const uint64_t *offsets;       // 4^nt + 1 cumulative record offsets
-};
-
-int parse_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes, DbFile &f) {
-  const uint8_t *p = (const uint8_t *)kdb_image;
-  if (kdb_bytes < 56 || memcmp(p, "JFLISTDN", 8) != 0)                     // krakendb.cpp:32,67-68
-    return fail(ctx, KUQ_E_DB_FORMAT, "database in improper format");
-  uint64_t key_bits, val_len, key_ct;
-  memcpy(&key_bits, p + 8, 8);
-  memcpy(&val_len, p + 16, 8);
-  memcpy(&key_ct, p + 48, 8);
-  if (val_len != 4) return fail(ctx, KUQ_E_DB_FORMAT, "can only handle 4 byte DB values");   // :73-74
-  uint32_t k = (uint32_t)(key_bits / 2);
-  uint64_t key_len = key_bits / 8 + !!(key_bits % 8);
-  if (key_bits > 62)
-    return fail(ctx, KUQ_E_UNSUPPORTED_K, "k = %u (key_len %llu): k-mers up to 31 bases are supported", k,
-                (unsigned long long)key_len);
-  const uint64_t pair_sz = key_len + 4;                                      // pair_size(), krakendb.cpp:76,176
-  uint64_t header = 72 + 2 * (4 + 8 * key_bits);                           // :177
-  if (kdb_bytes < header + key_ct * pair_sz) return fail(ctx, KUQ_E_DB_FORMAT, "database file truncated");
-  const uint8_t *q = (const uint8_t *)idx_image;
-  uint32_t idx_type;
-  if (idx_bytes < 8) return fail(ctx, KUQ_E_DB_FORMAT, "illegal Kraken DB index format");
-  if (memcmp(q, "KRAKIDX", 7) == 0) idx_type = 1;
-  else if (memcmp(q, "KRAKIX2", 7) == 0) idx_type = 2;
-  else return fail(ctx, KUQ_E_DB_FORMAT, "illegal Kraken DB index format");  // :541
-  uint32_t nt = q[7];
-  if (nt < 1 || nt > 15 || nt > k) return fail(ctx, KUQ_E_DB_FORMAT, "index minimizer length %u out of range", nt);
-  uint64_t n_bins = 1ull << (2 * nt);
-  if (idx_bytes < 8 + 8 * (n_bins + 1)) return fail(ctx, KUQ_E_DB_FORMAT, "index file truncated");
-  f.records = p + header;
-  f.key_ct = key_ct; f.pair_sz = pair_sz;
-  f.k = k; f.nt = nt; f.idx_type = idx_type;
-  f.offsets = (const uint64_t *)(q + 8);
-  return KUQ_OK;
+int parse_images(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes, DbFile &f) {
+  std::string err;
+  const int rc = parse_db(kdb_image, kdb_bytes, idx_image, idx_bytes, f, err);
+  return rc ? fail(ctx, rc, "%s", err.c_str()) : KUQ_OK;
 }
 
 // records [offsets[bin_lo], offsets[bin_hi]) of f → d_pairs (12-byte layout), offsets [bin_lo, bin_hi] → d_offsets.
@@ -1734,29 +1690,31 @@ int upload_db(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi, u
 }  // namespace
 
 namespace {
-// bins [bin_lo, bin_hi) of f (validated by the caller; may be empty) become the first database of the context
-int stage_first(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi) {
-  uint64_t rec_lo = f.offsets[bin_lo], rec_hi = f.offsets[bin_hi];
+// Bins [bin_lo, bin_hi) of f (validated by the caller; may be empty) join the staged databases; `first`: they replace
+// whatever the context held.  The taxonomy numbering survives a re-stage (chunked mode) as long as the new range only
+// holds numbered taxids; the sparse-tier keys of the old records leave with them into the set.  A range that fails to
+// stage is not kept.
+int stage_range(kuq_ctx *ctx, const DbFile &f, uint64_t bin_lo, uint64_t bin_hi, bool first) {
+  const uint64_t rec_lo = f.offsets[bin_lo], rec_hi = f.offsets[bin_hi];
   if (rec_hi < rec_lo || rec_hi > f.key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
-  // taxonomy numbering survives a re-stage (chunked mode) as long as the new range only holds numbered taxids; the
-  // sparse-tier keys of the records leave with them into the set
-  { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
-  stream_close(ctx);
-  free_db(ctx);
-  ctx->k = f.k; ctx->nt = f.nt; ctx->idx_type = f.idx_type;
-  ctx->bin_lo = bin_lo; ctx->bin_hi = bin_hi;
-  ctx->rec_base = rec_lo;
-  ctx->key_ct = rec_hi - rec_lo;
-  ctx->db_owned = true;
-  CU(ctx->d_pairs_owned.alloc(ctx->key_ct * 12 + SLACK));
-  CU(ctx->d_offsets_owned.alloc(bin_hi - bin_lo + 1));
-  ctx->d_pairs = ctx->d_pairs_owned;
-  ctx->d_offsets = ctx->d_offsets_owned;
-  int rc = upload_db(ctx, f, bin_lo, bin_hi, ctx->d_pairs, ctx->d_offsets_owned);
-  if (rc) return rc;
-  ctx->db_staged = true;
-  rc = collect_taxids(ctx);
-  if (rc) return rc;
+  if (first) {
+    { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
+    stream_close(ctx);
+    free_db(ctx);
+    ctx->k = f.k;
+  }
+  ctx->dbs.emplace_back();
+  StagedDb &e = ctx->dbs.back();
+  auto drop = [&](int code) { ctx->dbs.pop_back(); return code; };
+  const uint64_t key_ct = rec_hi - rec_lo;
+  if (e.own_pairs.alloc(key_ct * 12 + SLACK) != cudaSuccess || e.own_offsets.alloc(bin_hi - bin_lo + 1) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return drop(fail(ctx, KUQ_E_NOMEM, "no room for database %zu (%llu records)", ctx->dbs.size(), (unsigned long long)key_ct));
+  }
+  e.range = DbRange{e.own_pairs, e.own_offsets, key_ct, rec_lo, bin_lo, bin_hi, f.nt, f.idx_type};
+  int rc = upload_db(ctx, f, bin_lo, bin_hi, e.own_pairs, e.own_offsets);
+  if (!rc) rc = collect_taxids(ctx, e);
+  if (rc) return drop(rc);
   if (ctx->finalized) return remap_db(ctx);
   return KUQ_OK;
 }
@@ -1767,12 +1725,11 @@ int kuq_stage_db(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const 
   if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
   CU(cudaSetDevice(ctx->device));
   DbFile f;
-  int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
+  int rc = parse_images(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
   if (rc) return rc;
-  const uint64_t n_bins = 1ull << (2 * f.nt);
-  if (bin_hi == 0 || bin_hi > n_bins) bin_hi = n_bins;
+  if (bin_hi == 0 || bin_hi > f.n_bins) bin_hi = f.n_bins;
   if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
-  return stage_first(ctx, f, bin_lo, bin_hi);
+  return stage_range(ctx, f, bin_lo, bin_hi, true);
 }
 
 int kuq_stage_db_append_range(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image,
@@ -1780,33 +1737,18 @@ int kuq_stage_db_append_range(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_
   if (!ctx || !kdb_image || !idx_image) return KUQ_E_INVALID_ARG;
   CU(cudaSetDevice(ctx->device));
   DbFile f;
-  int rc = parse_db(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
+  int rc = parse_images(ctx, kdb_image, kdb_bytes, idx_image, idx_bytes, f);
   if (rc) return rc;
-  const uint64_t n_bins = 1ull << (2 * f.nt);
-  if (bin_hi == 0) bin_hi = n_bins;                  // (0, 0) = the whole database; lo == hi != 0 = an empty slice
-  if (bin_lo > bin_hi || bin_hi > n_bins)
+  if (bin_hi == 0) bin_hi = f.n_bins;                // (0, 0) = the whole database; lo == hi != 0 = an empty slice
+  if (bin_lo > bin_hi || bin_hi > f.n_bins)
     return fail(ctx, KUQ_E_INVALID_ARG, "minimizer range [%llu, %llu) outside the %llu bins of nt = %u", (unsigned long long)bin_lo,
-                (unsigned long long)bin_hi, (unsigned long long)n_bins, f.nt);
-  if (!ctx->db_staged || ctx->stream_open) return stage_first(ctx, f, bin_lo, bin_hi);
-  if (f.k != ctx->k) return fail(ctx, KUQ_E_INVALID_ARG, "the databases differ in k: %u vs %u", ctx->k, f.k);
-  if (f.offsets[n_bins] != f.key_ct || f.offsets[bin_lo] > f.offsets[bin_hi])
-    return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
-  ctx->more.emplace_back();
-  kuq_ctx::ExtraDb &e = ctx->more.back();
-  e.rec_base = f.offsets[bin_lo];
-  e.key_ct = f.offsets[bin_hi] - e.rec_base;
-  e.bin_lo = bin_lo; e.bin_hi = bin_hi;
-  e.nt = f.nt; e.idx_type = f.idx_type;
-  auto drop = [&](int code) { ctx->more.pop_back(); return code; };
-  if (e.d_pairs.alloc(e.key_ct * 12 + SLACK) != cudaSuccess || e.d_offsets.alloc(bin_hi - bin_lo + 1) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return drop(fail(ctx, KUQ_E_NOMEM, "no room for database %zu (%llu records)", ctx->more.size() + 1, (unsigned long long)e.key_ct));
+                (unsigned long long)bin_hi, (unsigned long long)f.n_bins, f.nt);
+  const bool first = ctx->dbs.empty() || ctx->stream_open;
+  if (!first) {
+    if (f.k != ctx->k) return fail(ctx, KUQ_E_INVALID_ARG, "the databases differ in k: %u vs %u", ctx->k, f.k);
+    if (f.offsets[f.n_bins] != f.key_ct) return fail(ctx, KUQ_E_DB_FORMAT, "index offsets inconsistent with key count");
   }
-  rc = upload_db(ctx, f, bin_lo, bin_hi, e.d_pairs, e.d_offsets);
-  if (!rc) rc = collect_taxids(ctx, e.d_pairs, e.key_ct, e.d_tx_keys, e.d_tx_dense, e.d_tx_counts, e.tx_cap, e.taxids, e.counts);
-  if (rc) return drop(rc);
-  if (ctx->finalized) return remap_db(ctx);
-  return KUQ_OK;
+  return stage_range(ctx, f, bin_lo, bin_hi, first);
 }
 
 int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes, const void *idx_image, uint64_t idx_bytes) {
@@ -1815,7 +1757,7 @@ int kuq_stage_db_append(kuq_ctx *ctx, const void *kdb_image, uint64_t kdb_bytes,
 
 int kuq_db_runs(kuq_ctx *ctx, uint32_t *n_runs) {
   if (!ctx || !n_runs) return KUQ_E_INVALID_ARG;
-  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
+  if (ctx->dbs.empty()) return fail(ctx, KUQ_E_STATE, "no database staged");
   *n_runs = count_runs(ctx);
   return KUQ_OK;
 }
@@ -1831,17 +1773,12 @@ int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uin
   if (bin_lo >= bin_hi) return fail(ctx, KUQ_E_INVALID_ARG, "empty minimizer range");
   { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
   free_db(ctx);
-  ctx->k = k; ctx->nt = nt; ctx->idx_type = idx_type;
-  ctx->bin_lo = bin_lo; ctx->bin_hi = bin_hi;
-  ctx->db_owned = false;
-  ctx->d_pairs = (uint8_t *)d_pairs;
-  ctx->d_offsets = d_offsets;
+  ctx->k = k;
   uint64_t first = 0;
   CU(cudaMemcpy(&first, d_offsets, 8, cudaMemcpyDeviceToHost));
-  ctx->rec_base = first;
-  ctx->key_ct = key_ct;
-  ctx->db_staged = true;
-  int rc = collect_taxids(ctx);
+  ctx->dbs.emplace_back();
+  ctx->dbs[0].range = DbRange{(uint8_t *)d_pairs, d_offsets, key_ct, first, bin_lo, bin_hi, nt, idx_type};
+  int rc = collect_taxids(ctx, ctx->dbs[0]);
   if (rc) return rc;
   if (ctx->finalized) return remap_db(ctx);
   return KUQ_OK;
@@ -1849,10 +1786,9 @@ int kuq_attach_db_device(kuq_ctx *ctx, void *d_pairs, uint64_t key_ct, const uin
 
 int kuq_db_taxids(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n) {
   if (!ctx || !n) return KUQ_E_INVALID_ARG;
-  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
-  std::vector<std::pair<uint32_t, uint64_t>> all;          // over the appended databases too (counts summed)
-  for (size_t i = 0; i < ctx->db_taxids.size(); i++) all.emplace_back(ctx->db_taxids[i], ctx->db_taxid_counts[i]);
-  for (auto &e : ctx->more)
+  if (ctx->dbs.empty()) return fail(ctx, KUQ_E_STATE, "no database staged");
+  std::vector<std::pair<uint32_t, uint64_t>> all;          // over every staged range (counts summed)
+  for (auto &e : ctx->dbs)
     for (size_t i = 0; i < e.taxids.size(); i++) all.emplace_back(e.taxids[i], e.counts[i]);
   std::sort(all.begin(), all.end());
   std::vector<std::pair<uint32_t, uint64_t>> u;
@@ -2306,7 +2242,7 @@ int kuq_lookup_device_peers_run(kuq_ctx *ctx, uint32_t slot, const char *d_bases
                                 uint32_t n_reads, uint64_t total_bases, uint32_t *const *d_codes_peers,
                                 const uint64_t *base_bounds, uint32_t n_peers, uint32_t run) {
   if (!ctx) return KUQ_E_INVALID_ARG;
-  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
+  if (ctx->dbs.empty()) return fail(ctx, KUQ_E_STATE, "no database staged");
   const uint32_t n_runs = count_runs(ctx);
   if (run >= n_runs) return fail(ctx, KUQ_E_INVALID_ARG, "run %u of %u", run, n_runs);
   return peers_call(ctx, slot, d_bases, d_read_offsets, n_reads, total_bases, d_codes_peers, base_bounds, n_peers, (int)run);
@@ -3052,7 +2988,7 @@ void stream_close(kuq_ctx *ctx) {
   ctx->copy_stream.reset();
   ctx->d_stream_missing.reset();
   ctx->d_stream_land.reset();
-  if (ctx->stream_open) { ctx->d_pairs = nullptr; ctx->d_offsets = nullptr; ctx->db_staged = false; }
+  if (ctx->stream_open) ctx->dbs.clear();
   ctx->stream_open = false;
 }
 }  // namespace
@@ -3069,31 +3005,32 @@ int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, ui
   { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }
   free_db(ctx);
   stream_close(ctx);
-  ctx->k = k; ctx->nt = nt; ctx->idx_type = idx_type;
-  ctx->db_owned = false;
-  ctx->db_taxids = ctx->universe;
-  std::sort(ctx->db_taxids.begin(), ctx->db_taxids.end());
-  ctx->db_taxids.erase(std::unique(ctx->db_taxids.begin(), ctx->db_taxids.end()), ctx->db_taxids.end());
-  ctx->db_taxid_counts.assign(ctx->db_taxids.size(), 0);
-  ctx->db_staged = true;
+  ctx->k = k;
+  ctx->dbs.emplace_back();
+  StagedDb &db = ctx->dbs[0];
+  db.range.nt = nt; db.range.idx_type = idx_type;
+  db.taxids = ctx->universe;
+  std::sort(db.taxids.begin(), db.taxids.end());
+  db.taxids.erase(std::unique(db.taxids.begin(), db.taxids.end()), db.taxids.end());
+  db.counts.assign(db.taxids.size(), 0);
   int rc = finalize(ctx);
-  if (rc) { ctx->db_staged = false; return rc; }
+  if (rc) { ctx->dbs.clear(); return rc; }
   // device table taxid → dense id over the whole universe (what collect_taxids builds per staged range otherwise)
   uint32_t cap = 1u << 16;
-  while ((uint64_t)cap < 4ull * ctx->db_taxids.size()) cap <<= 1;
+  while ((uint64_t)cap < 4ull * db.taxids.size()) cap <<= 1;
   std::vector<uint32_t> keys(cap, 0), dense(cap, 0);
-  for (uint32_t t : ctx->db_taxids) {
+  for (uint32_t t : db.taxids) {
     uint32_t slot = host_hash_u32(t) & (cap - 1);
     while (keys[slot]) slot = (slot + 1) & (cap - 1);
     keys[slot] = t + 1;
     dense[slot] = ctx->dense_of_raw[t];
   }
-  CU(ctx->d_tx_keys.alloc(cap));
-  CU(ctx->d_tx_dense.alloc(cap));
-  CU(cudaMemcpy(ctx->d_tx_keys, keys.data(), cap * 4ull, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(ctx->d_tx_dense, dense.data(), cap * 4ull, cudaMemcpyHostToDevice));
-  ctx->tx_cap = cap;
-  ctx->db_remapped = true;                       // each range is remapped as it arrives
+  CU(db.d_tx_keys.alloc(cap));
+  CU(db.d_tx_dense.alloc(cap));
+  CU(cudaMemcpy(db.d_tx_keys, keys.data(), cap * 4ull, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(db.d_tx_dense, dense.data(), cap * 4ull, cudaMemcpyHostToDevice));
+  db.tx_cap = cap;
+  db.remapped = true;                            // each range is remapped as it arrives
   CU(ctx->copy_stream.alloc(cudaStreamNonBlocking));
   CU(ctx->d_stream_missing.alloc(1));
   CU(cudaMemset(ctx->d_stream_missing, 0, 4));
@@ -3111,7 +3048,6 @@ int kuq_stream_open(kuq_ctx *ctx, uint32_t k, uint32_t nt, uint32_t idx_type, ui
   ctx->stream_cap_records = max_records;
   ctx->stream_cap_bins = max_bins;
   ctx->stream_open = true;
-  ctx->key_ct = 0;
   return KUQ_OK;
 }
 
@@ -3146,11 +3082,13 @@ int kuq_stream_load(kuq_ctx *ctx, uint32_t buf, const void *host_records, uint64
     CU(cudaGetLastError());
   }
   CU(cudaMemcpyAsync(b.d_offsets, host_offsets, (bin_hi - bin_lo + 1) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
-  launch_remap_values(b.d_pairs, n_records, ctx->d_tx_keys, ctx->d_tx_dense, ctx->tx_cap - 1, ctx->d_stream_missing,
-                      ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1), ctx->copy_stream);
+  const StagedDb &db = ctx->dbs[0];
+  launch_remap_values(b.d_pairs, n_records, db.d_tx_keys, db.d_tx_dense, db.tx_cap - 1, ctx->d_stream_missing, kmer_mask(ctx->k),
+                      ctx->copy_stream);
   ctx->launches++;
   CU(cudaEventRecord(b.ready, ctx->copy_stream));
-  b.key_ct = n_records; b.rec_base = host_offsets[0]; b.bin_lo = bin_lo; b.bin_hi = bin_hi; b.loaded = true;
+  b.range = DbRange{b.d_pairs, b.d_offsets, n_records, host_offsets[0], bin_lo, bin_hi, db.range.nt, db.range.idx_type};
+  b.loaded = true;
   return KUQ_OK;
 }
 
@@ -3161,8 +3099,7 @@ int kuq_stream_use(kuq_ctx *ctx, uint32_t buf) {
   if (ctx->seen_dirty) { int hrc = harvest_seen(ctx, false); if (hrc) return hrc; }
   kuq_ctx::StreamBuf &b = ctx->sbuf[buf];
   for (auto &s : ctx->slots) CU(cudaStreamWaitEvent(s.stream, b.ready, 0));
-  ctx->d_pairs = b.d_pairs; ctx->d_offsets = b.d_offsets;
-  ctx->key_ct = b.key_ct; ctx->rec_base = b.rec_base; ctx->bin_lo = b.bin_lo; ctx->bin_hi = b.bin_hi;
+  ctx->dbs[0].range = b.range;
   return KUQ_OK;
 }
 
@@ -3175,8 +3112,9 @@ int kuq_stream_close(kuq_ctx *ctx) {
   { int hrc = harvest_seen(ctx, false, true); if (hrc) return hrc; }  // flags in the records go before the records do
   for (auto &b : ctx->sbuf) b = kuq_ctx::StreamBuf();
   ctx->d_stream_land.reset();
-  ctx->d_pairs = nullptr; ctx->d_offsets = nullptr;
-  ctx->key_ct = 0;
+  DbRange &r = ctx->dbs[0].range;
+  r.pairs = nullptr; r.offsets = nullptr;
+  r.key_ct = 0;
   return KUQ_OK;
 }
 
@@ -3346,8 +3284,9 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
   // flagged since the last harvest, or kept.  The flagged records are NOT inserted locally first: their keys go straight
   // into the export buffer (and the flags are cleared) — after the exchange every key is inserted exactly once, by its
   // owner.
-  const uint64_t key_mask = ctx->k >= 32 ? ~0ull : ((1ull << (2 * ctx->k)) - 1);
-  const bool records = (ctx->seen_dirty || ctx->kept) && ctx->d_pairs && ctx->key_ct;
+  const uint64_t key_mask = kmer_mask(ctx->k);
+  const DbRange &r = first_range(ctx);
+  const bool records = (ctx->seen_dirty || ctx->kept) && r.pairs && r.key_ct;
   return export_parts(ctx, n_parts, 8, reinterpret_cast<unsigned long long *>(d_keys_out), cap, counts,
                       reinterpret_cast<unsigned long long **>(alloc_out), SPARSE_TEXT,
                       [&](unsigned long long *cnt, unsigned long long *out, const unsigned long long *end, uint32_t *err, int pass) {
@@ -3355,7 +3294,7 @@ static int export_partitioned(kuq_ctx *ctx, uint32_t n_parts, uint64_t *d_keys_o
                                           end, err, pass, ctx->aux);
                         ctx->launches++;
                         if (!records) return;
-                        launch_keys_parts(1, nullptr, ctx->d_pairs, ctx->key_ct, key_mask, ctx->d_dense_flag, n_parts, cnt, out, end,
+                        launch_keys_parts(1, nullptr, r.pairs, r.key_ct, key_mask, ctx->d_dense_flag, n_parts, cnt, out, end,
                                           err, pass, ctx->aux);
                         ctx->launches++;
                         // the flags are gone: their keys live in the export buffer now (the kept records drop their flag
@@ -3458,8 +3397,9 @@ int kuq_layout_experiment(kuq_ctx *ctx, uint32_t slot, uint64_t n_positions, uin
   CU(cudaSetDevice(ctx->device));
   rc = ensure_ready(ctx);
   if (rc) return rc;
-  if (!ctx->db_staged || ctx->stream_open || !ctx->d_pairs) return fail(ctx, KUQ_E_STATE, "the experiment needs a staged (not streamed) database");
-  if (ctx->k != 31 || ctx->nt != 15) return fail(ctx, KUQ_E_INVALID_ARG, "the 8-byte record code is defined for k = 31, m = 15");
+  const DbRange &r = first_range(ctx);
+  if (ctx->stream_open || !r.pairs) return fail(ctx, KUQ_E_STATE, "the experiment needs a staged (not streamed) database");
+  if (ctx->k != 31 || r.nt != 15) return fail(ctx, KUQ_E_INVALID_ARG, "the 8-byte record code is defined for k = 31, m = 15");
   Slot &s = ctx->slots[slot];
   if (!s.timed || n_positions == 0 || n_positions > s.total_bases)
     return fail(ctx, KUQ_E_STATE, "run a batch on the slot first; n_positions must not exceed its text length");
@@ -3469,7 +3409,7 @@ int kuq_layout_experiment(kuq_ctx *ctx, uint32_t slot, uint64_t n_positions, uin
   if (s.windows_packed) launch_unpack_windows(p, n_positions, ctx->n_sm, s.stream);
   rc = refresh_reg_floor(ctx, s.total_bases, s.stream);     // the fused variants count
   if (rc) return rc;
-  const int erc = layout_experiment(p, ctx->key_ct, s.d_canon, s.d_bins, s.d_dense, n_positions, ctx->n_sm, s.stream, reps,
+  const int erc = layout_experiment(p, r.key_ct, s.d_canon, s.d_bins, s.d_dense, n_positions, ctx->n_sm, s.stream, reps,
                                     ctx->cfg.hll_mode == KUQ_HLL_DENSE_ONLY && s.windows_packed, out);
   ctx->snap_valid = false;
   ctx->launches += 3 + (s.windows_packed ? 1 : 0) + (uint64_t)KUQ_LAYOUT_VARIANTS * (reps + 2ull);
@@ -3842,12 +3782,13 @@ int kuq_set_lcas_batch(kuq_ctx *ctx, const char *bases, const uint64_t *piece_of
 
 int kuq_db_value_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t cap, uint32_t *n) {
   if (!ctx || !n) return KUQ_E_INVALID_ARG;
-  if (!ctx->db_staged) return fail(ctx, KUQ_E_STATE, "no database staged");
-  if (!ctx->more.empty()) return fail(ctx, KUQ_E_STATE, "several databases staged: count them one at a time");
+  if (ctx->dbs.empty()) return fail(ctx, KUQ_E_STATE, "no database staged");
+  if (ctx->dbs.size() > 1) return fail(ctx, KUQ_E_STATE, "several databases staged: count them one at a time");
+  const StagedDb &db = ctx->dbs[0];
   std::vector<std::pair<uint32_t, uint64_t>> u;
-  if (!ctx->db_remapped) {
+  if (!db.remapped) {
     // the values are still the taxids they were staged with, and staging counted them (collect_taxids)
-    for (size_t i = 0; i < ctx->db_taxids.size(); i++) u.emplace_back(ctx->db_taxids[i], ctx->db_taxid_counts[i]);
+    for (size_t i = 0; i < db.taxids.size(); i++) u.emplace_back(db.taxids[i], db.counts[i]);
   } else {
     CU(cudaSetDevice(ctx->device));
     for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
@@ -3857,7 +3798,7 @@ int kuq_db_value_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t
     CU(d_bad.alloc(1));
     CU(cudaMemsetAsync(d_counts, 0, ctx->n_taxa * 8ull, ctx->aux));
     CU(cudaMemsetAsync(d_bad, 0, 4, ctx->aux));
-    launch_value_counts(ctx->d_pairs, ctx->key_ct, ctx->n_taxa, d_counts, d_bad, ctx->aux);
+    launch_value_counts(db.range.pairs, db.range.key_ct, ctx->n_taxa, d_counts, d_bad, ctx->aux);
     CU(cudaGetLastError());
     ctx->launches++;
     std::vector<unsigned long long> c(ctx->n_taxa);
@@ -3882,20 +3823,22 @@ int kuq_db_value_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *count, uint32_t
 
 int kuq_export_db_values(kuq_ctx *ctx, void *kdb_image, uint64_t kdb_bytes) {
   if (!ctx || !kdb_image) return KUQ_E_INVALID_ARG;
-  if (!ctx->db_staged || !ctx->db_owned) return fail(ctx, KUQ_E_STATE, "no database staged from a host image");
+  if (ctx->dbs.empty() || !ctx->dbs[0].own_pairs) return fail(ctx, KUQ_E_STATE, "no database staged from a host image");
+  const StagedDb &db = ctx->dbs[0];
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
-  const uint64_t key_bits = 2ull * ctx->k, header = 72 + 2 * (4 + 8 * key_bits);
-  const uint64_t key_len = (key_bits + 7) / 8, pair_sz = key_len + 4;            // the file's records, not HBM's 12 bytes
-  if (kdb_bytes < header + (ctx->rec_base + ctx->key_ct) * pair_sz)
-    return fail(ctx, KUQ_E_INVALID_ARG, "image too small for %llu records", (unsigned long long)(ctx->rec_base + ctx->key_ct));
-  std::vector<uint8_t> rec(ctx->key_ct * 12);
-  CU(cudaMemcpy(rec.data(), ctx->d_pairs, rec.size(), cudaMemcpyDeviceToHost));
-  uint8_t *out = (uint8_t *)kdb_image + header + ctx->rec_base * pair_sz;       // a staged range: its records only
-  for (uint64_t i = 0; i < ctx->key_ct; i++) {
+  const uint64_t key_bits = 2ull * ctx->k, header = kdb_header_bytes(key_bits);
+  const uint64_t key_len = kdb_key_len(key_bits), pair_sz = key_len + 4;           // the file's records, not HBM's 12 bytes
+  const uint64_t rec_base = db.range.rec_base, key_ct = db.range.key_ct;
+  if (kdb_bytes < header + (rec_base + key_ct) * pair_sz)
+    return fail(ctx, KUQ_E_INVALID_ARG, "image too small for %llu records", (unsigned long long)(rec_base + key_ct));
+  std::vector<uint8_t> rec(key_ct * 12);
+  CU(cudaMemcpy(rec.data(), db.range.pairs, rec.size(), cudaMemcpyDeviceToHost));
+  uint8_t *out = (uint8_t *)kdb_image + header + rec_base * pair_sz;              // a staged range: its records only
+  for (uint64_t i = 0; i < key_ct; i++) {
     uint32_t v;
     memcpy(&v, rec.data() + i * 12 + 8, 4);
-    if (ctx->db_remapped) {                                 // dense id → taxid
+    if (db.remapped) {                                      // dense id → taxid
       if (v >= ctx->n_taxa) return fail(ctx, KUQ_E_STATE, "record %llu holds an unknown dense id %u", (unsigned long long)i, v);
       v = ctx->raw_of_dense[v];
     }

@@ -19,6 +19,7 @@
 // that order; C sorts one contiguous group of ranges per worker.  Workers write disjoint bytes of the host images.
 #include "../../include/kuq.h"
 #include "kuq_bounce.cuh"
+#include "kuq_dbfile.h"
 #include "kuq_kernels.cuh"
 #include "kuq_minimizer.cuh"
 #include "kuq_ranges.h"
@@ -286,23 +287,21 @@ int dbsort_device(const int *devices, uint32_t n_dev, const uint8_t *jdb, uint64
   if (jdb_bytes < 56 || memcmp(jdb, "JFLISTDN", 8) != 0)
     return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: not a Jellyfish-style database (krakendb.cpp:67)");
   if (nt < 1 || nt > 15) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: -n must be 1..15");
-  uint64_t key_bits, val_len, key_ct;
-  memcpy(&key_bits, jdb + 8, 8);
-  memcpy(&val_len, jdb + 16, 8);
-  memcpy(&key_ct, jdb + 48, 8);
-  if (val_len != 4) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: can only handle 4 byte DB values (krakendb.cpp:73-74)");
+  const KdbFile h = kdb_view(jdb);
+  const uint64_t key_bits = h.key_bits;
+  if (h.val_len != 4) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: can only handle 4 byte DB values (krakendb.cpp:73-74)");
   if (key_bits < 2 * nt || key_bits > 64)
     return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: key_bits %llu out of range", (unsigned long long)key_bits);
   Geometry g;
-  g.k = (uint32_t)(key_bits / 2);
+  g.k = h.k;
   g.nt = nt;
-  g.key_len = (uint32_t)(key_bits / 8 + !!(key_bits % 8));
+  g.key_len = (uint32_t)h.key_len;
   g.key_bits = key_bits;
-  g.pair_sz = g.key_len + 4;
-  g.header = 72 + 2 * (4 + 8 * key_bits);
-  g.n = key_ct;
+  g.pair_sz = h.pair_sz;
+  g.header = h.header_bytes;
+  g.n = h.key_ct;
   g.entries = 1ull << (2 * nt);
-  if (jdb_bytes < g.header + key_ct * g.pair_sz) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: image shorter than its header says");
+  if (jdb_bytes < g.header + g.n * g.pair_sz) return seterr(KUQ_E_DB_FORMAT, err, err_cap, "db_sort: image shorter than its header says");
   const uint64_t n = g.n, pair_sz = g.pair_sz, entries = g.entries;
   // one_budget decides whether the sort fits the first device in one piece; budget is then what every worker of the
   // passes may use, the same for all so that the plan does not depend on the devices
