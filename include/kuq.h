@@ -450,6 +450,29 @@ int kuq_exact_summary(kuq_ctx *ctx, uint64_t *d_count_out, int64_t *d_books_out)
 int kuq_set_exact_summary(kuq_ctx *ctx, const uint64_t *d_count, const int64_t *d_books);
 int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n);
 int kuq_exact_rollup_passes(kuq_ctx *ctx, uint32_t *passes);
+/* ---- the exact set spilled to host memory by k-mer part ---------------------------------------------------------------
+ * kuq_set_exact_spill(ctx, bytes > 0): when the table cannot grow before a batch (no device memory, or
+ * KUQ_EXACT_MAX_SLOTS), its pairs move to host memory instead of the batch failing with KUQ_E_NOMEM.  They go in rounds
+ * over slot ranges (KUQ_EXACT_MERGE_SLOTS, as kuq_merge_into) through a bounded device buffer and a pinned one, grouped
+ * into the 64 parts of kuq_exact_owner(kmer, 64); the table is emptied and takes the batch at the same capacity (an
+ * empty table that cannot take a batch's bound of one pair per window fails with KUQ_E_NOMEM).  The budget bounds the
+ * bytes of spilled pairs (16 each) held by all contexts of the process together: a spill that would pass it fails with
+ * KUQ_E_NOMEM.  0 (the default) turns spilling off.
+ * kuq_exact_spill_info: the times the table spilled since the last kuq_reset_counts, and the pairs held on the host now.
+ * From a context's first spill until kuq_exact_settle, every readout that would see a part of its set refuses with
+ * KUQ_E_STATE: kuq_read_counts, kuq_clade_counts, kuq_clade_counts_tree, kuq_exact_export, kuq_exact_export_partitioned*,
+ * kuq_exact_summary, kuq_exact_partition and the set union of kuq_merge_into (kuq_merge_counters_into still works).
+ * kuq_exact_settle(ctxs, n >= 1): every context spills what its table still holds (under its budget too); the parts of
+ * all contexts are cut into groups of consecutive parts that fit a table (a table smaller than the largest grows to it
+ * first where its device keeps room beside it for a round and the roll-up's sort), and one host thread per context imports each of its groups into its emptied table in rounds —
+ * duplicates from successive spills and from other contexts collapse — and sums the group's set sizes and roll-up books
+ * (kuq_exact_summary).  The sums are installed on ctxs[0] as kuq_set_exact_summary does; the host parts are freed and
+ * their bytes return to the budget.  A part whose pairs do not fit any table even with their duplicates collapsed fails
+ * with KUQ_E_NOMEM.  A failed settle keeps every host part (the contexts stay spilled), so it can run again.  Round
+ * buffers halve until they fit a full card.  The counters join ctxs[0] by kuq_merge_counters_into.  kuq_reset_counts drops the host parts. */
+int kuq_set_exact_spill(kuq_ctx *ctx, uint64_t host_budget_bytes);
+int kuq_exact_spill_info(kuq_ctx *ctx, uint64_t *spills, uint64_t *pairs_on_host);
+int kuq_exact_settle(kuq_ctx *const *ctxs, uint32_t n);
 /* ---- database sharded by minimizer range over the GPUs of a node (SURVEY.md §8(e).2) ------------------------------
  * Who counts: with kuq_set_shard_counting(on) the GPU that FINDS a hit does that hit's sketch work inside the lookup
  * half (kuq_lookup_device / kuq_lookup_device_peers): HLL register update and the record flag behind the sparse tier;

@@ -183,6 +183,9 @@ def load_library(rebuild_if_stale: bool = False):
         "kuq_set_exact_summary": (C.c_int, [vp, vp, vp]),
         "kuq_exact_partition": (C.c_int, [C.POINTER(vp), C.c_uint32]),
         "kuq_exact_rollup_passes": (C.c_int, [vp, u32p]),
+        "kuq_set_exact_spill": (C.c_int, [vp, C.c_uint64]),
+        "kuq_exact_spill_info": (C.c_int, [vp, u64p, u64p]),
+        "kuq_exact_settle": (C.c_int, [C.POINTER(vp), C.c_uint32]),
         "kuq_merge_counters_into": (C.c_int, [vp, vp]),
         "kuq_set_shard_counting": (C.c_int, [vp, C.c_int]),
         "kuq_set_stats": (C.c_int, [vp, C.c_int]),
@@ -740,6 +743,24 @@ class Classifier:
         summary is installed on the first one"""
         arr = (C.c_void_p * len(classifiers))(*[c.h for c in classifiers])
         classifiers[0]._ck(classifiers[0].L.kuq_exact_partition(arr, len(classifiers)))
+
+    def set_exact_spill(self, host_budget_bytes):
+        """kuq_set_exact_spill: a table that cannot grow spills to host memory, up to this many bytes of pairs over all
+        contexts of the process (0 = fail with KUQ_E_NOMEM instead)"""
+        self._ck(self.L.kuq_set_exact_spill(self.h, int(host_budget_bytes)))
+
+    def exact_spill_info(self):
+        """kuq_exact_spill_info: (times the table spilled since the last reset, pairs held in host memory now)"""
+        a, b = C.c_uint64(), C.c_uint64()
+        self._ck(self.L.kuq_exact_spill_info(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    @staticmethod
+    def exact_settle(classifiers):
+        """kuq_exact_settle: the spilled exact sets of these contexts counted part by part on all of them; the summed
+        summary is installed on the first one"""
+        arr = (C.c_void_p * len(classifiers))(*[c.h for c in classifiers])
+        classifiers[0]._ck(classifiers[0].L.kuq_exact_settle(arr, len(classifiers)))
 
     def layout_experiment(self, slot, n_positions, reps=5):
         """kuq_layout_experiment: record layout x search shape of the bin search, timed on the windows of the slot's

@@ -825,6 +825,10 @@ struct TaxDB {
 struct Clade { uint64_t reads = 0, kmers = 0, unique = 0; };
 
 static bool Exact_partitioned = false;   // classifyExact: the contexts hold the exact set's k-mer parts (kuq_exact_partition)
+#ifdef EXACT_COUNTING
+static bool Exact_union_needed = false;  // classifyExact: taxon 0 has children, so the report needs the whole set on one card
+#endif
+static bool Exact_settled = false;       // classifyExact: this sample's set spilled to host memory and was settled by part
 
 static void print_report(kuq_ctx *ctx, TaxDB &tax, ostream &out) {
   uint32_t n = 0;
@@ -854,7 +858,7 @@ static void print_report(kuq_ctx *ctx, TaxDB &tax, ostream &out) {
   }
   // an exact set partitioned over contexts has no member-list unions: every clade comes from the roll-up (the run kept
   // the union when taxon 0 has children, so the library's tree is this one)
-  if (Exact_partitioned) batch = true;
+  if (Exact_partitioned || Exact_settled) batch = true;
   if (batch) {
     vector<uint32_t> ids;
     vector<int> node;
@@ -2180,14 +2184,34 @@ static void end_sample(size_t si) {
   {
     double T0__ = now_s();
 #ifdef EXACT_COUNTING
-    if (Exact_partitioned) {
+    // a set that spilled to host memory (KUQ_EXACT_HOST_BUDGET) is counted part by part on every context instead
+    uint64_t spills = 0, spilled = 0;
+    for (kuq_ctx *c : All_ctx) {
+      uint64_t s = 0, p = 0;
+      if (kuq_exact_spill_info(c, &s, &p)) die(EX_SOFTWARE, kuq_last_error(c));
+      spills += s;
+      spilled += p;
+    }
+    Exact_settled = spilled > 0;
+    if (Exact_partitioned || Exact_settled) {
       for (size_t g = 1; g < All_ctx.size(); g++)
         if (kuq_merge_counters_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+    }
+    if (Exact_settled) {
+      double S0 = now_s();
+      if (kuq_exact_settle(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
+      fprintf(stderr, "classifyExact: the exact k-mer set spilled to host memory %llu times (%llu pairs held there at the end "
+                      "of the run) and was counted by k-mer part\n", (unsigned long long)spills, (unsigned long long)spilled);
+      if (Timing) fprintf(stderr, "[timing] exact set settled from host memory in %.3f s\n", now_s() - S0);
+    } else if (Exact_partitioned) {
       if (kuq_exact_partition(All_ctx.data(), (uint32_t)All_ctx.size())) die(EX_SOFTWARE, kuq_last_error(ctx));
     }
-#endif
-    for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned; g++)
+    for (size_t g = 1; g < All_ctx.size() && !Exact_partitioned && !Exact_settled; g++)
       if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+#else
+    for (size_t g = 1; g < All_ctx.size(); g++)
+      if (kuq_merge_into(ctx, All_ctx[g])) die(EX_SOFTWARE, kuq_last_error(ctx));
+#endif
     if (All_ctx.size() > 1) TICK("merge");
 #ifdef EXACT_COUNTING
     for (size_t g = 0; g < All_ctx.size() && Timing; g++) {
@@ -2667,7 +2691,11 @@ static void shard_loop(const vector<kuq_ctx *> &ctxs, uint32_t n_phases, bool mu
   const uint64_t R = n_phases;
   vector<Batch> batches;
   {
-    BatchReader input(files, batch_limits(96ull << 20, true, false), Extract_now);
+    // KUQ_SHARD_BATCH_READS closes a batch at the first unit boundary after that many reads (tests: a sharded run of a
+    // small input in several batches)
+    BatchLimits lim = batch_limits(96ull << 20, true, false);
+    if (const char *v = getenv("KUQ_SHARD_BATCH_READS")) lim.batch_reads = std::min<size_t>(lim.batch_reads, std::max<size_t>(1, strtoull(v, NULL, 10)));
+    BatchReader input(files, lim, Extract_now);
     for (Batch b; input.next(b);) batches.push_back(std::move(b));
     if (input.fail) die(input.fail, input.fail_msg);
   }
@@ -3088,7 +3116,20 @@ int main(int argc, char **argv) {
   // context: print_report counts those clades one by one, which needs every pair in one place.
   {
     auto z = tax.idx.find(0);
-    Exact_partitioned = All_ctx.size() > 1 && !(z != tax.idx.end() && !tax.e[z->second].children.empty());
+    Exact_union_needed = z != tax.idx.end() && !tax.e[z->second].children.empty();
+    Exact_partitioned = All_ctx.size() > 1 && !Exact_union_needed;
+  }
+  // KUQ_EXACT_HOST_BUDGET=<bytes>: a set that outgrows the devices spills to host memory by k-mer part, up to that many
+  // bytes of pairs over all contexts, and is counted part by part at the end of each sample (end_sample)
+  // A taxonomy with entries below taxon 0 counts those clades one by one from the whole set on one GPU, which a spilled
+  // set does not have: spilling stays off there, so a set that outgrows the card stops at its first failed growth.
+  if (const char *e = getenv("KUQ_EXACT_HOST_BUDGET")) {
+    const uint64_t budget = strtoull(e, NULL, 10);
+    if (Exact_union_needed && budget)
+      fprintf(stderr, "classifyExact: KUQ_EXACT_HOST_BUDGET is not used: this taxonomy has entries below taxon 0, whose clades "
+                      "need the whole exact k-mer set on one GPU\n");
+    for (kuq_ctx *c : All_ctx)
+      if (!Exact_union_needed && kuq_set_exact_spill(c, budget)) die(EX_SOFTWARE, kuq_last_error(c));
   }
 #endif
   Run.samples = samples;

@@ -6,12 +6,14 @@
 // double-precision Ertl estimator (hyperloglogplus.cpp:722-753).  There is no CPU classification path: without
 // an sm_90 device kuq_create fails with KUQ_E_NO_DEVICE.
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <string>
 #include <thread>
 #include <type_traits>
@@ -179,6 +181,12 @@ struct kuq_ctx {
   std::vector<uint32_t> exact_pre;        // preorder of every sketch taxon in the taxonomy (exact roll-up), built once
   DevBuf<uint32_t> d_exact_pre;
   uint32_t exact_rollup_passes = 0;       // k-mer passes of the last exact roll-up
+  // kuq_set_exact_spill: a table that cannot grow moves its pairs to host memory, grouped by owner part
+  // (exact_owner(k-mer, EXACT_MAX_PARTS)), and kuq_exact_settle counts the parts at the end
+  uint64_t spill_budget = 0;              // bytes of spilled pairs the process may hold (0 = no spilling)
+  uint64_t spills = 0;                    // times the table spilled since the last reset
+  uint64_t spilled_pairs = 0;             // pairs held in spill_parts (their bytes are taken from the budget)
+  std::vector<std::vector<ExactPair>> spill_parts[EXACT_MAX_PARTS];   // pieces of each part, one per round that had some
 
   // database streamed through HBM range by range (kuq_stream_*): two device buffers, one copy stream
   struct StreamBuf {
@@ -745,6 +753,14 @@ int batch_set_saturated(kuq_ctx *ctx) {
   return fail(ctx, KUQ_E_CAPACITY, "sparse-tier set saturated: raise kuq_config.sparse_set_slots (now %llu)", (unsigned long long)ctx->sparse.cap);
 }
 
+// Slots of a table per round when its pairs move between contexts or to the host: 2^22 (64 MiB of pairs), or
+// KUQ_EXACT_MERGE_SLOTS, so that tests of the rounds can use small tables
+uint64_t exact_round_slots() {
+  uint64_t round_slots = 1ull << 22;
+  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+  return round_slots;
+}
+
 // src's exact pairs go to the tables of dsts[0, n) in rounds over at most 2^22 slots of src's table (64 MiB of pairs per
 // round on each side; KUQ_EXACT_MERGE_SLOTS overrides it, so that tests of the rounds can use small tables).
 // `gather(lo, hi, buf, cap, counts)` compacts the slots [lo, hi) into buf on src's device, grouped by destination with
@@ -754,9 +770,7 @@ int batch_set_saturated(kuq_ctx *ctx) {
 template <typename Gather, typename Take>
 int move_rounds(kuq_ctx *report, const char *no_room, kuq_ctx *src, kuq_ctx *const *dsts, uint32_t n, Gather gather, Take take) {
   kuq_ctx *ctx = report;
-  uint64_t round_slots = 1ull << 22;
-  if (const char *e = getenv("KUQ_EXACT_MERGE_SLOTS")) round_slots = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
-  const uint64_t chunk = std::min(round_slots, src->exact.cap);
+  const uint64_t chunk = std::min(exact_round_slots(), src->exact.cap);
   DevBuf<ExactPair> send;
   std::vector<DevBuf<ExactPair>> recv(n);
   int rc = KUQ_OK;
@@ -804,6 +818,106 @@ int merge_exact_pairs(kuq_ctx *dst, kuq_ctx *src) {
       dst, "exact k-mer set merge: no room for %llu pairs on device %d", src, &dst, 1,
       [src](uint64_t lo, uint64_t hi, ExactPair *buf, uint64_t cap, uint64_t *counts) { return exact_export_range(src, lo, hi, buf, cap, counts); },
       [dst](uint32_t, const ExactPair *pairs, uint64_t m) { return exact_import(dst, pairs, m); });
+}
+
+// ---- the exact set spilled to host memory (kuq_set_exact_spill, kuq_exact_settle) -----------------------------------
+// Bytes of spilled pairs held by all contexts of the process; a spill takes its bytes before it copies anything.
+std::atomic<uint64_t> g_spill_bytes{0};
+
+bool take_spill_bytes(uint64_t bytes, uint64_t budget) {
+  uint64_t cur = g_spill_bytes.load();
+  do {
+    if (cur + bytes > budget) return false;
+  } while (!g_spill_bytes.compare_exchange_weak(cur, cur + bytes));
+  return true;
+}
+
+// the context's host parts go, and their bytes return to the budget
+void drop_spill(kuq_ctx *ctx) {
+  g_spill_bytes -= ctx->spilled_pairs * sizeof(ExactPair);
+  ctx->spilled_pairs = 0;
+  for (auto &part : ctx->spill_parts) std::vector<std::vector<ExactPair>>().swap(part);
+}
+
+int refuse_spilled(kuq_ctx *ctx, const char *call) {
+  return fail(ctx, KUQ_E_STATE, "%s: the exact k-mer set has spilled %llu pairs to host memory and the device holds only part of "
+                                "it: count it with kuq_exact_settle first", call, (unsigned long long)ctx->spilled_pairs);
+}
+
+// A device and a pinned buffer of `chunk` pairs for rounds between the host parts and a table.  The card may be full, so
+// `chunk` halves until both can be allocated (down to 1024 pairs); false when even that fails.
+bool round_buffers(uint64_t &chunk, DevBuf<ExactPair> &d_buf, HostBuf<ExactPair> &h_buf) {
+  for (;; chunk /= 2) {
+    if (d_buf.alloc(chunk) == cudaSuccess && h_buf.alloc(chunk) == cudaSuccess) return true;
+    (void)cudaGetLastError();
+    d_buf.reset();
+    if (chunk <= 1024) return false;
+  }
+}
+
+// Every pair of the table to the context's host parts, then the table is emptied (counts included) at the same
+// capacity.  Rounds over exact_round_slots() slots: the round's pairs grouped by owner part (the partitioned export's
+// kernel over a slot range) into a device buffer, through a pinned buffer into the parts.  The card is full when this
+// runs, so the round buffer halves until it can be allocated.  All slots idle.
+int spill_exact(kuq_ctx *ctx) {
+  ExactTable &t = ctx->exact;
+  uint64_t n = 0;
+  int rc = table_items(ctx, t, &n);
+  if (rc || !n) return rc;
+  const uint64_t bytes = n * sizeof(ExactPair);
+  if (!take_spill_bytes(bytes, ctx->spill_budget))
+    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: spilling %llu pairs (%.2f GiB) to host memory would pass the host budget of "
+                                  "%llu bytes (KUQ_EXACT_HOST_BUDGET), of which the process holds %llu already",
+                (unsigned long long)n, bytes / double(1ull << 30), (unsigned long long)ctx->spill_budget,
+                (unsigned long long)g_spill_bytes.load());
+  uint64_t chunk = std::min(exact_round_slots(), t.cap), moved = 0;
+  DevBuf<ExactPair> d_buf;
+  HostBuf<ExactPair> h_buf;
+  if (!round_buffers(chunk, d_buf, h_buf))
+    rc = fail(ctx, KUQ_E_NOMEM, "exact k-mer set: no memory for a spill round of %llu pairs on device %d", (unsigned long long)chunk, ctx->device);
+  uint64_t counts[EXACT_MAX_PARTS];
+  for (uint64_t lo = 0; lo < t.cap && !rc; lo += chunk) {
+    rc = exact_parts(ctx, lo, std::min(lo + chunk, t.cap), EXACT_MAX_PARTS, d_buf, chunk, counts);
+    uint64_t m = 0;
+    for (uint32_t j = 0; j < EXACT_MAX_PARTS && !rc; j++) m += counts[j];
+    if (rc || !m) continue;
+    if (cudaMemcpyAsync(h_buf, d_buf, m * sizeof(ExactPair), cudaMemcpyDeviceToHost, ctx->aux) != cudaSuccess ||
+        cudaStreamSynchronize(ctx->aux) != cudaSuccess) {
+      rc = fail(ctx, KUQ_E_CUDA, "exact k-mer set: spill copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+      break;
+    }
+    const ExactPair *at = h_buf;
+    for (uint32_t j = 0; j < EXACT_MAX_PARTS; j++) {
+      if (counts[j]) ctx->spill_parts[j].emplace_back(at, at + counts[j]);
+      at += counts[j];
+    }
+    moved += m;
+  }
+  // the budget holds what the parts hold; pairs still in the table after a failure stay there, and a set union does not
+  // mind holding a pair twice
+  ctx->spilled_pairs += moved;
+  g_spill_bytes -= (n - std::min(n, moved)) * sizeof(ExactPair);
+  if (rc) return rc;
+  if (moved != n) return fail(ctx, KUQ_E_CAPACITY, "internal: the spill moved %llu of %llu pairs", (unsigned long long)moved, (unsigned long long)n);
+  ctx->snap_valid = false;
+  return clear_table(ctx, t);
+}
+
+// Room for a batch's pairs (one per window).  A table that cannot grow spills when kuq_set_exact_spill allows it and
+// then takes the batch at its capacity.
+int reserve_batch_pairs(kuq_ctx *ctx, uint64_t windows) {
+  int rc = reserve_exact_inserts(ctx, windows);
+  if (rc != KUQ_E_NOMEM || !ctx->spill_budget) return rc;
+  rc = spill_exact(ctx);
+  if (rc) return rc;
+  ctx->spills++;
+  rc = make_room(ctx, ctx->exact, 0, windows);
+  if (rc)
+    return fail(ctx, KUQ_E_NOMEM, "exact k-mer set: an empty table of %llu slots cannot take a batch of up to %llu pairs, which needs "
+                                  "%llu slots: smaller batches, or more device memory",
+                (unsigned long long)ctx->exact.cap, (unsigned long long)windows,
+                (unsigned long long)slots_for(windows, ctx->exact.cap, 6));
+  return KUQ_OK;
 }
 
 // kuq_set_extract's slot buffer: one selection byte per read, then the batch's count of selected reads (u32)
@@ -1468,9 +1582,9 @@ int launch_on_slot(kuq_ctx *ctx, Slot &s, int mode, Params &p, int run = -1) {
     p.sparse = set_view(ctx, ctx->sparse);             // the set may have moved
   }
   // exact counting: the batch's windows go into the (taxon, k-mer) table, which grows before the batch when they could
-  // fill it
+  // fill it, or spills to host memory when it cannot grow (kuq_set_exact_spill)
   if ((mode == MODE_RESOLVE || mode == MODE_FUSED) && !(p.flags & 4u) && ctx->cfg.hll_mode == KUQ_HLL_EXACT && p.n_reads) {
-    int rrc = reserve_exact_inserts(ctx, s.total_bases);
+    int rrc = reserve_batch_pairs(ctx, s.total_bases);
     if (rrc) return rrc;
     p.exact = set_view(ctx, ctx->exact);
   }
@@ -1632,6 +1746,7 @@ void kuq_destroy(kuq_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
+  drop_spill(ctx);
   delete ctx;
 }
 
@@ -2535,6 +2650,7 @@ int kuq_counts_size(kuq_ctx *ctx, uint32_t *n) {
 int kuq_read_counts(kuq_ctx *ctx, uint32_t *taxid, uint64_t *n_reads, uint64_t *n_kmers, uint64_t *unique,
                     uint8_t *is_sparse, uint32_t cap) {
   if (!ctx) return KUQ_E_INVALID_ARG;
+  if (ctx->spilled_pairs) return refuse_spilled(ctx, "kuq_read_counts");
   CountsHost &h = ctx->snap;
   int rc = ctx->snap_valid ? KUQ_OK : fetch_counts(ctx, h);
   if (rc) return rc;
@@ -2571,6 +2687,7 @@ int kuq_clade_counts(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint64_t 
                      uint64_t *unique) {
   if (!ctx || (!taxids && n)) return KUQ_E_INVALID_ARG;
   if (!ctx->finalized) return fail(ctx, KUQ_E_STATE, "nothing classified yet");
+  if (ctx->spilled_pairs) return refuse_spilled(ctx, "kuq_clade_counts");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   if (!ctx->snap_valid) {
@@ -2669,6 +2786,7 @@ int kuq_clade_counts_tree(kuq_ctx *ctx, const uint32_t *taxids, uint32_t n, uint
                           uint64_t *unique) {
   if (!ctx || (!taxids && n)) return KUQ_E_INVALID_ARG;
   if (!ctx->finalized) return fail(ctx, KUQ_E_STATE, "nothing classified yet");
+  if (ctx->spilled_pairs) return refuse_spilled(ctx, "kuq_clade_counts_tree");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   if (!ctx->snap_valid) {
@@ -3161,6 +3279,11 @@ static int merge_into(kuq_ctx *dst, kuq_ctx *src, bool sets) {
       dst->cfg.hll_mode != src->cfg.hll_mode)
     return fail(ctx, KUQ_E_STATE, "the contexts number their taxa differently (different database / taxonomy / HLL mode)");
   const bool exact = dst->cfg.hll_mode == KUQ_HLL_EXACT;
+  if (exact && sets && (dst->spilled_pairs || src->spilled_pairs)) {
+    int rc = refuse_spilled(dst->spilled_pairs ? dst : src, "kuq_merge_into");
+    if (!dst->spilled_pairs) dst->err = src->err;
+    return rc;
+  }
   // src: flagged records → its set (skipping what dst already knows to be dense is a refinement left out)
   CU(cudaSetDevice(src->device));
   for (auto &s : src->slots) CU(cudaStreamSynchronize(s.stream));
@@ -3460,6 +3583,7 @@ int kuq_exact_export(kuq_ctx *ctx, void *d_pairs_out, uint64_t cap, uint64_t *n)
   if (rc) return rc;
   *n = 0;
   if (!ctx->exact.slots) return KUQ_OK;                           // not KUQ_HLL_EXACT
+  if (ctx->spilled_pairs) return refuse_spilled(ctx, "kuq_exact_export");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   return exact_export_range(ctx, 0, ctx->exact.cap, static_cast<ExactPair *>(d_pairs_out), d_pairs_out ? cap : 0, n);
@@ -3486,6 +3610,7 @@ static int exact_export_partitioned(kuq_ctx *ctx, uint32_t n_parts, void *d_pair
   if (rc) return rc;
   for (uint32_t j = 0; j < n_parts; j++) counts[j] = 0;
   if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_export_partitioned needs a KUQ_HLL_EXACT context");
+  if (ctx->spilled_pairs) return refuse_spilled(ctx, "kuq_exact_export_partitioned");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   return exact_parts(ctx, 0, ctx->exact.cap, n_parts, static_cast<ExactPair *>(d_pairs_out), cap, counts,
@@ -3523,6 +3648,7 @@ int kuq_exact_summary(kuq_ctx *ctx, uint64_t *d_count_out, int64_t *d_books_out)
   int rc = ensure_ready(ctx);
   if (rc) return rc;
   if (!ctx->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_summary needs a KUQ_HLL_EXACT context");
+  if (ctx->spilled_pairs) return refuse_spilled(ctx, "kuq_exact_summary");
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
   std::vector<long long> books;
@@ -3571,6 +3697,7 @@ int kuq_exact_partition(kuq_ctx *const *ctxs, uint32_t n) {
     int rc = ensure_ready(c);
     if (rc) { if (g) ctx->err = c->err; return rc; }
     if (!c->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_partition needs KUQ_HLL_EXACT contexts");
+    if (c->spilled_pairs) { rc = refuse_spilled(c, "kuq_exact_partition"); if (g) ctx->err = c->err; return rc; }
     if (c->n_taxa != ctx->n_taxa || c->n_sketch != ctx->n_sketch || c->raw_of_dense != ctx->raw_of_dense)
       return fail(ctx, KUQ_E_STATE, "the contexts number their taxa differently (different database / taxonomy)");
     CU(cudaSetDevice(c->device));
@@ -3634,6 +3761,179 @@ int kuq_exact_rollup_passes(kuq_ctx *ctx, uint32_t *passes) {
   return KUQ_OK;
 }
 
+int kuq_set_exact_spill(kuq_ctx *ctx, uint64_t host_budget_bytes) {
+  if (!ctx) return KUQ_E_INVALID_ARG;
+  if (ctx->cfg.hll_mode != KUQ_HLL_EXACT) return fail(ctx, KUQ_E_STATE, "kuq_set_exact_spill needs a KUQ_HLL_EXACT context");
+  ctx->spill_budget = host_budget_bytes;
+  return KUQ_OK;
+}
+
+int kuq_exact_spill_info(kuq_ctx *ctx, uint64_t *spills, uint64_t *pairs_on_host) {
+  if (!ctx) return KUQ_E_INVALID_ARG;
+  if (spills) *spills = ctx->spills;
+  if (pairs_on_host) *pairs_on_host = ctx->spilled_pairs;
+  return KUQ_OK;
+}
+
+// 1. every context spills what its table holds; 2. the EXACT_MAX_PARTS parts of all contexts are cut into groups of
+// consecutive parts that fit one table; 3. one host thread per context imports each of its groups into its emptied
+// table in rounds (duplicates from successive spills and from other contexts collapse) and adds the group's counters
+// and roll-up books to its sums; 4. the sums are installed on ctxs[0] and the host parts go.
+int kuq_exact_settle(kuq_ctx *const *ctxs, uint32_t n) {
+  if (!ctxs || n == 0) return KUQ_E_INVALID_ARG;
+  kuq_ctx *ctx = ctxs[0];
+  for (uint32_t g = 0; g < n; g++) {
+    if (!ctxs[g]) return KUQ_E_INVALID_ARG;
+    for (uint32_t h = 0; h < g; h++) if (ctxs[h] == ctxs[g]) return KUQ_E_INVALID_ARG;
+  }
+  int max_device = 0;
+  for (uint32_t g = 0; g < n; g++) {
+    kuq_ctx *c = ctxs[g];
+    int rc = ensure_ready(c);
+    if (rc) { if (g) ctx->err = c->err; return rc; }
+    if (!c->exact.slots) return fail(ctx, KUQ_E_STATE, "kuq_exact_settle needs KUQ_HLL_EXACT contexts");
+    if (c->n_taxa != ctx->n_taxa || c->n_sketch != ctx->n_sketch || c->raw_of_dense != ctx->raw_of_dense)
+      return fail(ctx, KUQ_E_STATE, "the contexts number their taxa differently (different database / taxonomy)");
+    max_device = std::max(max_device, c->device);
+  }
+  // 1. the pairs still on the devices join the host parts
+  for (uint32_t g = 0; g < n; g++) {
+    kuq_ctx *c = ctxs[g];
+    CU(cudaSetDevice(c->device));
+    for (auto &s : c->slots) CU(cudaStreamSynchronize(s.stream));
+    int rc = spill_exact(c);
+    if (rc) { if (g) ctx->err = c->err; cudaSetDevice(ctx->device); return rc; }
+  }
+  // 2. a table smaller than the largest grows to it (it is empty now) where its device keeps room beside the new table
+  //    for a round buffer and for half the new table's bytes of sort scratch (the roll-up sorts in passes when it has
+  //    less than its 32 B per pair); each table takes pairs up to the load of make_room.  Groups of consecutive parts whose spilled pairs fit the largest table; a part
+  //    larger than that is a group of its own, which fits only if its duplicates collapse enough.
+  uint64_t big = 0;
+  for (uint32_t g = 0; g < n; g++) big = std::max(big, ctxs[g]->exact.cap);
+  std::vector<uint64_t> room(n);
+  for (uint32_t g = 0; g < n; g++) {
+    kuq_ctx *c = ctxs[g];
+    CU(cudaSetDevice(c->device));
+    size_t free_b = 0, total_b = 0;
+    const uint64_t headroom = std::min(exact_round_slots(), big) * sizeof(ExactPair) + big * sizeof(ExactPair) / 2;
+    if (c->exact.cap < big && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= big * sizeof(ExactPair) + headroom &&
+        grow_table(c, c->exact, big) != KUQ_OK)
+      c->err.clear();
+    (void)cudaGetLastError();
+    room[g] = c->exact.cap * 8 / 10;
+  }
+  const uint64_t room_max = *std::max_element(room.begin(), room.end());
+  uint64_t part_pairs[EXACT_MAX_PARTS] = {};
+  for (uint32_t g = 0; g < n; g++)
+    for (uint32_t j = 0; j < EXACT_MAX_PARTS; j++)
+      for (auto &piece : ctxs[g]->spill_parts[j]) part_pairs[j] += piece.size();
+  struct Group { uint32_t lo, hi; uint64_t pairs; };
+  std::vector<Group> groups;
+  for (uint32_t j = 0; j < EXACT_MAX_PARTS; j++) {
+    if (!part_pairs[j]) continue;
+    if (groups.empty() || groups.back().pairs + part_pairs[j] > room_max) groups.push_back(Group{j, j, 0});
+    groups.back().hi = j + 1;
+    groups.back().pairs += part_pairs[j];
+  }
+  // 3. each group to the context with the fewest pairs so far among those whose table takes it (the largest if none)
+  std::vector<std::vector<Group>> work(n);
+  std::vector<uint64_t> load(n, 0);
+  for (const Group &gr : groups) {
+    uint32_t best = n;
+    for (uint32_t g = 0; g < n; g++)
+      if (room[g] >= std::min(gr.pairs, room_max) && (best == n || load[g] < load[best])) best = g;
+    work[best].push_back(gr);
+    load[best] += gr.pairs;
+  }
+  std::vector<std::vector<unsigned long long>> count_sum(n, std::vector<unsigned long long>(ctx->n_sketch, 0));
+  std::vector<std::vector<long long>> books_sum(n, std::vector<long long>(ctx->n_taxa, 0));
+  std::vector<int> status(n, KUQ_OK);
+  // the roll-up's sort sizes its scratch to the device's free memory: one sort at a time per device
+  std::vector<std::mutex> device_lock(max_device + 1);
+  auto settle_groups = [&](uint32_t g) -> int {
+    kuq_ctx *ctx = ctxs[g];                      // errors are reported on this context (CU)
+    if (work[g].empty()) return KUQ_OK;
+    CU(cudaSetDevice(ctx->device));
+    uint64_t chunk = std::min(exact_round_slots(), std::max<uint64_t>(room[g], 1));
+    DevBuf<ExactPair> d_buf;
+    HostBuf<ExactPair> h_buf;
+    if (!round_buffers(chunk, d_buf, h_buf))
+      return fail(ctx, KUQ_E_NOMEM, "exact k-mer set settle: no memory for a round of %llu pairs on device %d",
+                  (unsigned long long)chunk, ctx->device);
+    std::vector<unsigned long long> cnt(ctx->n_sketch);
+    std::vector<long long> books;
+    for (const Group &gr : work[g]) {
+      int rc = clear_table(ctx, ctx->exact);
+      // the group's pieces in rounds of up to `chunk` pairs: pieces are packed into the pinned buffer, and a piece
+      // larger than it is cut
+      uint64_t fill = 0;
+      auto flush = [&]() -> int {
+        if (!fill) return KUQ_OK;
+        CU(cudaMemcpyAsync(d_buf, h_buf, fill * sizeof(ExactPair), cudaMemcpyHostToDevice, ctx->aux));
+        CU(cudaStreamSynchronize(ctx->aux));
+        const uint64_t m = fill;
+        fill = 0;
+        return exact_import(ctx, d_buf, m);
+      };
+      for (uint32_t j = gr.lo; j < gr.hi && !rc; j++)
+        for (uint32_t s = 0; s < n && !rc; s++)
+          for (auto &piece : ctxs[s]->spill_parts[j]) {
+            for (uint64_t at = 0; at < piece.size() && !rc;) {
+              const uint64_t m = std::min<uint64_t>(piece.size() - at, chunk - fill);
+              memcpy(h_buf + fill, piece.data() + at, m * sizeof(ExactPair));
+              fill += m;
+              at += m;
+              if (fill == chunk) rc = flush();
+            }
+            if (rc) break;
+          }
+      if (!rc) rc = flush();
+      if (rc == KUQ_E_NOMEM)
+        return fail(ctx, KUQ_E_NOMEM, "exact k-mer set settle: parts %u to %u (%llu spilled pairs) do not fit the table of %llu "
+                                      "slots on device %d: %s", gr.lo, gr.hi - 1, (unsigned long long)gr.pairs,
+                    (unsigned long long)ctx->exact.cap, ctx->device, ctx->err.c_str());
+      if (rc) return rc;
+      {
+        std::lock_guard<std::mutex> lock(device_lock[ctx->device]);
+        rc = exact_books(ctx, books);
+      }
+      if (rc) return rc;
+      CU(cudaMemcpy(cnt.data(), ctx->exact.count, ctx->n_sketch * 8ull, cudaMemcpyDeviceToHost));
+      for (uint32_t d = 0; d < ctx->n_sketch; d++) count_sum[g][d] += cnt[d];
+      for (uint32_t d = 0; d < ctx->n_taxa; d++) books_sum[g][d] += books[d];
+    }
+    return KUQ_OK;
+  };
+  {
+    std::vector<std::thread> threads;
+    for (uint32_t g = 1; g < n; g++) threads.emplace_back([&, g] { status[g] = settle_groups(g); });
+    status[0] = settle_groups(0);
+    for (auto &t : threads) t.join();
+  }
+  // 4. a failure keeps every host part, so the set is not lost: the contexts stay spilled (their readouts refuse) and the
+  //    settle step can run again once there is more device memory (the pairs in the tables are spilled again, and a set
+  //    union does not mind them twice)
+  CU(cudaSetDevice(ctx->device));
+  for (uint32_t g = 0; g < n; g++)
+    if (status[g]) {
+      if (g) ctx->err = ctxs[g]->err;
+      return status[g];
+    }
+  // the host parts go; every table holds one group at most from now on
+  for (uint32_t g = 0; g < n; g++) {
+    kuq_ctx *c = ctxs[g];
+    drop_spill(c);
+    c->exact_partitioned = true;
+    c->merged_exact = false;
+    c->snap_valid = false;
+  }
+  for (uint32_t g = 1; g < n; g++) {
+    for (uint32_t d = 0; d < ctx->n_sketch; d++) count_sum[0][d] += count_sum[g][d];
+    for (uint32_t d = 0; d < ctx->n_taxa; d++) books_sum[0][d] += books_sum[g][d];
+  }
+  return set_exact_summary(ctx, count_sum[0], books_sum[0]);
+}
+
 int kuq_dense_taxids(kuq_ctx *ctx, uint32_t *taxid_of_dense, uint32_t cap, uint32_t *n) {
   if (!ctx || !n) return KUQ_E_INVALID_ARG;
   int rc = ensure_ready(ctx);
@@ -3648,6 +3948,8 @@ int kuq_dense_taxids(kuq_ctx *ctx, uint32_t *taxid_of_dense, uint32_t cap, uint3
 int kuq_reset_counts(kuq_ctx *ctx) {
   if (!ctx) return KUQ_E_INVALID_ARG;
   ctx->snap_valid = false;
+  drop_spill(ctx);
+  ctx->spills = 0;
   if (!ctx->finalized) return KUQ_OK;
   CU(cudaSetDevice(ctx->device));
   for (auto &s : ctx->slots) CU(cudaStreamSynchronize(s.stream));
